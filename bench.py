@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — M-LOAM per-scan hot path on B200 (contract: see the task statement / DESIGN.md §Measurement).
+"""bench.py — M-LOAM per-scan hot path on an H100 (DESIGN.md §Measurement).
 
 A "step" is one pass of the hot path over one synthetic rig frame (the sweeps of all LiDARs of the configuration):
     FeatureExtract::extractCloud per LiDAR -> extrinsic + laser id merge -> downsampleCurrentScan -> scan2MapOptimization with
@@ -24,6 +24,9 @@ e2e         : the same through the C-ABI call a user makes (mloam_frame) with HO
 roofline    : k_match_knn (dominant) and the map build (the streaming kernel), algorithmic bytes / CUDA-event time.
 cpu_baseline: the CPU restatement of the reference path (oracle/, kd-tree = the reference's own nanoflann from oracle/_ref)
               on the same frames, reference threading.  --impl reference: that CPU path as the timed arm.
+--dump-outputs DIR: after the timed steps, what the last timed step returned to its caller (pose, solve statistics; for the
+              calibration step also the extrinsic) as DIR/<name>.npy in float64.  The inputs are seeded: the same arguments give
+              the same inputs on every run, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -116,9 +119,9 @@ def make_workload(syn, cfg: dict, n_gpus: int, rank: int, n_frames: int, map_kin
 
 
 class ClockSampler:
-    """SM clock / throttle reasons DURING the timed region (B200_PROFILING.md's clocks line), sampled in-process
-    through NVML every 10 ms — an `nvidia-smi -lms` child was seen to stall kernel submission for milliseconds at a
-    time on these hosts, which is not what a 1.5 ms step should be measured next to.  Falls back to that child when
+    """SM clock / throttle reasons DURING the timed region, sampled in-process through NVML every 10 ms — an
+    `nvidia-smi -lms` child was seen to stall kernel submission for milliseconds at a time, which is not what a
+    millisecond-scale step should be measured next to.  Falls back to that child when
     NVML is not importable."""
 
     REASONS = (("hw_slowdown", "nvmlClocksEventReasonHwSlowdown"), ("hw_thermal_slowdown", "nvmlClocksEventReasonHwThermalSlowdown"),
@@ -481,6 +484,23 @@ def config_blurb(name, cfg, n_gpus, args, wl):
             "l2": "256 MiB buffer written between timed steps (L2 flush)"}
 
 
+STAT_SCALARS = ("ran", "n_surf", "n_corner", "lm_iterations", "degenerate", "termination", "final_cost", "n_surf_in", "n_corner_in")
+
+
+def dump_outputs(out_dir: str, R: dict) -> None:
+    """The arrays a caller of the timed path received in its last timed step, as out_dir/<name>.npy (float64, a few hundred
+    bytes in all): the pose [7], the extrinsic [7] of the calibration step, the solver's eigenvalues [6] and normal matrix
+    [6, 6], and each scalar of the solve statistics."""
+    os.makedirs(out_dir, exist_ok=True)
+    st = R["last_stats"]
+    arrays = {"pose": R["last_pose"], "eig": st["eig"], "H": st["H"]}
+    if "last_ext" in R:
+        arrays["ext_cal"] = R["last_ext"]
+    arrays.update({k: st[k] for k in STAT_SCALARS})
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.asarray(a, np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -495,6 +515,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-lookahead", action="store_true", help="do not announce sweep k+1 while frame k runs (no overlap of extraction with the solve)")
     ap.add_argument("--no-c4", action="store_true", help="skip the extra C4-on-one-GPU measurement of the default run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the last timed step returned as DIR/<name>.npy")
     args = ap.parse_args()
 
     if args.gpus > 1 and "WORLD_SIZE" not in os.environ and args.impl == "ours":
@@ -602,6 +623,8 @@ def main():
             dist.destroy_process_group()
         return 0
 
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, R)
     wl = R["wl"]
     config = config_blurb(cfg_name, cfg, n_gpus, args, wl)
     if R.get("exchange"):
@@ -615,22 +638,15 @@ def main():
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (burst copy)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "nominal HBM3 bandwidth of the H100 SXM data sheet (3.35 TB/s)"
     roofline, stage_ms = None, None
     if "prof" in R:
         prof, ps = R["prof"], R["prof_steps"]
         match_ms, match_launches = prof["match"]
         alg = R["feats_prof"] * cfg["gn_iters"] * KNN_BYTES_PER_FEATURE
         ach = (alg / 1e9) / (match_ms / 1e3) if match_ms > 0 else 0.0
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "r02_match_traffic.json")
-        if os.path.exists(tp):
-            try:
-                traffic = json.load(open(tp)).get("dram_bytes_per_launch")
-            except Exception:
-                traffic = None
         roofline = {"bound": "hbm", "kernel": "k_match_knn<5> (pointAssociateToMap + exact 5-NN over the dense voxel grid, one warp per feature, TMA-staged rows)",
-                    "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic, "peak_source": peak_src,
+                    "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": None, "peak_source": peak_src,
                     "algorithmic_bytes_per_feature": KNN_BYTES_PER_FEATURE, "avg_launch_us": 1e3 * match_ms / max(1, match_launches), "launches": match_launches,
                     "note": "the submap is L2-resident and a launch moves ~1 MB of compulsory bytes: latency-bound, not HBM-bound (DESIGN.md 4)"}
         mb_ach = R["map_build_points"] * MAP_BYTES_PER_POINT / 1e9 / (R["map_build_ms"] / 1e3)

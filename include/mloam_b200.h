@@ -1,4 +1,4 @@
-/* mloam_b200.h — C ABI of the B200-native M-LOAM per-scan hot path.
+/* mloam_b200.h — C ABI of the H100-native M-LOAM per-scan hot path.
  *
  * Plain C, POD only, no torch / Eigen / PCL / Ceres types.  Every entry point names the reference
  * interface (file:line, relative to gogojjh/M-LOAM) it replaces.  All functions return 0 on success

@@ -2,7 +2,7 @@
 
 Plumbing for tests/ and bench.py only — the product is the shared library and the C++ host shim under
 m-loam_b200/host/.  There is NO CPU fallback: importing works anywhere (so the symbol table can be checked
-on a CPU box), but creating a Context without a B200 raises.
+on a CPU box), but creating a Context without an H100 raises.
 
 The directory name carries a hyphen, so load it with tests/conftest.py's `load_mloam()` (importlib) or
     importlib.util.spec_from_file_location("mloam_b200", ".../m-loam_b200/__init__.py")
@@ -56,8 +56,8 @@ class SolveStats(C.Structure):
 
 
 class _Stats(dict):
-    """Solve statistics as a dict; the two array entries ("eig", "H") are materialised on first access (a frame call every
-    0.7 ms should not pay for arrays nobody reads)."""
+    """Solve statistics as a dict; the two array entries ("eig", "H") are materialised on first access (a per-frame call
+    should not pay for arrays nobody reads)."""
 
     def __init__(self, st: "SolveStats"):
         super().__init__(ran=st.ran, n_surf=st.n_surf, n_corner=st.n_corner, lm_iterations=st.lm_iterations, degenerate=st.degenerate,
@@ -87,7 +87,7 @@ class Features(C.Structure):
 
 
 def build(force: bool = False) -> str:
-    """Compile libmloam_b200.so for sm_100a in-tree (nvcc cross-compiles without a GPU)."""
+    """Compile libmloam_b200.so for sm_90a in-tree (nvcc cross-compiles without a GPU)."""
     srcs = []
     for d in (os.path.join(HERE, "csrc"), os.path.join(ROOT, "include")):
         srcs += [os.path.join(d, f) for f in os.listdir(d) if f.endswith((".cu", ".cuh", ".h"))]
@@ -144,7 +144,7 @@ class Context:
         self.params = params if params is not None else default_params()
         rc = lib().mloam_ctx_create(device, C.byref(self.params), C.byref(self._h))
         if rc != 0:
-            raise MloamError(f"mloam_ctx_create failed ({rc}): a B200 (sm_100a) device is required, there is no CPU path")
+            raise MloamError(f"mloam_ctx_create failed ({rc}): an H100 (sm_90a) device is required, there is no CPU path")
 
     def close(self):
         if self._h:

@@ -51,7 +51,7 @@ void prof_collect(Ctx *c) {
 
 extern "C" {
 
-const char *mloam_version(void) { return "mloam_b200 0.1 (sm_100a)"; }
+const char *mloam_version(void) { return "mloam_b200 0.1 (sm_90a)"; }
 
 void mloam_default_params(mloam_params_t *p) {
   memset(p, 0, sizeof(*p));
@@ -82,8 +82,8 @@ int mloam_ctx_create(int device, const mloam_params_t *params, mloam_ctx_t **out
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return MLOAM_E_NO_DEVICE;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return MLOAM_E_NO_DEVICE;
-  if (prop.major != 10) {
-    fprintf(stderr, "mloam_b200: device %d is sm_%d%d; this library carries sm_100a code only\n", device, prop.major,
+  if (prop.major != 9) {
+    fprintf(stderr, "mloam_b200: device %d is sm_%d%d; this library carries sm_90a code only\n", device, prop.major,
             prop.minor);
     return MLOAM_E_NO_DEVICE;
   }

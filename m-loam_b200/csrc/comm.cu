@@ -1,5 +1,5 @@
 // comm.cu — multi-GPU plumbing: one LiDAR per GPU, one all-reduce of the packed normal equations per LM
-// evaluation (SURVEY.md §8e).  NCCL over NVLink 5 / NVSwitch; the collective is enqueued on the context stream
+// evaluation (SURVEY.md §8e).  NCCL over NVLink / NVSwitch; the collective is enqueued on the context stream
 // between the block-partial reduction and the LM step, so an iteration never returns to the host.
 #include <dlfcn.h>
 #include <nccl.h>  // types and prototypes only: the library is bound at run time (see nccl_api())

@@ -1,4 +1,4 @@
-// common.cuh — shared device-side types and small math for the M-LOAM hot-path kernels (sm_100a).
+// common.cuh — shared device-side types and small math for the M-LOAM hot-path kernels (sm_90a).
 //
 // All translation units are compiled with -fmad=false: every float/double operation rounds once, in
 // the order written, so the float gates of the reference (kNN distances, line/plane fits,

@@ -119,7 +119,7 @@ struct MatchCfg {
 
 struct Ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t stream = nullptr;
   bool own_stream = true;
   cudaStream_t stream2 = nullptr;        // side stream: submap upload + build run concurrently with extraction
@@ -227,7 +227,7 @@ struct Ctx {
   DevBuf stamps;
   int stamp_n = 0;
   std::vector<std::string> stamp_labels;
-  int knn_min_blocks = 4;          // k_match_knn variant: resident CTAs per SM it is compiled for (MLOAM_KNN_MB = 2 | 3 | 4)
+  int knn_min_blocks = 2;          // k_match_knn variant: resident CTAs per SM it is compiled for (MLOAM_KNN_MB = 2 | 3 | 4); 2 is fastest on the H100
   int use_seeds = 1;               // seed the kNN of re-association iterations > 0 with the previous neighbour lists
   int s2m_ran = 0;
   int lm_min_corr = 0;              // lm_init_state: minimum matched features for a Solve (tracker: 10)

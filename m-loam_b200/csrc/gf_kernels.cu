@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(GF_THREADS) k_gf_select(GfArgs a) {
   const int tid = threadIdx.x, lane = tid & 31;
   const int n = a.d_n ? min(a.n, *a.d_n) : a.n;
   // The selection is a chain of dependent pool operations (16-step Fenwick descents, visited marks) issued by ONE thread: in
-  // global memory every step is an L2 round trip (~4 us per pick measured); the pool lives in shared memory whenever it fits
+  // global memory every step is an L2 round trip; the pool lives in shared memory whenever it fits
   // (a.smem_ints words of dynamic shared memory: Fenwick tree first, then the visited marks).
   extern __shared__ int gf_smem[];
   int *const fen = (n + 1 <= a.smem_ints) ? gf_smem : a.fen;

@@ -73,7 +73,7 @@ __device__ __forceinline__ int warp_excl_scan(int v, int lane, int *total) {
   return inc - v;
 }
 
-// ------------------------------------------------------------------------------------------- mbarrier / TMA (sm_100a)
+// ------------------------------------------------------------------------------------------- mbarrier / TMA (sm_90a)
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void knn_smem_init(KnnSmem &ks, int lane, unsigned = 0u) {
   if (lane == 0) {

@@ -1,4 +1,4 @@
-// map_kernels.cu — GPU map build (direct-indexed voxel grid, common.cuh) and the stand-alone exact kNN (sm_100a).
+// map_kernels.cu — GPU map build (direct-indexed voxel grid, common.cuh) and the stand-alone exact kNN (sm_90a).
 //
 //   map build  : replaces pcl::KdTreeFLANN::setInputCloud (lidar_mapper_keyframe.cpp:433-434): a counting sort of the
 //                points by cell over a dense grid — bounding box, per-cell counts (one atomicAdd per point gives its rank

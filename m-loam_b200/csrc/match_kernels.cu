@@ -36,10 +36,10 @@ struct KnnSet {
   unsigned char *heavy_out;       // this launch's verdict, for the next one
 };
 
-// Scheduling of the searches inside a launch.  Queries differ by 10x in cost (a kept neighbour list: ~2.5k cycles, a
-// real search: 10-30k) and a launch is only as fast as its slowest warp, so the few features that needed a real search
+// Scheduling of the searches inside a launch.  Queries differ by about 10x in cost (a kept neighbour list is a re-rank,
+// a real search scans rows of cells) and a launch is only as fast as its slowest warp, so the few features that needed a real search
 // in the previous re-association iteration are listed (atomic append — a few dozen per launch, not one atomic per
-// query: 20k increments of ONE address cost ~1 ns each at the L2 and were the longest part of the launch) and taken
+// query: tens of thousands of increments of ONE address serialise at the L2 and were the longest part of the launch) and taken
 // first, one per warp; everything else is a static stride.  cnt[3] rotates: a launch reads cnt_in, appends to cnt_out
 // and clears cnt_zero for the launch after the next.
 struct HeavyQ {
@@ -51,8 +51,9 @@ struct HeavyQ {
 };
 
 // MB: resident CTAs per SM the kernel is compiled for (register budget 65536 / (256 * MB)).  The search is a chain of
-// dependent warp-wide operations (prefix loads -> point loads -> REDUX / ballot / shuffle rounds): issue slots are only
-// filled when many warps are resident, so the default trades a few spilled registers for twice the warps.
+// dependent warp-wide operations (prefix loads -> point loads -> REDUX / ballot / shuffle rounds).  MB = 3 and 4 buy more
+// resident warps with spilled registers (local-memory round trips inside that chain); on the H100 the spill-free MB = 2
+// variant (106 registers) runs the C2 frame about 9 % faster than MB = 4, so it is the default (Ctx::knn_min_blocks).
 template <int K, int MB>
 __global__ void __launch_bounds__(MWARPS * 32, MB)
     k_match_knn(KnnSet a, KnnSet b, const double *__restrict__ pose7, float min_match_sq_dis, HeavyQ hq,
@@ -329,8 +330,8 @@ int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_
     unsigned *path_stats = (c->prof_on && !getenv("MLOAM_KNN_NO_STATS")) ? reinterpret_cast<unsigned *>(c->scratch[7].as<char>() + kKnnPathStatsOffset) : nullptr;
     unsigned *trace = nullptr;
     if (c->knn_trace_on) {
-      MLOAM_CUDA_OK(c, c->knn_trace.reserve(16 * (size_t)(n_upper + 1) + 16 * 8 * 4 * 148 + 64));
-      MLOAM_CUDA_OK(c, cudaMemsetAsync(c->knn_trace.p, 0, 16 * (size_t)(n_upper + 1) + 16 * 8 * 4 * 148, st));
+      MLOAM_CUDA_OK(c, c->knn_trace.reserve(16 * (size_t)(n_upper + 1) + 16 * (size_t)MWARPS * 4 * c->sm_count + 64));
+      MLOAM_CUDA_OK(c, cudaMemsetAsync(c->knn_trace.p, 0, 16 * (size_t)(n_upper + 1) + 16 * (size_t)MWARPS * 4 * c->sm_count, st));
       trace = c->knn_trace.as<unsigned>();
     }
     const int mb = c->knn_min_blocks;

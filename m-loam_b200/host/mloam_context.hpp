@@ -33,7 +33,7 @@ class ThreadContext {
  private:
   explicit ThreadContext(int device) {
     if (mloam_ctx_create(device, &params(), &ctx_) != MLOAM_OK)
-      throw std::runtime_error("mloam_ctx_create failed: a B200 (sm_100a) device is required — there is no CPU path");
+      throw std::runtime_error("mloam_ctx_create failed: an H100 (sm_90a) device is required — there is no CPU path");
   }
   ~ThreadContext() { mloam_ctx_destroy(ctx_); }
   mloam_ctx_t *ctx_ = nullptr;

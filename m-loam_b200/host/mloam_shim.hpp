@@ -1,6 +1,6 @@
 // mloam_shim.hpp — C++ host side above the C ABI (include/mloam_b200.h): the reference's class surface for the
 // hot path, so that L4/L4' code (Estimator, lidar_mapper process()) keeps compiling against the same names,
-// argument meaning and error behaviour while the work runs in the sm_100a kernels.
+// argument meaning and error behaviour while the work runs in the sm_90a kernels.
 //
 //   reference type / function                                       here
 //   common::PointI, PointICloud (type.h:20-23)                      common::PointI, common::PointICloud (POD stand-ins

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Generate the committed golden fixtures of tests/golden/ (run in the build container, where /root/reference exists).
+"""Generate the committed golden fixtures of tests/golden/ (run where the reference checkout exists and oracle/_ref has been built from it).
 
     python tests/golden/make_golden.py
 
+knn_nanoflann_20k.npz  REFERENCE-DERIVED: the same kd-tree's answers on the seeded 20k-point case of the CPU suite.
 knn_nanoflann.npz   REFERENCE-DERIVED: neighbour indices and float squared distances returned by the reference's own
                     kd-tree (nanoflann.hpp vendored at /root/reference/mloam_loop/include/mloam_loop/scan_context/,
                     compiled in place into oracle/_ref/libref_knn.so) on a seeded map / query set.  This is the one
@@ -34,9 +35,28 @@ def small_case():
     return surf_map, corner_map, cloud, ss, se, init
 
 
+def knn_tree_case():
+    """Seeded 20k-point map and 500 queries of test_oracle_cpu.test_knn_tree_vs_brute_and_reference_nanoflann."""
+    rng = np.random.default_rng(1)
+    m = np.concatenate([rng.uniform(-20, 20, (20000, 3)), np.zeros((20000, 1))], 1).astype(np.float32)
+    q = np.concatenate([rng.uniform(-20, 20, (500, 3)), np.zeros((500, 1))], 1).astype(np.float32)
+    return m, q
+
+
+def make_knn_tree_fixture():
+    """knn_nanoflann_20k.npz: the reference nanoflann's answers on knn_tree_case() (the inputs are regenerated from the seed;
+    their first rows are stored so that a change of the generator is caught)."""
+    m, q = knn_tree_case()
+    out = {"map_head": m[:8], "query_head": q[:8]}
+    for k in (1, 5, 10):
+        out[f"idx{k}"], out[f"sqd{k}"] = orc.ref_knn(m, q, k)
+    np.savez_compressed(os.path.join(HERE, "knn_nanoflann_20k.npz"), **out)
+
+
 def main():
     # ---- reference nanoflann
-    assert orc.ref_lib() is not None, "oracle/_ref/libref_knn.so missing: run `make -C oracle ref` where /root/reference exists"
+    assert orc.ref_lib() is not None, "oracle/_ref/libref_knn.so missing: run `make -C oracle ref` where the reference checkout exists"
+    make_knn_tree_fixture()
     rng = np.random.default_rng(2024)
     m = np.concatenate([rng.uniform(-8, 8, (6000, 3)), np.zeros((6000, 1))], 1).astype(np.float32)
     q = np.concatenate([rng.uniform(-8.5, 8.5, (300, 3)), np.zeros((300, 1))], 1).astype(np.float32)
@@ -66,7 +86,7 @@ def main():
     import synthetic as syn
     surf_f, corner_f = syn.keyframe_map_features(syn.make_scene(), orc.extract_cloud, orc.voxel_grid, use_cache=False)
     np.savez_compressed(os.path.join(HERE, "submap_keyframes_filtered.npz"), surf=surf_f, corner=corner_f, tag=f"{syn.SEED}_30_64x2048")
-    for name in ("knn_nanoflann.npz", "oracle_small.npz", "submap_keyframes_filtered.npz"):
+    for name in ("knn_nanoflann.npz", "knn_nanoflann_20k.npz", "oracle_small.npz", "submap_keyframes_filtered.npz"):
         print(name, os.path.getsize(os.path.join(HERE, name)), "bytes")
 
 

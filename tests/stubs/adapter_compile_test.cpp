@@ -1,6 +1,6 @@
 // Compile check of m-loam_b200/host/mloam_adapter.hpp against the stub third-party headers in this directory: instantiates every class
 // and template with the reference's call shapes (lidar_tracker.cpp:27-99, lidar_mapper.h:193-283, estimator.cpp:696-779,1135-1149).
-// It is compiled and linked (against libmloam_b200.so), never run: the calls need a B200.
+// It is compiled and linked (against libmloam_b200.so), never run: the calls need an H100.
 #include <Eigen/Dense>
 #include <ceres/ceres.h>
 #include <pcl/point_cloud.h>

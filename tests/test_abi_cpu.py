@@ -1,4 +1,4 @@
-"""CPU tests: the C-ABI library builds for sm_100a, loads, and exports every symbol include/mloam_b200.h declares;
+"""CPU tests: the C-ABI library builds for sm_90a, loads, and exports every symbol include/mloam_b200.h declares;
 without a device, context creation fails loudly (no CPU fallback)."""
 import os
 import re
@@ -15,7 +15,7 @@ def test_library_loads_and_exports_header_symbols(mloam):
     for sym in declared:
         assert hasattr(lib, sym), f"{sym} declared in include/mloam_b200.h but not exported"
     assert set(declared) == set(mloam.ABI_SYMBOLS)
-    assert b"sm_100a" in lib.mloam_version()
+    assert b"sm_90a" in lib.mloam_version()
 
 
 def test_struct_layouts_match_defaults(mloam):
@@ -51,12 +51,12 @@ def test_no_device_fails_loudly(mloam):
         mloam.Context(0)
 
 
-def test_only_sm100a_sass_is_embedded(mloam):
+def test_only_sm90a_sass_is_embedded(mloam):
     import subprocess
 
     out = subprocess.run(["/usr/local/cuda/bin/cuobjdump", "-lelf", mloam.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_cpp_host_shim_compiles_links_and_refuses_to_run_without_gpu(mloam):

@@ -85,7 +85,7 @@ def test_two_gpu_frame_parity(exchange):
     import torch
 
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs (run tests/multi_gpu_check.py under torchrun with gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs (tests/multi_gpu_check.py runs it under torchrun)")
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
            "--master-port", "29533" if exchange == "p2p" else "29534", os.path.join(ROOT, "tests", "multi_gpu_check.py")]
     out = subprocess.run(cmd, capture_output=True, text=True, timeout=600, env=dict(os.environ, MLOAM_EXCHANGE=exchange))
@@ -98,7 +98,7 @@ def test_two_gpu_calibration_parity():
     import torch
 
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs (run tests/multi_gpu_calib_check.py under torchrun with gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs (tests/multi_gpu_calib_check.py runs it under torchrun)")
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
            "--master-port", "29541", os.path.join(ROOT, "tests", "multi_gpu_calib_check.py")]
     out = subprocess.run(cmd, capture_output=True, text=True, timeout=600)

@@ -18,13 +18,18 @@ def rand_pose(rng):
 
 
 def test_knn_tree_vs_brute_and_reference_nanoflann():
-    rng = np.random.default_rng(1)
-    m = np.concatenate([rng.uniform(-20, 20, (20000, 3)), np.zeros((20000, 1))], 1).astype(np.float32)
-    q = np.concatenate([rng.uniform(-20, 20, (500, 3)), np.zeros((500, 1))], 1).astype(np.float32)
+    """Oracle kd-tree vs brute force vs the reference's own nanoflann: its answers are stored in
+    tests/golden/knn_nanoflann_20k.npz (make_golden.py), and compared live as well where oracle/_ref is built."""
+    from golden.make_golden import knn_tree_case
+
+    m, q = knn_tree_case()
+    g = np.load(os.path.join(GOLDEN, "knn_nanoflann_20k.npz"))
+    assert np.array_equal(m[:8], g["map_head"]) and np.array_equal(q[:8], g["query_head"])
     for k in (1, 5, 10):
         i_t, d_t = orc.knn(m, q, k)
         i_b, d_b = orc.knn(m, q, k, brute=True)
         assert np.array_equal(i_t, i_b) and np.array_equal(d_t, d_b)
+        assert np.array_equal(i_t, g[f"idx{k}"]) and np.array_equal(d_t, g[f"sqd{k}"])
         if orc.ref_lib() is not None:  # the reference's vendored nanoflann, compiled where it lies
             i_r, d_r = orc.ref_knn(m, q, k)
             assert np.array_equal(d_t, d_r)

@@ -89,7 +89,7 @@ def seeded_trace():
     ms, k = ctx.profile_get("match")
     print(f"scan2map: k_match_knn {1e3 * ms / max(k, 1):7.1f} us avg over {k} launches; features corner {corner.shape[0]} surf {surf.shape[0]}")
     n = corner.shape[0] + surf.shape[0]
-    nw = 8 * 4 * 148
+    nw = 8 * 4 * torch.cuda.get_device_properties(0).multi_processor_count
     full = np.zeros((n + 1 + nw, 4), np.uint32)
     rc = m.lib().mloam_debug_knn_trace(ctx._h, full.ctypes.data_as(C.c_void_p), n + 1 + nw)
     tr = full[:n]
