@@ -149,7 +149,7 @@ void mloam_ctx_destroy(mloam_ctx_t *h) {
   }
   for (int i = 0; i < 4; i++) c->scan_pts[i].release(), c->feat_valid[i].release(), c->feat_coeff[i].release(), c->feat_nn[i].release(), c->knn_pos[i].release(), c->knn_changed[i].release(), c->knn_anchor[i].release(), c->knn_heavy[i].release();
   for (int i = 0; i < 2; i++) c->gf_work[i].release();
-  c->knn_heavy_list.release(), c->knn_trace.release();
+  c->knn_heavy_list.release(), c->knn_trace.release(), c->knn_spec.release();
   c->partials.release(), c->lm_state.release();
   for (auto &s : c->scratch) s.release();
   c->frame_main.release(), c->frame_alt.release(), c->next_in.release(), c->stamps.release();

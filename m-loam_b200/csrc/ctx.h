@@ -24,11 +24,22 @@ struct FitSet {
   int n;
   const int *d_n;
   const int *pos;        // n * K from k_match_knn
+  int half;              // double-buffered lists (SpecState): features per half, half 1 starts at pos + half * K; 0: one buffer
   unsigned char *valid;  // out
   float *coeff;          // out: n * 6
   int *nn;               // out (nullable): n * K original map indices
   int is_plane;
   const unsigned char *changed;  // nullable: 0 -> same neighbours as the previous iteration, valid/coeff already hold the fit
+};
+// Speculative re-association (plain scan2map, max_inner == 1, one GPU): the matcher of GN iteration i + 1 searches at the
+// candidate pose of iteration i while that candidate is evaluated.  The neighbour lists and anchors are double-buffered; the
+// matcher reads half `sel` and writes the other one.  The next evaluation at x decides on the device which half is valid:
+// the lists matched at xc are the right ones iff x == xc bitwise (the step was taken); otherwise x did not move, the lists of
+// half `sel` still hold, and so do valid / coeff.  Written by the k_linearize tail only, read by k_match_knn / k_linearize.
+struct SpecState {
+  double xc[7];  // pose the next matcher searches at: the candidate of the last mode-1 tail (x at the start of a solve)
+  int sel;       // half of the lists / anchors valid at LMState::x (before the evaluation at x commits the speculation); 0 at solve start
+  int pad;
 };
 // A fit whose launch the matcher left to the first evaluation of the solve (k_linearize pass 0)
 struct PendingFit {
@@ -142,6 +153,7 @@ struct Ctx {
   DevBuf knn_pos[4];              // int[n_neigh] per query: neighbour positions handed from k_match_knn to k_match_fit
   DevBuf knn_changed[4];          // unsigned char per query: neighbour list differs from the previous iteration's
   DevBuf knn_anchor[4];           // float4 per query: position of its last real search + tolerated displacement
+  DevBuf knn_spec;                // SpecState of the speculative scan2map schedule
   DevBuf gf_work[2];              // good-feature selection scratch per set (Jacobian rows, pool tree, mask, ...)
   DevBuf knn_heavy[4];            // 2 x unsigned char per query: "needed a real search" verdicts of the last two launches
   DevBuf knn_heavy_list;          // 3 rotating counters + 2 lists of feature indices that needed a real search (match_kernels.cu HeavyQ)
@@ -236,6 +248,8 @@ struct Ctx {
                                    // (grid barrier between them); MLOAM_FUSE_ITER=0 restores the three launches
   PendingFit pending_fit;          // set by match_pair_device(defer_fit), consumed by the next linearize_device(lm_mode 1)
   bool lin_two_pass = false;       // request (scan2map_enqueue) -> linearize_device clears it when it could not honour it
+  SpecState *lin_spec = nullptr;   // scan2map_enqueue -> the next linearize_device(lm_mode 1): commit the speculation (SpecState) ...
+  bool lin_spec_publish = false;   // ... and publish the new candidate for the next matcher
   int want_eig = 1;                // k_lm mode 1: always run the 6x6 eigen-solver (1) or only when degenerate (0)
   bool lidar_merge = false;        // mloam_set_lidars was given extrinsics: features go through the rig merge (also for one LiDAR)
   int n_lidars = 1;                // LiDARs batched into one frame of this context (mloam_set_lidars)
@@ -298,8 +312,9 @@ struct MatchJob {
 };
 // buf_base: which pair of the context's per-set buffers (knn_pos / knn_anchor / ...) the jobs use: 0 (sets 0, 1) or 2 (sets 2, 3)
 // defer_fit: skip the fit launch and leave the fit to the next linearize_device(lm_mode 1) on this context (Ctx::pending_fit)
+// d_sel (speculative schedule, with defer_fit): double-buffered lists, read half *d_sel and write the other (SpecState::sel)
 int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_pose7, const MatchCfg &cfg, int *d_work, int buf_base = 0,
-                      bool defer_fit = false);
+                      bool defer_fit = false, const int *d_sel = nullptr);
 
 // track_kernels.cu
 int match_from_scan_device(Ctx *c, int slot, int type, const float4 *d_pts, int n, const double *d_pose7, unsigned char *d_valid,
@@ -324,7 +339,12 @@ struct FeatSet {
 //   0: none (partials only, reduced into d_out28 if non-null)   1: begin Solve   2: iterate
 int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, const double *d_pose7,
                      int use_state, int lm_mode, double *d_out29);
-int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, double eig_thre);
+// Evaluation at LMState::xc + the acceptance step (mode 2) of a solve with max_inner == 1, as the second pass of
+// k_linearize computes it, but accumulating only g, cost and row counts (H at xc is never read with one LM iteration).
+// Small blocks with a register cap, so that it runs beside the speculative matcher of the next GN iteration.
+int eval_candidate_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a);
+// spec (nullable): also start SpecState::xc at the initial pose
+int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, double eig_thre, SpecState *spec = nullptr);
 void eig_report_host(const double *H36, double *w6);  // ascending eigenvalues of a symmetric 6x6 (host side)
 int factor_evaluate_device(Ctx *c, int kind, int n, const double *d_points, const double *d_coeffs, const double *d_sqrt_info,
                            const double *d_params, double *d_res, double *d_jac);

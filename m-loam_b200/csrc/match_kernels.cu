@@ -32,6 +32,7 @@ struct KnnSet {
   int seeded;          // pos holds this set's result of the previous re-association iteration on the SAME map
   unsigned char *changed;  // out (nullable): 1 when the neighbour list differs from the seed (or there was none)
   float4 *anchor;      // per feature: map-frame position of its last real search + the displacement it tolerates
+  int half;            // double-buffered pos / anchor (SpecState): features per half; 0: read and write in place
   const unsigned char *heavy_in;  // nullable: 1 where the previous launch had to search (ball / blind) — those go first
   unsigned char *heavy_out;       // this launch's verdict, for the next one
 };
@@ -56,7 +57,7 @@ struct HeavyQ {
 // variant (106 registers) runs the C2 frame about 9 % faster than MB = 4, so it is the default (Ctx::knn_min_blocks).
 template <int K, int MB>
 __global__ void __launch_bounds__(MWARPS * 32, MB)
-    k_match_knn(KnnSet a, KnnSet b, const double *__restrict__ pose7, float min_match_sq_dis, HeavyQ hq,
+    k_match_knn(KnnSet a, KnnSet b, const double *__restrict__ pose7, float min_match_sq_dis, HeavyQ hq, const int *__restrict__ d_sel,
                 unsigned *__restrict__ path_stats, unsigned tma_min, unsigned *__restrict__ trace) {
   __shared__ KnnSmem ksm[MWARPS];
   const int lane = threadIdx.x & 31;
@@ -71,6 +72,7 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
   const int na = a.d_n ? min(a.n, *a.d_n) : a.n;
   const int nb = b.d_n ? min(b.n, *b.d_n) : b.n;
   const int n = na + nb;
+  const int h_in = d_sel ? (*d_sel & 1) : 0;  // double-buffered sets: read half h_in, write the other
   // Schedule: first the listed heavy features of the previous launch (one per warp), then a static stride over the rest.
   const int gw = blockIdx.x * MWARPS + (threadIdx.x >> 5), n_warps = gridDim.x * MWARPS;
   if (hq.cnt_zero && gw == 0 && lane == 0) *hq.cnt_zero = 0;
@@ -98,10 +100,13 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
     const float3 sel = associate(s_pose, p.x, p.y, p.z);  // pointAssociateToMap, utility.h:103-117
     const GridP &g = s_grid[in_a ? 0 : 1];
     Best best;  // selection width K + 1: lane K holds the nearest scanned point outside the K-set (feeds the anchor's slack)
-    int *const pos_out = (in_a ? a.pos : b.pos) + (size_t)j * K;
+    const int hs = in_a ? a.half : b.half, o_in = h_in ? hs : 0, o_out = hs - o_in;
+    const int *const pos_in = (in_a ? a.pos : b.pos) + (size_t)(j + o_in) * K;
+    int *const pos_out = (in_a ? a.pos : b.pos) + (size_t)(j + o_out) * K;
     const int seeded = in_a ? a.seeded : b.seeded;
     unsigned char *const changed = in_a ? a.changed : b.changed;
-    float4 *const anchor = (in_a ? a.anchor : b.anchor) + j;
+    const float4 *const anchor_in = (in_a ? a.anchor : b.anchor) + j + o_in;
+    float4 *const anchor = (in_a ? a.anchor : b.anchor) + j + o_out;  // every query writes its complete state to the out half
     // Temporal coherence between re-association iterations (all three shortcuts are exact, see knn.cuh):
     //   keep    the query moved less than the anchor's slack since its last real search: the K-set cannot have
     //           changed, only its order — recompute the K distances and re-rank (no cell probes, no scan)
@@ -111,8 +116,8 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
     bool done = false;
     float r2 = 3.0e38f;
     if (seeded) {
-      if (lane < K) prev = pos_out[lane];
-      const float4 an = *anchor;
+      if (lane < K) prev = pos_in[lane];
+      const float4 an = *anchor_in;
       const float mx = sel.x - an.x, my = sel.y - an.y, mz = sel.z - an.z;
       const float moved = sqrtf(mx * mx + my * my + mz * mz);
       const bool within = an.w > 0.0f && moved + 2e-5f < an.w;
@@ -121,6 +126,7 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
         if (within) {
           done = true;
           path = 1;
+          if (lane == 0 && o_out != o_in) *anchor = an;
         }
       } else {
         unsigned long long key = MLOAM_KEY_NONE;
@@ -147,6 +153,8 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
           if (!(r2 < min_match_sq_dis)) {  // :407,571,667,814 — the slack of a match says nothing about a rejection
             newpos = -1;
             if (lane == 0) *anchor = make_float4(sel.x, sel.y, sel.z, 0.0f);
+          } else if (lane == 0 && o_out != o_in) {
+            *anchor = an;
           }
           done = true;
           path = 0;
@@ -248,7 +256,8 @@ __global__ void __launch_bounds__(128) k_match_fit(FitSet a, FitSet b, const dou
 // ------------------------------------------------------------------------------------------------ launchers
 // Match up to two feature sets (corner against MLOAM_MAP_CORNER-like slot, surf against a surf slot) in one
 // kNN launch + one fit launch.  Sets with n == 0 are skipped.
-int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_pose7, const MatchCfg &cfg, int *d_work, int buf_base, bool defer_fit) {
+int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_pose7, const MatchCfg &cfg, int *d_work, int buf_base, bool defer_fit,
+                      const int *d_sel) {
   (void)d_work;
   if (n_jobs < 1 || n_jobs > 2 || (buf_base != 0 && buf_base != 2)) {
     c->err = "match: 1 or 2 jobs";
@@ -279,14 +288,16 @@ int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_
       return MLOAM_E_INVALID;
     }
     DevBuf &pb = c->knn_pos[buf_base + t];
-    MLOAM_CUDA_OK(c, pb.reserve(sizeof(int) * (size_t)K * (size_t)(J.n + 1)));
+    const int halves = d_sel ? 2 : 1;  // double-buffered (speculative schedule): half 1 follows half 0
+    MLOAM_CUDA_OK(c, pb.reserve(sizeof(int) * (size_t)K * (size_t)(J.n + 1) * halves));
     k.map = c->maps[J.slot].view();
     DevBuf &cb = c->knn_changed[buf_base + t];
     MLOAM_CUDA_OK(c, cb.reserve((size_t)(J.n + 1)));
     k.pts = J.pts, k.n = J.n, k.d_n = J.d_n, k.pos = pb.as<int>();
     DevBuf &ab = c->knn_anchor[buf_base + t];
-    MLOAM_CUDA_OK(c, ab.reserve(sizeof(float4) * (size_t)(J.n + 1)));
+    MLOAM_CUDA_OK(c, ab.reserve(sizeof(float4) * (size_t)(J.n + 1) * halves));
     k.seeded = J.seeded, k.changed = cb.as<unsigned char>(), k.anchor = ab.as<float4>();
+    k.half = d_sel ? J.n + 1 : 0;
     // search verdicts ("had to search") alternate between two halves from launch to launch: read the previous, write the next
     DevBuf &hb = c->knn_heavy[buf_base + t];
     const size_t half = ((size_t)J.n + 256) & ~(size_t)255;
@@ -295,9 +306,13 @@ int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_
     k.heavy_out = hb.as<unsigned char>() + half * (size_t)(J.seeded ? (c->knn_parity ^ 1) : c->knn_parity);
     flip = flip || J.seeded;
     f.changed = (J.seeded && !J.nn) ? cb.as<unsigned char>() : nullptr;
-    f.sorted = k.map.sorted, f.pts = J.pts, f.n = J.n, f.d_n = J.d_n, f.pos = pb.as<int>();
+    f.sorted = k.map.sorted, f.pts = J.pts, f.n = J.n, f.d_n = J.d_n, f.pos = pb.as<int>(), f.half = k.half;
     f.valid = J.valid, f.coeff = J.coeff, f.nn = J.nn, f.is_plane = J.type == 's' ? 1 : 0;
     n_upper += J.n;
+  }
+  if (d_sel && (!defer_fit || fs[0].nn || fs[1].nn)) {  // only the deferred fit knows which half is valid
+    c->err = "match: double-buffered lists need the deferred fit";
+    return MLOAM_E_STATE;
   }
   if (n_upper <= 0) return MLOAM_OK;
   // heavy list of the launch: 2 lists x n_upper ints + 3 rotating counters (zeroed with the buffer; k_lm_init re-zeroes
@@ -338,7 +353,7 @@ int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_
     int nb = (n_upper + MWARPS - 1) / MWARPS;
     if (nb > mb * c->sm_count) nb = mb * c->sm_count;  // all CTAs resident; warps pull / stride over the features
 #define MLOAM_LAUNCH_KNN(KK, MBB) \
-  k_match_knn<KK, MBB><<<nb, MWARPS * 32, 0, st>>>(ks[0], ks[1], d_pose7, cfg.min_match_sq_dis, hq, path_stats, c->knn_tma_min, trace)
+  k_match_knn<KK, MBB><<<nb, MWARPS * 32, 0, st>>>(ks[0], ks[1], d_pose7, cfg.min_match_sq_dis, hq, d_sel, path_stats, c->knn_tma_min, trace)
     if (K == 5) {
       if (mb == 2) MLOAM_LAUNCH_KNN(5, 2);
       else if (mb == 3) MLOAM_LAUNCH_KNN(5, 3);

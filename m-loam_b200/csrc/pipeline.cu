@@ -39,10 +39,20 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7) {
   if (rc) return rc;
   rc = reserve_feat(c, 1, S.n_surf);
   if (rc) return rc;
-  rc = lm_init_state(c, pose_init7, P.max_inner, P.eig_thre);
+  // Speculative re-association (one LM iteration per GN iteration, no good-feature selection, one GPU): GN iteration i + 1's
+  // matcher needs only the pose it searches at, which is the candidate xc_i whenever iteration i's step is taken.  So it starts
+  // as soon as the evaluation at x_i has produced xc_i, next to the evaluation at xc_i that decides the step; the evaluation at
+  // x_{i+1} then takes its lists when x_{i+1} == xc_i, or keeps iteration i's lists and fit (SpecState).
+  const bool spec = c->fuse_iter && P.max_inner == 1 && P.gf_method == 0 && !c->nccl_comm;
+  SpecState *d_spec = nullptr;
+  if (spec) {
+    MLOAM_CUDA_OK(c, c->knn_spec.reserve(sizeof(SpecState)));
+    d_spec = c->knn_spec.as<SpecState>();
+  }
+  rc = lm_init_state(c, pose_init7, P.max_inner, P.eig_thre, d_spec);
   if (rc) return rc;
   LMState *st = c->lm_state.as<LMState>();
-  const double *d_pose = st->x;  // first member
+  const double *d_pose = spec ? d_spec->xc : st->x;  // where the matcher searches
   const double sinfo = map_sqrt_info(P.cov_trace);
   const MatchCfg cfg = match_cfg(c);
   int *h_done = reinterpret_cast<int *>(reinterpret_cast<char *>(c->pinned) + 2048);
@@ -50,20 +60,23 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7) {
   FeatSet sets[2] = {
       FeatSet{S.corner, c->feat_valid[0].as<unsigned char>(), c->feat_coeff[0].as<float>(), nc_use, 0, S.d_n_corner, S.sinfo_corner},
       FeatSet{S.surf, c->feat_valid[1].as<unsigned char>(), c->feat_coeff[1].as<float>(), ns_use, 1, S.d_n_surf, S.sinfo_surf}};
+  // :503-532  match corner then surf at pose_wmap_curr (wo_gf: every feature)
+  auto match = [&](int outer) {
+    // From the second iteration on the same features meet the same maps at a slightly moved pose: the previous
+    // neighbour lists seed the search (exact, see knn.cuh) and unchanged lists keep their line / plane fit.
+    const int seeded = (outer > 0 && c->use_seeds) ? 1 : 0;
+    MatchJob jobs[2] = {
+        MatchJob{MLOAM_MAP_CORNER, 'c', S.corner, nc_use, S.d_n_corner, c->feat_valid[0].as<unsigned char>(),
+                 c->feat_coeff[0].as<float>(), nullptr, seeded},
+        MatchJob{MLOAM_MAP_SURF, 's', S.surf, ns_use, S.d_n_surf, c->feat_valid[1].as<unsigned char>(),
+                 c->feat_coeff[1].as<float>(), nullptr, seeded}};
+    // without good-feature selection nothing reads the fit before the solve: its launch folds into the first evaluation
+    const bool defer_fit = c->fuse_iter && P.gf_method == 0;
+    return match_pair_device(c, jobs, 2, d_pose, cfg, &st->work[0], 0, defer_fit, spec ? &d_spec->sel : nullptr);
+  };
   for (int outer = 0; outer < P.max_outer; outer++) {
-    // :503-532  match corner then surf at pose_wmap_curr (wo_gf: every feature)
-    {
-      // From the second iteration on the same features meet the same maps at a slightly moved pose: the previous
-      // neighbour lists seed the search (exact, see knn.cuh) and unchanged lists keep their line / plane fit.
-      const int seeded = (outer > 0 && c->use_seeds) ? 1 : 0;
-      MatchJob jobs[2] = {
-          MatchJob{MLOAM_MAP_CORNER, 'c', S.corner, nc_use, S.d_n_corner, c->feat_valid[0].as<unsigned char>(),
-                   c->feat_coeff[0].as<float>(), nullptr, seeded},
-          MatchJob{MLOAM_MAP_SURF, 's', S.surf, ns_use, S.d_n_surf, c->feat_valid[1].as<unsigned char>(),
-                   c->feat_coeff[1].as<float>(), nullptr, seeded}};
-      // without good-feature selection nothing reads the fit before the solve: its launch folds into the first evaluation
-      const bool defer_fit = c->fuse_iter && P.gf_method == 0;
-      rc = match_pair_device(c, jobs, 2, d_pose, cfg, &st->work[0], 0, defer_fit);
+    if (!spec || outer == 0) {  // speculative: the previous iteration enqueued this one's matcher
+      rc = match(outer);
       if (rc) return rc;
       stamp(c, "match");
     }
@@ -94,14 +107,38 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7) {
     // :537-582 residual blocks + Evaluate -> J^T J -> evalDegenracy, and iteration 0 of ceres::Solve.  The device
     // only needs the degeneracy decision; scan2map_finish fills in the eigenvalue report of the last iteration.
     if (P.gf_method != 0) stamp(c, "gf");
+    const bool speculate = spec && outer + 1 < P.max_outer;  // the last iteration has no next matcher to start early
     c->want_eig = 0;
-    c->lin_two_pass = c->fuse_iter && P.max_inner == 1;  // the one LM iteration's second evaluation rides in the same launch
+    // the one LM iteration's second evaluation rides in the same launch, unless it goes next to the speculative matcher
+    c->lin_two_pass = c->fuse_iter && P.max_inner == 1 && !speculate;
+    c->lin_spec = d_spec, c->lin_spec_publish = speculate;
     rc = linearize_device(c, sets, 2, sinfo, P.huber_a, nullptr, 1, 1, nullptr);
     c->want_eig = 1;
     const bool second_done = c->lin_two_pass;
-    c->lin_two_pass = false;
+    c->lin_two_pass = false, c->lin_spec = nullptr, c->lin_spec_publish = false;
     if (rc) return rc;
     stamp(c, second_done ? "linearize x2" : "linearize");
+    if (speculate) {
+      // fork: {matcher of iteration outer + 1 at the published candidate} || {evaluation at the candidate + acceptance}.  The
+      // branches share only read-only inputs: the matcher writes the spare half of the lists, the changed and heavy flags; the
+      // evaluation writes LMState and the partials.  With stage profiling on they stay serial, like the other forks.
+      const bool fork = !c->prof_on;
+      if (fork) {
+        MLOAM_CUDA_OK(c, cudaEventRecord(c->ev_fork3, c->stream));
+        MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream3, c->ev_fork3, 0));
+      }
+      cudaStream_t main_stream = c->stream;
+      if (fork) c->stream = c->stream3;
+      rc = match(outer + 1);
+      c->stream = main_stream;
+      if (rc) return rc;
+      if (fork) MLOAM_CUDA_OK(c, cudaEventRecord(c->ev_join3, c->stream3));
+      rc = eval_candidate_device(c, sets, 2, sinfo, P.huber_a);
+      if (rc) return rc;
+      if (fork) MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream, c->ev_join3, 0));
+      stamp(c, "match || candidate");
+      continue;
+    }
     // :586-596 ceres::Solve, at most max_inner LM iterations; the device raises `done`
     for (int it = 0; it < P.max_inner && !second_done; it++) {
       rc = linearize_device(c, sets, 2, sinfo, P.huber_a, nullptr, 2, 2, nullptr);

@@ -54,7 +54,32 @@ struct LinArgs {
   FitSet fit[2];
   float fit_min_plane_dis;
   int fit_check_fov;
+  // speculative schedule (SpecState, with the deferred fit): fit from the lists matched at spec->xc only when x is that pose,
+  // commit the choice in the tail and, with spec_publish, hand the new candidate to the next matcher
+  SpecState *spec;
+  int spec_publish;
 };
+
+// Loss-corrected row of one point-to-plane / point-to-line feature at pose P: returns r and scales J by sqrt(rho'(r^2)); *rho = Huber(r^2).
+__device__ __forceinline__ double map_factor_row(const PoseR &P, const FeatSetDev &fs, int i, double sqrt_info, double huber_a, double *J,
+                                                 double *rho) {
+  const float4 pf = __ldg(fs.pts + i);
+  const D3 p{(double)pf.x, (double)pf.y, (double)pf.z};
+  const float *cf = fs.coeff + (size_t)i * 6;
+  const double si = fs.sinfo ? fs.sinfo[i] : sqrt_info;  // per-feature weight when mapping is uncertainty-aware
+  double r;
+  if (fs.is_plane) {
+    r = plane_factor(P, p, D3{(double)cf[0], (double)cf[1], (double)cf[2]}, (double)cf[3], si, J, true);
+  } else {
+    r = edge_factor(P, p, D3{(double)cf[0], (double)cf[1], (double)cf[2]}, D3{(double)cf[3], (double)cf[4], (double)cf[5]}, si, J, true);
+  }
+  double rho1;
+  huber(huber_a, r * r, rho, &rho1);
+  const double sc = sqrt(rho1);
+#pragma unroll
+  for (int k = 0; k < 6; k++) J[k] = sc * J[k];
+  return sc * r;
+}
 
 __device__ __noinline__ void lm_tail(const double *partials, int n_blocks, LMState *gst, int mode, double eig_thre, int want_eig, double *out_ne,
                                      const P2PView *p2p);
@@ -70,6 +95,15 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
   }
   volatile unsigned *const gen = a.ticket + 1;
   const unsigned gen0 = a.two_pass ? *gen : 0u;  // read before this block's ticket: the release cannot have happened yet
+  // speculative schedule: the lists the last matcher wrote (half sel ^ 1) were matched at spec->xc; they are the lists at x iff
+  // x is that pose bit for bit (the step was taken).  Otherwise x did not move and the lists, valid and coeff of half sel stand.
+  int spec_sel = 0;
+  bool spec_hit = true;
+  if (a.spec) {
+    spec_sel = a.spec->sel & 1;  // read as k_match_knn reads it
+#pragma unroll
+    for (int k = 0; k < 7; k++) spec_hit = spec_hit && __double_as_longlong(a.state->x[k]) == __double_as_longlong(a.spec->xc[k]);
+  }
 #pragma unroll 1
   for (int pass = 0; pass < (a.two_pass ? 2 : 1); pass++) {
   double xs[7];
@@ -110,17 +144,18 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
     // the last thread downwards, so that a thread evaluates one feature of either set instead of one of each.
     const int G = gridDim.x * blockDim.x, gid = blockIdx.x * blockDim.x + threadIdx.x;
     for (int i = (s & 1) ? G - 1 - gid : gid; i < fn; i += G) {
-      if (KFIT > 0 && pass == 0 && a.fit[s].pos) {  // deferred fit: this thread is the only one that touches feature i
+      if (KFIT > 0 && pass == 0 && a.fit[s].pos && spec_hit) {  // deferred fit: this thread is the only one that touches feature i
+        constexpr int KF = KFIT > 0 ? KFIT : 5;
         const PoseD T = pose_from_param(xs);
-        fit_one<(KFIT > 0 ? KFIT : 5)>(a.fit[s], i, T, a.fit_min_plane_dis, a.fit_check_fov);
+        FitSet f = a.fit[s];
+        f.pos += (size_t)(spec_sel ^ 1) * f.half * KF;  // half 0 when the lists are not double-buffered (f.half == 0)
+        fit_one<KF>(f, i, T, a.fit_min_plane_dis, a.fit_check_fov);
       }
       if (!fs.valid[i] || (fs.mask && !fs.mask[i])) continue;
-      const float4 pf = __ldg(fs.pts + i);
-      const D3 p{(double)pf.x, (double)pf.y, (double)pf.z};
-      const float *cf = fs.coeff + (size_t)i * 6;
-      double J[6];
-      double r;
       if (fs.is_plane == 2) {
+        const float4 pf = __ldg(fs.pts + i);
+        const D3 p{(double)pf.x, (double)pf.y, (double)pf.z};
+        const float *cf = fs.coeff + (size_t)i * 6;
         // LidarScanEdgeFactorVector (tracker, lidar_tracker.cpp:89): one 3-row residual BLOCK, the loss acts on
         // its squared norm (Ceres applies rho per block)
         double r3[3], J3[18];
@@ -148,19 +183,8 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
         else acc[NE_H + NE_G + 2] += 1.0;
         continue;
       }
-      const double si = fs.sinfo ? fs.sinfo[i] : a.sqrt_info;  // per-feature weight when mapping is uncertainty-aware
-      if (fs.is_plane) {
-        r = plane_factor(P, p, D3{(double)cf[0], (double)cf[1], (double)cf[2]}, (double)cf[3], si, J, true);
-      } else {
-        r = edge_factor(P, p, D3{(double)cf[0], (double)cf[1], (double)cf[2]}, D3{(double)cf[3], (double)cf[4], (double)cf[5]},
-                        si, J, true);
-      }
-      double rho, rho1;
-      huber(a.huber_a, r * r, &rho, &rho1);
-      const double sc = sqrt(rho1);
-      r = sc * r;
-#pragma unroll
-      for (int k = 0; k < 6; k++) J[k] = sc * J[k];
+      double J[6], rho;
+      const double r = map_factor_row(P, fs, i, a.sqrt_info, a.huber_a, J, &rho);
       int q = 0;
 #pragma unroll
       for (int i0 = 0; i0 < 6; i0++)
@@ -216,6 +240,11 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
   __threadfence();  // the state (written by all threads of this block) before the ticket reset and the release
   __syncthreads();
   if (threadIdx.x == 0) {
+    if (a.spec && pass == 0) {  // every block has read sel and fitted: commit, and publish where the next matcher searches
+      if (spec_hit) a.spec->sel = spec_sel ^ 1;
+      if (a.spec_publish)
+        for (int k = 0; k < 7; k++) a.spec->xc[k] = __ldcg(&a.state_rw->xc[k]);
+    }
     *a.ticket = 0u;
     if (a.two_pass && pass == 0) {
       __threadfence();
@@ -639,8 +668,127 @@ __global__ void __launch_bounds__(LM_THREADS) k_lm(const double *__restrict__ pa
   lm_tail(partials, n_blocks, st, mode, eig_thre, want_eig, out_ne, nullptr);
 }
 
-__global__ void k_lm_init(LMState *st, const double *pose7, int max_inner, int min_corr) {
+// ---------------------------------------------------------------------------------------- candidate evaluation
+// k_eval_candidate: pass 1 of k_linearize (evaluation at xc + mode-2 tail) for a solve with max_inner == 1, in blocks small
+// enough to run beside the speculative matcher: two k_match_knn CTAs (2 x 256 threads x 112 allocated registers = 57344)
+// leave 8192 registers of an SM, i.e. one block of 64 threads at <= 128 registers.  H at xc is never read with one LM
+// iteration (the next Solve's mode 1 overwrites LMState::H, the stats report H0), so only g, cost and the row counts are
+// accumulated.  Bit-identical to k_linearize: a thread evaluates the same features (blocks of 64 tile k_linearize's blocks of
+// 256), the per-component warp butterfly is the same addition tree as k_linearize's packed one, and the tail adds the warp
+// sums in k_linearize's order (8 warps per block, then lm_tail's fixed order over the blocks).
+constexpr int CAND_THREADS = 64;
+constexpr int NE_CAND = 9;  // g | cost | rows(set 0) | rows(set 1) = NE_PACK components 21..29
+constexpr int LIN_WARPS = LIN_THREADS / 32;
+
+__device__ __noinline__ void cand_tail(const double *wsums, int n_lin_blocks, LMState *gst, double eig_thre) {
+  __shared__ double bsum[64][NE_CAND];       // per k_linearize block (n_lin_blocks <= 64)
+  __shared__ double vsum[LM_THREADS / 32][NE_CAND];
+  __shared__ double ne[NE_PACK];
+  __shared__ LMState s;
+  constexpr int kWords = (int)(sizeof(LMState) / 8);
+  const long long t0 = clock64();
+  {
+    const unsigned long long *src = reinterpret_cast<const unsigned long long *>(gst);
+    unsigned long long *dst = reinterpret_cast<unsigned long long *>(&s);
+    for (int k = threadIdx.x; k < kWords; k += CAND_THREADS) dst[k] = __ldcg(src + k);
+  }
+  // k_linearize's block partial: its 8 warp sums in warp order
+  for (int b = threadIdx.x; b < n_lin_blocks; b += CAND_THREADS) {
+#pragma unroll 3
+    for (int q = 0; q < NE_CAND; q++) {
+      double t[LIN_WARPS];
+#pragma unroll
+      for (int w = 0; w < LIN_WARPS; w++) t[w] = __ldcg(wsums + (size_t)(b * LIN_WARPS + w) * NE_CAND + q);
+      double v = 0.0;
+#pragma unroll
+      for (int w = 0; w < LIN_WARPS; w++) v += t[w];
+      bsum[b][q] = v;
+    }
+  }
+  __syncthreads();
+  // lm_tail's order: "warp" w of 8 sums blocks w, w + 8, ...; then the 8 in order (H components: sums of zeros)
+  for (int task = threadIdx.x; task < (LM_THREADS / 32) * NE_CAND; task += CAND_THREADS) {
+    const int w = task / NE_CAND, q = task % NE_CAND;
+    double v = 0.0;
+    for (int b = w; b < n_lin_blocks; b += LM_THREADS / 32) v += bsum[b][q];
+    vsum[w][q] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < NE_PACK) {
+    double t = 0.0;
+    if (threadIdx.x >= NE_H)
+#pragma unroll
+      for (int w = 0; w < LM_THREADS / 32; w++) t += vsum[w][threadIdx.x - NE_H];
+    ne[threadIdx.x] = t;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    s.work[0] = 0, s.work[1] = 0;
+    const long long t1 = clock64();
+    lm_advance(&s, ne, 2, eig_thre, 1);
+    s.dbg_cycles[0] += t1 - t0, s.dbg_cycles[1] += clock64() - t1, s.dbg_cycles[2] += 1;
+  }
+  __syncthreads();
+  {
+    const unsigned long long *src = reinterpret_cast<const unsigned long long *>(&s);
+    unsigned long long *dst = reinterpret_cast<unsigned long long *>(gst);
+    for (int k = threadIdx.x; k < kWords; k += CAND_THREADS) dst[k] = src[k];
+  }
+}
+
+// grid: LIN_THREADS / CAND_THREADS blocks per k_linearize block; wsums: NE_CAND doubles per warp
+__global__ void __launch_bounds__(CAND_THREADS, 8) k_eval_candidate(LinArgs a, double *__restrict__ wsums) {
+  __shared__ bool is_last;
+  if (a.state->done) return;  // the step of the evaluation at x ended the Solve
+  double xs[7];
+#pragma unroll
+  for (int k = 0; k < 7; k++) xs[k] = a.state->xc[k];
+  const PoseR P = make_poser(xs);
+  double acc[NE_CAND];
+#pragma unroll
+  for (int k = 0; k < NE_CAND; k++) acc[k] = 0.0;
+  const int G = gridDim.x * blockDim.x, gid = blockIdx.x * blockDim.x + threadIdx.x;
+  for (int s = 0; s < a.n_sets; s++) {
+    const FeatSetDev fs = a.set[s];
+    const int fn = fs.d_n ? min(fs.n, *fs.d_n) : fs.n;
+    for (int i = (s & 1) ? G - 1 - gid : gid; i < fn; i += G) {  // k_linearize's assignment
+      if (!fs.valid[i] || (fs.mask && !fs.mask[i])) continue;
+      double J[6], rho;
+      const double r = map_factor_row(P, fs, i, a.sqrt_info, a.huber_a, J, &rho);
+#pragma unroll
+      for (int k = 0; k < 6; k++) acc[k] += J[k] * r;
+      acc[6] += 0.5 * rho;
+      if (s == 0) acc[7] += 1.0;
+      else acc[8] += 1.0;
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < NE_CAND; k++)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc[k] += __shfl_xor_sync(MLOAM_FULL_MASK, acc[k], o);
+  if ((threadIdx.x & 31) == 0) {
+    double *w = wsums + (size_t)(gid >> 5) * NE_CAND;
+#pragma unroll
+    for (int k = 0; k < NE_CAND; k++) w[k] = acc[k];
+  }
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) is_last = atomicAdd(a.ticket, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  cand_tail(wsums, (int)(gridDim.x / (LIN_THREADS / CAND_THREADS)), a.state_rw, a.eig_thre);
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) *a.ticket = 0u;
+}
+
+__global__ void k_lm_init(LMState *st, const double *pose7, int max_inner, int min_corr, SpecState *spec) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
+    if (spec) {  // the first matcher of a solve is blind: any half will do, but sel must be 0 or 1 (fresh memory is not)
+      for (int k = 0; k < 7; k++) spec->xc[k] = pose7[k];
+      spec->sel = 0;
+    }
     for (int k = 0; k < 7; k++) st->x[k] = pose7[k], st->xc[k] = pose7[k];
     st->max_inner = max_inner;
     st->min_corr = min_corr, st->skipped = 0;
@@ -654,7 +802,7 @@ __global__ void k_lm_init(LMState *st, const double *pose7, int max_inner, int m
   }
 }
 
-int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, double eig_thre) {
+int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, double eig_thre, SpecState *spec) {
   (void)eig_thre;
   MLOAM_CUDA_OK(c, c->lm_state.reserve(sizeof(LMState) + 64));
   // stage the pose through pinned memory so the copy is truly asynchronous
@@ -662,15 +810,17 @@ int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, double eig_th
   for (int k = 0; k < 7; k++) stage[k] = pose7_host[k];
   double *d_stage = c->scratch[7].as<double>();
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_stage, stage, 7 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  k_lm_init<<<1, 32, 0, c->stream>>>(c->lm_state.as<LMState>(), d_stage, max_inner, c->lm_min_corr);
+  k_lm_init<<<1, 32, 0, c->stream>>>(c->lm_state.as<LMState>(), d_stage, max_inner, c->lm_min_corr, spec);
   c->launches++;
   MLOAM_CUDA_OK(c, cudaGetLastError());
   return MLOAM_OK;
 }
 
-int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, const double *d_pose7,
-                     int use_state, int lm_mode, double *d_out30) {
-  LinArgs a;
+// What k_linearize and k_eval_candidate share: the feature sets, the grid (k_eval_candidate runs LIN_THREADS / CAND_THREADS
+// blocks per k_linearize block) and c->partials = [NE_PACK doubles per k_linearize block, max_nb + 2 of them][ticket +
+// generation word][NE_CAND doubles per k_eval_candidate warp].
+static int lin_setup(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, LinArgs &a, int *nb_out, double **wsums) {
+  memset(&a, 0, sizeof(a));
   int n_total = 0;
   for (int s = 0; s < 2; s++) {
     if (s < n_sets) {
@@ -683,11 +833,10 @@ int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, 
       a.set[s].sinfo = nullptr, a.set[s].mask = nullptr;
     }
   }
-  const int want_eig = c->want_eig;
-  a.n_sets = n_sets, a.sqrt_info = sqrt_info, a.huber_a = huber_a, a.pose = d_pose7;
+  a.n_sets = n_sets, a.sqrt_info = sqrt_info, a.huber_a = huber_a;
   a.state = c->lm_state.as<LMState>();
-  a.use_state = use_state;
-  a.respect_done = (lm_mode == 2) ? 1 : 0;
+  a.state_rw = c->lm_state.as<LMState>();
+  a.eig_thre = c->lm_eig_thre >= 0.0 ? c->lm_eig_thre : c->params.eig_thre;
   int nb = (n_total + LIN_THREADS - 1) / LIN_THREADS;
   if (nb < 1) nb = 1;
   // n_total is a launch upper bound (device-side counts are usually far smaller): 64 blocks x 256 threads cover a
@@ -695,27 +844,47 @@ int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, 
   const int max_nb = c->sm_count;
   if (nb > max_nb) nb = max_nb;
   if (nb > 64) nb = 64;
-  MLOAM_CUDA_OK(c, c->partials.reserve(sizeof(double) * NE_PACK * (size_t)(max_nb + 3)));
-  unsigned *ticket = reinterpret_cast<unsigned *>(c->partials.as<double>() + (size_t)NE_PACK * (max_nb + 2));
+  const size_t wsums_at = (size_t)NE_PACK * (max_nb + 3);
+  MLOAM_CUDA_OK(c, c->partials.reserve(sizeof(double) * (wsums_at + (size_t)NE_CAND * 64 * LIN_WARPS)));
+  a.ticket = reinterpret_cast<unsigned *>(c->partials.as<double>() + (size_t)NE_PACK * (max_nb + 2));
   if (c->ticket_zeroed_for != c->partials.p) {  // a fresh partials buffer: the last-block ticket starts at zero
-    MLOAM_CUDA_OK(c, cudaMemsetAsync(ticket, 0, sizeof(double), c->stream));
+    MLOAM_CUDA_OK(c, cudaMemsetAsync(a.ticket, 0, sizeof(double), c->stream));
     c->ticket_zeroed_for = c->partials.p;
   }
-  const double eig_thre = c->lm_eig_thre >= 0.0 ? c->lm_eig_thre : c->params.eig_thre;
+  *nb_out = nb;
+  *wsums = c->partials.as<double>() + wsums_at;
+  return MLOAM_OK;
+}
+
+int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, const double *d_pose7,
+                     int use_state, int lm_mode, double *d_out30) {
+  LinArgs a;
+  int nb = 0;
+  double *wsums = nullptr;
+  int rc = lin_setup(c, sets, n_sets, sqrt_info, huber_a, a, &nb, &wsums);
+  if (rc) return rc;
+  const int max_nb = c->sm_count;
+  const int want_eig = c->want_eig;
+  a.pose = d_pose7;
+  a.use_state = use_state;
+  a.respect_done = (lm_mode == 2) ? 1 : 0;
   const bool collective = c->nccl_comm && c->p2p_collective;  // sum over the ranks wanted for this solve
   const bool fused = lm_mode != 0 && (!collective || c->p2p_on) && !d_out30;
   // only the collective solves (scan2map on every rank in lock-step) exchange; per-rank solves on the same context — the tracker,
   // mloam_normal_equations — stay local (c->p2p_collective is raised by scan2map_enqueue alone)
   a.p2p = (fused && c->p2p_on && c->p2p_collective) ? static_cast<const P2PView *>(c->p2p_view) : nullptr;
-  a.lm_mode = fused ? lm_mode : 0, a.want_eig = want_eig, a.eig_thre = eig_thre, a.ticket = ticket;
-  a.state_rw = c->lm_state.as<LMState>();
+  a.lm_mode = fused ? lm_mode : 0, a.want_eig = want_eig;
   // both evaluations of an LM iteration in one launch: only with the fused tail (the barrier is released by the block that ran it)
   a.two_pass = (c->lin_two_pass && fused && lm_mode == 1) ? 1 : 0;
   c->lin_two_pass = a.two_pass != 0;
+  // the speculative schedule's commit rides in the fused tail of the evaluation at x
+  if (c->lin_spec && !(fused && lm_mode == 1 && !a.p2p)) {
+    c->err = "linearize: the speculative schedule needs the fused single-GPU evaluation at x";
+    return MLOAM_E_STATE;
+  }
+  a.spec = c->lin_spec, a.spec_publish = c->lin_spec_publish ? 1 : 0;
   // a fit the matcher deferred to this evaluation
   int kfit = 0;
-  memset(a.fit, 0, sizeof(a.fit));
-  a.fit_min_plane_dis = 0.f, a.fit_check_fov = 0;
   if (c->pending_fit.K) {
     if (lm_mode != 1 || n_sets != 2 || (c->pending_fit.K != 5 && c->pending_fit.K != 10)) {
       c->err = "linearize: a deferred fit is pending but this is not the first evaluation of a solve";
@@ -757,6 +926,19 @@ int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, 
                                   d_out30);
     c->launches++;
   }
+  MLOAM_CUDA_OK(c, cudaGetLastError());
+  return MLOAM_OK;
+}
+
+int eval_candidate_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a) {
+  LinArgs a;
+  int nb = 0;
+  double *wsums = nullptr;
+  int rc = lin_setup(c, sets, n_sets, sqrt_info, huber_a, a, &nb, &wsums);
+  if (rc) return rc;
+  ProfScope ps(c, "candidate");
+  k_eval_candidate<<<nb * (LIN_THREADS / CAND_THREADS), CAND_THREADS, 0, c->stream>>>(a, wsums);
+  c->launches++;
   MLOAM_CUDA_OK(c, cudaGetLastError());
   return MLOAM_OK;
 }
