@@ -256,6 +256,32 @@ int mloam_set_extrinsic(mloam_ctx_t *ctx, const double *ext7);
  * (lidar_mapper_keyframe.cpp:356-639).  n_lidars = 1 restores the single-LiDAR path. */
 int mloam_set_lidars(mloam_ctx_t *ctx, int n_lidars, const double *ext7);
 
+/* ---- uncertainty-aware mapping (with_ua) in mloam_frame*: the configuration every mapper launch file of the reference runs
+ *      (the launch files under estimator/launch set -with_ua=true).
+ * mloam_set_uncertainty: with_ua != 0 turns the with_ua branches of the frame on; 0 restores the with_ua = false path exactly.
+ *   ext_cov36: per LiDAR of the context (n_lidars after mloam_set_lidars, one in the single-LiDAR path) the row-major 6x6 covariance
+ *   [translation | rotation] of its extrinsic, pose_ext[l].cov_, as the /extrinsics message delivers it every frame
+ *   (lidar_mapper_keyframe.cpp:1043); cov_meas9 = COV_MEASUREMENT; trace_threshold = TRACE_THRESHOLD_MAPPING.  May be called before
+ *   every frame: the values are staged, a captured frame replays with them.  Call it after mloam_set_lidars.  A context with a
+ *   communicator (mloam_comm_init / mloam_comm_p2p_init) rejects with_ua frames with MLOAM_E_STATE.
+ *   With with_ua, a frame runs downsampleCurrentScan's uncertainty loop (:356-421) after the scan filters: per point
+ *   idx = int(intensity) (the laser id of the rig merge; 0 in the single-LiDAR path without mloam_set_lidars extrinsics),
+ *   pointAssociateToMap with pose_ext[idx]^-1, evalPointUncertainty under pose_ext[idx] (associate_uct.hpp:196-215), dropped when
+ *   trace > TRACE_THRESHOLD_MAPPING; every residual is weighted by sqrt_info of its point's covariance (extractCov + clamp, :541-560,
+ *   lidar_map_factor.hpp:34,41), good-feature selection included (lidar_mapper.h:130-174); stats->n_*_in count the gated scans.
+ * mloam_pose_covariance: pose_wmap_curr.cov_ (:632) of the last mloam_frame* / mloam_scan2map* solve: cov_mapping = H^-1 with H the
+ *   loss-corrected J^T J evaluated at the pose the last Solve returned, with the last association (:600-610), inverted by partial-pivot
+ *   LU as Eigen's 6x6 inverse.  mloam_scan2map_ua counts as with_ua.  Zeros without with_ua (:621), when the map gate rejected the
+ *   frame (:637) and when the last evaluation had no residual rows (Eigen would return inf / NaN there).  The rule "zero while there
+ *   are <= 10 keyframes" (:607-608) is the caller's, which knows the keyframe count.
+ * mloam_frame_scan: the down-sampled (and, with with_ua, gated) scans of the last mloam_frame* call in the base frame with their
+ *   PointIWithCov::cov_vec (float xx xy xz yy yz zz; zeros without with_ua) — laser_cloud_{surf,corner}_cov, what saveKeyframe stores
+ *   (:671-677) and mloam_submap_assemble later takes.  Outputs are nullable; capacities in points.  MLOAM_E_STATE before any frame. */
+int mloam_set_uncertainty(mloam_ctx_t *ctx, int with_ua, const double *ext_cov36, const double *cov_meas9, double trace_threshold);
+int mloam_pose_covariance(mloam_ctx_t *ctx, double *cov36);
+int mloam_frame_scan(mloam_ctx_t *ctx, mloam_point_t *h_surf, float *h_surf_cov6, int cap_surf, int *n_surf, mloam_point_t *h_corner,
+                     float *h_corner_cov6, int cap_corner, int *n_corner);
+
 /* ---- FeatureExtract::matchCornerFromScan / matchSurfFromScan (feature_extract.hpp:131-376) against the map slot
  * built (mloam_map_build, cell ~1.3 m) from the previous sweep's less-sharp / less-flat features, which must be in
  * the reference's ring-sorted order (int(intensity) = ring).  type 'c': coeffs = [X_closest; X_second];

@@ -30,6 +30,7 @@ ABI_SYMBOLS = [
     "mloam_map_build_device", "mloam_map_size", "mloam_knn", "mloam_match_from_map", "mloam_factor_evaluate",
     "mloam_normal_equations", "mloam_pose_plus", "mloam_scan2map", "mloam_scan2map_device", "mloam_frame",
     "mloam_frame_device", "mloam_set_extrinsic", "mloam_set_lidars", "mloam_calib_frame", "mloam_compound_pose_cov", "mloam_cloud_uct_associate", "mloam_voxel_downsample_cov", "mloam_submap_assemble", "mloam_good_features_odom", "mloam_local_map_build", "mloam_match_from_scan", "mloam_track_cloud", "mloam_odom_solve", "mloam_point_uncertainty", "mloam_scan2map_ua", "mloam_good_features", "mloam_comm_unique_id", "mloam_comm_init", "mloam_comm_destroy", "mloam_comm_p2p_export", "mloam_comm_p2p_init", "mloam_comm_p2p_reset",
+    "mloam_set_uncertainty", "mloam_pose_covariance", "mloam_frame_scan",
 ]
 
 
@@ -503,6 +504,31 @@ class Context:
     def set_lidars(self, n_lidars: int, ext7=None):
         e = None if ext7 is None else np.ascontiguousarray(ext7, np.float64).reshape(-1)
         self._ck(lib().mloam_set_lidars(self._h, n_lidars, _p(e)))
+
+    def set_uncertainty(self, with_ua: bool, ext_cov=None, cov_meas=None, trace_threshold: float = 0.0):
+        """with_ua frames (mloam_set_uncertainty): ext_cov [n_lidars, 6, 6] extrinsic covariances [translation | rotation],
+        cov_meas 3x3 COV_MEASUREMENT, trace_threshold TRACE_THRESHOLD_MAPPING.  Call after set_lidars; may be called before every frame."""
+        if not with_ua:
+            self._ck(lib().mloam_set_uncertainty(self._h, 0, None, None, C.c_double(0.0)))
+            return
+        ec = np.ascontiguousarray(ext_cov, np.float64).reshape(-1)
+        cm = np.ascontiguousarray(cov_meas, np.float64).reshape(9)
+        self._ck(lib().mloam_set_uncertainty(self._h, 1, _p(ec), _p(cm), C.c_double(trace_threshold)))
+
+    def pose_covariance(self) -> np.ndarray:
+        """pose_wmap_curr.cov_ of the last frame / scan2map solve (6x6, [translation | rotation]; zeros without with_ua)."""
+        out = np.zeros(36)
+        self._ck(lib().mloam_pose_covariance(self._h, _p(out)))
+        return out.reshape(6, 6)
+
+    def frame_scan(self):
+        """The down-sampled (with with_ua: gated) scans of the last frame with cov_vec: (surf [n,4], surf_cov6 [n,6], corner, corner_cov6)."""
+        ns, nc = C.c_int(0), C.c_int(0)
+        self._ck(lib().mloam_frame_scan(self._h, None, None, 0, C.byref(ns), None, None, 0, C.byref(nc)))
+        sp, sc = np.zeros((max(ns.value, 1), 4), np.float32), np.zeros((max(ns.value, 1), 6), np.float32)
+        cp, cc = np.zeros((max(nc.value, 1), 4), np.float32), np.zeros((max(nc.value, 1), 6), np.float32)
+        self._ck(lib().mloam_frame_scan(self._h, _p(sp), _p(sc), sp.shape[0], C.byref(ns), _p(cp), _p(cc), cp.shape[0], C.byref(nc)))
+        return sp[:ns.value].copy(), sc[:ns.value].copy(), cp[:nc.value].copy(), cc[:nc.value].copy()
 
     def set_extrinsic(self, ext7=None):
         e = None if ext7 is None else np.ascontiguousarray(ext7, np.float64)

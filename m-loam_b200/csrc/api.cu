@@ -152,7 +152,7 @@ void mloam_ctx_destroy(mloam_ctx_t *h) {
   c->knn_heavy_list.release(), c->knn_trace.release(), c->knn_spec.release();
   c->partials.release(), c->lm_state.release();
   for (auto &s : c->scratch) s.release();
-  c->frame_main.release(), c->frame_alt.release(), c->next_in.release(), c->stamps.release();
+  c->frame_main.release(), c->frame_alt.release(), c->next_in.release(), c->stamps.release(), c->ua_scan.release(), c->pose_cov.release();
   if (c->pinned) cudaFreeHost(c->pinned);
   if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
   if (c->stream2) cudaStreamSynchronize(c->stream2), cudaStreamDestroy(c->stream2);

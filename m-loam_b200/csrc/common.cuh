@@ -165,6 +165,14 @@ struct P2PView {
   int nranks, rank;
 };
 
+// sqrt_info of a scan point with covariance (with_ua): extractCov (point_with_cov.hpp:202-214) turns the float cov_vec into a
+// Matrix3d, the factor takes sqrt(1 / trace) clamped as lidar_map_factor.hpp:34,41
+__device__ inline double cov6_sqrt_info(const float *c6) {
+  const double tr = (double)c6[0] + (double)c6[3] + (double)c6[5];
+  const double s = sqrt(1 / tr);
+  return s >= 3.0 ? 1.0 : s / 3.0;
+}
+
 // ------------------------------------------------------------------ LM state (device resident)
 // Everything ceres::Solve keeps between iterations for one 6-dof (or 12-dof) block, plus the packed
 // normal equations the reduction writes.  NE_MAX covers 12x12 (78 upper + 12 + cost + rows).

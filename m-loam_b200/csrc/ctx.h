@@ -189,6 +189,7 @@ struct Ctx {
     int n_corner;
     const int *d_n_corner;
     const double *sinfo_surf, *sinfo_corner;  // nullable per-feature sqrt_info (uncertainty-aware mapping)
+    const float *cov6_surf, *cov6_corner;     // nullable PointIWithCov::cov_vec per feature (with_ua frame: gated scans)
   };
   // Sweep look-ahead (mloam_frame_set_next*): while frame k is matched and solved, the features of sweep k+1 are extracted and
   // down-sampled on a side stream into the other half of a double buffer — the reference runs the two stages in different nodes
@@ -266,7 +267,24 @@ struct Ctx {
   void *p2p_view = nullptr;        // device copy of the P2PView the kernels read
   bool p2p_on = false;
   bool p2p_collective = false;     // the solve being enqueued is the collective one (all ranks in lock-step): sum over the ranks
+  // uncertainty-aware mapping in the frame path (mloam_set_uncertainty): the per-point uncertainty + trace gate of
+  // downsampleCurrentScan (lidar_mapper_keyframe.cpp:356-421) between the scan filters and the solve, and the pose covariance
+  // H^-1 at the returned pose (:600-610).  The covariances reach the device through the pinned block (kPinnedUct), so a
+  // captured frame replays with new values.
+  int with_ua = 0;
+  double ua_ext_cov[MLOAM_MAX_LIDARS][36];  // per LiDAR: pose_ext[l].cov_, row-major [translation | rotation]
+  double ua_cov_meas[9];                    // COV_MEASUREMENT
+  double ua_trace_threshold = 0.0;          // TRACE_THRESHOLD_MAPPING
+  DevBuf ua_scan;                  // gated scans of the last with_ua frame (points, cov6, sqrt_info, counts) + its staged configuration
+  DevBuf pose_cov;                 // 36 doubles: H^-1 of the last solve (k_pose_cov), copied back with LMState
+  bool s2m_cov = false;            // the solve being enqueued reports H^-1 (with_ua frame, mloam_scan2map_ua)
+  double pose_cov36[36] = {0};     // pose_wmap_curr.cov_ of the last mloam_frame* / mloam_scan2map* call
+  bool last_scan_valid = false;    // last_scan describes the scan of the last mloam_frame* call (mloam_frame_scan)
+  ScanRef last_scan{};
 };
+
+constexpr size_t kPinnedUct = 49152;      // inside Ctx::pinned: UctFrame (256 B) + MLOAM_MAX_LIDARS UctLaser of the with_ua frame stage
+constexpr size_t kPinnedPoseCov = 57344;  // inside Ctx::pinned: 36 doubles, H^-1 of the last solve
 
 // RAII-less helper: bracket a kernel (or a few) with events when profiling is on.
 struct ProfScope {
@@ -359,6 +377,13 @@ int gf_select_set_device(Ctx *c, int t, const FeatSet &fs, const double *d_pose7
 
 // uct_kernels.cu: per-point sqrt_info from PointIWithCov::cov_vec (float[6] per point)
 int sqrt_info_device(Ctx *c, const float *d_cov6, int n, double *d_sinfo);
+// submap.cu: the with_ua stage of a frame (downsampleCurrentScan, lidar_mapper_keyframe.cpp:356-421) on c->stream.  The scans of *S
+// (device counts) -> per point ext^-1 -> evalPointUncertainty under pose_ext -> trace gate -> stable compaction into Ctx::ua_scan with
+// cov6 and sqrt_info; *S then points at the gated scans.  ua_stage_host writes the staged configuration (replays re-run it).
+int ua_scan_stage(Ctx *c, Ctx::ScanRef *S);
+void ua_stage_host(Ctx *c);
+// solve_kernels.cu: Ctx::pose_cov <- LMState::H^-1 (partial-pivot LU), zeros when the last evaluation had no residual rows
+int pose_cov_device(Ctx *c);
 
 // comm.cu: in-place sum over ranks on the context stream (no-op without a communicator)
 int comm_allreduce_doubles(Ctx *c, double *d_buf, int count);

@@ -154,6 +154,12 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7) {
   char *pin = reinterpret_cast<char *>(c->pinned);
   LMState *hs = reinterpret_cast<LMState *>(pin + 4096);
   int *h_cnt = reinterpret_cast<int *>(pin + 3072);
+  if (c->s2m_cov) {  // with_ua: cov_mapping = H^-1 at the returned pose (:600-610), one more tiny launch inside the frame
+    rc = pose_cov_device(c);
+    if (rc) return rc;
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(pin + kPinnedPoseCov, c->pose_cov.p, 36 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    stamp(c, "pose covariance");
+  }
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(hs, st, sizeof(LMState), cudaMemcpyDeviceToHost, c->stream));
   if (S.d_n_surf) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_cnt, S.d_n_surf, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   if (S.d_n_corner) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_cnt + 1, S.d_n_corner, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -163,6 +169,7 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7) {
 int scan2map_finish(Ctx *c, const ScanRef &S, const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
   if (stats) memset(stats, 0, sizeof(*stats));
   for (int k = 0; k < 7; k++) pose_out7[k] = pose_init7[k];
+  memset(c->pose_cov36, 0, sizeof(c->pose_cov36));  // pose_wmap_curr.cov_: zero without with_ua (:621) and for a map-gated frame (:637)
   if (!c->s2m_ran) return MLOAM_OK;
   char *pin = reinterpret_cast<char *>(c->pinned);
   const LMState *hs = reinterpret_cast<const LMState *>(pin + 4096);
@@ -171,6 +178,7 @@ int scan2map_finish(Ctx *c, const ScanRef &S, const double *pose_init7, double *
   if (!S.d_n_surf) h_cnt[0] = S.n_surf;
   if (!S.d_n_corner) h_cnt[1] = S.n_corner;
   for (int k = 0; k < 7; k++) pose_out7[k] = hs->x[k];
+  if (c->s2m_cov && hs->termination != 8 && hs->termination != 9) memcpy(c->pose_cov36, pin + kPinnedPoseCov, sizeof(c->pose_cov36));
   if (hs->termination == 9) {  // the peer-memory exchange timed out or the ranks lost lock-step: the summed state is not trustworthy
     for (int k = 0; k < 7; k++) pose_out7[k] = pose_init7[k];
     if (stats) stats->ran = 1, stats->termination = 9;
@@ -392,6 +400,11 @@ int frame_enqueue(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start,
   }
   c->next.set = false;
   stamp(c, have ? "features (prefetched)" : "extract + voxel");
+  if (c->with_ua) {  // downsampleCurrentScan's per-point uncertainty + trace gate: on the main stream with the covariances of THIS call
+    rc = ua_scan_stage(c, &S);
+    if (rc) return rc;
+    stamp(c, "uncertainty + gate");
+  }
   if (forked) MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream, c->ev_join, 0));  // join the map-build branch
   if (forked) stamp(c, "map build join");
   *S_out = S;
@@ -442,6 +455,10 @@ int frame_run(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, con
               const float4 *d_surf_map, int n_surf_map, const float4 *d_corner_map, int n_corner_map, int rebuild_maps,
               const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
   ScanRef S{};
+  if (c->with_ua && c->nccl_comm)
+    return fail(c, MLOAM_E_STATE, "frame: uncertainty-aware frames (mloam_set_uncertainty) are single-GPU only; detach the communicator or set with_ua = 0");
+  c->s2m_cov = c->with_ua != 0;
+  c->last_scan_valid = false;
   const bool can_graph = c->use_graphs && c->params.max_inner == 1 && !c->prof_on && (!c->nccl_comm || c->p2p_on);
   if (can_graph) {
     unsigned long long key = 1469598103934665603ull;
@@ -460,6 +477,7 @@ int frame_run(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, con
     key = fnv1a(key, &c->lidar_merge, sizeof(c->lidar_merge));
     key = fnv1a(key, c->lidar_ext, sizeof(double) * 7 * (size_t)c->n_lidars);
     key = fnv1a(key, &c->stream, sizeof(c->stream));
+    key = fnv1a(key, &c->with_ua, sizeof(c->with_ua));  // the covariances and the threshold are staged, not part of the key
     {  // look-ahead: which half holds this sweep's features (or that they are extracted now), and the announced next sweep
       const void *key_now = c->cloud_key ? c->cloud_key : static_cast<const void *>(d_cloud);
       const bool have = frame_has_prefetched(c, key_now, n, n_scans);
@@ -479,6 +497,7 @@ int frame_run(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, con
       for (int k = 0; k < 7; k++) stage[k] = pose_init7[k];  // the captured H2D node reads this at execution time
       if (c->has_ext)
         for (int k = 0; k < 7; k++) stage[32 + k] = c->ext[k];
+      if (c->with_ua) ua_stage_host(c);  // read by the captured H2D node of the with_ua stage
       MLOAM_CUDA_OK(c, cudaGraphLaunch(e->exec, c->stream));
       c->launches += e->launches;
       c->s2m_ran = e->s2m_ran;
@@ -486,6 +505,7 @@ int frame_run(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, con
       c->frame_parity = (frame_has_prefetched(c, c->cloud_key ? c->cloud_key : static_cast<const void *>(d_cloud), n, n_scans) ? c->prefetched.parity : c->frame_parity) ^ 1;
       c->prefetched = e->prefetched_out;
       c->next.set = false;
+      c->last_scan = e->S, c->last_scan_valid = true;
       return scan2map_finish(c, e->S, pose_init7, pose_out7, stats);
     }
     if (e && e->seen >= 1) {  // second sighting: capture
@@ -508,6 +528,7 @@ int frame_run(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, con
         cudaGraphDestroy(graph);
         MLOAM_CUDA_OK(c, cudaGraphLaunch(e->exec, c->stream));
         c->launches += e->launches;
+        c->last_scan = S, c->last_scan_valid = true;
         return scan2map_finish(c, S, pose_init7, pose_out7, stats);
       }
       if (graph) cudaGraphDestroy(graph);
@@ -529,6 +550,7 @@ int frame_run(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, con
   int rc = frame_enqueue(c, d_cloud, n, d_scan_start, d_scan_end, n_scans, d_surf_map, n_surf_map, d_corner_map, n_corner_map,
                          rebuild_maps, pose_init7, &S);
   if (rc) return rc;
+  c->last_scan = S, c->last_scan_valid = true;
   return scan2map_finish(c, S, pose_init7, pose_out7, stats);
 }
 
@@ -543,6 +565,7 @@ int mloam_scan2map_device(mloam_ctx_t *h, const mloam_point_t *d_surf_scan, int 
   cudaSetDevice(h->c.device);
   ScanRef S{reinterpret_cast<const float4 *>(d_surf_scan), n_surf, nullptr, reinterpret_cast<const float4 *>(d_corner_scan), n_corner,
             nullptr};
+  h->c.s2m_cov = false;
   return scan2map_run(&h->c, S, pose_init7, pose_out7, stats);
 }
 
@@ -558,6 +581,7 @@ int mloam_scan2map(mloam_ctx_t *h, const mloam_point_t *h_surf_scan, int n_surf,
   if (n_surf > 0)
     MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->scan_pts[1].p, h_surf_scan, sizeof(float4) * (size_t)n_surf, cudaMemcpyHostToDevice, c->stream));
   ScanRef S{c->scan_pts[1].as<float4>(), n_surf, nullptr, c->scan_pts[0].as<float4>(), n_corner, nullptr};
+  c->s2m_cov = false;
   return scan2map_run(c, S, pose_init7, pose_out7, stats);
 }
 
@@ -589,7 +613,10 @@ int mloam_scan2map_ua(mloam_ctx_t *h, const mloam_point_t *h_surf_scan, int n_su
   }
   ScanRef S{c->scan_pts[1].as<float4>(), n_surf, nullptr, c->scan_pts[0].as<float4>(), n_corner, nullptr, sin[1]->as<double>(),
             sin[0]->as<double>()};
-  return scan2map_run(c, S, pose_init7, pose_out7, stats);
+  c->s2m_cov = true;  // with_ua: pose_wmap_curr.cov_ = H^-1 at the returned pose (mloam_pose_covariance)
+  const int rc = scan2map_run(c, S, pose_init7, pose_out7, stats);
+  c->s2m_cov = false;
+  return rc;
 }
 
 // ------------------------------------------------------------------------------------------ extractCloud
@@ -602,6 +629,7 @@ int mloam_extract_features(mloam_ctx_t *h, const mloam_point_t *h_cloud, int n, 
   out->n_sharp = out->n_less_sharp = out->n_flat = out->n_less_flat = 0;
   if (n == 0) return MLOAM_OK;
   c->prefetched.valid = false;  // this call reuses half 0 of the frame feature buffers
+  c->last_scan_valid = false;
   FrameBufs F;
   int rc = frame_bufs(c, n, &F);
   if (rc) return rc;
@@ -805,6 +833,62 @@ int mloam_set_lidars(mloam_ctx_t *h, int n_lidars, const double *ext7) {
   c->lidar_merge = ext7 != nullptr;  // also for ONE LiDAR with an extrinsic: same float transform + laser id as in a rig
   for (int l = 0; l < n_lidars; l++)
     for (int k = 0; k < 7; k++) c->lidar_ext[l][k] = ext7 ? ext7[7 * l + k] : (k == 6 ? 1.0 : 0.0);
+  return MLOAM_OK;
+}
+
+// ------------------------------------------------------------------------------------------ uncertainty-aware frames
+int mloam_set_uncertainty(mloam_ctx_t *h, int with_ua, const double *ext_cov36, const double *cov_meas9, double trace_threshold) {
+  if (!h) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (with_ua && (!ext_cov36 || !cov_meas9)) return MLOAM_E_INVALID;
+  c->with_ua = with_ua ? 1 : 0;
+  if (!with_ua) return MLOAM_OK;
+  const int n_lasers = (c->n_lidars > 1 || c->lidar_merge) ? c->n_lidars : 1;
+  for (int l = 0; l < MLOAM_MAX_LIDARS; l++)
+    for (int k = 0; k < 36; k++) c->ua_ext_cov[l][k] = l < n_lasers ? ext_cov36[36 * l + k] : 0.0;
+  memcpy(c->ua_cov_meas, cov_meas9, sizeof(c->ua_cov_meas));
+  c->ua_trace_threshold = trace_threshold;
+  return MLOAM_OK;
+}
+
+int mloam_pose_covariance(mloam_ctx_t *h, double *cov36) {
+  if (!h || !cov36) return MLOAM_E_INVALID;
+  memcpy(cov36, h->c.pose_cov36, sizeof(h->c.pose_cov36));
+  return MLOAM_OK;
+}
+
+int mloam_frame_scan(mloam_ctx_t *h, mloam_point_t *h_surf, float *h_surf_cov6, int cap_surf, int *n_surf, mloam_point_t *h_corner,
+                     float *h_corner_cov6, int cap_corner, int *n_corner) {
+  if (!h) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (!c->last_scan_valid) return fail(c, MLOAM_E_STATE, "frame_scan: no mloam_frame / mloam_frame_device call has run since the last reset");
+  cudaSetDevice(c->device);
+  const ScanRef &S = c->last_scan;
+  cudaStream_t st = c->stream;
+  int *hc = reinterpret_cast<int *>(reinterpret_cast<char *>(c->pinned) + 3072);
+  hc[0] = S.n_surf, hc[1] = S.n_corner;
+  if (S.d_n_surf) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, S.d_n_surf, sizeof(int), cudaMemcpyDeviceToHost, st));
+  if (S.d_n_corner) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc + 1, S.d_n_corner, sizeof(int), cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  const int ns = hc[0] < S.n_surf ? hc[0] : S.n_surf, nc = hc[1] < S.n_corner ? hc[1] : S.n_corner;
+  if (n_surf) *n_surf = ns;
+  if (n_corner) *n_corner = nc;
+  if ((h_surf || h_surf_cov6) && ns > cap_surf) return fail(c, MLOAM_E_INVALID, "frame_scan: surf capacity too small");
+  if ((h_corner || h_corner_cov6) && nc > cap_corner) return fail(c, MLOAM_E_INVALID, "frame_scan: corner capacity too small");
+  const float4 *pts[2] = {S.surf, S.corner};
+  const float *cov[2] = {S.cov6_surf, S.cov6_corner};
+  mloam_point_t *hp[2] = {h_surf, h_corner};
+  float *hcv[2] = {h_surf_cov6, h_corner_cov6};
+  const int cnt[2] = {ns, nc};
+  for (int t = 0; t < 2; t++) {
+    if (cnt[t] <= 0) continue;
+    if (hp[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hp[t], pts[t], sizeof(float4) * (size_t)cnt[t], cudaMemcpyDeviceToHost, st));
+    if (hcv[t]) {
+      if (cov[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hcv[t], cov[t], sizeof(float) * 6 * (size_t)cnt[t], cudaMemcpyDeviceToHost, st));
+      else memset(hcv[t], 0, sizeof(float) * 6 * (size_t)cnt[t]);  // with_ua = false: PointIWithCov(point, Zero) (:378-386)
+    }
+  }
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
   return MLOAM_OK;
 }
 

@@ -816,6 +816,65 @@ int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, double eig_th
   return MLOAM_OK;
 }
 
+// ---------------------------------------------------------------------------------------- pose covariance
+// cov_mapping = mat_H.inverse() after the last Solve (lidar_mapper_keyframe.cpp:600-610): LMState::H is the loss-corrected J^T J
+// at the accepted x, evaluated with the last association — problem.Evaluate at the pose the Solve returns.  Eigen's 6x6 inverse
+// is a partial-pivot LU (first largest |pivot| of the column, rows swapped, multipliers divided by the pivot, rank-1 update of the
+// trailing block) followed by L U X = P I solved column by column.  A last evaluation with no residual rows gives zeros (Eigen
+// would return inf / NaN there).  The speculative schedule keeps the two-pass k_linearize for the last GN iteration, so H is
+// accumulated at the final candidate too (k_eval_candidate does not accumulate H).
+__global__ void k_pose_cov(const LMState *__restrict__ st, double *__restrict__ out) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  if (st->rows <= 0) {
+    for (int i = 0; i < 36; i++) out[i] = 0.0;
+    return;
+  }
+  double A[36];
+  int perm[6];
+  for (int i = 0; i < 36; i++) A[i] = st->H[i];
+  for (int i = 0; i < 6; i++) perm[i] = i;
+  for (int k = 0; k < 6; k++) {
+    int piv = k;
+    double best = fabs(A[k * 6 + k]);
+    for (int i = k + 1; i < 6; i++)
+      if (fabs(A[i * 6 + k]) > best) best = fabs(A[i * 6 + k]), piv = i;
+    if (piv != k) {
+      for (int j = 0; j < 6; j++) {
+        const double t = A[k * 6 + j];
+        A[k * 6 + j] = A[piv * 6 + j], A[piv * 6 + j] = t;
+      }
+      const int t = perm[k];
+      perm[k] = perm[piv], perm[piv] = t;
+    }
+    if (A[k * 6 + k] != 0.0)
+      for (int i = k + 1; i < 6; i++) A[i * 6 + k] /= A[k * 6 + k];
+    for (int i = k + 1; i < 6; i++)
+      for (int j = k + 1; j < 6; j++) A[i * 6 + j] -= A[i * 6 + k] * A[k * 6 + j];
+  }
+  for (int col = 0; col < 6; col++) {
+    double y[6];
+    for (int i = 0; i < 6; i++) {  // L y = P e_col (unit lower)
+      double s = perm[i] == col ? 1.0 : 0.0;
+      for (int j = 0; j < i; j++) s -= A[i * 6 + j] * y[j];
+      y[i] = s;
+    }
+    for (int i = 5; i >= 0; i--) {  // U x = y
+      double s = y[i];
+      for (int j = i + 1; j < 6; j++) s -= A[i * 6 + j] * y[j];
+      y[i] = s / A[i * 6 + i];
+    }
+    for (int i = 0; i < 6; i++) out[i * 6 + col] = y[i];
+  }
+}
+
+int pose_cov_device(Ctx *c) {
+  MLOAM_CUDA_OK(c, c->pose_cov.reserve(36 * sizeof(double)));
+  k_pose_cov<<<1, 32, 0, c->stream>>>(c->lm_state.as<LMState>(), c->pose_cov.as<double>());
+  c->launches++;
+  MLOAM_CUDA_OK(c, cudaGetLastError());
+  return MLOAM_OK;
+}
+
 // What k_linearize and k_eval_candidate share: the feature sets, the grid (k_eval_candidate runs LIN_THREADS / CAND_THREADS
 // blocks per k_linearize block) and c->partials = [NE_PACK doubles per k_linearize block, max_nb + 2 of them][ticket +
 // generation word][NE_CAND doubles per k_eval_candidate warp].

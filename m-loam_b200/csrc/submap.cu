@@ -24,12 +24,21 @@ struct UctFrame {
   double cov_meas[9];
   double trace_threshold;
   int with_ua, n_lasers;
+  int scan_frame;  // 1: the scan of a with_ua frame (downsampleCurrentScan, lidar_mapper_keyframe.cpp:376-387): no pose_global transform
 };
 
+// d_f (nullable): the frame read from device memory instead of `f` (staged by a captured H2D copy, so that a replay sees new values).
+// d_n (nullable): device-side point count, n is then the launch bound; points beyond it are not kept.
 __global__ void k_uct_associate(const float4 *__restrict__ pts, int n, UctFrame f, const UctLaser *__restrict__ lasers, float4 *__restrict__ out,
-                                float *__restrict__ cov6, float *__restrict__ trace, int *__restrict__ keep) {
+                                float *__restrict__ cov6, float *__restrict__ trace, int *__restrict__ keep, const UctFrame *__restrict__ d_f = nullptr,
+                                const int *__restrict__ d_n = nullptr) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  if (d_n && i >= *d_n) {
+    keep[i] = 0;
+    return;
+  }
+  if (d_f) f = *d_f;
   const float4 po = pts[i];
   int ind = (int)po.w;  // laser id in the intensity (:1143)
   ind = ind < 0 ? 0 : (ind >= f.n_lasers ? f.n_lasers - 1 : ind);
@@ -66,8 +75,12 @@ __global__ void k_uct_associate(const float4 *__restrict__ pts, int n, UctFrame 
       }
     if (C[0] + C[3] + C[5] > f.trace_threshold) ok = 0;  // :1150
   }
-  const float3 pc = associate(pose_from_param(f.pose_global), po.x, po.y, po.z);  // :1152
-  out[i] = make_float4(pc.x, pc.y, pc.z, po.w);
+  if (f.scan_frame) {
+    out[i] = po;  // the scan stays in the base frame; only its covariance is attached (PointIWithCov(point_ori, cov), :385-386)
+  } else {
+    const float3 pc = associate(pose_from_param(f.pose_global), po.x, po.y, po.z);  // :1152
+    out[i] = make_float4(pc.x, pc.y, pc.z, po.w);
+  }
 #pragma unroll
   for (int k = 0; k < 6; k++) cov6[(size_t)i * 6 + k] = (float)C[k];  // updateCov (point_with_cov.hpp:187-196)
   trace[i] = (float)(C[0] + C[3] + C[5]);
@@ -76,7 +89,7 @@ __global__ void k_uct_associate(const float4 *__restrict__ pts, int n, UctFrame 
 
 __global__ void k_compact_cov(const float4 *__restrict__ pts, const float *__restrict__ cov6, const float *__restrict__ trace, const int *__restrict__ keep,
                               const int *__restrict__ slot, int n, int dst_off, const int *__restrict__ d_dst_off, float4 *__restrict__ out,
-                              float *__restrict__ cov6_out, float *__restrict__ trace_out) {
+                              float *__restrict__ cov6_out, float *__restrict__ trace_out, double *__restrict__ sinfo_out = nullptr) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n || !keep[i]) return;
   const int o = (d_dst_off ? *d_dst_off : dst_off) + slot[i];
@@ -84,6 +97,7 @@ __global__ void k_compact_cov(const float4 *__restrict__ pts, const float *__res
 #pragma unroll
   for (int k = 0; k < 6; k++) cov6_out[(size_t)o * 6 + k] = cov6[(size_t)i * 6 + k];
   trace_out[o] = trace[i];
+  if (sinfo_out) sinfo_out[o] = cov6_sqrt_info(cov6 + (size_t)i * 6);  // the factor's weight (extractCov + lidar_map_factor.hpp:34,41)
 }
 __global__ void k_add_count(int *total, const int *part) {
   if (threadIdx.x == 0 && blockIdx.x == 0) *total += *part;
@@ -202,6 +216,86 @@ static void fill_lasers(int n_lasers, const double *ext7, const double *pose_com
   }
 }
 
+// ---- the with_ua stage of a frame: downsampleCurrentScan's uncertainty loop (lidar_mapper_keyframe.cpp:376-407) for both scans.
+// Per point, idx = int(intensity) (the laser id of the rig merge; 0 in the single-LiDAR path without it, where intensity still
+// holds the ring): pointAssociateToMap with pose_ext[idx]^-1, evalPointUncertainty under pose_ext[idx] with its covariance, dropped
+// when trace > TRACE_THRESHOLD_MAPPING; the kept points keep their order.  This is cloudUCTAssociateToMap's per-point work with the
+// extrinsic as the compound pose and no pose_global transform, so k_uct_associate + k_compact_cov do it.
+static_assert(sizeof(UctFrame) <= 256, "UctFrame is staged in 256 B");
+static_assert(256 + sizeof(UctLaser) * MLOAM_MAX_LIDARS <= kPinnedPoseCov - kPinnedUct, "pinned staging of the with_ua stage");
+
+void ua_stage_host(Ctx *c) {
+  char *pin = reinterpret_cast<char *>(c->pinned) + kPinnedUct;
+  UctFrame *f = reinterpret_cast<UctFrame *>(pin);
+  UctLaser *L = reinterpret_cast<UctLaser *>(pin + 256);
+  const bool merged = c->n_lidars > 1 || c->lidar_merge;
+  const int n_lasers = merged ? c->n_lidars : 1;
+  memset(f, 0, 256);
+  for (int k = 0; k < 7; k++) f->pose_global[k] = k == 6 ? 1.0 : 0.0;
+  memcpy(f->cov_meas, c->ua_cov_meas, sizeof(f->cov_meas));
+  f->trace_threshold = c->ua_trace_threshold, f->with_ua = 1, f->n_lasers = n_lasers, f->scan_frame = 1;
+  for (int l = 0; l < n_lasers; l++) {
+    // pose_ext[idx]: the extrinsic the features were moved to the base frame with (identity when there is none)
+    const double *e = merged ? c->lidar_ext[l] : c->ext;
+    pose_inverse(e, L[l].ext_inv);
+    for (int k = 0; k < 7; k++) L[l].compound[k] = e[k];
+    for (int k = 0; k < 36; k++) L[l].cov[k] = c->ua_ext_cov[l][k];
+  }
+}
+
+int ua_scan_stage(Ctx *c, Ctx::ScanRef *S) {
+  const int ncap[2] = {S->n_corner, S->n_surf};
+  const float4 *pts[2] = {S->corner, S->surf};
+  const int *d_n[2] = {S->d_n_corner, S->d_n_surf};
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    size_t o = off;
+    off += (bytes + 255) & ~(size_t)255;
+    return o;
+  };
+  const size_t o_cfg = take(256 + sizeof(UctLaser) * MLOAM_MAX_LIDARS);
+  struct Set {
+    size_t staged, cov6, trace, keep, slot, tmp, out, ocov6, otrace, osinfo, count;
+  } o[2];
+  for (int t = 0; t < 2; t++) {
+    const size_t N1 = (size_t)(ncap[t] > 0 ? ncap[t] : 0) + 16;
+    o[t].staged = take(16 * N1), o[t].cov6 = take(24 * N1), o[t].trace = take(4 * N1), o[t].keep = take(4 * N1), o[t].slot = take(4 * N1);
+    o[t].tmp = take(4 * (N1 / 2048 + 8)), o[t].out = take(16 * N1), o[t].ocov6 = take(24 * N1), o[t].otrace = take(4 * N1);
+    o[t].osinfo = take(8 * N1), o[t].count = take(64);
+  }
+  MLOAM_CUDA_OK(c, c->ua_scan.reserve(off));
+  char *p = c->ua_scan.as<char>();
+  ua_stage_host(c);
+  cudaStream_t st = c->stream;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(p + o_cfg, reinterpret_cast<char *>(c->pinned) + kPinnedUct, 256 + sizeof(UctLaser) * MLOAM_MAX_LIDARS,
+                                   cudaMemcpyHostToDevice, st));
+  const UctFrame *d_f = reinterpret_cast<const UctFrame *>(p + o_cfg);
+  const UctLaser *d_l = reinterpret_cast<const UctLaser *>(p + o_cfg + 256);
+  const UctFrame f_unused{};
+  for (int t = 0; t < 2; t++) {
+    const int n = ncap[t];
+    float4 *staged = reinterpret_cast<float4 *>(p + o[t].staged), *out = reinterpret_cast<float4 *>(p + o[t].out);
+    float *cov6 = reinterpret_cast<float *>(p + o[t].cov6), *trace = reinterpret_cast<float *>(p + o[t].trace);
+    float *ocov6 = reinterpret_cast<float *>(p + o[t].ocov6), *otrace = reinterpret_cast<float *>(p + o[t].otrace);
+    int *keep = reinterpret_cast<int *>(p + o[t].keep), *slot = reinterpret_cast<int *>(p + o[t].slot), *tmp = reinterpret_cast<int *>(p + o[t].tmp);
+    int *count = reinterpret_cast<int *>(p + o[t].count);
+    double *osinfo = reinterpret_cast<double *>(p + o[t].osinfo);
+    if (n > 0) {
+      k_uct_associate<<<(n + 127) / 128, 128, 0, st>>>(pts[t], n, f_unused, d_l, staged, cov6, trace, keep, d_f, d_n[t]);
+      c->launches++;
+    }
+    scan_exclusive(c, keep, slot, n, tmp, count);  // the gated count lands where the solve reads its feature count
+    if (n > 0) {
+      k_compact_cov<<<(n + 255) / 256, 256, 0, st>>>(staged, cov6, trace, keep, slot, n, 0, nullptr, out, ocov6, otrace, osinfo);
+      c->launches++;
+    }
+    MLOAM_CUDA_OK(c, cudaGetLastError());
+    if (t == 0) S->corner = out, S->d_n_corner = count, S->sinfo_corner = osinfo, S->cov6_corner = ocov6;
+    else S->surf = out, S->d_n_surf = count, S->sinfo_surf = osinfo, S->cov6_surf = ocov6;
+  }
+  return MLOAM_OK;
+}
+
 }  // namespace mloam
 
 using namespace mloam;
@@ -268,7 +362,7 @@ int mloam_cloud_uct_associate(mloam_ctx_t *h, const mloam_point_t *h_pts, int n,
   fill_lasers(n_lasers, ext7, pose_compound7, cov_compound36, L);
   UctFrame f;
   memcpy(f.pose_global, pose_global7, sizeof(f.pose_global)), memcpy(f.cov_meas, cov_meas9, sizeof(f.cov_meas));
-  f.trace_threshold = trace_threshold, f.with_ua = with_ua ? 1 : 0, f.n_lasers = n_lasers;
+  f.trace_threshold = trace_threshold, f.with_ua = with_ua ? 1 : 0, f.n_lasers = n_lasers, f.scan_frame = 0;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_in, h_pts, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, st));
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_l, L.data(), sizeof(UctLaser) * n_lasers, cudaMemcpyHostToDevice, st));
   MLOAM_CUDA_OK(c, cudaMemsetAsync(d_total, 0, sizeof(int), st));
@@ -372,7 +466,7 @@ int mloam_submap_assemble(mloam_ctx_t *h, int slot, int n_keyframes, const mloam
   for (int k = 0; k < n_keyframes; k++) {  // `+=` keyframe after keyframe (:338-342)
     UctFrame f;
     memcpy(f.pose_global, poses7 + 7 * (size_t)k, sizeof(f.pose_global)), memcpy(f.cov_meas, cov_meas9, sizeof(f.cov_meas));
-    f.trace_threshold = trace_threshold_assoc, f.with_ua = with_ua ? 1 : 0, f.n_lasers = n_lasers;
+    f.trace_threshold = trace_threshold_assoc, f.with_ua = with_ua ? 1 : 0, f.n_lasers = n_lasers, f.scan_frame = 0;
     rc = uct_associate_append(c, d_in + off, counts[k], f, d_l + (size_t)k * n_lasers, B, d_mid, d_mc6, d_mtr, d_total);
     if (rc) return rc;
     off += (size_t)counts[k];

@@ -53,10 +53,7 @@ __global__ void k_point_uncertainty(const float4 *__restrict__ pts, int n, UctAr
 __global__ void k_sqrt_info(const float *__restrict__ cov6, int n, double *__restrict__ sinfo) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  // extractCov (point_with_cov.hpp:202-214): float cov_vec -> Matrix3d; trace summed in double
-  const double tr = (double)cov6[(size_t)i * 6] + (double)cov6[(size_t)i * 6 + 3] + (double)cov6[(size_t)i * 6 + 5];
-  const double s = sqrt(1 / tr);
-  sinfo[i] = s >= 3.0 ? 1.0 : s / 3.0;
+  sinfo[i] = cov6_sqrt_info(cov6 + (size_t)i * 6);
 }
 
 int sqrt_info_device(Ctx *c, const float *d_cov6, int n, double *d_sinfo) {
