@@ -258,7 +258,8 @@ __device__ __forceinline__ float slab_gap(float q, int c_abs, float cell, float 
 // ball), restricted to the cube of Chebyshev radius clip_r (cells) around the query's cell (cx, cy, cz) when
 // clip_r >= 0, and without the cube of radius skip_r that has been scanned already when skip_r >= 0.
 // `bound2` shrinks while scanning: lim2 = min(max_sqdist, K-th so far) is what the result needs; prune(lim2) adds the
-// caller's padding.  Returns false when the scan needs more than max_slots row slots (nothing scanned).
+// caller's padding.  Returns false when the scan needs more than max_slots row slots (nothing scanned); the blind
+// search passes an unbounded max_slots, so it always scans.
 template <int K, int N, typename Prune>
 __device__ __forceinline__ bool scan_ball(const MapView &map, const GridP &g, KnnSmem &ks, float qx, float qy, float qz, int cx, int cy, int cz,
                                           int clip_r, int skip_r, float &lim2, Prune prune, int max_slots, int lane, Best &out, KnnDbg *dbg) {
@@ -274,8 +275,8 @@ __device__ __forceinline__ bool scan_ball(const MapView &map, const GridP &g, Kn
   }
   ylo = max(ylo, 0), yhi = min(yhi, g.ny - 1), zlo = max(zlo, 0), zhi = min(zhi, g.nz - 1);
   if (ylo > yhi || zlo > zhi || xmin > xmax) return true;
+  // clamped to the grid: wy * wz <= ny * nz <= n_cells (< 2^28), so the row count fits an int whatever the ball's size
   const int wy = yhi - ylo + 1, wz = zhi - zlo + 1;
-  if (wy > 4096 || wz > 4096) return false;
   const int n_rows = wy * wz;
   // a row through the skipped cube splits into the part left of it and the part right of it: those rows get two slots
   const int sw = 2 * skip_r + 1;
