@@ -273,7 +273,8 @@ int mloam_set_lidars(mloam_ctx_t *ctx, int n_lidars, const double *ext7);
  *   loss-corrected J^T J evaluated at the pose the last Solve returned, with the last association (:600-610), inverted by partial-pivot
  *   LU as Eigen's 6x6 inverse.  mloam_scan2map_ua counts as with_ua.  Zeros without with_ua (:621), when the map gate rejected the
  *   frame (:637) and when the last evaluation had no residual rows (Eigen would return inf / NaN there).  The rule "zero while there
- *   are <= 10 keyframes" (:607-608) is the caller's, which knows the keyframe count.
+ *   are <= 10 keyframes" (:607-608) is the caller's, which knows the keyframe count — or the keyframe store's, when
+ *   mloam_keyframe_save takes the covariance itself (cov36 = NULL).
  * mloam_frame_scan: the down-sampled (and, with with_ua, gated) scans of the last mloam_frame* call in the base frame with their
  *   PointIWithCov::cov_vec (float xx xy xz yy yz zz; zeros without with_ua) — laser_cloud_{surf,corner}_cov, what saveKeyframe stores
  *   (:671-677) and mloam_submap_assemble later takes.  Outputs are nullable; capacities in points.  MLOAM_E_STATE before any frame. */
@@ -281,6 +282,45 @@ int mloam_set_uncertainty(mloam_ctx_t *ctx, int with_ua, const double *ext_cov36
 int mloam_pose_covariance(mloam_ctx_t *ctx, double *cov36);
 int mloam_frame_scan(mloam_ctx_t *ctx, mloam_point_t *h_surf, float *h_surf_cov6, int cap_surf, int *n_surf, mloam_point_t *h_corner,
                      float *h_corner_cov6, int cap_corner, int *n_corner);
+
+/* ---- the mapper's keyframe store, kept on the device: saveKeyframe -> clearCloud -> extractSurroundingKeyFrames
+ *      (lidar_mapper_keyframe.cpp:641-683, :921-927 at :1101, :254-354).  The mapper loop of process() (:1062-1101) becomes
+ *        mloam_set_lidars / mloam_set_uncertainty (the frame's /extrinsics, :1028-1046, read BEFORE the submap as the reference does:
+ *        a keyframe entering the surrounding set is associated with the values in effect at the mloam_keyframe_submap call);
+ *        pred = pose_wmap_wodom * pose_wodom_curr;  mloam_keyframe_submap(pred);  mloam_frame(..., rebuild_maps = 0, pred);
+ *        mloam_keyframe_save(NULL, NULL);  pose_wmap_wodom = pose_out * pose_wodom_curr^-1
+ *      and no point of a keyframe crosses PCIe.  Single-GPU: a context with a communicator gets MLOAM_E_STATE.
+ * mloam_keyframes_init: an empty store (DISTANCE_KEYFRAMES [m], ORIENTATION_KEYFRAMES [deg], SURROUNDING_KF_RADIUS [m], MAP_SUR_KF_RES [m],
+ *   TRACE_THRESHOLD_MAPPING for the submap association gate and both map filters) and empty map slots MLOAM_MAP_SURF / MLOAM_MAP_CORNER,
+ *   so that the first frames fail the map gate (:429).  The map filters use params.surf_leaf / corner_leaf (MAP_SURF_RES / MAP_CORNER_RES,
+ *   the leaves of the scan filters too, :1278-1289).
+ * mloam_keyframe_save: saveKeyframe for the last mloam_frame* call.  Saved when it is the first keyframe, the float distance of the positions
+ *   to the previous keyframe is > DISTANCE_KEYFRAMES, or Eigen's angularDistance 2 atan2(|(q q_prev^-1).vec|, |(q q_prev^-1).w|) in degrees
+ *   is > ORIENTATION_KEYFRAMES.  A saved keyframe keeps the frame's down-sampled, gated scans (as mloam_frame_scan returns them), copied
+ *   device to device, and marks the submap stale (clearCloud).  pose7 / cov36 NULL: the frame's pose and mloam_pose_covariance, zeroed
+ *   while the store holds <= 10 keyframes (:607-608; the count before this save is the one the solve saw); explicit values let a caller
+ *   correct keyframe poses.  *saved (nullable) = 1 when saved.  MLOAM_E_STATE if no frame has run since the last save or init.
+ * mloam_keyframe_submap: extractSurroundingKeyFrames at the frame's initial guess pose_pred7 (transformAssociateToMap).  Nothing to do
+ *   without keyframes, or while both filtered maps hold points (the reference rebuilds while either is empty).  Otherwise: the keyframes
+ *   with float squared distance d2 < radius^2 of the prediction, ascending (d2, id); ids that left the set are dropped, survivors keep
+ *   their order, new ids are appended in radius order; a new id's clouds are associated ONCE (cloudUCTAssociateToMap with its pose and
+ *   covariance and the extrinsics / covariances of mloam_set_lidars / mloam_set_uncertainty at that moment) and cached on the device while
+ *   it stays in the set; the set's positions go through VoxelGridCovarianceMLOAM<PointI>(MAP_SUR_KF_RES) with intensity = position in the
+ *   set (the last one per voxel wins); the chosen cached clouds are appended in filter order to the merged clouds (emptied by a save only),
+ *   filtered with VoxelGridCovarianceMLOAM<PointIWithCov> and built into the two map slots.  *rebuilt (nullable) = 1 when it rebuilt.
+ *   *n_surf / *n_corner: the current map sizes; h_* (nullable, capacities in points) receive the maps and their cov_vec.
+ * mloam_keyframe_query: keyframe count, surrounding_existing_keyframes_id in order, the keyframe ids the position filter chose in the last
+ *   rebuild (filter order).  Outputs nullable.
+ * mloam_keyframe_scan: keyframe `id`'s pose, covariance and stored scans (points + cov_vec; outputs nullable, capacities in points). */
+int mloam_keyframes_init(mloam_ctx_t *ctx, double distance_keyframes, double orientation_keyframes_deg, double surrounding_kf_radius,
+                         double map_sur_kf_res, double trace_threshold);
+int mloam_keyframe_save(mloam_ctx_t *ctx, const double *pose7, const double *cov36, int *saved);
+int mloam_keyframe_submap(mloam_ctx_t *ctx, const double *pose_pred7, int *rebuilt, mloam_point_t *h_surf, float *h_surf_cov6, int cap_surf,
+                          int *n_surf, mloam_point_t *h_corner, float *h_corner_cov6, int cap_corner, int *n_corner);
+int mloam_keyframe_query(mloam_ctx_t *ctx, int *n_keyframes, int *h_surrounding, int cap_surrounding, int *n_surrounding, int *h_chosen,
+                         int cap_chosen, int *n_chosen);
+int mloam_keyframe_scan(mloam_ctx_t *ctx, int id, double *pose7, double *cov36, mloam_point_t *h_surf, float *h_surf_cov6, int cap_surf,
+                        int *n_surf, mloam_point_t *h_corner, float *h_corner_cov6, int cap_corner, int *n_corner);
 
 /* ---- FeatureExtract::matchCornerFromScan / matchSurfFromScan (feature_extract.hpp:131-376) against the map slot
  * built (mloam_map_build, cell ~1.3 m) from the previous sweep's less-sharp / less-flat features, which must be in

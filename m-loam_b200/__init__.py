@@ -31,6 +31,7 @@ ABI_SYMBOLS = [
     "mloam_normal_equations", "mloam_pose_plus", "mloam_scan2map", "mloam_scan2map_device", "mloam_frame",
     "mloam_frame_device", "mloam_set_extrinsic", "mloam_set_lidars", "mloam_calib_frame", "mloam_compound_pose_cov", "mloam_cloud_uct_associate", "mloam_voxel_downsample_cov", "mloam_submap_assemble", "mloam_good_features_odom", "mloam_local_map_build", "mloam_match_from_scan", "mloam_track_cloud", "mloam_odom_solve", "mloam_point_uncertainty", "mloam_scan2map_ua", "mloam_good_features", "mloam_comm_unique_id", "mloam_comm_init", "mloam_comm_destroy", "mloam_comm_p2p_export", "mloam_comm_p2p_init", "mloam_comm_p2p_reset",
     "mloam_set_uncertainty", "mloam_pose_covariance", "mloam_frame_scan",
+    "mloam_keyframes_init", "mloam_keyframe_save", "mloam_keyframe_submap", "mloam_keyframe_query", "mloam_keyframe_scan",
 ]
 
 
@@ -529,6 +530,60 @@ class Context:
         cp, cc = np.zeros((max(nc.value, 1), 4), np.float32), np.zeros((max(nc.value, 1), 6), np.float32)
         self._ck(lib().mloam_frame_scan(self._h, _p(sp), _p(sc), sp.shape[0], C.byref(ns), _p(cp), _p(cc), cp.shape[0], C.byref(nc)))
         return sp[:ns.value].copy(), sc[:ns.value].copy(), cp[:nc.value].copy(), cc[:nc.value].copy()
+
+    # ---- keyframe store (saveKeyframe / extractSurroundingKeyFrames on the device)
+    def keyframes_init(self, distance_keyframes: float, orientation_keyframes_deg: float, surrounding_kf_radius: float, map_sur_kf_res: float,
+                       trace_threshold: float):
+        """Empty keyframe store and empty map slots (the first frames fail the map gate)."""
+        self._ck(lib().mloam_keyframes_init(self._h, C.c_double(distance_keyframes), C.c_double(orientation_keyframes_deg),
+                                            C.c_double(surrounding_kf_radius), C.c_double(map_sur_kf_res), C.c_double(trace_threshold)))
+
+    def keyframe_save(self, pose7=None, cov=None) -> bool:
+        """saveKeyframe for the last frame; None: the frame's pose / covariance (zero while <= 10 keyframes).  True when saved."""
+        p = None if pose7 is None else np.ascontiguousarray(pose7, np.float64)
+        cv = None if cov is None else np.ascontiguousarray(cov, np.float64).reshape(36)
+        saved = C.c_int(0)
+        self._ck(lib().mloam_keyframe_save(self._h, _p(p), _p(cv), C.byref(saved)))
+        return bool(saved.value)
+
+    def keyframe_submap(self, pose_pred7, want_output: bool = False):
+        """extractSurroundingKeyFrames at the prediction.  Returns (rebuilt, n_surf, n_corner), plus
+        (surf [n,4], surf_cov6, corner, corner_cov6) with want_output."""
+        pp = np.ascontiguousarray(pose_pred7, np.float64)
+        rb, ns, nc = C.c_int(0), C.c_int(0), C.c_int(0)
+        if not want_output:
+            self._ck(lib().mloam_keyframe_submap(self._h, _p(pp), C.byref(rb), None, None, 0, C.byref(ns), None, None, 0, C.byref(nc)))
+            return bool(rb.value), ns.value, nc.value
+        # a filtered map holds at most as many points as all stored keyframes together
+        cap = [1, 1]
+        for k in range(self.keyframe_query()[0]):
+            a, b = C.c_int(0), C.c_int(0)
+            self._ck(lib().mloam_keyframe_scan(self._h, k, None, None, None, None, 0, C.byref(a), None, None, 0, C.byref(b)))
+            cap[0] += a.value
+            cap[1] += b.value
+        sp, sc = np.zeros((cap[0], 4), np.float32), np.zeros((cap[0], 6), np.float32)
+        cp, cc = np.zeros((cap[1], 4), np.float32), np.zeros((cap[1], 6), np.float32)
+        self._ck(lib().mloam_keyframe_submap(self._h, _p(pp), C.byref(rb), _p(sp), _p(sc), cap[0], C.byref(ns), _p(cp), _p(cc), cap[1], C.byref(nc)))
+        return bool(rb.value), sp[:ns.value].copy(), sc[:ns.value].copy(), cp[:nc.value].copy(), cc[:nc.value].copy()
+
+    def keyframe_query(self):
+        """(keyframe count, surrounding ids in order, ids chosen by the last rebuild's position filter)."""
+        nk, ns, nch = C.c_int(0), C.c_int(0), C.c_int(0)
+        self._ck(lib().mloam_keyframe_query(self._h, C.byref(nk), None, 0, C.byref(ns), None, 0, C.byref(nch)))
+        sur, ch = np.zeros(max(ns.value, 1), np.int32), np.zeros(max(nch.value, 1), np.int32)
+        self._ck(lib().mloam_keyframe_query(self._h, C.byref(nk), _p(sur), sur.shape[0], C.byref(ns), _p(ch), ch.shape[0], C.byref(nch)))
+        return nk.value, sur[:ns.value].tolist(), ch[:nch.value].tolist()
+
+    def keyframe_scan(self, kf_id: int):
+        """Keyframe kf_id as stored: (pose7, cov 6x6, surf [n,4], surf_cov6, corner, corner_cov6)."""
+        pose, cov = np.zeros(7), np.zeros(36)
+        ns, nc = C.c_int(0), C.c_int(0)
+        self._ck(lib().mloam_keyframe_scan(self._h, int(kf_id), None, None, None, None, 0, C.byref(ns), None, None, 0, C.byref(nc)))
+        sp, sc = np.zeros((max(ns.value, 1), 4), np.float32), np.zeros((max(ns.value, 1), 6), np.float32)
+        cp, cc = np.zeros((max(nc.value, 1), 4), np.float32), np.zeros((max(nc.value, 1), 6), np.float32)
+        self._ck(lib().mloam_keyframe_scan(self._h, int(kf_id), _p(pose), _p(cov), _p(sp), _p(sc), sp.shape[0], C.byref(ns), _p(cp), _p(cc),
+                                           cp.shape[0], C.byref(nc)))
+        return pose, cov.reshape(6, 6), sp[:ns.value].copy(), sc[:ns.value].copy(), cp[:nc.value].copy(), cc[:nc.value].copy()
 
     def set_extrinsic(self, ext7=None):
         e = None if ext7 is None else np.ascontiguousarray(ext7, np.float64)

@@ -139,6 +139,7 @@ void mloam_ctx_destroy(mloam_ctx_t *h) {
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
   mloam_comm_destroy(h);
+  keyframes_release(c);
   for (auto &g : c->graphs)
     if (g.exec) cudaGraphExecDestroy(g.exec);
   c->graphs.clear();

@@ -128,6 +128,8 @@ struct MatchCfg {
   int n_neigh, check_fov;
 };
 
+struct KeyframeStore;
+
 struct Ctx {
   int device = 0;
   int sm_count = 132;
@@ -281,6 +283,10 @@ struct Ctx {
   double pose_cov36[36] = {0};     // pose_wmap_curr.cov_ of the last mloam_frame* / mloam_scan2map* call
   bool last_scan_valid = false;    // last_scan describes the scan of the last mloam_frame* call (mloam_frame_scan)
   ScanRef last_scan{};
+  // keyframe store (keyframe.cu, mloam_keyframes_init): saveKeyframe / extractSurroundingKeyFrames on device-resident keyframes
+  KeyframeStore *kf = nullptr;
+  double last_pose7[7] = {0, 0, 0, 0, 0, 0, 1};  // pose_wmap_curr returned by the last mloam_frame* call
+  bool frame_since_save = false;   // an mloam_frame* call has run since the last mloam_keyframe_save / mloam_keyframes_init
 };
 
 constexpr size_t kPinnedUct = 49152;      // inside Ctx::pinned: UctFrame (256 B) + MLOAM_MAX_LIDARS UctLaser of the with_ua frame stage
@@ -384,6 +390,8 @@ int ua_scan_stage(Ctx *c, Ctx::ScanRef *S);
 void ua_stage_host(Ctx *c);
 // solve_kernels.cu: Ctx::pose_cov <- LMState::H^-1 (partial-pivot LU), zeros when the last evaluation had no residual rows
 int pose_cov_device(Ctx *c);
+// keyframe.cu: frees the keyframe store (mloam_ctx_destroy)
+void keyframes_release(Ctx *c);
 
 // comm.cu: in-place sum over ranks on the context stream (no-op without a communicator)
 int comm_allreduce_doubles(Ctx *c, double *d_buf, int count);

@@ -478,6 +478,13 @@ int frame_run(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, con
     key = fnv1a(key, c->lidar_ext, sizeof(double) * 7 * (size_t)c->n_lidars);
     key = fnv1a(key, &c->stream, sizeof(c->stream));
     key = fnv1a(key, &c->with_ua, sizeof(c->with_ua));  // the covariances and the threshold are staged, not part of the key
+    if (!rebuild_maps) {
+      // the map-size gate (scan2map_enqueue) is decided on the host at capture: with maps built outside the frame (mloam_map_build*,
+      // mloam_submap_assemble, mloam_keyframe_submap) a graph captured while it failed must not be replayed once it passes, and back
+      const MapStorage &MS = c->maps[MLOAM_MAP_SURF], &MC = c->maps[MLOAM_MAP_CORNER];
+      const int gate = (MS.built && MC.built && MS.m > 50 && MC.m > 10) ? 1 : 0;
+      key = fnv1a(key, &gate, sizeof(gate));
+    }
     {  // look-ahead: which half holds this sweep's features (or that they are extracted now), and the announced next sweep
       const void *key_now = c->cloud_key ? c->cloud_key : static_cast<const void *>(d_cloud);
       const bool have = frame_has_prefetched(c, key_now, n, n_scans);
@@ -750,6 +757,7 @@ int mloam_frame_device(mloam_ctx_t *h, const mloam_point_t *d_cloud, int n, cons
                  reinterpret_cast<const float4 *>(d_surf_map), n_surf_map, reinterpret_cast<const float4 *>(d_corner_map),
                  n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
   c->next_pending = false, c->next.set = false;
+  if (rc == MLOAM_OK) memcpy(c->last_pose7, pose_out7, sizeof(c->last_pose7)), c->frame_since_save = true;  // mloam_keyframe_save
   return rc;
 }
 
@@ -822,6 +830,7 @@ int mloam_frame(mloam_ctx_t *h, const mloam_point_t *h_cloud, int n, const int *
   const int rc = frame_run(c, d_cloud, n, d_ss, d_se, n_scans, d_sm, n_surf_map, d_cm, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
   c->cloud_key = nullptr;
   c->maps_pending = false, c->next_pending = false, c->next.set = false;
+  if (rc == MLOAM_OK) memcpy(c->last_pose7, pose_out7, sizeof(c->last_pose7)), c->frame_since_save = true;  // mloam_keyframe_save
   return rc;
 }
 
