@@ -110,14 +110,13 @@ int mloam_ctx_create(int device, const mloam_params_t *params, mloam_ctx_t **out
       cudaEventCreateWithFlags(&c->ev_fork5, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&c->ev_join5, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&c->ev_next, cudaEventDisableTiming) != cudaSuccess ||
-      cudaMallocHost(&c->pinned, kPinnedBytes) != cudaSuccess || c->lm_state.reserve(sizeof(LMState) + 64) != cudaSuccess ||
-      c->scratch[7].reserve(4096) != cudaSuccess) {
+      cudaMallocHost(reinterpret_cast<void **>(&c->pinned), sizeof(PinnedBlock)) != cudaSuccess ||
+      c->lm_state.reserve(sizeof(LMState) + 64) != cudaSuccess || c->ctl.reserve(sizeof(DevCtl)) != cudaSuccess) {
     delete h;
     return MLOAM_E_CUDA;
   }
-  c->pinned_cap = kPinnedBytes;
-  memset(c->pinned, 0, kPinnedBytes);
-  cudaMemset(c->scratch[7].p, 0, 4096);
+  memset(c->pinned, 0, sizeof(PinnedBlock));
+  cudaMemset(c->ctl.p, 0, sizeof(DevCtl));
   if (const char *e = getenv("MLOAM_DISABLE_GRAPHS")) c->use_graphs = (e[0] == '0' || e[0] == '\0') ? 1 : 0;
   if (const char *e = getenv("MLOAM_KNN_TRACE")) c->knn_trace_on = e[0] == '1';
   if (const char *e = getenv("MLOAM_KNN_MB")) {
@@ -152,7 +151,9 @@ void mloam_ctx_destroy(mloam_ctx_t *h) {
   for (int i = 0; i < 2; i++) c->gf_work[i].release();
   c->knn_heavy_list.release(), c->knn_trace.release(), c->knn_spec.release();
   c->partials.release(), c->lm_state.release();
-  for (auto &s : c->scratch) s.release();
+  for (DevBuf *b : {&c->sweep_in, &c->map_in[0], &c->map_in[1], &c->extract_work, &c->voxel_work, &c->voxel_corner, &c->voxel_surf,
+                    &c->host_work, &c->odom_work, &c->ctl})
+    b->release();
   c->frame_main.release(), c->frame_alt.release(), c->next_in.release(), c->stamps.release(), c->ua_scan.release(), c->pose_cov.release();
   if (c->pinned) cudaFreeHost(c->pinned);
   if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
@@ -212,35 +213,29 @@ int mloam_profile_get(mloam_ctx_t *h, const char *name, double *ms_total, long l
     return MLOAM_OK;
   }
   // query counts / SM cycles of the matcher's search paths (k_match_knn), reported through `launches`
-  if (!strncmp(name, "knn_slow_rec", 12) && name[12] >= '0' && name[12] <= '9') {
-    long long v = 0;
-    MLOAM_CUDA_OK(c, cudaMemcpy(&v, c->scratch[7].as<char>() + kKnnPathStatsOffset + 160 + 8 * (size_t)(name[12] - '0'), 8, cudaMemcpyDeviceToHost));
-    if (ms_total) *ms_total = 0.0;
-    if (launches) *launches = v;
-    return MLOAM_OK;
+  const bool slow_rec = !strncmp(name, "knn_slow_rec", 12) && name[12] >= '0' && name[12] <= '9';
+  if (slow_rec || !strncmp(name, "knn_", 4)) {
+    KnnPathStats s;
+    MLOAM_CUDA_OK(c, cudaMemcpy(&s, &c->ctl.as<DevCtl>()->knn_stats, sizeof(s), cudaMemcpyDeviceToHost));
+    static const char *kBlind[8] = {"knn_blind_cycles_coarse", "knn_blind_cycles_ring1", "knn_blind_cycles_finish", "knn_blind_ring1_points",
+                                    "knn_blind_finish_points", "knn_blind_finish_blocks", "knn_blind_finish_cells", "knn_blind_finish_queries"};
+    static const char *kPaths[12] = {"knn_keep_matched", "knn_keep_rejected", "knn_ball", "knn_blind", "knn_max_query_cycles",
+                                     "knn_queries_over_32k_cycles", "knn_queries_over_64k_cycles", "knn_cycles_keep_matched",
+                                     "knn_cycles_keep_rejected", "knn_cycles_ball", "knn_cycles_blind", "knn_slowest_query"};
+    const unsigned long long paths[12] = {s.queries[0], s.queries[1], s.queries[2], s.queries[3], s.max_query_cycles, s.over_32k, s.over_64k,
+                                          s.cycles[0], s.cycles[1], s.cycles[2], s.cycles[3], s.slowest};
+    bool found = slow_rec;
+    long long v = slow_rec ? s.slow_rec[name[12] - '0'] : 0;
+    for (int k = 0; k < 8 && !found; k++)
+      if (!strcmp(name, kBlind[k])) v = (long long)s.blind[k], found = true;
+    for (int k = 0; k < 12 && !found; k++)
+      if (!strcmp(name, kPaths[k])) v = (long long)paths[k], found = true;
+    if (found) {
+      if (ms_total) *ms_total = 0.0;
+      if (launches) *launches = v;
+      return MLOAM_OK;
+    }
   }
-  static const char *kBlind[8] = {"knn_blind_cycles_coarse", "knn_blind_cycles_ring1", "knn_blind_cycles_finish", "knn_blind_ring1_points",
-                                  "knn_blind_finish_points", "knn_blind_finish_blocks", "knn_blind_finish_cells", "knn_blind_finish_queries"};
-  for (int k = 0; k < 8; k++)
-    if (!strcmp(name, kBlind[k])) {
-      unsigned long long v = 0;
-      MLOAM_CUDA_OK(c, cudaMemcpy(&v, c->scratch[7].as<char>() + kKnnPathStatsOffset + 96 + 8 * (size_t)k, 8, cudaMemcpyDeviceToHost));
-      if (ms_total) *ms_total = 0.0;
-      if (launches) *launches = (long long)v;
-      return MLOAM_OK;
-    }
-  static const char *kPaths[12] = {"knn_keep_matched", "knn_keep_rejected", "knn_ball", "knn_blind", "knn_max_query_cycles",
-                                   "knn_queries_over_32k_cycles", "knn_queries_over_64k_cycles", "knn_cycles_keep_matched",
-                                   "knn_cycles_keep_rejected", "knn_cycles_ball", "knn_cycles_blind", "knn_slowest_query"};
-  for (int k = 0; k < 12; k++)
-    if (!strcmp(name, kPaths[k])) {
-      unsigned long long v = 0;
-      const size_t off = kKnnPathStatsOffset + (k < 7 ? 4 * (size_t)k : 32 + 8 * (size_t)(k - 7));
-      MLOAM_CUDA_OK(c, cudaMemcpy(&v, c->scratch[7].as<char>() + off, k < 7 ? 4 : 8, cudaMemcpyDeviceToHost));
-      if (ms_total) *ms_total = 0.0;
-      if (launches) *launches = (long long)v;
-      return MLOAM_OK;
-    }
   auto it = c->prof.find(name);
   if (ms_total) *ms_total = it == c->prof.end() ? 0.0 : it->second.ms;
   if (launches) *launches = it == c->prof.end() ? 0 : it->second.launches;
@@ -250,7 +245,7 @@ int mloam_profile_reset(mloam_ctx_t *h) {
   if (!h) return MLOAM_E_INVALID;
   cudaStreamSynchronize(h->c.stream);
   prof_collect(&h->c);
-  cudaMemset(h->c.scratch[7].as<char>() + kKnnPathStatsOffset, 0, 256);
+  cudaMemset(&h->c.ctl.as<DevCtl>()->knn_stats, 0, sizeof(KnnPathStats));
   h->c.prof.clear();
   return MLOAM_OK;
 }
@@ -267,7 +262,7 @@ int mloam_map_build(mloam_ctx_t *h, int slot, const mloam_point_t *h_pts, int m,
   if (!h || (!h_pts && m > 0) || m < 0) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
   cudaSetDevice(c->device);
-  DevBuf &stage = c->scratch[0];
+  DevBuf &stage = c->sweep_in;
   MLOAM_CUDA_OK(c, stage.reserve(sizeof(float4) * (size_t)(m + 1)));
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(stage.p, h_pts, sizeof(float4) * (size_t)m, cudaMemcpyHostToDevice, c->stream));
   return map_build_device(c, slot, stage.as<float4>(), m, pick_cell(c, cell));
@@ -323,20 +318,22 @@ int mloam_knn(mloam_ctx_t *h, int slot, const mloam_point_t *h_q, int nq, const 
   Ctx *c = &h->c;
   cudaSetDevice(c->device);
   if (nq == 0) return MLOAM_OK;
-  MLOAM_CUDA_OK(c, c->scratch[1].reserve(sizeof(float4) * (size_t)nq));
-  MLOAM_CUDA_OK(c, c->scratch[2].reserve(sizeof(int) * (size_t)nq * k));
-  MLOAM_CUDA_OK(c, c->scratch[3].reserve(sizeof(float) * (size_t)nq * k));
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->scratch[1].p, h_q, sizeof(float4) * (size_t)nq, cudaMemcpyHostToDevice, c->stream));
+  float4 *d_q;
+  int *d_idx;
+  float *d_sqd;
+  MLOAM_CUDA_OK(c, carve(c->host_work, [&](Carve &cv) {
+    d_q = cv.take<float4>(nq), d_idx = cv.take<int>((size_t)nq * k), d_sqd = cv.take<float>((size_t)nq * k);
+  }));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_q, h_q, sizeof(float4) * (size_t)nq, cudaMemcpyHostToDevice, c->stream));
   double *d_pose = nullptr;
   if (pose7) {
     int rc = upload_pose(c, pose7, &d_pose);
     if (rc) return rc;
   }
-  int rc = knn_device(c, slot, c->scratch[1].as<float4>(), nq, d_pose, k, max_sqdist, c->scratch[2].as<int>(),
-                      c->scratch[3].as<float>());
+  int rc = knn_device(c, slot, d_q, nq, d_pose, k, max_sqdist, d_idx, d_sqd);
   if (rc) return rc;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_idx, c->scratch[2].p, sizeof(int) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream));
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_sqdist, c->scratch[3].p, sizeof(float) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_idx, d_idx, sizeof(int) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_sqdist, d_sqd, sizeof(float) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
   return MLOAM_OK;
 }
@@ -381,24 +378,21 @@ int mloam_factor_evaluate(mloam_ctx_t *h, int kind, int n, const double *h_point
   const int rows = kind == 2 ? 3 : 1;
   const int cols = kind >= 3 ? 21 : 7;
   const int np = kind >= 3 ? 21 : 7;
-  DevBuf &dp = c->scratch[1], &dc = c->scratch[2], &ds = c->scratch[3], &dr = c->scratch[4], &dj = c->scratch[5], &dx = c->scratch[6];
-  MLOAM_CUDA_OK(c, dp.reserve(sizeof(double) * 3 * (size_t)n));
-  MLOAM_CUDA_OK(c, dc.reserve(sizeof(double) * 6 * (size_t)n));
-  MLOAM_CUDA_OK(c, ds.reserve(sizeof(double) * (size_t)n));
-  MLOAM_CUDA_OK(c, dr.reserve(sizeof(double) * rows * (size_t)n));
-  MLOAM_CUDA_OK(c, dj.reserve(sizeof(double) * rows * cols * (size_t)n));
-  MLOAM_CUDA_OK(c, dx.reserve(sizeof(double) * 32));
+  double *dp, *dc, *ds, *dr, *dj, *dx;
+  MLOAM_CUDA_OK(c, carve(c->host_work, [&](Carve &cv) {
+    dp = cv.take<double>(3 * (size_t)n), dc = cv.take<double>(6 * (size_t)n), ds = cv.take<double>(n);
+    dr = cv.take<double>(rows * (size_t)n), dj = cv.take<double>(rows * cols * (size_t)n), dx = cv.take<double>(32);
+  }));
   cudaStream_t st = c->stream;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(dp.p, h_points, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice, st));
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(dc.p, h_coeffs, sizeof(double) * 6 * (size_t)n, cudaMemcpyHostToDevice, st));
-  if (h_sqrt_info) MLOAM_CUDA_OK(c, cudaMemcpyAsync(ds.p, h_sqrt_info, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice, st));
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(dx.p, h_params, sizeof(double) * np, cudaMemcpyHostToDevice, st));
-  int rc = factor_evaluate_device(c, kind, n, dp.as<double>(), dc.as<double>(), h_sqrt_info ? ds.as<double>() : nullptr,
-                                  dx.as<double>(), dr.as<double>(), h_jacobians ? dj.as<double>() : nullptr);
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(dp, h_points, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice, st));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(dc, h_coeffs, sizeof(double) * 6 * (size_t)n, cudaMemcpyHostToDevice, st));
+  if (h_sqrt_info) MLOAM_CUDA_OK(c, cudaMemcpyAsync(ds, h_sqrt_info, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice, st));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(dx, h_params, sizeof(double) * np, cudaMemcpyHostToDevice, st));
+  int rc = factor_evaluate_device(c, kind, n, dp, dc, h_sqrt_info ? ds : nullptr, dx, dr, h_jacobians ? dj : nullptr);
   if (rc) return rc;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_residuals, dr.p, sizeof(double) * rows * (size_t)n, cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_residuals, dr, sizeof(double) * rows * (size_t)n, cudaMemcpyDeviceToHost, st));
   if (h_jacobians)
-    MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_jacobians, dj.p, sizeof(double) * rows * cols * (size_t)n, cudaMemcpyDeviceToHost, st));
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_jacobians, dj, sizeof(double) * rows * cols * (size_t)n, cudaMemcpyDeviceToHost, st));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
   return MLOAM_OK;
 }
@@ -433,11 +427,11 @@ int mloam_normal_equations(mloam_ctx_t *h, int n, const unsigned char *h_types, 
   double *d_pose;
   int rc = upload_pose(c, pose7, &d_pose);
   if (rc) return rc;
-  MLOAM_CUDA_OK(c, c->scratch[6].reserve(sizeof(double) * 32));
-  rc = linearize_device(c, sets, 2, sqrt_info, huber_a, d_pose, 0, 0, c->scratch[6].as<double>());
+  double *d_ne = c->ctl.as<DevCtl>()->normal_eq;
+  rc = linearize_device(c, sets, 2, sqrt_info, huber_a, d_pose, 0, 0, d_ne);
   if (rc) return rc;
-  double *ne = reinterpret_cast<double *>(c->pinned) + 64;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(ne, c->scratch[6].p, sizeof(double) * 30, cudaMemcpyDeviceToHost, c->stream));
+  double *ne = c->pinned->normal_eq;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(ne, d_ne, sizeof(double) * 30, cudaMemcpyDeviceToHost, c->stream));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
   int q = 0;
   for (int i = 0; i < 6; i++)
@@ -454,12 +448,11 @@ int mloam_pose_plus(mloam_ctx_t *h, const double *x7, const double *delta6, cons
   if (!h || !x7 || !delta6 || !out7) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
   cudaSetDevice(c->device);
-  double *stage = reinterpret_cast<double *>(c->pinned) + 128;
+  double *stage = c->pinned->pose_plus;
   for (int k = 0; k < 7; k++) stage[k] = x7[k];
   for (int k = 0; k < 6; k++) stage[8 + k] = delta6[k];
   for (int k = 0; k < 36; k++) stage[16 + k] = V36 ? V36[k] : (k % 7 == 0 ? 1.0 : 0.0);
-  MLOAM_CUDA_OK(c, c->scratch[6].reserve(sizeof(double) * 64));
-  double *d = c->scratch[6].as<double>();
+  double *d = c->ctl.as<DevCtl>()->pose_plus;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d, stage, sizeof(double) * 52, cudaMemcpyHostToDevice, c->stream));
   k_pose_plus<<<1, 32, 0, c->stream>>>(d, d + 8, d + 16, d + 56);
   c->launches++;

@@ -7,6 +7,7 @@
 
 #include "../../include/mloam_b200.h"
 #include "common.cuh"
+#include "layout.h"
 
 namespace mloam {
 
@@ -75,10 +76,96 @@ struct DevBuf {
   }
 };
 
+// Reserve `b` for the regions `layout` (a callable on a Carve &) takes, then point them into it: a layout lists its regions once.
+template <typename Layout>
+cudaError_t carve(DevBuf &b, Layout &&layout) {
+  Carve sizing;
+  layout(sizing);
+  const cudaError_t e = b.reserve(sizing.size);
+  if (e != cudaSuccess) return e;
+  Carve cv(b.p);
+  layout(cv);
+  return cudaSuccess;
+}
+
 #define MLOAM_MAX_RINGS 1024  // rings of one (possibly multi-LiDAR) extraction
 #define MLOAM_MAX_LIDARS 16
 
-constexpr size_t kMapStatsOffset = 16384;  // pinned: 64 B per map slot, the GridHdr head of the slot's last build (auto cell)
+// the per-point association with uncertainty (uct.h): per LiDAR of the rig, and per run
+struct UctLaser {
+  double ext_inv[7];   // pose_ext[n].inverse()
+  double compound[7];  // pose_global * pose_ext[n]
+  double cov[36];      // its covariance (compoundPoseWithCov)
+};
+struct UctFrame {
+  double pose_global[7];
+  double cov_meas[9];
+  double trace_threshold;
+  int with_ua, n_lasers;
+  int scan_frame;  // 1: the scan of a with_ua frame (downsampleCurrentScan, lidar_mapper_keyframe.cpp:376-387): no pose_global transform
+};
+static_assert(sizeof(UctFrame) <= 256, "UctFrame is staged in 256 B");
+// the configuration of a frame's with_ua stage, copied to the device as one block (submap.cu ua_scan_stage)
+struct UaStage {
+  UctFrame frame;
+  alignas(256) UctLaser lasers[MLOAM_MAX_LIDARS];
+};
+static_assert(sizeof(UaStage) == 256 + sizeof(UctLaser) * MLOAM_MAX_LIDARS, "with_ua stage layout");
+
+// The context's pinned host block (Ctx::pinned): staging of small host-to-device copies and landing of small read-backs, so that
+// they are truly asynchronous.
+struct PinnedBlock {
+  // Read by captured copies: a frame graph copies these to the device at execution time, so every replay writes them again first
+  // (pipeline.cu stage_frame_inputs).
+  double pose[7];                   // lm_init_state: the initial pose of a solve
+  double ext[7];                    // features_enqueue: the single sensor -> base extrinsic
+  float rig[MLOAM_MAX_LIDARS][12];  // features_enqueue: the rig's float 3x4 extrinsics of the merge
+  UaStage ua;                       // ua_scan_stage: the with_ua configuration
+  // Written by captured copies (landing of a frame's results) and by the host-buffer entry points, one call at a time
+  LMState lm;                       // LMState mirror
+  int counts[192];                  // count read-backs; mloam_project_cloud: [0] count, [64..] scan starts, [128..] scan ends
+  double pose_cov[36];              // H^-1 of the last solve (with_ua)
+  GridHdr map_hdr[MLOAM_NUM_MAPS];  // map_build_device: the GridHdr head of each slot's last build (auto cell)
+  int done;                         // LM done-flag poll of the solves with max_inner > 1
+  double upload_pose[7];            // upload_pose
+  double odom_x[28];                // odometry / calibration / good-feature poses (DevCtl::odom_x)
+  alignas(16) unsigned char odom[4096];  // OdomState mirror (odom_kernels.cu)
+  double normal_eq[30];             // mloam_normal_equations read-back
+  double pose_plus[64];             // mloam_pose_plus: x | delta | V in, result at [56]
+  int scan_info[2][MLOAM_MAX_RINGS];       // mloam_frame: ScanInfo of the sweep (start | end)
+  int scan_info_next[2][MLOAM_MAX_RINGS];  // ... and of the announced next sweep, copied on stream4
+};
+
+// Matcher counters of k_match_knn with stage profiling on (mloam_profile_get "knn_*"); zeroed at creation and by mloam_profile_reset
+struct KnnPathStats {
+  unsigned queries[4];           // per search path: 0 keep (matched), 1 keep (rejected), 2 ball, 3 blind
+  unsigned max_query_cycles;
+  unsigned over_32k, over_64k;   // queries over 32k / 64k cycles
+  unsigned pad0;
+  unsigned long long cycles[4];  // SM cycles per path
+  unsigned long long slowest;    // cycles << 32 | path << 30 | set << 29 | feature index
+  unsigned long long pad1[3];
+  unsigned long long blind[8];   // blind searches: 0, cycles of ring 1 / ball, ring-1 points, ball points / steps / rows, queries with a ball
+  long long slow_rec[10];        // one blind query over 90k cycles
+  long long pad2[2];
+};
+static_assert(sizeof(KnnPathStats) == 256 && offsetof(KnnPathStats, cycles) == 32 && offsetof(KnnPathStats, blind) == 96 &&
+                  offsetof(KnnPathStats, slow_rec) == 160,
+              "k_match_knn addresses the counters by these offsets");
+
+// Device control words (Ctx::ctl): the device ends of the pinned staging and small fixed-size results
+struct DevCtl {
+  double pose[8];                       // PinnedBlock::pose
+  double upload_pose[8];                // PinnedBlock::upload_pose
+  double ext[8];                        // PinnedBlock::ext
+  double odom_x[32];                    // PinnedBlock::odom_x: 21 (odometry, good features) or 28 (calibration) doubles
+  double match_pose[2][8];              // calibration: the poses its two feature groups are matched at
+  double normal_eq[32];                 // mloam_normal_equations
+  double pose_plus[64];                 // mloam_pose_plus
+  float rig[MLOAM_MAX_LIDARS][12];      // PinnedBlock::rig
+  int merge_off[2 * (MLOAM_MAX_LIDARS + 1)];  // merge_lidars_device: per-LiDAR feature offsets
+  KnnPathStats knn_stats;
+};
 
 struct MapStorage {
   DevBuf sorted, orig, cells, rank_of, tile_sums, hdr;
@@ -99,9 +186,9 @@ struct MapStorage {
   // Sticky auto cell: a cell edge that gives a few points per occupied cell lets the 3x3x3 neighbourhood of a query
   // hold its K neighbours (knn.cuh ring 1).  Decided from the header the previous build of this slot copied to pinned
   // memory (possibly one build stale — it only steers speed, never results).  Power-of-two edges only.
-  float auto_cell_pick(const void *pinned, int slot) {
+  float auto_cell_pick(const PinnedBlock *pinned, int slot) {
     if (built && pinned) {
-      const GridHdr *h = reinterpret_cast<const GridHdr *>(reinterpret_cast<const char *>(pinned) + kMapStatsOffset + 64 * slot);
+      const GridHdr *h = &pinned->map_hdr[slot];
       if (h->n_occupied > 0 && h->n_sorted > 0 && h->cell > 0.f) {
         const float avg = (float)h->n_sorted / (float)h->n_occupied;
         float cur = h->cell;
@@ -113,9 +200,6 @@ struct MapStorage {
     return auto_cell;
   }
 };
-
-constexpr size_t kPinnedScanInfo = 32768, kPinnedScanInfoNext = 40960;  // 2 x MLOAM_MAX_RINGS ints each inside Ctx::pinned (ScanInfo staging of mloam_frame / of the announced sweep)
-constexpr size_t kKnnPathStatsOffset = 3072;  // 64 B of matcher counters inside Ctx::scratch[7] (zeroed at creation / profile reset)
 
 struct ProfSlot {
   double ms = 0;
@@ -164,9 +248,19 @@ struct Ctx {
   DevBuf partials;                // per-block packed normal equations
   DevBuf lm_state;                // LMState
   void *ticket_zeroed_for = nullptr;  // partials allocation whose last-block ticket has been zeroed
-  DevBuf scratch[10];             // general scratch (knn outputs, factor batches, extraction, voxel)
-  void *pinned = nullptr;         // pinned host staging (LMState mirror + small results)
-  size_t pinned_cap = 0;
+  // Work buffers, named by their role in a frame.  The host-buffer entry points, each one synchronous call, stage through them too.
+  DevBuf sweep_in;                // mloam_frame: the sweep + its ScanInfo.  Host entry points: their input
+  DevBuf map_in[2];               // mloam_frame: the surf / corner submap uploads on stream2.  Host entry points: [0] their output
+  DevBuf extract_work;            // extract_device (extract_work_layout); the look-ahead branch reuses it after the current extraction
+  DevBuf voxel_work;              // voxel filters of the host entry points and of the keyframe submap
+  DevBuf voxel_corner, voxel_surf;  // the frame's two scan filters, on two streams at once; the look-ahead branch forks after them
+  DevBuf host_work;               // host entry points: work and output staging (good features, kNN, factors, scan2map_ua, ...)
+  DevBuf odom_work;               // OdomState + partials of mloam_odom_solve / mloam_calib_frame
+  // association work (uct.h uct_bufs) of the keyframe submap and the host entry points: never inside a frame, so it shares the
+  // corner submap upload's allocation
+  DevBuf &assoc_work() { return map_in[1]; }
+  DevBuf ctl;                     // DevCtl
+  PinnedBlock *pinned = nullptr;
 
   // profiling with CUDA events on `stream`
   bool prof_on = false;
@@ -271,7 +365,7 @@ struct Ctx {
   bool p2p_collective = false;     // the solve being enqueued is the collective one (all ranks in lock-step): sum over the ranks
   // uncertainty-aware mapping in the frame path (mloam_set_uncertainty): the per-point uncertainty + trace gate of
   // downsampleCurrentScan (lidar_mapper_keyframe.cpp:356-421) between the scan filters and the solve, and the pose covariance
-  // H^-1 at the returned pose (:600-610).  The covariances reach the device through the pinned block (kPinnedUct), so a
+  // H^-1 at the returned pose (:600-610).  The covariances reach the device through the pinned block (PinnedBlock::ua), so a
   // captured frame replays with new values.
   int with_ua = 0;
   double ua_ext_cov[MLOAM_MAX_LIDARS][36];  // per LiDAR: pose_ext[l].cov_, row-major [translation | rotation]
@@ -288,9 +382,6 @@ struct Ctx {
   double last_pose7[7] = {0, 0, 0, 0, 0, 0, 1};  // pose_wmap_curr returned by the last mloam_frame* call
   bool frame_since_save = false;   // an mloam_frame* call has run since the last mloam_keyframe_save / mloam_keyframes_init
 };
-
-constexpr size_t kPinnedUct = 49152;      // inside Ctx::pinned: UctFrame (256 B) + MLOAM_MAX_LIDARS UctLaser of the with_ua frame stage
-constexpr size_t kPinnedPoseCov = 57344;  // inside Ctx::pinned: 36 doubles, H^-1 of the last solve
 
 // RAII-less helper: bracket a kernel (or a few) with events when profiling is on.
 struct ProfScope {
@@ -385,9 +476,13 @@ int gf_select_set_device(Ctx *c, int t, const FeatSet &fs, const double *d_pose7
 int sqrt_info_device(Ctx *c, const float *d_cov6, int n, double *d_sinfo);
 // submap.cu: the with_ua stage of a frame (downsampleCurrentScan, lidar_mapper_keyframe.cpp:356-421) on c->stream.  The scans of *S
 // (device counts) -> per point ext^-1 -> evalPointUncertainty under pose_ext -> trace gate -> stable compaction into Ctx::ua_scan with
-// cov6 and sqrt_info; *S then points at the gated scans.  ua_stage_host writes the staged configuration (replays re-run it).
+// cov6 and sqrt_info; *S then points at the gated scans.  ua_stage_host writes the staged configuration (PinnedBlock::ua).
 int ua_scan_stage(Ctx *c, Ctx::ScanRef *S);
 void ua_stage_host(Ctx *c);
+// pipeline.cu: writers of the pinned fields a captured frame graph reads (PinnedBlock), shared by the enqueue and the replay paths
+void stage_pose(Ctx *c, const double *pose7);
+void stage_ext(Ctx *c);
+void stage_rig(Ctx *c);
 // solve_kernels.cu: Ctx::pose_cov <- LMState::H^-1 (partial-pivot LU), zeros when the last evaluation had no residual rows
 int pose_cov_device(Ctx *c);
 // keyframe.cu: frees the keyframe store (mloam_ctx_destroy)
@@ -403,6 +498,18 @@ struct ExtractOut {
 };
 int extract_device(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, const int *d_scan_end, int n_scans,
                    ExtractOut out, float *d_curv_or_null, int *d_label_or_null);
+// extract_device's work in Ctx::extract_work for n points in n_scans rings
+struct RingStage;
+struct ExtractWork {
+  float *curv;
+  int *label;
+  unsigned char *gap;
+  RingStage *stage;
+  int *ring_cnt;  // per-ring less-flat centroid counts
+  int *status;
+  float4 *less_flat;  // staged less-flat centroids
+};
+void extract_work_layout(Carve &cv, int n, int n_scans, ExtractWork *W);
 // in place: segment l of d_pts (points [d_off[l], d_off[l + 1])) <- float 3x4 matrix l times the point, intensity kept
 void stamp(Ctx *c, const char *label);  // api.cu
 int project_cloud_device(Ctx *c, const float4 *d_in, int n, int vertical_scans, int horizon_scans, double roi_range, float4 *d_out,
@@ -410,7 +517,7 @@ int project_cloud_device(Ctx *c, const float4 *d_in, int n, int vertical_scans, 
 int transform_segments_device(Ctx *c, float4 *d_pts, int n, const int *d_off, int n_seg, const float *d_mat12);
 // VoxelGridCovarianceMLOAM<PointIWithCov>::filter: covariance-weighted merge per voxel (cov6 + trace per point in and out)
 int voxel_downsample_cov_device(Ctx *c, const float4 *d_in, const float *d_cov6, const float *d_trace, int n, const int *d_n_in, float leaf,
-                                float trace_threshold, float4 *d_out, float *d_cov6_out, float *d_trace_out, int *d_n_out, int work_slot = 5);
+                                float trace_threshold, float4 *d_out, float *d_cov6_out, float *d_trace_out, int *d_n_out, DevBuf &work);
 // exclusive scan of ints on the context stream (extract_kernels.cu); tmp holds ceil(n / 2048) ints
 void scan_exclusive(Ctx *c, const int *d_in, int *d_out, int n, int *d_tmp, int *d_total);
 // After a batched extraction over the concatenated sweeps of n_lidars LiDARs: move the less-sharp / less-flat features of LiDAR l into
@@ -420,7 +527,7 @@ int merge_lidars_device(Ctx *c, ExtractOut out, int n_cap_less, int n_cap_lflat,
                         int *d_off);
 // d_n_in (nullable): device-side input count (n is then the upper bound the kernels are sized for).
 int voxel_downsample_device(Ctx *c, const float4 *d_in, int n, const int *d_n_in, float leaf, int intensity_last, float4 *d_out,
-                            int *d_n_out, int work_slot = 5);
+                            int *d_n_out, DevBuf &work);
 
 }  // namespace mloam
 

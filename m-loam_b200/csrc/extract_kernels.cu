@@ -422,26 +422,15 @@ static int voxel_work_reserve(Ctx *c, DevBuf &buf, int n, int n_seg, VoxelWork *
   const int nblk = (n + PRIM_TILE - 1) / PRIM_TILE + 1;
   const int n_hist = 256 * nblk;
   const int n_tmp = (std::max(n, n_hist) + PRIM_TILE - 1) / PRIM_TILE + 1;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    size_t o = off;
-    off += (bytes + 255) & ~(size_t)255;
-    return o;
-  };
-  const size_t o_box = take(sizeof(SegBox) * (size_t)(n_seg + 1));
-  const size_t o_k0 = take(8 * (size_t)(n + 1)), o_k1 = take(8 * (size_t)(n + 1));
-  const size_t o_v0 = take(4 * (size_t)(n + 1)), o_v1 = take(4 * (size_t)(n + 1));
-  const size_t o_hist = take(4 * (size_t)n_hist), o_tmp = take(4 * (size_t)n_tmp);
-  const size_t o_head = take(4 * (size_t)(n + 1)), o_slot = take(4 * (size_t)(n + 1));
-  const size_t o_ticket = take(16);
-  MLOAM_CUDA_OK(c, buf.reserve(off));
-  char *p = buf.as<char>();
-  w->box = reinterpret_cast<SegBox *>(p + o_box);
-  w->k0 = reinterpret_cast<unsigned long long *>(p + o_k0), w->k1 = reinterpret_cast<unsigned long long *>(p + o_k1);
-  w->v0 = reinterpret_cast<unsigned *>(p + o_v0), w->v1 = reinterpret_cast<unsigned *>(p + o_v1);
-  w->hist = reinterpret_cast<int *>(p + o_hist), w->tmp = reinterpret_cast<int *>(p + o_tmp);
-  w->head = reinterpret_cast<int *>(p + o_head), w->slot = reinterpret_cast<int *>(p + o_slot);
-  w->ticket = reinterpret_cast<unsigned *>(p + o_ticket);
+  const size_t n1 = (size_t)n + 1;
+  MLOAM_CUDA_OK(c, carve(buf, [&](Carve &cv) {
+    w->box = cv.take<SegBox>(n_seg + 1);
+    w->k0 = cv.take<unsigned long long>(n1), w->k1 = cv.take<unsigned long long>(n1);
+    w->v0 = cv.take<unsigned>(n1), w->v1 = cv.take<unsigned>(n1);
+    w->hist = cv.take<int>(n_hist), w->tmp = cv.take<int>(n_tmp);
+    w->head = cv.take<int>(n1), w->slot = cv.take<int>(n1);
+    w->ticket = cv.take<unsigned>(4);
+  }));
   return MLOAM_OK;
 }
 
@@ -504,11 +493,11 @@ int project_cloud_device(Ctx *c, const float4 *d_in, int n, int vertical_scans, 
   ProfScope ps(c, "project");
   const ProjectParam sp = project_param(vertical_scans, horizon_scans, roi_range);
   VoxelWork w;
-  int rc = voxel_work_reserve(c, c->scratch[5], n, 1, &w);
+  int rc = voxel_work_reserve(c, c->voxel_work, n, 1, &w);
   if (rc) return rc;
   const size_t n_pix = (size_t)vertical_scans * horizon_scans;
-  MLOAM_CUDA_OK(c, c->scratch[2].reserve(sizeof(int) * n_pix));
-  int *winner = c->scratch[2].as<int>();
+  MLOAM_CUDA_OK(c, c->host_work.reserve(sizeof(int) * n_pix));
+  int *winner = c->host_work.as<int>();
   cudaStream_t st = c->stream;
   MLOAM_CUDA_OK(c, cudaMemsetAsync(winner, 0x7f, sizeof(int) * n_pix, st));
   MLOAM_CUDA_OK(c, cudaMemsetAsync(w.ticket, 0, 16, st));
@@ -536,7 +525,7 @@ __global__ void k_voxel_small(const float4 *__restrict__ P, int n, const int *__
                               float4 *__restrict__ out, int *__restrict__ n_out);
 
 int voxel_downsample_device(Ctx *c, const float4 *d_in, int n, const int *d_n_in, float leaf, int intensity_last, float4 *d_out,
-                            int *d_n_out, int work_slot) {
+                            int *d_n_out, DevBuf &work) {
   if (!(leaf > 0.f) || n < 0) {
     c->err = "voxel_downsample: bad leaf / size";
     return MLOAM_E_INVALID;
@@ -554,7 +543,7 @@ int voxel_downsample_device(Ctx *c, const float4 *d_in, int n, const int *d_n_in
     return MLOAM_OK;
   }
   VoxelWork w;
-  int rc = voxel_work_reserve(c, c->scratch[work_slot], n, 1, &w);
+  int rc = voxel_work_reserve(c, work, n, 1, &w);
   if (rc) return rc;
   rc = voxel_pipeline(c, d_in, nullptr, nullptr, n, d_n_in, 1, leaf, intensity_last, w, d_out, d_n_out);
   if (rc) return rc;
@@ -564,14 +553,14 @@ int voxel_downsample_device(Ctx *c, const float4 *d_in, int n, const int *d_n_in
 
 // VoxelGridCovarianceMLOAM<PointIWithCov>::filter (lidar_mapper_keyframe.cpp:344-347): always the radix pipeline.
 int voxel_downsample_cov_device(Ctx *c, const float4 *d_in, const float *d_cov6, const float *d_trace, int n, const int *d_n_in, float leaf,
-                                float trace_threshold, float4 *d_out, float *d_cov6_out, float *d_trace_out, int *d_n_out, int work_slot) {
+                                float trace_threshold, float4 *d_out, float *d_cov6_out, float *d_trace_out, int *d_n_out, DevBuf &work) {
   if (!(leaf > 0.f) || n < 0) {
     c->err = "voxel_downsample_cov: bad leaf / size";
     return MLOAM_E_INVALID;
   }
   ProfScope ps(c, "voxel_cov");
   VoxelWork w;
-  int rc = voxel_work_reserve(c, c->scratch[work_slot], n, 1, &w);
+  int rc = voxel_work_reserve(c, work, n, 1, &w);
   if (rc) return rc;
   CovIO io{d_cov6, d_trace, d_cov6_out, d_trace_out, trace_threshold, nullptr, 0.f};
   rc = voxel_pipeline(c, d_in, nullptr, nullptr, n, d_n_in, 1, leaf, 0, w, d_out, d_n_out, &io);
@@ -1079,6 +1068,13 @@ int transform_segments_device(Ctx *c, float4 *d_pts, int n, const int *d_off, in
   return MLOAM_OK;
 }
 
+void extract_work_layout(Carve &cv, int n, int n_scans, ExtractWork *W) {
+  const size_t N1 = (size_t)n + 16;
+  W->curv = cv.take<float>(N1), W->label = cv.take<int>(N1), W->gap = cv.take<unsigned char>(N1);
+  W->stage = cv.take<RingStage>(n_scans), W->ring_cnt = cv.take<int>((size_t)n_scans + 2), W->status = cv.take<int>(4);
+  W->less_flat = cv.take<float4>(N1);
+}
+
 int extract_device(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, const int *d_scan_end, int n_scans,
                    ExtractOut out, float *d_curv_or_null, int *d_label_or_null) {
   if (n < 0 || n_scans <= 0 || n_scans > MLOAM_MAX_RINGS) {
@@ -1094,29 +1090,17 @@ int extract_device(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start
   }
   ProfScope ps(c, "extract");
   cudaStream_t st = c->stream;
-  // scratch[4]: curv | label | gap | stage | per-ring counts | status | staged less-flat centroids
-  DevBuf &B = c->scratch[4];
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    size_t o = off;
-    off += (bytes + 255) & ~(size_t)255;
-    return o;
-  };
-  const size_t N1 = (size_t)n + 16;
-  const size_t o_curv = take(4 * N1), o_label = take(4 * N1);
-  const size_t o_gap = take(N1), o_stage = take(sizeof(RingStage) * (size_t)n_scans), o_segb = take(4 * ((size_t)n_scans + 2));
-  const size_t o_status = take(16), o_lf = take(16 * N1);
-  MLOAM_CUDA_OK(c, B.reserve(off));
-  char *p = B.as<char>();
-  float *curv = reinterpret_cast<float *>(p + o_curv);
-  int *label = reinterpret_cast<int *>(p + o_label);
-  unsigned char *gap = reinterpret_cast<unsigned char *>(p + o_gap);
-  RingStage *stage = reinterpret_cast<RingStage *>(p + o_stage);
-  int *seg_begin = reinterpret_cast<int *>(p + o_segb);  // per-ring centroid counts
-  int *status = reinterpret_cast<int *>(p + o_status);
+  ExtractWork W;
+  MLOAM_CUDA_OK(c, carve(c->extract_work, [&](Carve &cv) { extract_work_layout(cv, n, n_scans, &W); }));
+  float *curv = W.curv;
+  int *label = W.label;
+  unsigned char *gap = W.gap;
+  RingStage *stage = W.stage;
+  int *seg_begin = W.ring_cnt;
+  int *status = W.status;
   c->d_extract_status = status;
   c->d_ring_stage = stage, c->d_ring_cnt = seg_begin;  // per-ring pick / centroid counts (multi-LiDAR merge)
-  float4 *lf = reinterpret_cast<float4 *>(p + o_lf);
+  float4 *lf = W.less_flat;
   MLOAM_CUDA_OK(c, cudaMemsetAsync(out.counts, 0, 4 * sizeof(int), st));
   MLOAM_CUDA_OK(c, cudaMemsetAsync(status, 0, sizeof(int), st));
   if (n == 0) return MLOAM_OK;

@@ -336,43 +336,48 @@ __global__ void __launch_bounds__(GF_THREADS) k_gf_select(GfArgs a) {
     for (int k = tid; k < s_num_sel; k += GF_THREADS) a.mask[a.sel[k]] = 1;
 }
 
+// The selection's work for n features in B (Jacobian rows | fen | visited | dist | sel | n_sel | H | mask, then the cov_vec staging of
+// the host path when cov != nullptr): *jaco and the work pointers of a are set, a.jaco = *jaco
+static int gf_work(Ctx *c, DevBuf &B, int n, GfArgs *a, double **jaco, float **cov) {
+  MLOAM_CUDA_OK(c, carve(B, [&](Carve &cv) {
+    a->jaco = *jaco = cv.take<double>(6 * (size_t)n), a->fen = cv.take<int>((size_t)n + 1), a->visited = cv.take<int>(n), a->dist = cv.take<float>(n);
+    a->sel = cv.take<int>(n), a->n_sel = cv.take<int>(4), a->H = cv.take<double>(36), a->mask = cv.take<unsigned char>((size_t)n + 16);
+    if (cov) *cov = cv.take<float>(6 * (size_t)n);
+  }));
+  return MLOAM_OK;
+}
+
+// k_gf_select over the rows of a.jaco (one CTA)
+static int gf_select_launch(Ctx *c, GfArgs &a) {
+  ProfScope ps(c, "gf_select");
+  a.smem_ints = kGfSmemInts;
+  if (!c->smem_opt_in_gf) {
+    MLOAM_CUDA_OK(c, cudaFuncSetAttribute(k_gf_select, cudaFuncAttributeMaxDynamicSharedMemorySize, kGfSmemInts * (int)sizeof(int)));
+    c->smem_opt_in_gf = true;
+  }
+  k_gf_select<<<1, GF_THREADS, kGfSmemInts * sizeof(int), c->stream>>>(a);
+  c->launches++;
+  MLOAM_CUDA_OK(c, cudaGetLastError());
+  return MLOAM_OK;
+}
+
 // Device-resident selection of one matched feature set (inside scan2MapOptimization): no host round trip.
 int gf_select_set_device(Ctx *c, int t, const FeatSet &fs, const double *d_pose7, double default_sinfo, int method, double gf_ratio,
                          unsigned long long seed, unsigned char **d_mask_out) {
   const int n = fs.n;
   *d_mask_out = nullptr;
   if (n <= 0) return MLOAM_OK;
-  DevBuf &B = c->gf_work[t];
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    size_t o = off;
-    off += (bytes + 255) & ~(size_t)255;
-    return o;
-  };
-  const size_t o_j = take(sizeof(double) * 6 * (size_t)n), o_fen = take(4 * ((size_t)n + 1)), o_vis = take(4 * (size_t)n);
-  const size_t o_dist = take(4 * (size_t)n), o_sel = take(4 * (size_t)n), o_ns = take(16), o_H = take(36 * 8), o_mask = take((size_t)n + 16);
-  MLOAM_CUDA_OK(c, B.reserve(off));
-  char *p = B.as<char>();
-  double *d_jaco = reinterpret_cast<double *>(p + o_j);
+  GfArgs a;
+  double *d_jaco;
+  int rc = gf_work(c, c->gf_work[t], n, &a, &d_jaco, nullptr);
+  if (rc) return rc;
   k_gf_jaco<<<(n + 127) / 128, 128, 0, c->stream>>>(fs.pts, fs.valid, fs.coeff, n, fs.d_n, fs.is_plane ? 1 : 0, nullptr, fs.sinfo, default_sinfo,
                                                    d_pose7, d_jaco);
-  GfArgs a;
+  c->launches++;
   a.method = method, a.gf_ratio = gf_ratio, a.seed = seed, a.n = n, a.d_n = fs.d_n;
-  a.matched = fs.valid, a.jaco = d_jaco, a.pts = fs.pts;
-  a.fen = reinterpret_cast<int *>(p + o_fen), a.visited = reinterpret_cast<int *>(p + o_vis), a.dist = reinterpret_cast<float *>(p + o_dist);
-  a.sel = reinterpret_cast<int *>(p + o_sel), a.n_sel = reinterpret_cast<int *>(p + o_ns), a.H = reinterpret_cast<double *>(p + o_H);
-  a.mask = reinterpret_cast<unsigned char *>(p + o_mask);
-  {
-    ProfScope ps(c, "gf_select");
-    a.smem_ints = kGfSmemInts;
-    if (!c->smem_opt_in_gf) {
-      MLOAM_CUDA_OK(c, cudaFuncSetAttribute(k_gf_select, cudaFuncAttributeMaxDynamicSharedMemorySize, kGfSmemInts * (int)sizeof(int)));
-      c->smem_opt_in_gf = true;
-    }
-    k_gf_select<<<1, GF_THREADS, kGfSmemInts * sizeof(int), c->stream>>>(a);
-  }
-  c->launches += 2;
-  MLOAM_CUDA_OK(c, cudaGetLastError());
+  a.matched = fs.valid, a.pts = fs.pts;
+  rc = gf_select_launch(c, a);
+  if (rc) return rc;
   *d_mask_out = a.mask;
   return MLOAM_OK;
 }
@@ -434,25 +439,16 @@ static int good_features_impl(mloam_ctx_t *h, int slot, int type, const mloam_po
   rc = match_from_map_device(c, slot, type, c->scan_pts[t].as<float4>(), n, nullptr, d_pose, mcfg,
                              c->feat_valid[t].as<unsigned char>(), c->feat_coeff[t].as<float>(), nullptr);
   if (rc) return rc;
-  // scratch[3]: jaco | cov6 | fen | visited | dist | sel | n_sel | H
-  DevBuf &B = c->scratch[3];
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    size_t o = off;
-    off += (bytes + 255) & ~(size_t)255;
-    return o;
-  };
-  const size_t o_j = take(sizeof(double) * 6 * (size_t)n), o_cov = take(sizeof(float) * 6 * (size_t)n), o_fen = take(4 * ((size_t)n + 1));
-  const size_t o_vis = take(4 * (size_t)n), o_dist = take(4 * (size_t)n), o_sel = take(4 * (size_t)n), o_ns = take(16), o_H = take(36 * 8);
-  MLOAM_CUDA_OK(c, B.reserve(off));
-  char *p = B.as<char>();
-  double *d_jaco = reinterpret_cast<double *>(p + o_j);
-  float *d_cov = h_cov6 ? reinterpret_cast<float *>(p + o_cov) : nullptr;
+  GfArgs a;
+  double *d_jaco;
+  float *d_cov = nullptr;
+  rc = gf_work(c, c->host_work, n, &a, &d_jaco, h_cov6 ? &d_cov : nullptr);
+  if (rc) return rc;
   if (h_cov6) MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_cov, h_cov6, sizeof(float) * 6 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
   if (odom_x21) {
-    double *stage = reinterpret_cast<double *>(c->pinned) + 200;
+    double *stage = c->pinned->odom_x;
     for (int k = 0; k < 21; k++) stage[k] = odom_x21[k];
-    double *d_x21 = c->scratch[7].as<double>() + 64;
+    double *d_x21 = c->ctl.as<DevCtl>()->odom_x;
     MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_x21, stage, 21 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
     k_gf_jaco_odom<<<(n + 127) / 128, 128, 0, c->stream>>>(c->scan_pts[t].as<float4>(), c->feat_valid[t].as<unsigned char>(), c->feat_coeff[t].as<float>(),
                                                           n, type == 's' ? 1 : 0, d_x21, d_jaco);
@@ -460,22 +456,11 @@ static int good_features_impl(mloam_ctx_t *h, int slot, int type, const mloam_po
     k_gf_jaco<<<(n + 127) / 128, 128, 0, c->stream>>>(c->scan_pts[t].as<float4>(), c->feat_valid[t].as<unsigned char>(), c->feat_coeff[t].as<float>(), n,
                                                      nullptr, type == 's' ? 1 : 0, d_cov, nullptr, map_sqrt_info(c->params.cov_trace), d_pose, d_jaco);
   }
-  GfArgs a;
+  c->launches++;
   a.method = method, a.gf_ratio = gf_ratio, a.seed = seed, a.n = n, a.d_n = nullptr, a.mask = nullptr;
-  a.matched = c->feat_valid[t].as<unsigned char>(), a.jaco = d_jaco, a.pts = c->scan_pts[t].as<float4>();
-  a.fen = reinterpret_cast<int *>(p + o_fen), a.visited = reinterpret_cast<int *>(p + o_vis), a.dist = reinterpret_cast<float *>(p + o_dist);
-  a.sel = reinterpret_cast<int *>(p + o_sel), a.n_sel = reinterpret_cast<int *>(p + o_ns), a.H = reinterpret_cast<double *>(p + o_H);
-  {
-    ProfScope ps(c, "gf_select");
-    a.smem_ints = kGfSmemInts;
-    if (!c->smem_opt_in_gf) {
-      MLOAM_CUDA_OK(c, cudaFuncSetAttribute(k_gf_select, cudaFuncAttributeMaxDynamicSharedMemorySize, kGfSmemInts * (int)sizeof(int)));
-      c->smem_opt_in_gf = true;
-    }
-    k_gf_select<<<1, GF_THREADS, kGfSmemInts * sizeof(int), c->stream>>>(a);
-  }
-  c->launches += 2;
-  MLOAM_CUDA_OK(c, cudaGetLastError());
+  a.matched = c->feat_valid[t].as<unsigned char>(), a.pts = c->scan_pts[t].as<float4>();
+  rc = gf_select_launch(c, a);
+  if (rc) return rc;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(n_sel, a.n_sel, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(H36, a.H, 36 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_sel, a.sel, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));

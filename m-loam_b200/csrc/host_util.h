@@ -5,7 +5,6 @@
 #include "ctx.h"
 
 namespace mloam {
-static const size_t kPinnedBytes = 1 << 16;
 
 inline int fail(Ctx *c, int code, const char *msg) {
   c->err = msg;
@@ -33,9 +32,9 @@ inline float pick_cell(const Ctx *c, float requested) {
 }
 
 inline int upload_pose(Ctx *c, const double *pose7, double **d_pose) {
-  double *stage = reinterpret_cast<double *>(c->pinned) + 16;
+  double *stage = c->pinned->upload_pose;
   for (int k = 0; k < 7; k++) stage[k] = pose7[k];
-  double *d = c->scratch[7].as<double>() + 16;
+  double *d = c->ctl.as<DevCtl>()->upload_pose;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d, stage, 7 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   *d_pose = d;
   return MLOAM_OK;

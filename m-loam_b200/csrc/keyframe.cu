@@ -21,8 +21,6 @@ namespace mloam {
 
 namespace {
 
-inline size_t al(size_t x) { return (x + 255) & ~(size_t)255; }
-
 // Grow-only device memory outside alloc_epoch(): frame graphs never reference the store, so its growth must not make them re-capture.
 struct RawBuf {
   char *p = nullptr;
@@ -63,12 +61,27 @@ __host__ __device__ inline EntLayout ent_layout(int n_surf, int n_corner) {
   const int n[2] = {n_surf, n_corner};
   for (int t = 0; t < 2; t++) {
     const size_t m = (size_t)n[t];
-    L.pts[t] = o, o += (16 * m + 255) & ~(size_t)255;
-    L.cov6[t] = o, o += (24 * m + 255) & ~(size_t)255;
-    L.trace[t] = o, o += (4 * m + 255) & ~(size_t)255;
+    L.pts[t] = o, o += align256(16 * m);
+    L.cov6[t] = o, o += align256(24 * m);
+    L.trace[t] = o, o += align256(4 * m);
   }
   L.bytes = o;
   return L;
+}
+
+// A keyframe's record in the arena (laser_cloud_{surf,corner}_cov of saveKeyframe): per cloud t (0 surf, 1 corner) its points, then its
+// cov_vec, sized for the stored counts n[t]
+struct KfRecord {
+  float4 *pts[2];
+  float *cov6[2];
+  size_t bytes;
+};
+inline KfRecord kf_record(char *base, const int n[2]) {
+  KfRecord R;
+  Carve cv(base);
+  for (int t = 0; t < 2; t++) R.pts[t] = cv.take<float4>(n[t]), R.cov6[t] = cv.take<float>(6 * (size_t)n[t]);
+  R.bytes = cv.size + 256;
+  return R;
 }
 
 struct GatherEnt {
@@ -144,7 +157,7 @@ struct KeyframeStore {
   int map_n[2] = {0, 0};        // laser_cloud_{surf,corner}_from_map_cov_ds sizes (0 after clearCloud)
   size_t merged_ub[2] = {0, 0}; // upper bound of laser_cloud_*_from_map_cov's device-side size
   RawBuf merged_pts[2], merged_cov6[2], merged_trace[2];  // laser_cloud_*_from_map_cov, kept until clearCloud
-  RawBuf filt[2];               // laser_cloud_*_from_map_cov_ds: points | cov_vec | cov_trace
+  RawBuf filt[2];               // laser_cloud_*_from_map_cov_ds (filt_layout)
   RawBuf ctl;                   // ints: [0..1] merged sizes, [2..3] filtered sizes, [4] position-filter count, [8..] staged counts
   RawBuf tab;                   // per rebuild: positions in | filter out | GatherEnt table | dst offsets | UctLaser of the entering keyframes
   std::vector<float4> h_pos;
@@ -158,6 +171,20 @@ struct KeyframeStore {
     ctl.release(), tab.release();
   }
   size_t filt_cap(int t) const { return merged_ub[t] + 16; }
+  // filtered map t: points | cov_vec | cov_trace, sized for filt_cap(t) points
+  struct Filt {
+    float4 *pts;
+    float *cov6, *trace;
+    size_t bytes;
+  };
+  Filt filt_layout(int t) const {
+    const size_t m = filt_cap(t);
+    Filt F;
+    Carve cv(filt[t].p);
+    F.pts = cv.take<float4>(m), F.cov6 = cv.take<float>(6 * m), F.trace = cv.take<float>(m);
+    F.bytes = cv.size;
+    return F;
+  }
 };
 
 void keyframes_release(Ctx *c) {
@@ -240,13 +267,13 @@ int mloam_keyframe_save(mloam_ctx_t *h, const double *pose7, const double *cov36
   // the last frame's gated scans (laser_cloud_{surf,corner}_cov, :675-676): their device-side counts decide the copy sizes
   const Ctx::ScanRef &R = c->last_scan;
   cudaStream_t st = c->stream;
-  int *hc = reinterpret_cast<int *>(reinterpret_cast<char *>(c->pinned) + 3072);
+  int *hc = c->pinned->counts;
   hc[0] = R.n_surf, hc[1] = R.n_corner;
   if (R.d_n_surf) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, R.d_n_surf, sizeof(int), cudaMemcpyDeviceToHost, st));
   if (R.d_n_corner) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc + 1, R.d_n_corner, sizeof(int), cudaMemcpyDeviceToHost, st));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
   k.n[0] = std::max(0, std::min(hc[0], R.n_surf)), k.n[1] = std::max(0, std::min(hc[1], R.n_corner));
-  const size_t need = al(16 * (size_t)k.n[0]) + al(24 * (size_t)k.n[0]) + al(16 * (size_t)k.n[1]) + al(24 * (size_t)k.n[1]) + 256;
+  const size_t need = kf_record(nullptr, k.n).bytes;
   if (S.chunks.empty() || S.chunk_used + need > S.chunks.back().cap) {  // a new chunk, twice the last one: O(log K) allocations
     RawBuf b;
     MLOAM_CUDA_OK(c, raw_grow(b, std::max(need, S.chunks.empty() ? (size_t)0 : 2 * S.chunks.back().cap), 0, st));
@@ -255,17 +282,14 @@ int mloam_keyframe_save(mloam_ctx_t *h, const double *pose7, const double *cov36
   }
   k.chunk = (int)S.chunks.size() - 1, k.off = S.chunk_used;
   S.chunk_used += need;
-  char *base = S.chunks[k.chunk].p + k.off;
+  const KfRecord rec = kf_record(S.chunks[k.chunk].p + k.off, k.n);
   const float4 *src[2] = {R.surf, R.corner};
   const float *srcc[2] = {R.cov6_surf, R.cov6_corner};
-  size_t o = 0;
   for (int t = 0; t < 2; t++) {
     const size_t m = (size_t)k.n[t];
-    if (m) MLOAM_CUDA_OK(c, cudaMemcpyAsync(base + o, src[t], 16 * m, cudaMemcpyDeviceToDevice, st));
-    o += al(16 * m);
-    if (m && srcc[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(base + o, srcc[t], 24 * m, cudaMemcpyDeviceToDevice, st));
-    else if (m) MLOAM_CUDA_OK(c, cudaMemsetAsync(base + o, 0, 24 * m, st));  // with_ua = false: PointIWithCov(point, Zero) (:378-386)
-    o += al(24 * m);
+    if (m) MLOAM_CUDA_OK(c, cudaMemcpyAsync(rec.pts[t], src[t], 16 * m, cudaMemcpyDeviceToDevice, st));
+    if (m && srcc[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(rec.cov6[t], srcc[t], 24 * m, cudaMemcpyDeviceToDevice, st));
+    else if (m) MLOAM_CUDA_OK(c, cudaMemsetAsync(rec.cov6[t], 0, 24 * m, st));  // with_ua = false: PointIWithCov(point, Zero) (:378-386)
   }
   S.kfs.push_back(k);
   S.prev_pt[0] = k.pos[0], S.prev_pt[1] = k.pos[1], S.prev_pt[2] = k.pos[2];
@@ -340,9 +364,20 @@ int mloam_keyframe_submap(mloam_ctx_t *h, const double *pose_pred7, int *rebuilt
     const bool merged = c->n_lidars > 1 || c->lidar_merge;
     const int n_lasers = merged ? c->n_lidars : 1;
     const size_t n_new = sur.size() - n_surv;
-    const size_t o_pos = 0, o_filt = al(16 * (size_t)(n_set + 1)), o_tab = o_filt + al(16 * (size_t)(n_set + 1));
-    const size_t o_dst = o_tab + al(sizeof(GatherEnt) * (size_t)(n_set + 1)), o_las = o_dst + al(8 * (size_t)(n_set + 1));
-    MLOAM_CUDA_OK(c, raw_grow(S.tab, o_las + sizeof(UctLaser) * MLOAM_MAX_LIDARS * (n_new + 1), 0, st));
+    float4 *d_pos, *d_chosen;
+    GatherEnt *d_tab;
+    int *d_dst;
+    UctLaser *d_las;
+    auto tab_layout = [&](Carve &cv) {
+      const size_t m = (size_t)(n_set + 1);
+      d_pos = cv.take<float4>(m), d_chosen = cv.take<float4>(m), d_tab = cv.take<GatherEnt>(m), d_dst = cv.take<int>(2 * m);
+      d_las = cv.take<UctLaser>(MLOAM_MAX_LIDARS * (n_new + 1));
+    };
+    Carve tab_size;
+    tab_layout(tab_size);
+    MLOAM_CUDA_OK(c, raw_grow(S.tab, tab_size.size, 0, st));
+    Carve tab_cv(S.tab.p);
+    tab_layout(tab_cv);
     // :311-322 cloudUCTAssociateToMap of each entering keyframe with its pose + covariance and the context's current extrinsics and
     // covariances (mloam_set_lidars / mloam_set_uncertainty; the with_ua = false branch without uncertainty)
     S.h_lasers.clear();
@@ -357,7 +392,6 @@ int mloam_keyframe_submap(mloam_ctx_t *h, const double *pose_pred7, int *rebuilt
       fill_lasers(n_lasers, ext7.data(), pc.data(), cc.data(), one);
       S.h_lasers.insert(S.h_lasers.end(), one.begin(), one.end());
     }
-    UctLaser *d_las = reinterpret_cast<UctLaser *>(S.tab.p + o_las);
     if (!S.h_lasers.empty())
       MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_las, S.h_lasers.data(), sizeof(UctLaser) * S.h_lasers.size(), cudaMemcpyHostToDevice, st));
     int n_max = 1;
@@ -375,11 +409,9 @@ int mloam_keyframe_submap(mloam_ctx_t *h, const double *pose_pred7, int *rebuilt
       UctFrame f;
       memcpy(f.pose_global, k.pose, sizeof(f.pose_global)), memcpy(f.cov_meas, c->ua_cov_meas, sizeof(f.cov_meas));
       f.trace_threshold = S.trace_thr, f.with_ua = c->with_ua ? 1 : 0, f.n_lasers = n_lasers, f.scan_frame = 0;
-      const char *kb = S.chunks[k.chunk].p + k.off;
-      const float4 *src[2] = {reinterpret_cast<const float4 *>(kb),
-                              reinterpret_cast<const float4 *>(kb + al(16 * (size_t)k.n[0]) + al(24 * (size_t)k.n[0]))};
+      const KfRecord rec = kf_record(S.chunks[k.chunk].p + k.off, k.n);
       for (int t = 0; t < 2; t++) {
-        rc = uct_associate_append(c, src[t], k.n[t], f, d_las + (i - n_surv) * n_lasers, B, reinterpret_cast<float4 *>(e + L.pts[t]),
+        rc = uct_associate_append(c, rec.pts[t], k.n[t], f, d_las + (i - n_surv) * n_lasers, B, reinterpret_cast<float4 *>(e + L.pts[t]),
                                   reinterpret_cast<float *>(e + L.cov6[t]), reinterpret_cast<float *>(e + L.trace[t]), reinterpret_cast<int *>(e) + t);
         if (rc) return rc;
       }
@@ -394,13 +426,11 @@ int mloam_keyframe_submap(mloam_ctx_t *h, const double *pose_pred7, int *rebuilt
       S.h_pos[i] = make_float4(k.pos[0], k.pos[1], k.pos[2], (float)i);
       S.h_tab[i].off = (long long)ent_off[i], S.h_tab[i].n[0] = k.n[0], S.h_tab[i].n[1] = k.n[1];
     }
-    float4 *d_pos = reinterpret_cast<float4 *>(S.tab.p + o_pos), *d_chosen = reinterpret_cast<float4 *>(S.tab.p + o_filt);
-    GatherEnt *d_tab = reinterpret_cast<GatherEnt *>(S.tab.p + o_tab);
-    int *d_dst = reinterpret_cast<int *>(S.tab.p + o_dst), *ctl = reinterpret_cast<int *>(S.ctl.p);
+    int *ctl = reinterpret_cast<int *>(S.ctl.p);
     if (n_set > 0) {
       MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_pos, S.h_pos.data(), sizeof(float4) * n_set, cudaMemcpyHostToDevice, st));
       MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_tab, S.h_tab.data(), sizeof(GatherEnt) * n_set, cudaMemcpyHostToDevice, st));
-      rc = voxel_downsample_device(c, d_pos, n_set, nullptr, S.sur_kf_res, 1, d_chosen, ctl + 4, 5);
+      rc = voxel_downsample_device(c, d_pos, n_set, nullptr, S.sur_kf_res, 1, d_chosen, ctl + 4, c->voxel_work);
       if (rc) return rc;
     } else {  // no keyframe within the radius: nothing is chosen, nothing appended (the reference's filters then see what the
               // merged clouds already hold — empty after a save — and the frame fails the map gate)
@@ -433,20 +463,18 @@ int mloam_keyframe_submap(mloam_ctx_t *h, const double *pose_pred7, int *rebuilt
     // by the host-side bound and reading the merged sizes from the device
     const float leaf[2] = {c->params.surf_leaf, c->params.corner_leaf};
     for (int t = 0; t < 2; t++) {
-      const size_t m = S.filt_cap(t);
-      MLOAM_CUDA_OK(c, raw_grow(S.filt[t], al(16 * m) + al(24 * m) + al(4 * m), 0, st));
-      char *fb = S.filt[t].p;
+      MLOAM_CUDA_OK(c, raw_grow(S.filt[t], S.filt_layout(t).bytes, 0, st));
       if (ub[t] == 0) {
         MLOAM_CUDA_OK(c, cudaMemsetAsync(ctl + 2 + t, 0, sizeof(int), st));
         continue;
       }
-      rc = voxel_downsample_cov_device(c, mo.pts[t], mo.cov6[t], mo.trace[t], (int)ub[t], ctl + t, leaf[t], (float)S.trace_thr,
-                                       reinterpret_cast<float4 *>(fb), reinterpret_cast<float *>(fb + al(16 * m)),
-                                       reinterpret_cast<float *>(fb + al(16 * m) + al(24 * m)), ctl + 2 + t, 5);
+      const KeyframeStore::Filt F = S.filt_layout(t);
+      rc = voxel_downsample_cov_device(c, mo.pts[t], mo.cov6[t], mo.trace[t], (int)ub[t], ctl + t, leaf[t], (float)S.trace_thr, F.pts, F.cov6,
+                                       F.trace, ctl + 2 + t, c->voxel_work);
       if (rc) return rc;
     }
     // the one host round trip of a rebuild: the map build is sized by the filtered counts; the chosen ids ride along
-    int *hc = reinterpret_cast<int *>(reinterpret_cast<char *>(c->pinned) + 3072);
+    int *hc = c->pinned->counts;
     MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, ctl, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
     S.h_chosen.resize(n_set);
     if (n_set > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(S.h_chosen.data(), d_chosen, sizeof(float4) * n_set, cudaMemcpyDeviceToHost, st));
@@ -470,9 +498,9 @@ int mloam_keyframe_submap(mloam_ctx_t *h, const double *pose_pred7, int *rebuilt
     const int m = S.map_n[t];
     if (!(hp[t] || hcv[t]) || m == 0) continue;
     if (m > cap[t]) return fail(c, MLOAM_E_INVALID, "keyframe_submap: output capacity too small");
-    const size_t fc = S.filt_cap(t);
-    if (hp[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hp[t], S.filt[t].p, sizeof(float4) * (size_t)m, cudaMemcpyDeviceToHost, st));
-    if (hcv[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hcv[t], S.filt[t].p + al(16 * fc), sizeof(float) * 6 * (size_t)m, cudaMemcpyDeviceToHost, st));
+    const KeyframeStore::Filt F = S.filt_layout(t);
+    if (hp[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hp[t], F.pts, sizeof(float4) * (size_t)m, cudaMemcpyDeviceToHost, st));
+    if (hcv[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hcv[t], F.cov6, sizeof(float) * 6 * (size_t)m, cudaMemcpyDeviceToHost, st));
     copied = true;
   }
   if (copied) MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));  // the map build itself stays queued ahead of the next frame on the stream
@@ -516,15 +544,12 @@ int mloam_keyframe_scan(mloam_ctx_t *h, int id, double *pose7, double *cov36, ml
   float *hcv[2] = {h_surf_cov6, h_corner_cov6};
   const int cap[2] = {cap_surf, cap_corner};
   cudaStream_t st = c->stream;
-  const char *base = S.chunks[k.chunk].p + k.off;
-  size_t o = 0;
+  const KfRecord rec = kf_record(S.chunks[k.chunk].p + k.off, k.n);
   for (int t = 0; t < 2; t++) {
     const size_t m = (size_t)k.n[t];
     if ((hp[t] || hcv[t]) && k.n[t] > cap[t]) return fail(c, MLOAM_E_INVALID, "keyframe_scan: capacity too small");
-    if (m && hp[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hp[t], base + o, 16 * m, cudaMemcpyDeviceToHost, st));
-    o += al(16 * m);
-    if (m && hcv[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hcv[t], base + o, 24 * m, cudaMemcpyDeviceToHost, st));
-    o += al(24 * m);
+    if (m && hp[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hp[t], rec.pts[t], 16 * m, cudaMemcpyDeviceToHost, st));
+    if (m && hcv[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hcv[t], rec.cov6[t], 24 * m, cudaMemcpyDeviceToHost, st));
   }
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
   return MLOAM_OK;

@@ -284,7 +284,7 @@ int map_build_device(Ctx *c, int slot, const float4 *d_pts, int m, float cell) {
   c->launches += m > 0 ? 8 : 5;
   // occupancy statistics for the next auto-cell decision of this slot (read lazily by auto_cell_pick; stale is fine)
   if (c->pinned)
-    MLOAM_CUDA_OK(c, cudaMemcpyAsync(reinterpret_cast<char *>(c->pinned) + kMapStatsOffset + 64 * slot, h, 48, cudaMemcpyDeviceToHost, st));
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(&c->pinned->map_hdr[slot], h, 48, cudaMemcpyDeviceToHost, st));
   MLOAM_CUDA_OK(c, cudaGetLastError());
   return MLOAM_OK;
 }

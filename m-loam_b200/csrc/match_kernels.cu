@@ -55,6 +55,8 @@ struct HeavyQ {
 // dependent warp-wide operations (prefix loads -> point loads -> REDUX / ballot / shuffle rounds).  MB = 3 and 4 buy more
 // resident warps with spilled registers (local-memory round trips inside that chain); on the H100 the spill-free MB = 2
 // variant (106 registers) runs the C2 frame about 9 % faster than MB = 4, so it is the default (Ctx::knn_min_blocks).
+// path_stats: the KnnPathStats (ctx.h) addressed as 32-bit words; KPS_WORD(field) is a field's word index
+#define KPS_WORD(field) (offsetof(KnnPathStats, field) / sizeof(unsigned))
 template <int K, int MB>
 __global__ void __launch_bounds__(MWARPS * 32, MB)
     k_match_knn(KnnSet a, KnnSet b, const double *__restrict__ pose7, float min_match_sq_dis, HeavyQ hq, const int *__restrict__ d_sel,
@@ -177,14 +179,14 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
           tr[1] = (unsigned)dbg.t_ring1, tr[2] = (unsigned)dbg.t_ball, tr[3] = ((unsigned)dbg.ring1_pts << 20) | ((unsigned)(dbg.ball_pts & 0xfff) << 8) | (unsigned)(dbg.ball_steps & 0xff);
         }
         if (path_stats && lane == 0) {
-          unsigned long long *q = reinterpret_cast<unsigned long long *>(path_stats + 24);
+          unsigned long long *q = reinterpret_cast<unsigned long long *>(path_stats + KPS_WORD(blind));
           atomicAdd(q + 0, 0ull), atomicAdd(q + 1, (unsigned long long)dbg.t_ring1);
           atomicAdd(q + 2, (unsigned long long)dbg.t_ball), atomicAdd(q + 3, (unsigned long long)dbg.ring1_pts);
           atomicAdd(q + 4, (unsigned long long)dbg.ball_pts), atomicAdd(q + 5, (unsigned long long)dbg.ball_steps);
           atomicAdd(q + 6, (unsigned long long)dbg.ball_rows), atomicAdd(q + 7, dbg.t_ball ? 1ull : 0ull);
           const long long dt_blind = clock64() - t_blind;
           if (dt_blind > 90000) {  // a record of one very slow blind query (benign race: any of them will do)
-            long long *rec = reinterpret_cast<long long *>(path_stats + 40);
+            long long *rec = reinterpret_cast<long long *>(path_stats + KPS_WORD(slow_rec));
             rec[0] = dt_blind, rec[1] = 0, rec[2] = dbg.t_ring1, rec[3] = dbg.t_ball, rec[4] = dbg.ring1_pts;
             rec[5] = dbg.ball_pts, rec[6] = dbg.ball_rows, rec[7] = dbg.ball_steps, rec[8] = (in_a ? 0 : 1) * 1000000 + j;
             rec[9] = (long long)(t_blind - t_query);
@@ -218,13 +220,13 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
     }
     if (path_stats && lane == 0) {  // stage profiling: queries and SM cycles per search path, slowest single query
       const unsigned long long dt = (unsigned long long)(clock64() - t_query);
-      atomicAdd(path_stats + path, 1u);
-      atomicAdd(reinterpret_cast<unsigned long long *>(path_stats + 8) + path, dt);
-      atomicMax(path_stats + 4, (unsigned)(dt > 0xffffffffull ? 0xffffffffull : dt));
-      if (dt > 32768ull) atomicAdd(path_stats + 5, 1u);
-      if (dt > 65536ull) atomicAdd(path_stats + 6, 1u);
+      atomicAdd(path_stats + KPS_WORD(queries) + path, 1u);
+      atomicAdd(reinterpret_cast<unsigned long long *>(path_stats + KPS_WORD(cycles)) + path, dt);
+      atomicMax(path_stats + KPS_WORD(max_query_cycles), (unsigned)(dt > 0xffffffffull ? 0xffffffffull : dt));
+      if (dt > 32768ull) atomicAdd(path_stats + KPS_WORD(over_32k), 1u);
+      if (dt > 65536ull) atomicAdd(path_stats + KPS_WORD(over_64k), 1u);
       // slowest query: cycles << 32 | path << 30 | set << 29 | feature index
-      atomicMax(reinterpret_cast<unsigned long long *>(path_stats + 16),
+      atomicMax(reinterpret_cast<unsigned long long *>(path_stats + KPS_WORD(slowest)),
                 (dt << 32) | ((unsigned long long)path << 30) | ((unsigned long long)(in_a ? 0 : 1) << 29) | (unsigned)(j & 0x1fffffff));
     }
     if (trace && lane == 0) trace[4 * (size_t)((in_a ? 0 : na) + j)] = (unsigned)(clock64() - t_query) | ((unsigned)path << 30);
@@ -342,7 +344,7 @@ int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_
   {
     ProfScope ps(c, "match");
     // with stage profiling on: how many queries took the keep (matched / rejected), ball and blind paths
-    unsigned *path_stats = (c->prof_on && !getenv("MLOAM_KNN_NO_STATS")) ? reinterpret_cast<unsigned *>(c->scratch[7].as<char>() + kKnnPathStatsOffset) : nullptr;
+    unsigned *path_stats = (c->prof_on && !getenv("MLOAM_KNN_NO_STATS")) ? reinterpret_cast<unsigned *>(&c->ctl.as<DevCtl>()->knn_stats) : nullptr;
     unsigned *trace = nullptr;
     if (c->knn_trace_on) {
       MLOAM_CUDA_OK(c, c->knn_trace.reserve(16 * (size_t)(n_upper + 1) + 16 * (size_t)MWARPS * 4 * c->sm_count + 64));

@@ -344,7 +344,7 @@ __global__ void k_odom_init(OdomState *st, const double *x21, int free_mask, int
 
 template <int D>
 static int odom_solve_run(Ctx *c, const OdomSets &sets, OdomState *st, int max_inner, int nb, double *partials) {
-  int *h_done = reinterpret_cast<int *>(reinterpret_cast<char *>(c->pinned) + 2048);
+  int *h_done = &c->pinned->done;
   k_odom_linearize<D><<<nb, OD_THREADS, 0, c->stream>>>(sets, st, 0, partials);
   k_odom_lm<D><<<1, OD_THREADS, 0, c->stream>>>(partials, nb, st, 1);
   c->launches += 2;
@@ -408,6 +408,18 @@ static int calib_eval(Ctx *c, const OdomSets &sets, OdomState *st, int nb, doubl
   return MLOAM_OK;
 }
 
+static_assert(sizeof(OdomState) <= sizeof(PinnedBlock::odom), "OdomState mirror in the pinned block");
+static OdomState *odom_mirror(Ctx *c) { return reinterpret_cast<OdomState *>(c->pinned->odom); }
+
+// Ctx::odom_work: OdomState, then the packed equations of nb blocks and spare rows (calib_eval sums the blocks into one of them)
+static int odom_work(Ctx *c, int nb, OdomState **st, double **partials) {
+  MLOAM_CUDA_OK(c, carve(c->odom_work, [&](Carve &cv) {
+    *st = cv.take<OdomState>(1);
+    *partials = cv.take<double>(96 * (size_t)(nb + 3));
+  }));
+  return MLOAM_OK;
+}
+
 }  // namespace mloam
 
 using namespace mloam;
@@ -443,13 +455,14 @@ extern "C" int mloam_calib_frame(mloam_ctx_t *h, const mloam_point_t *h_surf_ref
   }
   int nb = (n_max + OD_THREADS - 1) / OD_THREADS;
   nb = nb < 1 ? 1 : (nb > c->sm_count ? c->sm_count : nb);
-  MLOAM_CUDA_OK(c, c->scratch[6].reserve(sizeof(OdomState) + 512 + sizeof(double) * 96 * (size_t)(nb + 3)));
-  OdomState *st = c->scratch[6].as<OdomState>();
-  double *partials = reinterpret_cast<double *>(c->scratch[6].as<char>() + ((sizeof(OdomState) + 255) & ~(size_t)255));
-  double *stage = reinterpret_cast<double *>(c->pinned) + 200;
+  OdomState *st;
+  double *partials;
+  int rc = odom_work(c, nb, &st, &partials);
+  if (rc) return rc;
+  double *stage = c->pinned->odom_x;
   for (int k = 0; k < 7; k++) stage[k] = pose_pivot7[k], stage[7 + k] = pose_i7[k], stage[14 + k] = ext_cal7[k], stage[21 + k] = ext_ref7[k];
-  double *d_x = c->scratch[7].as<double>() + 64;  // 28 doubles; the two match poses follow at + 96 / + 104
-  double *d_pose_a = c->scratch[7].as<double>() + 96, *d_pose_b = c->scratch[7].as<double>() + 104;
+  DevCtl *ctl = c->ctl.as<DevCtl>();
+  double *d_x = ctl->odom_x, *d_pose_a = ctl->match_pose[0], *d_pose_b = ctl->match_pose[1];
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_x, stage, 28 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   k_odom_init<<<1, 32, 0, c->stream>>>(st, d_x, 3, max_inner, d_x + 21);
   c->launches++;
@@ -462,8 +475,7 @@ extern "C" int mloam_calib_frame(mloam_ctx_t *h, const mloam_point_t *h_surf_ref
   sets.sqrt_info = 1.0, sets.huber_a = huber_a;  // factors are built with s = 1.0 (estimator.cpp:696,733); Huber(1.0) (:602)
   MatchCfg cfg_ref{c->params.min_match_sq_dis, c->params.min_plane_dis, 5, 1};   // n_neigh 5, CHECK_FOV true (estimator.cpp:1135-1142)
   MatchCfg cfg_cal{c->params.min_match_sq_dis, c->params.min_plane_dis, 10, 1};  // n_neigh 10 for the other LiDARs
-  int *h_done = reinterpret_cast<int *>(reinterpret_cast<char *>(c->pinned) + 2048);
-  int rc = MLOAM_OK;
+  int *h_done = &c->pinned->done;
   for (int outer = 0; outer < max_outer && rc == MLOAM_OK; outer++) {
     k_calib_poses<<<1, 32, 0, c->stream>>>(st, d_pose_a, d_pose_b);
     c->launches++;
@@ -490,7 +502,7 @@ extern "C" int mloam_calib_frame(mloam_ctx_t *h, const mloam_point_t *h_surf_ref
     }
   }
   if (rc) return rc;
-  OdomState *hs = reinterpret_cast<OdomState *>(reinterpret_cast<char *>(c->pinned) + 8192);
+  OdomState *hs = odom_mirror(c);
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(hs, st, sizeof(OdomState), cudaMemcpyDeviceToHost, c->stream));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
   for (int k = 0; k < 7; k++) pose_i7[k] = hs->xi[k], ext_cal7[k] = hs->xe[k];
@@ -539,18 +551,19 @@ extern "C" int mloam_odom_solve(mloam_ctx_t *h, int n, const unsigned char *h_ty
   const int D = free_mask == 3 ? 12 : 6;
   int nb = (n_max + OD_THREADS - 1) / OD_THREADS;
   nb = nb < 1 ? 1 : (nb > c->sm_count ? c->sm_count : nb);
-  MLOAM_CUDA_OK(c, c->scratch[6].reserve(sizeof(OdomState) + 512 + sizeof(double) * 96 * (size_t)(nb + 1)));
-  OdomState *st = c->scratch[6].as<OdomState>();
-  double *partials = reinterpret_cast<double *>(c->scratch[6].as<char>() + ((sizeof(OdomState) + 255) & ~(size_t)255));
-  double *stage = reinterpret_cast<double *>(c->pinned) + 200;
+  OdomState *st;
+  double *partials;
+  int rc = odom_work(c, nb, &st, &partials);
+  if (rc) return rc;
+  double *stage = c->pinned->odom_x;
   for (int k = 0; k < 7; k++) stage[k] = pose_pivot7[k], stage[7 + k] = pose_i7[k], stage[14 + k] = ext7[k];
-  double *d_x = c->scratch[7].as<double>() + 64;
+  double *d_x = c->ctl.as<DevCtl>()->odom_x;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_x, stage, 21 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   k_odom_init<<<1, 32, 0, c->stream>>>(st, d_x, free_mask, max_iterations);
   c->launches++;
-  int rc = D == 12 ? odom_solve_run<12>(c, sets, st, max_iterations, nb, partials) : odom_solve_run<6>(c, sets, st, max_iterations, nb, partials);
+  rc = D == 12 ? odom_solve_run<12>(c, sets, st, max_iterations, nb, partials) : odom_solve_run<6>(c, sets, st, max_iterations, nb, partials);
   if (rc) return rc;
-  OdomState *hs = reinterpret_cast<OdomState *>(reinterpret_cast<char *>(c->pinned) + 8192);
+  OdomState *hs = odom_mirror(c);
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(hs, st, sizeof(OdomState), cudaMemcpyDeviceToHost, c->stream));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
   for (int k = 0; k < 7; k++) pose_i7[k] = hs->xi[k], ext7[k] = hs->xe[k];

@@ -805,11 +805,9 @@ __global__ void k_lm_init(LMState *st, const double *pose7, int max_inner, int m
 int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, double eig_thre, SpecState *spec) {
   (void)eig_thre;
   MLOAM_CUDA_OK(c, c->lm_state.reserve(sizeof(LMState) + 64));
-  // stage the pose through pinned memory so the copy is truly asynchronous
-  double *stage = reinterpret_cast<double *>(c->pinned);
-  for (int k = 0; k < 7; k++) stage[k] = pose7_host[k];
-  double *d_stage = c->scratch[7].as<double>();
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_stage, stage, 7 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  stage_pose(c, pose7_host);
+  double *d_stage = c->ctl.as<DevCtl>()->pose;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_stage, c->pinned->pose, 7 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   k_lm_init<<<1, 32, 0, c->stream>>>(c->lm_state.as<LMState>(), d_stage, max_inner, c->lm_min_corr, spec);
   c->launches++;
   MLOAM_CUDA_OK(c, cudaGetLastError());

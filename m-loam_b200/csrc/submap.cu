@@ -156,22 +156,14 @@ void pose_inverse(const double *x, double *out) {  // Pose::inverse (pose.cpp:99
 }
 }  // namespace
 
-int uct_bufs(Ctx *c, int n, UctBufs *B) {
-  DevBuf &buf = c->scratch[2];
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    size_t o = off;
-    off += (bytes + 255) & ~(size_t)255;
-    return o;
-  };
+void uct_bufs_layout(Carve &cv, int n, UctBufs *B) {
   const size_t N1 = (size_t)n + 16;
-  const size_t o_st = take(16 * N1), o_c6 = take(24 * N1), o_tr = take(4 * N1), o_keep = take(4 * N1), o_slot = take(4 * N1);
-  const size_t o_tmp = take(4 * (N1 / 2048 + 8)), o_cnt = take(64);
-  MLOAM_CUDA_OK(c, buf.reserve(off));
-  char *p = buf.as<char>();
-  B->staged = reinterpret_cast<float4 *>(p + o_st), B->cov6 = reinterpret_cast<float *>(p + o_c6), B->trace = reinterpret_cast<float *>(p + o_tr);
-  B->keep = reinterpret_cast<int *>(p + o_keep), B->slot = reinterpret_cast<int *>(p + o_slot), B->tmp = reinterpret_cast<int *>(p + o_tmp);
-  B->count = reinterpret_cast<int *>(p + o_cnt);
+  B->staged = cv.take<float4>(N1), B->cov6 = cv.take<float>(6 * N1), B->trace = cv.take<float>(N1);
+  B->keep = cv.take<int>(N1), B->slot = cv.take<int>(N1), B->tmp = cv.take<int>(N1 / 2048 + 8), B->count = cv.take<int>(16);
+}
+
+int uct_bufs(Ctx *c, int n, UctBufs *B) {
+  MLOAM_CUDA_OK(c, carve(c->assoc_work(), [&](Carve &cv) { uct_bufs_layout(cv, n, B); }));
   return MLOAM_OK;
 }
 
@@ -202,16 +194,12 @@ void fill_lasers(int n_lasers, const double *ext7, const double *pose_compound7,
 // holds the ring): pointAssociateToMap with pose_ext[idx]^-1, evalPointUncertainty under pose_ext[idx] with its covariance, dropped
 // when trace > TRACE_THRESHOLD_MAPPING; the kept points keep their order.  This is cloudUCTAssociateToMap's per-point work with the
 // extrinsic as the compound pose and no pose_global transform, so k_uct_associate + k_compact_cov do it.
-static_assert(sizeof(UctFrame) <= 256, "UctFrame is staged in 256 B");
-static_assert(256 + sizeof(UctLaser) * MLOAM_MAX_LIDARS <= kPinnedPoseCov - kPinnedUct, "pinned staging of the with_ua stage");
-
 void ua_stage_host(Ctx *c) {
-  char *pin = reinterpret_cast<char *>(c->pinned) + kPinnedUct;
-  UctFrame *f = reinterpret_cast<UctFrame *>(pin);
-  UctLaser *L = reinterpret_cast<UctLaser *>(pin + 256);
+  UctFrame *f = &c->pinned->ua.frame;
+  UctLaser *L = c->pinned->ua.lasers;
   const bool merged = c->n_lidars > 1 || c->lidar_merge;
   const int n_lasers = merged ? c->n_lidars : 1;
-  memset(f, 0, 256);
+  memset(f, 0, sizeof(*f));
   for (int k = 0; k < 7; k++) f->pose_global[k] = k == 6 ? 1.0 : 0.0;
   memcpy(f->cov_meas, c->ua_cov_meas, sizeof(f->cov_meas));
   f->trace_threshold = c->ua_trace_threshold, f->with_ua = 1, f->n_lasers = n_lasers, f->scan_frame = 1;
@@ -228,51 +216,40 @@ int ua_scan_stage(Ctx *c, Ctx::ScanRef *S) {
   const int ncap[2] = {S->n_corner, S->n_surf};
   const float4 *pts[2] = {S->corner, S->surf};
   const int *d_n[2] = {S->d_n_corner, S->d_n_surf};
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    size_t o = off;
-    off += (bytes + 255) & ~(size_t)255;
-    return o;
-  };
-  const size_t o_cfg = take(256 + sizeof(UctLaser) * MLOAM_MAX_LIDARS);
-  struct Set {
-    size_t staged, cov6, trace, keep, slot, tmp, out, ocov6, otrace, osinfo, count;
-  } o[2];
-  for (int t = 0; t < 2; t++) {
-    const size_t N1 = (size_t)(ncap[t] > 0 ? ncap[t] : 0) + 16;
-    o[t].staged = take(16 * N1), o[t].cov6 = take(24 * N1), o[t].trace = take(4 * N1), o[t].keep = take(4 * N1), o[t].slot = take(4 * N1);
-    o[t].tmp = take(4 * (N1 / 2048 + 8)), o[t].out = take(16 * N1), o[t].ocov6 = take(24 * N1), o[t].otrace = take(4 * N1);
-    o[t].osinfo = take(8 * N1), o[t].count = take(64);
-  }
-  MLOAM_CUDA_OK(c, c->ua_scan.reserve(off));
-  char *p = c->ua_scan.as<char>();
+  // Ctx::ua_scan: the staged configuration, then per scan the association work and the gated scan
+  UaStage *d_cfg = nullptr;
+  UctBufs B[2];
+  float4 *out[2];
+  float *ocov6[2], *otrace[2];
+  double *osinfo[2];
+  MLOAM_CUDA_OK(c, carve(c->ua_scan, [&](Carve &cv) {
+    d_cfg = cv.take<UaStage>(1);
+    for (int t = 0; t < 2; t++) {
+      const int n = ncap[t] > 0 ? ncap[t] : 0;
+      const size_t N1 = (size_t)n + 16;
+      uct_bufs_layout(cv, n, &B[t]);
+      out[t] = cv.take<float4>(N1), ocov6[t] = cv.take<float>(6 * N1), otrace[t] = cv.take<float>(N1), osinfo[t] = cv.take<double>(N1);
+    }
+  }));
   ua_stage_host(c);
   cudaStream_t st = c->stream;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(p + o_cfg, reinterpret_cast<char *>(c->pinned) + kPinnedUct, 256 + sizeof(UctLaser) * MLOAM_MAX_LIDARS,
-                                   cudaMemcpyHostToDevice, st));
-  const UctFrame *d_f = reinterpret_cast<const UctFrame *>(p + o_cfg);
-  const UctLaser *d_l = reinterpret_cast<const UctLaser *>(p + o_cfg + 256);
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_cfg, &c->pinned->ua, sizeof(UaStage), cudaMemcpyHostToDevice, st));
   const UctFrame f_unused{};
   for (int t = 0; t < 2; t++) {
     const int n = ncap[t];
-    float4 *staged = reinterpret_cast<float4 *>(p + o[t].staged), *out = reinterpret_cast<float4 *>(p + o[t].out);
-    float *cov6 = reinterpret_cast<float *>(p + o[t].cov6), *trace = reinterpret_cast<float *>(p + o[t].trace);
-    float *ocov6 = reinterpret_cast<float *>(p + o[t].ocov6), *otrace = reinterpret_cast<float *>(p + o[t].otrace);
-    int *keep = reinterpret_cast<int *>(p + o[t].keep), *slot = reinterpret_cast<int *>(p + o[t].slot), *tmp = reinterpret_cast<int *>(p + o[t].tmp);
-    int *count = reinterpret_cast<int *>(p + o[t].count);
-    double *osinfo = reinterpret_cast<double *>(p + o[t].osinfo);
+    const UctBufs &b = B[t];
     if (n > 0) {
-      k_uct_associate<<<(n + 127) / 128, 128, 0, st>>>(pts[t], n, f_unused, d_l, staged, cov6, trace, keep, d_f, d_n[t]);
+      k_uct_associate<<<(n + 127) / 128, 128, 0, st>>>(pts[t], n, f_unused, d_cfg->lasers, b.staged, b.cov6, b.trace, b.keep, &d_cfg->frame, d_n[t]);
       c->launches++;
     }
-    scan_exclusive(c, keep, slot, n, tmp, count);  // the gated count lands where the solve reads its feature count
+    scan_exclusive(c, b.keep, b.slot, n, b.tmp, b.count);  // the gated count lands where the solve reads its feature count
     if (n > 0) {
-      k_compact_cov<<<(n + 255) / 256, 256, 0, st>>>(staged, cov6, trace, keep, slot, n, 0, nullptr, out, ocov6, otrace, osinfo);
+      k_compact_cov<<<(n + 255) / 256, 256, 0, st>>>(b.staged, b.cov6, b.trace, b.keep, b.slot, n, 0, nullptr, out[t], ocov6[t], otrace[t], osinfo[t]);
       c->launches++;
     }
     MLOAM_CUDA_OK(c, cudaGetLastError());
-    if (t == 0) S->corner = out, S->d_n_corner = count, S->sinfo_corner = osinfo, S->cov6_corner = ocov6;
-    else S->surf = out, S->d_n_surf = count, S->sinfo_surf = osinfo, S->cov6_surf = ocov6;
+    if (t == 0) S->corner = out[t], S->d_n_corner = b.count, S->sinfo_corner = osinfo[t], S->cov6_corner = ocov6[t];
+    else S->surf = out[t], S->d_n_surf = b.count, S->sinfo_surf = osinfo[t], S->cov6_surf = ocov6[t];
   }
   return MLOAM_OK;
 }
@@ -330,15 +307,15 @@ int mloam_cloud_uct_associate(mloam_ctx_t *h, const mloam_point_t *h_pts, int n,
   UctBufs B;
   int rc = uct_bufs(c, n, &B);
   if (rc) return rc;
-  DevBuf &in = c->scratch[0], &outb = c->scratch[1];
-  MLOAM_CUDA_OK(c, in.reserve(sizeof(float4) * (size_t)n + sizeof(UctLaser) * MLOAM_MAX_LIDARS + 512));
-  MLOAM_CUDA_OK(c, outb.reserve((16 + 24 + 4) * ((size_t)n + 16) + 1024));
-  float4 *d_in = in.as<float4>();
-  UctLaser *d_l = reinterpret_cast<UctLaser *>(in.as<char>() + ((sizeof(float4) * (size_t)n + 255) & ~(size_t)255));
-  float4 *d_out = outb.as<float4>();
-  float *d_c6 = reinterpret_cast<float *>(outb.as<char>() + 16 * ((size_t)n + 16));
-  float *d_tr = d_c6 + 6 * ((size_t)n + 16);
-  int *d_total = reinterpret_cast<int *>(d_tr + ((size_t)n + 16));
+  const size_t N1 = (size_t)n + 16;
+  float4 *d_in, *d_out;
+  UctLaser *d_l;
+  float *d_c6, *d_tr;
+  int *d_total;
+  MLOAM_CUDA_OK(c, carve(c->sweep_in, [&](Carve &cv) { d_in = cv.take<float4>(n), d_l = cv.take<UctLaser>(MLOAM_MAX_LIDARS); }));
+  MLOAM_CUDA_OK(c, carve(c->map_in[0], [&](Carve &cv) {
+    d_out = cv.take<float4>(N1), d_c6 = cv.take<float>(6 * N1), d_tr = cv.take<float>(N1), d_total = cv.take<int>(16);
+  }));
   std::vector<UctLaser> L;
   fill_lasers(n_lasers, ext7, pose_compound7, cov_compound36, L);
   UctFrame f;
@@ -349,7 +326,7 @@ int mloam_cloud_uct_associate(mloam_ctx_t *h, const mloam_point_t *h_pts, int n,
   MLOAM_CUDA_OK(c, cudaMemsetAsync(d_total, 0, sizeof(int), st));
   rc = uct_associate_append(c, d_in, n, f, d_l, B, d_out, d_c6, d_tr, d_total);
   if (rc) return rc;
-  int *hc = reinterpret_cast<int *>(reinterpret_cast<char *>(c->pinned) + 3072);
+  int *hc = c->pinned->counts;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_total, sizeof(int), cudaMemcpyDeviceToHost, st));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));  // L (host vector) was read by the copy above
   *n_out = hc[0];
@@ -370,21 +347,20 @@ int mloam_voxel_downsample_cov(mloam_ctx_t *h, const mloam_point_t *h_pts, const
   *n_out = 0;
   if (n == 0) return MLOAM_OK;
   cudaStream_t st = c->stream;
-  DevBuf &in = c->scratch[0], &outb = c->scratch[1];
   const size_t N1 = (size_t)n + 16;
-  MLOAM_CUDA_OK(c, in.reserve(44 * N1 + 512));
-  MLOAM_CUDA_OK(c, outb.reserve(44 * N1 + 1024));
-  float4 *d_in = in.as<float4>();
-  float *d_c6 = reinterpret_cast<float *>(in.as<char>() + 16 * N1), *d_tr = d_c6 + 6 * N1;
-  float4 *d_out = outb.as<float4>();
-  float *d_oc6 = reinterpret_cast<float *>(outb.as<char>() + 16 * N1), *d_otr = d_oc6 + 6 * N1;
-  int *d_cnt = reinterpret_cast<int *>(d_otr + N1);
+  float4 *d_in, *d_out;
+  float *d_c6, *d_tr, *d_oc6, *d_otr;
+  int *d_cnt;
+  MLOAM_CUDA_OK(c, carve(c->sweep_in, [&](Carve &cv) { d_in = cv.take<float4>(N1), d_c6 = cv.take<float>(6 * N1), d_tr = cv.take<float>(N1); }));
+  MLOAM_CUDA_OK(c, carve(c->map_in[0], [&](Carve &cv) {
+    d_out = cv.take<float4>(N1), d_oc6 = cv.take<float>(6 * N1), d_otr = cv.take<float>(N1), d_cnt = cv.take<int>(16);
+  }));
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_in, h_pts, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, st));
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_c6, h_cov6, sizeof(float) * 6 * (size_t)n, cudaMemcpyHostToDevice, st));
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_tr, h_trace, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, st));
-  int rc = voxel_downsample_cov_device(c, d_in, d_c6, d_tr, n, nullptr, leaf, trace_threshold, d_out, d_oc6, d_otr, d_cnt, 5);
+  int rc = voxel_downsample_cov_device(c, d_in, d_c6, d_tr, n, nullptr, leaf, trace_threshold, d_out, d_oc6, d_otr, d_cnt, c->voxel_work);
   if (rc) return rc;
-  int *hc = reinterpret_cast<int *>(reinterpret_cast<char *>(c->pinned) + 3072);
+  int *hc = c->pinned->counts;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, st));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
   *n_out = hc[0];
@@ -420,19 +396,20 @@ int mloam_submap_assemble(mloam_ctx_t *h, int slot, int n_keyframes, const mloam
   UctBufs B;
   int rc = uct_bufs(c, n_max, &B);
   if (rc) return rc;
-  DevBuf &in = c->scratch[0], &mid = c->scratch[1], &fin = c->scratch[3];
   const size_t N1 = (size_t)n + 16;
-  MLOAM_CUDA_OK(c, in.reserve(sizeof(float4) * N1 + sizeof(UctLaser) * MLOAM_MAX_LIDARS * (size_t)(n_keyframes + 1) + 512));
-  MLOAM_CUDA_OK(c, mid.reserve(44 * N1 + 1024));
-  MLOAM_CUDA_OK(c, fin.reserve(44 * N1 + 1024));
-  float4 *d_in = in.as<float4>();
-  UctLaser *d_l = reinterpret_cast<UctLaser *>(in.as<char>() + ((sizeof(float4) * N1 + 255) & ~(size_t)255));
-  float4 *d_mid = mid.as<float4>();
-  float *d_mc6 = reinterpret_cast<float *>(mid.as<char>() + 16 * N1), *d_mtr = d_mc6 + 6 * N1;
-  int *d_total = reinterpret_cast<int *>(d_mtr + N1);
-  float4 *d_fin = fin.as<float4>();
-  float *d_fc6 = reinterpret_cast<float *>(fin.as<char>() + 16 * N1), *d_ftr = d_fc6 + 6 * N1;
-  int *d_cnt = reinterpret_cast<int *>(d_ftr + N1);
+  float4 *d_in, *d_mid, *d_fin;
+  UctLaser *d_l;
+  float *d_mc6, *d_mtr, *d_fc6, *d_ftr;
+  int *d_total, *d_cnt;
+  MLOAM_CUDA_OK(c, carve(c->sweep_in, [&](Carve &cv) {
+    d_in = cv.take<float4>(N1), d_l = cv.take<UctLaser>(MLOAM_MAX_LIDARS * (size_t)(n_keyframes + 1));
+  }));
+  MLOAM_CUDA_OK(c, carve(c->map_in[0], [&](Carve &cv) {
+    d_mid = cv.take<float4>(N1), d_mc6 = cv.take<float>(6 * N1), d_mtr = cv.take<float>(N1), d_total = cv.take<int>(16);
+  }));
+  MLOAM_CUDA_OK(c, carve(c->host_work, [&](Carve &cv) {
+    d_fin = cv.take<float4>(N1), d_fc6 = cv.take<float>(6 * N1), d_ftr = cv.take<float>(N1), d_cnt = cv.take<int>(16);
+  }));
   // all keyframe clouds and all per-(keyframe, LiDAR) compound poses go up in two copies
   std::vector<UctLaser> L((size_t)n_keyframes * n_lasers);
   for (int k = 0; k < n_keyframes; k++) {
@@ -453,9 +430,9 @@ int mloam_submap_assemble(mloam_ctx_t *h, int slot, int n_keyframes, const mloam
     off += (size_t)counts[k];
   }
   // VoxelGridCovarianceMLOAM over the merged cloud (:344-347): the merged size is only known on the device
-  rc = voxel_downsample_cov_device(c, d_mid, d_mc6, d_mtr, n, d_total, leaf, trace_threshold_filter, d_fin, d_fc6, d_ftr, d_cnt, 5);
+  rc = voxel_downsample_cov_device(c, d_mid, d_mc6, d_mtr, n, d_total, leaf, trace_threshold_filter, d_fin, d_fc6, d_ftr, d_cnt, c->voxel_work);
   if (rc) return rc;
-  int *hc = reinterpret_cast<int *>(reinterpret_cast<char *>(c->pinned) + 3072);
+  int *hc = c->pinned->counts;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, st));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));  // the map build is sized by the submap's point count
   const int m = hc[0];
@@ -493,23 +470,20 @@ int mloam_local_map_build(mloam_ctx_t *h, int slot, int n_frames, const mloam_po
       mats[12 * k + 4 * r + 3] = (float)e[r];
     }
   }
-  DevBuf &in = c->scratch[0], &outb = c->scratch[1];
   const size_t N1 = (size_t)n + 16;
-  MLOAM_CUDA_OK(c, in.reserve(16 * N1 + 4 * off.size() + 4 * mats.size() + 1024));
-  MLOAM_CUDA_OK(c, outb.reserve(16 * N1 + 256));
-  float4 *d_in = in.as<float4>();
-  int *d_off = reinterpret_cast<int *>(in.as<char>() + ((16 * N1 + 255) & ~(size_t)255));
-  float *d_mat = reinterpret_cast<float *>(d_off + ((off.size() + 63) & ~(size_t)63));
-  float4 *d_out = outb.as<float4>();
-  int *d_cnt = reinterpret_cast<int *>(outb.as<char>() + 16 * N1);
+  float4 *d_in, *d_out;
+  int *d_off, *d_cnt;
+  float *d_mat;
+  MLOAM_CUDA_OK(c, carve(c->sweep_in, [&](Carve &cv) { d_in = cv.take<float4>(N1), d_off = cv.take<int>(off.size()), d_mat = cv.take<float>(mats.size()); }));
+  MLOAM_CUDA_OK(c, carve(c->map_in[0], [&](Carve &cv) { d_out = cv.take<float4>(N1), d_cnt = cv.take<int>(16); }));
   if (n > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_in, h_pts, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, st));
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_off, off.data(), sizeof(int) * off.size(), cudaMemcpyHostToDevice, st));
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_mat, mats.data(), sizeof(float) * mats.size(), cudaMemcpyHostToDevice, st));
   int rc = transform_segments_device(c, d_in, n, d_off, n_frames, d_mat);
   if (rc) return rc;
-  rc = voxel_downsample_device(c, d_in, n, nullptr, leaf, 0, d_out, d_cnt, 5);  // pcl::VoxelGrid<PointI>: every field averaged
+  rc = voxel_downsample_device(c, d_in, n, nullptr, leaf, 0, d_out, d_cnt, c->voxel_work);  // pcl::VoxelGrid<PointI>: every field averaged
   if (rc) return rc;
-  int *hc = reinterpret_cast<int *>(reinterpret_cast<char *>(c->pinned) + 3072);
+  int *hc = c->pinned->counts;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, st));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));  // also: the host vectors above have been consumed
   const int m = hc[0];

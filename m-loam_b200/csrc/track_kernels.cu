@@ -178,7 +178,7 @@ int track_cloud_device(Ctx *c, const float4 *d_prev_less_sharp, int n_pls, const
   c->lm_min_corr = 0;
   if (rc) return rc;
   LMState *st = c->lm_state.as<LMState>();
-  int *h_done = reinterpret_cast<int *>(reinterpret_cast<char *>(c->pinned) + 2048);
+  int *h_done = &c->pinned->done;
   FeatSet sets[2] = {FeatSet{d_cur_sharp, c->feat_valid[0].as<unsigned char>(), c->feat_coeff[0].as<float>(), n_cs, 2, nullptr},
                      FeatSet{d_cur_flat, c->feat_valid[1].as<unsigned char>(), c->feat_coeff[1].as<float>(), n_cf, 1, nullptr}};
   for (int outer = 0; outer < max_outer && rc == MLOAM_OK; outer++) {
@@ -206,7 +206,7 @@ int track_cloud_device(Ctx *c, const float4 *d_prev_less_sharp, int n_pls, const
   }
   c->lm_eig_thre = -1.0;
   if (rc) return rc;
-  LMState *hs = reinterpret_cast<LMState *>(reinterpret_cast<char *>(c->pinned) + 4096);
+  LMState *hs = &c->pinned->lm;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(hs, st, sizeof(LMState), cudaMemcpyDeviceToHost, c->stream));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
   // :126-128 Pose(q, t) normalises
@@ -239,7 +239,7 @@ int mloam_track_cloud(mloam_ctx_t *h, const mloam_point_t *h_prev_less_sharp, in
   const int ns[4] = {n_pls, n_plf, n_cs, n_cf};
   const mloam_point_t *hp[4] = {h_prev_less_sharp, h_prev_less_flat, h_cur_sharp, h_cur_flat};
   float4 *dp[4];
-  DevBuf *bufs[4] = {&c->scratch[0], &c->scratch[1], &c->scan_pts[0], &c->scan_pts[1]};
+  DevBuf *bufs[4] = {&c->sweep_in, &c->map_in[0], &c->scan_pts[0], &c->scan_pts[1]};
   for (int k = 0; k < 4; k++) {
     if (ns[k] > 0 && !hp[k]) return MLOAM_E_INVALID;
     MLOAM_CUDA_OK(c, bufs[k]->reserve(sizeof(float4) * (size_t)(ns[k] + 1)));
@@ -261,18 +261,18 @@ int mloam_match_from_scan(mloam_ctx_t *h, int slot, int type, const mloam_point_
   MLOAM_CUDA_OK(c, c->scan_pts[t].reserve(sizeof(float4) * (size_t)n));
   int rc = reserve_feat(c, t, n);
   if (rc) return rc;
-  MLOAM_CUDA_OK(c, c->scratch[3].reserve(sizeof(int) * 3 * (size_t)n));
+  MLOAM_CUDA_OK(c, c->host_work.reserve(sizeof(int) * 3 * (size_t)n));
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->scan_pts[t].p, h_pts, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
   double *d_pose;
   rc = upload_pose(c, pose7, &d_pose);
   if (rc) return rc;
   rc = match_from_scan_device(c, slot, type, c->scan_pts[t].as<float4>(), n, d_pose, c->feat_valid[t].as<unsigned char>(),
-                              c->feat_coeff[t].as<float>(), c->scratch[3].as<int>());
+                              c->feat_coeff[t].as<float>(), c->host_work.as<int>());
   if (rc) return rc;
   std::vector<float> cf((size_t)n * 6);
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_valid, c->feat_valid[t].p, (size_t)n, cudaMemcpyDeviceToHost, c->stream));
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(cf.data(), c->feat_coeff[t].p, sizeof(float) * 6 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
-  if (h_nn3) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_nn3, c->scratch[3].p, sizeof(int) * 3 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+  if (h_nn3) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_nn3, c->host_work.p, sizeof(int) * 3 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
   for (size_t i = 0; i < (size_t)n * 6; i++) h_coeffs[i] = (double)cf[i];
   return MLOAM_OK;

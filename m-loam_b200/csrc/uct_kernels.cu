@@ -74,17 +74,17 @@ extern "C" int mloam_point_uncertainty(mloam_ctx_t *h, const mloam_point_t *h_pt
   Ctx *c = &h->c;
   cudaSetDevice(c->device);
   if (n == 0) return MLOAM_OK;
-  MLOAM_CUDA_OK(c, c->scratch[1].reserve(sizeof(float4) * (size_t)n));
-  MLOAM_CUDA_OK(c, c->scratch[2].reserve(sizeof(float) * 6 * (size_t)n));
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->scratch[1].p, h_pts, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
+  MLOAM_CUDA_OK(c, c->sweep_in.reserve(sizeof(float4) * (size_t)n));
+  MLOAM_CUDA_OK(c, c->map_in[0].reserve(sizeof(float) * 6 * (size_t)n));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->sweep_in.p, h_pts, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
   UctArgs a;
   memcpy(a.pose, pose7, sizeof(a.pose));
   memcpy(a.cov_pose, cov_pose36, sizeof(a.cov_pose));
   memcpy(a.cov_meas, cov_meas9, sizeof(a.cov_meas));
-  k_point_uncertainty<<<(n + 127) / 128, 128, 0, c->stream>>>(c->scratch[1].as<float4>(), n, a, c->scratch[2].as<float>());
+  k_point_uncertainty<<<(n + 127) / 128, 128, 0, c->stream>>>(c->sweep_in.as<float4>(), n, a, c->map_in[0].as<float>());
   c->launches++;
   MLOAM_CUDA_OK(c, cudaGetLastError());
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_cov6, c->scratch[2].p, sizeof(float) * 6 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_cov6, c->map_in[0].p, sizeof(float) * 6 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
   return MLOAM_OK;
 }

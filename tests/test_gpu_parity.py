@@ -738,6 +738,55 @@ def test_frame_graph_replay_equals_stream_path(mloam, c1):
     g.close()
 
 
+def test_frame_graph_replay_after_rig_change(mloam):
+    """A rig frame's graph replays with the extrinsics of its key: the merge's float 3x4 matrices, like the pose, are staged again
+    before every replay.  Frames A, A, A, A, B, B, A on the same host arrays (the graph keys repeat; the key also holds the parity
+    of the feature double buffer, so a key comes back every second frame): frames 3 and 4 capture rig A's two graphs, frame 7
+    replays the first of them after the frames of rig B staged B's matrices, and must equal frame 3 and the stream path bit for bit."""
+    import os
+
+    scene = syn.make_scene()
+    traj = syn.trajectory(8)
+    surf_map, corner_map = syn.make_submap(scene, 200_000)
+    cloud, ss, se, ext_a = syn.make_multi_sweep(scene, traj[4], 2, 16, 1024, seed=41)
+    init = syn.perturb_pose(traj[4], np.random.Generator(np.random.PCG64(43)))
+    # rig B: the second LiDAR moved by 0.3 m and turned by 5 deg of yaw
+    ext_b = ext_a.copy()
+    ext_b[1, 0] += 0.3
+    h = np.deg2rad(5.0) / 2
+    (x1, y1, z1, w1), (x2, y2, z2, w2) = (0.0, 0.0, np.sin(h), np.cos(h)), ext_a[1, 3:]
+    ext_b[1, 3:] = [w1 * x2 + x1 * w2 + y1 * z2 - z1 * y2, w1 * y2 - x1 * z2 + y1 * w2 + z1 * x2,
+                    w1 * z2 + x1 * y2 - y1 * x2 + z1 * w2, w1 * w2 - x1 * x2 - y1 * y2 - z1 * z2]
+    p = mloam.default_params()
+    p.n_scans, p.max_outer, p.max_inner, p.map_cell, p.max_ring_points = 16, 4, 1, 0.25, 1024
+
+    def run(c):
+        out = []
+        for e in (ext_a, ext_a, ext_a, ext_a, ext_b, ext_b, ext_a):
+            c.set_lidars(2, e)
+            pose, st = c.frame(cloud, ss, se, surf_map, corner_map, init)
+            out.append((pose, st, c.frame_scan()))
+        c.close()
+        return out
+
+    def same(x, y):
+        (pa, sa, ca), (pb, sb, cb) = x, y
+        return (np.array_equal(pa, pb) and sa.keys() == sb.keys() and all(np.array_equal(sa[k], sb[k]) for k in sa)
+                and all(np.array_equal(u, v) for u, v in zip(ca, cb)))
+
+    os.environ["MLOAM_DISABLE_GRAPHS"] = "1"
+    try:
+        plain = mloam.Context(0, p)
+    finally:
+        os.environ.pop("MLOAM_DISABLE_GRAPHS")
+    ref = run(plain)
+    got = run(mloam.Context(0, p))
+    assert not np.array_equal(got[4][0], got[3][0])  # the rigs differ in the result
+    assert same(got[6], got[2])
+    for k in range(7):
+        assert same(got[k], ref[k]), k
+
+
 @pytest.mark.parametrize("n_lidars", [1, 2])
 @pytest.mark.parametrize("gf", [0, orc.GF_GD])
 def test_frame_lookahead_is_exact(mloam, n_lidars, gf):
