@@ -126,6 +126,46 @@ int mloam_profile_reset(mloam_ctx_t *ctx);
 int mloam_project_cloud(mloam_ctx_t *ctx, const mloam_point_t *h_cloud, int n, int vertical_scans, int horizon_scans, double roi_range,
                         mloam_point_t *h_out, int *n_out, int *h_scan_start, int *h_scan_end);
 
+/* ---- raw driver sweeps: the three steps before extractCloud in Estimator::inputCloud (estimator.cpp:249-261), per LiDAR —
+ *      pcl::removeNaNFromPointCloud in the driver node (rosNodeRVKITTI.cpp:154-161, rosNodeRVOxford.cpp:170-177), then
+ *      FeatureExtract::calTimestamp (feature_extract.cpp:25-114), then segmentCloud with segment_cloud: 0 (as mloam_project_cloud).
+ * mloam_cal_timestamp: removeNaN + calTimestamp of ONE LiDAR's sweep: h_out (capacity n) receives the points with a finite x, y and z, in
+ *   input order, intensity = relative time; *n_out their count.  time_field 0: the time from the azimuth (calTimestamp(PointCloud),
+ *   :54-114: -atan2 of the first and last point, the half_passed wrap, (ori - start) / (end - start) * scan_period); time_field 1: from the
+ *   point's timestamp field in microseconds carried in the intensity lane (calTimestamp(PointITimeCloud), :38-52: timestamp * 1e-6).  The
+ *   cloud's own intensity is discarded either way.  scan_period = SCAN_PERIOD (parameters.h:78).
+ * mloam_set_front_end: the front end of mloam_frame_raw*: vertical_scans 16 / 32 / 64, horizon_scans and roi_range as mloam_project_cloud
+ *   takes them, scan_period and time_field as mloam_cal_timestamp.  MLOAM_E_INVALID for another vertical_scans, and when a nonzero
+ *   params.max_ring_points is below horizon_scans (a projected ring holds up to horizon_scans points).
+ * mloam_frame_raw / mloam_frame_raw_device: mloam_frame / mloam_frame_device on the rig's RAW sweeps, concatenated LiDAR-major, h_counts[l]
+ *   points of LiDAR l (n_lidars of mloam_set_lidars, one without it; counts always in host memory).  Per LiDAR removeNaN + calTimestamp +
+ *   projection onto a range image of its own run on the device, batched over the rig; the ring-ordered sweep (LiDAR-major, ring-major,
+ *   n_lidars x vertical_scans rings of ScanInfo) goes to extractCloud without a host round trip.  Results are identical to mloam_frame* on
+ *   the concatenation of the per-LiDAR mloam_cal_timestamp + mloam_project_cloud outputs with the ScanInfo offset by each LiDAR's start.
+ *   with_ua, the keyframe store, mloam_frame_scan and mloam_pose_covariance work as after mloam_frame.  MLOAM_E_INVALID when a count is 0
+ *   (the node's empty_check, rosNodeRVOxford.cpp:216-220); MLOAM_E_STATE without mloam_set_front_end and on a context with a communicator.
+ *   The check is on the counts as passed: a LiDAR whose points are ALL non-finite passes it and contributes empty rings to the frame,
+ *   whereas the node runs removeNaNFromPointCloud before empty_check (rosNodeRVOxford.cpp:175, :216-220) and skips that frame.  Counting
+ *   the finite points would need a device-to-host read-back before the frame; a caller that can receive such sweeps checks them itself
+ *   (mloam_cal_timestamp returns the finite count). 
+ * mloam_front_end: the front end of mloam_frame_raw alone, host-in / host-out: h_out (capacity = sum of counts) receives the ring-ordered
+ *   sweep, *n_out its size, h_scan_start / h_scan_end the n_lidars x vertical_scans rings of its ScanInfo.
+ * mloam_frame_set_next_raw / mloam_frame_set_next_raw_device: the look-ahead of mloam_frame_set_next* for raw sweeps (the front end runs in
+ *   the look-ahead branch too); picked up by the next mloam_frame_raw* call with the same pointer and counts.  NULL withdraws. */
+int mloam_cal_timestamp(mloam_ctx_t *ctx, const mloam_point_t *h_cloud, int n, int time_field, float scan_period, mloam_point_t *h_out,
+                        int *n_out);
+int mloam_set_front_end(mloam_ctx_t *ctx, int vertical_scans, int horizon_scans, double roi_range, float scan_period, int time_field);
+int mloam_front_end(mloam_ctx_t *ctx, const mloam_point_t *h_raw, const int *h_counts, mloam_point_t *h_out, int *n_out, int *h_scan_start,
+                    int *h_scan_end);
+int mloam_frame_raw(mloam_ctx_t *ctx, const mloam_point_t *h_raw, const int *h_counts, const mloam_point_t *h_surf_map, int n_surf_map,
+                    const mloam_point_t *h_corner_map, int n_corner_map, int rebuild_maps, const double *pose_init7, double *pose_out7,
+                    mloam_solve_stats_t *stats);
+int mloam_frame_raw_device(mloam_ctx_t *ctx, const mloam_point_t *d_raw, const int *h_counts, const mloam_point_t *d_surf_map,
+                           int n_surf_map, const mloam_point_t *d_corner_map, int n_corner_map, int rebuild_maps,
+                           const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats);
+int mloam_frame_set_next_raw(mloam_ctx_t *ctx, const mloam_point_t *h_raw, const int *h_counts);
+int mloam_frame_set_next_raw_device(mloam_ctx_t *ctx, const mloam_point_t *d_raw, const int *h_counts);
+
 /* ---- FeatureExtract::extractCloud (feature_extract.cpp:118-297) -------------------------------- */
 int mloam_extract_features(mloam_ctx_t *ctx, const mloam_point_t *h_cloud, int n, const int *h_scan_start,
                            const int *h_scan_end, int n_scans, mloam_features_t *out);

@@ -32,6 +32,8 @@ ABI_SYMBOLS = [
     "mloam_frame_device", "mloam_set_extrinsic", "mloam_set_lidars", "mloam_calib_frame", "mloam_compound_pose_cov", "mloam_cloud_uct_associate", "mloam_voxel_downsample_cov", "mloam_submap_assemble", "mloam_good_features_odom", "mloam_local_map_build", "mloam_match_from_scan", "mloam_track_cloud", "mloam_odom_solve", "mloam_point_uncertainty", "mloam_scan2map_ua", "mloam_good_features", "mloam_comm_unique_id", "mloam_comm_init", "mloam_comm_destroy", "mloam_comm_p2p_export", "mloam_comm_p2p_init", "mloam_comm_p2p_reset",
     "mloam_set_uncertainty", "mloam_pose_covariance", "mloam_frame_scan",
     "mloam_keyframes_init", "mloam_keyframe_save", "mloam_keyframe_submap", "mloam_keyframe_query", "mloam_keyframe_scan",
+    "mloam_cal_timestamp", "mloam_set_front_end", "mloam_front_end", "mloam_frame_raw", "mloam_frame_raw_device", "mloam_frame_set_next_raw",
+    "mloam_frame_set_next_raw_device",
 ]
 
 
@@ -299,6 +301,70 @@ class Context:
         self._ck(lib().mloam_project_cloud(self._h, _p(pts), pts.shape[0], int(vertical_scans), int(horizon_scans), C.c_double(roi_range), _p(out),
                                            C.byref(n), _p(ss), _p(se)))
         return out[: n.value].copy(), ss, se
+
+    # ---- raw driver sweeps (removeNaN + calTimestamp + projection on the device)
+    def cal_timestamp(self, cloud, time_field: bool = False, scan_period: float = 0.1):
+        """removeNaNFromPointCloud + FeatureExtract::calTimestamp of one LiDAR's sweep -> the finite points, intensity = relative time.
+        time_field: the timestamp [us] is in the intensity column (PointITimeCloud overload)."""
+        pts = _cloud(cloud)
+        out = np.empty((max(pts.shape[0], 1), 4), np.float32)
+        n = C.c_int(0)
+        self._ck(lib().mloam_cal_timestamp(self._h, _p(pts), pts.shape[0], int(time_field), C.c_float(scan_period), _p(out), C.byref(n)))
+        return out[: n.value].copy()
+
+    def set_front_end(self, vertical_scans: int, horizon_scans: int, roi_range: float = 0.5, scan_period: float = 0.1, time_field: bool = False):
+        self._ck(lib().mloam_set_front_end(self._h, int(vertical_scans), int(horizon_scans), C.c_double(roi_range), C.c_float(scan_period),
+                                           int(time_field)))
+
+    def front_end(self, raw, counts):
+        """The front end of frame_raw() alone -> (ring-ordered sweep, scan_start, scan_end); the first n_lidars x vertical_scans entries
+        of scan_start / scan_end are the sweep's ScanInfo."""
+        raw = _cloud(raw)
+        cnt = np.ascontiguousarray(counts, np.int32)
+        out = np.empty((max(raw.shape[0], 1), 4), np.float32)
+        n_rings = 1024
+        ss, se = np.zeros(n_rings, np.int32), np.zeros(n_rings, np.int32)
+        n = C.c_int(0)
+        self._ck(lib().mloam_front_end(self._h, _p(raw), _p(cnt), _p(out), C.byref(n), _p(ss), _p(se)))
+        return out[: n.value].copy(), ss, se
+
+    def frame_raw(self, raw, counts, surf_map, corner_map, pose_init7, rebuild_maps: bool = True):
+        """mloam_frame on the rig's raw sweeps (concatenated LiDAR-major, counts[l] points of LiDAR l)."""
+        raw = _cloud(raw)
+        cnt = np.ascontiguousarray(counts, np.int32)
+        sm = None if surf_map is None else _cloud(surf_map)
+        cm = None if corner_map is None else _cloud(corner_map)
+        pi = np.ascontiguousarray(pose_init7, np.float64)
+        out = np.zeros(7)
+        st = SolveStats()
+        self._ck(lib().mloam_frame_raw(self._h, _p(raw), _p(cnt), _p(sm), 0 if sm is None else sm.shape[0], _p(cm),
+                                       0 if cm is None else cm.shape[0], int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
+        return out, st.as_dict()
+
+    def frame_raw_device(self, d_raw: int, counts, d_surf_map: int, n_surf_map: int, d_corner_map: int, n_corner_map: int, pose_init7,
+                         rebuild_maps: bool = True):
+        cnt = np.ascontiguousarray(counts, np.int32)
+        pi = np.ascontiguousarray(pose_init7, np.float64)
+        out = np.zeros(7)
+        st = SolveStats()
+        self._ck(lib().mloam_frame_raw_device(self._h, C.c_void_p(d_raw), _p(cnt), C.c_void_p(d_surf_map), n_surf_map, C.c_void_p(d_corner_map),
+                                              n_corner_map, int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
+        return out, st.as_dict()
+
+    def frame_set_next_raw(self, raw, counts):
+        """Announce the raw sweeps of the next frame_raw() call (pass the SAME array to it).  None withdraws."""
+        if raw is None:
+            self._next_keep = None
+            self._ck(lib().mloam_frame_set_next_raw(self._h, None, None))
+            return
+        raw = _cloud(raw)
+        cnt = np.ascontiguousarray(counts, np.int32)
+        self._next_keep = (raw, cnt)  # must outlive the coming frame call
+        self._ck(lib().mloam_frame_set_next_raw(self._h, _p(raw), _p(cnt)))
+
+    def frame_set_next_raw_device(self, d_raw: int, counts):
+        cnt = None if d_raw is None else np.ascontiguousarray(counts, np.int32)
+        self._ck(lib().mloam_frame_set_next_raw_device(self._h, None if d_raw is None else C.c_void_p(d_raw), _p(cnt)))
 
     # ---- orchestrators
     def scan2map(self, surf_scan, corner_scan, pose_init7):

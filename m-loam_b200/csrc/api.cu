@@ -152,7 +152,7 @@ void mloam_ctx_destroy(mloam_ctx_t *h) {
   c->knn_heavy_list.release(), c->knn_trace.release(), c->knn_spec.release();
   c->partials.release(), c->lm_state.release();
   for (DevBuf *b : {&c->sweep_in, &c->map_in[0], &c->map_in[1], &c->extract_work, &c->voxel_work, &c->voxel_corner, &c->voxel_surf,
-                    &c->host_work, &c->odom_work, &c->ctl})
+                    &c->host_work, &c->odom_work, &c->ctl, &c->front_work, &c->front_out})
     b->release();
   c->frame_main.release(), c->frame_alt.release(), c->next_in.release(), c->stamps.release(), c->ua_scan.release(), c->pose_cov.release();
   if (c->pinned) cudaFreeHost(c->pinned);

@@ -91,6 +91,21 @@ cudaError_t carve(DevBuf &b, Layout &&layout) {
 #define MLOAM_MAX_RINGS 1024  // rings of one (possibly multi-LiDAR) extraction
 #define MLOAM_MAX_LIDARS 16
 
+// A rig's raw sweeps concatenated LiDAR-major: LiDAR l owns points [off[l], off[l + 1]).  Zero-initialised past n_lidars (hashed whole).
+struct RigLayout {
+  int n_lidars;
+  int off[MLOAM_MAX_LIDARS + 1];
+};
+// The front end of raw frames (mloam_set_front_end): removeNaNFromPointCloud + FeatureExtract::calTimestamp + the range-image projection
+// of segment_cloud: 0, per LiDAR (estimator.cpp:249-261).  No padding: hashed whole into the frame graph key.
+struct FrontEnd {
+  int vertical_scans, horizon_scans;
+  double roi_range;
+  float scan_period;
+  int time_field;  // 0: time from the azimuth; 1: from the point's timestamp [us] in the w lane (PointITimeCloud overload)
+};
+static_assert(sizeof(FrontEnd) == 24 && sizeof(RigLayout) == 4 * (MLOAM_MAX_LIDARS + 2), "hashed whole: no padding");
+
 // the per-point association with uncertainty (uct.h): per LiDAR of the rig, and per run
 struct UctLaser {
   double ext_inv[7];   // pose_ext[n].inverse()
@@ -295,6 +310,8 @@ struct Ctx {
     bool host = false;          // key_ptr is a host pointer (mloam_frame) / a device pointer (mloam_frame_device)
     const void *key_ptr = nullptr;
     int n = 0, n_scans = 0, parity = 0;
+    bool raw = false;           // features of a raw sweep (mloam_frame_raw*) with this layout
+    RigLayout L{};
     ScanRef S{};
   };
   struct NextSweep {
@@ -303,7 +320,16 @@ struct Ctx {
     const float4 *d_cloud = nullptr;    // where the sweep is (or will be, after the pending H2D) on the device
     const int *d_scan_start = nullptr, *d_scan_end = nullptr;
     int n = 0, n_scans = 0;
+    bool raw = false;                   // a raw sweep (mloam_frame_set_next_raw*): the front end runs before extraction
+    RigLayout L{};
   };
+  // raw frames (mloam_set_front_end, mloam_frame_raw*): the front end runs inside features_enqueue, on the main stream and in the look-ahead
+  // branch.  Its work (winner images, sort) and output (projected cloud + ScanInfo) have buffers of their own: the look-ahead reuses them
+  // after the main stream's front end, while the main stream runs the with_ua stage and the solve.
+  FrontEnd front{};
+  bool front_set = false;
+  const RigLayout *raw_now = nullptr;  // the raw sweep of the frame being enqueued (nullptr: a ring-ordered sweep)
+  DevBuf front_work, front_out;
   Features prefetched;             // features of the sweep announced with the previous frame, ready when that frame returned
   NextSweep next;                  // announced for the frame being enqueued (consumed by it)
   const void *cloud_key = nullptr; // mloam_frame: the HOST pointer of the sweep being processed (look-ahead matches on it)
@@ -512,8 +538,15 @@ struct ExtractWork {
 void extract_work_layout(Carve &cv, int n, int n_scans, ExtractWork *W);
 // in place: segment l of d_pts (points [d_off[l], d_off[l + 1])) <- float 3x4 matrix l times the point, intensity kept
 void stamp(Ctx *c, const char *label);  // api.cu
-int project_cloud_device(Ctx *c, const float4 *d_in, int n, int vertical_scans, int horizon_scans, double roi_range, float4 *d_out,
-                         int *d_scan_start, int *d_scan_end, int *d_n_out);
+// Range-image projection of the LiDARs of layout L (each with a vertical_scans x horizon_scans image of its own): output LiDAR-major,
+// ring-major, input order within a ring, packed; ScanInfo of L.n_lidars x vertical_scans rings (+5 / -6).  fe (nullable): removeNaN +
+// calTimestamp of every LiDAR first, and the output's tail past the projected count zeroed.  Work in `work`.
+int project_cloud_device(Ctx *c, const float4 *d_in, const RigLayout &L, int vertical_scans, int horizon_scans, double roi_range,
+                         const FrontEnd *fe, float4 *d_out, int *d_scan_start, int *d_scan_end, int *d_n_out, DevBuf &work);
+// removeNaN + calTimestamp of the LiDARs of L, compacted: d_out receives the finite points in input order with w = relative time,
+// *d_n_out their count.
+int front_times_device(Ctx *c, const float4 *d_in, const RigLayout &L, int time_field, float scan_period, float4 *d_out, int *d_n_out,
+                       DevBuf &work);
 int transform_segments_device(Ctx *c, float4 *d_pts, int n, const int *d_off, int n_seg, const float *d_mat12);
 // VoxelGridCovarianceMLOAM<PointIWithCov>::filter: covariance-weighted merge per voxel (cov6 + trace per point in and out)
 int voxel_downsample_cov_device(Ctx *c, const float4 *d_in, const float *d_cov6, const float *d_trace, int n, const int *d_n_in, float leaf,

@@ -12,6 +12,7 @@
 //
 // Float arithmetic follows the reference's evaluation order; integer/index results are exact.
 #include "ctx.h"
+#include "cal_timestamp.cuh"
 #include "project.cuh"
 #include "primitives.cuh"
 
@@ -439,38 +440,45 @@ static int voxel_work_reserve(Ctx *c, DevBuf &buf, int n, int n_seg, VoxelWork *
 // every point gets a (row, column) pixel of the vertical_scans x horizon_scans range image, the first point (input order) of a pixel wins,
 // intensity += row, and the output is the rows concatenated, each in input order; ScanInfo = [row begin + 5, row end - 6].
 // The float arithmetic follows the reference expression by expression (explicitly rounded operations, fdlibm atanf / atan2f — fd_atan.cuh).
-__global__ void k_project_pixels(const float4 *__restrict__ P, int n, ProjectParam sp, int *__restrict__ pix, int *__restrict__ winner) {
+// Batched over a rig (RigLayout): LiDAR l has an image of its own and its rows are rows l * vertical_scans + r of the output.
+__device__ __forceinline__ int rig_lidar_of(const RigLayout &L, int i) {
+  int l = 0;
+  while (l + 1 < L.n_lidars && i >= L.off[l + 1]) l++;
+  return l;
+}
+__global__ void k_project_pixels(const float4 *__restrict__ P, int n, ProjectParam sp, RigLayout L, int *__restrict__ pix,
+                                 int *__restrict__ winner) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   int row = 0;
-  const int px = project_pixel(sp, P[i], &row);
+  int px = project_pixel(sp, P[i], &row);
+  if (px >= 0 && L.n_lidars > 1) px += rig_lidar_of(L, i) * sp.vertical_scans * sp.horizon_scans;
   pix[i] = px;
   if (px >= 0) atomicMin(&winner[px], i);
 }
 __global__ void k_project_keys(const int *__restrict__ pix, const int *__restrict__ winner, int n, int horizon_scans,
-                               unsigned long long *__restrict__ keys, unsigned *__restrict__ vals) {
+                               unsigned long long none, unsigned long long *__restrict__ keys, unsigned *__restrict__ vals) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int px = pix[i];
-  keys[i] = (px >= 0 && winner[px] == i) ? (unsigned long long)(px / horizon_scans) : 255ull;
+  keys[i] = (px >= 0 && winner[px] == i) ? (unsigned long long)(px / horizon_scans) : none;  // (lidar, row)
   vals[i] = (unsigned)i;
 }
 __global__ void k_project_emit(const float4 *__restrict__ P, const unsigned long long *__restrict__ keys, const unsigned *__restrict__ vals,
-                               int n, float4 *__restrict__ out) {
+                               int n, unsigned long long none, int vertical_scans, float4 *__restrict__ out) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n) return;
   const unsigned long long k = keys[j];
-  if (k >= 255ull) return;
+  if (k >= none) return;
   float4 p = P[vals[j]];
-  p.w = __fadd_rn(p.w, (float)(int)k);
+  p.w = __fadd_rn(p.w, (float)(int)(k % (unsigned long long)vertical_scans));
   out[j] = p;
 }
-// thread r <= vertical_scans: first sorted position whose row is >= r
-__global__ void k_project_rows(const unsigned long long *__restrict__ keys, int n, int vertical_scans, int *__restrict__ scan_start,
+// r in 0..n_rows: first sorted position whose (lidar, row) key is >= r
+__global__ void k_project_rows(const unsigned long long *__restrict__ keys, int n, int n_rows, int *__restrict__ scan_start,
                                int *__restrict__ scan_end, int *__restrict__ n_out) {
-  __shared__ int begin[257];
-  const int r = threadIdx.x;
-  if (r <= vertical_scans) {
+  __shared__ int begin[MLOAM_MAX_RINGS + 1];
+  for (int r = threadIdx.x; r <= n_rows; r += blockDim.x) {
     int lo = 0, hi = n;
     while (lo < hi) {
       const int mid = (lo + hi) >> 1;
@@ -480,37 +488,171 @@ __global__ void k_project_rows(const unsigned long long *__restrict__ keys, int 
     begin[r] = lo;
   }
   __syncthreads();
-  if (r < vertical_scans) scan_start[r] = begin[r] + 5, scan_end[r] = begin[r + 1] - 6;
-  if (r == vertical_scans) *n_out = begin[r];
+  for (int r = threadIdx.x; r <= n_rows; r += blockDim.x) {
+    if (r < n_rows) scan_start[r] = begin[r] + 5, scan_end[r] = begin[r + 1] - 6;
+    else *n_out = begin[r];
+  }
 }
 
-int project_cloud_device(Ctx *c, const float4 *d_in, int n, int vertical_scans, int horizon_scans, double roi_range, float4 *d_out,
-                         int *d_scan_start, int *d_scan_end, int *d_n_out) {
-  if (n <= 0 || horizon_scans <= 0 || (vertical_scans != 16 && vertical_scans != 32 && vertical_scans != 64)) {
+// ------------------------------------------------------------------------------------------ calTimestamp
+// FeatureExtract::calTimestamp (feature_extract.cpp:25-114, cal_timestamp.cuh) per LiDAR of a rig after removeNaNFromPointCloud, without a
+// compaction: ends[l] / ends[16 + l] = first / last finite point of LiDAR l, ends[32 + l] = its flip index (first point whose first-half
+// angle sets half_passed).  The start / end angles of every LiDAR (findStartEndAngle) are computed once per CTA of k_front_flip into shared
+// memory, and CTA 0 leaves them in `angles` (start | end) for k_front_times.  The timed cloud keeps the input order; a dropped point
+// becomes an all-NaN point, which no pixel takes.
+__global__ void k_front_ends(const float4 *__restrict__ P, int n, RigLayout L, int *__restrict__ ends) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || !ts_finite(P[i])) return;
+  const int l = rig_lidar_of(L, i);
+  atomicMin(&ends[l], i);
+  atomicMax(&ends[MLOAM_MAX_LIDARS + l], i);
+}
+__global__ void k_front_flip(const float4 *__restrict__ P, int n, RigLayout L, int *__restrict__ ends, float *__restrict__ angles) {
+  __shared__ float ang[2 * MLOAM_MAX_LIDARS];
+  const int t = threadIdx.x;
+  if (t < L.n_lidars) {
+    float start_ori = 0.f, end_ori = 0.f;
+    if (ends[MLOAM_MAX_LIDARS + t] >= 0) ts_start_end(P[ends[t]], P[ends[MLOAM_MAX_LIDARS + t]], &start_ori, &end_ori);  // else: no finite point
+    ang[t] = start_ori, ang[MLOAM_MAX_LIDARS + t] = end_ori;
+    if (blockIdx.x == 0) angles[t] = start_ori, angles[MLOAM_MAX_LIDARS + t] = end_ori;
+  }
+  __syncthreads();
+  const int i = blockIdx.x * blockDim.x + t;
+  if (i >= n) return;
+  const float4 p = P[i];
+  if (!ts_finite(p)) return;
+  const int l = rig_lidar_of(L, i);
+  bool flips;
+  ts_ori_first_half(p, ang[l], &flips);
+  if (flips) atomicMin(&ends[2 * MLOAM_MAX_LIDARS + l], i);
+}
+__global__ void k_front_times(const float4 *__restrict__ P, int n, RigLayout L, int time_field, float scan_period, const int *__restrict__ ends,
+                              const float *__restrict__ angles, float4 *__restrict__ out, int *__restrict__ keep) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 p = P[i];
+  const bool fin = ts_finite(p);
+  if (keep) keep[i] = fin ? 1 : 0;
+  if (!fin) {
+    const float q = __int_as_float(0x7fc00000);
+    out[i] = make_float4(q, q, q, q);
+    return;
+  }
+  float t;
+  if (time_field) t = ts_from_stamp(p.w);
+  else {
+    const int l = rig_lidar_of(L, i);
+    t = ts_point_time_at(p, i - L.off[l], angles[l], angles[MLOAM_MAX_LIDARS + l], ends[2 * MLOAM_MAX_LIDARS + l] - L.off[l], 0, scan_period);
+  }
+  out[i] = make_float4(p.x, p.y, p.z, t);
+}
+
+// work of project_cloud_device / front_times_device in `buf` for n points and n_pix pixels
+struct ProjectWork {
+  SortBufs sb;
+  int *pix, *winner, *ends;
+  float *angles;
+  float4 *timed;
+};
+static int project_work_reserve(Ctx *c, DevBuf &buf, int n, size_t n_pix, ProjectWork *w) {
+  const int nblk = (n + PRIM_TILE - 1) / PRIM_TILE + 1;
+  const int n_hist = 256 * nblk;
+  const int n_tmp = (std::max(n, n_hist) + PRIM_TILE - 1) / PRIM_TILE + 1;
+  const size_t n1 = (size_t)n + 1;
+  MLOAM_CUDA_OK(c, carve(buf, [&](Carve &cv) {
+    w->sb.k0 = cv.take<unsigned long long>(n1), w->sb.k1 = cv.take<unsigned long long>(n1);
+    w->sb.v0 = cv.take<unsigned>(n1), w->sb.v1 = cv.take<unsigned>(n1);
+    w->sb.hist = cv.take<int>(n_hist), w->sb.tmp = cv.take<int>(n_tmp), w->sb.ticket = cv.take<unsigned>(4);
+    w->pix = cv.take<int>(n1), w->winner = cv.take<int>(n_pix), w->ends = cv.take<int>(3 * MLOAM_MAX_LIDARS);
+    w->angles = cv.take<float>(2 * MLOAM_MAX_LIDARS);
+    w->timed = cv.take<float4>(n1);
+  }));
+  return MLOAM_OK;
+}
+
+static int front_times(Ctx *c, const float4 *d_in, const RigLayout &L, int time_field, float scan_period, const ProjectWork &w, float4 *d_out,
+                       int *d_keep) {
+  const int n = L.off[L.n_lidars];
+  if (n <= 0) return MLOAM_OK;
+  ProfScope ps(c, "front_end");
+  cudaStream_t st = c->stream;
+  const int nb = (n + 255) / 256;
+  if (!time_field) {
+    MLOAM_CUDA_OK(c, cudaMemsetAsync(w.ends, 0x7f, sizeof(int) * 3 * MLOAM_MAX_LIDARS, st));
+    MLOAM_CUDA_OK(c, cudaMemsetAsync(w.ends + MLOAM_MAX_LIDARS, 0xff, sizeof(int) * MLOAM_MAX_LIDARS, st));
+    k_front_ends<<<nb, 256, 0, st>>>(d_in, n, L, w.ends);
+    k_front_flip<<<nb, 256, 0, st>>>(d_in, n, L, w.ends, w.angles);
+    c->launches += 2;
+  }
+  k_front_times<<<nb, 256, 0, st>>>(d_in, n, L, time_field, scan_period, w.ends, w.angles, d_out, d_keep);
+  c->launches++;
+  MLOAM_CUDA_OK(c, cudaGetLastError());
+  return MLOAM_OK;
+}
+__global__ void k_front_compact(const float4 *__restrict__ timed, const int *__restrict__ keep, const int *__restrict__ slot, int n,
+                                float4 *__restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && keep[i]) out[slot[i]] = timed[i];
+}
+int front_times_device(Ctx *c, const float4 *d_in, const RigLayout &L, int time_field, float scan_period, float4 *d_out, int *d_n_out,
+                       DevBuf &work) {
+  const int n = L.off[L.n_lidars];
+  ProjectWork w;
+  int rc = project_work_reserve(c, work, n, 1, &w);
+  if (rc) return rc;
+  rc = front_times(c, d_in, L, time_field, scan_period, w, w.timed, w.pix);
+  if (rc) return rc;
+  int *slot = reinterpret_cast<int *>(w.sb.v0);
+  scan_exclusive(c, w.pix, slot, n, w.sb.tmp, d_n_out);
+  k_front_compact<<<(n + 255) / 256, 256, 0, c->stream>>>(w.timed, w.pix, slot, n, d_out);
+  c->launches++;
+  MLOAM_CUDA_OK(c, cudaGetLastError());
+  return MLOAM_OK;
+}
+
+int project_cloud_device(Ctx *c, const float4 *d_in, const RigLayout &L, int vertical_scans, int horizon_scans, double roi_range,
+                         const FrontEnd *fe, float4 *d_out, int *d_scan_start, int *d_scan_end, int *d_n_out, DevBuf &work) {
+  const int n = L.off[L.n_lidars];
+  if (L.n_lidars < 1 || L.n_lidars > MLOAM_MAX_LIDARS) {
+    c->err = "project_cloud: the rig must have 1 to 16 LiDARs";
+    return MLOAM_E_INVALID;
+  }
+  if (n <= 0 || horizon_scans <= 0) {
+    c->err = "project_cloud: empty cloud or horizon_scans <= 0";
+    return MLOAM_E_INVALID;
+  }
+  if (vertical_scans != 16 && vertical_scans != 32 && vertical_scans != 64) {
     c->err = "project_cloud: vertical_scans must be 16, 32 or 64 (ImageSegmenter::setParameter)";
     return MLOAM_E_INVALID;
   }
-  ProfScope ps(c, "project");
   const ProjectParam sp = project_param(vertical_scans, horizon_scans, roi_range);
-  VoxelWork w;
-  int rc = voxel_work_reserve(c, c->voxel_work, n, 1, &w);
+  const size_t n_pix = (size_t)L.n_lidars * vertical_scans * horizon_scans;
+  ProjectWork w;
+  int rc = project_work_reserve(c, work, n, n_pix, &w);
   if (rc) return rc;
-  const size_t n_pix = (size_t)vertical_scans * horizon_scans;
-  MLOAM_CUDA_OK(c, c->host_work.reserve(sizeof(int) * n_pix));
-  int *winner = c->host_work.as<int>();
+  if (fe) {  // removeNaN + calTimestamp of every LiDAR first: the projection reads the timed cloud
+    rc = front_times(c, d_in, L, fe->time_field, fe->scan_period, w, w.timed, nullptr);
+    if (rc) return rc;
+    d_in = w.timed;
+  }
+  ProfScope ps(c, "project");
   cudaStream_t st = c->stream;
-  MLOAM_CUDA_OK(c, cudaMemsetAsync(winner, 0x7f, sizeof(int) * n_pix, st));
-  MLOAM_CUDA_OK(c, cudaMemsetAsync(w.ticket, 0, 16, st));
+  const int n_rows = L.n_lidars * vertical_scans;
+  const int nbits = n_rows < 255 ? 8 : 16;  // (lidar, row) keys; all-ones = no pixel, sorts last
+  const unsigned long long none = (1ull << nbits) - 1;
+  MLOAM_CUDA_OK(c, cudaMemsetAsync(w.winner, 0x7f, sizeof(int) * n_pix, st));
+  MLOAM_CUDA_OK(c, cudaMemsetAsync(w.sb.ticket, 0, 16, st));
+  // a frame extracts the projected cloud with the raw size as its capacity: the tail past the projected count is zeros, never stale data
+  if (fe) MLOAM_CUDA_OK(c, cudaMemsetAsync(d_out, 0, sizeof(float4) * (size_t)n, st));
   const int nb = (n + 255) / 256;
-  k_project_pixels<<<nb, 256, 0, st>>>(d_in, n, sp, w.head, winner);
-  k_project_keys<<<nb, 256, 0, st>>>(w.head, winner, n, horizon_scans, w.k0, w.v0);
+  k_project_pixels<<<nb, 256, 0, st>>>(d_in, n, sp, L, w.pix, w.winner);
+  k_project_keys<<<nb, 256, 0, st>>>(w.pix, w.winner, n, horizon_scans, none, w.sb.k0, w.sb.v0);
   c->launches += 2;
-  SortBufs sb{w.k0, w.k1, w.v0, w.v1, w.hist, w.tmp, w.ticket};
-  const int cur = radix_sort(c, sb, n, nullptr, 8);
-  const unsigned long long *ks = cur ? w.k1 : w.k0;
-  const unsigned *vs = cur ? w.v1 : w.v0;
-  k_project_emit<<<nb, 256, 0, st>>>(d_in, ks, vs, n, d_out);
-  k_project_rows<<<1, 96, 0, st>>>(ks, n, vertical_scans, d_scan_start, d_scan_end, d_n_out);
+  const int cur = radix_sort(c, w.sb, n, nullptr, nbits);
+  const unsigned long long *ks = cur ? w.sb.k1 : w.sb.k0;
+  const unsigned *vs = cur ? w.sb.v1 : w.sb.v0;
+  k_project_emit<<<nb, 256, 0, st>>>(d_in, ks, vs, n, none, vertical_scans, d_out);
+  k_project_rows<<<1, 256, 0, st>>>(ks, n, n_rows, d_scan_start, d_scan_end, d_n_out);
   c->launches += 2;
   MLOAM_CUDA_OK(c, cudaGetLastError());
   return MLOAM_OK;

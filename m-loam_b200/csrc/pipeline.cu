@@ -282,17 +282,34 @@ void stage_frame_inputs(Ctx *c, const double *pose7) {
 
 bool frame_has_prefetched(const Ctx *c, const void *key_ptr, int n, int n_scans) {
   const Ctx::Features &f = c->prefetched;
-  return f.valid && c->use_lookahead && !c->prof_on && f.key_ptr == key_ptr && f.n == n && f.n_scans == n_scans;
+  // a raw sweep's features are taken by a raw frame with the same per-LiDAR counts only, and a ring-ordered sweep's by a ring-ordered frame
+  const bool same_kind = c->raw_now ? (f.raw && std::memcmp(&f.L, c->raw_now, sizeof(RigLayout)) == 0) : !f.raw;
+  return f.valid && c->use_lookahead && !c->prof_on && f.key_ptr == key_ptr && f.n == n && f.n_scans == n_scans && same_kind;
 }
 
 // extractCloud + (multi-LiDAR merge | base-frame transform) + downsampleCurrentScan of one sweep on c->stream, into half `parity` of the
-// feature double buffer.  `side` / ev_fork_v / ev_join_v: the stream and events of the corner-filter fork.
+// feature double buffer.  `side` / ev_fork_v / ev_join_v: the stream and events of the corner-filter fork.  raw (nullable): d_cloud is
+// the rig's raw sweeps with this layout — the front end (removeNaN + calTimestamp + projection, Ctx::front) makes the ring-ordered sweep
+// and its ScanInfo on the device first, and extraction takes them with the raw size n as capacity (no count comes back to the host).
 int features_enqueue(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, const int *d_scan_end, int n_scans, int parity,
-                     cudaStream_t side, cudaEvent_t ev_fork_v, cudaEvent_t ev_join_v, ScanRef *S_out) {
+                     cudaStream_t side, cudaEvent_t ev_fork_v, cudaEvent_t ev_join_v, const RigLayout *raw, ScanRef *S_out) {
   const mloam_params_t &P = c->params;
   FrameBufs F;
   int rc = frame_bufs(c, n, &F, parity);
   if (rc) return rc;
+  if (raw) {
+    const FrontEnd &fe = c->front;
+    float4 *proj;
+    int *ss, *n_proj;
+    MLOAM_CUDA_OK(c, carve(c->front_out, [&](Carve &cv) {
+      proj = cv.take<float4>((size_t)n + 1), ss = cv.take<int>(2 * (size_t)n_scans), n_proj = cv.take<int>(4);
+    }));
+    rc = project_cloud_device(c, d_cloud, *raw, fe.vertical_scans, fe.horizon_scans, fe.roi_range, &fe, proj, ss, ss + n_scans, n_proj,
+                              c->front_work);
+    if (rc) return rc;
+    stamp(c, "front end");
+    d_cloud = proj, d_scan_start = ss, d_scan_end = ss + n_scans;
+  }
   rc = extract_device(c, d_cloud, n, d_scan_start, d_scan_end, n_scans, F.ex, nullptr, nullptr);
   if (rc) return rc;
   stamp(c, "extract");
@@ -386,7 +403,7 @@ int frame_enqueue(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start,
   if (have) {
     S = c->prefetched.S, parity = c->prefetched.parity;
   } else {
-    rc = features_enqueue(c, d_cloud, n, d_scan_start, d_scan_end, n_scans, parity, c->stream3, c->ev_fork3, c->ev_join3, &S);
+    rc = features_enqueue(c, d_cloud, n, d_scan_start, d_scan_end, n_scans, parity, c->stream3, c->ev_fork3, c->ev_join3, c->raw_now, &S);
     if (rc) return rc;
   }
   c->prefetched.valid = false;
@@ -408,13 +425,15 @@ int frame_enqueue(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start,
     c->stream = c->stream4;
     c->stamp_mute = true;
     ScanRef Sn{};
-    rc = features_enqueue(c, nx.d_cloud, nx.n, nx.d_scan_start, nx.d_scan_end, nx.n_scans, parity ^ 1, c->stream5, c->ev_fork5, c->ev_join5, &Sn);
+    rc = features_enqueue(c, nx.d_cloud, nx.n, nx.d_scan_start, nx.d_scan_end, nx.n_scans, parity ^ 1, c->stream5, c->ev_fork5, c->ev_join5,
+                          nx.raw ? &nx.L : nullptr, &Sn);
     c->stamp_mute = false;
     c->stream = main_stream;
     if (rc) return rc;
     MLOAM_CUDA_OK(c, cudaEventRecord(c->ev_join4, c->stream4));
     ahead = true;
     nf.valid = true, nf.host = nx.host, nf.key_ptr = nx.key_ptr, nf.n = nx.n, nf.n_scans = nx.n_scans, nf.parity = parity ^ 1, nf.S = Sn;
+    nf.raw = nx.raw, nf.L = nx.L;
   }
   c->next.set = false;
   stamp(c, have ? "features (prefetched)" : "extract + voxel");
@@ -444,6 +463,13 @@ int stage_next_sweep(Ctx *c) {
   SweepIn D;
   int rc = sweep_bufs(c, c->next_in, n, ns, &D);
   if (rc) return rc;
+  if (c->next.raw) {  // a raw sweep has no ScanInfo: the front end of the look-ahead branch makes it
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.cloud, c->next.key_ptr, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, c->stream4));
+    MLOAM_CUDA_OK(c, cudaEventRecord(c->ev_next, c->stream4));
+    c->next.d_cloud = D.cloud;
+    c->next_pending = true;
+    return MLOAM_OK;
+  }
   // ScanInfo goes through the context's pinned block: an async copy from pageable memory would block the host behind the sweep's copy
   int(*pin)[MLOAM_MAX_RINGS] = c->pinned->scan_info_next;
   std::memcpy(pin[0], c->next_host_ss, sizeof(int) * ns), std::memcpy(pin[1], c->next_host_se, sizeof(int) * ns);
@@ -494,6 +520,10 @@ int frame_run(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, con
     key = fnv1a(key, c->lidar_ext, sizeof(double) * 7 * (size_t)c->n_lidars);
     key = fnv1a(key, &c->stream, sizeof(c->stream));
     key = fnv1a(key, &c->with_ua, sizeof(c->with_ua));  // the covariances and the threshold are staged, not part of the key
+    if (c->raw_now) {  // raw frame: the per-LiDAR counts and the front-end parameters are kernel arguments of the captured front end
+      key = fnv1a(key, c->raw_now, sizeof(RigLayout));
+      key = fnv1a(key, &c->front, sizeof(c->front));
+    }
     if (!rebuild_maps) {
       // the map-size gate (scan2map_enqueue) is decided on the host at capture: with maps built outside the frame (mloam_map_build*,
       // mloam_submap_assemble, mloam_keyframe_submap) a graph captured while it failed must not be replayed once it passes, and back
@@ -511,6 +541,7 @@ int frame_run(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, con
                            ahead ? static_cast<const void *>(c->next.d_scan_start) : nullptr, ahead ? static_cast<const void *>(c->next.d_scan_end) : nullptr};
       key = fnv1a(key, la, sizeof(la));
       key = fnv1a(key, lp, sizeof(lp));
+      if (ahead && c->next.raw) key = fnv1a(key, &c->next.L, sizeof(RigLayout)), key = fnv1a(key, &c->front, sizeof(c->front));
     }
     Ctx::GraphEntry *e = nullptr;
     for (auto &g : c->graphs)
@@ -571,6 +602,79 @@ int frame_run(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, con
   if (rc) return rc;
   c->last_scan = S, c->last_scan_valid = true;
   return scan2map_finish(c, S, pose_init7, pose_out7, stats);
+}
+
+// The layout of a rig's raw sweeps (h_counts[l] points of LiDAR l, n_lidars of mloam_set_lidars) and its ring count, after the checks
+// every raw entry point makes
+int raw_layout(Ctx *c, const int *h_counts, RigLayout *L, int *n_scans) {
+  if (!c->front_set) return fail(c, MLOAM_E_STATE, "frame_raw: call mloam_set_front_end first");
+  if (c->nccl_comm) return fail(c, MLOAM_E_STATE, "frame_raw: raw frames are single-GPU only; detach the communicator");
+  if (!h_counts) return MLOAM_E_INVALID;
+  const FrontEnd &fe = c->front;
+  if (c->params.max_ring_points > 0 && c->params.max_ring_points < fe.horizon_scans)
+    return fail(c, MLOAM_E_INVALID, "frame_raw: params.max_ring_points is below horizon_scans (a projected ring holds up to horizon_scans points)");
+  *L = RigLayout{};
+  L->n_lidars = c->n_lidars;
+  long long total = 0;
+  for (int l = 0; l < c->n_lidars; l++) {
+    if (h_counts[l] <= 0)  // the driver node's empty_check (rosNodeRVOxford.cpp:216-220)
+      return fail(c, MLOAM_E_INVALID, "frame_raw: every LiDAR of the rig needs a non-empty sweep");
+    L->off[l] = (int)total;
+    total += h_counts[l];
+    if (total > (1 << 30)) return fail(c, MLOAM_E_INVALID, "frame_raw: sweeps too large");
+  }
+  L->off[c->n_lidars] = (int)total;
+  *n_scans = c->n_lidars * fe.vertical_scans;
+  return MLOAM_OK;
+}
+struct RawScope {  // Ctx::raw_now for the duration of one entry point
+  Ctx *c;
+  RawScope(Ctx *cc, const RigLayout *L) : c(cc) { c->raw_now = L; }
+  ~RawScope() { c->raw_now = nullptr; }
+};
+
+// mloam_frame / mloam_frame_raw: the sweep (+ its ScanInfo, unless it is a raw sweep: Ctx::raw_now) and the submaps go up, then frame_run
+int frame_host(Ctx *c, const mloam_point_t *h_cloud, int n, const int *h_scan_start, const int *h_scan_end, int n_scans,
+               const mloam_point_t *h_surf_map, int n_surf_map, const mloam_point_t *h_corner_map, int n_corner_map, int rebuild_maps,
+               const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
+  cudaSetDevice(c->device);
+  cudaStream_t st = c->stream;
+  SweepIn D;
+  int rc = sweep_bufs(c, c->sweep_in, n, n_scans, &D);
+  if (rc) return rc;
+  // the sweep was announced with the previous frame and its features are ready (look-ahead): nothing to copy
+  const bool have = c->prefetched.host && frame_has_prefetched(c, h_cloud, n, n_scans);
+  if (!have) {
+    if (!c->raw_now) {  // a raw sweep has no ScanInfo yet: the front end makes it on the device
+      int(*pin)[MLOAM_MAX_RINGS] = c->pinned->scan_info;
+      std::memcpy(pin[0], h_scan_start, sizeof(int) * n_scans), std::memcpy(pin[1], h_scan_end, sizeof(int) * n_scans);
+      MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.scan_start, pin[0], sizeof(int) * n_scans, cudaMemcpyHostToDevice, st));
+      MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.scan_end, pin[1], sizeof(int) * n_scans, cudaMemcpyHostToDevice, st));
+    }
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.cloud, h_cloud, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, st));
+  }
+  rc = stage_next_sweep(c);
+  if (rc) return rc;
+  const float4 *d_sm = nullptr, *d_cm = nullptr;
+  if (rebuild_maps) {
+    if (!h_surf_map || !h_corner_map || n_surf_map < 0 || n_corner_map < 0) return MLOAM_E_INVALID;
+    DevBuf &ms = c->map_in[0], &mc = c->map_in[1];
+    MLOAM_CUDA_OK(c, ms.reserve(sizeof(float4) * (size_t)(n_surf_map + 1)));
+    MLOAM_CUDA_OK(c, mc.reserve(sizeof(float4) * (size_t)(n_corner_map + 1)));
+    // The submaps (16 B/point, ~8x the sweep) go up on the side stream so that the copy overlaps extraction and scan
+    // down-sampling of the sweep; the map-build branch of frame_enqueue is ordered after ev_maps.
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(ms.p, h_surf_map, sizeof(float4) * (size_t)n_surf_map, cudaMemcpyHostToDevice, c->stream2));
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(mc.p, h_corner_map, sizeof(float4) * (size_t)n_corner_map, cudaMemcpyHostToDevice, c->stream2));
+    MLOAM_CUDA_OK(c, cudaEventRecord(c->ev_maps, c->stream2));
+    c->maps_pending = true;
+    d_sm = ms.as<float4>(), d_cm = mc.as<float4>();
+  }
+  c->cloud_key = h_cloud;
+  rc = frame_run(c, D.cloud, n, D.scan_start, D.scan_end, n_scans, d_sm, n_surf_map, d_cm, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+  c->cloud_key = nullptr;
+  c->maps_pending = false, c->next_pending = false, c->next.set = false;
+  if (rc == MLOAM_OK) memcpy(c->last_pose7, pose_out7, sizeof(c->last_pose7)), c->frame_since_save = true;  // mloam_keyframe_save
+  return rc;
 }
 
 }  // namespace
@@ -718,7 +822,10 @@ int mloam_project_cloud(mloam_ctx_t *h, const mloam_point_t *h_cloud, int n, int
   MLOAM_CUDA_OK(c, carve(c->map_in[0], [&](Carve &cv) { d_out = cv.take<float4>(n), d_meta = cv.take<int>(192); }));
   cudaStream_t st = c->stream;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->sweep_in.p, h_cloud, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, st));
-  int rc = project_cloud_device(c, c->sweep_in.as<float4>(), n, vertical_scans, horizon_scans, roi_range, d_out, d_meta + 64, d_meta + 128, d_meta);
+  RigLayout L{};
+  L.n_lidars = 1, L.off[1] = n;
+  int rc = project_cloud_device(c, c->sweep_in.as<float4>(), L, vertical_scans, horizon_scans, roi_range, nullptr, d_out, d_meta + 64,
+                                d_meta + 128, d_meta, c->front_work);
   if (rc) return rc;
   int *hc = c->pinned->counts;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_meta, sizeof(int) * 192, cudaMemcpyDeviceToHost, st));
@@ -802,43 +909,146 @@ int mloam_frame(mloam_ctx_t *h, const mloam_point_t *h_cloud, int n, const int *
                 const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
   if (!h || !pose_init7 || !pose_out7 || n <= 0 || !h_cloud || !h_scan_start || !h_scan_end || n_scans <= 0 || n_scans > MLOAM_MAX_RINGS)
     return MLOAM_E_INVALID;
+  return frame_host(&h->c, h_cloud, n, h_scan_start, h_scan_end, n_scans, h_surf_map, n_surf_map, h_corner_map, n_corner_map, rebuild_maps,
+                    pose_init7, pose_out7, stats);
+}
+
+// ------------------------------------------------------------------------------------------ raw driver sweeps
+// removeNaNFromPointCloud (rosNodeRVKITTI.cpp:154-161, rosNodeRVOxford.cpp:170-177) + FeatureExtract::calTimestamp (feature_extract.cpp:25-114)
+int mloam_cal_timestamp(mloam_ctx_t *h, const mloam_point_t *h_cloud, int n, int time_field, float scan_period, mloam_point_t *h_out,
+                        int *n_out) {
+  if (!h || n < 0 || !n_out || (n > 0 && (!h_cloud || !h_out))) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
   cudaSetDevice(c->device);
+  *n_out = 0;
+  if (n == 0) return MLOAM_OK;
+  MLOAM_CUDA_OK(c, c->sweep_in.reserve(sizeof(float4) * (size_t)n));
+  float4 *d_out;
+  int *d_cnt;
+  MLOAM_CUDA_OK(c, carve(c->map_in[0], [&](Carve &cv) { d_out = cv.take<float4>(n), d_cnt = cv.take<int>(16); }));
   cudaStream_t st = c->stream;
-  SweepIn D;
-  int rc = sweep_bufs(c, c->sweep_in, n, n_scans, &D);
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->sweep_in.p, h_cloud, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, st));
+  RigLayout L{};
+  L.n_lidars = 1, L.off[1] = n;
+  int rc = front_times_device(c, c->sweep_in.as<float4>(), L, time_field ? 1 : 0, scan_period, d_out, d_cnt, c->front_work);
   if (rc) return rc;
-  // the sweep was announced with the previous frame and its features are ready (look-ahead): nothing to copy
-  const bool have = c->prefetched.host && frame_has_prefetched(c, h_cloud, n, n_scans);
-  if (!have) {
-    int(*pin)[MLOAM_MAX_RINGS] = c->pinned->scan_info;
-    std::memcpy(pin[0], h_scan_start, sizeof(int) * n_scans), std::memcpy(pin[1], h_scan_end, sizeof(int) * n_scans);
-    MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.scan_start, pin[0], sizeof(int) * n_scans, cudaMemcpyHostToDevice, st));
-    MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.scan_end, pin[1], sizeof(int) * n_scans, cudaMemcpyHostToDevice, st));
-    MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.cloud, h_cloud, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, st));
-  }
+  int *hc = c->pinned->counts;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  *n_out = hc[0];
+  if (hc[0] > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_out, d_out, sizeof(float4) * (size_t)hc[0], cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  return MLOAM_OK;
+}
+
+int mloam_set_front_end(mloam_ctx_t *h, int vertical_scans, int horizon_scans, double roi_range, float scan_period, int time_field) {
+  if (!h) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (vertical_scans != 16 && vertical_scans != 32 && vertical_scans != 64)
+    return fail(c, MLOAM_E_INVALID, "set_front_end: vertical_scans must be 16, 32 or 64 (ImageSegmenter::setParameter)");
+  if (horizon_scans <= 0 || !(scan_period > 0.f)) return fail(c, MLOAM_E_INVALID, "set_front_end: horizon_scans and scan_period must be positive");
+  if (c->params.max_ring_points > 0 && c->params.max_ring_points < horizon_scans)
+    return fail(c, MLOAM_E_INVALID, "set_front_end: params.max_ring_points is below horizon_scans (a projected ring holds up to horizon_scans points)");
+  c->front = FrontEnd{vertical_scans, horizon_scans, roi_range, scan_period, time_field ? 1 : 0};
+  c->front_set = true;
+  c->prefetched.valid = false;  // look-ahead features were made with the previous front end
+  return MLOAM_OK;
+}
+
+int mloam_front_end(mloam_ctx_t *h, const mloam_point_t *h_raw, const int *h_counts, mloam_point_t *h_out, int *n_out, int *h_scan_start,
+                    int *h_scan_end) {
+  if (!h || !h_raw || !h_out || !n_out || !h_scan_start || !h_scan_end) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  *n_out = 0;
+  RigLayout L;
+  int n_scans = 0;
+  int rc = raw_layout(c, h_counts, &L, &n_scans);
+  if (rc) return rc;
+  cudaSetDevice(c->device);
+  const int n = L.off[L.n_lidars];
+  c->prefetched.valid = false;  // the front end's output buffer is the frame's
+  MLOAM_CUDA_OK(c, c->sweep_in.reserve(sizeof(float4) * (size_t)n));
+  float4 *d_out;
+  int *d_meta;  // [0] count, then scan starts, scan ends
+  MLOAM_CUDA_OK(c, carve(c->front_out, [&](Carve &cv) { d_out = cv.take<float4>((size_t)n + 1), d_meta = cv.take<int>(4 + 2 * (size_t)n_scans); }));
+  cudaStream_t st = c->stream;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->sweep_in.p, h_raw, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, st));
+  const FrontEnd &fe = c->front;
+  rc = project_cloud_device(c, c->sweep_in.as<float4>(), L, fe.vertical_scans, fe.horizon_scans, fe.roi_range, &fe, d_out, d_meta + 4,
+                            d_meta + 4 + n_scans, d_meta, c->front_work);
+  if (rc) return rc;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_start, d_meta + 4, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_end, d_meta + 4 + n_scans, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
+  int *hc = c->pinned->counts;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_meta, sizeof(int), cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  *n_out = hc[0];
+  if (hc[0] > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_out, d_out, sizeof(float4) * (size_t)hc[0], cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  return MLOAM_OK;
+}
+
+int mloam_frame_raw(mloam_ctx_t *h, const mloam_point_t *h_raw, const int *h_counts, const mloam_point_t *h_surf_map, int n_surf_map,
+                    const mloam_point_t *h_corner_map, int n_corner_map, int rebuild_maps, const double *pose_init7, double *pose_out7,
+                    mloam_solve_stats_t *stats) {
+  if (!h || !pose_init7 || !pose_out7 || !h_raw) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  RigLayout L;
+  int n_scans = 0;
+  int rc = raw_layout(c, h_counts, &L, &n_scans);
+  if (rc) return rc;
+  RawScope raw(c, &L);
+  return frame_host(c, h_raw, L.off[L.n_lidars], nullptr, nullptr, n_scans, h_surf_map, n_surf_map, h_corner_map, n_corner_map, rebuild_maps,
+                    pose_init7, pose_out7, stats);
+}
+
+int mloam_frame_raw_device(mloam_ctx_t *h, const mloam_point_t *d_raw, const int *h_counts, const mloam_point_t *d_surf_map, int n_surf_map,
+                           const mloam_point_t *d_corner_map, int n_corner_map, int rebuild_maps, const double *pose_init7, double *pose_out7,
+                           mloam_solve_stats_t *stats) {
+  if (!h || !pose_init7 || !pose_out7 || !d_raw) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  RigLayout L;
+  int n_scans = 0;
+  int rc = raw_layout(c, h_counts, &L, &n_scans);
+  if (rc) return rc;
+  cudaSetDevice(c->device);
+  RawScope raw(c, &L);
   rc = stage_next_sweep(c);
   if (rc) return rc;
-  const float4 *d_sm = nullptr, *d_cm = nullptr;
-  if (rebuild_maps) {
-    if (!h_surf_map || !h_corner_map || n_surf_map < 0 || n_corner_map < 0) return MLOAM_E_INVALID;
-    DevBuf &ms = c->map_in[0], &mc = c->map_in[1];
-    MLOAM_CUDA_OK(c, ms.reserve(sizeof(float4) * (size_t)(n_surf_map + 1)));
-    MLOAM_CUDA_OK(c, mc.reserve(sizeof(float4) * (size_t)(n_corner_map + 1)));
-    // The submaps (16 B/point, ~8x the sweep) go up on the side stream so that the copy overlaps extraction and scan
-    // down-sampling of the sweep; the map-build branch of frame_enqueue is ordered after ev_maps.
-    MLOAM_CUDA_OK(c, cudaMemcpyAsync(ms.p, h_surf_map, sizeof(float4) * (size_t)n_surf_map, cudaMemcpyHostToDevice, c->stream2));
-    MLOAM_CUDA_OK(c, cudaMemcpyAsync(mc.p, h_corner_map, sizeof(float4) * (size_t)n_corner_map, cudaMemcpyHostToDevice, c->stream2));
-    MLOAM_CUDA_OK(c, cudaEventRecord(c->ev_maps, c->stream2));
-    c->maps_pending = true;
-    d_sm = ms.as<float4>(), d_cm = mc.as<float4>();
-  }
-  c->cloud_key = h_cloud;
-  rc = frame_run(c, D.cloud, n, D.scan_start, D.scan_end, n_scans, d_sm, n_surf_map, d_cm, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
-  c->cloud_key = nullptr;
-  c->maps_pending = false, c->next_pending = false, c->next.set = false;
+  rc = frame_run(c, reinterpret_cast<const float4 *>(d_raw), L.off[L.n_lidars], nullptr, nullptr, n_scans,
+                 reinterpret_cast<const float4 *>(d_surf_map), n_surf_map, reinterpret_cast<const float4 *>(d_corner_map), n_corner_map,
+                 rebuild_maps, pose_init7, pose_out7, stats);
+  c->next_pending = false, c->next.set = false;
   if (rc == MLOAM_OK) memcpy(c->last_pose7, pose_out7, sizeof(c->last_pose7)), c->frame_since_save = true;  // mloam_keyframe_save
   return rc;
+}
+
+// Look-ahead for raw frames: as mloam_frame_set_next*, picked up by the next mloam_frame_raw* call with the same pointer and counts
+int mloam_frame_set_next_raw(mloam_ctx_t *h, const mloam_point_t *h_raw, const int *h_counts) {
+  if (!h) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  c->next = Ctx::NextSweep{};
+  if (!h_raw) return MLOAM_OK;  // withdraw
+  RigLayout L;
+  int n_scans = 0;
+  const int rc = raw_layout(c, h_counts, &L, &n_scans);
+  if (rc) return rc;
+  c->next.set = true, c->next.host = true, c->next.key_ptr = h_raw, c->next.n = L.off[L.n_lidars], c->next.n_scans = n_scans;
+  c->next.raw = true, c->next.L = L;
+  return MLOAM_OK;
+}
+int mloam_frame_set_next_raw_device(mloam_ctx_t *h, const mloam_point_t *d_raw, const int *h_counts) {
+  if (!h) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  c->next = Ctx::NextSweep{};
+  if (!d_raw) return MLOAM_OK;  // withdraw
+  RigLayout L;
+  int n_scans = 0;
+  const int rc = raw_layout(c, h_counts, &L, &n_scans);
+  if (rc) return rc;
+  c->next.set = true, c->next.host = false, c->next.key_ptr = d_raw, c->next.d_cloud = reinterpret_cast<const float4 *>(d_raw);
+  c->next.n = L.off[L.n_lidars], c->next.n_scans = n_scans, c->next.raw = true, c->next.L = L;
+  return MLOAM_OK;
 }
 
 int mloam_set_lidars(mloam_ctx_t *h, int n_lidars, const double *ext7) {

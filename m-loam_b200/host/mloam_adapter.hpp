@@ -85,6 +85,7 @@ class KdTreeFLANN {
 // range image, first point of a pixel wins, intensity += ring, ring-ordered output, ScanInfo) runs on the GPU; the BFS labelling of
 // `segment_cloud: 1` (image_segmenter.hpp:160-360) is not provided and throws.
 extern double ROI_RANGE;  // parameters.h:86
+extern float SCAN_PERIOD;  // parameters.h:78
 class ImageSegmenter {
  public:
   ImageSegmenter() {}
@@ -139,6 +140,30 @@ class FeatureExtract {
     mloam::unpackCloud(b2.data(), f.n_flat, cloud_feature["surf_points_flat"]);
     mloam::unpackCloud(b3.data(), f.n_less_flat, cloud_feature["surf_points_less_flat"]);
   }
+  void calTimestampPacked(const std::vector<mloam_point_t> &in, int time_field, common::PointICloud &laser_cloud_out) {
+    mloam_ctx_t *ctx = mloam::ThreadContext::get();
+    std::vector<mloam_point_t> out(in.size() + 1);
+    int n_out = 0;
+    mloam::check(ctx, mloam_cal_timestamp(ctx, in.data(), (int)in.size(), time_field, SCAN_PERIOD, out.data(), &n_out), "mloam_cal_timestamp");
+    mloam::unpackCloud(out.data(), n_out, laser_cloud_out);
+  }
+
+#ifdef POINTWITHTIME_HPP
+  // calTimestamp (feature_extract.hpp:68-72, feature_extract.cpp:38-114) on the GPU, provided where mloam_pcl/point_with_time.hpp is included
+  // first (as feature_extract.hpp:42 does).  The reference gets clouds the driver node already passed through removeNaNFromPointCloud;
+  // here a point with a non-finite x, y or z is dropped, so both orders give the same cloud.  SCAN_PERIOD: parameters.h:78.
+  void calTimestamp(const common::PointCloud &laser_cloud_in, common::PointICloud &laser_cloud_out) {
+    std::vector<mloam_point_t> in(laser_cloud_in.size());
+    for (size_t i = 0; i < in.size(); i++) in[i] = mloam_point_t{laser_cloud_in.points[i].x, laser_cloud_in.points[i].y, laser_cloud_in.points[i].z, 0.f};
+    calTimestampPacked(in, 0, laser_cloud_out);
+  }
+  void calTimestamp(const common::PointITimeCloud &laser_cloud_in, common::PointICloud &laser_cloud_out) {
+    std::vector<mloam_point_t> in(laser_cloud_in.size());  // PointXYZIWithTime::timestamp [us] rides in the w lane
+    for (size_t i = 0; i < in.size(); i++)
+      in[i] = mloam_point_t{laser_cloud_in.points[i].x, laser_cloud_in.points[i].y, laser_cloud_in.points[i].z, laser_cloud_in.points[i].timestamp};
+    calTimestampPacked(in, 1, laser_cloud_out);
+  }
+#endif
 
   template <typename PointType>
   void matchCornerFromScan(const typename mloam::KdTreeFLANN<PointType>::Ptr &kdtree_corner_from_scan, const typename pcl::PointCloud<PointType> &cloud_scan,
