@@ -95,20 +95,13 @@ int mloam_ctx_create(int device, const mloam_params_t *params, mloam_ctx_t **out
   c->sm_count = prop.multiProcessorCount;
   if (params) c->params = *params;
   else mloam_default_params(&c->params);
-  if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming) != cudaSuccess ||
+  bool branches_ok = true;
+  for (Branch *b : {&c->br_maps, &c->br_scan, &c->br_ahead, &c->br_ahead_scan})
+    branches_ok = branches_ok && cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking) == cudaSuccess &&
+                  cudaEventCreateWithFlags(&b->fork, cudaEventDisableTiming) == cudaSuccess &&
+                  cudaEventCreateWithFlags(&b->join, cudaEventDisableTiming) == cudaSuccess;
+  if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess || !branches_ok ||
       cudaEventCreateWithFlags(&c->ev_maps, cudaEventDisableTiming) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&c->stream3, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreateWithFlags(&c->ev_fork3, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&c->ev_join3, cudaEventDisableTiming) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&c->stream4, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&c->stream5, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreateWithFlags(&c->ev_fork4, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&c->ev_join4, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&c->ev_fork5, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&c->ev_join5, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&c->ev_next, cudaEventDisableTiming) != cudaSuccess ||
       cudaMallocHost(reinterpret_cast<void **>(&c->pinned), sizeof(PinnedBlock)) != cudaSuccess ||
       c->lm_state.reserve(sizeof(LMState) + 64) != cudaSuccess || c->ctl.reserve(sizeof(DevCtl)) != cudaSuccess) {
@@ -157,16 +150,12 @@ void mloam_ctx_destroy(mloam_ctx_t *h) {
   c->frame_main.release(), c->frame_alt.release(), c->next_in.release(), c->stamps.release(), c->ua_scan.release(), c->pose_cov.release();
   if (c->pinned) cudaFreeHost(c->pinned);
   if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
-  if (c->stream2) cudaStreamSynchronize(c->stream2), cudaStreamDestroy(c->stream2);
-  if (c->ev_fork) cudaEventDestroy(c->ev_fork);
-  if (c->ev_join) cudaEventDestroy(c->ev_join);
-  if (c->ev_maps) cudaEventDestroy(c->ev_maps);
-  if (c->stream3) cudaStreamSynchronize(c->stream3), cudaStreamDestroy(c->stream3);
-  if (c->ev_fork3) cudaEventDestroy(c->ev_fork3);
-  if (c->ev_join3) cudaEventDestroy(c->ev_join3);
-  if (c->stream4) cudaStreamSynchronize(c->stream4), cudaStreamDestroy(c->stream4);
-  if (c->stream5) cudaStreamSynchronize(c->stream5), cudaStreamDestroy(c->stream5);
-  for (cudaEvent_t ev : {c->ev_fork4, c->ev_join4, c->ev_fork5, c->ev_join5, c->ev_next})
+  for (Branch *b : {&c->br_maps, &c->br_scan, &c->br_ahead, &c->br_ahead_scan}) {
+    if (b->stream) cudaStreamSynchronize(b->stream), cudaStreamDestroy(b->stream);
+    for (cudaEvent_t ev : {b->fork, b->join})
+      if (ev) cudaEventDestroy(ev);
+  }
+  for (cudaEvent_t ev : {c->ev_maps, c->ev_next})
     if (ev) cudaEventDestroy(ev);
   delete h;
 }
@@ -428,7 +417,7 @@ int mloam_normal_equations(mloam_ctx_t *h, int n, const unsigned char *h_types, 
   int rc = upload_pose(c, pose7, &d_pose);
   if (rc) return rc;
   double *d_ne = c->ctl.as<DevCtl>()->normal_eq;
-  rc = linearize_device(c, sets, 2, sqrt_info, huber_a, d_pose, 0, 0, d_ne);
+  rc = linearize_device(c, sets, 2, sqrt_info, huber_a, d_pose, 0, 0, d_ne, LinOpts{c->params.eig_thre});
   if (rc) return rc;
   double *ne = c->pinned->normal_eq;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(ne, d_ne, sizeof(double) * 30, cudaMemcpyDeviceToHost, c->stream));

@@ -49,6 +49,16 @@ struct PendingFit {
   float min_plane_dis = 0.f;
   int check_fov = 0;
 };
+// Settings of one linearize_device call
+struct LinOpts {
+  double eig_thre;                  // evalDegenracy threshold (params.eig_thre; the tracker disables it with 0)
+  int want_eig = 1;                 // k_lm mode 1: always run the 6x6 eigen-solver (1) or only when degenerate (0)
+  bool collective = false;          // the collective solve (scan2map on every rank in lock-step): sum over the ranks
+  bool two_pass = false;            // both evaluations of the LM iteration in one launch, if the launch can (lm_mode 1, fused tail)
+  SpecState *spec = nullptr;        // speculative schedule (lm_mode 1): commit the speculation ...
+  bool spec_publish = false;        // ... and publish the new candidate for the next matcher
+  const PendingFit *fit = nullptr;  // the fit the matcher deferred to this evaluation (lm_mode 1)
+};
 
 // Grow-only device buffer (cudaMalloc only when capacity is exceeded; steady-state frames allocate nothing).
 struct DevBuf {
@@ -106,6 +116,18 @@ struct FrontEnd {
 };
 static_assert(sizeof(FrontEnd) == 24 && sizeof(RigLayout) == 4 * (MLOAM_MAX_LIDARS + 2), "hashed whole: no padding");
 
+// One sweep of a frame (mloam_frame*) or announced for the next one (mloam_frame_set_next*)
+struct Sweep {
+  const void *key = nullptr;             // the caller's cloud pointer (host or device): the look-ahead matches on it
+  const float4 *cloud = nullptr;         // the sweep on the device (a host sweep: where its copy goes)
+  const int *scan_start = nullptr, *scan_end = nullptr;      // its ScanInfo on the device; none for a raw sweep (the front end makes it)
+  const int *h_scan_start = nullptr, *h_scan_end = nullptr;  // a host sweep's ScanInfo in host memory
+  int n = 0, n_scans = 0;
+  bool host = false;                     // key is a host pointer
+  bool raw = false;                      // the rig's raw sweeps with layout L: the front end runs before extraction
+  RigLayout L{};
+};
+
 // the per-point association with uncertainty (uct.h): per LiDAR of the rig, and per run
 struct UctLaser {
   double ext_inv[7];   // pose_ext[n].inverse()
@@ -148,7 +170,7 @@ struct PinnedBlock {
   double normal_eq[30];             // mloam_normal_equations read-back
   double pose_plus[64];             // mloam_pose_plus: x | delta | V in, result at [56]
   int scan_info[2][MLOAM_MAX_RINGS];       // mloam_frame: ScanInfo of the sweep (start | end)
-  int scan_info_next[2][MLOAM_MAX_RINGS];  // ... and of the announced next sweep, copied on stream4
+  int scan_info_next[2][MLOAM_MAX_RINGS];  // ... and of the announced next sweep, copied on Ctx::br_ahead
 };
 
 // Matcher counters of k_match_knn with stage profiling on (mloam_profile_get "knn_*"); zeroed at creation and by mloam_profile_reset
@@ -229,16 +251,21 @@ struct MatchCfg {
 
 struct KeyframeStore;
 
+// A side stream with the events of its fork from and its join into Ctx::stream (pipeline.cu on_branch)
+struct Branch {
+  cudaStream_t stream = nullptr;
+  cudaEvent_t fork = nullptr, join = nullptr;
+};
+
 struct Ctx {
   int device = 0;
   int sm_count = 132;
   cudaStream_t stream = nullptr;
   bool own_stream = true;
-  cudaStream_t stream2 = nullptr;        // side stream: submap upload + build run concurrently with extraction
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  cudaStream_t stream3 = nullptr;        // side stream: corner-scan voxel filter next to the surf-scan one
-  cudaEvent_t ev_fork3 = nullptr, ev_join3 = nullptr;
-  cudaEvent_t ev_maps = nullptr;         // recorded on stream2 after the host API's submap H2D copies
+  Branch br_maps;                        // submap upload + build, concurrently with extraction
+  Branch br_scan;                        // corner-scan voxel filter next to the surf-scan one; corner good-feature selection; speculative matcher
+  Branch br_ahead, br_ahead_scan;        // look-ahead extraction and its corner-voxel fork
+  cudaEvent_t ev_maps = nullptr;         // recorded on br_maps after the host API's submap H2D copies
   bool maps_pending = false;             // the map-build branch must wait on ev_maps (external to a captured graph)
   mloam_params_t params;
   std::string err;
@@ -265,7 +292,7 @@ struct Ctx {
   void *ticket_zeroed_for = nullptr;  // partials allocation whose last-block ticket has been zeroed
   // Work buffers, named by their role in a frame.  The host-buffer entry points, each one synchronous call, stage through them too.
   DevBuf sweep_in;                // mloam_frame: the sweep + its ScanInfo.  Host entry points: their input
-  DevBuf map_in[2];               // mloam_frame: the surf / corner submap uploads on stream2.  Host entry points: [0] their output
+  DevBuf map_in[2];               // mloam_frame: the surf / corner submap uploads on br_maps.  Host entry points: [0] their output
   DevBuf extract_work;            // extract_device (extract_work_layout); the look-ahead branch reuses it after the current extraction
   DevBuf voxel_work;              // voxel filters of the host entry points and of the keyframe submap
   DevBuf voxel_corner, voxel_surf;  // the frame's two scan filters, on two streams at once; the look-ahead branch forks after them
@@ -307,40 +334,28 @@ struct Ctx {
   // (estimator -> lidar_mapper), so they overlap there too.  `Features` describes one half.
   struct Features {
     bool valid = false;
-    bool host = false;          // key_ptr is a host pointer (mloam_frame) / a device pointer (mloam_frame_device)
-    const void *key_ptr = nullptr;
-    int n = 0, n_scans = 0, parity = 0;
-    bool raw = false;           // features of a raw sweep (mloam_frame_raw*) with this layout
-    RigLayout L{};
+    int parity = 0;
+    Sweep sw;                   // the sweep they were extracted from
     ScanRef S{};
   };
   struct NextSweep {
-    bool set = false, host = false;
-    const void *key_ptr = nullptr;      // what the caller will pass as the cloud of the next frame
-    const float4 *d_cloud = nullptr;    // where the sweep is (or will be, after the pending H2D) on the device
-    const int *d_scan_start = nullptr, *d_scan_end = nullptr;
-    int n = 0, n_scans = 0;
-    bool raw = false;                   // a raw sweep (mloam_frame_set_next_raw*): the front end runs before extraction
-    RigLayout L{};
+    bool set = false;
+    Sweep sw;                   // a host sweep's device buffers are set when its copy is enqueued (pipeline.cu stage_next_sweep)
   };
   // raw frames (mloam_set_front_end, mloam_frame_raw*): the front end runs inside features_enqueue, on the main stream and in the look-ahead
   // branch.  Its work (winner images, sort) and output (projected cloud + ScanInfo) have buffers of their own: the look-ahead reuses them
   // after the main stream's front end, while the main stream runs the with_ua stage and the solve.
   FrontEnd front{};
   bool front_set = false;
-  const RigLayout *raw_now = nullptr;  // the raw sweep of the frame being enqueued (nullptr: a ring-ordered sweep)
   DevBuf front_work, front_out;
   Features prefetched;             // features of the sweep announced with the previous frame, ready when that frame returned
   NextSweep next;                  // announced for the frame being enqueued (consumed by it)
-  const void *cloud_key = nullptr; // mloam_frame: the HOST pointer of the sweep being processed (look-ahead matches on it)
-  const int *next_host_ss = nullptr, *next_host_se = nullptr;  // ScanInfo of a sweep announced from host memory
-  bool next_pending = false;       // its H2D copy was enqueued on stream4 outside of any capture (ev_next)
+  bool next_pending = false;       // its H2D copy was enqueued on br_ahead outside of any capture (ev_next)
   int frame_parity = 0;
   int use_lookahead = 1;           // MLOAM_LOOKAHEAD=0: announcements are ignored
   bool stamp_mute = false;
   DevBuf frame_main, frame_alt, next_in;  // the two halves of the frame feature double buffer; the announced sweep's staging
-  cudaStream_t stream4 = nullptr, stream5 = nullptr;  // look-ahead extraction and its corner-voxel fork
-  cudaEvent_t ev_fork4 = nullptr, ev_join4 = nullptr, ev_fork5 = nullptr, ev_join5 = nullptr, ev_next = nullptr;
+  cudaEvent_t ev_next = nullptr;
   struct GraphEntry {
     unsigned long long key = 0, epoch = 0;
     cudaGraphExec_t exec = nullptr;
@@ -364,16 +379,8 @@ struct Ctx {
   std::vector<std::string> stamp_labels;
   int knn_min_blocks = 2;          // k_match_knn variant: resident CTAs per SM it is compiled for (MLOAM_KNN_MB = 2 | 3 | 4); 2 is fastest on the H100
   int use_seeds = 1;               // seed the kNN of re-association iterations > 0 with the previous neighbour lists
-  int s2m_ran = 0;
-  int lm_min_corr = 0;              // lm_init_state: minimum matched features for a Solve (tracker: 10)
-  double lm_eig_thre = -1.0;        // < 0: use params.eig_thre; the tracker disables evalDegenracy with 0
   int fuse_iter = 1;               // scan2map: fit inside the first evaluation + both evaluations of an LM iteration in ONE launch
                                    // (grid barrier between them); MLOAM_FUSE_ITER=0 restores the three launches
-  PendingFit pending_fit;          // set by match_pair_device(defer_fit), consumed by the next linearize_device(lm_mode 1)
-  bool lin_two_pass = false;       // request (scan2map_enqueue) -> linearize_device clears it when it could not honour it
-  SpecState *lin_spec = nullptr;   // scan2map_enqueue -> the next linearize_device(lm_mode 1): commit the speculation (SpecState) ...
-  bool lin_spec_publish = false;   // ... and publish the new candidate for the next matcher
-  int want_eig = 1;                // k_lm mode 1: always run the 6x6 eigen-solver (1) or only when degenerate (0)
   bool lidar_merge = false;        // mloam_set_lidars was given extrinsics: features go through the rig merge (also for one LiDAR)
   int n_lidars = 1;                // LiDARs batched into one frame of this context (mloam_set_lidars)
   double lidar_ext[MLOAM_MAX_LIDARS][7];  // their sensor -> base extrinsics
@@ -388,7 +395,6 @@ struct Ctx {
   void *p2p_peer[MLOAM_P2P_MAX_RANKS] = {nullptr};
   void *p2p_view = nullptr;        // device copy of the P2PView the kernels read
   bool p2p_on = false;
-  bool p2p_collective = false;     // the solve being enqueued is the collective one (all ranks in lock-step): sum over the ranks
   // uncertainty-aware mapping in the frame path (mloam_set_uncertainty): the per-point uncertainty + trace gate of
   // downsampleCurrentScan (lidar_mapper_keyframe.cpp:356-421) between the scan filters and the solve, and the pose covariance
   // H^-1 at the returned pose (:600-610).  The covariances reach the device through the pinned block (PinnedBlock::ua), so a
@@ -399,7 +405,6 @@ struct Ctx {
   double ua_trace_threshold = 0.0;          // TRACE_THRESHOLD_MAPPING
   DevBuf ua_scan;                  // gated scans of the last with_ua frame (points, cov6, sqrt_info, counts) + its staged configuration
   DevBuf pose_cov;                 // 36 doubles: H^-1 of the last solve (k_pose_cov), copied back with LMState
-  bool s2m_cov = false;            // the solve being enqueued reports H^-1 (with_ua frame, mloam_scan2map_ua)
   double pose_cov36[36] = {0};     // pose_wmap_curr.cov_ of the last mloam_frame* / mloam_scan2map* call
   bool last_scan_valid = false;    // last_scan describes the scan of the last mloam_frame* call (mloam_frame_scan)
   ScanRef last_scan{};
@@ -436,7 +441,7 @@ int knn_device(Ctx *c, int slot, const float4 *d_q, int nq, const double *d_pose
 // type 'c' / 's'.  d_pose7 device pointer to 7 doubles.  Outputs: valid[n], coeff[n*6] float, nn[n*n_neigh] (nullable)
 // d_n (nullable): device-side feature count, n is then the launch upper bound.
 int match_from_map_device(Ctx *c, int slot, int type, const float4 *d_pts, int n, const int *d_n, const double *d_pose7,
-                          const MatchCfg &cfg, unsigned char *d_valid, float *d_coeff, int *d_nn, int *d_work = nullptr);
+                          const MatchCfg &cfg, unsigned char *d_valid, float *d_coeff, int *d_nn);
 
 // match_kernels.cu: one kNN launch + one fit launch over up to two feature sets
 struct MatchJob {
@@ -452,10 +457,11 @@ struct MatchJob {
                             // lists (Ctx::knn_pos) seed the search and unchanged lists keep their fit
 };
 // buf_base: which pair of the context's per-set buffers (knn_pos / knn_anchor / ...) the jobs use: 0 (sets 0, 1) or 2 (sets 2, 3)
-// defer_fit: skip the fit launch and leave the fit to the next linearize_device(lm_mode 1) on this context (Ctx::pending_fit)
-// d_sel (speculative schedule, with defer_fit): double-buffered lists, read half *d_sel and write the other (SpecState::sel)
-int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_pose7, const MatchCfg &cfg, int *d_work, int buf_base = 0,
-                      bool defer_fit = false, const int *d_sel = nullptr);
+// defer (nullable): skip the fit launch and write the fit into *defer for the caller's next linearize_device(lm_mode 1) (LinOpts::fit);
+// defer->K == 0 when the fit was launched here (a job wants neighbour indices) or nothing was matched.  nullptr: fit now.
+// d_sel (speculative schedule, with defer): double-buffered lists, read half *d_sel and write the other (SpecState::sel)
+int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_pose7, const MatchCfg &cfg, int buf_base = 0,
+                      PendingFit *defer = nullptr, const int *d_sel = nullptr);
 
 // track_kernels.cu
 int match_from_scan_device(Ctx *c, int slot, int type, const float4 *d_pts, int n, const double *d_pose7, unsigned char *d_valid,
@@ -478,14 +484,15 @@ struct FeatSet {
 // Accumulate loss-corrected normal equations of both feature sets at pose *d_pose7 (or LMState x / xc when
 // use_state != 0: 1 -> x, 2 -> xc) into c->partials, then run the LM state machine step (`lm_mode`):
 //   0: none (partials only, reduced into d_out28 if non-null)   1: begin Solve   2: iterate
+// two_pass_done (nullable): whether the launch ran both evaluations of the LM iteration (LinOpts::two_pass honoured)
 int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, const double *d_pose7,
-                     int use_state, int lm_mode, double *d_out29);
+                     int use_state, int lm_mode, double *d_out29, const LinOpts &o, bool *two_pass_done = nullptr);
 // Evaluation at LMState::xc + the acceptance step (mode 2) of a solve with max_inner == 1, as the second pass of
 // k_linearize computes it, but accumulating only g, cost and row counts (H at xc is never read with one LM iteration).
 // Small blocks with a register cap, so that it runs beside the speculative matcher of the next GN iteration.
-int eval_candidate_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a);
-// spec (nullable): also start SpecState::xc at the initial pose
-int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, double eig_thre, SpecState *spec = nullptr);
+int eval_candidate_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, double eig_thre);
+// min_corr: minimum matched features for a Solve (tracker: 10); spec (nullable): also start SpecState::xc at the initial pose
+int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, int min_corr, SpecState *spec = nullptr);
 void eig_report_host(const double *H36, double *w6);  // ascending eigenvalues of a symmetric 6x6 (host side)
 int factor_evaluate_device(Ctx *c, int kind, int n, const double *d_points, const double *d_coeffs, const double *d_sqrt_info,
                            const double *d_params, double *d_res, double *d_jac);

@@ -802,13 +802,12 @@ __global__ void k_lm_init(LMState *st, const double *pose7, int max_inner, int m
   }
 }
 
-int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, double eig_thre, SpecState *spec) {
-  (void)eig_thre;
+int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, int min_corr, SpecState *spec) {
   MLOAM_CUDA_OK(c, c->lm_state.reserve(sizeof(LMState) + 64));
   stage_pose(c, pose7_host);
   double *d_stage = c->ctl.as<DevCtl>()->pose;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_stage, c->pinned->pose, 7 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  k_lm_init<<<1, 32, 0, c->stream>>>(c->lm_state.as<LMState>(), d_stage, max_inner, c->lm_min_corr, spec);
+  k_lm_init<<<1, 32, 0, c->stream>>>(c->lm_state.as<LMState>(), d_stage, max_inner, min_corr, spec);
   c->launches++;
   MLOAM_CUDA_OK(c, cudaGetLastError());
   return MLOAM_OK;
@@ -876,7 +875,8 @@ int pose_cov_device(Ctx *c) {
 // What k_linearize and k_eval_candidate share: the feature sets, the grid (k_eval_candidate runs LIN_THREADS / CAND_THREADS
 // blocks per k_linearize block) and c->partials = [NE_PACK doubles per k_linearize block, max_nb + 2 of them][ticket +
 // generation word][NE_CAND doubles per k_eval_candidate warp].
-static int lin_setup(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, LinArgs &a, int *nb_out, double **wsums) {
+static int lin_setup(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, double eig_thre, LinArgs &a, int *nb_out,
+                     double **wsums) {
   memset(&a, 0, sizeof(a));
   int n_total = 0;
   for (int s = 0; s < 2; s++) {
@@ -893,7 +893,7 @@ static int lin_setup(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, 
   a.n_sets = n_sets, a.sqrt_info = sqrt_info, a.huber_a = huber_a;
   a.state = c->lm_state.as<LMState>();
   a.state_rw = c->lm_state.as<LMState>();
-  a.eig_thre = c->lm_eig_thre >= 0.0 ? c->lm_eig_thre : c->params.eig_thre;
+  a.eig_thre = eig_thre;
   int nb = (n_total + LIN_THREADS - 1) / LIN_THREADS;
   if (nb < 1) nb = 1;
   // n_total is a launch upper bound (device-side counts are usually far smaller): 64 blocks x 256 threads cover a
@@ -914,44 +914,41 @@ static int lin_setup(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, 
 }
 
 int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, const double *d_pose7,
-                     int use_state, int lm_mode, double *d_out30) {
+                     int use_state, int lm_mode, double *d_out30, const LinOpts &o, bool *two_pass_done) {
   LinArgs a;
   int nb = 0;
   double *wsums = nullptr;
-  int rc = lin_setup(c, sets, n_sets, sqrt_info, huber_a, a, &nb, &wsums);
+  int rc = lin_setup(c, sets, n_sets, sqrt_info, huber_a, o.eig_thre, a, &nb, &wsums);
   if (rc) return rc;
   const int max_nb = c->sm_count;
-  const int want_eig = c->want_eig;
   a.pose = d_pose7;
   a.use_state = use_state;
   a.respect_done = (lm_mode == 2) ? 1 : 0;
-  const bool collective = c->nccl_comm && c->p2p_collective;  // sum over the ranks wanted for this solve
+  const bool collective = c->nccl_comm && o.collective;  // sum over the ranks wanted for this solve
   const bool fused = lm_mode != 0 && (!collective || c->p2p_on) && !d_out30;
   // only the collective solves (scan2map on every rank in lock-step) exchange; per-rank solves on the same context — the tracker,
-  // mloam_normal_equations — stay local (c->p2p_collective is raised by scan2map_enqueue alone)
-  a.p2p = (fused && c->p2p_on && c->p2p_collective) ? static_cast<const P2PView *>(c->p2p_view) : nullptr;
-  a.lm_mode = fused ? lm_mode : 0, a.want_eig = want_eig;
+  // mloam_normal_equations — stay local
+  a.p2p = (fused && c->p2p_on && o.collective) ? static_cast<const P2PView *>(c->p2p_view) : nullptr;
+  a.lm_mode = fused ? lm_mode : 0, a.want_eig = o.want_eig;
   // both evaluations of an LM iteration in one launch: only with the fused tail (the barrier is released by the block that ran it)
-  a.two_pass = (c->lin_two_pass && fused && lm_mode == 1) ? 1 : 0;
-  c->lin_two_pass = a.two_pass != 0;
+  a.two_pass = (o.two_pass && fused && lm_mode == 1) ? 1 : 0;
+  if (two_pass_done) *two_pass_done = a.two_pass != 0;
   // the speculative schedule's commit rides in the fused tail of the evaluation at x
-  if (c->lin_spec && !(fused && lm_mode == 1 && !a.p2p)) {
+  if (o.spec && !(fused && lm_mode == 1 && !a.p2p)) {
     c->err = "linearize: the speculative schedule needs the fused single-GPU evaluation at x";
     return MLOAM_E_STATE;
   }
-  a.spec = c->lin_spec, a.spec_publish = c->lin_spec_publish ? 1 : 0;
+  a.spec = o.spec, a.spec_publish = o.spec_publish ? 1 : 0;
   // a fit the matcher deferred to this evaluation
   int kfit = 0;
-  if (c->pending_fit.K) {
-    if (lm_mode != 1 || n_sets != 2 || (c->pending_fit.K != 5 && c->pending_fit.K != 10)) {
+  if (o.fit && o.fit->K) {
+    if (lm_mode != 1 || n_sets != 2 || (o.fit->K != 5 && o.fit->K != 10)) {
       c->err = "linearize: a deferred fit is pending but this is not the first evaluation of a solve";
-      c->pending_fit.K = 0;
       return MLOAM_E_STATE;
     }
-    kfit = c->pending_fit.K;
-    a.fit[0] = c->pending_fit.set[0], a.fit[1] = c->pending_fit.set[1];
-    a.fit_min_plane_dis = c->pending_fit.min_plane_dis, a.fit_check_fov = c->pending_fit.check_fov;
-    c->pending_fit.K = 0;
+    kfit = o.fit->K;
+    a.fit[0] = o.fit->set[0], a.fit[1] = o.fit->set[1];
+    a.fit_min_plane_dis = o.fit->min_plane_dis, a.fit_check_fov = o.fit->check_fov;
   }
   {
     ProfScope ps(c, "linearize");
@@ -975,23 +972,22 @@ int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, 
     int rc = comm_allreduce_doubles(c, ne, NE_PACK);
     if (rc) return rc;
     ProfScope ps(c, "lm");
-    k_lm<<<1, LM_THREADS, 0, c->stream>>>(ne, 1, c->lm_state.as<LMState>(), lm_mode, (c->lm_eig_thre >= 0.0 ? c->lm_eig_thre : c->params.eig_thre), want_eig, d_out30);
+    k_lm<<<1, LM_THREADS, 0, c->stream>>>(ne, 1, c->lm_state.as<LMState>(), lm_mode, o.eig_thre, o.want_eig, d_out30);
     c->launches++;
   } else {
     ProfScope ps(c, "lm");
-    k_lm<<<1, LM_THREADS, 0, c->stream>>>(c->partials.as<double>(), nb, c->lm_state.as<LMState>(), lm_mode, (c->lm_eig_thre >= 0.0 ? c->lm_eig_thre : c->params.eig_thre), want_eig,
-                                  d_out30);
+    k_lm<<<1, LM_THREADS, 0, c->stream>>>(c->partials.as<double>(), nb, c->lm_state.as<LMState>(), lm_mode, o.eig_thre, o.want_eig, d_out30);
     c->launches++;
   }
   MLOAM_CUDA_OK(c, cudaGetLastError());
   return MLOAM_OK;
 }
 
-int eval_candidate_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a) {
+int eval_candidate_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, double eig_thre) {
   LinArgs a;
   int nb = 0;
   double *wsums = nullptr;
-  int rc = lin_setup(c, sets, n_sets, sqrt_info, huber_a, a, &nb, &wsums);
+  int rc = lin_setup(c, sets, n_sets, sqrt_info, huber_a, eig_thre, a, &nb, &wsums);
   if (rc) return rc;
   ProfScope ps(c, "candidate");
   k_eval_candidate<<<nb * (LIN_THREADS / CAND_THREADS), CAND_THREADS, 0, c->stream>>>(a, wsums);
