@@ -120,6 +120,7 @@ int mloam_ctx_create(int device, const mloam_params_t *params, mloam_ctx_t **out
   if (const char *e = getenv("MLOAM_LOOKAHEAD")) c->use_lookahead = (e[0] == '0') ? 0 : 1;
   if (const char *e = getenv("MLOAM_STAMP")) c->stamp_on = e[0] == '1';
   if (const char *e = getenv("MLOAM_FUSE_ITER")) c->fuse_iter = (e[0] == '0') ? 0 : 1;
+  if (const char *e = getenv("MLOAM_LM_TAIL")) c->lm_tail_serial = strcmp(e, "serial") == 0 ? 1 : 0;
   if (const char *e = getenv("MLOAM_DISABLE_SEEDS")) c->use_seeds = (e[0] == '0' || e[0] == '\0') ? 1 : 0;
   *out = h;
   return MLOAM_OK;

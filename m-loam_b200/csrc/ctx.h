@@ -381,6 +381,7 @@ struct Ctx {
   int use_seeds = 1;               // seed the kNN of re-association iterations > 0 with the previous neighbour lists
   int fuse_iter = 1;               // scan2map: fit inside the first evaluation + both evaluations of an LM iteration in ONE launch
                                    // (grid barrier between them); MLOAM_FUSE_ITER=0 restores the three launches
+  int lm_tail_serial = 0;          // the LM step on one thread of the tail block (MLOAM_LM_TAIL=serial) instead of one warp; bit-identical
   bool lidar_merge = false;        // mloam_set_lidars was given extrinsics: features go through the rig merge (also for one LiDAR)
   int n_lidars = 1;                // LiDARs batched into one frame of this context (mloam_set_lidars)
   double lidar_ext[MLOAM_MAX_LIDARS][7];  // their sensor -> base extrinsics

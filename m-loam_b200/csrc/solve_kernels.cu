@@ -10,6 +10,8 @@
 //                 6x6 Cholesky, step acceptance, radius update, tolerances, degeneracy remap) on a shared-memory copy of
 //                 the device-resident state — the host only reads the final state back.
 //   k_lm        : the same tail as a stand-alone kernel (NCCL path, mloam_normal_equations).
+#include <cstddef>
+
 #include "ctx.h"
 #include "factors.cuh"
 #include "match_fit.cuh"
@@ -41,6 +43,7 @@ struct LinArgs {
   int respect_done;
   // fused LM tail (single GPU): the block that finishes last reduces the partials and advances the state machine
   int lm_mode;             // 1 | 2, or 0: no tail (partials only)
+  int lm_serial;           // the tail's state machine on one thread (MLOAM_LM_TAIL=serial) instead of one warp
   int want_eig;
   double eig_thre;
   unsigned *ticket;        // zero between launches
@@ -81,8 +84,9 @@ __device__ __forceinline__ double map_factor_row(const PoseR &P, const FeatSetDe
   return sc * r;
 }
 
+template <bool SERIAL>
 __device__ __noinline__ void lm_tail(const double *partials, int n_blocks, LMState *gst, int mode, double eig_thre, int want_eig, double *out_ne,
-                                     const P2PView *p2p);
+                                     const P2PView *p2p, double *xc_pub);
 
 template <int KFIT>
 __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__restrict__ partials) {
@@ -236,15 +240,17 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
     return;
   }
   __threadfence();
-  lm_tail(partials, (int)gridDim.x, a.state_rw, pass == 0 ? a.lm_mode : 2, a.eig_thre, pass == 0 ? a.want_eig : 1, nullptr, a.p2p);
+  // with spec_publish the tail also copies the new candidate to where the next matcher searches (every block has read the old one)
+  {
+    const int mode = pass == 0 ? a.lm_mode : 2, want_eig = pass == 0 ? a.want_eig : 1;
+    double *const xc_pub = (a.spec && a.spec_publish && pass == 0) ? a.spec->xc : nullptr;
+    if (a.lm_serial) lm_tail<true>(partials, (int)gridDim.x, a.state_rw, mode, a.eig_thre, want_eig, nullptr, a.p2p, xc_pub);
+    else lm_tail<false>(partials, (int)gridDim.x, a.state_rw, mode, a.eig_thre, want_eig, nullptr, a.p2p, xc_pub);
+  }
   __threadfence();  // the state (written by all threads of this block) before the ticket reset and the release
   __syncthreads();
   if (threadIdx.x == 0) {
-    if (a.spec && pass == 0) {  // every block has read sel and fitted: commit, and publish where the next matcher searches
-      if (spec_hit) a.spec->sel = spec_sel ^ 1;
-      if (a.spec_publish)
-        for (int k = 0; k < 7; k++) a.spec->xc[k] = __ldcg(&a.state_rw->xc[k]);
-    }
+    if (a.spec && pass == 0 && spec_hit) a.spec->sel = spec_sel ^ 1;  // every block has read sel and fitted: commit
     *a.ticket = 0u;
     if (a.two_pass && pass == 0) {
       __threadfence();
@@ -448,8 +454,33 @@ __device__ void unpack_ne(const double *ne, double *H, double *g) {
   for (int k = 0; k < 6; k++) g[k] = ne[NE_H + k];
 }
 
+// evalDegenracy's eigen-decomposition of st->H and the remapped V_update (PoseLocalParameterization::setParameter) of a (nearly)
+// degenerate Solve; one thread.
+__device__ void eig_remap(LMState *st, double eig_thre) {
+  double w[6], Vf[36], Vp[36];
+  eig_sym6(st->H, w, Vf);
+  for (int i = 0; i < 36; i++) Vp[i] = Vf[i];
+  for (int j = 0; j < 6; j++) {
+    if (w[j] < eig_thre) {
+      for (int k = 0; k < 6; k++) Vp[k * 6 + j] = 0.0;
+      st->is_degenerate = 1;
+    } else {
+      break;
+    }
+  }
+  for (int i = 0; i < 6; i++) st->eig[i] = w[i];
+  if (st->is_degenerate)
+    for (int i = 0; i < 6; i++)
+      for (int j = 0; j < 6; j++) {
+        double s = 0;
+        for (int k = 0; k < 6; k++) s += Vf[i * 6 + k] * Vp[j * 6 + k];
+        st->V_update[i * 6 + j] = s;
+      }
+}
+
 // One thread advances the state machine on a shared-memory copy of the state (lm_tail stages it in and out).
 // mode 1: begin a Solve with the evaluation at x.  mode 2: digest the evaluation at xc.
+// The reference for lm_advance_warp (MLOAM_LM_TAIL=serial).
 __device__ void lm_advance(LMState *st, const double *ne, int mode, double eig_thre, int want_eig) {
   double H[36], g[6];
   unpack_ne(ne, H, g);
@@ -482,27 +513,7 @@ __device__ void lm_advance(LMState *st, const double *ne, int mode, double eig_t
       double inv_diag[6];
       if (chol6(S, inv_diag)) need_eig = false;
     }
-    if (need_eig) {
-      double w[6], Vf[36], Vp[36];
-      eig_sym6(H, w, Vf);
-      for (int i = 0; i < 36; i++) Vp[i] = Vf[i];
-      for (int j = 0; j < 6; j++) {
-        if (w[j] < eig_thre) {
-          for (int k = 0; k < 6; k++) Vp[k * 6 + j] = 0.0;
-          st->is_degenerate = 1;
-        } else {
-          break;
-        }
-      }
-      for (int i = 0; i < 6; i++) st->eig[i] = w[i];
-      if (st->is_degenerate)
-        for (int i = 0; i < 6; i++)
-          for (int j = 0; j < 6; j++) {
-            double s = 0;
-            for (int k = 0; k < 6; k++) s += Vf[i * 6 + k] * Vp[j * 6 + k];
-            st->V_update[i * 6 + j] = s;
-          }
-    }
+    if (need_eig) eig_remap(st, eig_thre);
     double xn = 0;
     for (int k = 0; k < 7; k++) xn += st->x[k] * st->x[k];
     st->x_norm = sqrt(xn);
@@ -556,10 +567,286 @@ __device__ void lm_advance(LMState *st, const double *ne, int mode, double eig_t
   lm_compute_step(st);
 }
 
+// ---------------------------------------------------------------------------------------- the LM step on one warp
+// lm_advance on the 32 lanes of warp 0 of the tail block, with the serial code's operations in its order (everything is compiled
+// -fmad=false, so the state is bit-identical).  A 6x6 is held by rows: lane 8 q + i owns row i of group q's matrix (rows 6 and 7 of a
+// group are padding), so group 0 factors the damped LM system while group 1 factors H - eig_thre I for the degeneracy test, in one
+// instruction stream; each column's pivot row is broadcast by shuffle.  The Jacobi scaling takes one lane per column, the gradient
+// test and the candidate pose run their pose_plus side by side on lanes 0 and 1, and scalars are computed redundantly by every lane
+// (no divergence, no broadcast).  Only lane 0 writes scalar fields of the shared state; __syncwarp orders reads, writes and re-reads.
+
+// chol6 by rows: lane (lane & ~7) + i holds row i in a[]; inv_diag[j] = 1 / L[j][j] of the lane's group.  Returns chol6's verdict
+// for the lane's group; after a failed pivot the group computes on with NaNs and the factor is not used.
+__device__ __forceinline__ bool chol6_rows(double a[6], double inv_diag[6]) {
+  const int lane = threadIdx.x & 31, base = lane & ~7, r = lane & 7;
+  bool ok = true;
+#pragma unroll
+  for (int j = 0; j < 6; j++) {
+    double d = a[j];
+#pragma unroll
+    for (int k = 0; k < j; k++) d -= a[k] * a[k];
+    d = __shfl_sync(MLOAM_FULL_MASK, d, base + j);
+    ok = ok && d > 0.0;
+    d = sqrt(d);
+    const double inv = 1.0 / d;
+    inv_diag[j] = inv;
+    double pj[6];
+#pragma unroll
+    for (int k = 0; k < j; k++) pj[k] = __shfl_sync(MLOAM_FULL_MASK, a[k], base + j);
+    if (r == j) a[j] = d;
+    if (r > j) {
+      double s = a[j];
+#pragma unroll
+      for (int k = 0; k < j; k++) s -= a[k] * pj[k];
+      a[j] = s * inv;
+    }
+  }
+  return ok;
+}
+
+struct StepTry {
+  bool ok;          // lm_compute_step's ok: the damped system factored, the step is finite and the model cost decreases
+  bool deg_ok;      // with the degeneracy test: H - eig_thre I is positive definite
+  double mcc;       // model cost change
+  double step[6];   // scaled step
+  double diag[6];   // LM diagonal the step used
+};
+
+// The arithmetic of one pass of lm_compute_step's loop (not its bookkeeping) on the state st: group 0 solves the damped scaled
+// system, group 1 factors H - eig_thre I (read with deg_test).  Every lane returns the same values.
+__device__ __forceinline__ StepTry lm_try_step_warp(const LMState *st, bool deg_test, double eig_thre) {
+  const int lane = threadIdx.x & 31, grp = lane >> 3, r = min(lane & 7, 5);
+  double gs[6], hs[6], a[6];
+#pragma unroll
+  for (int b = 0; b < 6; b++) {
+    gs[b] = st->scale[b] * st->g[b];
+    hs[b] = st->scale[r] * st->H[r * 6 + b] * st->scale[b];
+  }
+  const double hrr = st->scale[r] * st->H[r * 7] * st->scale[r];
+  const double dg = st->reuse_diagonal ? st->diag[r] : fmin(fmax(hrr, kMinDiag), kMaxDiag);
+  const double l = sqrt(dg / st->radius);
+#pragma unroll
+  for (int b = 0; b < 6; b++) {
+    const double h = st->H[r * 6 + b];
+    a[b] = grp == 1 ? (b == r ? h - eig_thre : h) : (b == r ? hs[b] + l * l : hs[b]);
+  }
+  double inv[6];
+  const bool ok_grp = chol6_rows(a, inv);
+  StepTry t;
+  t.ok = __shfl_sync(MLOAM_FULL_MASK, (int)ok_grp, 0) != 0;
+  t.deg_ok = __shfl_sync(MLOAM_FULL_MASK, (int)ok_grp, 8) != 0 && deg_test;
+  t.mcc = 0.0;
+#pragma unroll
+  for (int j = 0; j < 6; j++) {
+    inv[j] = __shfl_sync(MLOAM_FULL_MASK, inv[j], 0);
+    t.diag[j] = __shfl_sync(MLOAM_FULL_MASK, dg, j);
+    t.step[j] = 0.0;
+  }
+  if (t.ok) {  // every lane solves with group 0's factor
+    double L[36];
+#pragma unroll
+    for (int i = 1; i < 6; i++)
+#pragma unroll
+      for (int k = 0; k < i; k++) L[i * 6 + k] = __shfl_sync(MLOAM_FULL_MASK, a[k], i);
+    chol6_solve(L, inv, gs, t.step);
+#pragma unroll
+    for (int j = 0; j < 6; j++) {
+      t.step[j] = -t.step[j];
+      if (!isfinite(t.step[j])) t.ok = false;
+    }
+  }
+  if (t.ok) {
+    double hr = 0;  // row r of Hs times the step
+#pragma unroll
+    for (int b = 0; b < 6; b++) hr += hs[b] * t.step[b];
+    double sg = 0, sHs = 0;
+#pragma unroll
+    for (int q = 0; q < 6; q++) {
+      sg += t.step[q] * gs[q];
+      sHs += t.step[q] * __shfl_sync(MLOAM_FULL_MASK, hr, q);
+    }
+    t.mcc = -(sg + 0.5 * sHs);
+    if (t.mcc < 0) t.ok = false;
+  }
+  return t;
+}
+
+// lm_compute_step on the warp.  first / xc_first: the arithmetic of the loop's first pass and its candidate pose, already done by
+// the caller (mode 1), or null.
+__device__ void lm_compute_step_warp(LMState *st, const StepTry *first, const double *xc_first) {
+  const int lane = threadIdx.x & 31;
+  while (true) {
+    if (st->iteration >= st->max_inner) {
+      __syncwarp();
+      if (lane == 0) st->done = 1, st->termination = 0;
+      return;
+    }
+    StepTry t;
+    double xc[7];
+    if (first) {
+      t = *first;
+#pragma unroll
+      for (int k = 0; k < 7; k++) xc[k] = xc_first[k];
+      first = nullptr;
+    } else {
+      t = lm_try_step_warp(st, false, 0.0);
+      if (t.ok) {
+        double delta[6];
+#pragma unroll
+        for (int j = 0; j < 6; j++) delta[j] = t.step[j] * st->scale[j];
+        pose_plus(st->x, delta, st->V_update, xc);
+      }
+    }
+    const bool reuse = st->reuse_diagonal != 0;
+    const int num_invalid = st->num_invalid + 1;
+    const double radius = st->radius * 0.5;
+    __syncwarp();
+    if (lane == 0) {
+      if (!reuse)
+        for (int j = 0; j < 6; j++) st->diag[j] = t.diag[j];
+      st->reuse_diagonal = 1;
+      st->iteration++;
+      st->total_iterations++;
+      if (!t.ok) {
+        st->num_invalid = num_invalid;
+        if (num_invalid >= 5) st->done = 1, st->termination = 4;
+        else st->radius = radius;
+      } else {
+        st->num_invalid = 0;
+        for (int k = 0; k < 7; k++) st->xc[k] = xc[k];
+        st->model_cost_change = t.mcc;
+      }
+    }
+    __syncwarp();
+    if (t.ok || num_invalid >= 5) return;
+  }
+}
+
+// lm_advance on warp 0 of the tail block (all 32 lanes call it); st is the shared-memory copy of the state.
+__device__ void lm_advance_warp(LMState *st, const double *ne, int mode, double eig_thre, int want_eig) {
+  const int lane = threadIdx.x & 31;
+  const double cost = ne[NE_H + NE_G];
+  if (mode == 1) {
+    for (int e = lane; e < 36; e += 32) {  // unpack_ne: both triangles take the packed upper entry
+      const int i = e / 6, j = e % 6, lo = min(i, j), hi = max(i, j);
+      const double h = ne[lo * 6 - lo * (lo - 1) / 2 + hi - lo];
+      st->H[e] = h, st->H0[e] = h;
+    }
+    const int n0 = (int)ne[NE_H + NE_G + 1], n1 = (int)ne[NE_H + NE_G + 2], rows = n0 + n1;
+    const bool skip = rows < st->min_corr;
+    double x[7];
+#pragma unroll
+    for (int k = 0; k < 7; k++) x[k] = st->x[k];
+    if (lane == 0) {
+      for (int i = 0; i < 6; i++) st->g[i] = ne[NE_H + i];
+      st->cost = cost, st->initial_cost = cost;
+      st->n_valid[0] = n0, st->n_valid[1] = n1, st->rows = rows, st->skipped = 0;
+      for (int k = 0; k < 7; k++) st->xc[k] = x[k];
+      if (skip) st->done = 1, st->termination = 5, st->skipped = 1;  // "less correspondence": pose untouched
+    }
+    if (skip) return;
+    bool need_eig = rows > 0 && eig_thre > 0.0;
+    const bool deg_test = need_eig && !want_eig;
+    double xn = 0;
+#pragma unroll
+    for (int k = 0; k < 7; k++) xn += x[k] * x[k];
+    __syncwarp();  // H
+    for (int e = lane; e < 36; e += 32) st->V_update[e] = (e % 7 == 0) ? 1.0 : 0.0;
+    if (lane < 6) st->eig[lane] = 0.0, st->scale[lane] = 1.0 / (1.0 + sqrt(st->H[lane * 7]));
+    if (lane == 0) {
+      st->is_degenerate = 0;
+      st->x_norm = sqrt(xn);
+      st->radius = 1e4, st->decrease_factor = 2.0, st->reuse_diagonal = 0;
+      st->iteration = 0, st->num_invalid = 0, st->done = 0, st->termination = 0;
+    }
+    __syncwarp();
+    // V_update does not enter the step: factor it (group 0) next to the degeneracy test (group 1)
+    const StepTry t = lm_try_step_warp(st, deg_test, eig_thre);
+    if (t.deg_ok) need_eig = false;
+    if (need_eig) {  // (nearly) degenerate, or the eigenvalue report was asked for: the Jacobi solver on one lane
+      if (lane == 0) eig_remap(st, eig_thre);
+      __syncwarp();
+    }
+    // gradient_max_norm (even lanes) and the candidate pose of the step (odd lanes), with the final V_update
+    double dv[6], xp[7];
+#pragma unroll
+    for (int j = 0; j < 6; j++) dv[j] = (lane & 1) ? t.step[j] * st->scale[j] : -st->g[j];
+    pose_plus(x, dv, st->V_update, xp);
+    double m = 0;
+#pragma unroll
+    for (int k = 0; k < 7; k++) m = fmax(m, fabs(x[k] - xp[k]));
+    m = __shfl_sync(MLOAM_FULL_MASK, m, 0);
+    double xc[7];
+#pragma unroll
+    for (int k = 0; k < 7; k++) xc[k] = __shfl_sync(MLOAM_FULL_MASK, xp[k], 1);
+    if (m <= kGradTol) {
+      if (lane == 0) st->done = 1, st->termination = 3;
+      return;
+    }
+    lm_compute_step_warp(st, &t, xc);
+    return;
+  }
+  // mode 2
+  if (st->done) return;
+  double x[7], xc[7];
+#pragma unroll
+  for (int k = 0; k < 7; k++) x[k] = st->x[k], xc[k] = st->xc[k];
+  double sn = 0;
+#pragma unroll
+  for (int k = 0; k < 7; k++) sn += (x[k] - xc[k]) * (x[k] - xc[k]);
+  sn = sqrt(sn);
+  if (sn <= kParamTol * (st->x_norm + kParamTol)) {
+    if (lane == 0) st->done = 1, st->termination = 2;
+    return;
+  }
+  const double cost_change = st->cost - cost;
+  if (fabs(cost_change) <= kFuncTol * st->cost) {
+    if (lane == 0) st->done = 1, st->termination = 1;
+    return;
+  }
+  const double rel = cost_change / st->model_cost_change;
+  if (rel > kMinRelDecrease) {
+    const double t = 2.0 * rel - 1.0;
+    double radius = st->radius / fmax(1.0 / 3.0, 1.0 - t * t * t);
+    radius = fmin(kMaxRadius, radius);
+    double xn = 0;
+#pragma unroll
+    for (int k = 0; k < 7; k++) xn += xc[k] * xc[k];
+    double neg[6], xp[7];
+#pragma unroll
+    for (int j = 0; j < 6; j++) neg[j] = -ne[NE_H + j];
+    pose_plus(xc, neg, st->V_update, xp);  // gradient_max_norm at the accepted pose
+    double m = 0;
+#pragma unroll
+    for (int k = 0; k < 7; k++) m = fmax(m, fabs(xc[k] - xp[k]));
+    __syncwarp();
+    for (int e = lane; e < 36; e += 32) {
+      const int i = e / 6, j = e % 6, lo = min(i, j), hi = max(i, j);
+      st->H[e] = ne[lo * 6 - lo * (lo - 1) / 2 + hi - lo];
+    }
+    if (lane == 0) {
+      st->radius = radius, st->decrease_factor = 2.0, st->reuse_diagonal = 0;
+      for (int k = 0; k < 7; k++) st->x[k] = xc[k];
+      st->x_norm = sqrt(xn);
+      for (int i = 0; i < 6; i++) st->g[i] = ne[NE_H + i];
+      st->cost = cost;
+      if (m <= kGradTol) st->done = 1, st->termination = 3;
+    }
+    __syncwarp();
+    if (m <= kGradTol) return;
+  } else {
+    const double radius = st->radius / st->decrease_factor, df = st->decrease_factor * 2.0;
+    __syncwarp();
+    if (lane == 0) st->radius = radius, st->decrease_factor = df, st->reuse_diagonal = 1;
+    __syncwarp();
+  }
+  lm_compute_step_warp(st, nullptr, nullptr);
+}
+
 // Called by all LM_THREADS threads of one block.  Block partials -> packed normal equations in a fixed order
 // (deterministic): warp w sums blocks w, w+8, ... for component `lane`, then the 8 warp sums are added in warp order.
 // The LM state lives in global memory between launches; it is staged through shared memory here because the
-// single-threaded state machine touches it a few hundred times (each a dependent L2 round trip otherwise).
+// state machine touches it a few hundred times (each a dependent L2 round trip otherwise).
 //
 // Multi-GPU (p2p != nullptr): one LiDAR per GPU, the LM step needs the SUM of every rank's normal equations.  The
 // reduction, the exchange and the step are one kernel: this block stores its 30 doubles into slot[rank] of every
@@ -567,21 +854,65 @@ __device__ void lm_advance(LMState *st, const double *ne, int mode, double eig_t
 // flags carry this exchange's epoch, and adds the slots in rank order — the same order on every rank, so all ranks
 // advance bit-identical states.  Slots and flags are double-buffered by the parity of the epoch: a rank can only be
 // one exchange ahead of the slowest one, so a slot is never overwritten before it has been read.
-__device__ __noinline__ void lm_tail(const double *partials, int n_blocks, LMState *gst, int mode, double eig_thre, int want_eig, double *out_ne,
-                                     const P2PView *p2p) {
-  __shared__ double ne[NE_PACK];
-  __shared__ unsigned long long p2p_epoch;
-  __shared__ int p2p_timeout;
-  __shared__ double wsum[LM_THREADS / 32][32];
-  __shared__ LMState s;
-  static_assert(sizeof(LMState) % 8 == 0, "LMState is staged as 8-byte words");
-  constexpr int kWords = (int)(sizeof(LMState) / 8);
-  const long long t0 = clock64();
-  if (mode != 0) {
-    const unsigned long long *src = reinterpret_cast<const unsigned long long *>(gst);
-    unsigned long long *dst = reinterpret_cast<unsigned long long *>(&s);
-    for (int k = threadIdx.x; k < kWords; k += LM_THREADS) dst[k] = __ldcg(src + k);
+//
+// SERIAL: the state machine on thread 0 (lm_advance, MLOAM_LM_TAIL=serial) instead of warp 0 (lm_advance_warp); bit-identical.
+// Two instances rather than a run-time branch, so that the warp tail does not carry the serial code's registers and stack.
+// xc_pub (or null): 7 doubles that receive the new candidate pose, copied from the shared state.
+
+// Words of LMState a tail stages: mode 2 never reads eig or H0 and never writes V_update, eig or H0.
+static_assert(sizeof(LMState) % 8 == 0, "LMState is staged as 8-byte words");
+constexpr int kStateWords = (int)(sizeof(LMState) / 8);
+constexpr int kVupdateWord = (int)(offsetof(LMState, V_update) / 8), kEigWord = (int)(offsetof(LMState, eig) / 8);
+constexpr int kH0EndWord = (int)(offsetof(LMState, initial_cost) / 8);
+static_assert(kEigWord == kVupdateWord + 36 && kH0EndWord == kEigWord + 6 + 36, "V_update, eig and H0 are adjacent");
+__device__ __forceinline__ void stage_state_in(LMState *s, const LMState *gst, int mode, int nthreads) {
+  const unsigned long long *src = reinterpret_cast<const unsigned long long *>(gst);
+  unsigned long long *dst = reinterpret_cast<unsigned long long *>(s);
+  for (int k = threadIdx.x; k < kStateWords; k += nthreads)
+    if (mode != 2 || k < kEigWord || k >= kH0EndWord) dst[k] = __ldcg(src + k);
+}
+__device__ __forceinline__ void stage_state_out(const LMState *s, LMState *gst, int mode, int nthreads) {
+  const unsigned long long *src = reinterpret_cast<const unsigned long long *>(s);
+  unsigned long long *dst = reinterpret_cast<unsigned long long *>(gst);
+  for (int k = threadIdx.x; k < kStateWords; k += nthreads)
+    if (mode != 2 || k < kVupdateWord || k >= kH0EndWord) dst[k] = src[k];
+}
+
+// Runs the state machine on the staged state s (thread 0 serially, or warp 0) and keeps the cycle counters.  Called by all threads.
+template <bool SERIAL>
+__device__ __forceinline__ void lm_run(LMState *s, const double *ne, int mode, double eig_thre, int want_eig, long long t0, bool failed) {
+  if (threadIdx.x >= 32) return;
+  const long long t1 = clock64();
+  if (SERIAL) {
+    if (threadIdx.x == 0) lm_advance(s, ne, mode, eig_thre, want_eig);
+  } else {
+    lm_advance_warp(s, ne, mode, eig_thre, want_eig);
+    __syncwarp();
   }
+  if (threadIdx.x == 0) {
+    s->work[0] = 0, s->work[1] = 0;  // re-arm the match work queues
+    if (failed) s->done = 1, s->termination = 9;  // the peer-memory exchange failed: the state is not trustworthy
+    s->dbg_cycles[0] += t1 - t0, s->dbg_cycles[1] += clock64() - t1, s->dbg_cycles[2] += 1;
+  }
+}
+
+// Shared memory of the tails, at namespace scope so that both instances of a tail in one kernel use the same allocation.
+__shared__ double tail_ne[NE_PACK];
+__shared__ LMState tail_state;
+__shared__ unsigned long long tail_p2p_epoch;
+__shared__ int tail_p2p_timeout;
+__shared__ double tail_wsum[LM_THREADS / 32][32];
+
+template <bool SERIAL>
+__device__ __noinline__ void lm_tail(const double *partials, int n_blocks, LMState *gst, int mode, double eig_thre, int want_eig, double *out_ne,
+                                     const P2PView *p2p, double *xc_pub) {
+  double *const ne = tail_ne;
+  unsigned long long &p2p_epoch = tail_p2p_epoch;
+  int &p2p_timeout = tail_p2p_timeout;
+  double (*const wsum)[32] = tail_wsum;
+  LMState &s = tail_state;
+  const long long t0 = clock64();
+  if (mode != 0) stage_state_in(&s, gst, mode, LM_THREADS);
   {
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     constexpr int S = LM_THREADS / 32;
@@ -648,24 +979,16 @@ __device__ __noinline__ void lm_tail(const double *partials, int n_blocks, LMSta
     if (threadIdx.x == 0) *p2p->epoch = ep + 1ull;
     __syncthreads();
   }
-  if (threadIdx.x == 0) {
-    s.work[0] = 0, s.work[1] = 0;  // re-arm the match work queues
-    const long long t1 = clock64();
-    lm_advance(&s, ne, mode, eig_thre, want_eig);
-    if (p2p && p2p_timeout) s.done = 1, s.termination = 9;  // exchange failed: the state is not trustworthy
-    s.dbg_cycles[0] += t1 - t0, s.dbg_cycles[1] += clock64() - t1, s.dbg_cycles[2] += 1;
-  }
+  lm_run<SERIAL>(&s, ne, mode, eig_thre, want_eig, t0, p2p && p2p_timeout);
   __syncthreads();
-  {
-    const unsigned long long *src = reinterpret_cast<const unsigned long long *>(&s);
-    unsigned long long *dst = reinterpret_cast<unsigned long long *>(gst);
-    for (int k = threadIdx.x; k < kWords; k += LM_THREADS) dst[k] = src[k];
-  }
+  stage_state_out(&s, gst, mode, LM_THREADS);
+  if (xc_pub && threadIdx.x < 7) xc_pub[threadIdx.x] = s.xc[threadIdx.x];
 }
 
 __global__ void __launch_bounds__(LM_THREADS) k_lm(const double *__restrict__ partials, int n_blocks, LMState *st, int mode, double eig_thre,
-                                                  int want_eig, double *__restrict__ out_ne) {
-  lm_tail(partials, n_blocks, st, mode, eig_thre, want_eig, out_ne, nullptr);
+                                                  int want_eig, double *__restrict__ out_ne, int serial) {
+  if (serial) lm_tail<true>(partials, n_blocks, st, mode, eig_thre, want_eig, out_ne, nullptr, nullptr);
+  else lm_tail<false>(partials, n_blocks, st, mode, eig_thre, want_eig, out_ne, nullptr, nullptr);
 }
 
 // ---------------------------------------------------------------------------------------- candidate evaluation
@@ -680,18 +1003,17 @@ constexpr int CAND_THREADS = 64;
 constexpr int NE_CAND = 9;  // g | cost | rows(set 0) | rows(set 1) = NE_PACK components 21..29
 constexpr int LIN_WARPS = LIN_THREADS / 32;
 
+__shared__ double cand_bsum[64][NE_CAND];  // per k_linearize block (n_lin_blocks <= 64)
+__shared__ double cand_vsum[LM_THREADS / 32][NE_CAND];
+
+template <bool SERIAL>
 __device__ __noinline__ void cand_tail(const double *wsums, int n_lin_blocks, LMState *gst, double eig_thre) {
-  __shared__ double bsum[64][NE_CAND];       // per k_linearize block (n_lin_blocks <= 64)
-  __shared__ double vsum[LM_THREADS / 32][NE_CAND];
-  __shared__ double ne[NE_PACK];
-  __shared__ LMState s;
-  constexpr int kWords = (int)(sizeof(LMState) / 8);
+  double (*const bsum)[NE_CAND] = cand_bsum;
+  double (*const vsum)[NE_CAND] = cand_vsum;
+  double *const ne = tail_ne;
+  LMState &s = tail_state;
   const long long t0 = clock64();
-  {
-    const unsigned long long *src = reinterpret_cast<const unsigned long long *>(gst);
-    unsigned long long *dst = reinterpret_cast<unsigned long long *>(&s);
-    for (int k = threadIdx.x; k < kWords; k += CAND_THREADS) dst[k] = __ldcg(src + k);
-  }
+  stage_state_in(&s, gst, 2, CAND_THREADS);
   // k_linearize's block partial: its 8 warp sums in warp order
   for (int b = threadIdx.x; b < n_lin_blocks; b += CAND_THREADS) {
 #pragma unroll 3
@@ -722,18 +1044,9 @@ __device__ __noinline__ void cand_tail(const double *wsums, int n_lin_blocks, LM
     ne[threadIdx.x] = t;
   }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    s.work[0] = 0, s.work[1] = 0;
-    const long long t1 = clock64();
-    lm_advance(&s, ne, 2, eig_thre, 1);
-    s.dbg_cycles[0] += t1 - t0, s.dbg_cycles[1] += clock64() - t1, s.dbg_cycles[2] += 1;
-  }
+  lm_run<SERIAL>(&s, ne, 2, eig_thre, 1, t0, false);
   __syncthreads();
-  {
-    const unsigned long long *src = reinterpret_cast<const unsigned long long *>(&s);
-    unsigned long long *dst = reinterpret_cast<unsigned long long *>(gst);
-    for (int k = threadIdx.x; k < kWords; k += CAND_THREADS) dst[k] = src[k];
-  }
+  stage_state_out(&s, gst, 2, CAND_THREADS);
 }
 
 // grid: LIN_THREADS / CAND_THREADS blocks per k_linearize block; wsums: NE_CAND doubles per warp
@@ -777,7 +1090,8 @@ __global__ void __launch_bounds__(CAND_THREADS, 8) k_eval_candidate(LinArgs a, d
   __syncthreads();
   if (!is_last) return;
   __threadfence();
-  cand_tail(wsums, (int)(gridDim.x / (LIN_THREADS / CAND_THREADS)), a.state_rw, a.eig_thre);
+  if (a.lm_serial) cand_tail<true>(wsums, (int)(gridDim.x / (LIN_THREADS / CAND_THREADS)), a.state_rw, a.eig_thre);
+  else cand_tail<false>(wsums, (int)(gridDim.x / (LIN_THREADS / CAND_THREADS)), a.state_rw, a.eig_thre);
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) *a.ticket = 0u;
@@ -894,6 +1208,7 @@ static int lin_setup(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, 
   a.state = c->lm_state.as<LMState>();
   a.state_rw = c->lm_state.as<LMState>();
   a.eig_thre = eig_thre;
+  a.lm_serial = c->lm_tail_serial;
   int nb = (n_total + LIN_THREADS - 1) / LIN_THREADS;
   if (nb < 1) nb = 1;
   // n_total is a launch upper bound (device-side counts are usually far smaller): 64 blocks x 256 threads cover a
@@ -966,17 +1281,17 @@ int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, 
     double *ne = c->partials.as<double>() + (size_t)NE_PACK * max_nb;
     {
       ProfScope ps(c, "lm");
-      k_lm<<<1, LM_THREADS, 0, c->stream>>>(c->partials.as<double>(), nb, c->lm_state.as<LMState>(), 0, 0.0, 0, ne);
+      k_lm<<<1, LM_THREADS, 0, c->stream>>>(c->partials.as<double>(), nb, c->lm_state.as<LMState>(), 0, 0.0, 0, ne, c->lm_tail_serial);
       c->launches++;
     }
     int rc = comm_allreduce_doubles(c, ne, NE_PACK);
     if (rc) return rc;
     ProfScope ps(c, "lm");
-    k_lm<<<1, LM_THREADS, 0, c->stream>>>(ne, 1, c->lm_state.as<LMState>(), lm_mode, o.eig_thre, o.want_eig, d_out30);
+    k_lm<<<1, LM_THREADS, 0, c->stream>>>(ne, 1, c->lm_state.as<LMState>(), lm_mode, o.eig_thre, o.want_eig, d_out30, c->lm_tail_serial);
     c->launches++;
   } else {
     ProfScope ps(c, "lm");
-    k_lm<<<1, LM_THREADS, 0, c->stream>>>(c->partials.as<double>(), nb, c->lm_state.as<LMState>(), lm_mode, o.eig_thre, o.want_eig, d_out30);
+    k_lm<<<1, LM_THREADS, 0, c->stream>>>(c->partials.as<double>(), nb, c->lm_state.as<LMState>(), lm_mode, o.eig_thre, o.want_eig, d_out30, c->lm_tail_serial);
     c->launches++;
   }
   MLOAM_CUDA_OK(c, cudaGetLastError());
