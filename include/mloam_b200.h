@@ -362,6 +362,36 @@ int mloam_keyframe_query(mloam_ctx_t *ctx, int *n_keyframes, int *h_surrounding,
 int mloam_keyframe_scan(mloam_ctx_t *ctx, int id, double *pose7, double *cov36, mloam_point_t *h_surf, float *h_surf_cov6, int cap_surf,
                         int *n_surf, mloam_point_t *h_corner, float *h_corner_cov6, int cap_corner, int *n_corner);
 
+/* ---- the global map of the keyframe store: pubGlobalMap (lidar_mapper_keyframe.cpp:780-851) and saveGlobalMap (:853-919) on the device.
+ * mloam_global_map: the keyframes offered to the position filter are
+ *   MLOAM_GLOBAL_MAP_SURROUND  those with float squared distance d2 < (float)(radius^2) of the float position of center7, ascending
+ *                              (d2, id) (:804-808); center7 NULL: the position the last mloam_keyframe_save call tested (pose_point_cur,
+ *                              the last frame's pose unless the caller passed one); radius = GLOBALMAP_KF_RADIUS (1000 m)
+ *   MLOAM_GLOBAL_MAP_SAVE      every keyframe in id order (:862-863; the reference does not clear global_map_keyframes there, so a list
+ *                              the publisher left would sit in front: restated as the state in which the publisher never ran)
+ *   -> VoxelGridCovarianceMLOAM<PointI>(kf_leaf = 10 m, :1293) with intensity = id, the last id of a voxel wins -> per chosen keyframe in
+ *   filter order, cloudUCTAssociateToMap of its clouds with its stored pose and covariance and the CURRENT extrinsics / covariances
+ *   (mloam_set_lidars / mloam_set_uncertainty) and the store's TRACE_THRESHOLD_MAPPING; SURROUND appends surf then corner to map 0,
+ *   SAVE appends surf to map 0 and corner to map 1 -> VoxelGridCovarianceMLOAM<PointIWithCov>(leaf, TRACE_THRESHOLD_MAPPING) of each map
+ *   (leaf: MAP_SURF_RES for SURROUND, 2 * MAP_SURF_RES for both maps of SAVE).  The store keeps no outlier clouds (laser_cloud_outlier_cov,
+ *   :673-681), so the reference's outlier appends (:825-827, :871-873) are left out and the maps hold surf and corner points only.  One
+ *   batched association per map: the launch count does not grow with the keyframes (a fixed 15 more when over 2048 keyframes reach the
+ *   position filter).
+ *   Outputs (nullable): the chosen count and the two map sizes (map 1 is empty for SURROUND).  No keyframe offered: MLOAM_OK, empty
+ *   result, no launch.  MLOAM_E_STATE without mloam_keyframes_init or with a communicator; MLOAM_E_INVALID over 2^31 map points.  A call
+ *   that fails leaves an empty result (no chosen ids, empty maps).  The
+ *   result stays on the device until the next mloam_global_map or mloam_keyframes_init call; the mapper's own state (submap cache, map
+ *   slots, surrounding set) is not touched.  Runs on the context stream between frames.
+ * mloam_global_map_read: map `which` (0, 1) and its cov_vec (nullable; cap in points).  *n = the map's size, also when cap is too small
+ *   (MLOAM_E_INVALID), so a caller can size its buffers and read again.
+ * mloam_global_map_chosen: the chosen keyframe ids in filter order, with the same capacity rule. */
+#define MLOAM_GLOBAL_MAP_SURROUND 0
+#define MLOAM_GLOBAL_MAP_SAVE 1
+int mloam_global_map(mloam_ctx_t *ctx, int mode, const double *center7, double radius, double kf_leaf, float leaf, int *n_chosen, int *n_map0,
+                     int *n_map1);
+int mloam_global_map_read(mloam_ctx_t *ctx, int which, mloam_point_t *h_pts, float *h_cov6, int cap, int *n);
+int mloam_global_map_chosen(mloam_ctx_t *ctx, int *h_ids, int cap, int *n);
+
 /* ---- FeatureExtract::matchCornerFromScan / matchSurfFromScan (feature_extract.hpp:131-376) against the map slot
  * built (mloam_map_build, cell ~1.3 m) from the previous sweep's less-sharp / less-flat features, which must be in
  * the reference's ring-sorted order (int(intensity) = ring).  type 'c': coeffs = [X_closest; X_second];

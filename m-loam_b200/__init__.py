@@ -20,6 +20,7 @@ ROOT = os.path.dirname(HERE)
 LIB_PATH = os.environ.get("MLOAM_LIB", os.path.join(HERE, "libmloam_b200.so"))
 
 MAP_CORNER, MAP_SURF, MAP_SCAN_CORNER, MAP_SCAN_SURF = 0, 1, 2, 3
+GLOBAL_MAP_SURROUND, GLOBAL_MAP_SAVE = 0, 1  # mloam_global_map modes: pubGlobalMap, saveGlobalMap
 E_NO_DEVICE = -2
 
 # every entry point include/mloam_b200.h declares
@@ -32,6 +33,7 @@ ABI_SYMBOLS = [
     "mloam_frame_device", "mloam_set_extrinsic", "mloam_set_lidars", "mloam_calib_frame", "mloam_compound_pose_cov", "mloam_cloud_uct_associate", "mloam_voxel_downsample_cov", "mloam_submap_assemble", "mloam_good_features_odom", "mloam_local_map_build", "mloam_match_from_scan", "mloam_track_cloud", "mloam_odom_solve", "mloam_point_uncertainty", "mloam_scan2map_ua", "mloam_good_features", "mloam_comm_unique_id", "mloam_comm_init", "mloam_comm_destroy", "mloam_comm_p2p_export", "mloam_comm_p2p_init", "mloam_comm_p2p_reset",
     "mloam_set_uncertainty", "mloam_pose_covariance", "mloam_frame_scan",
     "mloam_keyframes_init", "mloam_keyframe_save", "mloam_keyframe_submap", "mloam_keyframe_query", "mloam_keyframe_scan",
+    "mloam_global_map", "mloam_global_map_read", "mloam_global_map_chosen",
     "mloam_cal_timestamp", "mloam_set_front_end", "mloam_front_end", "mloam_frame_raw", "mloam_frame_raw_device", "mloam_frame_set_next_raw",
     "mloam_frame_set_next_raw_device",
 ]
@@ -650,6 +652,32 @@ class Context:
         self._ck(lib().mloam_keyframe_scan(self._h, int(kf_id), _p(pose), _p(cov), _p(sp), _p(sc), sp.shape[0], C.byref(ns), _p(cp), _p(cc),
                                            cp.shape[0], C.byref(nc)))
         return pose, cov.reshape(6, 6), sp[:ns.value].copy(), sc[:ns.value].copy(), cp[:nc.value].copy(), cc[:nc.value].copy()
+
+    # ---- global map of the keyframe store (pubGlobalMap / saveGlobalMap on the device)
+    def global_map(self, mode: int, center=None, radius: float = 1000.0, kf_leaf: float = 10.0, leaf: float | None = None):
+        """GLOBAL_MAP_SURROUND: (map [n,4], cov6) of the keyframes within `radius` of center (None: the last tested frame position),
+        leaf default params.surf_leaf.  GLOBAL_MAP_SAVE: (surf [n,4], surf_cov6, corner [m,4], corner_cov6) of every keyframe, leaf
+        default 2 * params.surf_leaf.  The chosen keyframe ids: global_map_chosen()."""
+        if leaf is None:
+            leaf = self.params.surf_leaf * (2.0 if mode == GLOBAL_MAP_SAVE else 1.0)
+        ct = None if center is None else np.ascontiguousarray(center, np.float64)
+        nch, n0, n1 = C.c_int(0), C.c_int(0), C.c_int(0)
+        self._ck(lib().mloam_global_map(self._h, int(mode), _p(ct), C.c_double(radius), C.c_double(kf_leaf), C.c_float(leaf), C.byref(nch),
+                                        C.byref(n0), C.byref(n1)))
+        out = []
+        for which, n in enumerate((n0.value, n1.value)[:1 if mode == GLOBAL_MAP_SURROUND else 2]):
+            p, c6, got = np.zeros((max(n, 1), 4), np.float32), np.zeros((max(n, 1), 6), np.float32), C.c_int(0)
+            self._ck(lib().mloam_global_map_read(self._h, which, _p(p), _p(c6), p.shape[0], C.byref(got)))
+            out += [p[:got.value], c6[:got.value]]
+        return tuple(out)
+
+    def global_map_chosen(self):
+        """Keyframe ids the last global_map's position filter chose, in filter order."""
+        n = C.c_int(0)
+        self._ck(lib().mloam_global_map_chosen(self._h, None, 0, C.byref(n)))
+        ids = np.zeros(max(n.value, 1), np.int32)
+        self._ck(lib().mloam_global_map_chosen(self._h, _p(ids), ids.shape[0], C.byref(n)))
+        return ids[:n.value].tolist()
 
     def set_extrinsic(self, ext7=None):
         e = None if ext7 is None else np.ascontiguousarray(ext7, np.float64)

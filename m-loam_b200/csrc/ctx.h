@@ -64,13 +64,14 @@ struct LinOpts {
 struct DevBuf {
   void *p = nullptr;
   size_t cap = 0;
+  bool in_graphs = true;  // false: no frame graph references the buffer, so its reallocation leaves the captured graphs valid
   cudaError_t reserve(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
     size_t want = bytes + bytes / 4 + 256;
     if (p) cudaFree(p);
     p = nullptr;
     cap = 0;
-    alloc_epoch()++;
+    if (in_graphs) alloc_epoch()++;
     cudaError_t e = cudaMalloc(&p, want);
     if (e == cudaSuccess) cap = want;
     return e;

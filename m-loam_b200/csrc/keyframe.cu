@@ -7,6 +7,9 @@
 //                          keyframe), the keyframe-position filter (:325-338), `+=` of the chosen cached clouds (k_gather_*), the two
 //                          covariance filters (:344-347) and the map build into MLOAM_MAP_SURF / MLOAM_MAP_CORNER
 //   mloam_keyframe_query / mloam_keyframe_scan   what a caller that publishes keyframes needs
+//   mloam_global_map       pubGlobalMap (:780-851) / saveGlobalMap (:853-919): radius search or every keyframe, the keyframe-position
+//                          filter, one batched cloudUCTAssociateToMap over every cloud of the chosen keyframes (k_uct_associate_seg,
+//                          submap.cu) and the covariance filter, into buffers of its own; _read / _chosen return the result
 // No point of a keyframe crosses PCIe: only poses, counts and the ids of the surrounding set do.
 #include <algorithm>
 #include <cmath>
@@ -164,11 +167,26 @@ struct KeyframeStore {
   std::vector<GatherEnt> h_tab;
   std::vector<UctLaser> h_lasers;
   std::vector<float4> h_chosen;
+  float cur_pt[3] = {0.f, 0.f, 0.f};  // pose_point_cur: the position the last mloam_keyframe_save call tested (:643-645)
+  // the last mloam_global_map: its own work and result buffers (no frame graph references them, and the mapper's submap state is never
+  // touched), sized by its input
+  struct GlobalMap {
+    DevBuf tab{nullptr, 0, false};        // positions in | position filter out | count | segments | keyframe poses | UctLaser blocks
+    DevBuf assoc{nullptr, 0, false};      // UctBufs of the larger map input
+    DevBuf merged{nullptr, 0, false};     // the associated, gated cloud of one map: points | cov_vec | trace
+    DevBuf voxel{nullptr, 0, false};      // the filters' work
+    DevBuf out[2] = {{nullptr, 0, false}, {nullptr, 0, false}};  // filtered map t: points | cov_vec | trace | count
+    int n[2] = {0, 0};                    // filtered sizes
+    const float4 *pts[2] = {nullptr, nullptr};
+    const float *cov6[2] = {nullptr, nullptr};
+    std::vector<int> chosen;              // keyframe ids the position filter chose, in filter order
+  } gm;
   void release() {
     for (auto &b : chunks) b.release();
     chunks.clear();
     for (int t = 0; t < 2; t++) cache[t].release(), merged_pts[t].release(), merged_cov6[t].release(), merged_trace[t].release(), filt[t].release();
     ctl.release(), tab.release();
+    for (DevBuf *b : {&gm.tab, &gm.assoc, &gm.merged, &gm.voxel, &gm.out[0], &gm.out[1]}) b->release();
   }
   size_t filt_cap(int t) const { return merged_ub[t] + 16; }
   // filtered map t: points | cov_vec | cov_trace, sized for filt_cap(t) points
@@ -214,6 +232,21 @@ bool keyframe_due(const KeyframeStore &S, const double *pose7) {
   return ang / 3.14159265358979323846 * 180.0 > S.orient_kf_deg;  // / M_PI * 180
 }
 
+// pcl::KdTreeFLANN::radiusSearch over pose_keyframes_3d around the float PointI q (L2_Simple in float): the keyframes with
+// d2 < (float)(radius^2) (FLANN's RadiusResultSet), ascending (d2, id)
+std::vector<std::pair<float, int>> radius_hits(const KeyframeStore &S, const float q[3], double radius) {
+  const float r2 = (float)(radius * radius);
+  std::vector<std::pair<float, int>> hits;
+  for (int k = 0; k < (int)S.kfs.size(); k++) {
+    const float dx = S.kfs[k].pos[0] - q[0], dy = S.kfs[k].pos[1] - q[1], dz = S.kfs[k].pos[2] - q[2];
+    float d2 = 0.f;
+    d2 += dx * dx, d2 += dy * dy, d2 += dz * dz;
+    if (d2 < r2) hits.push_back({d2, k});
+  }
+  std::sort(hits.begin(), hits.end());
+  return hits;
+}
+
 }  // namespace
 }  // namespace mloam
 
@@ -257,6 +290,7 @@ int mloam_keyframe_save(mloam_ctx_t *h, const double *pose7, const double *cov36
   KeyframeStore &S = *c->kf;
   c->frame_since_save = false;  // one decision per frame
   const double *pose = pose7 ? pose7 : c->last_pose7;
+  for (int q = 0; q < 3; q++) S.cur_pt[q] = (float)pose[q];
   if (!keyframe_due(S, pose)) return MLOAM_OK;
   KeyframeStore::Kf k;
   memcpy(k.pose, pose, sizeof(k.pose));
@@ -317,15 +351,7 @@ int mloam_keyframe_submap(mloam_ctx_t *h, const double *pose_pred7, int *rebuilt
     // :263-272 radius search over pose_keyframes_3d with the float PointI of the prediction (pcl::KdTreeFLANN, L2_Simple in float):
     // d2 < radius^2 (FLANN's RadiusResultSet), ascending (d2, id)
     const float q[3] = {(float)pose_pred7[0], (float)pose_pred7[1], (float)pose_pred7[2]};
-    const float r2 = (float)(S.radius * S.radius);
-    std::vector<std::pair<float, int>> hits;
-    for (int k = 0; k < (int)S.kfs.size(); k++) {
-      const float dx = S.kfs[k].pos[0] - q[0], dy = S.kfs[k].pos[1] - q[1], dz = S.kfs[k].pos[2] - q[2];
-      float d2 = 0.f;
-      d2 += dx * dx, d2 += dy * dy, d2 += dz * dz;
-      if (d2 < r2) hits.push_back({d2, k});
-    }
-    std::sort(hits.begin(), hits.end());
+    const std::vector<std::pair<float, int>> hits = radius_hits(S, q, S.radius);
     std::vector<char> in_radius(S.kfs.size(), 0), in_set(S.kfs.size(), 0);
     for (const auto &x : hits) in_radius[x.second] = 1;
     // :274-292 drop the ids that left, survivors keep their order; :294-323 append the new ids in radius order
@@ -552,6 +578,177 @@ int mloam_keyframe_scan(mloam_ctx_t *h, int id, double *pose7, double *cov36, ml
     if (m && hcv[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hcv[t], rec.cov6[t], 24 * m, cudaMemcpyDeviceToHost, st));
   }
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  return MLOAM_OK;
+}
+
+int mloam_global_map(mloam_ctx_t *h, int mode, const double *center7, double radius, double kf_leaf, float leaf, int *n_chosen, int *n_map0,
+                     int *n_map1) {
+  if (n_chosen) *n_chosen = 0;
+  if (n_map0) *n_map0 = 0;
+  if (n_map1) *n_map1 = 0;
+  if (!h || (mode != MLOAM_GLOBAL_MAP_SURROUND && mode != MLOAM_GLOBAL_MAP_SAVE) || !(kf_leaf > 0.0) || !(leaf > 0.f) ||
+      (mode == MLOAM_GLOBAL_MAP_SURROUND && !(radius > 0.0)))
+    return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (multi_gpu(c)) return fail(c, MLOAM_E_STATE, "global_map: the keyframe store is single-GPU only; detach the communicator");
+  if (!c->kf) return fail(c, MLOAM_E_STATE, "global_map: call mloam_keyframes_init first");
+  cudaSetDevice(c->device);
+  KeyframeStore &S = *c->kf;
+  KeyframeStore::GlobalMap &G = S.gm;
+  // the result is committed at the end: a call that fails leaves an empty result, never a part of one
+  G.n[0] = G.n[1] = 0;
+  G.chosen.clear();
+  std::vector<int> chosen;
+  // the keyframes offered to the position filter, in order: pubGlobalMap's radius search around pose_point_cur (:804-808), or
+  // saveGlobalMap's every keyframe in id order (:862-863; global_map_keyframes taken as empty before, as when the publisher never ran)
+  std::vector<int> cand;
+  if (mode == MLOAM_GLOBAL_MAP_SURROUND) {
+    const float q[3] = {center7 ? (float)center7[0] : S.cur_pt[0], center7 ? (float)center7[1] : S.cur_pt[1], center7 ? (float)center7[2] : S.cur_pt[2]};
+    for (const auto &x : radius_hits(S, q, radius)) cand.push_back(x.second);
+  } else {
+    for (int k = 0; k < (int)S.kfs.size(); k++) cand.push_back(k);
+  }
+  if (cand.empty()) return MLOAM_OK;
+  cudaStream_t st = c->stream;
+  const int n_cand = (int)cand.size();
+  const bool merged = c->n_lidars > 1 || c->lidar_merge;
+  const int n_lasers = merged ? c->n_lidars : 1;
+  // the position filter (down_size_filter_global_map_keyframes, VoxelGridCovarianceMLOAM<PointI>(kf_leaf), :809-810): intensity = id,
+  // the last id of a voxel wins; its choice goes to the host, which lays out the association
+  float4 *d_pos, *d_ds;
+  int *d_cnt;
+  MLOAM_CUDA_OK(c, carve(G.tab, [&](Carve &cv) {
+    d_pos = cv.take<float4>(n_cand), d_ds = cv.take<float4>(n_cand + 16), d_cnt = cv.take<int>(16);
+  }));
+  std::vector<float4> h_pos(n_cand);
+  for (int i = 0; i < n_cand; i++) {
+    const KeyframeStore::Kf &k = S.kfs[cand[i]];
+    h_pos[i] = make_float4(k.pos[0], k.pos[1], k.pos[2], (float)cand[i]);
+  }
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_pos, h_pos.data(), sizeof(float4) * n_cand, cudaMemcpyHostToDevice, st));
+  int rc = voxel_downsample_device(c, d_pos, n_cand, nullptr, (float)kf_leaf, 1, d_ds, d_cnt, G.voxel);
+  if (rc) return rc;
+  int *hc = c->pinned->counts;
+  std::vector<float4> h_ds(n_cand);
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_ds.data(), d_ds, sizeof(float4) * n_cand, cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  const int n_ch = std::max(0, std::min(hc[0], n_cand));
+  for (int i = 0; i < n_ch; i++) chosen.push_back((int)h_ds[i].w);
+  // per chosen keyframe in filter order (:814-828 / :866-881): cloudUCTAssociateToMap of each cloud with the keyframe's pose and
+  // covariance and the context's current extrinsics and covariances (as mloam_keyframe_submap).  pubGlobalMap appends surf then
+  // corner to one map; saveGlobalMap appends surf to the surf map and corner to the corner map.  The outlier clouds the reference
+  // appends after surf (and after corner in pubGlobalMap) are not stored, i.e. empty.
+  const int n_maps = mode == MLOAM_GLOBAL_MAP_SURROUND ? 1 : 2;
+  std::vector<UctSeg> segs;
+  int seg_n[2] = {0, 0};
+  size_t tot[2] = {0, 0};
+  for (int m = 0; m < n_maps; m++)
+    for (int i = 0; i < n_ch; i++) {
+      const KeyframeStore::Kf &k = S.kfs[chosen[i]];
+      const KfRecord rec = kf_record(S.chunks[k.chunk].p + k.off, k.n);
+      for (int t = 0; t < 2; t++) {
+        if ((n_maps == 2 && t != m) || k.n[t] == 0) continue;
+        if (tot[m] + (size_t)k.n[t] > 0x7fffff00ull) return fail(c, MLOAM_E_INVALID, "global_map: more than 2^31 map points");
+        segs.push_back(UctSeg{rec.pts[t], (int)tot[m], k.n[t], i});
+        tot[m] += (size_t)k.n[t], seg_n[m]++;
+      }
+    }
+  std::vector<double> h_kpose(7 * (size_t)n_ch);
+  std::vector<UctLaser> h_las;
+  std::vector<double> ext7(7 * (size_t)n_lasers), pc(7 * (size_t)n_lasers), cc(36 * (size_t)n_lasers);
+  const double zero36[36] = {0};
+  for (int l = 0; l < n_lasers; l++) memcpy(&ext7[7 * l], merged ? c->lidar_ext[l] : c->ext, 7 * sizeof(double));
+  for (int i = 0; i < n_ch; i++) {
+    const KeyframeStore::Kf &k = S.kfs[chosen[i]];
+    memcpy(&h_kpose[7 * (size_t)i], k.pose, sizeof(k.pose));
+    for (int l = 0; l < n_lasers; l++)
+      mloam_compound_pose_cov(k.pose, k.cov, &ext7[7 * l], c->with_ua ? c->ua_ext_cov[l] : zero36, &pc[7 * l], &cc[36 * l]);
+    std::vector<UctLaser> one;
+    fill_lasers(n_lasers, ext7.data(), pc.data(), cc.data(), one);
+    h_las.insert(h_las.end(), one.begin(), one.end());
+  }
+  UctSeg *d_seg;
+  double *d_kpose;
+  UctLaser *d_las;
+  MLOAM_CUDA_OK(c, carve(G.tab, [&](Carve &cv) {
+    d_pos = cv.take<float4>(n_cand), d_ds = cv.take<float4>(n_cand + 16), d_cnt = cv.take<int>(16);
+    d_seg = cv.take<UctSeg>(segs.size() + 1), d_kpose = cv.take<double>(h_kpose.size() + 7), d_las = cv.take<UctLaser>(h_las.size() + 1);
+  }));
+  if (!segs.empty()) MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_seg, segs.data(), sizeof(UctSeg) * segs.size(), cudaMemcpyHostToDevice, st));
+  if (n_ch) {
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_kpose, h_kpose.data(), sizeof(double) * h_kpose.size(), cudaMemcpyHostToDevice, st));
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_las, h_las.data(), sizeof(UctLaser) * h_las.size(), cudaMemcpyHostToDevice, st));
+  }
+  // one batched association per map, then VoxelGridCovarianceMLOAM<PointIWithCov>(leaf, TRACE_THRESHOLD_MAPPING) (:840-843 / :894-899),
+  // every buffer sized by this map's input
+  const int n_max = (int)std::max(tot[0], tot[1]);
+  const size_t N1 = (size_t)n_max + 16;
+  UctBufs B;
+  float4 *mp;
+  float *mc6, *mtr;
+  MLOAM_CUDA_OK(c, carve(G.assoc, [&](Carve &cv) { uct_bufs_layout(cv, n_max, &B); }));
+  MLOAM_CUDA_OK(c, carve(G.merged, [&](Carve &cv) { mp = cv.take<float4>(N1), mc6 = cv.take<float>(6 * N1), mtr = cv.take<float>(N1); }));
+  UctFrame f;
+  memset(&f, 0, sizeof(f));
+  memcpy(f.cov_meas, c->ua_cov_meas, sizeof(f.cov_meas));
+  f.trace_threshold = S.trace_thr, f.with_ua = c->with_ua ? 1 : 0, f.n_lasers = n_lasers, f.scan_frame = 0;
+  int *d_out_n[2] = {nullptr, nullptr};
+  int seg0 = 0;
+  for (int m = 0; m < n_maps; m++) {
+    const size_t M1 = tot[m] + 16;
+    float4 *op;
+    float *oc6, *otr;
+    MLOAM_CUDA_OK(c, carve(G.out[m], [&](Carve &cv) {
+      op = cv.take<float4>(M1), oc6 = cv.take<float>(6 * M1), otr = cv.take<float>(M1), d_out_n[m] = cv.take<int>(16);
+    }));
+    G.pts[m] = op, G.cov6[m] = oc6;
+    if (tot[m] == 0) {
+      MLOAM_CUDA_OK(c, cudaMemsetAsync(d_out_n[m], 0, sizeof(int), st));
+    } else {
+      rc = uct_associate_segments(c, d_seg + seg0, seg_n[m], (int)tot[m], f, d_kpose, d_las, B, mp, mc6, mtr);
+      if (rc) return rc;
+      rc = voxel_downsample_cov_device(c, mp, mc6, mtr, (int)tot[m], B.count, leaf, (float)S.trace_thr, op, oc6, otr, d_out_n[m], G.voxel);
+      if (rc) return rc;
+    }
+    seg0 += seg_n[m];
+  }
+  for (int m = 0; m < n_maps; m++) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc + m, d_out_n[m], sizeof(int), cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));  // also: the host tables above have been consumed
+  for (int m = 0; m < n_maps; m++) G.n[m] = hc[m];
+  G.chosen.swap(chosen);
+  if (n_chosen) *n_chosen = (int)G.chosen.size();
+  if (n_map0) *n_map0 = G.n[0];
+  if (n_map1) *n_map1 = G.n[1];
+  return MLOAM_OK;
+}
+
+int mloam_global_map_read(mloam_ctx_t *h, int which, mloam_point_t *h_pts, float *h_cov6, int cap, int *n) {
+  if (!h || which < 0 || which > 1) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (!c->kf) return fail(c, MLOAM_E_STATE, "global_map_read: call mloam_keyframes_init first");
+  const KeyframeStore::GlobalMap &G = c->kf->gm;
+  const int m = G.n[which];
+  if (n) *n = m;
+  if (!(h_pts || h_cov6) || m == 0) return MLOAM_OK;
+  if (m > cap) return fail(c, MLOAM_E_INVALID, "global_map_read: capacity too small (*n holds the map's size)");
+  cudaSetDevice(c->device);
+  cudaStream_t st = c->stream;
+  if (h_pts) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_pts, G.pts[which], sizeof(float4) * (size_t)m, cudaMemcpyDeviceToHost, st));
+  if (h_cov6) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_cov6, G.cov6[which], sizeof(float) * 6 * (size_t)m, cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  return MLOAM_OK;
+}
+
+int mloam_global_map_chosen(mloam_ctx_t *h, int *h_ids, int cap, int *n) {
+  if (!h) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (!c->kf) return fail(c, MLOAM_E_STATE, "global_map_chosen: call mloam_keyframes_init first");
+  const std::vector<int> &ch = c->kf->gm.chosen;
+  if (n) *n = (int)ch.size();
+  if (!h_ids) return MLOAM_OK;
+  if ((int)ch.size() > cap) return fail(c, MLOAM_E_INVALID, "global_map_chosen: capacity too small (*n holds the count)");
+  std::copy(ch.begin(), ch.end(), h_ids);
   return MLOAM_OK;
 }
 

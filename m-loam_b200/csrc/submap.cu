@@ -15,19 +15,10 @@
 
 namespace mloam {
 
-// d_f (nullable): the frame read from device memory instead of `f` (staged by a captured H2D copy, so that a replay sees new values).
-// d_n (nullable): device-side point count, n is then the launch bound; points beyond it are not kept.
-__global__ void k_uct_associate(const float4 *__restrict__ pts, int n, UctFrame f, const UctLaser *__restrict__ lasers, float4 *__restrict__ out,
-                                float *__restrict__ cov6, float *__restrict__ trace, int *__restrict__ keep, const UctFrame *__restrict__ d_f = nullptr,
-                                const int *__restrict__ d_n = nullptr) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  if (d_n && i >= *d_n) {
-    keep[i] = 0;
-    return;
-  }
-  if (d_f) f = *d_f;
-  const float4 po = pts[i];
+// One point of cloudUCTAssociateToMap: its associated point, cov_vec and trace at index i of out / cov6 / trace, and whether it passes
+// the trace gate.  pose_global: f.pose_global, or the keyframe pose of a batched run (k_uct_associate_seg).
+__device__ __forceinline__ int uct_point(const float4 po, const UctFrame &f, const double *pose_global, const UctLaser *__restrict__ lasers,
+                                         size_t i, float4 *__restrict__ out, float *__restrict__ cov6, float *__restrict__ trace) {
   int ind = (int)po.w;  // laser id in the intensity (:1143)
   ind = ind < 0 ? 0 : (ind >= f.n_lasers ? f.n_lasers - 1 : ind);
   double C[6] = {0, 0, 0, 0, 0, 0};
@@ -66,13 +57,46 @@ __global__ void k_uct_associate(const float4 *__restrict__ pts, int n, UctFrame 
   if (f.scan_frame) {
     out[i] = po;  // the scan stays in the base frame; only its covariance is attached (PointIWithCov(point_ori, cov), :385-386)
   } else {
-    const float3 pc = associate(pose_from_param(f.pose_global), po.x, po.y, po.z);  // :1152
+    const float3 pc = associate(pose_from_param(pose_global), po.x, po.y, po.z);  // :1152
     out[i] = make_float4(pc.x, pc.y, pc.z, po.w);
   }
 #pragma unroll
-  for (int k = 0; k < 6; k++) cov6[(size_t)i * 6 + k] = (float)C[k];  // updateCov (point_with_cov.hpp:187-196)
+  for (int k = 0; k < 6; k++) cov6[i * 6 + k] = (float)C[k];  // updateCov (point_with_cov.hpp:187-196)
   trace[i] = (float)(C[0] + C[3] + C[5]);
-  keep[i] = ok;
+  return ok;
+}
+
+// d_f (nullable): the frame read from device memory instead of `f` (staged by a captured H2D copy, so that a replay sees new values).
+// d_n (nullable): device-side point count, n is then the launch bound; points beyond it are not kept.
+__global__ void k_uct_associate(const float4 *__restrict__ pts, int n, UctFrame f, const UctLaser *__restrict__ lasers, float4 *__restrict__ out,
+                                float *__restrict__ cov6, float *__restrict__ trace, int *__restrict__ keep, const UctFrame *__restrict__ d_f = nullptr,
+                                const int *__restrict__ d_n = nullptr) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (d_n && i >= *d_n) {
+    keep[i] = 0;
+    return;
+  }
+  if (d_f) f = *d_f;
+  keep[i] = uct_point(pts[i], f, f.pose_global, lasers, (size_t)i, out, cov6, trace);
+}
+
+// The association of many keyframe clouds in one launch: point i of the concatenated input belongs to the last segment whose begin is
+// <= i (segments are non-empty and in output order); it is read straight from the keyframe's record and associated with that keyframe's
+// pose (kf_pose7[7 * kf]) and UctLaser block (lasers[f.n_lasers * kf]).
+__global__ void k_uct_associate_seg(const UctSeg *__restrict__ seg, int n_seg, int n, UctFrame f, const double *__restrict__ kf_pose7,
+                                    const UctLaser *__restrict__ lasers, float4 *__restrict__ out, float *__restrict__ cov6,
+                                    float *__restrict__ trace, int *__restrict__ keep) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int lo = 0, hi = n_seg - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (seg[mid].begin <= i) lo = mid;
+    else hi = mid - 1;
+  }
+  const UctSeg s = seg[lo];
+  keep[i] = uct_point(s.pts[i - s.begin], f, kf_pose7 + 7 * (size_t)s.kf, lasers + (size_t)f.n_lasers * s.kf, (size_t)i, out, cov6, trace);
 }
 
 __global__ void k_compact_cov(const float4 *__restrict__ pts, const float *__restrict__ cov6, const float *__restrict__ trace, const int *__restrict__ keep,
@@ -176,6 +200,22 @@ int uct_associate_append(Ctx *c, const float4 *d_pts, int n, const UctFrame &f, 
   k_compact_cov<<<(n + 255) / 256, 256, 0, st>>>(B.staged, B.cov6, B.trace, B.keep, B.slot, n, 0, d_total, d_out, d_cov6_out, d_trace_out);
   k_add_count<<<1, 32, 0, st>>>(d_total, B.count);
   c->launches += 3;
+  MLOAM_CUDA_OK(c, cudaGetLastError());
+  return MLOAM_OK;
+}
+
+int uct_associate_segments(Ctx *c, const UctSeg *d_seg, int n_seg, int n, const UctFrame &f, const double *d_kf_pose7, const UctLaser *d_lasers,
+                           const UctBufs &B, float4 *d_out, float *d_cov6_out, float *d_trace_out) {
+  cudaStream_t st = c->stream;
+  if (n <= 0 || n_seg <= 0) {
+    MLOAM_CUDA_OK(c, cudaMemsetAsync(B.count, 0, sizeof(int), st));
+    return MLOAM_OK;
+  }
+  k_uct_associate_seg<<<(n + 127) / 128, 128, 0, st>>>(d_seg, n_seg, n, f, d_kf_pose7, d_lasers, B.staged, B.cov6, B.trace, B.keep);
+  c->launches++;
+  scan_exclusive(c, B.keep, B.slot, n, B.tmp, B.count);
+  k_compact_cov<<<(n + 255) / 256, 256, 0, st>>>(B.staged, B.cov6, B.trace, B.keep, B.slot, n, 0, nullptr, d_out, d_cov6_out, d_trace_out);
+  c->launches++;
   MLOAM_CUDA_OK(c, cudaGetLastError());
   return MLOAM_OK;
 }
