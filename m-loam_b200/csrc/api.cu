@@ -112,6 +112,7 @@ int mloam_ctx_create(int device, const mloam_params_t *params, mloam_ctx_t **out
   cudaMemset(c->ctl.p, 0, sizeof(DevCtl));
   if (const char *e = getenv("MLOAM_DISABLE_GRAPHS")) c->use_graphs = (e[0] == '0' || e[0] == '\0') ? 1 : 0;
   if (const char *e = getenv("MLOAM_KNN_TRACE")) c->knn_trace_on = e[0] == '1';
+  if (const char *e = getenv("MLOAM_LIN_TRACE")) c->lin_trace_on = e[0] == '1';
   if (const char *e = getenv("MLOAM_KNN_MB")) {
     const int v = atoi(e);
     if (v >= 2 && v <= 4) c->knn_min_blocks = v;
@@ -143,7 +144,7 @@ void mloam_ctx_destroy(mloam_ctx_t *h) {
   }
   for (int i = 0; i < 4; i++) c->scan_pts[i].release(), c->feat_valid[i].release(), c->feat_coeff[i].release(), c->feat_nn[i].release(), c->knn_pos[i].release(), c->knn_changed[i].release(), c->knn_anchor[i].release(), c->knn_heavy[i].release();
   for (int i = 0; i < 2; i++) c->gf_work[i].release();
-  c->knn_heavy_list.release(), c->knn_trace.release(), c->knn_spec.release();
+  c->knn_heavy_list.release(), c->knn_trace.release(), c->lin_trace.release(), c->knn_spec.release();
   c->partials.release(), c->lm_state.release();
   for (DevBuf *b : {&c->sweep_in, &c->map_in[0], &c->map_in[1], &c->extract_work, &c->voxel_work, &c->voxel_corner, &c->voxel_surf,
                     &c->host_work, &c->odom_work, &c->ctl, &c->front_work, &c->front_out})
@@ -295,6 +296,16 @@ int mloam_debug_knn_trace(mloam_ctx_t *h, unsigned *out, int n_queries) {
   cudaSetDevice(h->c.device);
   if (cudaStreamSynchronize(h->c.stream) != cudaSuccess) return MLOAM_E_CUDA;
   return cudaMemcpy(out, h->c.knn_trace.p, 16 * (size_t)n_queries, cudaMemcpyDeviceToHost) == cudaSuccess ? MLOAM_OK : MLOAM_E_CUDA;
+}
+
+// Diagnosis only (not part of include/mloam_b200.h): the k_linearize phase stamps of the last solve (MLOAM_LIN_TRACE=1), `n_words`
+// 64-bit words from slot 0 on; *n_slots: the evaluations at x the solve traced.
+int mloam_debug_lin_trace(mloam_ctx_t *h, unsigned long long *out, int n_words, int *n_slots) {
+  if (!h || !out || !n_slots || n_words <= 0 || h->c.lin_trace.cap < 8 * (size_t)n_words) return MLOAM_E_INVALID;
+  cudaSetDevice(h->c.device);
+  *n_slots = h->c.lin_trace_n;
+  if (cudaStreamSynchronize(h->c.stream) != cudaSuccess) return MLOAM_E_CUDA;
+  return cudaMemcpy(out, h->c.lin_trace.p, 8 * (size_t)n_words, cudaMemcpyDeviceToHost) == cudaSuccess ? MLOAM_OK : MLOAM_E_CUDA;
 }
 
 int mloam_map_size(mloam_ctx_t *h, int slot) {

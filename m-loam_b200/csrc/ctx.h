@@ -372,6 +372,11 @@ struct Ctx {
   unsigned knn_tma_min = 8;        // kNN staging: runs of >= this many points use TMA bulk copies, shorter ones 16 B loads (MLOAM_KNN_TMA_MIN)
   DevBuf knn_trace;                // MLOAM_KNN_TRACE=1: 4 words per query of the last k_match_knn launch (diagnosis, tools/knn_micro.py)
   bool knn_trace_on = false;
+  // MLOAM_LIN_TRACE=1 (diagnosis, tools/trace_replay.py --phases): %globaltimer / clock64 stamps at the phase boundaries of
+  // k_linearize's pass 0, one slot per evaluation at x of the last solve (LIN_TRACE_SLOTS slots of LIN_TRACE_WORDS words)
+  DevBuf lin_trace;
+  bool lin_trace_on = false;
+  int lin_trace_n = 0;
   // MLOAM_STAMP=1 (diagnosis, tools/stamp_frame.py): one-thread kernels that write %globaltimer between the stages of a frame, so that
   // the stage times of a GRAPH REPLAY can be read (the event scopes of mloam_profile_enable force the stream path and add launch gaps)
   bool stamp_on = false;

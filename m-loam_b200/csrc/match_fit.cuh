@@ -21,11 +21,14 @@ __device__ __forceinline__ bool in_laser_fov(const PoseD &T, const float3 &sel) 
 }
 
 
+// Returns whether it fitted (false: the list is unchanged and valid / coeff stand).  ok_out / coeff_out (nullable) receive what it
+// stores, so that a caller that evaluates the feature next need not read it back.
 template <int K>
-__device__ __forceinline__ void fit_one(const FitSet &s, int j, const PoseD &T, float min_plane_dis, int check_fov) {
+__device__ __forceinline__ bool fit_one(const FitSet &s, int j, const PoseD &T, float min_plane_dis, int check_fov, bool *ok_out = nullptr,
+                                        float *coeff_out = nullptr) {
   // The fit depends on the map points only: with an unchanged neighbour list the previous iteration's valid / coeff
   // stand (the FOV gate depends on the pose, so it disables the shortcut).
-  if (s.changed && !check_fov && !s.changed[j]) return;
+  if (s.changed && !check_fov && !s.changed[j]) return false;
   const int *ps = s.pos + (size_t)j * K;
   bool ok = ps[0] >= 0;
   float out[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -89,6 +92,12 @@ __device__ __forceinline__ void fit_one(const FitSet &s, int j, const PoseD &T, 
 #pragma unroll
     for (int k = 0; k < K; k++) s.nn[(size_t)j * K + k] = ok ? idx[k] : -1;
   }
+  if (ok_out) {
+    *ok_out = ok;
+#pragma unroll
+    for (int k = 0; k < 6; k++) coeff_out[k] = ok ? out[k] : 0.f;
+  }
+  return true;
 }
 
 

@@ -66,6 +66,7 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool wa
   }
   rc = lm_init_state(c, pose_init7, P.max_inner, 0, d_spec);
   if (rc) return rc;
+  c->lin_trace_n = 0;  // MLOAM_LIN_TRACE: this solve's evaluations at x take the trace slots from 0 on
   LMState *st = c->lm_state.as<LMState>();
   const double *d_pose = spec ? d_spec->xc : st->x;  // where the matcher searches
   const double sinfo = map_sqrt_info(P.cov_trace);

@@ -61,14 +61,30 @@ struct LinArgs {
   // commit the choice in the tail and, with spec_publish, hand the new candidate to the next matcher
   SpecState *spec;
   int spec_publish;
+  // MLOAM_LIN_TRACE=1 only (the k_linearize<KFIT, true> instance): LIN_TRACE_BLOCK words per block of pass 0's phase stamps
+  unsigned long long *trace;
 };
 
+// Phase stamps of pass 0 (diagnosis).  Per block: for warp w, words 4w..4w+3 = [%globaltimer at entry (lane 0), ns from there to
+// the end of the feature loop (slowest lane), fit cycles (slowest lane, clock64), feature-loop cycles (slowest lane)]; then words
+// 32..35 = %globaltimer of thread 0 after the block partial is written, after the ticket, and (last block only) at the tail's
+// start and end.
+constexpr int LIN_TRACE_BLOCK = 64;
+constexpr int LIN_TRACE_SLOT = 64 * LIN_TRACE_BLOCK;  // <= 64 blocks
+constexpr int LIN_TRACE_SLOTS = 16;
+
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+
 // Loss-corrected row of one point-to-plane / point-to-line feature at pose P: returns r and scales J by sqrt(rho'(r^2)); *rho = Huber(r^2).
-__device__ __forceinline__ double map_factor_row(const PoseR &P, const FeatSetDev &fs, int i, double sqrt_info, double huber_a, double *J,
-                                                 double *rho) {
+// cf: the feature's 6 coefficients (fs.coeff + 6 i, or the fit just computed).
+__device__ __forceinline__ double map_factor_row(const PoseR &P, const FeatSetDev &fs, int i, const float (&cf)[6], double sqrt_info,
+                                                 double huber_a, double *J, double *rho) {
   const float4 pf = __ldg(fs.pts + i);
   const D3 p{(double)pf.x, (double)pf.y, (double)pf.z};
-  const float *cf = fs.coeff + (size_t)i * 6;
   const double si = fs.sinfo ? fs.sinfo[i] : sqrt_info;  // per-feature weight when mapping is uncertainty-aware
   double r;
   if (fs.is_plane) {
@@ -83,16 +99,40 @@ __device__ __forceinline__ double map_factor_row(const PoseR &P, const FeatSetDe
   for (int k = 0; k < 6; k++) J[k] = sc * J[k];
   return sc * r;
 }
+__device__ __forceinline__ double map_factor_row(const PoseR &P, const FeatSetDev &fs, int i, double sqrt_info, double huber_a, double *J,
+                                                 double *rho) {
+  float cf[6];
+#pragma unroll
+  for (int k = 0; k < 6; k++) cf[k] = fs.coeff[(size_t)i * 6 + k];
+  return map_factor_row(P, fs, i, cf, sqrt_info, huber_a, J, rho);
+}
 
 template <bool SERIAL>
 __device__ __noinline__ void lm_tail(const double *partials, int n_blocks, LMState *gst, int mode, double eig_thre, int want_eig, double *out_ne,
                                      const P2PView *p2p, double *xc_pub);
 
-template <int KFIT>
+// One offset of k_linearize's warp butterfly.  O is a template argument so that every index of v is a constant: with a loop over
+// the offsets the compiler kept v in local memory (a 256 B store and dependent reloads per thread on the way to the block partial).
+template <int O>
+__device__ __forceinline__ void butterfly_stage(double (&v)[32], int lane) {
+  const bool upper = (lane & O) != 0;
+#pragma unroll
+  for (int k = 0; k < O; k++) {
+    const double send = upper ? v[k] : v[k + O];
+    const double keep = upper ? v[k + O] : v[k];
+    v[k] = keep + __shfl_xor_sync(MLOAM_FULL_MASK, send, O);
+  }
+}
+
+template <int KFIT, bool TRACE = false>
 __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__restrict__ partials) {
   __shared__ double sm[LIN_THREADS / 32][NE_PACK];
   __shared__ bool is_last;
   __shared__ int barrier_failed;
+  unsigned long long *const tr = TRACE ? a.trace + (size_t)blockIdx.x * LIN_TRACE_BLOCK : nullptr;
+  unsigned long long t_entry = 0ull;
+  long long c_entry = 0ll, c_fit = 0ll;
+  if (TRACE) t_entry = global_ns(), c_entry = clock64();
   if (a.respect_done && a.state && a.state->done) {  // Solve already terminated: nothing to evaluate
     if (a.lm_mode != 0 && blockIdx.x == 0 && threadIdx.x == 0) a.state_rw->work[0] = 0, a.state_rw->work[1] = 0;
     return;
@@ -101,13 +141,18 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
   const unsigned gen0 = a.two_pass ? *gen : 0u;  // read before this block's ticket: the release cannot have happened yet
   // speculative schedule: the lists the last matcher wrote (half sel ^ 1) were matched at spec->xc; they are the lists at x iff
   // x is that pose bit for bit (the step was taken).  Otherwise x did not move and the lists, valid and coeff of half sel stand.
+  // Every load here is independent of the others (no short-circuit between them), so they are in flight together.
   int spec_sel = 0;
   bool spec_hit = true;
   if (a.spec) {
     spec_sel = a.spec->sel & 1;  // read as k_match_knn reads it
 #pragma unroll
-    for (int k = 0; k < 7; k++) spec_hit = spec_hit && __double_as_longlong(a.state->x[k]) == __double_as_longlong(a.spec->xc[k]);
+    for (int k = 0; k < 7; k++) spec_hit = spec_hit & (__double_as_longlong(a.state->x[k]) == __double_as_longlong(a.spec->xc[k]));
   }
+  // the device-side feature counts are written before the launch and read by both passes
+  int set_n[2];
+#pragma unroll
+  for (int s = 0; s < 2; s++) set_n[s] = s < a.n_sets ? (a.set[s].d_n ? min(a.set[s].n, *a.set[s].d_n) : a.set[s].n) : 0;
 #pragma unroll 1
   for (int pass = 0; pass < (a.two_pass ? 2 : 1); pass++) {
   double xs[7];
@@ -143,19 +188,26 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
   for (int k = 0; k < NE_PACK; k++) acc[k] = 0.0;
   for (int s = 0; s < a.n_sets; s++) {
     const FeatSetDev fs = a.set[s];
-    const int fn = fs.d_n ? min(fs.n, *fs.d_n) : fs.n;
+    const int fn = set_n[s & 1];
     // Both sets keep their features at the low indices of a much larger launch bound: the second set is handed out from
     // the last thread downwards, so that a thread evaluates one feature of either set instead of one of each.
     const int G = gridDim.x * blockDim.x, gid = blockIdx.x * blockDim.x + threadIdx.x;
     for (int i = (s & 1) ? G - 1 - gid : gid; i < fn; i += G) {
+      // valid as it stands, read before the fit so that the two loads overlap; a fit replaces it (and coeff) from registers
+      bool valid = fs.valid[i] != 0, fitted = false;
+      float fit_c[6];
       if (KFIT > 0 && pass == 0 && a.fit[s].pos && spec_hit) {  // deferred fit: this thread is the only one that touches feature i
         constexpr int KF = KFIT > 0 ? KFIT : 5;
         const PoseD T = pose_from_param(xs);
         FitSet f = a.fit[s];
         f.pos += (size_t)(spec_sel ^ 1) * f.half * KF;  // half 0 when the lists are not double-buffered (f.half == 0)
-        fit_one<KF>(f, i, T, a.fit_min_plane_dis, a.fit_check_fov);
+        const long long c0 = TRACE ? clock64() : 0ll;
+        bool fit_ok = false;
+        fitted = fit_one<KF>(f, i, T, a.fit_min_plane_dis, a.fit_check_fov, &fit_ok, fit_c);
+        if (fitted) valid = fit_ok;
+        if (TRACE) c_fit += clock64() - c0;
       }
-      if (!fs.valid[i] || (fs.mask && !fs.mask[i])) continue;
+      if (!valid || (fs.mask && !fs.mask[i])) continue;
       if (fs.is_plane == 2) {
         const float4 pf = __ldg(fs.pts + i);
         const D3 p{(double)pf.x, (double)pf.y, (double)pf.z};
@@ -187,8 +239,11 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
         else acc[NE_H + NE_G + 2] += 1.0;
         continue;
       }
+      float cf[6];
+#pragma unroll
+      for (int k = 0; k < 6; k++) cf[k] = fitted ? fit_c[k] : fs.coeff[(size_t)i * 6 + k];
       double J[6], rho;
-      const double r = map_factor_row(P, fs, i, a.sqrt_info, a.huber_a, J, &rho);
+      const double r = map_factor_row(P, fs, i, cf, a.sqrt_info, a.huber_a, J, &rho);
       int q = 0;
 #pragma unroll
       for (int i0 = 0; i0 < 6; i0++)
@@ -205,20 +260,22 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
   // keeps the half of its remaining components selected by its bit o and adds the partner's partial sums of that
   // half; after offsets 16..1 lane L holds the warp total of component L.
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (TRACE && pass == 0) {
+    const unsigned long long t0 = __shfl_sync(MLOAM_FULL_MASK, t_entry, 0);
+    const unsigned loop_ns = __reduce_max_sync(MLOAM_FULL_MASK, (unsigned)(global_ns() - t0));
+    const unsigned loop_cyc = __reduce_max_sync(MLOAM_FULL_MASK, (unsigned)(clock64() - c_entry));
+    const unsigned fit_cyc = __reduce_max_sync(MLOAM_FULL_MASK, (unsigned)c_fit);
+    if (lane == 0) tr[4 * wid] = t0, tr[4 * wid + 1] = loop_ns, tr[4 * wid + 2] = fit_cyc, tr[4 * wid + 3] = loop_cyc;
+  }
   {
     double v[32];
 #pragma unroll
     for (int k = 0; k < 32; k++) v[k] = k < NE_PACK ? acc[k] : 0.0;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const bool upper = (lane & o) != 0;
-#pragma unroll
-      for (int k = 0; k < o; k++) {
-        const double send = upper ? v[k] : v[k + o];
-        const double keep = upper ? v[k + o] : v[k];
-        v[k] = keep + __shfl_xor_sync(MLOAM_FULL_MASK, send, o);
-      }
-    }
+    butterfly_stage<16>(v, lane);
+    butterfly_stage<8>(v, lane);
+    butterfly_stage<4>(v, lane);
+    butterfly_stage<2>(v, lane);
+    butterfly_stage<1>(v, lane);
     if (lane < NE_PACK) sm[wid][lane] = v[0];
   }
   __syncthreads();
@@ -227,6 +284,7 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
 #pragma unroll
     for (int w = 0; w < LIN_THREADS / 32; w++) v += sm[w][threadIdx.x];
     partials[(size_t)blockIdx.x * NE_PACK + threadIdx.x] = v;
+    if (TRACE && pass == 0 && threadIdx.x == 0) tr[32] = global_ns();
   }
   if (a.lm_mode == 0) return;
   // ---- fused tail: the last block to arrive sums the partials in block order (so the result does not depend on
@@ -235,6 +293,7 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
   __syncthreads();
   if (threadIdx.x == 0) is_last = atomicAdd(a.ticket, 1u) == gridDim.x - 1;
   __syncthreads();
+  if (TRACE && pass == 0 && threadIdx.x == 0) tr[33] = global_ns(), tr[34] = 0ull, tr[35] = 0ull;
   if (!is_last) {
     if (a.two_pass && pass == 0) continue;  // on to the barrier of pass 1
     return;
@@ -244,11 +303,13 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
   {
     const int mode = pass == 0 ? a.lm_mode : 2, want_eig = pass == 0 ? a.want_eig : 1;
     double *const xc_pub = (a.spec && a.spec_publish && pass == 0) ? a.spec->xc : nullptr;
+    if (TRACE && pass == 0 && threadIdx.x == 0) tr[34] = global_ns();
     if (a.lm_serial) lm_tail<true>(partials, (int)gridDim.x, a.state_rw, mode, a.eig_thre, want_eig, nullptr, a.p2p, xc_pub);
     else lm_tail<false>(partials, (int)gridDim.x, a.state_rw, mode, a.eig_thre, want_eig, nullptr, a.p2p, xc_pub);
   }
   __threadfence();  // the state (written by all threads of this block) before the ticket reset and the release
   __syncthreads();
+  if (TRACE && pass == 0 && threadIdx.x == 0) tr[35] = global_ns();
   if (threadIdx.x == 0) {
     if (a.spec && pass == 0 && spec_hit) a.spec->sel = spec_sel ^ 1;  // every block has read sel and fitted: commit
     *a.ticket = 0u;
@@ -1265,11 +1326,27 @@ int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, 
     a.fit[0] = o.fit->set[0], a.fit[1] = o.fit->set[1];
     a.fit_min_plane_dis = o.fit->min_plane_dis, a.fit_check_fov = o.fit->check_fov;
   }
+  // phase stamps of the evaluations at x of a fused solve, one slot each (scan2map_enqueue restarts the count)
+  if (c->lin_trace_on && fused && lm_mode == 1 && c->lin_trace_n < LIN_TRACE_SLOTS) {
+    const size_t bytes = sizeof(unsigned long long) * LIN_TRACE_SLOT * LIN_TRACE_SLOTS;
+    if (c->lin_trace.cap < bytes) {
+      MLOAM_CUDA_OK(c, c->lin_trace.reserve(bytes));
+      MLOAM_CUDA_OK(c, cudaMemsetAsync(c->lin_trace.p, 0, c->lin_trace.cap, c->stream));
+    }
+    a.trace = c->lin_trace.as<unsigned long long>() + (size_t)LIN_TRACE_SLOT * c->lin_trace_n++;
+  }
   {
     ProfScope ps(c, "linearize");
-    if (kfit == 5) k_linearize<5><<<nb, LIN_THREADS, 0, c->stream>>>(a, c->partials.as<double>());
-    else if (kfit == 10) k_linearize<10><<<nb, LIN_THREADS, 0, c->stream>>>(a, c->partials.as<double>());
-    else k_linearize<0><<<nb, LIN_THREADS, 0, c->stream>>>(a, c->partials.as<double>());
+    double *const pt = c->partials.as<double>();
+    if (a.trace) {
+      if (kfit == 5) k_linearize<5, true><<<nb, LIN_THREADS, 0, c->stream>>>(a, pt);
+      else if (kfit == 10) k_linearize<10, true><<<nb, LIN_THREADS, 0, c->stream>>>(a, pt);
+      else k_linearize<0, true><<<nb, LIN_THREADS, 0, c->stream>>>(a, pt);
+    } else {
+      if (kfit == 5) k_linearize<5><<<nb, LIN_THREADS, 0, c->stream>>>(a, pt);
+      else if (kfit == 10) k_linearize<10><<<nb, LIN_THREADS, 0, c->stream>>>(a, pt);
+      else k_linearize<0><<<nb, LIN_THREADS, 0, c->stream>>>(a, pt);
+    }
     c->launches++;
   }
   if (fused) {

@@ -2,10 +2,16 @@
 """Kernel timeline of graph-replayed C2 frames (64 x 2048 sweep, 1M-point keyframe submap, 10 GN iterations, inputs resident on
 the device as in bench.py) with torch.profiler: device time per kernel and frame, and how much of each candidate evaluation
 (k_eval_candidate) runs while the speculative matcher (k_match_knn) of the next GN iteration is running.
-  python tools/trace_replay.py OUT_DIR [frames]      (writes OUT_DIR/replay.pt.trace.json)"""
+  python tools/trace_replay.py OUT_DIR [frames] [--phases]      (writes OUT_DIR/replay.pt.trace.json)
+--phases: afterwards, the same frames on a second context with MLOAM_LIN_TRACE=1 (no profiler): the phase split of k_linearize's
+pass 0 per GN iteration from %globaltimer / clock64 stamps inside the kernel (feature loop = fit + evaluation, block reduction,
+ticket, LM tail)."""
+import ctypes as C
 import json
 import os
 import sys
+
+import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -14,9 +20,28 @@ import bench  # noqa: E402
 import synthetic as syn  # noqa: E402
 
 
+LIN_TRACE_BLOCK, LIN_TRACE_SLOT = 64, 64 * 64  # solve_kernels.cu
+
+
+def phases(tr):
+    """One traced k_linearize pass 0 (LIN_TRACE_SLOT words) -> phase boundaries [us] from the first warp's entry."""
+    blk = tr.reshape(64, LIN_TRACE_BLOCK)
+    blk = blk[blk[:, 0] != 0]
+    warps = blk[:, :32].reshape(-1, 4).astype(np.int64)  # [entry, loop ns, fit cycles, loop cycles] per warp
+    t0 = int(warps[:, 0].min())
+    loop_end = int((warps[:, 0] + warps[:, 1]).max())
+    fit_share = float(np.mean(warps[:, 2] / np.maximum(warps[:, 3], 1)))  # of a warp's feature-loop cycles
+    last = blk[blk[:, 34] != 0]
+    us = lambda t: (int(t) - t0) / 1000.0  # noqa: E731
+    return {"blocks": len(blk), "loop_end": us(loop_end), "fit_share": fit_share, "reduced": us(blk[:, 32].max()),
+            "ticket": us(last[0, 33]) if len(last) else float("nan"), "tail_start": us(last[0, 34]) if len(last) else float("nan"),
+            "tail_end": us(last[0, 35]) if len(last) else float("nan")}
+
+
 def main():
-    out = sys.argv[1]
-    n_frames = int(sys.argv[2]) if len(sys.argv) > 2 else 5
+    args = [a for a in sys.argv[1:] if not a.startswith("--")]
+    out = args[0]
+    n_frames = int(args[1]) if len(args) > 1 else 5
     import torch
     from torch.profiler import ProfilerActivity, profile
 
@@ -70,10 +95,45 @@ def main():
           f"{100.0 * both / tc if tc else 0.0:.1f} % of its time next to a running k_match_knn")
     print(f"k_match_knn: {sum(b - a for a, b in knn) / max(1, len(knn)):.1f} us each; "
           f"k_linearize: {sum(b - a for a, b in lin) / max(1, len(lin)):.1f} us each")
+    per_frame = len(lin) // n_frames  # the last k_linearize of a frame runs both passes, the others pass 0 only
+    if per_frame > 1:
+        lin.sort()
+        two = [lin[f * per_frame + per_frame - 1] for f in range(n_frames)]
+        one = [x for k, x in enumerate(lin) if k % per_frame != per_frame - 1]
+        print(f"k_linearize pass 0 only: {sum(b - a for a, b in one) / len(one):.1f} us each; "
+              f"two-pass (last GN iteration): {sum(b - a for a, b in two) / len(two):.1f} us each")
     starts = sorted(e["ts"] for e in ev)
     ends = sorted(e["ts"] + e["dur"] for e in ev)
     print(f"first kernel to last kernel: {(ends[-1] - starts[0]) / n_frames:.1f} us per frame")
     ctx.close()
+    if "--phases" not in sys.argv:
+        return
+    os.environ["MLOAM_LIN_TRACE"] = "1"  # read at context creation
+    ctx = m.Context(0, p)
+    step(True)
+    for _ in range(4):
+        step(False)
+    rows = []
+    buf = np.zeros(16 * LIN_TRACE_SLOT, dtype=np.uint64)
+    for _ in range(n_frames):
+        step(False)
+        n_slots = C.c_int(0)
+        rc = m.lib().mloam_debug_lin_trace(ctx._h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n_slots))
+        assert rc == 0, rc
+        rows.append([phases(buf[s * LIN_TRACE_SLOT:(s + 1) * LIN_TRACE_SLOT]) for s in range(n_slots.value)])
+    ctx.close()
+    keys = ["loop_end", "reduced", "ticket", "tail_start", "tail_end"]
+    print(f"k_linearize pass 0 phase boundaries, us from the first warp's entry, mean of {n_frames} replayed frames "
+          f"({rows[0][0]['blocks']} blocks); fit = share of the feature loop's cycles spent in fit_one")
+    print(f"  {'GN it':>5s} " + " ".join(f"{k:>10s}" for k in keys) + f" {'fit share':>10s}")
+    for s in range(len(rows[0])):
+        mean = {k: float(np.mean([r[s][k] for r in rows])) for k in keys + ["fit_share"]}
+        print(f"  {s:5d} " + " ".join(f"{mean[k]:10.2f}" for k in keys) + f" {mean['fit_share']:10.2f}")
+    spec = [r[s] for r in rows for s in range(len(r) - 1)]
+    if spec:
+        mean = {k: float(np.mean([x[k] for x in spec])) for k in keys + ["fit_share"]}
+        print("  speculative iterations (all but the last): " + ", ".join(f"{k} {mean[k]:.2f}" for k in keys) +
+              f", fit share {mean['fit_share']:.2f}")
 
 
 if __name__ == "__main__":
