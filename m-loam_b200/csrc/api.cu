@@ -121,6 +121,7 @@ int mloam_ctx_create(int device, const mloam_params_t *params, mloam_ctx_t **out
   if (const char *e = getenv("MLOAM_LOOKAHEAD")) c->use_lookahead = (e[0] == '0') ? 0 : 1;
   if (const char *e = getenv("MLOAM_STAMP")) c->stamp_on = e[0] == '1';
   if (const char *e = getenv("MLOAM_FUSE_ITER")) c->fuse_iter = (e[0] == '0') ? 0 : 1;
+  if (const char *e = getenv("MLOAM_PDL")) c->use_pdl = (e[0] == '0') ? 0 : 1;
   if (const char *e = getenv("MLOAM_LM_TAIL")) c->lm_tail_serial = strcmp(e, "serial") == 0 ? 1 : 0;
   if (const char *e = getenv("MLOAM_DISABLE_SEEDS")) c->use_seeds = (e[0] == '0' || e[0] == '\0') ? 1 : 0;
   *out = h;
@@ -292,10 +293,27 @@ const char *mloam_debug_stamp_label(mloam_ctx_t *h, int i) {
 
 // Diagnosis only (not part of include/mloam_b200.h): per-query words of the last traced k_match_knn launch.
 int mloam_debug_knn_trace(mloam_ctx_t *h, unsigned *out, int n_queries) {
-  if (!h || !out || n_queries <= 0 || h->c.knn_trace.cap < 16 * (size_t)n_queries) return MLOAM_E_INVALID;  // n_queries may include the timeline tail
-  cudaSetDevice(h->c.device);
-  if (cudaStreamSynchronize(h->c.stream) != cudaSuccess) return MLOAM_E_CUDA;
-  return cudaMemcpy(out, h->c.knn_trace.p, 16 * (size_t)n_queries, cudaMemcpyDeviceToHost) == cudaSuccess ? MLOAM_OK : MLOAM_E_CUDA;
+  const Ctx *c = h ? &h->c : nullptr;
+  if (!c || !out || n_queries <= 0 || c->knn_trace_n <= 0 || c->knn_trace_slot < 16 * (size_t)n_queries)  // n_queries may include the timeline tail
+    return MLOAM_E_INVALID;
+  cudaSetDevice(c->device);
+  if (cudaStreamSynchronize(c->stream) != cudaSuccess) return MLOAM_E_CUDA;
+  const unsigned char *slot = c->knn_trace.as<unsigned char>() + c->knn_trace_slot * (size_t)(c->knn_trace_n - 1);
+  return cudaMemcpy(out, slot, 16 * (size_t)n_queries, cudaMemcpyDeviceToHost) == cudaSuccess ? MLOAM_OK : MLOAM_E_CUDA;
+}
+
+// Diagnosis only (not part of include/mloam_b200.h): the per-warp [enter, exit] %globaltimer pairs of traced k_match_knn launch `slot`
+// of the last solve (MLOAM_KNN_TRACE=1), `n_pairs` of them (zeros for warps the launch did not have); *n_slots: the launches traced.
+int mloam_debug_knn_timeline(mloam_ctx_t *h, int slot, unsigned long long *out, int n_pairs, int *n_slots) {
+  const Ctx *c = h ? &h->c : nullptr;
+  if (!c || !out || !n_slots || slot < 0 || slot >= KNN_TRACE_SLOTS || n_pairs <= 0 ||
+      c->knn_trace_slot - c->knn_trace_timeline < 16 * (size_t)n_pairs)
+    return MLOAM_E_INVALID;
+  cudaSetDevice(c->device);
+  *n_slots = c->knn_trace_n;
+  if (cudaStreamSynchronize(c->stream) != cudaSuccess) return MLOAM_E_CUDA;
+  const unsigned char *tl = c->knn_trace.as<unsigned char>() + c->knn_trace_slot * (size_t)slot + c->knn_trace_timeline;
+  return cudaMemcpy(out, tl, 16 * (size_t)n_pairs, cudaMemcpyDeviceToHost) == cudaSuccess ? MLOAM_OK : MLOAM_E_CUDA;
 }
 
 // Diagnosis only (not part of include/mloam_b200.h): the k_linearize phase stamps of the last solve (MLOAM_LIN_TRACE=1), `n_words`
@@ -306,6 +324,15 @@ int mloam_debug_lin_trace(mloam_ctx_t *h, unsigned long long *out, int n_words, 
   *n_slots = h->c.lin_trace_n;
   if (cudaStreamSynchronize(h->c.stream) != cudaSuccess) return MLOAM_E_CUDA;
   return cudaMemcpy(out, h->c.lin_trace.p, 8 * (size_t)n_words, cudaMemcpyDeviceToHost) == cudaSuccess ? MLOAM_OK : MLOAM_E_CUDA;
+}
+
+// Diagnosis only (not part of include/mloam_b200.h): the programmatic edges (programmatic dependent launch along the GN chain) of the
+// last instantiated frame graph, and whether the last frame ran from a frame graph.
+int mloam_debug_pdl(mloam_ctx_t *h, int *prog_edges, int *from_graph) {
+  if (!h || !prog_edges || !from_graph) return MLOAM_E_INVALID;
+  *prog_edges = h->c.graph_pdl_edges;
+  *from_graph = h->c.frame_from_graph ? 1 : 0;
+  return MLOAM_OK;
 }
 
 int mloam_map_size(mloam_ctx_t *h, int slot) {

@@ -32,6 +32,24 @@ struct FitSet {
   int is_plane;
   const unsigned char *changed;  // nullable: 0 -> same neighbours as the previous iteration, valid/coeff already hold the fit
 };
+constexpr int KNN_TRACE_SLOTS = 16;  // MLOAM_KNN_TRACE=1: traced k_match_knn launches per solve (Ctx::knn_trace)
+
+// Launch of a kernel of the single-GPU scan2map GN chain.  pdl: programmatic dependent launch (programmatic stream serialisation; a
+// programmatic edge in a captured graph) — the kernel's CTAs are placed and run their prologue while the kernel before it on the stream
+// finishes.  Every kernel launched so executes cudaGridDependencySynchronize before its first read of anything the kernels before it
+// write, and none triggers its dependents before that wait, so everything two or more launches back is complete when a kernel starts.
+// !pdl: an ordinary launch (stage profiling, multi-GPU, MLOAM_PDL=0).
+template <typename... P, typename... A>
+cudaError_t launch_chain(bool pdl, void (*kernel)(P...), unsigned grid, unsigned block, cudaStream_t st, A &&...args) {
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid), cfg.blockDim = dim3(block), cfg.dynamicSmemBytes = 0, cfg.stream = st;
+  cfg.attrs = &attr, cfg.numAttrs = pdl ? 1 : 0;
+  return cudaLaunchKernelEx(&cfg, kernel, static_cast<A &&>(args)...);
+}
+
 // Speculative re-association (plain scan2map, max_inner == 1, one GPU): the matcher of GN iteration i + 1 searches at the
 // candidate pose of iteration i while that candidate is evaluated.  The neighbour lists and anchors are double-buffered; the
 // matcher reads half `sel` and writes the other one.  The next evaluation at x decides on the device which half is valid:
@@ -58,6 +76,7 @@ struct LinOpts {
   SpecState *spec = nullptr;        // speculative schedule (lm_mode 1): commit the speculation ...
   bool spec_publish = false;        // ... and publish the new candidate for the next matcher
   const PendingFit *fit = nullptr;  // the fit the matcher deferred to this evaluation (lm_mode 1)
+  bool pdl = false;                 // launch_chain: programmatic dependent launch (single-GPU scan2map chain)
 };
 
 // Grow-only device buffer (cudaMalloc only when capacity is exceeded; steady-state frames allocate nothing).
@@ -370,8 +389,12 @@ struct Ctx {
   long long graph_capture_failures = 0;  // frames that fell back to the stream path because their capture failed (mloam_profile_get "graph_capture_failures")
   int use_graphs = 1;
   unsigned knn_tma_min = 8;        // kNN staging: runs of >= this many points use TMA bulk copies, shorter ones 16 B loads (MLOAM_KNN_TMA_MIN)
-  DevBuf knn_trace;                // MLOAM_KNN_TRACE=1: 4 words per query of the last k_match_knn launch (diagnosis, tools/knn_micro.py)
+  // MLOAM_KNN_TRACE=1 (diagnosis, tools/knn_micro.py, tools/trace_replay.py --phases): per k_match_knn launch of the last solve
+  // (KNN_TRACE_SLOTS slots of knn_trace_slot bytes) 4 words per query, then the per-warp [enter, exit] %globaltimer timeline
+  DevBuf knn_trace;
   bool knn_trace_on = false;
+  int knn_trace_n = 0;             // slots written since the last solve began
+  size_t knn_trace_slot = 0, knn_trace_timeline = 0;  // bytes per slot; where in a slot the timeline begins
   // MLOAM_LIN_TRACE=1 (diagnosis, tools/trace_replay.py --phases): %globaltimer / clock64 stamps at the phase boundaries of
   // k_linearize's pass 0, one slot per evaluation at x of the last solve (LIN_TRACE_SLOTS slots of LIN_TRACE_WORDS words)
   DevBuf lin_trace;
@@ -388,6 +411,10 @@ struct Ctx {
   int fuse_iter = 1;               // scan2map: fit inside the first evaluation + both evaluations of an LM iteration in ONE launch
                                    // (grid barrier between them); MLOAM_FUSE_ITER=0 restores the three launches
   int lm_tail_serial = 0;          // the LM step on one thread of the tail block (MLOAM_LM_TAIL=serial) instead of one warp; bit-identical
+  int use_pdl = 1;                 // scan2map's GN chain with programmatic dependent launch (launch_chain); MLOAM_PDL=0: ordinary launches,
+                                   // the reference the tests compare against
+  int graph_pdl_edges = 0;         // programmatic edges of the last instantiated frame graph (mloam_debug_pdl)
+  bool frame_from_graph = false;   // the last frame ran from a frame graph
   bool lidar_merge = false;        // mloam_set_lidars was given extrinsics: features go through the rig merge (also for one LiDAR)
   int n_lidars = 1;                // LiDARs batched into one frame of this context (mloam_set_lidars)
   double lidar_ext[MLOAM_MAX_LIDARS][7];  // their sensor -> base extrinsics
@@ -467,8 +494,9 @@ struct MatchJob {
 // defer (nullable): skip the fit launch and write the fit into *defer for the caller's next linearize_device(lm_mode 1) (LinOpts::fit);
 // defer->K == 0 when the fit was launched here (a job wants neighbour indices) or nothing was matched.  nullptr: fit now.
 // d_sel (speculative schedule, with defer): double-buffered lists, read half *d_sel and write the other (SpecState::sel)
+// pdl: the kNN launch is a link of scan2map's GN chain (launch_chain)
 int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_pose7, const MatchCfg &cfg, int buf_base = 0,
-                      PendingFit *defer = nullptr, const int *d_sel = nullptr);
+                      PendingFit *defer = nullptr, const int *d_sel = nullptr, bool pdl = false);
 
 // track_kernels.cu
 int match_from_scan_device(Ctx *c, int slot, int type, const float4 *d_pts, int n, const double *d_pose7, unsigned char *d_valid,
@@ -497,9 +525,10 @@ int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, 
 // Evaluation at LMState::xc + the acceptance step (mode 2) of a solve with max_inner == 1, as the second pass of
 // k_linearize computes it, but accumulating only g, cost and row counts (H at xc is never read with one LM iteration).
 // Small blocks with a register cap, so that it runs beside the speculative matcher of the next GN iteration.
-int eval_candidate_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, double eig_thre);
-// min_corr: minimum matched features for a Solve (tracker: 10); spec (nullable): also start SpecState::xc at the initial pose
-int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, int min_corr, SpecState *spec = nullptr);
+int eval_candidate_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, double eig_thre, bool pdl);
+// min_corr: minimum matched features for a Solve (tracker: 10); spec (nullable): also start SpecState::xc at the initial pose;
+// pdl: launch_chain
+int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, int min_corr, SpecState *spec = nullptr, bool pdl = false);
 void eig_report_host(const double *H36, double *w6);  // ascending eigenvalues of a symmetric 6x6 (host side)
 int factor_evaluate_device(Ctx *c, int kind, int n, const double *d_points, const double *d_coeffs, const double *d_sqrt_info,
                            const double *d_params, double *d_res, double *d_jac);
@@ -524,7 +553,7 @@ void stage_pose(Ctx *c, const double *pose7);
 void stage_ext(Ctx *c);
 void stage_rig(Ctx *c);
 // solve_kernels.cu: Ctx::pose_cov <- LMState::H^-1 (partial-pivot LU), zeros when the last evaluation had no residual rows
-int pose_cov_device(Ctx *c);
+int pose_cov_device(Ctx *c, bool pdl);
 // keyframe.cu: frees the keyframe store (mloam_ctx_destroy)
 void keyframes_release(Ctx *c);
 

@@ -64,29 +64,38 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
   __shared__ KnnSmem ksm[MWARPS];
   const int lane = threadIdx.x & 31;
   KnnSmem &ks = ksm[threadIdx.x >> 5];
-  unsigned long long t_enter = 0ull;
-  if (trace) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_enter));
+  // Prologue: nothing here reads what the kernel before this one on the GN chain (k_linearize) writes.  The maps and the device
+  // feature counts were built before the solve; the heavy list and its count were written by the previous matcher, which is two
+  // launches back and complete (no kernel of the chain triggers its dependents before its own grid-dependency wait).
   knn_smem_init(ks, lane, tma_min);
   __shared__ GridP s_grid[2];
   __shared__ PoseD s_pose;
-  if (threadIdx.x == 0) s_grid[0] = load_grid(a.map), s_grid[1] = load_grid(b.map), s_pose = pose_from_param(pose7);
-  __syncthreads();
+  if (threadIdx.x == 0) s_grid[0] = load_grid(a.map), s_grid[1] = load_grid(b.map);
   const int na = a.d_n ? min(a.n, *a.d_n) : a.n;
   const int nb = b.d_n ? min(b.n, *b.d_n) : b.n;
   const int n = na + nb;
-  const int h_in = d_sel ? (*d_sel & 1) : 0;  // double-buffered sets: read half h_in, write the other
   // Schedule: first the listed heavy features of the previous launch (one per warp), then a static stride over the rest.
   const int gw = blockIdx.x * MWARPS + (threadIdx.x >> 5), n_warps = gridDim.x * MWARPS;
-  if (hq.cnt_zero && gw == 0 && lane == 0) *hq.cnt_zero = 0;
   const bool listed = hq.list_in != nullptr;
   const int n_heavy = listed ? min(__ldg(hq.cnt_in), n) : 0;
   const int it_a = n_heavy > gw ? (n_heavy - gw + n_warps - 1) / n_warps : 0;
   const int it_b = n > gw ? (n - gw + n_warps - 1) / n_warps : 0;
+  const int first_listed = it_a > 0 ? __ldg(hq.list_in + gw) : 0;
+  // Programmatic dependent launch: the pose searched at (SpecState::xc, published by k_linearize's tail), d_sel (committed there)
+  // and the lists, anchors, changed flags and fit inputs k_linearize reads are only touched after the previous kernel completed
+  cudaGridDependencySynchronize();
+  cudaTriggerProgrammaticLaunchCompletion();
+  unsigned long long t_enter = 0ull;
+  if (trace) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_enter));
+  if (threadIdx.x == 0) s_pose = pose_from_param(pose7);
+  __syncthreads();
+  const int h_in = d_sel ? (*d_sel & 1) : 0;  // double-buffered sets: read half h_in, write the other
+  if (hq.cnt_zero && gw == 0 && lane == 0) *hq.cnt_zero = 0;
 #pragma unroll 1
   for (int it = 0; it < it_a + it_b; it++) {
     int i;
     if (it < it_a) {
-      i = __ldg(hq.list_in + gw + it * n_warps);
+      i = it == 0 ? first_listed : __ldg(hq.list_in + gw + it * n_warps);
     } else {
       i = gw + (it - it_a) * n_warps;
       if (listed) {  // listed ones have been done above
@@ -259,7 +268,7 @@ __global__ void __launch_bounds__(128) k_match_fit(FitSet a, FitSet b, const dou
 // Match up to two feature sets (corner against MLOAM_MAP_CORNER-like slot, surf against a surf slot) in one
 // kNN launch + one fit launch.  Sets with n == 0 are skipped.
 int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_pose7, const MatchCfg &cfg, int buf_base, PendingFit *defer,
-                      const int *d_sel) {
+                      const int *d_sel, bool pdl) {
   if (defer) defer->K = 0;
   if (n_jobs < 1 || n_jobs > 2 || (buf_base != 0 && buf_base != 2)) {
     c->err = "match: 1 or 2 jobs";
@@ -345,27 +354,27 @@ int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_
     ProfScope ps(c, "match");
     // with stage profiling on: how many queries took the keep (matched / rejected), ball and blind paths
     unsigned *path_stats = (c->prof_on && !getenv("MLOAM_KNN_NO_STATS")) ? reinterpret_cast<unsigned *>(&c->ctl.as<DevCtl>()->knn_stats) : nullptr;
+    // one trace slot per launch of a solve: the launch that starts it clears them all, so that no clear sits between the launches of
+    // the GN chain
     unsigned *trace = nullptr;
     if (c->knn_trace_on) {
-      MLOAM_CUDA_OK(c, c->knn_trace.reserve(16 * (size_t)(n_upper + 1) + 16 * (size_t)MWARPS * 4 * c->sm_count + 64));
-      MLOAM_CUDA_OK(c, cudaMemsetAsync(c->knn_trace.p, 0, 16 * (size_t)(n_upper + 1) + 16 * (size_t)MWARPS * 4 * c->sm_count, st));
-      trace = c->knn_trace.as<unsigned>();
+      const size_t slot = 16 * (size_t)(n_upper + 1) + 16 * (size_t)MWARPS * 4 * c->sm_count;
+      if (!flip || slot != c->knn_trace_slot) {
+        MLOAM_CUDA_OK(c, c->knn_trace.reserve(slot * KNN_TRACE_SLOTS));
+        MLOAM_CUDA_OK(c, cudaMemsetAsync(c->knn_trace.p, 0, slot * KNN_TRACE_SLOTS, st));
+        c->knn_trace_slot = slot, c->knn_trace_timeline = 16 * (size_t)(n_upper + 1), c->knn_trace_n = 0;
+      }
+      const int s = c->knn_trace_n < KNN_TRACE_SLOTS ? c->knn_trace_n++ : KNN_TRACE_SLOTS - 1;
+      trace = reinterpret_cast<unsigned *>(c->knn_trace.as<unsigned char>() + slot * (size_t)s);
     }
     const int mb = c->knn_min_blocks;
     int nb = (n_upper + MWARPS - 1) / MWARPS;
     if (nb > mb * c->sm_count) nb = mb * c->sm_count;  // all CTAs resident; warps pull / stride over the features
-#define MLOAM_LAUNCH_KNN(KK, MBB) \
-  k_match_knn<KK, MBB><<<nb, MWARPS * 32, 0, st>>>(ks[0], ks[1], d_pose7, cfg.min_match_sq_dis, hq, d_sel, path_stats, c->knn_tma_min, trace)
-    if (K == 5) {
-      if (mb == 2) MLOAM_LAUNCH_KNN(5, 2);
-      else if (mb == 3) MLOAM_LAUNCH_KNN(5, 3);
-      else MLOAM_LAUNCH_KNN(5, 4);
-    } else {
-      if (mb == 2) MLOAM_LAUNCH_KNN(10, 2);
-      else if (mb == 3) MLOAM_LAUNCH_KNN(10, 3);
-      else MLOAM_LAUNCH_KNN(10, 4);
-    }
-#undef MLOAM_LAUNCH_KNN
+    void (*k)(KnnSet, KnnSet, const double *, float, HeavyQ, const int *, unsigned *, unsigned, unsigned *);
+    if (K == 5) k = mb == 2 ? k_match_knn<5, 2> : (mb == 3 ? k_match_knn<5, 3> : k_match_knn<5, 4>);
+    else k = mb == 2 ? k_match_knn<10, 2> : (mb == 3 ? k_match_knn<10, 3> : k_match_knn<10, 4>);
+    MLOAM_CUDA_OK(c, launch_chain(pdl, k, nb, MWARPS * 32, st, ks[0], ks[1], d_pose7, cfg.min_match_sq_dis, hq, d_sel, path_stats,
+                                  c->knn_tma_min, trace));
     c->launches++;
   }
   if (defer && !fs[0].nn && !fs[1].nn) {

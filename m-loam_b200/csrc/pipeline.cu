@@ -64,7 +64,11 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool wa
     MLOAM_CUDA_OK(c, c->knn_spec.reserve(sizeof(SpecState)));
     d_spec = c->knn_spec.as<SpecState>();
   }
-  rc = lm_init_state(c, pose_init7, P.max_inner, 0, d_spec);
+  // programmatic dependent launch along the chain (launch_chain); the event scopes of stage profiling sit between the kernels, and
+  // multi-GPU keeps its NCCL calls and peer-memory flags between ordinary launches
+  const bool pdl = c->use_pdl && !c->prof_on && !c->nccl_comm && !c->p2p_on;
+  first.pdl = iter.pdl = pdl;
+  rc = lm_init_state(c, pose_init7, P.max_inner, 0, d_spec, pdl);
   if (rc) return rc;
   c->lin_trace_n = 0;  // MLOAM_LIN_TRACE: this solve's evaluations at x take the trace slots from 0 on
   LMState *st = c->lm_state.as<LMState>();
@@ -91,7 +95,7 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool wa
                  c->feat_coeff[0].as<float>(), nullptr, seeded},
         MatchJob{MLOAM_MAP_SURF, 's', S.surf, ns_use, S.d_n_surf, c->feat_valid[1].as<unsigned char>(),
                  c->feat_coeff[1].as<float>(), nullptr, seeded}};
-    return match_pair_device(c, jobs, 2, d_pose, cfg, 0, defer_fit ? &pending : nullptr, spec ? &d_spec->sel : nullptr);
+    return match_pair_device(c, jobs, 2, d_pose, cfg, 0, defer_fit ? &pending : nullptr, spec ? &d_spec->sel : nullptr, pdl);
   };
   for (int outer = 0; outer < P.max_outer; outer++) {
     if (!spec || outer == 0) {  // speculative: the previous iteration enqueued this one's matcher
@@ -129,13 +133,15 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool wa
     if (rc) return rc;
     stamp(c, second_done ? "linearize x2" : "linearize");
     if (speculate) {
-      // fork: {matcher of iteration outer + 1 at the published candidate} || {evaluation at the candidate + acceptance}.  The
-      // branches share only read-only inputs: the matcher writes the spare half of the lists, the changed and heavy flags; the
-      // evaluation writes LMState and the partials.  With stage profiling on they stay serial, like the other forks.
+      // fork: {evaluation at the candidate + acceptance} on the side branch || {matcher of iteration outer + 1 at the published
+      // candidate} on the main stream, right behind k_linearize, so that the critical path k_linearize -> k_match_knn -> k_linearize
+      // is one stream (programmatic edges with pdl).  The branches share only read-only inputs: the matcher writes the spare half of
+      // the lists, the changed and heavy flags; the evaluation writes LMState and the partials.  With stage profiling on they stay
+      // serial, like the other forks.
       const bool fork = !c->prof_on;
-      rc = on_branch(c, c->br_scan, fork, [&] { return match(outer + 1); });
+      rc = on_branch(c, c->br_scan, fork, [&] { return eval_candidate_device(c, sets, 2, sinfo, P.huber_a, P.eig_thre, pdl); });
       if (rc) return rc;
-      rc = eval_candidate_device(c, sets, 2, sinfo, P.huber_a, P.eig_thre);
+      rc = match(outer + 1);
       if (rc) return rc;
       if (fork) MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream, c->br_scan.join, 0));
       stamp(c, "match || candidate");
@@ -156,7 +162,7 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool wa
   LMState *hs = &c->pinned->lm;
   int *h_cnt = c->pinned->counts;
   if (want_cov) {  // with_ua: cov_mapping = H^-1 at the returned pose (:600-610), one more tiny launch inside the frame
-    rc = pose_cov_device(c);
+    rc = pose_cov_device(c, pdl);
     if (rc) return rc;
     MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->pinned->pose_cov, c->pose_cov.p, 36 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
     stamp(c, "pose covariance");
@@ -469,6 +475,18 @@ int stage_next_sweep(Ctx *c) {
   return MLOAM_OK;
 }
 
+// Edges of a captured graph that launch_chain made programmatic (-1: the edges could not be read)
+int count_programmatic_edges(cudaGraph_t g) {
+  size_t n = 0;
+  if (cudaGraphGetEdges_v2(g, nullptr, nullptr, nullptr, &n) != cudaSuccess) return -1;
+  std::vector<cudaGraphNode_t> from(n), to(n);
+  std::vector<cudaGraphEdgeData> data(n);
+  if (n && cudaGraphGetEdges_v2(g, from.data(), to.data(), data.data(), &n) != cudaSuccess) return -1;
+  int k = 0;
+  for (size_t i = 0; i < n; i++) k += data[i].type == cudaGraphDependencyTypeProgrammatic ? 1 : 0;
+  return k;
+}
+
 unsigned long long fnv1a(unsigned long long h, const void *p, size_t n) {
   const unsigned char *b = static_cast<const unsigned char *>(p);
   for (size_t i = 0; i < n; i++) h = (h ^ b[i]) * 1099511628211ull;
@@ -488,6 +506,7 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
     return fail(c, MLOAM_E_STATE, "frame: uncertainty-aware frames (mloam_set_uncertainty) are single-GPU only; detach the communicator or set with_ua = 0");
   const bool want_cov = c->with_ua != 0;
   c->last_scan_valid = false;
+  c->frame_from_graph = false;
   const bool can_graph = c->use_graphs && c->params.max_inner == 1 && !c->prof_on && (!c->nccl_comm || c->p2p_on);
   if (can_graph) {
     unsigned long long key = 1469598103934665603ull;
@@ -535,6 +554,7 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
     if (e && e->exec && e->epoch == alloc_epoch()) {
       stage_frame_inputs(c, pose_init7);  // the captured H2D nodes read them at execution time
       MLOAM_CUDA_OK(c, cudaGraphLaunch(e->exec, c->stream));
+      c->frame_from_graph = true;
       c->launches += e->launches;
       frame_advance(c, parity, e->prefetched_out);
       c->last_scan = e->S, c->last_scan_valid = true;
@@ -556,8 +576,10 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
         e->launches = (int)(c->launches - l0), e->epoch = ep0, e->S = S, e->s2m_ran = ran;
         e->prefetched_out = c->prefetched;
         c->launches = l0;
+        c->graph_pdl_edges = count_programmatic_edges(graph);
         cudaGraphDestroy(graph);
         MLOAM_CUDA_OK(c, cudaGraphLaunch(e->exec, c->stream));
+        c->frame_from_graph = true;
         c->launches += e->launches;
         c->last_scan = S, c->last_scan_valid = true;
         return scan2map_finish(c, S, pose_init7, want_cov, ran, pose_out7, stats);

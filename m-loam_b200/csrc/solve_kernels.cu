@@ -130,6 +130,10 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
   __shared__ bool is_last;
   __shared__ int barrier_failed;
   unsigned long long *const tr = TRACE ? a.trace + (size_t)blockIdx.x * LIN_TRACE_BLOCK : nullptr;
+  // Programmatic dependent launch: everything below reads what the previous kernel of the GN chain writes (state->done / x, the
+  // SpecState, the matcher's lists for the fit, the ticket and generation word k_eval_candidate shares), so the wait comes first
+  cudaGridDependencySynchronize();
+  cudaTriggerProgrammaticLaunchCompletion();
   unsigned long long t_entry = 0ull;
   long long c_entry = 0ll, c_fit = 0ll;
   if (TRACE) t_entry = global_ns(), c_entry = clock64();
@@ -1113,6 +1117,9 @@ __device__ __noinline__ void cand_tail(const double *wsums, int n_lin_blocks, LM
 // grid: LIN_THREADS / CAND_THREADS blocks per k_linearize block; wsums: NE_CAND doubles per warp
 __global__ void __launch_bounds__(CAND_THREADS, 8) k_eval_candidate(LinArgs a, double *__restrict__ wsums) {
   __shared__ bool is_last;
+  // Programmatic dependent launch: state->done, xc and the valid / coefficient arrays come from k_linearize's pass 0
+  cudaGridDependencySynchronize();
+  cudaTriggerProgrammaticLaunchCompletion();
   if (a.state->done) return;  // the step of the evaluation at x ended the Solve
   double xs[7];
 #pragma unroll
@@ -1159,6 +1166,7 @@ __global__ void __launch_bounds__(CAND_THREADS, 8) k_eval_candidate(LinArgs a, d
 }
 
 __global__ void k_lm_init(LMState *st, const double *pose7, int max_inner, int min_corr, SpecState *spec) {
+  cudaGridDependencySynchronize();  // programmatic dependent launch: the kernel before may still read the state and SpecState it resets
   if (threadIdx.x == 0 && blockIdx.x == 0) {
     if (spec) {  // the first matcher of a solve is blind: any half will do, but sel must be 0 or 1 (fresh memory is not)
       for (int k = 0; k < 7; k++) spec->xc[k] = pose7[k];
@@ -1177,14 +1185,13 @@ __global__ void k_lm_init(LMState *st, const double *pose7, int max_inner, int m
   }
 }
 
-int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, int min_corr, SpecState *spec) {
+int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, int min_corr, SpecState *spec, bool pdl) {
   MLOAM_CUDA_OK(c, c->lm_state.reserve(sizeof(LMState) + 64));
   stage_pose(c, pose7_host);
   double *d_stage = c->ctl.as<DevCtl>()->pose;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_stage, c->pinned->pose, 7 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  k_lm_init<<<1, 32, 0, c->stream>>>(c->lm_state.as<LMState>(), d_stage, max_inner, min_corr, spec);
+  MLOAM_CUDA_OK(c, launch_chain(pdl, k_lm_init, 1, 32, c->stream, c->lm_state.as<LMState>(), d_stage, max_inner, min_corr, spec));
   c->launches++;
-  MLOAM_CUDA_OK(c, cudaGetLastError());
   return MLOAM_OK;
 }
 
@@ -1196,6 +1203,7 @@ int lm_init_state(Ctx *c, const double *pose7_host, int max_inner, int min_corr,
 // would return inf / NaN there).  The speculative schedule keeps the two-pass k_linearize for the last GN iteration, so H is
 // accumulated at the final candidate too (k_eval_candidate does not accumulate H).
 __global__ void k_pose_cov(const LMState *__restrict__ st, double *__restrict__ out) {
+  cudaGridDependencySynchronize();  // programmatic dependent launch: H and rows come from the last k_linearize's tail
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   if (st->rows <= 0) {
     for (int i = 0; i < 36; i++) out[i] = 0.0;
@@ -1239,11 +1247,10 @@ __global__ void k_pose_cov(const LMState *__restrict__ st, double *__restrict__ 
   }
 }
 
-int pose_cov_device(Ctx *c) {
+int pose_cov_device(Ctx *c, bool pdl) {
   MLOAM_CUDA_OK(c, c->pose_cov.reserve(36 * sizeof(double)));
-  k_pose_cov<<<1, 32, 0, c->stream>>>(c->lm_state.as<LMState>(), c->pose_cov.as<double>());
+  MLOAM_CUDA_OK(c, launch_chain(pdl, k_pose_cov, 1, 32, c->stream, c->lm_state.as<const LMState>(), c->pose_cov.as<double>()));
   c->launches++;
-  MLOAM_CUDA_OK(c, cudaGetLastError());
   return MLOAM_OK;
 }
 
@@ -1338,15 +1345,10 @@ int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, 
   {
     ProfScope ps(c, "linearize");
     double *const pt = c->partials.as<double>();
-    if (a.trace) {
-      if (kfit == 5) k_linearize<5, true><<<nb, LIN_THREADS, 0, c->stream>>>(a, pt);
-      else if (kfit == 10) k_linearize<10, true><<<nb, LIN_THREADS, 0, c->stream>>>(a, pt);
-      else k_linearize<0, true><<<nb, LIN_THREADS, 0, c->stream>>>(a, pt);
-    } else {
-      if (kfit == 5) k_linearize<5><<<nb, LIN_THREADS, 0, c->stream>>>(a, pt);
-      else if (kfit == 10) k_linearize<10><<<nb, LIN_THREADS, 0, c->stream>>>(a, pt);
-      else k_linearize<0><<<nb, LIN_THREADS, 0, c->stream>>>(a, pt);
-    }
+    void (*k)(LinArgs, double *);
+    if (a.trace) k = kfit == 5 ? k_linearize<5, true> : (kfit == 10 ? k_linearize<10, true> : k_linearize<0, true>);
+    else k = kfit == 5 ? k_linearize<5> : (kfit == 10 ? k_linearize<10> : k_linearize<0>);
+    MLOAM_CUDA_OK(c, launch_chain(o.pdl, k, nb, LIN_THREADS, c->stream, a, pt));
     c->launches++;
   }
   if (fused) {
@@ -1375,16 +1377,15 @@ int linearize_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, 
   return MLOAM_OK;
 }
 
-int eval_candidate_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, double eig_thre) {
+int eval_candidate_device(Ctx *c, const FeatSet *sets, int n_sets, double sqrt_info, double huber_a, double eig_thre, bool pdl) {
   LinArgs a;
   int nb = 0;
   double *wsums = nullptr;
   int rc = lin_setup(c, sets, n_sets, sqrt_info, huber_a, eig_thre, a, &nb, &wsums);
   if (rc) return rc;
   ProfScope ps(c, "candidate");
-  k_eval_candidate<<<nb * (LIN_THREADS / CAND_THREADS), CAND_THREADS, 0, c->stream>>>(a, wsums);
+  MLOAM_CUDA_OK(c, launch_chain(pdl, k_eval_candidate, nb * (LIN_THREADS / CAND_THREADS), CAND_THREADS, c->stream, a, wsums));
   c->launches++;
-  MLOAM_CUDA_OK(c, cudaGetLastError());
   return MLOAM_OK;
 }
 

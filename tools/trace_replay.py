@@ -3,9 +3,10 @@
 the device as in bench.py) with torch.profiler: device time per kernel and frame, and how much of each candidate evaluation
 (k_eval_candidate) runs while the speculative matcher (k_match_knn) of the next GN iteration is running.
   python tools/trace_replay.py OUT_DIR [frames] [--phases]      (writes OUT_DIR/replay.pt.trace.json)
---phases: afterwards, the same frames on a second context with MLOAM_LIN_TRACE=1 (no profiler): the phase split of k_linearize's
-pass 0 per GN iteration from %globaltimer / clock64 stamps inside the kernel (feature loop = fit + evaluation, block reduction,
-ticket, LM tail)."""
+--phases: afterwards, the same frames on a second context with MLOAM_LIN_TRACE=1 and MLOAM_KNN_TRACE=1 (no profiler): the phase
+split of k_linearize's pass 0 per GN iteration from %globaltimer / clock64 stamps inside the kernel (feature loop = fit + evaluation,
+block reduction, ticket, LM tail), and the GN chain's kernel boundaries from those stamps and k_match_knn's per-warp timelines.
+MLOAM_PDL is passed through (read at context creation)."""
 import ctypes as C
 import json
 import os
@@ -35,7 +36,21 @@ def phases(tr):
     us = lambda t: (int(t) - t0) / 1000.0  # noqa: E731
     return {"blocks": len(blk), "loop_end": us(loop_end), "fit_share": fit_share, "reduced": us(blk[:, 32].max()),
             "ticket": us(last[0, 33]) if len(last) else float("nan"), "tail_start": us(last[0, 34]) if len(last) else float("nan"),
-            "tail_end": us(last[0, 35]) if len(last) else float("nan")}
+            "tail_end": us(last[0, 35]) if len(last) else float("nan"), "t_entry": t0, "t_tail_end": int(last[0, 35]) if len(last) else 0}
+
+
+def chain_gaps(lin, knn):
+    """The GN chain's kernel boundaries of one frame [us], from the k_linearize slots (phases()) and the k_match_knn timelines
+    ([enter, exit] per warp, enter taken after the grid-dependency wait): per GN iteration i, (a) the tail end of k_linearize i ->
+    the first warp of matcher i + 1, (b) the last warp of matcher i -> the first block of k_linearize i."""
+    spans = []
+    for tl in knn:
+        tl = tl[tl[:, 0] != 0].astype(np.int64)
+        spans.append((int(tl[:, 0].min()), int(tl[:, 1].max())))
+    n = min(len(lin), len(spans))
+    b = [(lin[i]["t_entry"] - spans[i][1]) / 1000.0 for i in range(n)]
+    a = [(spans[i + 1][0] - lin[i]["t_tail_end"]) / 1000.0 for i in range(n - 1)]
+    return a, b
 
 
 def main():
@@ -109,18 +124,28 @@ def main():
     if "--phases" not in sys.argv:
         return
     os.environ["MLOAM_LIN_TRACE"] = "1"  # read at context creation
+    os.environ["MLOAM_KNN_TRACE"] = "1"
     ctx = m.Context(0, p)
     step(True)
     for _ in range(4):
         step(False)
-    rows = []
+    rows, gaps = [], []
     buf = np.zeros(16 * LIN_TRACE_SLOT, dtype=np.uint64)
+    n_pairs = 8 * 4 * torch.cuda.get_device_properties(0).multi_processor_count  # k_match_knn: MWARPS x up to 4 CTAs per SM
+    tl = np.zeros((n_pairs, 2), dtype=np.uint64)
     for _ in range(n_frames):
         step(False)
         n_slots = C.c_int(0)
         rc = m.lib().mloam_debug_lin_trace(ctx._h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n_slots))
         assert rc == 0, rc
         rows.append([phases(buf[s * LIN_TRACE_SLOT:(s + 1) * LIN_TRACE_SLOT]) for s in range(n_slots.value)])
+        knn, s, n_knn = [], 0, C.c_int(1)
+        while s < n_knn.value:
+            rc = m.lib().mloam_debug_knn_timeline(ctx._h, s, tl.ctypes.data_as(C.c_void_p), n_pairs, C.byref(n_knn))
+            assert rc == 0, rc
+            knn.append(tl.copy())
+            s += 1
+        gaps.append(chain_gaps(rows[-1], knn))
     ctx.close()
     keys = ["loop_end", "reduced", "ticket", "tail_start", "tail_end"]
     print(f"k_linearize pass 0 phase boundaries, us from the first warp's entry, mean of {n_frames} replayed frames "
@@ -134,6 +159,17 @@ def main():
         mean = {k: float(np.mean([x[k] for x in spec])) for k in keys + ["fit_share"]}
         print("  speculative iterations (all but the last): " + ", ".join(f"{k} {mean[k]:.2f}" for k in keys) +
               f", fit share {mean['fit_share']:.2f}")
+    ga = np.array([g[0] for g in gaps])
+    gb = np.array([g[1] for g in gaps])
+    print(f"GN chain boundaries, us, mean of {n_frames} replayed frames: (a) k_linearize tail end -> first k_match_knn warp of the "
+          f"next iteration, (b) last k_match_knn warp -> first k_linearize block (negative: the next kernel was already running)")
+    print(f"  {'GN it':>5s} {'(a)':>8s} {'(b)':>8s}")
+    for i in range(gb.shape[1]):
+        a_i = f"{ga[:, i].mean():8.2f}" if i < ga.shape[1] else f"{'':8s}"
+        print(f"  {i:5d} {a_i} {gb[:, i].mean():8.2f}")
+    per = ga.sum(axis=1) + gb.sum(axis=1)
+    print(f"  per frame: sum (a) {ga.sum(axis=1).mean():.1f}, sum (b) {gb.sum(axis=1).mean():.1f}, total {per.mean():.1f} "
+          f"(min {per.min():.1f}, max {per.max():.1f})")
 
 
 if __name__ == "__main__":
