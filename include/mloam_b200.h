@@ -323,6 +323,26 @@ int mloam_pose_covariance(mloam_ctx_t *ctx, double *cov36);
 int mloam_frame_scan(mloam_ctx_t *ctx, mloam_point_t *h_surf, float *h_surf_cov6, int cap_surf, int *n_surf, mloam_point_t *h_corner,
                      float *h_corner_cov6, int cap_corner, int *n_corner);
 
+/* ---- the outlier cloud of segment_cloud: 0 (laser_cloud_outlier_cov, lidar_mapper_keyframe.cpp:366-418), what the keyframe store keeps as a
+ *      keyframe's third cloud (:673-681) and the global map appends (:818-827, :873-882).  Off by default.
+ * mloam_set_outlier: map_outlier_res > 0 turns it on with that leaf (MAP_OUTLIER_RES, e.g. 0.8 in the KITTI / Oxford / UTBM
+ *   configurations); 0 turns it off.  Call it after mloam_set_lidars.  The leaf is staged: a captured frame replays with a new one.
+ *   MLOAM_E_INVALID for a negative or non-finite leaf; MLOAM_E_STATE on a context with a communicator (single-GPU, like with_ua).
+ *   With it on, every mloam_frame* call also builds the frame's outlier cloud, with one more launch: per LiDAR l the first point of its
+ *   part of the ring-ordered sweep (ImageSegmenter::segmentCloud's laser_cloud_out.points[0], image_segmenter.hpp:390; index
+ *   scan_start[l x R] - 5 of an mloam_frame* concatenation, R = rings per LiDAR; the projection's first point of LiDAR l in mloam_frame_raw*;
+ *   none for a LiDAR whose part is empty) -> moved with the float 3x4 matrix of its extrinsic, intensity = l (pubPointCloud,
+ *   visualization.cpp:40-52, :89-104; in the single-LiDAR path the extrinsic of mloam_set_extrinsic, identity without one) -> concatenated
+ *   LiDAR by LiDAR -> VoxelGridCovarianceMLOAM<PointI>(map_outlier_res) -> with with_ua the scans' trace gate under the extrinsic
+ *   covariances of the call, else zero cov_vec.  Poses, statistics, mloam_frame_scan and the submaps do not change.
+ * mloam_frame_outlier: that cloud of the last mloam_frame* call, in the base frame, intensity = laser id, with its cov_vec (as
+ *   mloam_frame_scan).  Outputs nullable; *n = the cloud's size, also when cap is too small (MLOAM_E_INVALID).  MLOAM_E_STATE before any
+ *   frame or when the last frame ran with the outlier cloud off.
+ * mloam_keyframe_outlier: keyframe `id`'s stored outlier cloud (empty for a keyframe saved while it was off), with the same rules. */
+int mloam_set_outlier(mloam_ctx_t *ctx, float map_outlier_res);
+int mloam_frame_outlier(mloam_ctx_t *ctx, mloam_point_t *h_pts, float *h_cov6, int cap, int *n);
+int mloam_keyframe_outlier(mloam_ctx_t *ctx, int id, mloam_point_t *h_pts, float *h_cov6, int cap, int *n);
+
 /* ---- the mapper's keyframe store, kept on the device: saveKeyframe -> clearCloud -> extractSurroundingKeyFrames
  *      (lidar_mapper_keyframe.cpp:641-683, :921-927 at :1101, :254-354).  The mapper loop of process() (:1062-1101) becomes
  *        mloam_set_lidars / mloam_set_uncertainty (the frame's /extrinsics, :1028-1046, read BEFORE the submap as the reference does:
@@ -336,8 +356,9 @@ int mloam_frame_scan(mloam_ctx_t *ctx, mloam_point_t *h_surf, float *h_surf_cov6
  *   the leaves of the scan filters too, :1278-1289).
  * mloam_keyframe_save: saveKeyframe for the last mloam_frame* call.  Saved when it is the first keyframe, the float distance of the positions
  *   to the previous keyframe is > DISTANCE_KEYFRAMES, or Eigen's angularDistance 2 atan2(|(q q_prev^-1).vec|, |(q q_prev^-1).w|) in degrees
- *   is > ORIENTATION_KEYFRAMES.  A saved keyframe keeps the frame's down-sampled, gated scans (as mloam_frame_scan returns them), copied
- *   device to device, and marks the submap stale (clearCloud).  pose7 / cov36 NULL: the frame's pose and mloam_pose_covariance, zeroed
+ *   is > ORIENTATION_KEYFRAMES.  A saved keyframe keeps the frame's down-sampled, gated scans (as mloam_frame_scan returns them) and its
+ *   outlier cloud (mloam_frame_outlier; empty when the frame ran without it), copied device to device, and marks the submap stale
+ *   (clearCloud).  pose7 / cov36 NULL: the frame's pose and mloam_pose_covariance, zeroed
  *   while the store holds <= 10 keyframes (:607-608; the count before this save is the one the solve saw); explicit values let a caller
  *   correct keyframe poses.  *saved (nullable) = 1 when saved.  MLOAM_E_STATE if no frame has run since the last save or init.
  * mloam_keyframe_submap: extractSurroundingKeyFrames at the frame's initial guess pose_pred7 (transformAssociateToMap).  Nothing to do
@@ -371,10 +392,10 @@ int mloam_keyframe_scan(mloam_ctx_t *ctx, int id, double *pose7, double *cov36, 
  *                              the publisher left would sit in front: restated as the state in which the publisher never ran)
  *   -> VoxelGridCovarianceMLOAM<PointI>(kf_leaf = 10 m, :1293) with intensity = id, the last id of a voxel wins -> per chosen keyframe in
  *   filter order, cloudUCTAssociateToMap of its clouds with its stored pose and covariance and the CURRENT extrinsics / covariances
- *   (mloam_set_lidars / mloam_set_uncertainty) and the store's TRACE_THRESHOLD_MAPPING; SURROUND appends surf then corner to map 0,
- *   SAVE appends surf to map 0 and corner to map 1 -> VoxelGridCovarianceMLOAM<PointIWithCov>(leaf, TRACE_THRESHOLD_MAPPING) of each map
- *   (leaf: MAP_SURF_RES for SURROUND, 2 * MAP_SURF_RES for both maps of SAVE).  The store keeps no outlier clouds (laser_cloud_outlier_cov,
- *   :673-681), so the reference's outlier appends (:825-827, :871-873) are left out and the maps hold surf and corner points only.  One
+ *   (mloam_set_lidars / mloam_set_uncertainty) and the store's TRACE_THRESHOLD_MAPPING; SURROUND appends surf, corner, then outlier to map
+ *   0 (:818-827), SAVE appends surf then outlier to map 0 and corner to map 1 (:873-882) -> VoxelGridCovarianceMLOAM<PointIWithCov>(leaf,
+ *   TRACE_THRESHOLD_MAPPING) of each map (leaf: MAP_SURF_RES for SURROUND, 2 * MAP_SURF_RES for both maps of SAVE).  The outlier clouds are
+ *   those the keyframes were saved with (mloam_set_outlier); a store without any gives the maps of surf and corner points alone.  One
  *   batched association per map: the launch count does not grow with the keyframes (a fixed 15 more when over 2048 keyframes reach the
  *   position filter).
  *   Outputs (nullable): the chosen count and the two map sizes (map 1 is empty for SURROUND).  No keyframe offered: MLOAM_OK, empty

@@ -35,7 +35,7 @@ ABI_SYMBOLS = [
     "mloam_keyframes_init", "mloam_keyframe_save", "mloam_keyframe_submap", "mloam_keyframe_query", "mloam_keyframe_scan",
     "mloam_global_map", "mloam_global_map_read", "mloam_global_map_chosen",
     "mloam_cal_timestamp", "mloam_set_front_end", "mloam_front_end", "mloam_frame_raw", "mloam_frame_raw_device", "mloam_frame_set_next_raw",
-    "mloam_frame_set_next_raw_device",
+    "mloam_frame_set_next_raw_device", "mloam_set_outlier", "mloam_frame_outlier", "mloam_keyframe_outlier",
 ]
 
 
@@ -598,6 +598,25 @@ class Context:
         cp, cc = np.zeros((max(nc.value, 1), 4), np.float32), np.zeros((max(nc.value, 1), 6), np.float32)
         self._ck(lib().mloam_frame_scan(self._h, _p(sp), _p(sc), sp.shape[0], C.byref(ns), _p(cp), _p(cc), cp.shape[0], C.byref(nc)))
         return sp[:ns.value].copy(), sc[:ns.value].copy(), cp[:nc.value].copy(), cc[:nc.value].copy()
+
+    def set_outlier(self, map_outlier_res: float):
+        """The outlier cloud of segment_cloud: 0 (mloam_set_outlier): leaf MAP_OUTLIER_RES > 0 turns it on, 0 off.  Call after set_lidars."""
+        self._ck(lib().mloam_set_outlier(self._h, C.c_float(map_outlier_res)))
+
+    def _outlier(self, fn, *lead):
+        n = C.c_int(0)
+        self._ck(fn(self._h, *lead, None, None, 0, C.byref(n)))
+        p, c6 = np.zeros((max(n.value, 1), 4), np.float32), np.zeros((max(n.value, 1), 6), np.float32)
+        self._ck(fn(self._h, *lead, _p(p), _p(c6), p.shape[0], C.byref(n)))
+        return p[:n.value].copy(), c6[:n.value].copy()
+
+    def frame_outlier(self):
+        """laser_cloud_outlier_cov of the last frame: (points [n,4] in the base frame, intensity = laser id; cov6 [n,6])."""
+        return self._outlier(lib().mloam_frame_outlier)
+
+    def keyframe_outlier(self, kf_id: int):
+        """Keyframe kf_id's stored outlier cloud: (points [n,4], cov6 [n,6])."""
+        return self._outlier(lib().mloam_keyframe_outlier, C.c_int(int(kf_id)))
 
     # ---- keyframe store (saveKeyframe / extractSurroundingKeyFrames on the device)
     def keyframes_init(self, distance_keyframes: float, orientation_keyframes_deg: float, surrounding_kf_radius: float, map_sur_kf_res: float,

@@ -168,6 +168,13 @@ struct UaStage {
   alignas(256) UctLaser lasers[MLOAM_MAX_LIDARS];
 };
 static_assert(sizeof(UaStage) == 256 + sizeof(UctLaser) * MLOAM_MAX_LIDARS, "with_ua stage layout");
+// the configuration of a frame's outlier stage (mloam_set_outlier; submap.cu outlier_stage), copied to the device as one block
+struct OutlierStage {
+  float leaf;                        // MAP_OUTLIER_RES
+  int n_lasers;                      // LiDARs of the frame (first points recorded by the extraction)
+  int pad[2];
+  float mat[MLOAM_MAX_LIDARS][12];   // per LiDAR the float 3x4 extrinsic of pubPointCloud's transformPointCloud (identity without one)
+};
 
 // The context's pinned host block (Ctx::pinned): staging of small host-to-device copies and landing of small read-backs, so that
 // they are truly asynchronous.
@@ -178,6 +185,7 @@ struct PinnedBlock {
   double ext[7];                    // features_enqueue: the single sensor -> base extrinsic
   float rig[MLOAM_MAX_LIDARS][12];  // features_enqueue: the rig's float 3x4 extrinsics of the merge
   UaStage ua;                       // ua_scan_stage: the with_ua configuration
+  OutlierStage outlier;             // outlier_stage: the outlier cloud's configuration
   // Written by captured copies (landing of a frame's results) and by the host-buffer entry points, one call at a time
   LMState lm;                       // LMState mirror
   int counts[192];                  // count read-backs; mloam_project_cloud: [0] count, [64..] scan starts, [128..] scan ends
@@ -348,6 +356,14 @@ struct Ctx {
     const int *d_n_corner;
     const double *sinfo_surf, *sinfo_corner;  // nullable per-feature sqrt_info (uncertainty-aware mapping)
     const float *cov6_surf, *cov6_corner;     // nullable PointIWithCov::cov_vec per feature (with_ua frame: gated scans)
+    // the raw first point of each LiDAR's part of the ring-ordered sweep (first_ok[l] = 0: the part is empty), recorded by the
+    // extraction into the sweep's half of the feature double buffer (ExtractOut::first)
+    const float4 *first;
+    const int *first_ok;
+    // laser_cloud_outlier_cov of the frame (mloam_set_outlier; null when the outlier stage did not run): points, cov_vec, device count
+    const float4 *outlier;
+    const float *cov6_outlier;
+    const int *d_n_outlier;
   };
   // Sweep look-ahead (mloam_frame_set_next*): while frame k is matched and solved, the features of sweep k+1 are extracted and
   // down-sampled on a side stream into the other half of a double buffer — the reference runs the two stages in different nodes
@@ -439,6 +455,12 @@ struct Ctx {
   double ua_trace_threshold = 0.0;          // TRACE_THRESHOLD_MAPPING
   DevBuf ua_scan;                  // gated scans of the last with_ua frame (points, cov6, sqrt_info, counts) + its staged configuration
   DevBuf pose_cov;                 // 36 doubles: H^-1 of the last solve (k_pose_cov), copied back with LMState
+  // the outlier cloud of segment_cloud: 0 (mloam_set_outlier): per LiDAR the first point of its ring-ordered sweep -> base frame ->
+  // VoxelGridCovarianceMLOAM<PointI>(MAP_OUTLIER_RES) -> the with_ua gate (lidar_mapper_keyframe.cpp:366-418), one launch next to the
+  // with_ua stage.  The leaf reaches the device through the pinned block (PinnedBlock::outlier), so a captured frame replays with it.
+  bool outlier_on = false;
+  float outlier_leaf = 0.f;
+  DevBuf outlier;                  // the staged configuration, the frame's outlier cloud (points, cov_vec) and its count
   double pose_cov36[36] = {0};     // pose_wmap_curr.cov_ of the last mloam_frame* / mloam_scan2map* call
   bool last_scan_valid = false;    // last_scan describes the scan of the last mloam_frame* call (mloam_frame_scan)
   ScanRef last_scan{};
@@ -546,8 +568,15 @@ int sqrt_info_device(Ctx *c, const float *d_cov6, int n, double *d_sinfo);
 // submap.cu: the with_ua stage of a frame (downsampleCurrentScan, lidar_mapper_keyframe.cpp:356-421) on c->stream.  The scans of *S
 // (device counts) -> per point ext^-1 -> evalPointUncertainty under pose_ext -> trace gate -> stable compaction into Ctx::ua_scan with
 // cov6 and sqrt_info; *S then points at the gated scans.  ua_stage_host writes the staged configuration (PinnedBlock::ua).
-int ua_scan_stage(Ctx *c, Ctx::ScanRef *S);
+// d_cfg (nullable): where the staged configuration lies on the device (the outlier stage reads its with_ua part)
+int ua_scan_stage(Ctx *c, Ctx::ScanRef *S, const UaStage **d_cfg = nullptr);
 void ua_stage_host(Ctx *c);
+// submap.cu: the outlier stage of a frame (downsampleCurrentScan, lidar_mapper_keyframe.cpp:366-418) on c->stream, after ua_scan_stage:
+// the first points S->first of the LiDARs' parts of the sweep -> float extrinsic, intensity = laser id -> VoxelGridCovarianceMLOAM<PointI>
+// (MAP_OUTLIER_RES) -> with d_ua (the with_ua stage's configuration) the trace gate, else zero cov_vec -> Ctx::outlier, *S's outlier
+// fields.  One single-CTA launch.  stage_outlier writes the staged configuration (PinnedBlock::outlier).
+int outlier_stage(Ctx *c, Ctx::ScanRef *S, const UaStage *d_ua);
+void stage_outlier(Ctx *c);
 // pipeline.cu: writers of the pinned fields a captured frame graph reads (PinnedBlock), shared by the enqueue and the replay paths
 void stage_pose(Ctx *c, const double *pose7);
 void stage_ext(Ctx *c);
@@ -564,6 +593,11 @@ int comm_allreduce_doubles(Ctx *c, double *d_buf, int count);
 struct ExtractOut {
   float4 *sharp, *less_sharp, *flat, *less_flat;  // device buffers, capacity n each
   int *counts;                                     // device int[4]
+  // nullable: the first point of each LiDAR's part of the sweep (rings l * first_rings .. (l + 1) * first_rings - 1), first_ok[l] = 0
+  // when the part is empty (image_segmenter.hpp:390's laser_cloud_out.points[0], the outlier cloud of segment_cloud: 0)
+  float4 *first = nullptr;
+  int *first_ok = nullptr;
+  int first_rings = 0;
 };
 int extract_device(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, const int *d_scan_end, int n_scans,
                    ExtractOut out, float *d_curv_or_null, int *d_label_or_null);

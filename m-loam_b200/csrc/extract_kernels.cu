@@ -1099,9 +1099,20 @@ __device__ void voxel_in_cta(const float4 *__restrict__ P, const int *__restrict
 
 __global__ void __launch_bounds__(RV_THREADS)
     k_ring_voxel(const float4 *__restrict__ P, const int *__restrict__ label, int n, const int *__restrict__ scan_start,
-                 const int *__restrict__ scan_end, float inv, float4 *__restrict__ stage_out, int *__restrict__ ring_cnt, int smem_keys) {
+                 const int *__restrict__ scan_end, float inv, float4 *__restrict__ stage_out, int *__restrict__ ring_cnt, int smem_keys,
+                 float4 *__restrict__ first = nullptr, int *__restrict__ first_ok = nullptr, int first_rings = 0) {
   const int ring = blockIdx.x;
   const int s = scan_start[ring], e = scan_end[ring];
+  // the first ring of LiDAR l records laser_cloud_out.points[0] of its part (image_segmenter.hpp:390): the part starts at
+  // scan_start - 5 of its first ring, and holds sum (end - start + 11) points over its rings (0: empty, no point)
+  if (first && threadIdx.x == 0 && ring % first_rings == 0) {
+    int cnt = 0;
+    for (int r = ring; r < ring + first_rings; r++) cnt += scan_end[r] - scan_start[r] + 11;
+    const int at = s - 5, l = ring / first_rings;
+    const int ok = (cnt > 0 && at >= 0 && at < n) ? 1 : 0;
+    first_ok[l] = ok;
+    if (ok) first[l] = P[at];
+  }
   const int len = e - s;
   // the rings k_ring_pick processes (:155, the on-chip window check and the sort capacity of this launch)
   if (len < 6 || len + 10 > RING_MAX || s - 5 < 0 || e + 5 > n || len > smem_keys) {
@@ -1219,7 +1230,8 @@ void extract_work_layout(Carve &cv, int n, int n_scans, ExtractWork *W) {
 
 int extract_device(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, const int *d_scan_end, int n_scans,
                    ExtractOut out, float *d_curv_or_null, int *d_label_or_null) {
-  if (n < 0 || n_scans <= 0 || n_scans > MLOAM_MAX_RINGS) {
+  if (n < 0 || n_scans <= 0 || n_scans > MLOAM_MAX_RINGS || (out.first && (out.first_rings <= 0 || n_scans % out.first_rings != 0 ||
+                                                                              n_scans / out.first_rings > MLOAM_MAX_LIDARS))) {
     c->err = "extract: n_scans must be in 1..1024 (rings of all LiDARs of a batched extraction)";
     return MLOAM_E_INVALID;
   }
@@ -1262,7 +1274,8 @@ int extract_device(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start
     smem_opt_in = true;
   }
   k_ring_voxel<<<n_scans, RV_THREADS, (size_t)smem_keys * sizeof(unsigned long long), st>>>(d_cloud, label, n, d_scan_start, d_scan_end, 1.0f / 0.2f,
-                                                                                              lf, seg_begin, smem_keys);
+                                                                                              lf, seg_begin, smem_keys, out.first, out.first_ok,
+                                                                                              out.first_rings);
   k_ring_voxel_emit<<<n_scans, 128, 0, st>>>(lf, seg_begin, d_scan_start, n_scans, out.less_flat, out.counts + 3);
   c->launches += 5;
   if (d_curv_or_null) MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_curv_or_null, curv, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));

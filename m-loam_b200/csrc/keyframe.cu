@@ -1,12 +1,12 @@
 // keyframe.cu — the mapper's keyframe state machine with the keyframes kept on the device (lidar_mapper_keyframe.cpp):
 //   mloam_keyframes_init   an empty store: no keyframes, empty surrounding set, empty map slots (the first frame fails the map gate, :429)
-//   mloam_keyframe_save    saveKeyframe (:641-683): distance / angle test, the last frame's gated scans appended device to device to a
-//                          grow-only arena; a save marks the submap stale (clearCloud, :921-927, called at :1101)
+//   mloam_keyframe_save    saveKeyframe (:641-683): distance / angle test, the last frame's gated scans and outlier cloud appended device
+//                          to device to a grow-only arena; a save marks the submap stale (clearCloud, :921-927, called at :1101)
 //   mloam_keyframe_submap  extractSurroundingKeyFrames (:254-354): radius search over the keyframe positions, the surrounding-set
 //                          bookkeeping (:274-323) with a device cache of the associated clouds (cloudUCTAssociateToMap once per entering
 //                          keyframe), the keyframe-position filter (:325-338), `+=` of the chosen cached clouds (k_gather_*), the two
 //                          covariance filters (:344-347) and the map build into MLOAM_MAP_SURF / MLOAM_MAP_CORNER
-//   mloam_keyframe_query / mloam_keyframe_scan   what a caller that publishes keyframes needs
+//   mloam_keyframe_query / mloam_keyframe_scan / mloam_keyframe_outlier   what a caller that publishes keyframes needs
 //   mloam_global_map       pubGlobalMap (:780-851) / saveGlobalMap (:853-919): radius search or every keyframe, the keyframe-position
 //                          filter, one batched cloudUCTAssociateToMap over every cloud of the chosen keyframes (k_uct_associate_seg,
 //                          submap.cu) and the covariance filter, into buffers of its own; _read / _chosen return the result
@@ -72,17 +72,17 @@ __host__ __device__ inline EntLayout ent_layout(int n_surf, int n_corner) {
   return L;
 }
 
-// A keyframe's record in the arena (laser_cloud_{surf,corner}_cov of saveKeyframe): per cloud t (0 surf, 1 corner) its points, then its
-// cov_vec, sized for the stored counts n[t]
+// A keyframe's record in the arena (laser_cloud_{surf,corner,outlier}_cov of saveKeyframe): per cloud t (0 surf, 1 corner, 2 outlier) its
+// points, then its cov_vec, sized for the stored counts n[t]
 struct KfRecord {
-  float4 *pts[2];
-  float *cov6[2];
+  float4 *pts[3];
+  float *cov6[3];
   size_t bytes;
 };
-inline KfRecord kf_record(char *base, const int n[2]) {
+inline KfRecord kf_record(char *base, const int n[3]) {
   KfRecord R;
   Carve cv(base);
-  for (int t = 0; t < 2; t++) R.pts[t] = cv.take<float4>(n[t]), R.cov6[t] = cv.take<float>(6 * (size_t)n[t]);
+  for (int t = 0; t < 3; t++) R.pts[t] = cv.take<float4>(n[t]), R.cov6[t] = cv.take<float>(6 * (size_t)n[t]);
   R.bytes = cv.size + 256;
   return R;
 }
@@ -144,8 +144,8 @@ struct KeyframeStore {
     double pose[7], cov[36];  // pose_keyframes_6d
     float pos[3];             // pose_keyframes_3d (intensity = id)
     int chunk;
-    size_t off;               // in its chunk: surf points | surf cov_vec | corner points | corner cov_vec
-    int n[2];                 // stored points: [0] surf, [1] corner
+    size_t off;               // in its chunk: surf points | surf cov_vec | corner points | corner cov_vec | outlier points | outlier cov_vec
+    int n[3];                 // stored points: [0] surf, [1] corner, [2] outlier (0 when the frame ran without the outlier cloud)
   };
   std::vector<Kf> kfs;
   std::vector<RawBuf> chunks;  // keyframe arena; a keyframe lies in one chunk and chunks never move, so growth keeps every keyframe valid
@@ -305,8 +305,11 @@ int mloam_keyframe_save(mloam_ctx_t *h, const double *pose7, const double *cov36
   hc[0] = R.n_surf, hc[1] = R.n_corner;
   if (R.d_n_surf) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, R.d_n_surf, sizeof(int), cudaMemcpyDeviceToHost, st));
   if (R.d_n_corner) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc + 1, R.d_n_corner, sizeof(int), cudaMemcpyDeviceToHost, st));
+  hc[2] = 0;  // laser_cloud_outlier_cov (:677): empty when the frame ran without the outlier cloud
+  if (R.d_n_outlier) MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc + 2, R.d_n_outlier, sizeof(int), cudaMemcpyDeviceToHost, st));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
   k.n[0] = std::max(0, std::min(hc[0], R.n_surf)), k.n[1] = std::max(0, std::min(hc[1], R.n_corner));
+  k.n[2] = std::max(0, std::min(hc[2], MLOAM_MAX_LIDARS));
   const size_t need = kf_record(nullptr, k.n).bytes;
   if (S.chunks.empty() || S.chunk_used + need > S.chunks.back().cap) {  // a new chunk, twice the last one: O(log K) allocations
     RawBuf b;
@@ -317,9 +320,9 @@ int mloam_keyframe_save(mloam_ctx_t *h, const double *pose7, const double *cov36
   k.chunk = (int)S.chunks.size() - 1, k.off = S.chunk_used;
   S.chunk_used += need;
   const KfRecord rec = kf_record(S.chunks[k.chunk].p + k.off, k.n);
-  const float4 *src[2] = {R.surf, R.corner};
-  const float *srcc[2] = {R.cov6_surf, R.cov6_corner};
-  for (int t = 0; t < 2; t++) {
+  const float4 *src[3] = {R.surf, R.corner, R.outlier};
+  const float *srcc[3] = {R.cov6_surf, R.cov6_corner, R.cov6_outlier};
+  for (int t = 0; t < 3; t++) {
     const size_t m = (size_t)k.n[t];
     if (m) MLOAM_CUDA_OK(c, cudaMemcpyAsync(rec.pts[t], src[t], 16 * m, cudaMemcpyDeviceToDevice, st));
     if (m && srcc[t]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(rec.cov6[t], srcc[t], 24 * m, cudaMemcpyDeviceToDevice, st));
@@ -581,6 +584,27 @@ int mloam_keyframe_scan(mloam_ctx_t *h, int id, double *pose7, double *cov36, ml
   return MLOAM_OK;
 }
 
+int mloam_keyframe_outlier(mloam_ctx_t *h, int id, mloam_point_t *h_pts, float *h_cov6, int cap, int *n) {
+  if (!h) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (n) *n = 0;
+  if (!c->kf) return fail(c, MLOAM_E_STATE, "keyframe_outlier: call mloam_keyframes_init first");
+  const KeyframeStore &S = *c->kf;
+  if (id < 0 || id >= (int)S.kfs.size()) return fail(c, MLOAM_E_INVALID, "keyframe_outlier: no such keyframe");
+  const KeyframeStore::Kf &k = S.kfs[id];
+  const int m = k.n[2];
+  if (n) *n = m;
+  if (!(h_pts || h_cov6) || m == 0) return MLOAM_OK;
+  if (m > cap) return fail(c, MLOAM_E_INVALID, "keyframe_outlier: capacity too small (*n holds the cloud's size)");
+  cudaSetDevice(c->device);
+  cudaStream_t st = c->stream;
+  const KfRecord rec = kf_record(S.chunks[k.chunk].p + k.off, k.n);
+  if (h_pts) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_pts, rec.pts[2], 16 * (size_t)m, cudaMemcpyDeviceToHost, st));
+  if (h_cov6) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_cov6, rec.cov6[2], 24 * (size_t)m, cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  return MLOAM_OK;
+}
+
 int mloam_global_map(mloam_ctx_t *h, int mode, const double *center7, double radius, double kf_leaf, float leaf, int *n_chosen, int *n_map0,
                      int *n_map1) {
   if (n_chosen) *n_chosen = 0;
@@ -636,10 +660,11 @@ int mloam_global_map(mloam_ctx_t *h, int mode, const double *center7, double rad
   const int n_ch = std::max(0, std::min(hc[0], n_cand));
   for (int i = 0; i < n_ch; i++) chosen.push_back((int)h_ds[i].w);
   // per chosen keyframe in filter order (:814-828 / :866-881): cloudUCTAssociateToMap of each cloud with the keyframe's pose and
-  // covariance and the context's current extrinsics and covariances (as mloam_keyframe_submap).  pubGlobalMap appends surf then
-  // corner to one map; saveGlobalMap appends surf to the surf map and corner to the corner map.  The outlier clouds the reference
-  // appends after surf (and after corner in pubGlobalMap) are not stored, i.e. empty.
+  // covariance and the context's current extrinsics and covariances (as mloam_keyframe_submap).  pubGlobalMap appends surf, corner
+  // and outlier to one map (:818-827); saveGlobalMap appends surf then outlier to the surf map and corner to the corner map
+  // (:873-882).  A keyframe saved without the outlier cloud has an empty one and adds no segment.
   const int n_maps = mode == MLOAM_GLOBAL_MAP_SURROUND ? 1 : 2;
+  static const int order_surround[3] = {0, 1, 2}, order_save[2][2] = {{0, 2}, {1, -1}};
   std::vector<UctSeg> segs;
   int seg_n[2] = {0, 0};
   size_t tot[2] = {0, 0};
@@ -647,8 +672,11 @@ int mloam_global_map(mloam_ctx_t *h, int mode, const double *center7, double rad
     for (int i = 0; i < n_ch; i++) {
       const KeyframeStore::Kf &k = S.kfs[chosen[i]];
       const KfRecord rec = kf_record(S.chunks[k.chunk].p + k.off, k.n);
-      for (int t = 0; t < 2; t++) {
-        if ((n_maps == 2 && t != m) || k.n[t] == 0) continue;
+      const int *order = n_maps == 1 ? order_surround : order_save[m];
+      const int n_order = n_maps == 1 ? 3 : 2;
+      for (int j = 0; j < n_order; j++) {
+        const int t = order[j];
+        if (t < 0 || k.n[t] == 0) continue;
         if (tot[m] + (size_t)k.n[t] > 0x7fffff00ull) return fail(c, MLOAM_E_INVALID, "global_map: more than 2^31 map points");
         segs.push_back(UctSeg{rec.pts[t], (int)tot[m], k.n[t], i});
         tot[m] += (size_t)k.n[t], seg_n[m]++;

@@ -236,6 +236,8 @@ struct FrameBufs {
   ExtractOut ex;
   float4 *corner_ds, *surf_ds;
   int *n_corner_ds, *n_surf_ds;  // device counts
+  float4 *first;                 // the LiDARs' first points (ExtractOut::first) and their flags
+  int *first_ok;
 };
 int frame_bufs(Ctx *c, int n, FrameBufs *F, int parity = 0) {
   const size_t N1 = (size_t)n + 16;
@@ -243,6 +245,7 @@ int frame_bufs(Ctx *c, int n, FrameBufs *F, int parity = 0) {
     F->ex.sharp = cv.take<float4>(N1), F->ex.less_sharp = cv.take<float4>(N1), F->ex.flat = cv.take<float4>(N1);
     F->ex.less_flat = cv.take<float4>(N1), F->corner_ds = cv.take<float4>(N1), F->surf_ds = cv.take<float4>(N1);
     F->ex.counts = cv.take<int>(16);  // [0..3]
+    F->first = cv.take<float4>(MLOAM_MAX_LIDARS), F->first_ok = cv.take<int>(MLOAM_MAX_LIDARS);
   }));
   F->n_corner_ds = F->ex.counts + 4, F->n_surf_ds = F->ex.counts + 5;
   return MLOAM_OK;
@@ -287,6 +290,7 @@ void stage_frame_inputs(Ctx *c, const double *pose7) {
   if (rig_merge(c)) stage_rig(c);
   else if (c->has_ext) stage_ext(c);
   if (c->with_ua) ua_stage_host(c);
+  if (c->outlier_on) stage_outlier(c);
 }
 
 // Whether the look-ahead of the previous frame made the features of sw: same caller pointer and sizes; a raw sweep's features are taken by
@@ -323,6 +327,10 @@ int features_enqueue(Ctx *c, const Sweep &sw, int parity, const Branch &side, Sc
     stamp(c, "front end");
     d_cloud = proj, d_scan_start = ss, d_scan_end = ss + n_scans;
   }
+  // every frame's extraction records each LiDAR's first point, so that features extracted ahead serve a frame with the outlier cloud on
+  const int n_parts = rig_merge(c) ? c->n_lidars : 1;
+  if (n_scans % n_parts == 0) F.ex.first = F.first, F.ex.first_ok = F.first_ok, F.ex.first_rings = n_scans / n_parts;  // else the merge
+                                                                                                                       // below rejects it
   rc = extract_device(c, d_cloud, n, d_scan_start, d_scan_end, n_scans, F.ex, nullptr, nullptr);
   if (rc) return rc;
   stamp(c, "extract");
@@ -358,6 +366,7 @@ int features_enqueue(Ctx *c, const Sweep &sw, int parity, const Branch &side, Sc
   if (fork_voxel) MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream, side.join, 0));
   stamp(c, "voxel (surf; corner on the side stream)");
   ScanRef S{F.surf_ds, n, F.n_surf_ds, F.corner_ds, less_cap, F.n_corner_ds};
+  S.first = F.ex.first, S.first_ok = F.ex.first_ok;
   *S_out = S;
   return MLOAM_OK;
 }
@@ -425,10 +434,16 @@ int frame_enqueue(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *
     nf.valid = true, nf.parity = parity ^ 1, nf.sw = nx;
   }
   stamp(c, have ? "features (prefetched)" : "extract + voxel");
+  const UaStage *d_ua = nullptr;
   if (c->with_ua) {  // downsampleCurrentScan's per-point uncertainty + trace gate: on the main stream with the covariances of THIS call
-    rc = ua_scan_stage(c, &S);
+    rc = ua_scan_stage(c, &S, &d_ua);
     if (rc) return rc;
     stamp(c, "uncertainty + gate");
+  }
+  if (c->outlier_on) {  // the outlier cloud (:366-418): the recorded first points -> base frame -> filter -> the same gate, one launch
+    rc = outlier_stage(c, &S, d_ua);
+    if (rc) return rc;
+    stamp(c, "outlier cloud");
   }
   if (fork_maps) {  // join the map-build branch
     MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream, c->br_maps.join, 0));
@@ -504,6 +519,8 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
   ScanRef S{};
   if (c->with_ua && c->nccl_comm)
     return fail(c, MLOAM_E_STATE, "frame: uncertainty-aware frames (mloam_set_uncertainty) are single-GPU only; detach the communicator or set with_ua = 0");
+  if (c->outlier_on && c->nccl_comm)  // turned on before the communicator was attached
+    return fail(c, MLOAM_E_STATE, "frame: the outlier cloud (mloam_set_outlier) is single-GPU only; detach the communicator or set it to 0");
   const bool want_cov = c->with_ua != 0;
   c->last_scan_valid = false;
   c->frame_from_graph = false;
@@ -526,6 +543,10 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
     key = fnv1a(key, c->lidar_ext, sizeof(double) * 7 * (size_t)c->n_lidars);
     key = fnv1a(key, &c->stream, sizeof(c->stream));
     key = fnv1a(key, &c->with_ua, sizeof(c->with_ua));  // the covariances and the threshold are staged, not part of the key
+    if (c->outlier_on) {  // the outlier stage's launch (its leaf is staged); a context that never turns it on keeps its keys
+      const int on = 1;
+      key = fnv1a(key, &on, sizeof(on));
+    }
     if (sw.raw) {  // raw frame: the per-LiDAR counts and the front-end parameters are kernel arguments of the captured front end
       key = fnv1a(key, &sw.L, sizeof(RigLayout));
       key = fnv1a(key, &c->front, sizeof(c->front));
@@ -1033,6 +1054,39 @@ int mloam_set_uncertainty(mloam_ctx_t *h, int with_ua, const double *ext_cov36, 
     for (int k = 0; k < 36; k++) c->ua_ext_cov[l][k] = l < n_lasers ? ext_cov36[36 * l + k] : 0.0;
   memcpy(c->ua_cov_meas, cov_meas9, sizeof(c->ua_cov_meas));
   c->ua_trace_threshold = trace_threshold;
+  return MLOAM_OK;
+}
+
+// ------------------------------------------------------------------------------------------ outlier cloud (segment_cloud: 0)
+int mloam_set_outlier(mloam_ctx_t *h, float map_outlier_res) {
+  if (!h || !(map_outlier_res >= 0.f) || map_outlier_res > 3.0e38f) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (c->nccl_comm || c->p2p_on)
+    return fail(c, MLOAM_E_STATE, "set_outlier: the outlier cloud is single-GPU only, like with_ua; detach the communicator");
+  c->outlier_on = map_outlier_res > 0.f;
+  c->outlier_leaf = c->outlier_on ? map_outlier_res : 0.f;
+  return MLOAM_OK;
+}
+
+int mloam_frame_outlier(mloam_ctx_t *h, mloam_point_t *h_pts, float *h_cov6, int cap, int *n) {
+  if (!h) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (n) *n = 0;
+  if (!c->last_scan_valid) return fail(c, MLOAM_E_STATE, "frame_outlier: no mloam_frame* call has run since the last reset");
+  const ScanRef &S = c->last_scan;
+  if (!S.d_n_outlier) return fail(c, MLOAM_E_STATE, "frame_outlier: the last frame ran without the outlier cloud (mloam_set_outlier)");
+  cudaSetDevice(c->device);
+  cudaStream_t st = c->stream;
+  int *hc = c->pinned->counts;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, S.d_n_outlier, sizeof(int), cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  const int m = hc[0];
+  if (n) *n = m;
+  if (!(h_pts || h_cov6) || m == 0) return MLOAM_OK;
+  if (m > cap) return fail(c, MLOAM_E_INVALID, "frame_outlier: capacity too small (*n holds the cloud's size)");
+  if (h_pts) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_pts, S.outlier, sizeof(float4) * (size_t)m, cudaMemcpyDeviceToHost, st));
+  if (h_cov6) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_cov6, S.cov6_outlier, sizeof(float) * 6 * (size_t)m, cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
   return MLOAM_OK;
 }
 

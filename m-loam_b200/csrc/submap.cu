@@ -252,7 +252,7 @@ void ua_stage_host(Ctx *c) {
   }
 }
 
-int ua_scan_stage(Ctx *c, Ctx::ScanRef *S) {
+int ua_scan_stage(Ctx *c, Ctx::ScanRef *S, const UaStage **d_cfg_out) {
   const int ncap[2] = {S->n_corner, S->n_surf};
   const float4 *pts[2] = {S->corner, S->surf};
   const int *d_n[2] = {S->d_n_corner, S->d_n_surf};
@@ -272,6 +272,7 @@ int ua_scan_stage(Ctx *c, Ctx::ScanRef *S) {
     }
   }));
   ua_stage_host(c);
+  if (d_cfg_out) *d_cfg_out = d_cfg;
   cudaStream_t st = c->stream;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_cfg, &c->pinned->ua, sizeof(UaStage), cudaMemcpyHostToDevice, st));
   const UctFrame f_unused{};
@@ -291,6 +292,147 @@ int ua_scan_stage(Ctx *c, Ctx::ScanRef *S) {
     if (t == 0) S->corner = out[t], S->d_n_corner = b.count, S->sinfo_corner = osinfo[t], S->cov6_corner = ocov6[t];
     else S->surf = out[t], S->d_n_surf = b.count, S->sinfo_surf = osinfo[t], S->cov6_surf = ocov6[t];
   }
+  return MLOAM_OK;
+}
+
+// ---- the outlier cloud of a frame with segment_cloud: 0 (lidar_mapper_keyframe.cpp:366-418).  ImageSegmenter::segmentCloud pushes one
+// point per LiDAR into laser_cloud_outlier, the first point of its ring-ordered cloud (image_segmenter.hpp:390; the extraction recorded
+// it, ExtractOut::first), pubPointCloud moves it to the base frame with the float extrinsic, intensity = n (visualization.cpp:40-52,
+// :89-104), and downsampleCurrentScan filters the merged cloud with VoxelGridCovarianceMLOAM<PointI>(MAP_OUTLIER_RES) (:366-368) and
+// gates it as the scans (:407-418).  At most MLOAM_MAX_LIDARS points: one warp, the filter on lane 0.
+void stage_outlier(Ctx *c) {
+  OutlierStage *o = &c->pinned->outlier;
+  memset(o, 0, sizeof(*o));
+  const bool merged = c->n_lidars > 1 || c->lidar_merge;
+  o->leaf = c->outlier_leaf, o->n_lasers = merged ? c->n_lidars : 1;
+  for (int l = 0; l < o->n_lasers; l++) {
+    // Pose(qbl, tbl).T_.cast<float>() (pose.cpp:34-41); in the single-LiDAR path the extrinsic of mloam_set_extrinsic, identity without one
+    const double *e = merged ? c->lidar_ext[l] : c->ext;
+    const M33 R = qmat(qnormalized(Q4{e[3], e[4], e[5], e[6]}));
+    for (int r = 0; r < 3; r++) {
+      for (int k = 0; k < 3; k++) o->mat[l][4 * r + k] = (float)R.m[3 * r + k];
+      o->mat[l][4 * r + 3] = (float)e[r];
+    }
+  }
+}
+
+namespace {
+
+// VoxelGridCovarianceMLOAM<PointI>::filter of a few points, serially (the indexing of pcl::VoxelGrid, voxel_grid_covariance_mloam_impl.hpp
+// :84-116, :206-250: bounding box over the finite points, voxel index, a stable sort by index, per voxel the float mean of x, y, z
+// accumulated in sorted order and the LAST point's intensity, :417-418,428).  An index space over int32 returns the input (:92-101).
+__device__ int voxel_few(const float4 *in, int n, float inv, float4 *out) {
+  float mn[3] = {3.4028235e38f, 3.4028235e38f, 3.4028235e38f}, mx[3] = {-3.4028235e38f, -3.4028235e38f, -3.4028235e38f};
+  int n_fin = 0;
+  for (int i = 0; i < n; i++) {
+    const float4 p = in[i];
+    if (!isfinite(p.x) || !isfinite(p.y) || !isfinite(p.z)) continue;
+    n_fin++;
+    mn[0] = fminf(mn[0], p.x), mn[1] = fminf(mn[1], p.y), mn[2] = fminf(mn[2], p.z);
+    mx[0] = fmaxf(mx[0], p.x), mx[1] = fmaxf(mx[1], p.y), mx[2] = fmaxf(mx[2], p.z);
+  }
+  if (n_fin == 0) return 0;
+  const long long dx = (long long)((mx[0] - mn[0]) * inv) + 1, dy = (long long)((mx[1] - mn[1]) * inv) + 1,
+                  dz = (long long)((mx[2] - mn[2]) * inv) + 1;
+  if (dx * dy * dz > 2147483647ll) {
+    for (int i = 0; i < n; i++) out[i] = in[i];
+    return n;
+  }
+  int minb[3], divb[3];
+  for (int d = 0; d < 3; d++) {
+    minb[d] = (int)floorf(mn[d] * inv);
+    divb[d] = (int)floorf(mx[d] * inv) - minb[d] + 1;
+  }
+  const int mul[3] = {1, divb[0], divb[0] * divb[1]};
+  unsigned key[MLOAM_MAX_LIDARS];
+  int ord[MLOAM_MAX_LIDARS], m = 0;
+  for (int i = 0; i < n; i++) {
+    const float4 p = in[i];
+    if (!isfinite(p.x) || !isfinite(p.y) || !isfinite(p.z)) continue;
+    const int i0 = (int)(floorf(p.x * inv) - (float)minb[0]), i1 = (int)(floorf(p.y * inv) - (float)minb[1]),
+              i2 = (int)(floorf(p.z * inv) - (float)minb[2]);
+    const unsigned k = (unsigned)(i0 * mul[0] + i1 * mul[1] + i2 * mul[2]);
+    int j = m++;  // insertion: equal keys keep their input order
+    while (j > 0 && key[j - 1] > k) key[j] = key[j - 1], ord[j] = ord[j - 1], j--;
+    key[j] = k, ord[j] = i;
+  }
+  int n_out = 0;
+  for (int a = 0; a < m;) {
+    int b = a + 1;
+    while (b < m && key[b] == key[a]) b++;
+    float sx = 0.f, sy = 0.f, sz = 0.f;
+    for (int j = a; j < b; j++) sx = sx + in[ord[j]].x, sy = sy + in[ord[j]].y, sz = sz + in[ord[j]].z;
+    const float cnt = (float)(b - a);
+    out[n_out++] = make_float4(sx / cnt, sy / cnt, sz / cnt, in[ord[b - 1]].w);
+    a = b;
+  }
+  return n_out;
+}
+
+// first[l] / first_ok[l]: the recorded first points; ua (nullable): the frame's with_ua configuration (the gate), else zero cov_vec
+__global__ void __launch_bounds__(32) k_outlier_scan(const float4 *__restrict__ first, const int *__restrict__ first_ok, const OutlierStage *__restrict__ cfg,
+                                                     const UaStage *__restrict__ ua, float4 *__restrict__ out, float *__restrict__ cov6_out,
+                                                     int *__restrict__ n_out) {
+  __shared__ float4 raw[MLOAM_MAX_LIDARS], ds[MLOAM_MAX_LIDARS], gated[MLOAM_MAX_LIDARS];
+  __shared__ float cov6[6 * MLOAM_MAX_LIDARS], trace[MLOAM_MAX_LIDARS];
+  __shared__ int n_ds;
+  const int lane = threadIdx.x;
+  const int L = cfg->n_lasers;
+  if (lane == 0) {
+    int n = 0;
+    for (int l = 0; l < L; l++) {
+      if (!first_ok[l]) continue;  // an empty part pushes no point (laser_cloud_out.points[0] of an empty cloud is not read)
+      const float4 p = first[l];
+      const float *m = cfg->mat[l];
+      // pcl::transformPointCloud (PCL 1.8 transforms.hpp): x' = m00 x + m01 y + m02 z + m03, float, left to right; intensity = n
+      float4 o;
+      o.x = m[0] * p.x + m[1] * p.y + m[2] * p.z + m[3];
+      o.y = m[4] * p.x + m[5] * p.y + m[6] * p.z + m[7];
+      o.z = m[8] * p.x + m[9] * p.y + m[10] * p.z + m[11];
+      o.w = (float)l;
+      raw[n++] = o;
+    }
+    n_ds = voxel_few(raw, n, 1.0f / cfg->leaf, ds);
+  }
+  __syncthreads();
+  UctFrame f;
+  if (ua) {
+    f = ua->frame;
+  } else {  // with_ua = false: PointIWithCov(point_ori, Zero) (:407-418)
+    memset(&f, 0, sizeof(f));
+    f.n_lasers = L, f.scan_frame = 1;
+  }
+  const int nd = n_ds;
+  int keep = 0;
+  if (lane < nd) keep = uct_point(ds[lane], f, f.pose_global, ua ? ua->lasers : nullptr, (size_t)lane, gated, cov6, trace);
+  const unsigned mask = __ballot_sync(0xffffffffu, keep);
+  if (keep) {
+    const int o = __popc(mask & ((1u << lane) - 1u));
+    out[o] = gated[lane];
+#pragma unroll
+    for (int k = 0; k < 6; k++) cov6_out[6 * o + k] = cov6[6 * lane + k];
+  }
+  if (lane == 0) *n_out = __popc(mask);
+}
+
+}  // namespace
+
+int outlier_stage(Ctx *c, Ctx::ScanRef *S, const UaStage *d_ua) {
+  if (!S->first) return fail(c, MLOAM_E_STATE, "frame: the sweep's first points were not recorded");
+  OutlierStage *d_cfg = nullptr;
+  float4 *out = nullptr;
+  float *cov6 = nullptr;
+  int *cnt = nullptr;
+  MLOAM_CUDA_OK(c, carve(c->outlier, [&](Carve &cv) {
+    d_cfg = cv.take<OutlierStage>(1), out = cv.take<float4>(MLOAM_MAX_LIDARS), cov6 = cv.take<float>(6 * MLOAM_MAX_LIDARS), cnt = cv.take<int>(16);
+  }));
+  stage_outlier(c);
+  cudaStream_t st = c->stream;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_cfg, &c->pinned->outlier, sizeof(OutlierStage), cudaMemcpyHostToDevice, st));
+  k_outlier_scan<<<1, 32, 0, st>>>(S->first, S->first_ok, d_cfg, d_ua, out, cov6, cnt);
+  c->launches++;
+  MLOAM_CUDA_OK(c, cudaGetLastError());
+  S->outlier = out, S->cov6_outlier = cov6, S->d_n_outlier = cnt;
   return MLOAM_OK;
 }
 
