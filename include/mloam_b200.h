@@ -343,6 +343,27 @@ int mloam_set_outlier(mloam_ctx_t *ctx, float map_outlier_res);
 int mloam_frame_outlier(mloam_ctx_t *ctx, mloam_point_t *h_pts, float *h_cov6, int cap, int *n);
 int mloam_keyframe_outlier(mloam_ctx_t *ctx, int id, mloam_point_t *h_pts, float *h_cov6, int cap, int *n);
 
+/* ---- DISTORTION: motion compensation of each sweep's features before the mapper sees them (Estimator::process, estimator.cpp:545-590
+ *      -> undistortMeasurements :376-408 -> TransformToEnd, utility.h:54-100).  Off by default.
+ * mloam_undistort_poses (host only, no context): pose_undist of a sweep from the odometry's relative pose pose_rlt7 of LiDAR idx_ref:
+ *   pose_undist[n] = Pose(qbl_n, tbl_n)^-1 * pose_rlt * Pose(qbl_n, tbl_n) for every LiDAR n (Pose::inverse / operator*, each Pose
+ *   normalising its quaternion); then out7s[n] = pose_undist[n] when estimate_extrinsic == 2, else pose_undist[idx_ref] for EVERY LiDAR
+ *   (the reference's :403-405).  ext7s / out7s: n_lidars x [t q]; the extrinsics' quaternions are normalised (Pose(qbl_n, tbl_n)).
+ *   pose_rlt7 is taken as the odometry's Pose holds it, i.e. with a unit quaternion, and is not normalised again: normalising an
+ *   already-normalised quaternion can move its last bits, and the reference uses pose_rlt_[IDX_REF] as stored.
+ * mloam_set_distortion: on = 1 with SCAN_PERIOD (> 0, e.g. 0.1), 0 off.  MLOAM_E_STATE on a context with a communicator.
+ * mloam_frame_undistort: the poses of the sweep of the NEXT mloam_frame* call, n_lidars x [t q] as mloam_undistort_poses returns them
+ *   (n_lidars: the LiDARs of mloam_set_lidars, 1 in the single-LiDAR path without its extrinsics); used as given.  A pose is consumed by
+ *   one call; with the feature on, a frame call without one gets MLOAM_E_STATE, with a wrong count MLOAM_E_INVALID.
+ *   With it on, every mloam_frame* call moves each LiDAR's corner_points_less_sharp and surf_points_less_flat, in the LiDAR's frame, with
+ *   TransformToEnd(p, pose[n], true, SCAN_PERIOD) — s = (intensity - int(intensity)) / SCAN_PERIOD in float, Eigen's slerp from the
+ *   identity, float stores — before the rig merge (or mloam_set_extrinsic's transform) and the scan filters: one more launch.  The sharp
+ *   and flat clouds and the outlier cloud (mloam_set_outlier) are not moved.  With the look-ahead the announced sweep is extracted ahead
+ *   and the rest runs at its call.  The poses are staged: a captured frame replays with new ones. */
+int mloam_undistort_poses(const double *pose_rlt7, int idx_ref, int n_lidars, const double *ext7s, int estimate_extrinsic, double *out7s);
+int mloam_set_distortion(mloam_ctx_t *ctx, int on, float scan_period);
+int mloam_frame_undistort(mloam_ctx_t *ctx, int n_lidars, const double *pose7);
+
 /* ---- the mapper's keyframe store, kept on the device: saveKeyframe -> clearCloud -> extractSurroundingKeyFrames
  *      (lidar_mapper_keyframe.cpp:641-683, :921-927 at :1101, :254-354).  The mapper loop of process() (:1062-1101) becomes
  *        mloam_set_lidars / mloam_set_uncertainty (the frame's /extrinsics, :1028-1046, read BEFORE the submap as the reference does:

@@ -36,6 +36,7 @@ ABI_SYMBOLS = [
     "mloam_global_map", "mloam_global_map_read", "mloam_global_map_chosen",
     "mloam_cal_timestamp", "mloam_set_front_end", "mloam_front_end", "mloam_frame_raw", "mloam_frame_raw_device", "mloam_frame_set_next_raw",
     "mloam_frame_set_next_raw_device", "mloam_set_outlier", "mloam_frame_outlier", "mloam_keyframe_outlier",
+    "mloam_undistort_poses", "mloam_set_distortion", "mloam_frame_undistort",
 ]
 
 
@@ -125,6 +126,18 @@ def default_params() -> Params:
     p = Params()
     lib().mloam_default_params(C.byref(p))
     return p
+
+
+def undistort_poses(pose_rlt7, idx_ref: int, ext7s, estimate_extrinsic: int = 0) -> np.ndarray:
+    """mloam_undistort_poses: the pose each LiDAR's features are undistorted with, [n_lidars, 7] ([t q]), from the odometry's relative pose
+    of LiDAR idx_ref and the extrinsics [n_lidars, 7] (every LiDAR takes idx_ref's unless estimate_extrinsic == 2)."""
+    r = np.ascontiguousarray(pose_rlt7, np.float64).reshape(7)
+    e = np.ascontiguousarray(ext7s, np.float64).reshape(-1, 7)
+    out = np.zeros_like(e)
+    rc = lib().mloam_undistort_poses(_p(r), int(idx_ref), e.shape[0], _p(e), int(estimate_extrinsic), _p(out))
+    if rc != 0:
+        raise ValueError(f"mloam_undistort_poses: {rc}")
+    return out
 
 
 def _cloud(a) -> np.ndarray:
@@ -598,6 +611,16 @@ class Context:
         cp, cc = np.zeros((max(nc.value, 1), 4), np.float32), np.zeros((max(nc.value, 1), 6), np.float32)
         self._ck(lib().mloam_frame_scan(self._h, _p(sp), _p(sc), sp.shape[0], C.byref(ns), _p(cp), _p(cc), cp.shape[0], C.byref(nc)))
         return sp[:ns.value].copy(), sc[:ns.value].copy(), cp[:nc.value].copy(), cc[:nc.value].copy()
+
+    def set_distortion(self, on: bool, scan_period: float = 0.1):
+        """DISTORTION (mloam_set_distortion): motion-compensate each sweep's less-sharp and less-flat features with the pose given by
+        frame_undistort before every frame call.  Call after set_lidars."""
+        self._ck(lib().mloam_set_distortion(self._h, int(bool(on)), C.c_float(scan_period)))
+
+    def frame_undistort(self, pose7s):
+        """The per-LiDAR pose_undist [n_lidars, 7] ([t q], as undistort_poses returns it) of the sweep of the next frame call."""
+        p = np.ascontiguousarray(pose7s, np.float64).reshape(-1, 7)
+        self._ck(lib().mloam_frame_undistort(self._h, p.shape[0], _p(p)))
 
     def set_outlier(self, map_outlier_res: float):
         """The outlier cloud of segment_cloud: 0 (mloam_set_outlier): leaf MAP_OUTLIER_RES > 0 turns it on, 0 off.  Call after set_lidars."""

@@ -8,6 +8,7 @@
 #include "../../include/mloam_b200.h"
 #include "common.cuh"
 #include "layout.h"
+#include "undistort.cuh"
 
 namespace mloam {
 
@@ -175,6 +176,13 @@ struct OutlierStage {
   int pad[2];
   float mat[MLOAM_MAX_LIDARS][12];   // per LiDAR the float 3x4 extrinsic of pubPointCloud's transformPointCloud (identity without one)
 };
+// the configuration of a frame's undistortion (mloam_set_distortion / mloam_frame_undistort; undistort.cu), copied to the device as one block
+struct UndistStage {
+  float scan_period;                       // SCAN_PERIOD
+  int n_lidars;                            // staged poses (the frame's LiDARs; 1 in the single-LiDAR path)
+  int pad[2];
+  ud::UndistPose pose[MLOAM_MAX_LIDARS];   // per LiDAR the pose TransformToEnd moves its features with
+};
 
 // The context's pinned host block (Ctx::pinned): staging of small host-to-device copies and landing of small read-backs, so that
 // they are truly asynchronous.
@@ -186,6 +194,7 @@ struct PinnedBlock {
   float rig[MLOAM_MAX_LIDARS][12];  // features_enqueue: the rig's float 3x4 extrinsics of the merge
   UaStage ua;                       // ua_scan_stage: the with_ua configuration
   OutlierStage outlier;             // outlier_stage: the outlier cloud's configuration
+  UndistStage undist;               // undistort_stage: the sweep's poses
   // Written by captured copies (landing of a frame's results) and by the host-buffer entry points, one call at a time
   LMState lm;                       // LMState mirror
   int counts[192];                  // count read-backs; mloam_project_cloud: [0] count, [64..] scan starts, [128..] scan ends
@@ -228,7 +237,6 @@ struct DevCtl {
   double normal_eq[32];                 // mloam_normal_equations
   double pose_plus[64];                 // mloam_pose_plus
   float rig[MLOAM_MAX_LIDARS][12];      // PinnedBlock::rig
-  int merge_off[2 * (MLOAM_MAX_LIDARS + 1)];  // merge_lidars_device: per-LiDAR feature offsets
   KnnPathStats knn_stats;
 };
 
@@ -373,6 +381,8 @@ struct Ctx {
     int parity = 0;
     Sweep sw;                   // the sweep they were extracted from
     ScanRef S{};
+    bool extract_only = false;  // the undistortion was on: the half holds the extraction only (undistortion, merge and the scan
+                                // filters run at the frame call, which knows the sweep's pose)
   };
   struct NextSweep {
     bool set = false;
@@ -461,6 +471,15 @@ struct Ctx {
   bool outlier_on = false;
   float outlier_leaf = 0.f;
   DevBuf outlier;                  // the staged configuration, the frame's outlier cloud (points, cov_vec) and its count
+  // DISTORTION (mloam_set_distortion): TransformToEnd of each LiDAR's less-sharp and less-flat features with the pose of
+  // mloam_frame_undistort (estimator.cpp:545-590, :376-408), one launch before the rig merge.  The poses reach the device through the
+  // pinned block (PinnedBlock::undist), so a captured frame replays with new ones.  A pose is consumed by one mloam_frame* call.
+  bool undist_on = false;
+  float undist_scan_period = 0.1f;
+  bool undist_set = false;         // a pose was given for the next mloam_frame* call
+  int undist_n = 0;
+  double undist_pose7[MLOAM_MAX_LIDARS][7];
+  DevBuf undist;                   // the staged configuration
   double pose_cov36[36] = {0};     // pose_wmap_curr.cov_ of the last mloam_frame* / mloam_scan2map* call
   bool last_scan_valid = false;    // last_scan describes the scan of the last mloam_frame* call (mloam_frame_scan)
   ScanRef last_scan{};
@@ -601,6 +620,11 @@ struct ExtractOut {
 };
 int extract_device(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start, const int *d_scan_end, int n_scans,
                    ExtractOut out, float *d_curv_or_null, int *d_label_or_null);
+// undistort.cu: TransformToEnd in place of the extraction's less-sharp (capacity cap_less, count out.counts[1]) and less-flat (cap_flat,
+// out.counts[3]) features on c->stream, LiDAR l's with the staged pose l; d_off (nullable, the rig's per-LiDAR offsets of the two clouds,
+// 2 x (n_lidars + 1)) finds a point's LiDAR, without it every point is LiDAR 0's.  One launch.  stage_undistort writes PinnedBlock::undist.
+int undistort_stage(Ctx *c, ExtractOut out, int cap_less, int cap_flat, const int *d_off, int n_lidars);
+void stage_undistort(Ctx *c);
 // extract_device's work in Ctx::extract_work for n points in n_scans rings
 struct RingStage;
 struct ExtractWork {
@@ -632,9 +656,11 @@ int voxel_downsample_cov_device(Ctx *c, const float4 *d_in, const float *d_cov6,
 void scan_exclusive(Ctx *c, const int *d_in, int *d_out, int n, int *d_tmp, int *d_total);
 // After a batched extraction over the concatenated sweeps of n_lidars LiDARs: move the less-sharp / less-flat features of LiDAR l into
 // the base frame with its float 3x4 extrinsic d_ext12[l] and set intensity = l (transformCloudFeature, visualization.cpp:40-52).
-// d_off: scratch for 2 x (n_lidars + 1) ints.
-int merge_lidars_device(Ctx *c, ExtractOut out, int n_cap_less, int n_cap_lflat, int n_lidars, int rings_per_lidar, const float *d_ext12,
-                        int *d_off);
+// d_off: the per-LiDAR offsets lidar_offsets_device wrote for this extraction.
+int merge_lidars_device(Ctx *c, ExtractOut out, int n_cap_less, int n_cap_lflat, int n_lidars, const float *d_ext12, const int *d_off);
+// Right after that batched extraction (it reads the extraction's per-ring counts in Ctx::extract_work): where each LiDAR's less-sharp
+// and less-flat features begin, d_off[0 .. n_lidars] and d_off[n_lidars + 1 .. 2 n_lidars + 1].  One launch.
+int lidar_offsets_device(Ctx *c, int n_lidars, int rings_per_lidar, int *d_off);
 // d_n_in (nullable): device-side input count (n is then the upper bound the kernels are sized for).
 int voxel_downsample_device(Ctx *c, const float4 *d_in, int n, const int *d_n_in, float leaf, int intensity_last, float4 *d_out,
                             int *d_n_out, DevBuf &work);

@@ -1197,16 +1197,26 @@ __global__ void k_merge_transform(float4 *__restrict__ pts, const int *__restric
   pts[i] = o;
 }
 
-int merge_lidars_device(Ctx *c, ExtractOut out, int n_cap_less, int n_cap_lflat, int n_lidars, int rings_per_lidar, const float *d_ext12, int *d_off) {
+int lidar_offsets_device(Ctx *c, int n_lidars, int rings_per_lidar, int *d_off) {
   if (n_lidars < 1 || n_lidars > MLOAM_MAX_LIDARS || !c->d_ring_stage) {
     c->err = "merge_lidars: 1..16 LiDARs, after an extraction";
     return MLOAM_E_INVALID;
   }
+  k_lidar_offsets<<<1, 32, 0, c->stream>>>(static_cast<const RingStage *>(c->d_ring_stage), c->d_ring_cnt, rings_per_lidar, n_lidars, d_off);
+  c->launches++;
+  MLOAM_CUDA_OK(c, cudaGetLastError());
+  return MLOAM_OK;
+}
+
+int merge_lidars_device(Ctx *c, ExtractOut out, int n_cap_less, int n_cap_lflat, int n_lidars, const float *d_ext12, const int *d_off) {
+  if (n_lidars < 1 || n_lidars > MLOAM_MAX_LIDARS) {
+    c->err = "merge_lidars: 1..16 LiDARs";
+    return MLOAM_E_INVALID;
+  }
   cudaStream_t st = c->stream;
-  k_lidar_offsets<<<1, 32, 0, st>>>(static_cast<const RingStage *>(c->d_ring_stage), c->d_ring_cnt, rings_per_lidar, n_lidars, d_off);
   if (n_cap_less > 0) k_merge_transform<<<(n_cap_less + 255) / 256, 256, 0, st>>>(out.less_sharp, d_off, n_lidars, d_ext12);
   if (n_cap_lflat > 0) k_merge_transform<<<(n_cap_lflat + 255) / 256, 256, 0, st>>>(out.less_flat, d_off + n_lidars + 1, n_lidars, d_ext12);
-  c->launches += 3;
+  c->launches += 2;
   MLOAM_CUDA_OK(c, cudaGetLastError());
   return MLOAM_OK;
 }

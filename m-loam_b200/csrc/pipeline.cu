@@ -238,6 +238,7 @@ struct FrameBufs {
   int *n_corner_ds, *n_surf_ds;  // device counts
   float4 *first;                 // the LiDARs' first points (ExtractOut::first) and their flags
   int *first_ok;
+  int *off;                      // rig merge: per-LiDAR offsets of the less-sharp and less-flat features (lidar_offsets_device)
 };
 int frame_bufs(Ctx *c, int n, FrameBufs *F, int parity = 0) {
   const size_t N1 = (size_t)n + 16;
@@ -246,6 +247,7 @@ int frame_bufs(Ctx *c, int n, FrameBufs *F, int parity = 0) {
     F->ex.less_flat = cv.take<float4>(N1), F->corner_ds = cv.take<float4>(N1), F->surf_ds = cv.take<float4>(N1);
     F->ex.counts = cv.take<int>(16);  // [0..3]
     F->first = cv.take<float4>(MLOAM_MAX_LIDARS), F->first_ok = cv.take<int>(MLOAM_MAX_LIDARS);
+    F->off = cv.take<int>(2 * (MLOAM_MAX_LIDARS + 1));
   }));
   F->n_corner_ds = F->ex.counts + 4, F->n_surf_ds = F->ex.counts + 5;
   return MLOAM_OK;
@@ -291,6 +293,7 @@ void stage_frame_inputs(Ctx *c, const double *pose7) {
   else if (c->has_ext) stage_ext(c);
   if (c->with_ua) ua_stage_host(c);
   if (c->outlier_on) stage_outlier(c);
+  if (c->undist_on) stage_undistort(c);
 }
 
 // Whether the look-ahead of the previous frame made the features of sw: same caller pointer and sizes; a raw sweep's features are taken by
@@ -299,15 +302,14 @@ bool frame_has_prefetched(const Ctx *c, const Sweep &sw) {
   const Ctx::Features &f = c->prefetched;
   const bool same_kind = sw.raw ? (f.sw.raw && std::memcmp(&f.sw.L, &sw.L, sizeof(RigLayout)) == 0) : !f.sw.raw;
   return f.valid && c->use_lookahead && !c->prof_on && f.sw.key == sw.key && f.sw.n == sw.n && f.sw.n_scans == sw.n_scans && same_kind &&
-         (f.sw.host || !sw.host);
+         (f.sw.host || !sw.host) && f.extract_only == c->undist_on;
 }
 
-// extractCloud + (multi-LiDAR merge | base-frame transform) + downsampleCurrentScan of sweep sw on c->stream, into half `parity` of the
-// feature double buffer; the corner filter forks onto branch `side`.  A raw sweep goes through the front end (removeNaN + calTimestamp +
-// projection, Ctx::front) first, which makes the ring-ordered sweep and its ScanInfo on the device; extraction takes them with the raw
-// size n as capacity (no count comes back to the host).
-int features_enqueue(Ctx *c, const Sweep &sw, int parity, const Branch &side, ScanRef *S_out) {
-  const mloam_params_t &P = c->params;
+// extractCloud of sweep sw on c->stream into half `parity` of the feature double buffer (*F), with the LiDARs' first points and, for the
+// rig merge, each LiDAR's feature offsets — everything that reads Ctx::extract_work.  A raw sweep goes through the front end (removeNaN +
+// calTimestamp + projection, Ctx::front) first, which makes the ring-ordered sweep and its ScanInfo on the device; extraction takes them
+// with the raw size n as capacity (no count comes back to the host).
+int extract_enqueue(Ctx *c, const Sweep &sw, int parity, FrameBufs *F_out) {
   const int n = sw.n, n_scans = sw.n_scans;
   FrameBufs F;
   int rc = frame_bufs(c, n, &F, parity);
@@ -333,16 +335,35 @@ int features_enqueue(Ctx *c, const Sweep &sw, int parity, const Branch &side, Sc
                                                                                                                        // below rejects it
   rc = extract_device(c, d_cloud, n, d_scan_start, d_scan_end, n_scans, F.ex, nullptr, nullptr);
   if (rc) return rc;
+  if (rig_merge(c)) {  // the merge below may run later (undistortion on): each LiDAR's offsets are kept with the sweep's features
+    if (n_scans % c->n_lidars != 0) return fail(c, MLOAM_E_INVALID, "frame: n_scans must be n_lidars x rings per LiDAR");
+    rc = lidar_offsets_device(c, c->n_lidars, n_scans / c->n_lidars, F.off);
+    if (rc) return rc;
+  }
   stamp(c, "extract");
+  *F_out = F;
+  return MLOAM_OK;
+}
+
+// [undistortion] + (multi-LiDAR merge | base-frame transform) + downsampleCurrentScan of the features extract_enqueue left in F, on
+// c->stream; the corner filter forks onto branch `side`.
+int scan_enqueue(Ctx *c, const Sweep &sw, const FrameBufs &F, const Branch &side, ScanRef *S_out) {
+  const mloam_params_t &P = c->params;
+  const int n = sw.n, n_scans = sw.n_scans;
+  int rc;
   const int less_cap = n < 120 * n_scans ? n : 120 * n_scans;  // <= 20 less-sharp picks x 6 sectors per ring
   DevCtl *ctl = c->ctl.as<DevCtl>();
+  if (c->undist_on) {  // undistortMeasurements (estimator.cpp:376-408): each LiDAR's less-* features in its own frame, before the merge
+    rc = undistort_stage(c, F.ex, less_cap, n, rig_merge(c) ? F.off : nullptr, rig_merge(c) ? c->n_lidars : 1);
+    if (rc) return rc;
+    stamp(c, "undistort");
+  }
   if (rig_merge(c)) {
     // batched sweeps of several LiDARs: features of LiDAR l go to the base frame with its extrinsic, intensity = l
     // (transformCloudFeature, visualization.cpp:40-52), LiDAR after LiDAR as pubPointCloud's `+=` (:93-104)
-    if (n_scans % c->n_lidars != 0) return fail(c, MLOAM_E_INVALID, "frame: n_scans must be n_lidars x rings per LiDAR");
     stage_rig(c);
     MLOAM_CUDA_OK(c, cudaMemcpyAsync(ctl->rig, c->pinned->rig, sizeof(float) * 12 * c->n_lidars, cudaMemcpyHostToDevice, c->stream));
-    rc = merge_lidars_device(c, F.ex, less_cap, n, c->n_lidars, n_scans / c->n_lidars, &ctl->rig[0][0], ctl->merge_off);
+    rc = merge_lidars_device(c, F.ex, less_cap, n, c->n_lidars, &ctl->rig[0][0], F.off);
     if (rc) return rc;
   } else if (c->has_ext) {  // features are handed to the mapper in the base frame
     stage_ext(c);
@@ -369,6 +390,14 @@ int features_enqueue(Ctx *c, const Sweep &sw, int parity, const Branch &side, Sc
   S.first = F.ex.first, S.first_ok = F.ex.first_ok;
   *S_out = S;
   return MLOAM_OK;
+}
+
+// The features of sweep sw, all steps: extract_enqueue + scan_enqueue
+int features_enqueue(Ctx *c, const Sweep &sw, int parity, const Branch &side, ScanRef *S_out) {
+  FrameBufs F;
+  int rc = extract_enqueue(c, sw, parity, &F);
+  if (rc) return rc;
+  return scan_enqueue(c, sw, F, side, S_out);
 }
 
 // mloam_frame copied inputs on a branch's stream outside of any capture, recorded in ev.  Run on that branch (forked), the stream path is
@@ -412,26 +441,39 @@ int frame_enqueue(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *
   c->stamp_n = 0;
   stamp(c, "start");
   ScanRef S{};
-  if (have) S = c->prefetched.S;
+  if (have && !c->prefetched.extract_only) S = c->prefetched.S;
   c->prefetched.valid = false;  // half `parity` is taken or overwritten here
   if (!have) {
     rc = features_enqueue(c, sw, parity, c->br_scan, &S);
     if (rc) return rc;
+  } else if (c->prefetched.extract_only) {  // undistortion on: the look-ahead extracted; this sweep's pose is known now
+    FrameBufs F;
+    rc = frame_bufs(c, sw.n, &F, parity);
+    F.ex.first = F.first, F.ex.first_ok = F.first_ok;  // recorded by the look-ahead's extraction (extract_enqueue)
+    if (rc == MLOAM_OK) rc = scan_enqueue(c, sw, F, c->br_scan, &S);
+    if (rc) return rc;
   }
   // look-ahead: the announced next sweep goes through the same steps on br_ahead into the other half while this frame is matched
-  // and solved (it reuses Ctx::extract_work, voxel_corner and voxel_surf of the block above, hence the fork AFTER it)
+  // and solved (it reuses Ctx::extract_work, voxel_corner and voxel_surf of the block above, hence the fork AFTER it).  With the
+  // undistortion on, the next sweep's pose comes with the next call: the branch extracts only (extract_work), and that call runs
+  // undistortion, merge and the scan filters on the main stream before it forks its own look-ahead.
   Ctx::Features nf{};
   if (c->next.set && c->use_lookahead && !c->prof_on) {
     const Sweep &nx = c->next.sw;
     c->stamp_mute = true;
     rc = on_branch(c, c->br_ahead, true, [&] {
       int r = c->next_pending ? wait_uploads(c, c->ev_next, true) : MLOAM_OK;  // mloam_frame copied the next sweep on br_ahead
-      if (r == MLOAM_OK) r = features_enqueue(c, nx, parity ^ 1, c->br_ahead_scan, &nf.S);
+      if (r == MLOAM_OK && c->undist_on) {
+        FrameBufs F;
+        r = extract_enqueue(c, nx, parity ^ 1, &F);
+      } else if (r == MLOAM_OK) {
+        r = features_enqueue(c, nx, parity ^ 1, c->br_ahead_scan, &nf.S);
+      }
       return r;
     });
     c->stamp_mute = false;
     if (rc) return rc;
-    nf.valid = true, nf.parity = parity ^ 1, nf.sw = nx;
+    nf.valid = true, nf.parity = parity ^ 1, nf.sw = nx, nf.extract_only = c->undist_on;
   }
   stamp(c, have ? "features (prefetched)" : "extract + voxel");
   const UaStage *d_ua = nullptr;
@@ -521,6 +563,8 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
     return fail(c, MLOAM_E_STATE, "frame: uncertainty-aware frames (mloam_set_uncertainty) are single-GPU only; detach the communicator or set with_ua = 0");
   if (c->outlier_on && c->nccl_comm)  // turned on before the communicator was attached
     return fail(c, MLOAM_E_STATE, "frame: the outlier cloud (mloam_set_outlier) is single-GPU only; detach the communicator or set it to 0");
+  if (c->undist_on && c->nccl_comm)
+    return fail(c, MLOAM_E_STATE, "frame: the undistortion (mloam_set_distortion) is single-GPU only; detach the communicator or turn it off");
   const bool want_cov = c->with_ua != 0;
   c->last_scan_valid = false;
   c->frame_from_graph = false;
@@ -546,6 +590,10 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
     if (c->outlier_on) {  // the outlier stage's launch (its leaf is staged); a context that never turns it on keeps its keys
       const int on = 1;
       key = fnv1a(key, &on, sizeof(on));
+    }
+    if (c->undist_on) {  // the undistortion's launch and the look-ahead's split (poses and scan period are staged)
+      const int on[2] = {'u', c->undist_n};
+      key = fnv1a(key, on, sizeof(on));
     }
     if (sw.raw) {  // raw frame: the per-LiDAR counts and the front-end parameters are kernel arguments of the captured front end
       key = fnv1a(key, &sw.L, sizeof(RigLayout));
@@ -685,6 +733,13 @@ int upload_submaps(Ctx *c, const mloam_point_t *h_surf_map, int n_surf_map, cons
 int frame_call(Ctx *c, Sweep sw, const mloam_point_t *surf_map, int n_surf_map, const mloam_point_t *corner_map, int n_corner_map,
                int rebuild_maps, const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
   if (sw.host && rebuild_maps && (!surf_map || !corner_map || n_surf_map < 0 || n_corner_map < 0)) return MLOAM_E_INVALID;
+  if (c->undist_on) {  // the sweep's pose_undist (mloam_frame_undistort), consumed by this call whatever it returns
+    const bool set = c->undist_set;
+    c->undist_set = false;
+    if (!set) return fail(c, MLOAM_E_STATE, "frame: the undistortion is on and no pose was given for this sweep (mloam_frame_undistort)");
+    if (c->undist_n != (rig_merge(c) ? c->n_lidars : 1))
+      return fail(c, MLOAM_E_INVALID, "frame: mloam_frame_undistort gave a pose count other than the frame's LiDARs (1 without the rig merge)");
+  }
   cudaSetDevice(c->device);
   // this sweep's features: extracted while the previous frame was solved (look-ahead), or now into the half after the previous frame's
   const bool have = frame_has_prefetched(c, sw);

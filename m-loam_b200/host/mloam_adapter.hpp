@@ -425,3 +425,41 @@ class ActiveFeatureSelection {
       for (int j = 0; j < 6; j++) sub_mat_H(i, j) = H[i * 6 + j];
   }
 };
+
+// ---- DISTORTION (estimator.cpp:545-590).  Estimator::process computes pose_undist and calls undistortMeasurements(pose_undist) on the
+// features the mapper takes; with the frame on the device those features are moved inside the next mloam_frame* call of ctx, the context
+// that runs the frames:
+//   mloam::setDistortion(ctx, DISTORTION, SCAN_PERIOD);                                    once, after mloam_set_lidars
+//   pose_undist = mloam::undistortPoses(pose_rlt_[IDX_REF], qbl_, tbl_);                    estimator.cpp:575-579
+//   mloam::undistortMeasurements(ctx, pose_undist, IDX_REF, ESTIMATE_EXTRINSIC);           in place of Estimator::undistortMeasurements
+namespace mloam {
+inline void setDistortion(mloam_ctx_t *ctx, bool on, float scan_period) {
+  check(ctx, mloam_set_distortion(ctx, on ? 1 : 0, scan_period), "mloam_set_distortion");
+}
+// pose_undist[n] = Pose(qbl[n], tbl[n]).inverse() * pose_rlt * Pose(qbl[n], tbl[n]) for every LiDAR n; pose_rlt as the Pose holds it
+inline std::vector<Pose> undistortPoses(const Pose &pose_rlt, const std::vector<Eigen::Quaterniond> &qbl, const std::vector<Eigen::Vector3d> &tbl) {
+  const size_t n = qbl.size();
+  std::vector<double> e(7 * n), out(7 * n);
+  for (size_t l = 0; l < n; l++) {
+    double *x = &e[7 * l];
+    x[0] = tbl[l](0), x[1] = tbl[l](1), x[2] = tbl[l](2), x[3] = qbl[l].x(), x[4] = qbl[l].y(), x[5] = qbl[l].z(), x[6] = qbl[l].w();
+  }
+  double r[7];
+  poseToParam(pose_rlt, r);
+  if (n == 0 || mloam_undistort_poses(r, 0, (int)n, e.data(), 2, out.data()) != MLOAM_OK)  // 2: every LiDAR its own
+    throw std::runtime_error("mloam_undistort_poses: 1..16 LiDARs");
+  std::vector<Pose> res(n);
+  for (size_t l = 0; l < n; l++) {
+    const double *o = &out[7 * l];
+    res[l].q_ = Eigen::Quaterniond(o[6], o[3], o[4], o[5]), res[l].t_ = Eigen::Vector3d(o[0], o[1], o[2]);  // normalised already
+  }
+  return res;
+}
+// undistortMeasurements (:376-408): LiDAR n's features move with pose_undist[n] when estimate_extrinsic == 2, else with
+// pose_undist[idx_ref]; the poses go to the next mloam_frame* call of ctx
+inline void undistortMeasurements(mloam_ctx_t *ctx, const std::vector<Pose> &pose_undist, size_t idx_ref, int estimate_extrinsic) {
+  std::vector<double> x(7 * pose_undist.size());
+  for (size_t l = 0; l < pose_undist.size(); l++) poseToParam(pose_undist[estimate_extrinsic == 2 ? l : idx_ref], &x[7 * l]);
+  check(ctx, mloam_frame_undistort(ctx, (int)pose_undist.size(), x.data()), "mloam_frame_undistort");
+}
+}  // namespace mloam

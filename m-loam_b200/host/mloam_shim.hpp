@@ -451,3 +451,32 @@ inline bool scan2MapOptimization(const common::PointICloud &laser_cloud_surf_fro
   return st.ran != 0;
 }
 }  // namespace mloam
+
+// ----------------------------------------------------------------------------------------------- DISTORTION
+namespace mloam {
+// The pose_undist of Estimator::process (estimator.cpp:575-579) and the per-LiDAR choice of undistortMeasurements (:376-408), for
+// mloam_frame_undistort: pose_ext[n]^-1 * pose_rlt * pose_ext[n], every LiDAR taking idx_ref's unless estimate_extrinsic == 2.
+inline std::vector<Pose> undistortPoses(const Pose &pose_rlt, int idx_ref, const std::vector<Pose> &pose_ext, int estimate_extrinsic) {
+  std::vector<double> e(7 * pose_ext.size()), out(7 * pose_ext.size());
+  for (size_t n = 0; n < pose_ext.size(); n++) pose_ext[n].toParam(&e[7 * n]);
+  double r[7];
+  pose_rlt.toParam(r);
+  if (mloam_undistort_poses(r, idx_ref, (int)pose_ext.size(), e.data(), estimate_extrinsic, out.data()) != MLOAM_OK)
+    throw std::runtime_error("mloam_undistort_poses: invalid arguments");
+  std::vector<Pose> res(pose_ext.size());
+  for (size_t n = 0; n < pose_ext.size(); n++) {
+    const double *o = &out[7 * n];
+    res[n].t_ = {{o[0], o[1], o[2]}}, res[n].q_ = {{o[3], o[4], o[5], o[6]}};  // as computed: already normalised
+  }
+  return res;
+}
+// mloam_set_distortion / mloam_frame_undistort on ctx, the context that runs the frames (the poses as undistortPoses returns them)
+inline void setDistortion(mloam_ctx_t *ctx, bool on, float scan_period) {
+  check(ctx, mloam_set_distortion(ctx, on ? 1 : 0, scan_period), "mloam_set_distortion");
+}
+inline void undistortMeasurements(mloam_ctx_t *ctx, const std::vector<Pose> &pose_undist) {
+  std::vector<double> x(7 * pose_undist.size());
+  for (size_t l = 0; l < pose_undist.size(); l++) pose_undist[l].toParam(&x[7 * l]);
+  check(ctx, mloam_frame_undistort(ctx, (int)pose_undist.size(), x.data()), "mloam_frame_undistort");
+}
+}  // namespace mloam
