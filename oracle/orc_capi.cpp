@@ -1,40 +1,17 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see orc_math.hpp header).
 // Flat C entry points over the restatement so tests/ and bench.py's cpu_baseline leg can drive it
-// through ctypes.  Clouds are float32 [n,4] (x,y,z,intensity); poses are double[7]
-// [tx ty tz qx qy qz qw].  Never linked into the product library.
-#include "orc_pipeline.hpp"
-#include "orc_gf.hpp"
-#include "orc_uct.hpp"
+// through ctypes: the single steps, scan2MapOptimization, the whole frame (orc_frame / orc_frame_multi), the
+// calibration step, the odometry solve and the tracker.  Clouds are float32 [n,4] (x,y,z,intensity); poses are
+// double[7] [tx ty tz qx qy qz qw] (orc_capi.hpp).  Never linked into the product library.
+#include "orc_capi.hpp"
 #include "orc_segment.hpp"
 #include <cstdio>
+#include <dlfcn.h>
 #ifdef _OPENMP
 #include <omp.h>
 #endif
 
 using namespace orc;
-
-static Cloud to_cloud(const float *p, int n) {
-  Cloud c(n);
-  if (n > 0) std::memcpy(c.data(), p, sizeof(PointI) * (size_t)n);
-  return c;
-}
-static Pose to_pose(const double *x) { return Pose{Q4{x[3], x[4], x[5], x[6]}, V3{x[0], x[1], x[2]}}; }
-
-// opts layout shared by the pipeline calls
-enum {
-  O_MAX_OUTER = 0, O_MAX_INNER, O_HUBER, O_EIG_THRE, O_N_NEIGH, O_CHECK_FOV, O_POINT_PLANE, O_POINT_EDGE,
-  O_COV_TRACE, O_DIST_SQ_THR, O_NEARBY_SCAN, O_MIN_MATCH_SQ, O_MIN_PLANE_DIS, O_GF_METHOD, O_GF_RATIO, O_GF_SEED, O_COUNT
-};
-static MatchParams mp_from(const double *o) {
-  MatchParams mp;
-  mp.distance_sq_threshold = (float)o[O_DIST_SQ_THR];
-  mp.nearby_scan = (float)o[O_NEARBY_SCAN];
-  mp.min_match_sq_dis = (float)o[O_MIN_MATCH_SQ];
-  mp.min_plane_dis = (float)o[O_MIN_PLANE_DIS];
-  return mp;
-}
-
-#include <dlfcn.h>
 
 std::vector<int> g_gf_groups_surf, g_gf_groups_corner;  // see orc_set_gf_groups
 
@@ -229,12 +206,7 @@ void orc_normal_eq(const unsigned char *types, const double *points, const doubl
 void orc_scan2map(const float *surf_map, int n_sm, const float *corner_map, int n_cm, const float *surf_scan, int n_ss,
                   const float *corner_scan, int n_cs, const double *pose_init7, const double *opts, double *pose_out7,
                   double *stats, double *H36) {
-  Scan2MapOptions o;
-  o.max_outer = (int)opts[O_MAX_OUTER], o.max_inner = (int)opts[O_MAX_INNER], o.huber_a = opts[O_HUBER];
-  o.eig_thre = opts[O_EIG_THRE], o.n_neigh = (int)opts[O_N_NEIGH], o.check_fov = opts[O_CHECK_FOV] != 0;
-  o.point_plane = opts[O_POINT_PLANE] != 0, o.point_edge = opts[O_POINT_EDGE] != 0, o.cov_trace = opts[O_COV_TRACE];
-  o.mp = mp_from(opts);
-  o.gf_method = (int)opts[O_GF_METHOD], o.gf_ratio = opts[O_GF_RATIO], o.gf_seed = (uint64_t)opts[O_GF_SEED];
+  Scan2MapOptions o = opts_from(opts);
   o.gf_groups_surf = g_gf_groups_surf, o.gf_groups_corner = g_gf_groups_corner;
   Cloud sm = to_cloud(surf_map, n_sm), cm = to_cloud(corner_map, n_cm), ss = to_cloud(surf_scan, n_ss),
         cs = to_cloud(corner_scan, n_cs);
@@ -260,12 +232,7 @@ void orc_point_uncertainty(const float *pts, int n, const double *pose7, const d
 void orc_scan2map_ua(const float *surf_map, int n_sm, const float *corner_map, int n_cm, const float *surf_scan, int n_ss,
                      const float *surf_cov6, const float *corner_scan, int n_cs, const float *corner_cov6, const double *pose_init7,
                      const double *opts, double *pose_out7, double *stats) {
-  Scan2MapOptions o;
-  o.max_outer = (int)opts[O_MAX_OUTER], o.max_inner = (int)opts[O_MAX_INNER], o.huber_a = opts[O_HUBER];
-  o.eig_thre = opts[O_EIG_THRE], o.n_neigh = (int)opts[O_N_NEIGH], o.check_fov = opts[O_CHECK_FOV] != 0;
-  o.point_plane = opts[O_POINT_PLANE] != 0, o.point_edge = opts[O_POINT_EDGE] != 0, o.cov_trace = opts[O_COV_TRACE];
-  o.mp = mp_from(opts);
-  o.gf_method = (int)opts[O_GF_METHOD], o.gf_ratio = opts[O_GF_RATIO], o.gf_seed = (uint64_t)opts[O_GF_SEED];
+  Scan2MapOptions o = opts_from(opts);
   std::vector<double> ts(n_ss), tc(n_cs);  // extractCov: float cov_vec -> Matrix3d; trace in double (point_with_cov.hpp:202-214)
   for (int i = 0; i < n_ss; i++) ts[i] = (double)surf_cov6[i * 6] + (double)surf_cov6[i * 6 + 3] + (double)surf_cov6[i * 6 + 5];
   for (int i = 0; i < n_cs; i++) tc[i] = (double)corner_cov6[i * 6] + (double)corner_cov6[i * 6 + 3] + (double)corner_cov6[i * 6 + 5];
@@ -336,22 +303,16 @@ void orc_frame(const float *cloud, int n, const int *scan_start, const int *scan
   }
 }
 
-// ---- the same for a multi-LiDAR frame (odometry node -> mapper hand-over): the concatenated sweeps of n_lidars LiDARs
-// (LiDAR-major, n_scans = n_lidars x rings; scan_start / scan_end index the concatenation).  Per LiDAR n
-// (estimator.cpp:249-263, OpenMP over the LiDARs): extractCloud on its rings; transformCloudFeature (visualization.cpp:40-52):
-// pcl::transformPointCloud with Pose(qbl, tbl).T_.cast<float>() — PCL 1.8 transforms.hpp evaluates
-// x' = m00 x + m01 y + m02 z + m03 in float — and intensity = n; `+=` LiDAR by LiDAR (pubPointCloud :93-104, ESTIMATE_EXTRINSIC
-// == 0); then the mapper: downsampleCurrentScan + scan2MapOptimization on the merged clouds.  ext7: n_lidars x [t q].
+// ---- the same for a multi-LiDAR frame (odometry node -> mapper hand-over): orc_capi.hpp's prepare_multi, then the mapper's
+// scan2MapOptimization on the merged clouds.  ext7: n_lidars x [t q].
 // threads > 1: the per-LiDAR extraction under OpenMP like the reference; the mapper part is single-threaded like the reference.
-static void prepare_multi(const float *cloud, int n, const int *scan_start, const int *scan_end, int n_scans, int n_lidars, const double *ext7,
-                          float corner_leaf, float surf_leaf, Cloud &cs, Cloud &ss, double *t_extract, double *t_down);
 
 // features of one LiDAR group as they enter scan2MapOptimization (per-LiDAR extractCloud, extrinsic + laser id, merged
 // down-sampling); out_* have capacity n points.  Used to restate the sharded (one group per GPU) multi-GPU frame.
 void orc_prepare_multi(const float *cloud, int n, const int *scan_start, const int *scan_end, int n_scans, int n_lidars, const double *ext7,
                        float corner_leaf, float surf_leaf, float *corner_out, int *n_corner, float *surf_out, int *n_surf) {
   Cloud cs, ss;
-  prepare_multi(cloud, n, scan_start, scan_end, n_scans, n_lidars, ext7, corner_leaf, surf_leaf, cs, ss, nullptr, nullptr);
+  prepare_multi(cloud, n, scan_start, scan_end, n_scans, n_lidars, ext7, nullptr, 0.f, corner_leaf, surf_leaf, cs, ss, nullptr, nullptr);
   *n_corner = (int)cs.size(), *n_surf = (int)ss.size();
   if (!cs.empty()) std::memcpy(corner_out, cs.data(), sizeof(PointI) * cs.size());
   if (!ss.empty()) std::memcpy(surf_out, ss.data(), sizeof(PointI) * ss.size());
@@ -369,7 +330,7 @@ void orc_frame_multi(const float *cloud, int n, const int *scan_start, const int
                      const double *pose_init7, const double *opts, double *pose_out7, double *stats) {
   Cloud cs, ss;
   double te = 0, td = 0;
-  prepare_multi(cloud, n, scan_start, scan_end, n_scans, n_lidars, ext7, corner_leaf, surf_leaf, cs, ss, &te, &td);
+  prepare_multi(cloud, n, scan_start, scan_end, n_scans, n_lidars, ext7, nullptr, 0.f, corner_leaf, surf_leaf, cs, ss, &te, &td);
   double st16[16];
   orc_scan2map(surf_map, n_sm, corner_map, n_cm, ss.empty() ? nullptr : &ss[0].x, (int)ss.size(),
                cs.empty() ? nullptr : &cs[0].x, (int)cs.size(), pose_init7, opts, pose_out7, st16, nullptr);
@@ -377,51 +338,6 @@ void orc_frame_multi(const float *cloud, int n, const int *scan_start, const int
     for (int i = 0; i < 16; i++) stats[i] = st16[i];
     stats[16] = te, stats[17] = td, stats[18] = (double)ss.size(), stats[19] = (double)cs.size();
   }
-}
-
-static void prepare_multi(const float *cloud, int n, const int *scan_start, const int *scan_end, int n_scans, int n_lidars, const double *ext7,
-                          float corner_leaf, float surf_leaf, Cloud &cs, Cloud &ss, double *t_extract, double *t_down) {
-  const int R = n_scans / n_lidars;
-  std::vector<CloudFeature> feats(n_lidars);
-  double t0 = now_s();
-#pragma omp parallel for schedule(dynamic, 1)
-  for (int l = 0; l < n_lidars; l++) {
-    // the LiDAR's own cloud: points [first ring begin - 5, last ring end + 6) of the concatenation (ScanInfo = ring_begin + 5 / ring_end - 6)
-    const int lo = scan_start[l * R] - 5, hi = (l + 1 < n_lidars) ? scan_start[(l + 1) * R] - 5 : n;
-    Cloud c = to_cloud(cloud + 4 * (size_t)lo, hi - lo);
-    ScanInfo si;
-    for (int r = 0; r < R; r++) si.scan_start_ind.push_back(scan_start[l * R + r] - lo), si.scan_end_ind.push_back(scan_end[l * R + r] - lo);
-    extract_cloud(c, si, R, feats[l]);
-  }
-  Cloud corner, surf;
-  for (int l = 0; l < n_lidars; l++) {
-    const double *e = ext7 + 7 * l;
-    const Pose T = make_pose(Q4{e[3], e[4], e[5], e[6]}, V3{e[0], e[1], e[2]});  // Pose(q, t) normalises q (pose.cpp:34-41)
-    const M3 Rm = qmat(T.q);
-    float m[12];
-    for (int r = 0; r < 3; r++) {
-      for (int k = 0; k < 3; k++) m[4 * r + k] = (float)Rm(r, k);
-      m[4 * r + 3] = (float)(r == 0 ? T.t.x : (r == 1 ? T.t.y : T.t.z));
-    }
-    auto xf = [&](const Cloud &in, Cloud &out) {
-      for (const PointI &p : in) {
-        PointI o;
-        o.x = m[0] * p.x + m[1] * p.y + m[2] * p.z + m[3];
-        o.y = m[4] * p.x + m[5] * p.y + m[6] * p.z + m[7];
-        o.z = m[8] * p.x + m[9] * p.y + m[10] * p.z + m[11];
-        o.intensity = (float)l;
-        out.push_back(o);
-      }
-    };
-    xf(feats[l].corner_points_less_sharp, corner);
-    xf(feats[l].surf_points_less_flat, surf);
-  }
-  double t1 = now_s();
-  voxel_grid(corner, corner_leaf, cs, true);  // lidar_mapper_keyframe.cpp:359-364
-  voxel_grid(surf, surf_leaf, ss, true);
-  double t2 = now_s();
-  if (t_extract) *t_extract = t1 - t0;
-  if (t_down) *t_down = t2 - t1;
 }
 
 // ---- online extrinsic calibration step (Estimator::optimizeMap with ESTIMATE_EXTRINSIC == 1, estimator.cpp:687-787, with the
@@ -496,22 +412,10 @@ void orc_local_map_build(int n_frames, const float *pts, const int *counts, cons
   Cloud merged;
   size_t off = 0;
   for (int k = 0; k < n_frames; k++) {
-    const double *e = pose_local7 + 7 * (size_t)k;
-    const Pose T = make_pose(Q4{e[3], e[4], e[5], e[6]}, V3{e[0], e[1], e[2]});
-    const M3 Rm = qmat(T.q);
-    float m[12];
-    for (int r = 0; r < 3; r++) {
-      for (int q = 0; q < 3; q++) m[4 * r + q] = (float)Rm(r, q);
-      m[4 * r + 3] = (float)(r == 0 ? T.t.x : (r == 1 ? T.t.y : T.t.z));
-    }
+    const FloatTransform xf(pose_local7 + 7 * (size_t)k);
     for (int i = 0; i < counts[k]; i++) {
       const float *p = pts + 4 * (off + i);
-      PointI o;
-      o.x = m[0] * p[0] + m[1] * p[1] + m[2] * p[2] + m[3];
-      o.y = m[4] * p[0] + m[5] * p[1] + m[6] * p[2] + m[7];
-      o.z = m[8] * p[0] + m[9] * p[1] + m[10] * p[2] + m[11];
-      o.intensity = p[3];
-      merged.push_back(o);
+      merged.push_back(xf(PointI{p[0], p[1], p[2], p[3]}, p[3]));
     }
     off += (size_t)counts[k];
   }
@@ -624,6 +528,29 @@ void orc_track_cloud(const float *prev_less_sharp, int n_pls, const float *prev_
   TrackResult r = track_cloud(a, b, c, d, to_pose(pose_ini7), o);
   pose_to_param(r.pose, pose_out7);
   if (stats) stats[0] = r.n_corner, stats[1] = r.n_surf, stats[2] = r.lm_iterations;
+}
+
+// ---- TransformToEnd (orc_capi.hpp) of n points (x y z intensity) with one pose [t q]
+void orc_undist_points(const float *pts, int n, const double *pose7, float scan_period, float *out) {
+  Cloud c = to_cloud(pts, n);
+  undistort_cloud(c, pose7, scan_period);
+  if (n > 0) std::memcpy(out, c.data(), sizeof(PointI) * (size_t)n);
+}
+
+// pose_undist of every LiDAR (out7: n_lidars x 7): Estimator::process, estimator.cpp:575-579, pose_undist[n] =
+// Pose(qbl_n, tbl_n).inverse() * pose_rlt_[IDX_REF] * Pose(qbl_n, tbl_n); every LiDAR takes IDX_REF's unless ESTIMATE_EXTRINSIC == 2
+void orc_undist_poses(const double *rlt7, int idx_ref, int n_lidars, const double *ext7, int estimate_extrinsic, double *out7) {
+  const Pose rlt = to_pose(rlt7);
+  std::vector<Pose> und(n_lidars);
+  for (int n = 0; n < n_lidars; n++) {
+    const double *e = ext7 + 7 * n;
+    const Pose ext = make_pose(Q4{e[3], e[4], e[5], e[6]}, V3{e[0], e[1], e[2]});
+    const Q4 &q = ext.q;  // Pose::inverse = Pose(q.inverse(), -(q.inverse() * t)), Quaternion::inverse = conj / squaredNorm
+    const double n2 = q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w;
+    const Q4 qi{-q.x / n2, -q.y / n2, -q.z / n2, q.w / n2};
+    und[n] = pose_mul(pose_mul(make_pose(qi, -qrot(qi, ext.t)), rlt), ext);
+  }
+  for (int n = 0; n < n_lidars; n++) pose_to_param(und[estimate_extrinsic == 2 ? n : idx_ref], out7 + 7 * n);
 }
 
 // OpenMP threads used by the parallel sections (1 = the reference's serial behaviour; tests always use 1).

@@ -1,35 +1,19 @@
 """Raw driver sweeps for the front-end tests: synthetic sweeps in firing order, the host builds of tests/host/front_end_host.cpp
 (the libm restatement of removeNaNFromPointCloud + FeatureExtract::calTimestamp, and csrc/cal_timestamp.cuh compiled for the host),
 and the front-end chain the reference runs per LiDAR (estimator.cpp:249-261): calTimestamp -> segmentCloud (segment_cloud: 0)."""
-import atexit
 import ctypes as C
 import math
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
+import host_build
 import oracle_lib as orc
 import synthetic as syn
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_host = None
-
 
 def host_lib():
-    """g++ -ffp-contract=off build of tests/host/front_end_host.cpp, in a temporary directory removed when the process exits."""
-    global _host
-    if _host is None:
-        td = tempfile.mkdtemp(prefix="front_end_host_")
-        atexit.register(shutil.rmtree, td, True)
-        so = os.path.join(td, "libfront_end_host.so")
-        out = subprocess.run(["g++", "-std=c++14", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-I" + os.path.join(ROOT, "m-loam_b200", "csrc"),
-                              os.path.join(ROOT, "tests", "host", "front_end_host.cpp"), "-o", so], capture_output=True, text=True)
-        assert out.returncode == 0, out.stderr[-3000:]
-        _host = C.CDLL(so)
-    return _host
+    """tests/host/front_end_host.cpp built for the host (host_build)."""
+    return host_build.load("front_end_host")
 
 
 def _run(fn, cloud, time_field, scan_period):

@@ -1,47 +1,16 @@
-"""Test infrastructure of the keyframe store: ctypes binding of the oracle's mapper state machine (oracle/orc_mapper.cpp: saveKeyframe,
-clearCloud, extractSurroundingKeyFrames and the process() driver), compiled on first use into a temporary directory keyed by the
-sources' hash (the tree is never written), and independent numpy restatements of the keyframe decision, the radius search, the
-surrounding-set bookkeeping and the keyframe-position filter."""
+"""Test infrastructure of the keyframe store: bindings of the oracle's mapper state machine (oracle/orc_mapper.cpp in oracle_lib's library:
+saveKeyframe with the optional outlier cloud, clearCloud, extractSurroundingKeyFrames and the process() driver), and independent numpy
+restatements of the keyframe decision, the radius search, the surrounding-set bookkeeping and the keyframe-position filter."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 import oracle_lib as orc
-import uncertainty_lib as ua
+import uncertainty_lib as ua  # noqa: F401  (tests reach the covariance generator as ml.ua)
 
-ORC_DIR = orc.ORC_DIR
 _p = orc._p
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        srcs = sorted(f for f in os.listdir(ORC_DIR) if f.endswith(".hpp")) + ["orc_ua.cpp", "orc_mapper.cpp"]
-        h = hashlib.sha256()
-        for f in srcs:
-            h.update(f.encode())
-            with open(os.path.join(ORC_DIR, f), "rb") as fh:
-                h.update(fh.read())
-        h.update(" ".join(ua.CXXFLAGS).encode())
-        so = os.path.join(tempfile.gettempdir(), f"mloam_orc_mapper_{os.getuid()}_{h.hexdigest()[:16]}.so")
-        if not os.path.exists(so):
-            tmp = f"{so}.{os.getpid()}.tmp"
-            subprocess.check_call(["/usr/bin/g++", *ua.CXXFLAGS, "-shared", "-o", tmp, os.path.join(ORC_DIR, "orc_mapper.cpp")])
-            os.replace(tmp, so)
-        _lib = C.CDLL(so)
-        _lib.orc_mapper_create.restype = C.c_void_p
-        _lib.orc_mapper_create.argtypes = [C.c_double] * 5 + [C.c_float] * 2
-        for f in ("orc_mapper_destroy", "orc_mapper_set_lidars", "orc_mapper_save", "orc_mapper_submap", "orc_mapper_query", "orc_mapper_map",
-                  "orc_mapper_reassoc_differs", "orc_mapper_process", "orc_mapper_keyframe"):
-            getattr(_lib, f).argtypes = None
-    return _lib
 
 
 def _f64(a, n=None):
@@ -53,12 +22,12 @@ class Mapper:
     """The oracle's keyframe store (one per mapper)."""
 
     def __init__(self, distance_keyframes, orientation_keyframes_deg, radius, sur_kf_res, trace_threshold, surf_leaf=0.4, corner_leaf=0.2):
-        self._h = C.c_void_p(lib().orc_mapper_create(distance_keyframes, orientation_keyframes_deg, radius, sur_kf_res, trace_threshold,
+        self._h = C.c_void_p(orc.lib().orc_mapper_create(distance_keyframes, orientation_keyframes_deg, radius, sur_kf_res, trace_threshold,
                                                      surf_leaf, corner_leaf))
 
     def close(self):
         if self._h:
-            lib().orc_mapper_destroy(self._h)
+            orc.lib().orc_mapper_destroy(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):
@@ -71,27 +40,29 @@ class Mapper:
         e = _f64(ext7).reshape(-1)
         ec = None if ext_cov is None else _f64(ext_cov).reshape(-1)
         cm = None if cov_meas is None else _f64(cov_meas, 9)
-        lib().orc_mapper_set_lidars(self._h, e.shape[0] // 7, _p(e), _p(ec), _p(cm), int(with_ua))
+        orc.lib().orc_mapper_set_lidars(self._h, e.shape[0] // 7, _p(e), _p(ec), _p(cm), int(with_ua))
 
-    def save(self, pose7, cov, surf, corner):
-        """saveKeyframe: (saved, (distance margin [m], angle margin [deg]))."""
+    def save(self, pose7, cov, surf, corner, outlier=None):
+        """saveKeyframe, with the keyframe's outlier cloud when given: (saved, (distance margin [m], angle margin [deg]))."""
         s, c = orc.cloud(surf), orc.cloud(corner)
+        o = None if outlier is None else orc.cloud(np.asarray(outlier, np.float32).reshape(-1, 4))
         m = np.zeros(2)
-        r = lib().orc_mapper_save(self._h, _p(_f64(pose7)), _p(_f64(cov, 36)), _p(s), s.shape[0], _p(c), c.shape[0], _p(m))
+        r = orc.lib().orc_mapper_save_outlier(self._h, _p(_f64(pose7)), _p(_f64(cov, 36)), _p(s), s.shape[0], _p(c), c.shape[0], _p(o),
+                                          0 if o is None else o.shape[0], _p(m))
         return bool(r), (m[0], m[1])
 
     def submap(self, pred7):
         """extractSurroundingKeyFrames: (rebuilt, min |d2 - radius^2|)."""
         rm = np.zeros(1)
-        r = lib().orc_mapper_submap(self._h, _p(_f64(pred7)), _p(rm))
+        r = orc.lib().orc_mapper_submap(self._h, _p(_f64(pred7)), _p(rm))
         return bool(r), float(rm[0])
 
     def query(self):
         """(keyframe count, surrounding ids, chosen ids, surf map size, corner map size)."""
         cnt = np.zeros(5, np.int32)
-        lib().orc_mapper_query(self._h, _p(cnt), None, None)
+        orc.lib().orc_mapper_query(self._h, _p(cnt), None, None)
         sur, ch = np.zeros(max(cnt[1], 1), np.int32), np.zeros(max(cnt[2], 1), np.int32)
-        lib().orc_mapper_query(self._h, _p(cnt), _p(sur), _p(ch))
+        orc.lib().orc_mapper_query(self._h, _p(cnt), _p(sur), _p(ch))
         return int(cnt[0]), sur[:cnt[1]].tolist(), ch[:cnt[2]].tolist(), int(cnt[3]), int(cnt[4])
 
     def maps(self):
@@ -100,25 +71,25 @@ class Mapper:
         out = []
         for t, n in ((0, ns), (1, nc)):
             p, c6 = np.zeros((max(n, 1), 4), np.float32), np.zeros((max(n, 1), 6), np.float32)
-            lib().orc_mapper_map(self._h, t, _p(p), _p(c6))
+            orc.lib().orc_mapper_map(self._h, t, _p(p), _p(c6))
             out += [p[:n], c6[:n]]
         return tuple(out)
 
     def keyframe(self, kf_id: int):
         """pose_keyframes_6d[kf_id]: (pose7, cov 6x6) as saveKeyframe stored them."""
         pose, cov = np.zeros(7), np.zeros(36)
-        lib().orc_mapper_keyframe(self._h, int(kf_id), _p(pose), _p(cov))
+        orc.lib().orc_mapper_keyframe(self._h, int(kf_id), _p(pose), _p(cov))
         return pose, cov.reshape(6, 6)
 
     def reassoc_differs(self) -> int:
-        return int(lib().orc_mapper_reassoc_differs(self._h))
+        return int(orc.lib().orc_mapper_reassoc_differs(self._h))
 
     def process(self, cloud, scan_start, scan_end, odom7, frame_trace_threshold, opts):
         """One process() pass: (pose, cov 6x6, info dict)."""
         pts = orc.cloud(cloud)
         ss, se = np.ascontiguousarray(scan_start, np.int32), np.ascontiguousarray(scan_end, np.int32)
         out, cov, info = np.zeros(7), np.zeros(36), np.zeros(8)
-        lib().orc_mapper_process(self._h, _p(pts), pts.shape[0], _p(ss), _p(se), ss.shape[0], _p(_f64(odom7)), C.c_double(frame_trace_threshold),
+        orc.lib().orc_mapper_process(self._h, _p(pts), pts.shape[0], _p(ss), _p(se), ss.shape[0], _p(_f64(odom7)), C.c_double(frame_trace_threshold),
                                  _p(np.ascontiguousarray(opts, np.float64)), _p(out), _p(cov), _p(info))
         keys = ("rebuilt", "ran", "saved", "dist_margin", "angle_margin", "radius_margin", "n_surf_in", "n_corner_in")
         return out, cov.reshape(6, 6), dict(zip(keys, info.tolist()))
@@ -127,13 +98,13 @@ class Mapper:
 def pose_mul(a, b):
     """Pose::operator* (pose.cpp:110-113) as the oracle's driver evaluates it."""
     out = np.zeros(7)
-    lib().orc_mapper_pose_mul(_p(_f64(a)), _p(_f64(b)), _p(out))
+    orc.lib().orc_mapper_pose_mul(_p(_f64(a)), _p(_f64(b)), _p(out))
     return out
 
 
 def pose_inv(a):
     out = np.zeros(7)
-    lib().orc_mapper_pose_inv(_p(_f64(a)), _p(out))
+    orc.lib().orc_mapper_pose_inv(_p(_f64(a)), _p(out))
     return out
 
 

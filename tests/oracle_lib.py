@@ -1,4 +1,5 @@
-"""ctypes binding of the CPU oracle (oracle/liborc.so) and of oracle/_ref/libref_knn.so.
+"""ctypes binding of the CPU oracle (oracle/liborc.so) and of oracle/_ref/libref_knn.so.  lib() is the one place that loads the
+oracle; uncertainty_lib, mapper_lib, global_map_lib, outlier_lib and undistort_lib bind their entry points through it.
 
 Test infrastructure: imported only by tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
 --impl reference legs.  The product package never imports this module.
@@ -46,6 +47,15 @@ def lib():
         _lib.orc_logdet.restype = C.c_double
         _lib.orc_map_sqrt_info.restype = C.c_double
         _lib.orc_map_sqrt_info.argtypes = [C.c_double]
+        _lib.orc_use_ref_tree.restype = C.c_int
+        _lib.orc_use_ref_tree.argtypes = [C.c_char_p]
+        # the keyframe store (mapper_lib.Mapper) and the global map hand out handles
+        _lib.orc_mapper_create.restype = C.c_void_p
+        _lib.orc_mapper_create.argtypes = [C.c_double] * 5 + [C.c_float] * 2
+        _lib.orc_global_map.restype = C.c_void_p
+        _lib.orc_global_map.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_double, C.c_double, C.c_float, C.c_void_p]
+        _lib.orc_global_map_read.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.orc_global_map_free.argtypes = [C.c_void_p]
         _lib.orc_set_threads(1)  # serial, like the reference's mapper; bench's all-cores arm raises it explicitly
     return _lib
 
@@ -413,8 +423,6 @@ def use_ref_tree(on: bool = True) -> bool:
     """Timed CPU arm only: build / search the kd-trees with the reference's nanoflann (oracle/_ref/libref_knn.so)."""
     path = os.path.join(ORC_DIR, "_ref", "libref_knn.so")
     L = lib()
-    L.orc_use_ref_tree.restype = C.c_int
-    L.orc_use_ref_tree.argtypes = [C.c_char_p]
     if on and os.path.exists(path):
         return bool(L.orc_use_ref_tree(path.encode()))
     L.orc_use_ref_tree(None)

@@ -1,14 +1,10 @@
 """Test infrastructure of the outlier cloud (mloam_set_outlier / mloam_frame_outlier / mloam_keyframe_outlier and the outlier appends of
-mloam_global_map): ctypes binding of the oracle's restatement (tests/host/orc_outlier.cpp over oracle/orc_mapper.cpp), compiled on first use
-into a temporary directory keyed by the sources' hash (the tree is never written), and an independent composition of the same steps in
-numpy from the oracle's single-step entry points."""
+mloam_global_map): the binding of the oracle's frame_outlier (oracle/orc_ua.cpp in oracle_lib's library; the keyframe store and the global
+map with outliers are mapper_lib.Mapper and global_map_lib.global_map), and an independent composition of the same steps in numpy from the
+oracle's single-step entry points."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
@@ -16,38 +12,8 @@ import global_map_lib as gml
 import oracle_lib as orc
 import uncertainty_lib as ua
 
-SRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "host", "orc_outlier.cpp")
 SURROUND, SAVE = gml.SURROUND, gml.SAVE
 _p = orc._p
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        h = hashlib.sha256()
-        for f in sorted(f for f in os.listdir(orc.ORC_DIR) if f.endswith((".hpp", ".cpp"))):
-            h.update(f.encode())
-            with open(os.path.join(orc.ORC_DIR, f), "rb") as fh:
-                h.update(fh.read())
-        with open(SRC, "rb") as fh:
-            h.update(fh.read())
-        h.update(" ".join(ua.CXXFLAGS).encode())
-        so = os.path.join(tempfile.gettempdir(), f"mloam_orc_outlier_{os.getuid()}_{h.hexdigest()[:16]}.so")
-        if not os.path.exists(so):
-            tmp = f"{so}.{os.getpid()}.tmp"
-            subprocess.check_call(["/usr/bin/g++", *ua.CXXFLAGS, "-shared", "-o", tmp, SRC])
-            os.replace(tmp, so)
-        _lib = C.CDLL(so)
-        _lib.orc_outlier_mapper_create.restype = C.c_void_p
-        _lib.orc_outlier_mapper_create.argtypes = [C.c_double] * 5 + [C.c_float] * 2
-        _lib.orc_outlier_global_map.restype = C.c_void_p
-        _lib.orc_outlier_global_map.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_double, C.c_double, C.c_float, C.c_void_p]
-        _lib.orc_outlier_global_map_read.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-        _lib.orc_outlier_global_map_free.argtypes = [C.c_void_p]
-        for f in ("orc_outlier_mapper_destroy", "orc_outlier_mapper_set_lidars", "orc_outlier_mapper_save", "orc_outlier_frame"):
-            getattr(_lib, f).argtypes = None
-    return _lib
 
 
 def frame_outlier(cloud, scan_start, n_lidars, ext7, ext_cov, cov_meas, with_ua, trace_threshold, leaf):
@@ -58,60 +24,9 @@ def frame_outlier(cloud, scan_start, n_lidars, ext7, ext_cov, cov_meas, with_ua,
     ec = np.ascontiguousarray(ext_cov if ext_cov is not None else np.zeros((n_lidars, 6, 6)), np.float64).reshape(-1)
     cm = np.ascontiguousarray(cov_meas, np.float64).reshape(9)
     out, c6, n = np.zeros((n_lidars, 4), np.float32), np.zeros((n_lidars, 6), np.float32), C.c_int(0)
-    lib().orc_outlier_frame(_p(pts), pts.shape[0], _p(ss), ss.shape[0], n_lidars, _p(e), _p(ec), _p(cm), int(with_ua),
-                            C.c_double(trace_threshold), C.c_float(leaf), _p(out), _p(c6), C.byref(n))
+    orc.lib().orc_outlier_frame(_p(pts), pts.shape[0], _p(ss), ss.shape[0], n_lidars, _p(e), _p(ec), _p(cm), int(with_ua),
+                                C.c_double(trace_threshold), C.c_float(leaf), _p(out), _p(c6), C.byref(n))
     return out[:n.value].copy(), c6[:n.value].copy()
-
-
-class Mapper:
-    """The oracle's keyframe store with an outlier cloud per keyframe, made and used by this module's library."""
-
-    def __init__(self, distance_keyframes, orientation_keyframes_deg, radius, sur_kf_res, trace_threshold, surf_leaf=0.4, corner_leaf=0.2):
-        self._h = C.c_void_p(lib().orc_outlier_mapper_create(distance_keyframes, orientation_keyframes_deg, radius, sur_kf_res, trace_threshold,
-                                                             surf_leaf, corner_leaf))
-
-    def close(self):
-        if self._h:
-            lib().orc_outlier_mapper_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def set_lidars(self, ext7, ext_cov, cov_meas, with_ua: bool):
-        e = np.ascontiguousarray(ext7, np.float64).reshape(-1)
-        ec = None if ext_cov is None else np.ascontiguousarray(ext_cov, np.float64).reshape(-1)
-        cm = None if cov_meas is None else np.ascontiguousarray(cov_meas, np.float64).reshape(9)
-        lib().orc_outlier_mapper_set_lidars(self._h, e.shape[0] // 7, _p(e), _p(ec), _p(cm), int(with_ua))
-
-    def save(self, pose7, cov, surf, corner, outlier):
-        """saveKeyframe with the three clouds: (saved, (distance margin [m], angle margin [deg]))."""
-        s, c, o = orc.cloud(surf), orc.cloud(corner), orc.cloud(np.asarray(outlier, np.float32).reshape(-1, 4))
-        m = np.zeros(2)
-        r = lib().orc_outlier_mapper_save(self._h, _p(np.ascontiguousarray(pose7, np.float64)), _p(np.ascontiguousarray(cov, np.float64).reshape(36)),
-                                          _p(s), s.shape[0], _p(c), c.shape[0], _p(o), o.shape[0], _p(m))
-        return bool(r), (m[0], m[1])
-
-
-def global_map(mapper: Mapper, mode: int, center7, radius: float, kf_leaf: float, leaf: float):
-    """The oracle's global map with the outlier appends: (chosen ids, [map 0 points, map 0 cov6, map 1 points, map 1 cov6])."""
-    ct = None if center7 is None else np.ascontiguousarray(center7, np.float64)
-    cnt = np.zeros(3, np.int32)
-    r = lib().orc_outlier_global_map(mapper._h.value, int(mode), _p(ct), float(radius), float(kf_leaf), float(leaf), _p(cnt))
-    try:
-        ch = np.zeros(max(cnt[0], 1), np.int32)
-        out = []
-        for which in (0, 1):
-            n = int(cnt[1 + which])
-            p, c6 = np.zeros((max(n, 1), 4), np.float32), np.zeros((max(n, 1), 6), np.float32)
-            lib().orc_outlier_global_map_read(r, which, _p(ch), _p(p), _p(c6))
-            out += [p[:n], c6[:n]]
-        return ch[:cnt[0]].tolist(), out
-    finally:
-        lib().orc_outlier_global_map_free(r)
 
 
 # ---------------------------------------------------------------------------------------- independent composition

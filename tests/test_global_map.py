@@ -1,5 +1,5 @@
 """The global map of the device keyframe store (mloam_global_map / _read / _chosen) against the oracle's pubGlobalMap / saveGlobalMap
-(tests/host/orc_global_map.cpp over oracle/orc_mapper.cpp's store): bit-identical chosen ids, points, cov_vec and sizes in both modes,
+(oracle/orc_mapper.cpp over its keyframe store): bit-identical chosen ids, points, cov_vec and sizes in both modes,
 1 and 3 LiDARs, with_ua on and off; a mapper loop that computes a global map after every keyframe is bit-identical to one that does not;
 the launch count does not grow with the keyframes; edges."""
 import ctypes as C
@@ -60,7 +60,7 @@ def test_global_map_bit_identical(mloam, n_lidars, with_ua):
     L = ext.shape[0]
     thr = 0.08 if with_ua else 10.0
     cx = mloam.Context(0, _params(mloam, 16 * L))
-    om = gl.Mapper(0.9, 5.0, 2.6, 1.5, thr)
+    om = ml.Mapper(0.9, 5.0, 2.6, 1.5, thr)
     rng = np.random.default_rng(11)
     n_saved = n_multi = 0
     try:
@@ -184,7 +184,7 @@ def test_edges(mloam):
     ext = sw[0][3]
     lib = mloam.lib()
     cx = mloam.Context(0, _params(mloam, 16))
-    om = gl.Mapper(1.0, 1.0, 30.0, 1.0, 10.0)
+    om = ml.Mapper(1.0, 1.0, 30.0, 1.0, 10.0)
     try:
         with pytest.raises(mloam.MloamError, match=f"error {E_STATE}"):
             cx.global_map(mloam.GLOBAL_MAP_SAVE)
@@ -233,7 +233,7 @@ def _identity_store(mloam, positions, trace_threshold):
     ident = np.array([[0, 0, 0, 0, 0, 0, 1.0]])
     cm = np.diag([0.25, 0.25, 0.5])
     cx = mloam.Context(0, _params(mloam, 16))
-    om = gl.Mapper(0.5, 1.0, 30.0, 1.0, trace_threshold)
+    om = ml.Mapper(0.5, 1.0, 30.0, 1.0, trace_threshold)
     cx.set_lidars(1, ident)
     cx.set_uncertainty(True, np.zeros((1, 6, 6)), cm, 1e3)
     om.set_lidars(ident, np.zeros((1, 6, 6)), cm, True)

@@ -1,4 +1,4 @@
-"""CPU tests of the oracle's global map (pubGlobalMap / saveGlobalMap, tests/host/orc_global_map.cpp) against an independent composition
+"""CPU tests of the oracle's global map (pubGlobalMap / saveGlobalMap, oracle/orc_mapper.cpp) against an independent composition
 of its steps: the radius selection and its order (with a keyframe exactly on the radius and one a float ulp inside), the keyframe-position
 filter with the last id of a voxel winning, the concatenation order of each mode, and the leaf each mode filters at."""
 import numpy as np
@@ -30,7 +30,7 @@ def _cloud(rng, n, n_lidars, centre):
 def _store(rng, n_kf, n_lidars, with_ua, spread=6.0, empty_surf=()):
     """An oracle store of n_kf keyframes (every save forced by a 2 m step) and what it holds: keyframes[id] = (pose, cov, surf, corner)."""
     ext, ext_cov = _ext(n_lidars), ua.ext_covariances(n_lidars, seed=4)
-    m = gl.Mapper(0.5, 1.0, 10.0, 1.0, 0.12 if with_ua else 10.0)
+    m = ml.Mapper(0.5, 1.0, 10.0, 1.0, 0.12 if with_ua else 10.0)
     m.set_lidars(ext, ext_cov, COV_MEAS, with_ua)
     kfs = []
     for k in range(n_kf):
@@ -99,7 +99,7 @@ def test_save_concatenation_order_differs_from_surround():
 def test_radius_edges_and_empty():
     """No keyframe: nothing chosen.  A keyframe at float d2 == (float)r^2 exactly is excluded, one a float ulp inside is included; a
     radius excluding every keyframe chooses nothing and yields empty maps."""
-    m = gl.Mapper(0.5, 1.0, 10.0, 1.0, 10.0)
+    m = ml.Mapper(0.5, 1.0, 10.0, 1.0, 10.0)
     m.set_lidars(_ext(1), None, None, False)
     try:
         assert gl.global_map(m, gl.SURROUND, syn.pose7([0, 0, 0], [0, 0, 0, 1.0]), 5.0, 1.0, 0.4)[0] == []
@@ -124,7 +124,7 @@ def test_radius_edges_and_empty():
 def test_position_filter_last_id_wins():
     """Several keyframes in one kf_leaf voxel: the filter keeps the id listed last (radius order for SURROUND, id order for SAVE), not the
     nearest one; the chosen ids follow voxel order."""
-    m = gl.Mapper(0.05, 1.0, 10.0, 1.0, 10.0)
+    m = ml.Mapper(0.05, 1.0, 10.0, 1.0, 10.0)
     m.set_lidars(_ext(1), None, None, False)
     xs = [1.0, 1.2, 1.1, 1.3, 25.0, 25.5]  # ids 0-3 in one 10 m voxel, 4-5 in another
     try:

@@ -1,5 +1,5 @@
 """GPU tests (-m gpu) of the outlier cloud of segment_cloud: 0 (mloam_set_outlier): the frame's laser_cloud_outlier_cov through the C ABI
-against the oracle (tests/host/orc_outlier.cpp) bit for bit — mloam_frame and mloam_frame_raw, 1 and 3 LiDARs, with_ua on and off, the
+against the oracle (oracle/orc_ua.cpp, oracle/orc_mapper.cpp) bit for bit — mloam_frame and mloam_frame_raw, 1 and 3 LiDARs, with_ua on and off, the
 look-ahead, graph replay and the stream path, its edges and the trace gate's boundary —, the frame's other results unchanged by it, the
 keyframe store's third cloud and the global maps with the outlier appends in the closed mapper loop, and the feature off exactly as before."""
 import math
@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import front_end_lib as fel
+import global_map_lib as gl
 import mapper_lib as ml
 import outlier_lib as ol
 import synthetic as syn
@@ -294,7 +295,7 @@ KF = dict(dist=0.3, orient=2.0, radius=6.0, res=1.0, thr=1e3)
 
 def _loop(mloam, n_lidars, with_ua, leaf, om=None):
     """The mapper loop of process() on the device (frames with the keyframe store, as test_keyframe_mapper.py runs it) with the outlier cloud
-    at `leaf`.  om (an outlier_lib.Mapper): every saved keyframe goes into it as stored on the device, and both global map modes are
+    at `leaf`.  om (a mapper_lib.Mapper): every saved keyframe goes into it as stored on the device, and both global map modes are
     compared with it after every keyframe.  Returns per frame (pose, saved) and the launch count of every mloam_global_map call."""
     sc = syn.make_scene()
     traj = syn.trajectory(N_LOOP)
@@ -342,9 +343,9 @@ def _loop(mloam, n_lidars, with_ua, leaf, om=None):
                     continue
                 if mode == mloam.GLOBAL_MAP_SURROUND:
                     kpose, kcov, sp, _, cp, _ = cx.keyframe_scan(kid)
-                    assert om.save(kpose, kcov, sp, cp, ko[0])[0], k
+                    assert om.save(kpose, kcov, sp, cp, outlier=ko[0])[0], k
                 leaf_m = p.surf_leaf * (2.0 if mode == mloam.GLOBAL_MAP_SAVE else 1.0)
-                ids, want = ol.global_map(om, mode, pose, 1000.0, 10.0, leaf_m)
+                ids, want = gl.global_map(om, mode, pose, 1000.0, 10.0, leaf_m)
                 assert cx.global_map_chosen() == ids, (k, mode)
                 for a, b in zip(g, want):
                     assert _same(a, b), (k, mode)
@@ -358,7 +359,7 @@ def _loop(mloam, n_lidars, with_ua, leaf, om=None):
 def test_closed_loop_keyframes_and_global_maps(mloam, n_lidars, with_ua):
     """Every keyframe's stored outlier cloud is its frame's; both global maps after every keyframe equal the oracle's bit for bit; the
     poses and keyframe decisions and the global map launch counts equal those of the run without the outlier cloud."""
-    om = ol.Mapper(KF["dist"], KF["orient"], KF["radius"], KF["res"], KF["thr"])
+    om = ml.Mapper(KF["dist"], KF["orient"], KF["radius"], KF["res"], KF["thr"])
     try:
         on, on_launches, n_kf = _loop(mloam, n_lidars, with_ua, LEAF, om)
     finally:

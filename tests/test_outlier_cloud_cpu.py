@@ -1,4 +1,4 @@
-"""CPU tests of the oracle's outlier cloud (segment_cloud: 0; tests/host/orc_outlier.cpp): laser_cloud_outlier_cov of a frame against a
+"""CPU tests of the oracle's outlier cloud (segment_cloud: 0; oracle/orc_ua.cpp, oracle/orc_mapper.cpp): laser_cloud_outlier_cov of a frame against a
 numpy composition of its four steps (the first point of each LiDAR's part of the sweep, the float 3x4 extrinsic in PCL's order with
 intensity = laser id, VoxelGridCovarianceMLOAM<PointI>(MAP_OUTLIER_RES), the with_ua trace gate), and the global maps with the outlier
 appends against the single steps concatenated in the reference's two orders (lidar_mapper_keyframe.cpp:818-827, :873-882)."""
@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 import global_map_lib as gl
+import mapper_lib as ml
 import outlier_lib as ol
 import synthetic as syn
 import uncertainty_lib as ua
@@ -112,11 +113,11 @@ def test_frame_outlier_trace_gate():
 
 
 def _stores(rng, n_kf, n_lidars, with_ua, outliers=True):
-    """The same keyframes saved into the outlier store and, without outliers, into the global-map store: keyframes[id] = (pose, cov, surf,
+    """The same keyframes saved into one store with their outlier clouds and into another without them: keyframes[id] = (pose, cov, surf,
     corner, outlier)."""
     ext, ext_cov = _ext(n_lidars), ua.ext_covariances(n_lidars, seed=4)
     thr = 0.12 if with_ua else 10.0
-    mo, mg = ol.Mapper(0.5, 1.0, 10.0, 1.0, thr), gl.Mapper(0.5, 1.0, 10.0, 1.0, thr)
+    mo, mg = ml.Mapper(0.5, 1.0, 10.0, 1.0, thr), ml.Mapper(0.5, 1.0, 10.0, 1.0, thr)
     for m in (mo, mg):
         m.set_lidars(ext, ext_cov, COV_MEAS, with_ua)
     kfs = []
@@ -130,7 +131,7 @@ def _stores(rng, n_kf, n_lidars, with_ua, outliers=True):
             p[:, :3] = rng.normal(0.0, 4.0, (n, 3)) + t
             p[:, 3] = rng.integers(0, n_lidars, n)
             cl.append(p)
-        assert mo.save(pose, cov, *cl)[0] and mg.save(pose, cov, cl[0], cl[1])[0]
+        assert mo.save(pose, cov, cl[0], cl[1], outlier=cl[2])[0] and mg.save(pose, cov, cl[0], cl[1])[0]
         kfs.append((pose, cov, *cl))
     return mo, mg, kfs, ext, ext_cov, thr
 
@@ -147,7 +148,7 @@ def test_global_map_outlier_orders(n_lidars, with_ua):
             centre = kfs[6][0]
             cand = gl.np_candidates(pos, mode, pos[6], 12.0)
             chosen = gl.np_chosen(pos, cand, 10.0)
-            ids, maps = ol.global_map(mo, mode, centre, 12.0, 10.0, leaf)
+            ids, maps = gl.global_map(mo, mode, centre, 12.0, 10.0, leaf)
             assert ids == chosen and len(chosen) >= 2
             want = ol.compose_global(kfs, ext, ext_cov, COV_MEAS, with_ua, thr, mode, chosen, leaf)
             for a, b in zip(maps, want):
@@ -162,13 +163,17 @@ def test_global_map_outlier_orders(n_lidars, with_ua):
 
 @pytest.mark.parametrize("with_ua", [False, True])
 def test_global_map_without_outliers_is_unchanged(with_ua):
-    """A store whose keyframes hold no outlier cloud gives exactly the maps of the global-map oracle."""
+    """A store whose keyframes hold empty outlier clouds, and one saved without them, give exactly the composition of surf and corner
+    alone over the same chosen ids."""
     rng = np.random.default_rng(21)
-    mo, mg, kfs, *_ = _stores(rng, 12, 3, with_ua, outliers=False)
+    mo, mg, kfs, ext, ext_cov, thr = _stores(rng, 12, 3, with_ua, outliers=False)
+    pos = np.array([k[0][:3] for k in kfs], np.float32)
     try:
         for mode, leaf in ((ol.SURROUND, 0.4), (ol.SAVE, 0.8)):
-            a_ids, a = ol.global_map(mo, mode, kfs[5][0], 1000.0, 10.0, leaf)
-            b_ids, b = gl.global_map(mg, mode, kfs[5][0], 1000.0, 10.0, leaf)
-            assert a_ids == b_ids and all(np.array_equal(x, y) for x, y in zip(a, b))
+            chosen = gl.np_chosen(pos, gl.np_candidates(pos, mode, pos[5], 1000.0), 10.0)
+            want = gl.compose([k[:4] for k in kfs], ext, ext_cov, COV_MEAS, with_ua, thr, mode, chosen, leaf)
+            for m in (mo, mg):
+                ids, maps = gl.global_map(m, mode, kfs[5][0], 1000.0, 10.0, leaf)
+                assert ids == chosen and all(np.array_equal(x, y) for x, y in zip(maps, want))
     finally:
         mo.close(), mg.close()

@@ -1,5 +1,5 @@
 """GPU tests (-m gpu) of the undistortion (DISTORTION: mloam_set_distortion / mloam_frame_undistort) through the C ABI: the scans entering
-the solve (mloam_frame_scan) bit-identical to the oracle's (tests/host/orc_undistort.cpp) — mloam_frame and mloam_frame_raw, 1 and 3
+the solve (mloam_frame_scan) bit-identical to the oracle's (oracle/orc_ua.cpp) — mloam_frame and mloam_frame_raw, 1 and 3
 LiDARs, with_ua on and off, the single-LiDAR paths —, pose and statistics within the frame parity tolerance of the oracle and bit-identical
 across the stream path, graph capture and replays with a new pose every call, with and without the look-ahead and a broken announcement;
 the outlier cloud untouched; the keyframe store and both global maps; the launch count; the edges; and the feature off exactly as before."""
@@ -10,8 +10,9 @@ import numpy as np
 import pytest
 
 import front_end_lib as fel
+import global_map_lib as gl
+import mapper_lib as ml
 import oracle_lib as orc
-import outlier_lib as ol
 import synthetic as syn
 import uncertainty_lib as ua
 import undistort_lib as udl
@@ -339,7 +340,7 @@ def test_keyframe_loop_and_global_maps(mloam, with_ua):
     p = mloam.default_params()
     p.n_scans, p.max_outer, p.max_inner, p.map_cell, p.max_ring_points = 16 * n_lidars, 10, 1, 0.5, 1024
     cx = mloam.Context(0, p)
-    om = ol.Mapper(kf["dist"], kf["orient"], kf["radius"], kf["res"], kf["thr"])
+    om = ml.Mapper(kf["dist"], kf["orient"], kf["radius"], kf["res"], kf["thr"])
     n_kf = 0
     try:
         cx.set_lidars(n_lidars, ext)
@@ -363,11 +364,11 @@ def test_keyframe_loop_and_global_maps(mloam, with_ua):
             kid = cx.keyframe_query()[0] - 1
             kpose, kcov, ksp, _, kcp, _ = cx.keyframe_scan(kid)
             assert _same(ksp, sp) and _same(kcp, cp), k
-            assert om.save(kpose, kcov, ksp, kcp, np.zeros((0, 4), np.float32))[0], k
+            assert om.save(kpose, kcov, ksp, kcp, outlier=np.zeros((0, 4), np.float32))[0], k
             for mode in (mloam.GLOBAL_MAP_SURROUND, mloam.GLOBAL_MAP_SAVE):
                 g = cx.global_map(mode, center=pose)
                 leaf_m = p.surf_leaf * (2.0 if mode == mloam.GLOBAL_MAP_SAVE else 1.0)
-                ids, want_g = ol.global_map(om, mode, pose, 1000.0, 10.0, leaf_m)
+                ids, want_g = gl.global_map(om, mode, pose, 1000.0, 10.0, leaf_m)
                 assert cx.global_map_chosen() == ids, (k, mode)
                 for a, b in zip(g, want_g):
                     assert _same(a, b), (k, mode)

@@ -1,59 +1,29 @@
-"""Test infrastructure of the undistortion (mloam_set_distortion / mloam_frame_undistort / mloam_undistort_poses): ctypes bindings of the
-oracle's restatement (tests/host/orc_undistort.cpp over oracle/orc_ua.cpp) and of the device header compiled for the host
-(tests/host/undistort_header.cpp over m-loam_b200/csrc/undistort.cuh), each compiled on first use into a temporary directory keyed by the
-sources' hash (the tree is never written); and a sweep seen by a sensor that moves during it, with its exact answer."""
+"""Test infrastructure of the undistortion (mloam_set_distortion / mloam_frame_undistort / mloam_undistort_poses): bindings of the
+oracle's restatement (oracle/orc_ua.cpp in oracle_lib's library) and of the device header compiled for the host
+(tests/host/undistort_header.cpp over m-loam_b200/csrc/undistort.cuh, host_build); and a sweep seen by a sensor that moves during it, with
+its exact answer."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
 import math
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
+import host_build
 import oracle_lib as orc
-import uncertainty_lib as ua
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ORC_SRC = os.path.join(HERE, "host", "orc_undistort.cpp")
-HDR_SRC = os.path.join(HERE, "host", "undistort_header.cpp")
-HEADER = os.path.join(os.path.dirname(HERE), "m-loam_b200", "csrc", "undistort.cuh")
 _p = orc._p
-_libs = {}
-
-
-def _build(tag, src, deps):
-    if tag not in _libs:
-        h = hashlib.sha256()
-        for f in sorted(deps) + [src]:
-            with open(f, "rb") as fh:
-                h.update(os.path.basename(f).encode() + fh.read())
-        h.update(" ".join(ua.CXXFLAGS).encode())
-        so = os.path.join(tempfile.gettempdir(), f"mloam_{tag}_{os.getuid()}_{h.hexdigest()[:16]}.so")
-        if not os.path.exists(so):
-            tmp = f"{so}.{os.getpid()}.tmp"
-            subprocess.check_call(["/usr/bin/g++", *ua.CXXFLAGS, "-shared", "-o", tmp, src])
-            os.replace(tmp, so)
-        _libs[tag] = C.CDLL(so)
-    return _libs[tag]
-
-
-def oracle():
-    deps = [os.path.join(orc.ORC_DIR, f) for f in os.listdir(orc.ORC_DIR) if f.endswith((".hpp", ".cpp"))]
-    return _build("orc_undist", ORC_SRC, deps)
 
 
 def header():
-    return _build("undist_header", HDR_SRC, [HEADER])
+    return host_build.load("undistort_header")
 
 
 def points(pts, pose7, scan_period=0.1):
     """The oracle's TransformToEnd of points [n,4] with one pose [t q]."""
     p = orc.cloud(pts)
     out = np.zeros_like(p)
-    oracle().orc_undist_points(_p(p), p.shape[0], _p(np.ascontiguousarray(pose7, np.float64)), C.c_float(scan_period), _p(out))
+    orc.lib().orc_undist_points(_p(p), p.shape[0], _p(np.ascontiguousarray(pose7, np.float64)), C.c_float(scan_period), _p(out))
     return out
 
 
@@ -70,7 +40,7 @@ def header_points(pts, pose7s, scan_period=0.1, use_libm=False):
 def poses(pose_rlt7, idx_ref, ext7, estimate_extrinsic):
     e = np.ascontiguousarray(ext7, np.float64).reshape(-1, 7)
     out = np.zeros_like(e)
-    oracle().orc_undist_poses(_p(np.ascontiguousarray(pose_rlt7, np.float64)), int(idx_ref), e.shape[0], _p(e), int(estimate_extrinsic), _p(out))
+    orc.lib().orc_undist_poses(_p(np.ascontiguousarray(pose_rlt7, np.float64)), int(idx_ref), e.shape[0], _p(e), int(estimate_extrinsic), _p(out))
     return out
 
 
@@ -87,10 +57,10 @@ def frame(cloud, scan_start, scan_end, n_lidars, ext7, pose7s, surf_map, corner_
     so, sc, co, cc = np.zeros((n, 4), np.float32), np.zeros((n, 6), np.float32), np.zeros((n, 4), np.float32), np.zeros((n, 6), np.float32)
     ns, nc = C.c_int(0), C.c_int(0)
     cmeas = f64(cov_meas if cov_meas is not None else np.zeros((3, 3)))
-    oracle().orc_undist_frame(_p(pts), n, _p(ss), _p(se), ss.shape[0], n_lidars, _p(f64(ext7)), _p(f64(single_ext7)), _p(f64(pose7s)),
-                              C.c_float(scan_period), _p(f64(ext_cov)), _p(cmeas), C.c_double(trace_threshold), _p(sm), sm.shape[0], _p(cm),
-                              cm.shape[0], C.c_float(corner_leaf), C.c_float(surf_leaf), _p(np.ascontiguousarray(pose_init, np.float64)),
-                              _p(opts), _p(out), _p(stats), _p(cov), _p(so), _p(sc), C.byref(ns), _p(co), _p(cc), C.byref(nc))
+    orc.lib().orc_frame_ua(_p(pts), n, _p(ss), _p(se), ss.shape[0], n_lidars, _p(f64(ext7)), _p(f64(single_ext7)), _p(f64(pose7s)),
+                           C.c_float(scan_period), _p(f64(ext_cov)), _p(cmeas), C.c_double(trace_threshold), _p(sm), sm.shape[0], _p(cm),
+                           cm.shape[0], C.c_float(corner_leaf), C.c_float(surf_leaf), _p(np.ascontiguousarray(pose_init, np.float64)),
+                           _p(opts), _p(out), _p(stats), _p(cov), None, _p(so), _p(sc), C.byref(ns), _p(co), _p(cc), C.byref(nc))
     names = ["ran", "n_surf", "n_corner", "lm_iterations", "final_cost", "degenerate"]
     st = {k: stats[i] for i, k in enumerate(names)}
     st.update(n_surf_in=int(stats[18]), n_corner_in=int(stats[19]))

@@ -51,7 +51,7 @@ def build(m, n_kf, sweeps, ext, ext_cov):
     cx.set_lidars(1, ext)
     cx.set_uncertainty(True, ext_cov, COV_MEAS, 1e3)
     cx.keyframes_init(2.0, 10.0, 50.0, 1.0, TRACE)
-    om = gl.Mapper(2.0, 10.0, 50.0, 1.0, TRACE)
+    om = ml.Mapper(2.0, 10.0, 50.0, 1.0, TRACE)
     om.set_lidars(ext, ext_cov, COV_MEAS, True)
     rng = np.random.default_rng(1)
     scans = {}
