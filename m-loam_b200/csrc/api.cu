@@ -118,6 +118,7 @@ int mloam_ctx_create(int device, const mloam_params_t *params, mloam_ctx_t **out
     if (v >= 2 && v <= 4) c->knn_min_blocks = v;
   }
   if (const char *e = getenv("MLOAM_KNN_TMA_MIN")) c->knn_tma_min = (unsigned)strtoul(e, nullptr, 10);
+  if (const char *e = getenv("MLOAM_KNN_SCHEDULE")) c->knn_all_searches = e[0] == '0';
   if (const char *e = getenv("MLOAM_LOOKAHEAD")) c->use_lookahead = (e[0] == '0') ? 0 : 1;
   if (const char *e = getenv("MLOAM_STAMP")) c->stamp_on = e[0] == '1';
   if (const char *e = getenv("MLOAM_FUSE_ITER")) c->fuse_iter = (e[0] == '0') ? 0 : 1;
@@ -301,6 +302,36 @@ int mloam_debug_knn_trace(mloam_ctx_t *h, unsigned *out, int n_queries) {
   if (cudaStreamSynchronize(c->stream) != cudaSuccess) return MLOAM_E_CUDA;
   const unsigned char *slot = c->knn_trace.as<unsigned char>() + c->knn_trace_slot * (size_t)(c->knn_trace_n - 1);
   return cudaMemcpy(out, slot, 16 * (size_t)n_queries, cudaMemcpyDeviceToHost) == cudaSuccess ? MLOAM_OK : MLOAM_E_CUDA;
+}
+
+// Diagnosis only (not part of include/mloam_b200.h): the matcher's state of set `set` (0 corner, 1 surf of scan2map) after the
+// last solve, features [0, n) of both halves: neighbours (2 x n x K original map indices, -1: rejected; the positions in the
+// cell-sorted map depend on the order of the build's atomics), anchor (2 x n float4 as 4 floats), changed (n bytes).  A set
+// that is not double-buffered repeats its one half.  *k: K.
+int mloam_debug_knn_lists(mloam_ctx_t *h, int set, int n, int *pos, float *anchor, unsigned char *changed, int *k) {
+  const Ctx *c = h ? &h->c : nullptr;
+  if (!c || set < 0 || set > 3 || n <= 0 || !pos || !anchor || !changed || !k || c->knn_k <= 0) return MLOAM_E_INVALID;
+  const int K = c->knn_k, half = c->knn_half[set];
+  if (c->knn_pos[set].cap < sizeof(int) * (size_t)K * (size_t)(half + n) || c->knn_anchor[set].cap < sizeof(float4) * (size_t)(half + n) ||
+      c->knn_changed[set].cap < (size_t)n)
+    return MLOAM_E_INVALID;
+  cudaSetDevice(c->device);
+  if (cudaStreamSynchronize(c->stream) != cudaSuccess) return MLOAM_E_CUDA;
+  *k = K;
+  for (int hh = 0; hh < 2; hh++) {
+    const size_t o = hh ? (size_t)half : 0;
+    if (cudaMemcpy(pos + (size_t)hh * n * K, c->knn_pos[set].as<int>() + o * K, sizeof(int) * (size_t)n * K, cudaMemcpyDeviceToHost) != cudaSuccess ||
+        cudaMemcpy(anchor + (size_t)hh * n * 4, c->knn_anchor[set].as<float4>() + o, sizeof(float4) * (size_t)n, cudaMemcpyDeviceToHost) != cudaSuccess)
+      return MLOAM_E_CUDA;
+  }
+  const MapView &mv = c->knn_map[set];
+  std::vector<float4> sorted((size_t)mv.m);
+  if (mv.m > 0 && cudaMemcpy(sorted.data(), mv.sorted, sizeof(float4) * (size_t)mv.m, cudaMemcpyDeviceToHost) != cudaSuccess) return MLOAM_E_CUDA;
+  for (size_t i = 0; i < 2 * (size_t)n * K; i++) {
+    if (pos[i] >= mv.m) return MLOAM_E_STATE;
+    if (pos[i] >= 0) memcpy(&pos[i], &sorted[(size_t)pos[i]].w, sizeof(int));
+  }
+  return cudaMemcpy(changed, c->knn_changed[set].p, (size_t)n, cudaMemcpyDeviceToHost) == cudaSuccess ? MLOAM_OK : MLOAM_E_CUDA;
 }
 
 // Diagnosis only (not part of include/mloam_b200.h): the per-warp [enter, exit] %globaltimer pairs of traced k_match_knn launch `slot`

@@ -323,6 +323,9 @@ struct Ctx {
   DevBuf knn_heavy_list;          // 3 rotating counters + 2 lists of feature indices that needed a real search (match_kernels.cu HeavyQ)
   int knn_rot = 0;                // launch ordinal inside the current solve (rotation of the heavy lists / counters)
   int knn_parity = 0;             // which half of knn_heavy the next seeded launch reads
+  int knn_half[4] = {0, 0, 0, 0}; // per set: features per half of knn_pos / knn_anchor in its last launch (0: one half)
+  int knn_k = 0;                  // neighbours per feature of the last launch
+  MapView knn_map[4] = {};        // per set: the map its last launch searched (mloam_debug_knn_lists)
   DevBuf partials;                // per-block packed normal equations
   DevBuf lm_state;                // LMState
   void *ticket_zeroed_for = nullptr;  // partials allocation whose last-block ticket has been zeroed
@@ -433,6 +436,9 @@ struct Ctx {
   int stamp_n = 0;
   std::vector<std::string> stamp_labels;
   int knn_min_blocks = 2;          // k_match_knn variant: resident CTAs per SM it is compiled for (MLOAM_KNN_MB = 2 | 3 | 4); 2 is fastest on the H100
+  // MLOAM_KNN_SCHEDULE=0: k_match_knn as before the shortened queries — every ball and blind search listed for the next launch
+  // (HeavyQ) and the selection unpruned by the search bound (scan_runs).  Same results; kept to compare the two
+  bool knn_all_searches = false;
   int use_seeds = 1;               // seed the kNN of re-association iterations > 0 with the previous neighbour lists
   int fuse_iter = 1;               // scan2map: fit inside the first evaluation + both evaluations of an LM iteration in ONE launch
                                    // (grid barrier between them); MLOAM_FUSE_ITER=0 restores the three launches

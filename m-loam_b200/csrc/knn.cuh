@@ -114,14 +114,18 @@ struct BestS {
 __device__ __forceinline__ bool key_less(unsigned da, unsigned ia, unsigned db, unsigned ib) { return da < db || (da == db && ia < ib); }
 
 // Stage the runs (one per lane: `count` points from sorted[start], count 0 = none), KNN_TILE points per step, and merge
-// them into the best list: the new list is the N smallest of (current best) U (staged points).
+// them into the best list: the new list is the N smallest of (current best) U (staged points with d2 <= bound).
 // Selection works on the 32-bit distance patterns (non-negative floats order like their bits): one REDUX per extracted
 // element, the index only breaks ties (rare, warp-uniform branch).  Once the list is full, a step whose candidates beat
 // the N-th at most N times inserts them one by one (ballot + popc gives the slot, one shuffle-up shifts the tail).
+// bound: float bits of the caller's squared distance bound, MLOAM_D_NONE for none.  A candidate takes part only if it
+// beats min(N-th, bound) — with an empty list too, so the points of a row that lie outside the caller's ball (rows are
+// clipped at cell granularity) cost one compare and no selection round.  Entries <= bound are those of the unbounded
+// list; the callers only look beyond the bound through min(explored, d) with explored below the bound (warp_knn).
 // Out of line on purpose: it is used from several places and every launch starts with a cold instruction cache.
 template <int N>
 __device__ __noinline__ Best scan_runs(const float4 *__restrict__ sorted, KnnSmem *ks, int start, int count, float qx, float qy, float qz,
-                                       Best best, int *n_points) {
+                                       Best best, int *n_points, unsigned bound) {
   constexpr int U = 2;  // candidates per lane and selection step
   const int lane = threadIdx.x & 31;
   int total;
@@ -157,14 +161,19 @@ __device__ __noinline__ Best scan_runs(const float4 *__restrict__ sorted, KnnSme
           cd[u] = __float_as_uint(d2), ci[u] = (unsigned)__float_as_int(v.w), cp[u] = -(base + t) - 2;
         }
       }
-      // how many candidates beat the current N-th?
+      // how many candidates beat min(N-th, bound)?  The bound as a key is (bound, 0xffffffff): d2 == bound still enters.
+      // The others cannot enter the list; they are dropped here so that the selection rounds end with the admitted ones.
       const unsigned nd = __shfl_sync(MLOAM_FULL_MASK, e.d, N - 1), ni = __shfl_sync(MLOAM_FULL_MASK, e.i, N - 1);
+      const bool by_bound = bound < nd;
+      const unsigned td = by_bound ? bound : nd, ti = by_bound ? 0xffffffffu : ni;
       unsigned beat[U];
       int n_beat = 0;
 #pragma unroll
       for (int u = 0; u < U; u++) {
-        beat[u] = __ballot_sync(MLOAM_FULL_MASK, key_less(cd[u], ci[u], nd, ni));
+        const bool in = key_less(cd[u], ci[u], td, ti);
+        beat[u] = __ballot_sync(MLOAM_FULL_MASK, in);
         n_beat += __popc(beat[u]);
+        if (!in) cd[u] = MLOAM_D_NONE;
       }
       if (n_beat == 0) continue;
       if (nd != MLOAM_D_NONE && n_beat <= N) {
@@ -259,10 +268,11 @@ __device__ __forceinline__ float slab_gap(float q, int c_abs, float cell, float 
 // clip_r >= 0, and without the cube of radius skip_r that has been scanned already when skip_r >= 0.
 // `bound2` shrinks while scanning: lim2 = min(max_sqdist, K-th so far) is what the result needs; prune(lim2) adds the
 // caller's padding.  Returns false when the scan needs more than max_slots row slots (nothing scanned); the blind
-// search passes an unbounded max_slots, so it always scans.
-template <int K, int N, typename Prune>
+// search passes an unbounded max_slots, so it always scans.  sel(bound2): the selection bound handed to scan_runs.
+template <int K, int N, typename Prune, typename Sel>
 __device__ __forceinline__ bool scan_ball(const MapView &map, const GridP &g, KnnSmem &ks, float qx, float qy, float qz, int cx, int cy, int cz,
-                                          int clip_r, int skip_r, float &lim2, Prune prune, int max_slots, int lane, Best &out, KnnDbg *dbg) {
+                                          int clip_r, int skip_r, float &lim2, Prune prune, int max_slots, int lane, Best &out, KnnDbg *dbg,
+                                          Sel sel) {
   const float eps = knn_eps(g, qx, qy, qz);
   float bound2 = prune(lim2);
   const float R = sqrtf(bound2) * 1.0002f + eps;
@@ -314,7 +324,7 @@ __device__ __forceinline__ bool scan_ball(const MapView &map, const GridP &g, Kn
     }
     if (dbg) dbg->ball_steps++, dbg->ball_rows += __popc(__ballot_sync(MLOAM_FULL_MASK, count > 0));
     if (!__any_sync(MLOAM_FULL_MASK, count > 0)) continue;
-    out = scan_runs<N>(map.sorted, &ks, start, count, qx, qy, qz, out, dbg ? &dbg->ball_pts : nullptr);
+    out = scan_runs<N>(map.sorted, &ks, start, count, qx, qy, qz, out, dbg ? &dbg->ball_pts : nullptr, sel(bound2));
     const unsigned long long kk = best_key(out, K - 1);
     if (kk != MLOAM_KEY_NONE) lim2 = fminf(lim2, key_d2(kk)), bound2 = fminf(bound2, prune(lim2));
   }
@@ -327,15 +337,20 @@ __device__ __forceinline__ bool scan_ball(const MapView &map, const GridP &g, Kn
 // cells that intersect that ball gives the exact result, ties included.  pad > 0 widens the ball so that the (K+1)-th
 // distance is seen too.  Returns false (nothing written) when the ball needs more than 32 rows.
 // *explored: every map point closer than this has been scanned.
+// sel_prune: the selection keeps only points with d2 <= rr * rr rounded up.  The K-set is inside (d2 <= r2); a point left
+// out has sqrtf(d2) >= rr > *explored, so min(*explored, d) — all the caller reads beyond the K-th — is unchanged.
 template <int K, int N>
 __device__ __forceinline__ bool warp_knn_seeded(const MapView &map, const GridP &g, KnnSmem &ks, float qx, float qy, float qz, float r2,
-                                                float pad, int lane, Best &out, float *explored) {
+                                                float pad, int lane, Best &out, float *explored, bool sel_prune = false) {
   const float eps = knn_eps(g, qx, qy, qz);
   const float rr = sqrtf(r2) * 1.0002f + eps + pad;
   float lim2 = rr * rr;
+  const unsigned sel = sel_prune ? __float_as_uint(__fmul_ru(rr, rr)) : MLOAM_D_NONE;
   Best b = best_none();
   // the ball is fixed (the seed bound): no shrinking, so that the explored radius is known
-  if (!scan_ball<K, N>(map, g, ks, qx, qy, qz, 0, 0, 0, -1, -1, lim2, [&](float) { return rr * rr; }, 32, lane, b, nullptr)) return false;
+  if (!scan_ball<K, N>(map, g, ks, qx, qy, qz, 0, 0, 0, -1, -1, lim2, [&](float) { return rr * rr; }, 32, lane, b, nullptr,
+                       [&](float) { return sel; }))
+    return false;
   out = b;
   *explored = fmaxf(rr - 2.0f * eps, 0.0f);
   return true;
@@ -360,9 +375,14 @@ __device__ __forceinline__ float cube_face_gap(const GridP &g, float qx, float q
 // (or how far from K neighbours a rejected query) is; the result inside the radius is unaffected.
 // REJECT_PARTIAL is kept for the callers' sake (every matcher gate only wants full K-sets); the grid search has no
 // separate partial path.
+// sel_prune: the selection keeps only points inside the current pruning bound (ring 1: prune(max_sqdist); then the
+// shrinking bound of the shells).  The bounds never drop below the final prune(lim2), so a point left out has
+// sqrtf(d2) >= sqrtf(prune(lim2)) > *explored: the K-set and lim2 are unchanged, and min(*explored, d) of the K-th and
+// (K+1)-th entries — all the callers read beyond the bound — is too.
 template <int K, bool REJECT_PARTIAL, int N = K>
 __device__ __forceinline__ void warp_knn(const MapView &map, const GridP &g, KnnSmem &ks, float qx, float qy, float qz, float max_sqdist,
-                                         int lane, Best &out, float *explored = nullptr, float pad = 0.0f, KnnDbg *dbg = nullptr) {
+                                         int lane, Best &out, float *explored = nullptr, float pad = 0.0f, KnnDbg *dbg = nullptr,
+                                         bool sel_prune = false) {
   long long t_mark = dbg ? clock64() : 0ll;
   out = best_none();
   if (explored) *explored = 0.0f;
@@ -370,6 +390,15 @@ __device__ __forceinline__ void warp_knn(const MapView &map, const GridP &g, Knn
   const int ax = (int)floorf(qx * g.inv_cell), ay = (int)floorf(qy * g.inv_cell), az = (int)floorf(qz * g.inv_cell);  // absolute cell
   const int cx = ax - g.ox, cy = ay - g.oy, cz = az - g.oz;
   const float eps = knn_eps(g, qx, qy, qz);
+  // lim2: min(radius^2, K-th so far) — what the result needs; cells are pruned against prune(lim2), which with pad > 0
+  // reaches pad beyond sqrt(lim2).
+  const float radius = sqrtf(max_sqdist);
+  auto prune = [&](float l2) {
+    if (!(pad > 0.0f)) return l2;
+    const float r = fminf(sqrtf(l2), radius) + pad;
+    return fmaxf(l2, r * r);
+  };
+  auto sel = [&](float bound2) { return sel_prune ? __float_as_uint(bound2) : MLOAM_D_NONE; };
   // ---- ring 1: 9 rows of (up to) 3 cells
   {
     int start = 0, count = 0;
@@ -379,20 +408,12 @@ __device__ __forceinline__ void warp_knn(const MapView &map, const GridP &g, Knn
       if (y >= 0 && y < g.ny && z >= 0 && z < g.nz && xl <= xh) row_run(map, g, y, z, xl, xh, &start, &count);
     }
     if (__any_sync(MLOAM_FULL_MASK, count > 0))
-      out = scan_runs<N>(map.sorted, &ks, start, count, qx, qy, qz, out, dbg ? &dbg->ring1_pts : nullptr);
+      out = scan_runs<N>(map.sorted, &ks, start, count, qx, qy, qz, out, dbg ? &dbg->ring1_pts : nullptr, sel(prune(max_sqdist)));
     if (dbg) {
       const long long t = clock64();
       dbg->t_ring1 = t - t_mark, t_mark = t;
     }
   }
-  // lim2: min(radius^2, K-th so far) — what the result needs; cells are pruned against prune(lim2), which with pad > 0
-  // reaches pad beyond sqrt(lim2).
-  const float radius = sqrtf(max_sqdist);
-  auto prune = [&](float l2) {
-    if (!(pad > 0.0f)) return l2;
-    const float r = fminf(sqrtf(l2), radius) + pad;
-    return fmaxf(l2, r * r);
-  };
   float lim2 = max_sqdist;
   {
     const unsigned long long kk = best_key(out, K - 1);
@@ -406,11 +427,11 @@ __device__ __forceinline__ void warp_knn(const MapView &map, const GridP &g, Knn
   for (int r = 2;; r++) {
     if (covered > 0.0f && covered * covered >= lim2) break;
     if (r > 5) {  // many thin shells left (tiny cells): one pass over the rest of the ball
-      scan_ball<K, N>(map, g, ks, qx, qy, qz, cx, cy, cz, -1, r - 1, lim2, prune, 1 << 30, lane, out, dbg);
+      scan_ball<K, N>(map, g, ks, qx, qy, qz, cx, cy, cz, -1, r - 1, lim2, prune, 1 << 30, lane, out, dbg, sel);
       covered = 3.0e38f;
       break;
     }
-    scan_ball<K, N>(map, g, ks, qx, qy, qz, cx, cy, cz, r, r - 1, lim2, prune, 1 << 30, lane, out, dbg);
+    scan_ball<K, N>(map, g, ks, qx, qy, qz, cx, cy, cz, r, r - 1, lim2, prune, 1 << 30, lane, out, dbg, sel);
     covered = cube_face_gap(g, qx, qy, qz, ax, ay, az, r, eps);
   }
   if (dbg) dbg->t_ball = clock64() - t_mark;

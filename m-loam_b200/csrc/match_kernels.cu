@@ -3,7 +3,7 @@
 //
 //   k_match_knn  one WARP per feature: pointAssociateToMap + exact K-nearest search in the dense voxel grid
 //                (knn.cuh) + the distance gate sqdist[K-1] < MIN_MATCH_SQ_DIS.  Corner and surf features share one
-//                launch; the features that needed a real search in the previous iteration are scheduled first (HeavyQ),
+//                launch; the features that had to search blind in the previous iteration are scheduled first (HeavyQ),
 //                so long queries — features in sparse regions — do not form the tail of the launch.  Output: K neighbour positions per feature (20 B).
 //   k_match_fit  one THREAD per feature: gathers the K neighbours (5 x 16 B), fits the line (mean + scatter +
 //                3x3 eigen) or the plane (5x3 column-pivoted QR), applies the lambda / plane-distance / FOV gates
@@ -33,34 +33,41 @@ struct KnnSet {
   unsigned char *changed;  // out (nullable): 1 when the neighbour list differs from the seed (or there was none)
   float4 *anchor;      // per feature: map-frame position of its last real search + the displacement it tolerates
   int half;            // double-buffered pos / anchor (SpecState): features per half; 0: read and write in place
-  const unsigned char *heavy_in;  // nullable: 1 where the previous launch had to search (ball / blind) — those go first
+  const unsigned char *heavy_in;  // nullable: 1 where the previous launch listed the query (HeavyQ) — those go first
   unsigned char *heavy_out;       // this launch's verdict, for the next one
 };
 
 // Scheduling of the searches inside a launch.  Queries differ by about 10x in cost (a kept neighbour list is a re-rank,
-// a real search scans rows of cells) and a launch is only as fast as its slowest warp, so the few features that needed a real search
-// in the previous re-association iteration are listed (atomic append — a few dozen per launch, not one atomic per
-// query: tens of thousands of increments of ONE address serialise at the L2 and were the longest part of the launch) and taken
-// first, one per warp; everything else is a static stride.  cnt[3] rotates: a launch reads cnt_in, appends to cnt_out
-// and clears cnt_zero for the launch after the next.
+// a ball search scans a few rows, a blind search grows shells) and a launch is only as fast as its slowest warp, so the
+// few features that searched blind in a seeded launch are listed (atomic append — a handful per launch, not one atomic per
+// query: tens of thousands of increments of ONE address serialise at the L2) and taken first by the next launch, one per
+// warp; everything else is a static stride.  A launch without seeds lists nothing: all its queries search blind, and in
+// the next launch they are seeded.  A stride skips the listed queries by a ballot over the list held in the lanes' registers
+// (at most 32 entries) or by their heavy_in byte (longer lists).  cnt[3] rotates: a launch reads cnt_in, appends to
+// cnt_out and clears cnt_zero for the launch after the next.
+// all_searches (MLOAM_KNN_SCHEDULE=0, the earlier schedule): list every ball and blind search, seeded or not.
 struct HeavyQ {
   const int *list_in;   // nullable (first iteration): global feature indices (corner set first)
   const int *cnt_in;
   int *list_out;
   int *cnt_out;
   int *cnt_zero;
+  int all_searches;
 };
 
 // MB: resident CTAs per SM the kernel is compiled for (register budget 65536 / (256 * MB)).  The search is a chain of
 // dependent warp-wide operations (prefix loads -> point loads -> REDUX / ballot / shuffle rounds).  MB = 3 and 4 buy more
 // resident warps with spilled registers (local-memory round trips inside that chain); on the H100 the spill-free MB = 2
-// variant (106 registers) runs the C2 frame about 9 % faster than MB = 4, so it is the default (Ctx::knn_min_blocks).
-// path_stats: the KnnPathStats (ctx.h) addressed as 32-bit words; KPS_WORD(field) is a field's word index
+// variant (104 registers, no spills; MB = 3 still spills) runs the C2 frame about 9 % faster than MB = 4, so it is the default (Ctx::knn_min_blocks).
+// STATS: the instance for stage profiling and MLOAM_KNN_TRACE=1, with the per-path counters (path_stats: the KnnPathStats
+// of ctx.h addressed as 32-bit words; KPS_WORD(field) is a field's word index) and the per-query trace; the production
+// instance is compiled without them.  sel_prune: bound-pruned selection (scan_runs), 0 under MLOAM_KNN_SCHEDULE=0.
 #define KPS_WORD(field) (offsetof(KnnPathStats, field) / sizeof(unsigned))
-template <int K, int MB>
+template <int K, int MB, bool STATS>
 __global__ void __launch_bounds__(MWARPS * 32, MB)
     k_match_knn(KnnSet a, KnnSet b, const double *__restrict__ pose7, float min_match_sq_dis, HeavyQ hq, const int *__restrict__ d_sel,
-                unsigned *__restrict__ path_stats, unsigned tma_min, unsigned *__restrict__ trace) {
+                unsigned *__restrict__ path_stats, unsigned tma_min, unsigned *__restrict__ trace, int sel_prune) {
+  if (!STATS) path_stats = nullptr, trace = nullptr;
   __shared__ KnnSmem ksm[MWARPS];
   const int lane = threadIdx.x & 31;
   KnnSmem &ks = ksm[threadIdx.x >> 5];
@@ -81,6 +88,7 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
   const int it_a = n_heavy > gw ? (n_heavy - gw + n_warps - 1) / n_warps : 0;
   const int it_b = n > gw ? (n - gw + n_warps - 1) / n_warps : 0;
   const int first_listed = it_a > 0 ? __ldg(hq.list_in + gw) : 0;
+  const int listed_lane = n_heavy <= 32 && lane < n_heavy ? __ldg(hq.list_in + lane) : -1;  // short list: in registers
   // Programmatic dependent launch: the pose searched at (SpecState::xc, published by k_linearize's tail), d_sel (committed there)
   // and the lists, anchors, changed flags and fit inputs k_linearize reads are only touched after the previous kernel completed
   cudaGridDependencySynchronize();
@@ -98,9 +106,11 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
       i = it == 0 ? first_listed : __ldg(hq.list_in + gw + it * n_warps);
     } else {
       i = gw + (it - it_a) * n_warps;
-      if (listed) {  // listed ones have been done above
+      if (n_heavy > 32) {  // listed ones have been done above
         const unsigned char *hin = i < na ? a.heavy_in : b.heavy_in;
         if (hin && hin[i < na ? i : i - na]) continue;
+      } else if (n_heavy > 0 && __any_sync(MLOAM_FULL_MASK, listed_lane == i)) {
+        continue;
       }
     }
     const float4 p = __ldg(i < na ? a.pts + i : b.pts + (i - na));
@@ -177,12 +187,12 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
       bool found = false;
       if (r2 < min_match_sq_dis)
         found = warp_knn_seeded<K, K + 1>(in_a ? a.map : b.map, g, ks, sel.x, sel.y, sel.z, r2, 0.1f * g.cell,
-                                             lane, best, &explored);
+                                             lane, best, &explored, sel_prune != 0);
       if (!found) {
         KnnDbg dbg = {0, 0, 0, 0, 0, 0};
         const long long t_blind = (path_stats || trace) ? clock64() : 0ll;
         warp_knn<K, true, K + 1>(in_a ? a.map : b.map, g, ks, sel.x, sel.y, sel.z, min_match_sq_dis, lane, best, &explored, 0.05f,
-                                 (path_stats || trace) ? &dbg : nullptr);
+                                 (path_stats || trace) ? &dbg : nullptr, sel_prune != 0);
         if (trace && lane == 0) {
           unsigned *tr = trace + 4 * (size_t)((in_a ? 0 : na) + j);
           tr[1] = (unsigned)dbg.t_ring1, tr[2] = (unsigned)dbg.t_ball, tr[3] = ((unsigned)dbg.ring1_pts << 20) | ((unsigned)(dbg.ball_pts & 0xfff) << 8) | (unsigned)(dbg.ball_steps & 0xff);
@@ -241,8 +251,9 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
     if (trace && lane == 0) trace[4 * (size_t)((in_a ? 0 : na) + j)] = (unsigned)(clock64() - t_query) | ((unsigned)path << 30);
     unsigned char *const hout = in_a ? a.heavy_out : b.heavy_out;
     if (hout && lane == 0) {
-      hout[j] = path >= 2 ? 1 : 0;
-      if (path >= 2 && hq.list_out) hq.list_out[atomicAdd(hq.cnt_out, 1)] = i;
+      const bool heavy = hq.all_searches ? path >= 2 : (path == 3 && seeded);
+      hout[j] = heavy ? 1 : 0;
+      if (heavy && hq.list_out) hq.list_out[atomicAdd(hq.cnt_out, 1)] = i;
     }
   }
   if (trace && lane == 0) {  // per-warp timeline after the per-query words: [enter, first query, exit] in ns
@@ -309,6 +320,7 @@ int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_
     MLOAM_CUDA_OK(c, ab.reserve(sizeof(float4) * (size_t)(J.n + 1) * halves));
     k.seeded = J.seeded, k.changed = cb.as<unsigned char>(), k.anchor = ab.as<float4>();
     k.half = d_sel ? J.n + 1 : 0;
+    c->knn_half[buf_base + t] = k.half, c->knn_k = K, c->knn_map[buf_base + t] = k.map;
     // search verdicts ("had to search") alternate between two halves from launch to launch: read the previous, write the next
     DevBuf &hb = c->knn_heavy[buf_base + t];
     const size_t half = ((size_t)J.n + 256) & ~(size_t)255;
@@ -328,7 +340,7 @@ int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_
   if (n_upper <= 0) return MLOAM_OK;
   // heavy list of the launch: 2 lists x n_upper ints + 3 rotating counters (zeroed with the buffer; k_lm_init re-zeroes
   // them at the start of every solve, where the rotation restarts)
-  HeavyQ hq{nullptr, nullptr, nullptr, nullptr, nullptr};
+  HeavyQ hq{nullptr, nullptr, nullptr, nullptr, nullptr, c->knn_all_searches ? 1 : 0};
   {
     DevBuf &hl = c->knn_heavy_list;
     const size_t ints = 2 * ((size_t)n_upper + 64) + 16;
@@ -370,11 +382,16 @@ int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_
     const int mb = c->knn_min_blocks;
     int nb = (n_upper + MWARPS - 1) / MWARPS;
     if (nb > mb * c->sm_count) nb = mb * c->sm_count;  // all CTAs resident; warps pull / stride over the features
-    void (*k)(KnnSet, KnnSet, const double *, float, HeavyQ, const int *, unsigned *, unsigned, unsigned *);
-    if (K == 5) k = mb == 2 ? k_match_knn<5, 2> : (mb == 3 ? k_match_knn<5, 3> : k_match_knn<5, 4>);
-    else k = mb == 2 ? k_match_knn<10, 2> : (mb == 3 ? k_match_knn<10, 3> : k_match_knn<10, 4>);
+    void (*k)(KnnSet, KnnSet, const double *, float, HeavyQ, const int *, unsigned *, unsigned, unsigned *, int);
+    if (path_stats || trace) {
+      if (K == 5) k = mb == 2 ? k_match_knn<5, 2, true> : (mb == 3 ? k_match_knn<5, 3, true> : k_match_knn<5, 4, true>);
+      else k = mb == 2 ? k_match_knn<10, 2, true> : (mb == 3 ? k_match_knn<10, 3, true> : k_match_knn<10, 4, true>);
+    } else {
+      if (K == 5) k = mb == 2 ? k_match_knn<5, 2, false> : (mb == 3 ? k_match_knn<5, 3, false> : k_match_knn<5, 4, false>);
+      else k = mb == 2 ? k_match_knn<10, 2, false> : (mb == 3 ? k_match_knn<10, 3, false> : k_match_knn<10, 4, false>);
+    }
     MLOAM_CUDA_OK(c, launch_chain(pdl, k, nb, MWARPS * 32, st, ks[0], ks[1], d_pose7, cfg.min_match_sq_dis, hq, d_sel, path_stats,
-                                  c->knn_tma_min, trace));
+                                  c->knn_tma_min, trace, c->knn_all_searches ? 0 : 1));
     c->launches++;
   }
   if (defer && !fs[0].nn && !fs[1].nn) {

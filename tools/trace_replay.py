@@ -110,6 +110,13 @@ def main():
           f"{100.0 * both / tc if tc else 0.0:.1f} % of its time next to a running k_match_knn")
     print(f"k_match_knn: {sum(b - a for a, b in knn) / max(1, len(knn)):.1f} us each; "
           f"k_linearize: {sum(b - a for a, b in lin) / max(1, len(lin)):.1f} us each")
+    knn_pf = len(knn) // n_frames  # a frame's first matcher launch searches blind, the later ones are seeded
+    if knn_pf > 1:
+        knn.sort()
+        first = [b - a for k, (a, b) in enumerate(knn) if k % knn_pf == 0]
+        seeded = [b - a for k, (a, b) in enumerate(knn) if k % knn_pf != 0]
+        print(f"k_match_knn per frame: {knn_pf} launches; first (blind) {np.mean(first):.1f} us, seeded {np.mean(seeded):.1f} us "
+              f"(min {np.min(seeded):.1f}, max {np.max(seeded):.1f})")
     per_frame = len(lin) // n_frames  # the last k_linearize of a frame runs both passes, the others pass 0 only
     if per_frame > 1:
         lin.sort()
@@ -170,6 +177,23 @@ def main():
     per = ga.sum(axis=1) + gb.sum(axis=1)
     print(f"  per frame: sum (a) {ga.sum(axis=1).mean():.1f}, sum (b) {gb.sum(axis=1).mean():.1f}, total {per.mean():.1f} "
           f"(min {per.min():.1f}, max {per.max():.1f})")
+    # queries and SM cycles per search path from stage profiling (stream path, instrumented matcher), per frame
+    os.environ["MLOAM_KNN_TRACE"] = "0"
+    ctx = m.Context(0, p)
+    step(True)
+    ctx.profile(True)
+    ctx.profile_reset()
+    for _ in range(n_frames):
+        step(False)
+    torch.cuda.synchronize()
+    print(f"k_match_knn per search path, stage profiling, per frame (mean of {n_frames}): queries, mean SM cycles per query")
+    for path in ("keep_matched", "keep_rejected", "ball", "blind"):
+        q = ctx.profile_get(f"knn_{path}")[1] / n_frames
+        cyc = ctx.profile_get(f"knn_cycles_{path}")[1] / n_frames
+        print(f"  {path:>13s} {q:9.1f} {cyc / max(q, 1e-9):9.0f}")
+    print(f"  slowest query {ctx.profile_get('knn_max_query_cycles')[1]:.0f} cycles; "
+          f"{ctx.profile_get('knn_queries_over_32k_cycles')[1] / n_frames:.1f} queries over 32k cycles per frame")
+    ctx.close()
 
 
 if __name__ == "__main__":
