@@ -64,7 +64,8 @@ typedef struct {
   float map_cell;              /* voxel-hash cell edge [m] for the scan-to-map maps (<= 0: auto) */
   float corner_leaf;           /* MAP_CORNER_RES (scan down-sampling before matching) */
   float surf_leaf;             /* MAP_SURF_RES */
-  int gf_method;               /* FLAGS_gf_method in scan2MapOptimization (:474-532): 0 wo_gf, 1 rnd, 2 fps, 3 gd_fix */
+  int gf_method;               /* FLAGS_gf_method in scan2MapOptimization (:474-532): 0 wo_gf, 1 rnd, 2 fps, 3 gd_fix
+                                  (gd_float: 3 and mloam_set_gf_float) */
   float gf_ratio;              /* FLAGS_gf_ratio_ini */
   unsigned gf_seed;            /* selection seed; outer iteration i, set s (0 corner, 1 surf) uses gf_seed + 2 i + s */
   int max_ring_points;         /* upper bound of the points of one ring (0: up to 12288); sizes the in-CTA sort of extractCloud so that
@@ -480,13 +481,43 @@ int mloam_calib_frame(mloam_ctx_t *ctx, const mloam_point_t *h_surf_ref, int n_s
  * estimator.cpp:1347-1517): match every feature of `h_pts` against map `slot` at pose7, evaluate its 1x6 Jacobian row
  * (evaluateFeatJacobianMatching, lidar_mapper.h:130-174; sqrt_info from the point's covariance h_cov6[n*6] — PointIWithCov::cov_vec —
  * or from params.cov_trace when null) and select gf_ratio * n features.
- * method: 0 wo_gf (all matched), 1 rnd, 2 fps, 3 gd_fix / gd_float (stochastic greedy on log det(H + J^T J)).
+ * method: 0 wo_gf (all matched), 1 rnd, 2 fps, 3 gd_fix / gd_float (stochastic greedy on log det(H + J^T J); the two differ in
+ * the ratio they are called with, see mloam_set_gf_float).
  * The reference's mt19937(random_device) becomes an explicit PCG32 `seed` and its wall-clock cap (MAX_FEATURE_SELECT_TIME)
  * is dropped; MAX_RANDOM_QUEUE_TIME = 20 is kept.  Outputs: h_sel[<= n] feature indices in selection order, *n_sel,
  * H36 = sub_mat_H (starts at 1e-6 I), optional h_matched[n] and h_jaco[n*6]. */
 int mloam_good_features(mloam_ctx_t *ctx, int slot, int type, const mloam_point_t *h_pts, int n, const float *h_cov6,
                         const double *pose7, int method, double gf_ratio, unsigned long long seed, int *h_sel, int *n_sel,
                         double *H36, unsigned char *h_matched, double *h_jaco);
+
+/* ---- ActiveFeatureSelection::evalFullHessian for one feature set (lidar_mapper.h:176-227): every feature of `h_pts` matched against
+ * map `slot` at pose7 (n_neigh 5, CHECK_FOV false, whatever the parameters say), the row of evaluateFeatJacobianMatching with the point's
+ * own covariance (h_cov6, or params.cov_trace when null), and J^T J of the matched ones added to H36 feature by feature in index order;
+ * *feat_num grows by their count.  Both are in-out as in the reference, so 's' then 'c' on one H36 = 1e-6 I is lidar_mapper_keyframe.cpp
+ * :461-467.  The sum is serial per element (no tree), so H36 equals the host loop bit for bit. */
+int mloam_full_hessian(mloam_ctx_t *ctx, int slot, int type, const mloam_point_t *h_pts, int n, const float *h_cov6, const double *pose7,
+                       double *H36, int *feat_num);
+
+/* ---- gf_method "gd_float" in mloam_scan2map* / mloam_frame* (lidar_mapper_keyframe.cpp:456-495): gd_fix (params.gf_method = 3) with the
+ * ratio adapted every 10th frame.  The context counts its solve calls (frame_cnt, :1059, incremented before the map gate :429); a call
+ * with frame_cnt % 10 == 0 that passes the gate evaluates, before its first selection, gf_deg_factor = logDet(1e-6 I + sum J^T J) over
+ * every matched surf, then corner feature (evalFullHessian; the rows are the ones the selection makes anyway) and sets the ratio of
+ * this and the following frames: params.gf_ratio (FLAGS_gf_ratio_ini) when gf_deg_factor > map_deg_thre (MAP_DEG_THRE, a float),
+ * 0.8 otherwise.  Until the first evaluation the ratio is min(1, params.gf_ratio) (:1248).  Everything stays on the device: the
+ * ratio is read there by the selection, never by the host, and neither it nor the threshold is part of a frame graph's key — a context
+ * replays two graphs (evaluation frame or not) whatever the ratio does.
+ * mloam_set_gf_float: on != 0 starts the mode with frame_cnt = 0 (MLOAM_E_STATE unless params.gf_method == 3; MLOAM_E_STATE with a
+ *   communicator: the features are sharded over the ranks and their 21 sums are not exchanged, like mloam_set_uncertainty the mode is
+ *   single-GPU only); on == 0 (the default) ends it, and then nothing of a frame differs from gd_fix.
+ * mloam_set_gf_float_threshold: MAP_DEG_THRE alone, frame_cnt and the ratio kept.
+ * mloam_gf_float_report: what the reference prints at :493 — the current ratio, gf_deg_factor and total_feat_num of the last
+ *   evaluation — whether the last solve call evaluated, and frame_cnt; read back with that call's results (any pointer may be NULL).
+ *   MLOAM_E_STATE before the first solve call.  gf_deg_factor is 2 x the sum of six device log() values over the Cholesky diagonal of
+ *   that matrix; the matrix itself is the host loop's sum over the device's rows bit for bit (mloam_full_hessian). */
+int mloam_set_gf_float(mloam_ctx_t *ctx, int on, float map_deg_thre);
+int mloam_set_gf_float_threshold(mloam_ctx_t *ctx, float map_deg_thre);
+int mloam_gf_float_report(mloam_ctx_t *ctx, double *ratio_cur, double *deg_factor, int *total_feat_num, int *evaluated_last_call,
+                          long long *frame_cnt);
 
 /* ---- Estimator::goodFeatureMatching, the odometry-side twin (estimator.cpp:1347-1517): features of frame i (sensor frame) against the local map
  * in `slot`, matched at pose_local = pivot^-1 * pose_i * ext (n_neigh 5, CHECK_FOV false); rows from evaluateFeatJacobian (:1273-1345):

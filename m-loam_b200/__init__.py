@@ -37,6 +37,7 @@ ABI_SYMBOLS = [
     "mloam_cal_timestamp", "mloam_set_front_end", "mloam_front_end", "mloam_frame_raw", "mloam_frame_raw_device", "mloam_frame_set_next_raw",
     "mloam_frame_set_next_raw_device", "mloam_set_outlier", "mloam_frame_outlier", "mloam_keyframe_outlier",
     "mloam_undistort_poses", "mloam_set_distortion", "mloam_frame_undistort",
+    "mloam_full_hessian", "mloam_set_gf_float", "mloam_set_gf_float_threshold", "mloam_gf_float_report",
 ]
 
 
@@ -512,6 +513,30 @@ class Context:
         self._ck(lib().mloam_good_features_odom(self._h, slot, ord(kind), _p(pts), n, _p(a), _p(b), _p(e), C.c_double(gf_ratio), C.c_ulonglong(seed),
                                                 _p(sel), C.byref(n_sel), _p(H), _p(matched), _p(jaco)))
         return {"sel": sel[:n_sel.value].copy(), "H": H.reshape(6, 6), "matched": matched[:n].astype(bool), "jaco": jaco[:n]}
+
+    def full_hessian(self, slot: int, kind: str, pts, pose7, cov6=None, H=None, feat_num: int = 0):
+        """evalFullHessian for one feature set: returns (H + sum J^T J over the matched features, feat_num + their count).  H None: 1e-6 I."""
+        pts = _cloud(pts)
+        n = pts.shape[0]
+        x = np.ascontiguousarray(pose7, np.float64)
+        Hm = (np.eye(6) * 1e-6 if H is None else np.array(H, np.float64)).reshape(36).copy()
+        cv = None if cov6 is None else np.ascontiguousarray(cov6, np.float32)
+        fn = C.c_int(feat_num)
+        self._ck(lib().mloam_full_hessian(self._h, slot, ord(kind), _p(pts), n, _p(cv), _p(x), _p(Hm), C.byref(fn)))
+        return Hm.reshape(6, 6), fn.value
+
+    def set_gf_float(self, on: bool, map_deg_thre: float = 0.0):
+        """gd_float (needs params.gf_method = 3): the ratio is adapted on the device every 10th solve call."""
+        self._ck(lib().mloam_set_gf_float(self._h, int(bool(on)), C.c_float(map_deg_thre)))
+
+    def set_gf_float_threshold(self, map_deg_thre: float):
+        self._ck(lib().mloam_set_gf_float_threshold(self._h, C.c_float(map_deg_thre)))
+
+    def gf_float_report(self):
+        r, f = C.c_double(0), C.c_double(0)
+        t, e, k = C.c_int(0), C.c_int(0), C.c_longlong(0)
+        self._ck(lib().mloam_gf_float_report(self._h, C.byref(r), C.byref(f), C.byref(t), C.byref(e), C.byref(k)))
+        return {"ratio_cur": r.value, "deg_factor": f.value, "total_feat_num": t.value, "evaluated": bool(e.value), "frame_cnt": k.value}
 
     # ---- submap assembly with uncertainty
     @staticmethod

@@ -152,7 +152,7 @@ void mloam_ctx_destroy(mloam_ctx_t *h) {
                     &c->host_work, &c->odom_work, &c->ctl, &c->front_work, &c->front_out})
     b->release();
   c->frame_main.release(), c->frame_alt.release(), c->next_in.release(), c->stamps.release(), c->ua_scan.release(), c->pose_cov.release();
-  c->outlier.release(), c->undist.release();
+  c->outlier.release(), c->undist.release(), c->gf_float.release();
   if (c->pinned) cudaFreeHost(c->pinned);
   if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
   for (Branch *b : {&c->br_maps, &c->br_scan, &c->br_ahead, &c->br_ahead_scan}) {
@@ -204,6 +204,11 @@ int mloam_profile_get(mloam_ctx_t *h, const char *name, double *ms_total, long l
   if (!strcmp(name, "graph_capture_failures")) {  // frames that ran on the stream path because their graph capture failed
     if (ms_total) *ms_total = 0.0;
     if (launches) *launches = c->graph_capture_failures;
+    return MLOAM_OK;
+  }
+  if (!strcmp(name, "graph_captures")) {  // frame graphs captured and instantiated so far
+    if (ms_total) *ms_total = 0.0;
+    if (launches) *launches = c->graph_captures;
     return MLOAM_OK;
   }
   // query counts / SM cycles of the matcher's search paths (k_match_knn), reported through `launches`

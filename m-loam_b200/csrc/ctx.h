@@ -184,6 +184,20 @@ struct UndistStage {
   ud::UndistPose pose[MLOAM_MAX_LIDARS];   // per LiDAR the pose TransformToEnd moves its features with
 };
 
+// gd_float (mloam_set_gf_float; gf_kernels.cu k_gf_full_hessian): what the mapper carries from frame to frame, on the device.
+// k_gf_select reads ratio_cur there, so the host never sees the ratio on a frame's path.
+struct GfFloatState {
+  double ratio_cur;    // gf_ratio_cur (lidar_mapper_keyframe.cpp:1248, :474-492)
+  double deg_factor;   // gf_deg_factor of the last evaluation (:470)
+  int total_feat_num;  // matched surf + corner features of the last evaluation
+  int evaluations;     // evaluations since the mode was turned on
+};
+// Ctx::gf_float: the state, then the device end of PinnedBlock::gf_float_cfg
+struct GfFloatDev {
+  GfFloatState st;
+  double cfg[2];
+};
+
 // The context's pinned host block (Ctx::pinned): staging of small host-to-device copies and landing of small read-backs, so that
 // they are truly asynchronous.
 struct PinnedBlock {
@@ -206,6 +220,8 @@ struct PinnedBlock {
   alignas(16) unsigned char odom[4096];  // OdomState mirror (odom_kernels.cu)
   double normal_eq[30];             // mloam_normal_equations read-back
   double pose_plus[64];             // mloam_pose_plus: x | delta | V in, result at [56]
+  double gf_float_cfg[2];           // scan2map_enqueue (gd_float): MAP_DEG_THRE | gf_ratio_ini, read by a captured copy like pose
+  GfFloatState gf_float;            // GfFloatState mirror, landed with LMState
   int scan_info[2][MLOAM_MAX_RINGS];       // mloam_frame: ScanInfo of the sweep (start | end)
   int scan_info_next[2][MLOAM_MAX_RINGS];  // ... and of the announced next sweep, copied on Ctx::br_ahead
 };
@@ -415,6 +431,7 @@ struct Ctx {
   std::vector<GraphEntry> graphs;
   bool smem_opt_in_gf = false;     // k_gf_select's 200 KB pool
   bool smem_opt_in[3] = {false, false, false};  // >48 KB dynamic shared memory enabled for k_voxel_small / k_ring_pick / k_ring_voxel
+  long long graph_captures = 0;          // frame graphs captured and instantiated (mloam_profile_get "graph_captures")
   long long graph_capture_failures = 0;  // frames that fell back to the stream path because their capture failed (mloam_profile_get "graph_capture_failures")
   int use_graphs = 1;
   unsigned knn_tma_min = 8;        // kNN staging: runs of >= this many points use TMA bulk copies, shorter ones 16 B loads (MLOAM_KNN_TMA_MIN)
@@ -486,6 +503,17 @@ struct Ctx {
   int undist_n = 0;
   double undist_pose7[MLOAM_MAX_LIDARS][7];
   DevBuf undist;                   // the staged configuration
+  // gd_float (mloam_set_gf_float): every 10th solve call that passes the map gate evaluates the full information matrix of the scan
+  // (evalFullHessian) from the Jacobian rows of outer iteration 0 and sets the ratio k_gf_select reads from GfFloatDev.  Allocated once,
+  // outside alloc_epoch(): turning the mode on re-captures nothing.  MAP_DEG_THRE and gf_ratio_ini are staged (PinnedBlock::gf_float_cfg).
+  bool gf_float_on = false;
+  float gf_float_thre = 0.f;
+  long long gf_float_frames = 0;   // frame_cnt (:1059): solve calls since the mode was turned on
+  bool gf_float_eval = false;      // this call's frame_cnt % 10 == 0
+  bool gf_float_evaluated = false; // ... and it passed the map gate: the last call evaluated
+  bool gf_float_reported = false;  // a solve call has run since the mode was turned on
+  DevBuf gf_float;                 // GfFloatDev
+  GfFloatState gf_float_host{};    // the state as the last solve call left it (mloam_gf_float_report)
   double pose_cov36[36] = {0};     // pose_wmap_curr.cov_ of the last mloam_frame* / mloam_scan2map* call
   bool last_scan_valid = false;    // last_scan describes the scan of the last mloam_frame* call (mloam_frame_scan)
   ScanRef last_scan{};
@@ -585,8 +613,13 @@ int transform_points_device(Ctx *c, float4 *d_pts, int n, const int *d_n, const 
 
 // gf_kernels.cu: good-feature selection of one matched feature set on the device (goodFeatureMatching inside
 // scan2MapOptimization): Jacobian rows + selection, result as a 0/1 mask over the features (set index t: 0 corner, 1 surf)
+// d_ratio (nullable): the ratio on the device (GfFloatState::ratio_cur), read in place of gf_ratio.  phase: 3 rows + selection,
+// 1 the Jacobian rows only, 2 the selection over the rows phase 1 left (an evaluation frame puts gf_full_hessian_device between them)
 int gf_select_set_device(Ctx *c, int t, const FeatSet &fs, const double *d_pose7, double default_sinfo, int method, double gf_ratio,
-                         unsigned long long seed, unsigned char **d_mask_out);
+                         unsigned long long seed, unsigned char **d_mask_out, const double *d_ratio = nullptr, int phase = 3);
+// evalFullHessian + the gd_float policy over the rows phase 1 left in Ctx::gf_work for sets[1] (surf) then sets[0] (corner): one launch
+int gf_full_hessian_device(Ctx *c, const FeatSet *sets);
+void stage_gf_float(Ctx *c);  // writes PinnedBlock::gf_float_cfg
 
 // uct_kernels.cu: per-point sqrt_info from PointIWithCov::cov_vec (float[6] per point)
 int sqrt_info_device(Ctx *c, const float *d_cov6, int n, double *d_sinfo);

@@ -11,8 +11,13 @@
 //     gd   stochastic greedy: lane 0 draws the round's candidates (same pool / visited bookkeeping as the reference),
 //          the warp evaluates their log-dets in parallel (6x6 Cholesky each) and picks the best;
 //     fps  farthest-point sampling: 1024 threads update the min-distance table and arg-max it per pick.
+// gd_float (lidar_mapper_keyframe.cpp:456-495): every 10th frame evalFullHessian (lidar_mapper.h:176-227) sums J^T J over every matched
+// feature at the pose and with the rows phase 1 already made; k_gf_full_hessian reduces them in the reference's order, takes the
+// log-determinant and leaves the ratio of the next ten frames on the device, where k_gf_select reads it.
 // The reference's mt19937(random_device) is replaced by an explicit PCG32 seed and its time cap is dropped — see
 // oracle/orc_gf.hpp for the restatement the kernels are checked against pick by pick.
+#include <cuda_pipeline.h>
+
 #include <vector>
 
 #include "ctx.h"
@@ -108,11 +113,8 @@ __device__ __forceinline__ void gf_add_outer(double *H, const double *j) {
   for (int a = 0; a < 6; a++)
     for (int b = 0; b < 6; b++) H[a * 6 + b] += j[a] * j[b];
 }
-// common::logDet(H + J^T J, true): LLT, 2 * sum log(diag)   (math.hpp:172-202)
-__device__ double gf_logdet_with(const double *H, const double *j) {
-  double A[36];
-  for (int a = 0; a < 6; a++)
-    for (int b = 0; b < 6; b++) A[a * 6 + b] = H[a * 6 + b] + j[a] * j[b];
+// common::logDet(A, true): LLT, 2 * sum log(diag)   (math.hpp:172-202); A is overwritten
+__device__ double gf_logdet(double *A) {
   double s = 0.0;
   for (int c = 0; c < 6; c++) {
     double d = A[c * 6 + c];
@@ -129,10 +131,89 @@ __device__ double gf_logdet_with(const double *H, const double *j) {
   }
   return 2.0 * s;
 }
+__device__ double gf_logdet_with(const double *H, const double *j) {  // logDet(H + J^T J, true)
+  double A[36];
+  for (int a = 0; a < 6; a++)
+    for (int b = 0; b < 6; b++) A[a * 6 + b] = H[a * 6 + b] + j[a] * j[b];
+  return gf_logdet(A);
+}
+
+// ---- evalFullHessian + the gd_float policy.  One CTA.  The reference adds J^T J feature by feature into one mat_H (surf, then corner),
+// and the factor feeds a threshold, so the sum keeps that order: thread e < 21 owns element e of the upper triangle and walks the
+// rows in index order, one multiply and one add per row like the host loop; the 21 chains are independent, so they run side by side.
+// All threads stage the next tile of rows into shared memory (cp.async, double-buffered) while the 21 walk the current one.
+// Unmatched features are walked too: k_gf_jaco left them all-zero rows, each product is +0 or -0, and x + (+-0) == x for every partial sum
+// that occurs (the diagonal starts at 1e-6 and grows; an off-diagonal starts at +0 and a sum of +0 with +-0 terms stays +0) — the same
+// bits as skipping them, without a flag test in the chain.
+constexpr int FH_THREADS = 256;
+constexpr int FH_TILE = 448;  // rows per tile: 2 x 21 KB of shared memory
+struct FhSet {
+  const double *jaco;            // n x 6, 16-byte aligned
+  const unsigned char *matched;
+  int n;
+  const int *d_n;                // nullable device-side count
+};
+__global__ void __launch_bounds__(FH_THREADS) k_gf_full_hessian(FhSet s0, FhSet s1, const double *H_in, const double *__restrict__ cfg,
+                                                                GfFloatState *__restrict__ st, double *H_out /* may be H_in */,
+                                                                int *__restrict__ feat_io) {
+  __shared__ __align__(16) double tile[2][FH_TILE * 6];
+  __shared__ double Hs[21], A[36];  // the triangle, then the full matrix the Cholesky overwrites
+  __shared__ int s_cnt;
+  const int tid = threadIdx.x;
+  int ea = 0, eb = 0;  // element tid of the upper triangle, row-major: (0,0) (0,1) ... (0,5) (1,1) ...
+  for (int e = 0, a = 0; a < 6; a++)
+    for (int b = a; b < 6; b++, e++)
+      if (e == tid) ea = a, eb = b;
+  double acc = H_in ? H_in[ea * 6 + eb] : (ea == eb ? 1e-6 : 0.0);  // mat_H = I * 1e-6 (:461)
+  if (tid == 0) s_cnt = 0;
+  __syncthreads();
+  int cnt = 0;
+  for (int set = 0; set < 2; set++) {
+    const FhSet S = set ? s1 : s0;
+    const int n = S.d_n ? min(S.n, *S.d_n) : S.n;
+    const int tiles = (n + FH_TILE - 1) / FH_TILE;
+    auto stage = [&](int k) {  // rows [k * FH_TILE, ...) -> tile[k & 1], 16 B per copy (a row is 3 of them)
+      const int rows = min(FH_TILE, n - k * FH_TILE);
+      const double *src = S.jaco + (size_t)k * FH_TILE * 6;
+      for (int q = tid; q < rows * 3; q += FH_THREADS) __pipeline_memcpy_async(&tile[k & 1][q * 2], src + q * 2, 16);
+      __pipeline_commit();
+    };
+    if (tiles > 0) stage(0);
+    for (int k = 0; k < tiles; k++) {
+      if (k + 1 < tiles) stage(k + 1);
+      __pipeline_wait_prior(k + 1 < tiles ? 1 : 0);
+      __syncthreads();
+      if (tid < 21) {
+        const double *r = tile[k & 1];
+        const int rows = min(FH_TILE, n - k * FH_TILE);
+        for (int i = 0; i < rows; i++) acc += r[i * 6 + ea] * r[i * 6 + eb];
+      }
+      __syncthreads();  // tile[k & 1] is staged again two iterations on
+    }
+    for (int i = tid; i < n; i += FH_THREADS) cnt += S.matched[i] ? 1 : 0;
+  }
+  if (tid < 21) Hs[tid] = acc;
+  if (cnt) atomicAdd(&s_cnt, cnt);
+  __syncthreads();
+  if (tid == 0) {
+    for (int e = 0, a = 0; a < 6; a++)
+      for (int b = a; b < 6; b++, e++) A[a * 6 + b] = A[b * 6 + a] = Hs[e];
+    if (H_out)
+      for (int i = 0; i < 36; i++) H_out[i] = A[i];
+    const int total = (feat_io ? *feat_io : 0) + s_cnt;
+    if (feat_io) *feat_io = total;
+    if (st) {  // :470-492
+      const double f = gf_logdet(A);
+      st->deg_factor = f, st->total_feat_num = total, st->evaluations += 1;
+      st->ratio_cur = f > cfg[0] ? cfg[1] : 0.8;  // <= MAP_DEG_THRE takes 0.8
+    }
+  }
+}
 
 struct GfArgs {
   int method;  // 0 wo_gf, 1 rnd, 2 fps, 3 gd
   double gf_ratio;
+  const double *d_ratio;  // nullable: the ratio on the device (gd_float, GfFloatState::ratio_cur), read in place of gf_ratio
   unsigned long long seed;
   int n;
   const int *d_n;  // nullable device-side feature count (n is then the upper bound the buffers are sized for)
@@ -170,7 +251,7 @@ __global__ void __launch_bounds__(GF_THREADS) k_gf_select(GfArgs a) {
   const unsigned char *const matched = matched_in_smem ? matched_s : a.matched;
   if (a.mask)
     for (int i = tid; i < n; i += GF_THREADS) a.mask[i] = 0;
-  const int num_use = (int)((size_t)((size_t)n * a.gf_ratio));  // static_cast<size_t>(num_all_features * gf_ratio), :248
+  const int num_use = (int)((size_t)((size_t)n * (a.d_ratio ? *a.d_ratio : a.gf_ratio)));  // static_cast<size_t>(num_all_features * gf_ratio), :248
   if (tid < 36) H[tid] = (tid % 7 == 0) ? 1e-6 : 0.0;              // sub_mat_H = I * 1e-6 (:504, :519)
   if (tid == 0) s_num_sel = 0, s_stop = 0, s_pick = -1;
   for (int i = tid; i <= n; i += GF_THREADS) fen[i] = i & -i;    // Fenwick tree of an all-ones array
@@ -363,7 +444,7 @@ static int gf_select_launch(Ctx *c, GfArgs &a) {
 
 // Device-resident selection of one matched feature set (inside scan2MapOptimization): no host round trip.
 int gf_select_set_device(Ctx *c, int t, const FeatSet &fs, const double *d_pose7, double default_sinfo, int method, double gf_ratio,
-                         unsigned long long seed, unsigned char **d_mask_out) {
+                         unsigned long long seed, unsigned char **d_mask_out, const double *d_ratio, int phase) {
   const int n = fs.n;
   *d_mask_out = nullptr;
   if (n <= 0) return MLOAM_OK;
@@ -371,15 +452,47 @@ int gf_select_set_device(Ctx *c, int t, const FeatSet &fs, const double *d_pose7
   double *d_jaco;
   int rc = gf_work(c, c->gf_work[t], n, &a, &d_jaco, nullptr);
   if (rc) return rc;
-  k_gf_jaco<<<(n + 127) / 128, 128, 0, c->stream>>>(fs.pts, fs.valid, fs.coeff, n, fs.d_n, fs.is_plane ? 1 : 0, nullptr, fs.sinfo, default_sinfo,
-                                                   d_pose7, d_jaco);
-  c->launches++;
-  a.method = method, a.gf_ratio = gf_ratio, a.seed = seed, a.n = n, a.d_n = fs.d_n;
+  if (phase & 1) {
+    k_gf_jaco<<<(n + 127) / 128, 128, 0, c->stream>>>(fs.pts, fs.valid, fs.coeff, n, fs.d_n, fs.is_plane ? 1 : 0, nullptr, fs.sinfo, default_sinfo,
+                                                     d_pose7, d_jaco);
+    c->launches++;
+  }
+  if (!(phase & 2)) return MLOAM_OK;
+  a.method = method, a.gf_ratio = gf_ratio, a.d_ratio = d_ratio, a.seed = seed, a.n = n, a.d_n = fs.d_n;
   a.matched = fs.valid, a.pts = fs.pts;
   rc = gf_select_launch(c, a);
   if (rc) return rc;
   *d_mask_out = a.mask;
   return MLOAM_OK;
+}
+
+static int full_hessian_launch(Ctx *c, const FhSet &s0, const FhSet &s1, const double *d_H_in, const double *d_cfg, GfFloatState *d_st,
+                               double *d_H_out, int *d_feat_io) {
+  ProfScope ps(c, "gf_full_hessian");
+  k_gf_full_hessian<<<1, FH_THREADS, 0, c->stream>>>(s0, s1, d_H_in, d_cfg, d_st, d_H_out, d_feat_io);
+  c->launches++;
+  MLOAM_CUDA_OK(c, cudaGetLastError());
+  return MLOAM_OK;
+}
+
+void stage_gf_float(Ctx *c) { c->pinned->gf_float_cfg[0] = (double)c->gf_float_thre, c->pinned->gf_float_cfg[1] = (double)c->params.gf_ratio; }
+
+int gf_full_hessian_device(Ctx *c, const FeatSet *sets) {
+  GfFloatDev *d = c->gf_float.as<GfFloatDev>();
+  stage_gf_float(c);
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(d->cfg, c->pinned->gf_float_cfg, sizeof(d->cfg), cudaMemcpyHostToDevice, c->stream));
+  FhSet fs[2];  // [0] surf (sets[1]), [1] corner (sets[0]): the order of :463-467
+  for (int k = 0; k < 2; k++) {
+    const FeatSet &S = sets[1 - k];
+    GfArgs a;
+    double *d_jaco = nullptr;
+    if (S.n > 0) {
+      const int rc = gf_work(c, c->gf_work[1 - k], S.n, &a, &d_jaco, nullptr);  // where phase 1 left the rows
+      if (rc) return rc;
+    }
+    fs[k] = FhSet{d_jaco, S.valid, S.n > 0 ? S.n : 0, S.d_n};
+  }
+  return full_hessian_launch(c, fs[0], fs[1], nullptr, d->cfg, &d->st, nullptr, nullptr);
 }
 
 }  // namespace mloam
@@ -415,6 +528,44 @@ extern "C" int mloam_good_features_odom(mloam_ctx_t *h, int slot, int type, cons
   return good_features_impl(h, slot, type, h_pts, n, nullptr, local, x21, gf_ratio == 1.0 ? 0 : 3, gf_ratio, seed, h_sel, n_sel, H36, h_matched, h_jaco);
 }
 
+// Phase 1 of a host-buffer call: the features go up, are matched against map `slot` at pose7 and get their Jacobian rows (odom_x21: the
+// odometry-side rows) in Ctx::host_work, whose regions *a and *d_jaco then name.  fixed5: n_neigh 5 and CHECK_FOV false whatever the
+// parameters say (estimator.cpp:1377; lidar_mapper.h:187,193).
+static int gf_rows_host(Ctx *c, int slot, int type, const mloam_point_t *h_pts, int n, const float *h_cov6, const double *pose7,
+                        const double *odom_x21, bool fixed5, GfArgs *a, double **d_jaco) {
+  const int t = type == 's' ? 1 : 0;
+  MLOAM_CUDA_OK(c, c->scan_pts[t].reserve(sizeof(float4) * (size_t)n));
+  int rc = reserve_feat(c, t, n);
+  if (rc) return rc;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->scan_pts[t].p, h_pts, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
+  double *d_pose;
+  rc = upload_pose(c, pose7, &d_pose);
+  if (rc) return rc;
+  MatchCfg mcfg = match_cfg(c);
+  if (fixed5) mcfg.n_neigh = 5, mcfg.check_fov = 0;
+  rc = match_from_map_device(c, slot, type, c->scan_pts[t].as<float4>(), n, nullptr, d_pose, mcfg,
+                             c->feat_valid[t].as<unsigned char>(), c->feat_coeff[t].as<float>(), nullptr);
+  if (rc) return rc;
+  float *d_cov = nullptr;
+  rc = gf_work(c, c->host_work, n, a, d_jaco, h_cov6 ? &d_cov : nullptr);
+  if (rc) return rc;
+  if (h_cov6) MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_cov, h_cov6, sizeof(float) * 6 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
+  if (odom_x21) {
+    double *stage = c->pinned->odom_x;
+    for (int k = 0; k < 21; k++) stage[k] = odom_x21[k];
+    double *d_x21 = c->ctl.as<DevCtl>()->odom_x;
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_x21, stage, 21 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    k_gf_jaco_odom<<<(n + 127) / 128, 128, 0, c->stream>>>(c->scan_pts[t].as<float4>(), c->feat_valid[t].as<unsigned char>(), c->feat_coeff[t].as<float>(),
+                                                          n, type == 's' ? 1 : 0, d_x21, *d_jaco);
+  } else {
+    k_gf_jaco<<<(n + 127) / 128, 128, 0, c->stream>>>(c->scan_pts[t].as<float4>(), c->feat_valid[t].as<unsigned char>(), c->feat_coeff[t].as<float>(), n,
+                                                     nullptr, type == 's' ? 1 : 0, d_cov, nullptr, map_sqrt_info(c->params.cov_trace), d_pose, *d_jaco);
+  }
+  c->launches++;
+  a->matched = c->feat_valid[t].as<unsigned char>(), a->pts = c->scan_pts[t].as<float4>();
+  return MLOAM_OK;
+}
+
 static int good_features_impl(mloam_ctx_t *h, int slot, int type, const mloam_point_t *h_pts, int n, const float *h_cov6, const double *pose7,
                               const double *odom_x21, int method, double gf_ratio, unsigned long long seed, int *h_sel, int *n_sel, double *H36,
                               unsigned char *h_matched, double *h_jaco) {
@@ -426,39 +577,11 @@ static int good_features_impl(mloam_ctx_t *h, int slot, int type, const mloam_po
   *n_sel = 0;
   for (int i = 0; i < 36; i++) H36[i] = (i % 7 == 0) ? 1e-6 : 0.0;
   if (n == 0) return MLOAM_OK;
-  const int t = type == 's' ? 1 : 0;
-  MLOAM_CUDA_OK(c, c->scan_pts[t].reserve(sizeof(float4) * (size_t)n));
-  int rc = reserve_feat(c, t, n);
-  if (rc) return rc;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->scan_pts[t].p, h_pts, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
-  double *d_pose;
-  rc = upload_pose(c, pose7, &d_pose);
-  if (rc) return rc;
-  MatchCfg mcfg = match_cfg(c);
-  if (odom_x21) mcfg.n_neigh = 5, mcfg.check_fov = 0;  // estimator.cpp:1377, :1393 / :1403
-  rc = match_from_map_device(c, slot, type, c->scan_pts[t].as<float4>(), n, nullptr, d_pose, mcfg,
-                             c->feat_valid[t].as<unsigned char>(), c->feat_coeff[t].as<float>(), nullptr);
-  if (rc) return rc;
   GfArgs a;
   double *d_jaco;
-  float *d_cov = nullptr;
-  rc = gf_work(c, c->host_work, n, &a, &d_jaco, h_cov6 ? &d_cov : nullptr);
+  int rc = gf_rows_host(c, slot, type, h_pts, n, h_cov6, pose7, odom_x21, odom_x21 != nullptr, &a, &d_jaco);
   if (rc) return rc;
-  if (h_cov6) MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_cov, h_cov6, sizeof(float) * 6 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
-  if (odom_x21) {
-    double *stage = c->pinned->odom_x;
-    for (int k = 0; k < 21; k++) stage[k] = odom_x21[k];
-    double *d_x21 = c->ctl.as<DevCtl>()->odom_x;
-    MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_x21, stage, 21 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-    k_gf_jaco_odom<<<(n + 127) / 128, 128, 0, c->stream>>>(c->scan_pts[t].as<float4>(), c->feat_valid[t].as<unsigned char>(), c->feat_coeff[t].as<float>(),
-                                                          n, type == 's' ? 1 : 0, d_x21, d_jaco);
-  } else {
-    k_gf_jaco<<<(n + 127) / 128, 128, 0, c->stream>>>(c->scan_pts[t].as<float4>(), c->feat_valid[t].as<unsigned char>(), c->feat_coeff[t].as<float>(), n,
-                                                     nullptr, type == 's' ? 1 : 0, d_cov, nullptr, map_sqrt_info(c->params.cov_trace), d_pose, d_jaco);
-  }
-  c->launches++;
-  a.method = method, a.gf_ratio = gf_ratio, a.seed = seed, a.n = n, a.d_n = nullptr, a.mask = nullptr;
-  a.matched = c->feat_valid[t].as<unsigned char>(), a.pts = c->scan_pts[t].as<float4>();
+  a.method = method, a.gf_ratio = gf_ratio, a.d_ratio = nullptr, a.seed = seed, a.n = n, a.d_n = nullptr, a.mask = nullptr;
   rc = gf_select_launch(c, a);
   if (rc) return rc;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(n_sel, a.n_sel, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -466,6 +589,28 @@ static int good_features_impl(mloam_ctx_t *h, int slot, int type, const mloam_po
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_sel, a.sel, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
   if (h_matched) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_matched, a.matched, (size_t)n, cudaMemcpyDeviceToHost, c->stream));
   if (h_jaco) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_jaco, d_jaco, sizeof(double) * 6 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
+  return MLOAM_OK;
+}
+
+// ActiveFeatureSelection::evalFullHessian (lidar_mapper.h:176-227) for one feature set: H36 and *feat_num accumulate
+extern "C" int mloam_full_hessian(mloam_ctx_t *h, int slot, int type, const mloam_point_t *h_pts, int n, const float *h_cov6, const double *pose7,
+                                  double *H36, int *feat_num) {
+  if (!h || n < 0 || !pose7 || !H36 || !feat_num || (n > 0 && !h_pts) || (type != 's' && type != 'c')) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  cudaSetDevice(c->device);
+  if (n == 0) return MLOAM_OK;
+  GfArgs a;
+  double *d_jaco;
+  int rc = gf_rows_host(c, slot, type, h_pts, n, h_cov6, pose7, nullptr, true, &a, &d_jaco);
+  if (rc) return rc;
+  // the caller's mat_H and feat_num go to the selection's H and n_sel words, and come back from there
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(a.H, H36, 36 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(a.n_sel, feat_num, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  rc = full_hessian_launch(c, FhSet{d_jaco, a.matched, n, nullptr}, FhSet{nullptr, nullptr, 0, nullptr}, a.H, nullptr, nullptr, a.H, a.n_sel);
+  if (rc) return rc;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(H36, a.H, 36 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(feat_num, a.n_sel, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
   return MLOAM_OK;
 }

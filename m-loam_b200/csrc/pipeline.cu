@@ -108,15 +108,28 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool wa
     sets[0].mask = sets[1].mask = nullptr;
     if (P.gf_method != 0) {
       unsigned char *mask[2] = {nullptr, nullptr};
-      auto select = [&](int t) {
+      // gd_float: the ratio is read on the device; an evaluation frame's first iteration makes both sets' rows, evaluates the full
+      // Hessian over them (which sets that ratio, :456-495) and only then selects
+      const double *d_ratio = c->gf_float_on ? &c->gf_float.as<GfFloatDev>()->st.ratio_cur : nullptr;
+      const bool eval = c->gf_float_on && c->gf_float_eval && outer == 0;
+      auto select = [&](int t, int phase) {
         if (sets[t].n <= 0) return MLOAM_OK;
         return gf_select_set_device(c, t, sets[t], d_pose, sinfo, P.gf_method, (double)P.gf_ratio,
-                                    (unsigned long long)P.gf_seed + 2ull * (unsigned long long)outer + (unsigned long long)t, &mask[t]);
+                                    (unsigned long long)P.gf_seed + 2ull * (unsigned long long)outer + (unsigned long long)t, &mask[t], d_ratio,
+                                    phase);
       };
+      if (eval) {
+        rc = select(0, 1);
+        if (rc == MLOAM_OK) rc = select(1, 1);
+        if (rc == MLOAM_OK) rc = gf_full_hessian_device(c, sets);
+        if (rc) return rc;
+        c->gf_float_evaluated = true;
+      }
+      const int phase = eval ? 2 : 3;
       // the two selections are independent single-CTA chains: corner on the side stream next to surf (also inside a captured graph)
       const bool fork_gf = !c->prof_on && sets[0].n > 0 && sets[1].n > 0;
-      rc = on_branch(c, c->br_scan, fork_gf, [&] { return select(0); });
-      if (rc == MLOAM_OK) rc = select(1);
+      rc = on_branch(c, c->br_scan, fork_gf, [&] { return select(0, phase); });
+      if (rc == MLOAM_OK) rc = select(1, phase);
       if (rc) return rc;
       if (fork_gf) MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream, c->br_scan.join, 0));
       sets[0].mask = mask[0], sets[1].mask = mask[1];
@@ -168,6 +181,8 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool wa
     stamp(c, "pose covariance");
   }
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(hs, st, sizeof(LMState), cudaMemcpyDeviceToHost, c->stream));
+  if (c->gf_float_on)  // the report (mloam_gf_float_report) lands with the frame's results
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(&c->pinned->gf_float, &c->gf_float.as<GfFloatDev>()->st, sizeof(GfFloatState), cudaMemcpyDeviceToHost, c->stream));
   if (S.d_n_surf) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_cnt, S.d_n_surf, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   if (S.d_n_corner) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_cnt + 1, S.d_n_corner, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   return MLOAM_OK;
@@ -182,6 +197,7 @@ int scan2map_finish(Ctx *c, const ScanRef &S, const double *pose_init7, bool wan
   const LMState *hs = &c->pinned->lm;
   int *h_cnt = c->pinned->counts;
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
+  if (c->gf_float_on) c->gf_float_host = c->pinned->gf_float;
   if (!S.d_n_surf) h_cnt[0] = S.n_surf;
   if (!S.d_n_corner) h_cnt[1] = S.n_corner;
   for (int k = 0; k < 7; k++) pose_out7[k] = hs->x[k];
@@ -224,9 +240,24 @@ int scan2map_finish(Ctx *c, const ScanRef &S, const double *pose_init7, bool wan
   return MLOAM_OK;
 }
 
+// gd_float: what every solve call does first.  frame_cnt advances before the map gate (lidar_mapper_keyframe.cpp:1059, :429); the 10th,
+// 20th, ... call evaluates if it passes the gate (scan2map_enqueue).
+int gf_float_begin(Ctx *c) {
+  if (!c->gf_float_on) return MLOAM_OK;
+  if (c->params.gf_method != 3) return fail(c, MLOAM_E_STATE, "gd_float is on (mloam_set_gf_float) and params.gf_method is no longer 3");
+  if (c->nccl_comm || c->p2p_on) return fail(c, MLOAM_E_STATE, "gd_float (mloam_set_gf_float) is single-GPU only; detach the communicator or turn it off");
+  c->gf_float_frames++;
+  c->gf_float_eval = c->gf_float_frames % 10 == 0;
+  c->gf_float_evaluated = false;
+  c->gf_float_reported = true;
+  return MLOAM_OK;
+}
+
 int scan2map_run(Ctx *c, const ScanRef &S, const double *pose_init7, bool want_cov, double *pose_out7, mloam_solve_stats_t *stats) {
   int ran = 0;
-  int rc = scan2map_enqueue(c, S, pose_init7, want_cov, &ran);
+  int rc = gf_float_begin(c);
+  if (rc) return rc;
+  rc = scan2map_enqueue(c, S, pose_init7, want_cov, &ran);
   if (rc) return rc;
   return scan2map_finish(c, S, pose_init7, want_cov, ran, pose_out7, stats);
 }
@@ -294,6 +325,7 @@ void stage_frame_inputs(Ctx *c, const double *pose7) {
   if (c->with_ua) ua_stage_host(c);
   if (c->outlier_on) stage_outlier(c);
   if (c->undist_on) stage_undistort(c);
+  if (c->gf_float_on) stage_gf_float(c);
 }
 
 // Whether the look-ahead of the previous frame made the features of sw: same caller pointer and sizes; a raw sweep's features are taken by
@@ -568,6 +600,10 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
   const bool want_cov = c->with_ua != 0;
   c->last_scan_valid = false;
   c->frame_from_graph = false;
+  {
+    const int rc = gf_float_begin(c);
+    if (rc) return rc;
+  }
   const bool can_graph = c->use_graphs && c->params.max_inner == 1 && !c->prof_on && (!c->nccl_comm || c->p2p_on);
   if (can_graph) {
     unsigned long long key = 1469598103934665603ull;
@@ -593,6 +629,10 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
     }
     if (c->undist_on) {  // the undistortion's launch and the look-ahead's split (poses and scan period are staged)
       const int on[2] = {'u', c->undist_n};
+      key = fnv1a(key, on, sizeof(on));
+    }
+    if (c->gf_float_on) {  // gd_float: the ratio's device read, and an evaluation frame's extra launch (threshold, gf_ratio_ini and the
+      const int on[2] = {'g', c->gf_float_eval ? 1 : 0};  // ratio itself are not in the key: they are staged or stay on the device)
       key = fnv1a(key, on, sizeof(on));
     }
     if (sw.raw) {  // raw frame: the per-LiDAR counts and the front-end parameters are kernel arguments of the captured front end
@@ -625,6 +665,7 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
       MLOAM_CUDA_OK(c, cudaGraphLaunch(e->exec, c->stream));
       c->frame_from_graph = true;
       c->launches += e->launches;
+      c->gf_float_evaluated = c->gf_float_on && c->gf_float_eval && e->s2m_ran;
       frame_advance(c, parity, e->prefetched_out);
       c->last_scan = e->S, c->last_scan_valid = true;
       return scan2map_finish(c, e->S, pose_init7, want_cov, e->s2m_ran, pose_out7, stats);
@@ -645,6 +686,7 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
         e->launches = (int)(c->launches - l0), e->epoch = ep0, e->S = S, e->s2m_ran = ran;
         e->prefetched_out = c->prefetched;
         c->launches = l0;
+        c->graph_captures++;
         c->graph_pdl_edges = count_programmatic_edges(graph);
         cudaGraphDestroy(graph);
         MLOAM_CUDA_OK(c, cudaGraphLaunch(e->exec, c->stream));
@@ -1142,6 +1184,52 @@ int mloam_frame_outlier(mloam_ctx_t *h, mloam_point_t *h_pts, float *h_cov6, int
   if (h_pts) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_pts, S.outlier, sizeof(float4) * (size_t)m, cudaMemcpyDeviceToHost, st));
   if (h_cov6) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_cov6, S.cov6_outlier, sizeof(float) * 6 * (size_t)m, cudaMemcpyDeviceToHost, st));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  return MLOAM_OK;
+}
+
+// ------------------------------------------------------------------------------------------ gd_float
+int mloam_set_gf_float(mloam_ctx_t *h, int on, float map_deg_thre) {
+  if (!h || (on && !(map_deg_thre == map_deg_thre))) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (!on) {
+    c->gf_float_on = false;
+    return MLOAM_OK;
+  }
+  if (c->params.gf_method != 3) return fail(c, MLOAM_E_STATE, "set_gf_float: gd_float is gd_fix with an adaptive ratio; set params.gf_method = 3 first");
+  if (c->nccl_comm || c->p2p_on)
+    return fail(c, MLOAM_E_STATE, "set_gf_float: gd_float is single-GPU only (the 21 sums of sharded features are not exchanged); detach the communicator");
+  cudaSetDevice(c->device);
+  c->gf_float.in_graphs = false;  // allocated once, so the graphs that hold its address stay valid
+  MLOAM_CUDA_OK(c, c->gf_float.reserve(sizeof(GfFloatDev)));
+  const double ini = (double)c->params.gf_ratio;
+  c->gf_float_host = GfFloatState{ini < 1.0 ? ini : 1.0, 0.0, 0, 0};  // gf_ratio_cur = std::min(1.0, FLAGS_gf_ratio_ini) (:1248)
+  c->pinned->gf_float = c->gf_float_host;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(&c->gf_float.as<GfFloatDev>()->st, &c->pinned->gf_float, sizeof(GfFloatState), cudaMemcpyHostToDevice, c->stream));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
+  c->gf_float_on = true, c->gf_float_thre = map_deg_thre;
+  c->gf_float_frames = 0, c->gf_float_eval = c->gf_float_evaluated = c->gf_float_reported = false;
+  return MLOAM_OK;
+}
+
+int mloam_set_gf_float_threshold(mloam_ctx_t *h, float map_deg_thre) {
+  if (!h || !(map_deg_thre == map_deg_thre)) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (!c->gf_float_on) return fail(c, MLOAM_E_STATE, "set_gf_float_threshold: gd_float is off (mloam_set_gf_float)");
+  c->gf_float_thre = map_deg_thre;
+  return MLOAM_OK;
+}
+
+int mloam_gf_float_report(mloam_ctx_t *h, double *ratio_cur, double *deg_factor, int *total_feat_num, int *evaluated_last_call, long long *frame_cnt) {
+  if (!h) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (!c->gf_float_on) return fail(c, MLOAM_E_STATE, "gf_float_report: gd_float is off (mloam_set_gf_float)");
+  if (!c->gf_float_reported) return fail(c, MLOAM_E_STATE, "gf_float_report: no solve call has run since gd_float was turned on");
+  const GfFloatState &g = c->gf_float_host;
+  if (ratio_cur) *ratio_cur = g.ratio_cur;
+  if (deg_factor) *deg_factor = g.deg_factor;
+  if (total_feat_num) *total_feat_num = g.total_feat_num;
+  if (evaluated_last_call) *evaluated_last_call = c->gf_float_evaluated ? 1 : 0;
+  if (frame_cnt) *frame_cnt = c->gf_float_frames;
   return MLOAM_OK;
 }
 

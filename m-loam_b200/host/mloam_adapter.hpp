@@ -389,7 +389,8 @@ class ActiveFeatureSelection {
                            Eigen::Matrix<double, 6, 6> &sub_mat_H) {
     (void)laser_map;
     mloam_ctx_t *ctx = mloam::ThreadContext::get();
-    const int method = gf_method == "wo_gf" ? 0 : gf_method == "rnd" ? 1 : gf_method == "fps" ? 2 : 3;  // gd_fix / gd_float
+    // gd_fix / gd_float are one selection; gd_float's ratio policy (lidar_mapper_keyframe.cpp:456-495) is mloam_set_gf_float
+    const int method = gf_method == "wo_gf" ? 0 : gf_method == "rnd" ? 1 : gf_method == "fps" ? 2 : 3;
     std::vector<mloam_point_t> pts = mloam::packCloud(laser_cloud);
     const int n = (int)pts.size();
     std::vector<float> cov6((size_t)n * 6 + 6);
@@ -423,6 +424,25 @@ class ActiveFeatureSelection {
     sel_feature_idx.assign(sel.begin(), sel.begin() + n_sel);
     for (int i = 0; i < 6; i++)
       for (int j = 0; j < 6; j++) sub_mat_H(i, j) = H[i * 6 + j];
+  }
+  // ActiveFeatureSelection::evalFullHessian with the reference's argument list (lidar_mapper.h:176-182): mat_H and feat_num accumulate
+  void evalFullHessian(const mloam::KdTreeFLANN<common::PointIWithCov>::Ptr &kdtree_from_map, const common::PointICovCloud &laser_map,
+                       const common::PointICovCloud &laser_cloud, const Pose &pose_local, const char feature_type,
+                       Eigen::Matrix<double, 6, 6> &mat_H, int &feat_num) {
+    (void)laser_map;
+    mloam_ctx_t *ctx = mloam::ThreadContext::get();
+    std::vector<mloam_point_t> pts = mloam::packCloud(laser_cloud);
+    const int n = (int)pts.size();
+    std::vector<float> cov6((size_t)n * 6 + 6);
+    for (int i = 0; i < n; i++)
+      for (int k = 0; k < 6; k++) cov6[(size_t)i * 6 + k] = laser_cloud.points[i].cov_vec[k];
+    double x[7], H[36];
+    mloam::poseToParam(pose_local, x);
+    for (int i = 0; i < 6; i++)
+      for (int j = 0; j < 6; j++) H[i * 6 + j] = mat_H(i, j);
+    mloam::check(ctx, mloam_full_hessian(ctx, kdtree_from_map->slot(), feature_type, pts.data(), n, cov6.data(), x, H, &feat_num), "mloam_full_hessian");
+    for (int i = 0; i < 6; i++)
+      for (int j = 0; j < 6; j++) mat_H(i, j) = H[i * 6 + j];
   }
 };
 

@@ -415,7 +415,8 @@ class ActiveFeatureSelection {
                            const char feature_type, const std::string &gf_method, const double gf_ratio, double sub_mat_H[36],
                            const float *cov_vec6 = nullptr) {
     mloam_ctx_t *ctx = mloam::ThreadContext::get();
-    const int method = gf_method == "wo_gf" ? 0 : gf_method == "rnd" ? 1 : gf_method == "fps" ? 2 : 3;  // gd_fix / gd_float
+    // gd_fix / gd_float are one selection; gd_float's ratio policy (lidar_mapper_keyframe.cpp:456-495) is mloam_set_gf_float
+    const int method = gf_method == "wo_gf" ? 0 : gf_method == "rnd" ? 1 : gf_method == "fps" ? 2 : 3;
     std::vector<mloam_point_t> pts = mloam::pack(laser_cloud);
     std::vector<int> sel(pts.size() + 1);
     int n_sel = 0;
@@ -424,6 +425,15 @@ class ActiveFeatureSelection {
     mloam::check(ctx, mloam_good_features(ctx, map_slot, feature_type, pts.data(), (int)pts.size(), cov_vec6, x, method, gf_ratio, seed++,
                                           sel.data(), &n_sel, sub_mat_H, nullptr, nullptr), "mloam_good_features");
     sel_feature_idx.assign(sel.begin(), sel.begin() + n_sel);
+  }
+  // ActiveFeatureSelection::evalFullHessian (lidar_mapper.h:176-227): mat_H (row-major 6x6) and feat_num accumulate, as in the reference
+  void evalFullHessian(int map_slot, const common::PointICloud &laser_cloud, const Pose &pose_local, const char feature_type, double mat_H[36],
+                       int &feat_num, const float *cov_vec6 = nullptr) {
+    mloam_ctx_t *ctx = mloam::ThreadContext::get();
+    std::vector<mloam_point_t> pts = mloam::pack(laser_cloud);
+    double x[7];
+    pose_local.toParam(x);
+    mloam::check(ctx, mloam_full_hessian(ctx, map_slot, feature_type, pts.data(), (int)pts.size(), cov_vec6, x, mat_H, &feat_num), "mloam_full_hessian");
   }
 };
 
