@@ -344,6 +344,41 @@ int mloam_set_outlier(mloam_ctx_t *ctx, float map_outlier_res);
 int mloam_frame_outlier(mloam_ctx_t *ctx, mloam_point_t *h_pts, float *h_cov6, int cap, int *n);
 int mloam_keyframe_outlier(mloam_ctx_t *ctx, int id, mloam_point_t *h_pts, float *h_cov6, int cap, int *n);
 
+/* ---- the registered clouds of a frame: pubPointCloud (lidar_mapper_keyframe.cpp:690-714), what the mapper publishes every frame after the
+ *      pose, moved into the world frame with pose_wmap_curr.  Off by default.
+ * mloam_set_registered: on = 1 turns it on, 0 off.  MLOAM_E_STATE on a context with a communicator (single-GPU, like with_ua).  Off, a
+ *   frame runs exactly as before: no launch, no copy, the same captured graphs.  On, every mloam_frame* call runs ONE more launch, after
+ *   the solve, and its extraction copies the ring-ordered sweep device to device into the sweep's own half of the feature double buffer
+ *   (the sweep's buffers may be reused before its frame ends: the look-ahead's staging, the projection's output, the caller's memory).
+ *   Poses, statistics, mloam_frame_scan, the outlier cloud and the keyframe store do not change.
+ * The clouds (which):
+ *   MLOAM_REGISTERED_FULL_RES  laser_cloud_full_res += laser_cloud_outlier (:693-699).  Per LiDAR l in order its part of the ring-ordered
+ *     sweep extractCloud received (feature_extract.cpp:281): of an mloam_frame* concatenation [scan_start[l R] - 5, scan_start[(l + 1) R] - 5),
+ *     the last part ending at n (R = rings per LiDAR; LiDAR 0's part starts at point 0); of mloam_frame_raw* the projected sweep.  Every
+ *     point, finite or not (the merged cloud is dense for PCL, estimator.cpp:255): with mloam_set_distortion on, TransformToEnd(p,
+ *     pose_undist[l], true, SCAN_PERIOD) with the poses of mloam_frame_undistort for this call (estimator.cpp:405); then to the base frame
+ *     as the frame moves its less-* features — the rig merge (mloam_set_lidars): the float 3x4 matrix of ext7[l], intensity = l
+ *     (transformCloudFeature, visualization.cpp:40-52); one LiDAR with mloam_set_extrinsic: pointAssociateToMap with it, intensity kept;
+ *     otherwise unchanged.  Then, ONLY with the outlier cloud on (mloam_set_outlier, which is how this library represents segment_cloud: 0's
+ *     laser_cloud_outlier), the outlier stage's input appended: per LiDAR whose part is not empty its first point, moved with the float
+ *     matrix of its extrinsic, intensity = l, not undistorted.  With it off the frame has no outlier cloud and nothing is appended.
+ *   MLOAM_REGISTERED_SURF      laser_cloud_surf_last (:701-706): the frame's surf_points_less_flat after the undistortion and the merge
+ *     (or the single extrinsic), before downsampleCurrentScan's filter and the with_ua gate.
+ *   MLOAM_REGISTERED_CORNER    laser_cloud_corner_last (:708-713): the same for corner_points_less_sharp.
+ *   Then every point: pointAssociateToMap(., pose_wmap_curr) (utility.h:103-117; q p + t in double, float stores, intensity kept) with the
+ *   pose the call returned in pose_out7: the solved pose, or the initial pose when the map gate rejected the frame (:429, :634-638).
+ * mloam_frame_registered: cloud `which` of the last mloam_frame* call into h_pts (nullable; capacity cap points); *n = its size, also when
+ *   cap is too small (MLOAM_E_INVALID).  MLOAM_E_INVALID for another `which`; MLOAM_E_STATE before any frame, when the last frame ran with
+ *   the feature off or failed, after an mloam_scan2map* call (a scan has no sweep), and on a context with a communicator.
+ * mloam_frame_registered_device: the same cloud in place, *d_pts in context memory, valid until the next mloam_frame* call; it spares
+ *   consumers on the GPU the PCIe copy (4 x 64 x 2048 points, about 8.4 MB a frame).  Both synchronise the context stream. */
+#define MLOAM_REGISTERED_FULL_RES 0
+#define MLOAM_REGISTERED_SURF 1
+#define MLOAM_REGISTERED_CORNER 2
+int mloam_set_registered(mloam_ctx_t *ctx, int on);
+int mloam_frame_registered(mloam_ctx_t *ctx, int which, mloam_point_t *h_pts, int cap, int *n);
+int mloam_frame_registered_device(mloam_ctx_t *ctx, int which, const mloam_point_t **d_pts, int *n);
+
 /* ---- DISTORTION: motion compensation of each sweep's features before the mapper sees them (Estimator::process, estimator.cpp:545-590
  *      -> undistortMeasurements :376-408 -> TransformToEnd, utility.h:54-100).  Off by default.
  * mloam_undistort_poses (host only, no context): pose_undist of a sweep from the odometry's relative pose pose_rlt7 of LiDAR idx_ref:

@@ -21,6 +21,7 @@ LIB_PATH = os.environ.get("MLOAM_LIB", os.path.join(HERE, "libmloam_b200.so"))
 
 MAP_CORNER, MAP_SURF, MAP_SCAN_CORNER, MAP_SCAN_SURF = 0, 1, 2, 3
 GLOBAL_MAP_SURROUND, GLOBAL_MAP_SAVE = 0, 1  # mloam_global_map modes: pubGlobalMap, saveGlobalMap
+REGISTERED_FULL_RES, REGISTERED_SURF, REGISTERED_CORNER = 0, 1, 2  # mloam_frame_registered clouds (pubPointCloud)
 E_NO_DEVICE = -2
 
 # every entry point include/mloam_b200.h declares
@@ -38,6 +39,7 @@ ABI_SYMBOLS = [
     "mloam_frame_set_next_raw_device", "mloam_set_outlier", "mloam_frame_outlier", "mloam_keyframe_outlier",
     "mloam_undistort_poses", "mloam_set_distortion", "mloam_frame_undistort",
     "mloam_full_hessian", "mloam_set_gf_float", "mloam_set_gf_float_threshold", "mloam_gf_float_report",
+    "mloam_set_registered", "mloam_frame_registered", "mloam_frame_registered_device",
 ]
 
 
@@ -161,6 +163,7 @@ class Context:
 
     def __init__(self, device: int = 0, params: Params | None = None):
         self._h = C.c_void_p()
+        self.device = device
         self.params = params if params is not None else default_params()
         rc = lib().mloam_ctx_create(device, C.byref(self.params), C.byref(self._h))
         if rc != 0:
@@ -665,6 +668,33 @@ class Context:
     def keyframe_outlier(self, kf_id: int):
         """Keyframe kf_id's stored outlier cloud: (points [n,4], cov6 [n,6])."""
         return self._outlier(lib().mloam_keyframe_outlier, C.c_int(int(kf_id)))
+
+    def set_registered(self, on: bool):
+        """pubPointCloud's clouds (mloam_set_registered): every frame call also moves the full-resolution sweep (with the outlier points when
+        set_outlier is on), surf_last and corner_last into the map frame with the returned pose."""
+        self._ck(lib().mloam_set_registered(self._h, int(bool(on))))
+
+    def frame_registered(self, which: int) -> np.ndarray:
+        """Registered cloud `which` (REGISTERED_FULL_RES / _SURF / _CORNER) of the last frame call: [n, 4] float32, intensity as documented."""
+        n = C.c_int(0)
+        self._ck(lib().mloam_frame_registered(self._h, int(which), None, 0, C.byref(n)))
+        p = np.zeros((max(n.value, 1), 4), np.float32)
+        self._ck(lib().mloam_frame_registered(self._h, int(which), _p(p), p.shape[0], C.byref(n)))
+        return p[:n.value].copy()
+
+    def frame_registered_device(self, which: int):
+        """The same cloud as a CUDA tensor [n, 4] float32: a device-to-device copy of the context's buffer, which the next frame call reuses."""
+        import torch
+
+        ptr, n = C.c_void_p(), C.c_int(0)
+        self._ck(lib().mloam_frame_registered_device(self._h, int(which), C.byref(ptr), C.byref(n)))
+        if n.value == 0:
+            return torch.zeros((0, 4), dtype=torch.float32, device=f"cuda:{self.device}")
+
+        class _View:  # the context's buffer as a CUDA array, viewed without a copy
+            __cuda_array_interface__ = {"shape": (n.value, 4), "typestr": "<f4", "data": (ptr.value, False), "version": 3, "strides": None}
+
+        return torch.as_tensor(_View(), device=f"cuda:{self.device}").clone()
 
     # ---- keyframe store (saveKeyframe / extractSurroundingKeyFrames on the device)
     def keyframes_init(self, distance_keyframes: float, orientation_keyframes_deg: float, surrounding_kf_radius: float, map_sur_kf_res: float,

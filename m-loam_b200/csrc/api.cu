@@ -152,7 +152,7 @@ void mloam_ctx_destroy(mloam_ctx_t *h) {
                     &c->host_work, &c->odom_work, &c->ctl, &c->front_work, &c->front_out})
     b->release();
   c->frame_main.release(), c->frame_alt.release(), c->next_in.release(), c->stamps.release(), c->ua_scan.release(), c->pose_cov.release();
-  c->outlier.release(), c->undist.release(), c->gf_float.release();
+  c->outlier.release(), c->undist.release(), c->gf_float.release(), c->registered.release();
   if (c->pinned) cudaFreeHost(c->pinned);
   if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
   for (Branch *b : {&c->br_maps, &c->br_scan, &c->br_ahead, &c->br_ahead_scan}) {

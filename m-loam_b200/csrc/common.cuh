@@ -87,6 +87,16 @@ __host__ __device__ inline float3 associate(const PoseD &T, float px, float py, 
   D3 v = qrot(T.q, D3{(double)px, (double)py, (double)pz}) + T.t;
   return make_float3((float)v.x, (float)v.y, (float)v.z);
 }
+// pcl::transformPointCloud with a float 3x4 matrix m = Pose(q, t).T_.cast<float>() (PCL 1.8 transforms.hpp): x' = m00 x + m01 y + m02 z + m03,
+// float, left to right; the intensity is the caller's (the rig merge and pubPointCloud set the laser id, the local map keeps it)
+__device__ inline float4 rig_transform(const float *m, const float4 p, float intensity) {
+  float4 o;
+  o.x = m[0] * p.x + m[1] * p.y + m[2] * p.z + m[3];
+  o.y = m[4] * p.x + m[5] * p.y + m[6] * p.z + m[7];
+  o.z = m[8] * p.x + m[9] * p.y + m[10] * p.z + m[11];
+  o.w = intensity;
+  return o;
+}
 
 // PoseLocalParameterization::Plus (pose_local_parameterization.cpp:26-46)
 __host__ __device__ inline void pose_plus(const double *x, const double *delta, const double *V, double *out) {

@@ -184,6 +184,14 @@ struct UndistStage {
   ud::UndistPose pose[MLOAM_MAX_LIDARS];   // per LiDAR the pose TransformToEnd moves its features with
 };
 
+// Ctx::registered carved for one frame (registered.cu registered_layout): the clouds [MLOAM_REGISTERED_FULL_RES | _SURF | _CORNER] with
+// their capacities and the kernel's device counts
+struct RegOut {
+  float4 *cloud[3];
+  int *counts;
+  int cap[3];
+};
+
 // gd_float (mloam_set_gf_float; gf_kernels.cu k_gf_full_hessian): what the mapper carries from frame to frame, on the device.
 // k_gf_select reads ratio_cur there, so the host never sees the ratio on a frame's path.
 struct GfFloatState {
@@ -402,6 +410,7 @@ struct Ctx {
     ScanRef S{};
     bool extract_only = false;  // the undistortion was on: the half holds the extraction only (undistortion, merge and the scan
                                 // filters run at the frame call, which knows the sweep's pose)
+    bool registered = false;    // the registered clouds were on: the half also holds the sweep itself (FrameBufs::reg_sweep)
   };
   struct NextSweep {
     bool set = false;
@@ -427,6 +436,7 @@ struct Ctx {
     int launches = 0, seen = 0, s2m_ran = 0;
     ScanRef S{};
     Features prefetched_out{};     // what the frame leaves in Ctx::prefetched
+    RegOut reg{};                  // where its registered clouds go (Ctx::reg_last)
   };
   std::vector<GraphEntry> graphs;
   bool smem_opt_in_gf = false;     // k_gf_select's 200 KB pool
@@ -514,6 +524,13 @@ struct Ctx {
   bool gf_float_reported = false;  // a solve call has run since the mode was turned on
   DevBuf gf_float;                 // GfFloatDev
   GfFloatState gf_float_host{};    // the state as the last solve call left it (mloam_gf_float_report)
+  // pubPointCloud (mloam_set_registered; registered.cu): the full-resolution sweep with its outlier points, surf_last and corner_last in
+  // the map frame, written by one launch at the end of every mloam_frame* call.  The extraction keeps the ring-ordered sweep in the
+  // sweep's half of the feature double buffer, because the sweep's own buffers are reused before the frame that registers it ends.
+  bool reg_on = false;
+  bool reg_valid = false;          // Ctx::registered holds the clouds of the last mloam_frame* call
+  DevBuf registered;               // the three clouds and their device counts (registered_layout)
+  RegOut reg_last{};               // where the last frame's clouds are
   double pose_cov36[36] = {0};     // pose_wmap_curr.cov_ of the last mloam_frame* / mloam_scan2map* call
   bool last_scan_valid = false;    // last_scan describes the scan of the last mloam_frame* call (mloam_frame_scan)
   ScanRef last_scan{};
@@ -635,6 +652,30 @@ void ua_stage_host(Ctx *c);
 // fields.  One single-CTA launch.  stage_outlier writes the staged configuration (PinnedBlock::outlier).
 int outlier_stage(Ctx *c, Ctx::ScanRef *S, const UaStage *d_ua);
 void stage_outlier(Ctx *c);
+// registered.cu: pubPointCloud (lidar_mapper_keyframe.cpp:690-714) of a frame, one launch on c->stream after the solve.  Per point of the
+// three clouds: [TransformToEnd] -> [the float rig matrix, intensity = laser id | pointAssociateToMap with the single extrinsic] for the sweep
+// (the less-* features and the outlier points arrive in the base frame already) -> pointAssociateToMap with *pose.
+struct RegArgs {
+  const float4 *sweep;              // the ring-ordered sweep in the sensor frame(s), LiDAR-major
+  int n_sweep;                      // its size, or the bound when d_n_sweep is set
+  const int *d_n_sweep;             // nullable: its size on the device (the projection count of a raw sweep)
+  const int *scan_start;            // its ScanInfo starts: LiDAR l's part begins at scan_start[l * rings_per_lidar] - 5
+  int rings_per_lidar, n_parts;     // n_parts LiDARs (1 without the rig merge)
+  int to_base;                      // 0 none, 1 the rig's float matrices (rig, intensity = l), 2 pointAssociateToMap with ext
+  const float *rig;                 // DevCtl::rig
+  const double *ext;                // DevCtl::ext
+  const UndistStage *undist;        // nullable: the frame's staged undistortion
+  const float4 *first;              // nullable: the outlier cloud's input, the LiDARs' first points (ExtractOut::first) ...
+  const int *first_ok;              // ... and their flags
+  const OutlierStage *outlier;      // ... and their float matrices
+  const float4 *less_flat, *less_sharp;  // in the base frame, after the undistortion and the merge; before the scan filters
+  int cap_flat, cap_sharp;
+  const int *n_flat, *n_sharp;      // device counts (ExtractOut::counts + 3, + 1)
+  const double *pose;               // pose_wmap_curr on the device: LMState::x, or the staged initial pose of a map-gated frame
+};
+// Ctx::registered for a frame of n_sweep sweep points and the given feature capacities
+int registered_layout(Ctx *c, int n_sweep, int cap_flat, int cap_sharp, RegOut *out);
+int registered_stage(Ctx *c, const RegArgs &a, const RegOut &out);
 // pipeline.cu: writers of the pinned fields a captured frame graph reads (PinnedBlock), shared by the enqueue and the replay paths
 void stage_pose(Ctx *c, const double *pose7);
 void stage_ext(Ctx *c);

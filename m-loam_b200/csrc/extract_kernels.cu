@@ -1186,15 +1186,8 @@ __global__ void k_merge_transform(float4 *__restrict__ pts, const int *__restric
   if (i >= off[n_lidars]) return;
   int l = 0;
   while (l + 1 < n_lidars && i >= off[l + 1]) l++;
-  const float *m = ext12 + 12 * l;
   const float4 p = pts[i];
-  // pcl::transformPointCloud (PCL 1.8 transforms.hpp): x' = m00 x + m01 y + m02 z + m03, float, left to right
-  float4 o;
-  o.x = m[0] * p.x + m[1] * p.y + m[2] * p.z + m[3];
-  o.y = m[4] * p.x + m[5] * p.y + m[6] * p.z + m[7];
-  o.z = m[8] * p.x + m[9] * p.y + m[10] * p.z + m[11];
-  o.w = set_id ? (float)l : p.w;  // p.intensity = n (rig merge) / kept (local map, estimator.cpp:1185-1186)
-  pts[i] = o;
+  pts[i] = rig_transform(ext12 + 12 * l, p, set_id ? (float)l : p.w);  // p.intensity = n (rig merge) / kept (local map, estimator.cpp:1185-1186)
 }
 
 int lidar_offsets_device(Ctx *c, int n_lidars, int rings_per_lidar, int *d_off) {

@@ -255,6 +255,7 @@ int gf_float_begin(Ctx *c) {
 
 int scan2map_run(Ctx *c, const ScanRef &S, const double *pose_init7, bool want_cov, double *pose_out7, mloam_solve_stats_t *stats) {
   int ran = 0;
+  c->reg_valid = false;  // a scan has no sweep: nothing to register
   int rc = gf_float_begin(c);
   if (rc) return rc;
   rc = scan2map_enqueue(c, S, pose_init7, want_cov, &ran);
@@ -270,8 +271,14 @@ struct FrameBufs {
   float4 *first;                 // the LiDARs' first points (ExtractOut::first) and their flags
   int *first_ok;
   int *off;                      // rig merge: per-LiDAR offsets of the less-sharp and less-flat features (lidar_offsets_device)
+  // the registered clouds (reg_scans > 0): the ring-ordered sweep the features were extracted from, and [0] its size on the device (a
+  // raw sweep's projection count), [16 ..] its ScanInfo starts
+  float4 *reg_sweep = nullptr;
+  int *reg_meta = nullptr;
 };
-int frame_bufs(Ctx *c, int n, FrameBufs *F, int parity = 0) {
+// reg_scans: the sweep's ring count when the half also keeps the sweep for the registered clouds; its regions come last, so the other
+// regions lie where they lie without them
+int frame_bufs(Ctx *c, int n, FrameBufs *F, int parity = 0, int reg_scans = 0) {
   const size_t N1 = (size_t)n + 16;
   MLOAM_CUDA_OK(c, carve(parity ? c->frame_alt : c->frame_main, [&](Carve &cv) {
     F->ex.sharp = cv.take<float4>(N1), F->ex.less_sharp = cv.take<float4>(N1), F->ex.flat = cv.take<float4>(N1);
@@ -279,6 +286,7 @@ int frame_bufs(Ctx *c, int n, FrameBufs *F, int parity = 0) {
     F->ex.counts = cv.take<int>(16);  // [0..3]
     F->first = cv.take<float4>(MLOAM_MAX_LIDARS), F->first_ok = cv.take<int>(MLOAM_MAX_LIDARS);
     F->off = cv.take<int>(2 * (MLOAM_MAX_LIDARS + 1));
+    if (reg_scans > 0) F->reg_sweep = cv.take<float4>(N1), F->reg_meta = cv.take<int>(16 + (size_t)reg_scans);
   }));
   F->n_corner_ds = F->ex.counts + 4, F->n_surf_ds = F->ex.counts + 5;
   return MLOAM_OK;
@@ -318,6 +326,9 @@ namespace {
 
 bool rig_merge(const Ctx *c) { return c->n_lidars > 1 || c->lidar_merge; }
 
+// capacity of a frame's less-sharp features: <= 20 picks x 6 sectors per ring
+int less_sharp_cap(int n, int n_scans) { return n < 120 * n_scans ? n : 120 * n_scans; }
+
 void stage_frame_inputs(Ctx *c, const double *pose7) {
   stage_pose(c, pose7);
   if (rig_merge(c)) stage_rig(c);
@@ -334,7 +345,7 @@ bool frame_has_prefetched(const Ctx *c, const Sweep &sw) {
   const Ctx::Features &f = c->prefetched;
   const bool same_kind = sw.raw ? (f.sw.raw && std::memcmp(&f.sw.L, &sw.L, sizeof(RigLayout)) == 0) : !f.sw.raw;
   return f.valid && c->use_lookahead && !c->prof_on && f.sw.key == sw.key && f.sw.n == sw.n && f.sw.n_scans == sw.n_scans && same_kind &&
-         (f.sw.host || !sw.host) && f.extract_only == c->undist_on;
+         (f.sw.host || !sw.host) && f.extract_only == c->undist_on && (f.registered || !c->reg_on);
 }
 
 // extractCloud of sweep sw on c->stream into half `parity` of the feature double buffer (*F), with the LiDARs' first points and, for the
@@ -344,7 +355,7 @@ bool frame_has_prefetched(const Ctx *c, const Sweep &sw) {
 int extract_enqueue(Ctx *c, const Sweep &sw, int parity, FrameBufs *F_out) {
   const int n = sw.n, n_scans = sw.n_scans;
   FrameBufs F;
-  int rc = frame_bufs(c, n, &F, parity);
+  int rc = frame_bufs(c, n, &F, parity, c->reg_on ? n_scans : 0);
   if (rc) return rc;
   const float4 *d_cloud = sw.cloud;
   const int *d_scan_start = sw.scan_start, *d_scan_end = sw.scan_end;
@@ -360,6 +371,11 @@ int extract_enqueue(Ctx *c, const Sweep &sw, int parity, FrameBufs *F_out) {
     if (rc) return rc;
     stamp(c, "front end");
     d_cloud = proj, d_scan_start = ss, d_scan_end = ss + n_scans;
+    if (c->reg_on) MLOAM_CUDA_OK(c, cudaMemcpyAsync(F.reg_meta, n_proj, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
+  }
+  if (c->reg_on) {  // the registered clouds need the sweep when its frame ends: by then next_in, front_out or the caller's buffer may be reused
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(F.reg_sweep, d_cloud, sizeof(float4) * (size_t)n, cudaMemcpyDeviceToDevice, c->stream));
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(F.reg_meta + 16, d_scan_start, sizeof(int) * (size_t)n_scans, cudaMemcpyDeviceToDevice, c->stream));
   }
   // every frame's extraction records each LiDAR's first point, so that features extracted ahead serve a frame with the outlier cloud on
   const int n_parts = rig_merge(c) ? c->n_lidars : 1;
@@ -383,7 +399,7 @@ int scan_enqueue(Ctx *c, const Sweep &sw, const FrameBufs &F, const Branch &side
   const mloam_params_t &P = c->params;
   const int n = sw.n, n_scans = sw.n_scans;
   int rc;
-  const int less_cap = n < 120 * n_scans ? n : 120 * n_scans;  // <= 20 less-sharp picks x 6 sectors per ring
+  const int less_cap = less_sharp_cap(n, n_scans);
   DevCtl *ctl = c->ctl.as<DevCtl>();
   if (c->undist_on) {  // undistortMeasurements (estimator.cpp:376-408): each LiDAR's less-* features in its own frame, before the merge
     rc = undistort_stage(c, F.ex, less_cap, n, rig_merge(c) ? F.off : nullptr, rig_merge(c) ? c->n_lidars : 1);
@@ -452,6 +468,40 @@ void frame_advance(Ctx *c, int parity, const Ctx::Features &nf) {
   c->prefetched = nf;
 }
 
+// pubPointCloud of sweep sw, whose features and copy are in half `parity`, on c->stream after the solve: k_registered at pose_wmap_curr,
+// LMState::x when the solve ran (ran), else the initial pose (the map gate keeps it, lidar_mapper_keyframe.cpp:429, :634-638)
+int registered_enqueue(Ctx *c, const Sweep &sw, int parity, int ran, const double *pose_init7) {
+  FrameBufs F;
+  int rc = frame_bufs(c, sw.n, &F, parity, sw.n_scans);  // the layout the extraction carved: nothing moves or grows
+  if (rc) return rc;
+  DevCtl *ctl = c->ctl.as<DevCtl>();
+  const double *d_pose;
+  if (ran) {
+    d_pose = c->lm_state.as<LMState>()->x;
+  } else {
+    stage_pose(c, pose_init7);
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(ctl->pose, c->pinned->pose, 7 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    d_pose = ctl->pose;
+  }
+  const bool merge = rig_merge(c);
+  const int less_cap = less_sharp_cap(sw.n, sw.n_scans);
+  RegArgs a{};
+  a.sweep = F.reg_sweep, a.n_sweep = sw.n, a.d_n_sweep = sw.raw ? F.reg_meta : nullptr, a.scan_start = F.reg_meta + 16;
+  a.n_parts = merge ? c->n_lidars : 1, a.rings_per_lidar = sw.n_scans / a.n_parts;
+  a.to_base = merge ? 1 : (c->has_ext ? 2 : 0), a.rig = &ctl->rig[0][0], a.ext = ctl->ext;  // as scan_enqueue staged them
+  a.undist = c->undist_on ? c->undist.as<UndistStage>() : nullptr;                          // undistort_stage's configuration
+  if (c->outlier_on) a.first = F.first, a.first_ok = F.first_ok, a.outlier = c->outlier.as<OutlierStage>();  // outlier_stage's
+  a.less_flat = F.ex.less_flat, a.less_sharp = F.ex.less_sharp, a.cap_flat = sw.n, a.cap_sharp = less_cap;
+  a.n_flat = F.ex.counts + 3, a.n_sharp = F.ex.counts + 1, a.pose = d_pose;
+  RegOut o;
+  rc = registered_layout(c, sw.n, sw.n, less_cap, &o);
+  if (rc == MLOAM_OK) rc = registered_stage(c, a, o);
+  if (rc) return rc;
+  c->reg_last = o;
+  stamp(c, "registered");
+  return MLOAM_OK;
+}
+
 // The features of sw — ready from the look-ahead when `have`, else extracted now into half `parity` — the look-ahead of the announced
 // sweep, the map builds (rebuild_maps) and the solve on c->stream.  *ran: scan2map_enqueue's.
 int frame_enqueue(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_surf_map, int n_surf_map, const float4 *d_corner_map,
@@ -480,7 +530,7 @@ int frame_enqueue(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *
     if (rc) return rc;
   } else if (c->prefetched.extract_only) {  // undistortion on: the look-ahead extracted; this sweep's pose is known now
     FrameBufs F;
-    rc = frame_bufs(c, sw.n, &F, parity);
+    rc = frame_bufs(c, sw.n, &F, parity, c->reg_on ? sw.n_scans : 0);
     F.ex.first = F.first, F.ex.first_ok = F.first_ok;  // recorded by the look-ahead's extraction (extract_enqueue)
     if (rc == MLOAM_OK) rc = scan_enqueue(c, sw, F, c->br_scan, &S);
     if (rc) return rc;
@@ -505,7 +555,7 @@ int frame_enqueue(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *
     });
     c->stamp_mute = false;
     if (rc) return rc;
-    nf.valid = true, nf.parity = parity ^ 1, nf.sw = nx, nf.extract_only = c->undist_on;
+    nf.valid = true, nf.parity = parity ^ 1, nf.sw = nx, nf.extract_only = c->undist_on, nf.registered = c->reg_on;
   }
   stamp(c, have ? "features (prefetched)" : "extract + voxel");
   const UaStage *d_ua = nullptr;
@@ -526,6 +576,10 @@ int frame_enqueue(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *
   *S_out = S;
   rc = scan2map_enqueue(c, S, pose_init7, c->with_ua != 0, ran);
   if (rc) return rc;
+  if (c->reg_on) {  // pubPointCloud (:690-714): after the solve, next to the look-ahead's tail
+    rc = registered_enqueue(c, sw, parity, *ran, pose_init7);
+    if (rc) return rc;
+  }
   if (nf.valid) {  // the frame ends when both branches have: the features of the next sweep are complete when this call returns
     MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream, c->br_ahead.join, 0));
     stamp(c, "look-ahead join");
@@ -597,6 +651,8 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
     return fail(c, MLOAM_E_STATE, "frame: the outlier cloud (mloam_set_outlier) is single-GPU only; detach the communicator or set it to 0");
   if (c->undist_on && c->nccl_comm)
     return fail(c, MLOAM_E_STATE, "frame: the undistortion (mloam_set_distortion) is single-GPU only; detach the communicator or turn it off");
+  if (c->reg_on && c->nccl_comm)
+    return fail(c, MLOAM_E_STATE, "frame: the registered clouds (mloam_set_registered) are single-GPU only; detach the communicator or turn them off");
   const bool want_cov = c->with_ua != 0;
   c->last_scan_valid = false;
   c->frame_from_graph = false;
@@ -630,6 +686,10 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
     if (c->undist_on) {  // the undistortion's launch and the look-ahead's split (poses and scan period are staged)
       const int on[2] = {'u', c->undist_n};
       key = fnv1a(key, on, sizeof(on));
+    }
+    if (c->reg_on) {  // pubPointCloud's launch and the sweep copies of the extraction; a context that never turns it on keeps its keys
+      const int on = 'r';
+      key = fnv1a(key, &on, sizeof(on));
     }
     if (c->gf_float_on) {  // gd_float: the ratio's device read, and an evaluation frame's extra launch (threshold, gf_ratio_ini and the
       const int on[2] = {'g', c->gf_float_eval ? 1 : 0};  // ratio itself are not in the key: they are staged or stay on the device)
@@ -668,6 +728,7 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
       c->gf_float_evaluated = c->gf_float_on && c->gf_float_eval && e->s2m_ran;
       frame_advance(c, parity, e->prefetched_out);
       c->last_scan = e->S, c->last_scan_valid = true;
+      c->reg_last = e->reg;
       return scan2map_finish(c, e->S, pose_init7, want_cov, e->s2m_ran, pose_out7, stats);
     }
     if (e && e->seen >= 1) {  // second sighting: capture
@@ -684,7 +745,7 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
       if (rc == MLOAM_OK && ce == cudaSuccess && graph && ep0 == alloc_epoch() &&
           cudaGraphInstantiate(&e->exec, graph, 0) == cudaSuccess) {
         e->launches = (int)(c->launches - l0), e->epoch = ep0, e->S = S, e->s2m_ran = ran;
-        e->prefetched_out = c->prefetched;
+        e->prefetched_out = c->prefetched, e->reg = c->reg_last;
         c->launches = l0;
         c->graph_captures++;
         c->graph_pdl_edges = count_programmatic_edges(graph);
@@ -774,6 +835,7 @@ int upload_submaps(Ctx *c, const mloam_point_t *h_surf_map, int n_surf_map, cons
 // consumes the announcement and the uploads.
 int frame_call(Ctx *c, Sweep sw, const mloam_point_t *surf_map, int n_surf_map, const mloam_point_t *corner_map, int n_corner_map,
                int rebuild_maps, const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
+  c->reg_valid = false;
   if (sw.host && rebuild_maps && (!surf_map || !corner_map || n_surf_map < 0 || n_corner_map < 0)) return MLOAM_E_INVALID;
   if (c->undist_on) {  // the sweep's pose_undist (mloam_frame_undistort), consumed by this call whatever it returns
     const bool set = c->undist_set;
@@ -794,6 +856,7 @@ int frame_call(Ctx *c, Sweep sw, const mloam_point_t *surf_map, int n_surf_map, 
   if (rc == MLOAM_OK) rc = frame_run(c, sw, have, parity, d_sm, n_surf_map, d_cm, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
   c->maps_pending = false, c->next_pending = false, c->next.set = false;
   if (rc == MLOAM_OK) memcpy(c->last_pose7, pose_out7, sizeof(c->last_pose7)), c->frame_since_save = true;  // mloam_keyframe_save
+  c->reg_valid = rc == MLOAM_OK && c->reg_on;  // mloam_frame_registered
   return rc;
 }
 

@@ -382,15 +382,7 @@ __global__ void __launch_bounds__(32) k_outlier_scan(const float4 *__restrict__ 
     int n = 0;
     for (int l = 0; l < L; l++) {
       if (!first_ok[l]) continue;  // an empty part pushes no point (laser_cloud_out.points[0] of an empty cloud is not read)
-      const float4 p = first[l];
-      const float *m = cfg->mat[l];
-      // pcl::transformPointCloud (PCL 1.8 transforms.hpp): x' = m00 x + m01 y + m02 z + m03, float, left to right; intensity = n
-      float4 o;
-      o.x = m[0] * p.x + m[1] * p.y + m[2] * p.z + m[3];
-      o.y = m[4] * p.x + m[5] * p.y + m[6] * p.z + m[7];
-      o.z = m[8] * p.x + m[9] * p.y + m[10] * p.z + m[11];
-      o.w = (float)l;
-      raw[n++] = o;
+      raw[n++] = rig_transform(cfg->mat[l], first[l], (float)l);  // pcl::transformPointCloud, intensity = n
     }
     n_ds = voxel_few(raw, n, 1.0f / cfg->leaf, ds);
   }

@@ -483,3 +483,23 @@ inline void undistortMeasurements(mloam_ctx_t *ctx, const std::vector<Pose> &pos
   check(ctx, mloam_frame_undistort(ctx, (int)pose_undist.size(), x.data()), "mloam_frame_undistort");
 }
 }  // namespace mloam
+
+// ---- pubPointCloud (lidar_mapper_keyframe.cpp:690-714): the registered clouds of the last mloam_frame* call of ctx, in the world frame
+//   mloam::setRegistered(ctx, true);                                                           once
+//   mloam::frameRegistered(ctx, laser_cloud_full_res, laser_cloud_surf_last, laser_cloud_corner_last);    after each mloam_frame*
+// in place of the three pointAssociateToMap loops; toROSMsg and publish stay the caller's.
+namespace mloam {
+inline void setRegistered(mloam_ctx_t *ctx, bool on) { check(ctx, mloam_set_registered(ctx, on ? 1 : 0), "mloam_set_registered"); }
+inline void frameRegistered(mloam_ctx_t *ctx, int which, common::PointICloud &out) {
+  int n = 0;
+  check(ctx, mloam_frame_registered(ctx, which, nullptr, 0, &n), "mloam_frame_registered");
+  std::vector<mloam_point_t> pts((size_t)n);
+  check(ctx, mloam_frame_registered(ctx, which, pts.data(), n, &n), "mloam_frame_registered");
+  unpackCloud(pts.data(), n, out);
+}
+inline void frameRegistered(mloam_ctx_t *ctx, common::PointICloud &full_res, common::PointICloud &surf_last, common::PointICloud &corner_last) {
+  frameRegistered(ctx, MLOAM_REGISTERED_FULL_RES, full_res);
+  frameRegistered(ctx, MLOAM_REGISTERED_SURF, surf_last);
+  frameRegistered(ctx, MLOAM_REGISTERED_CORNER, corner_last);
+}
+}  // namespace mloam

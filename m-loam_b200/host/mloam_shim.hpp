@@ -490,3 +490,23 @@ inline void undistortMeasurements(mloam_ctx_t *ctx, const std::vector<Pose> &pos
   check(ctx, mloam_frame_undistort(ctx, (int)pose_undist.size(), x.data()), "mloam_frame_undistort");
 }
 }  // namespace mloam
+
+// ----------------------------------------------------------------------------------------------- pubPointCloud
+namespace mloam {
+// mloam_set_registered / mloam_frame_registered on ctx: laser_cloud_full_res (with the outlier points when the outlier cloud is on),
+// laser_cloud_surf_last and laser_cloud_corner_last of the last mloam_frame* call, moved into the world frame with pose_wmap_curr
+// (lidar_mapper_keyframe.cpp:690-714)
+inline void setRegistered(mloam_ctx_t *ctx, bool on) { check(ctx, mloam_set_registered(ctx, on ? 1 : 0), "mloam_set_registered"); }
+inline void frameRegistered(mloam_ctx_t *ctx, int which, common::PointICloud &out) {
+  int n = 0;
+  check(ctx, mloam_frame_registered(ctx, which, nullptr, 0, &n), "mloam_frame_registered");
+  std::vector<mloam_point_t> pts((size_t)n);
+  check(ctx, mloam_frame_registered(ctx, which, pts.data(), n, &n), "mloam_frame_registered");
+  unpack(pts.data(), n, out);
+}
+inline void frameRegistered(mloam_ctx_t *ctx, common::PointICloud &full_res, common::PointICloud &surf_last, common::PointICloud &corner_last) {
+  frameRegistered(ctx, MLOAM_REGISTERED_FULL_RES, full_res);
+  frameRegistered(ctx, MLOAM_REGISTERED_SURF, surf_last);
+  frameRegistered(ctx, MLOAM_REGISTERED_CORNER, corner_last);
+}
+}  // namespace mloam
