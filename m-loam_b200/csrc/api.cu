@@ -115,7 +115,7 @@ int mloam_ctx_create(int device, const mloam_params_t *params, mloam_ctx_t **out
   if (const char *e = getenv("MLOAM_LIN_TRACE")) c->lin_trace_on = e[0] == '1';
   if (const char *e = getenv("MLOAM_KNN_MB")) {
     const int v = atoi(e);
-    if (v >= 2 && v <= 4) c->knn_min_blocks = v;
+    if (v == 2 || v == 3) c->knn_min_blocks = v;
   }
   if (const char *e = getenv("MLOAM_KNN_TMA_MIN")) c->knn_tma_min = (unsigned)strtoul(e, nullptr, 10);
   if (const char *e = getenv("MLOAM_KNN_SCHEDULE")) c->knn_all_searches = e[0] == '0';
@@ -296,6 +296,15 @@ int mloam_debug_stamps(mloam_ctx_t *h, unsigned long long *out_ns, int cap, int 
 const char *mloam_debug_stamp_label(mloam_ctx_t *h, int i) {
   if (!h || i < 0 || i >= (int)h->c.stamp_labels.size()) return "";
   return h->c.stamp_labels[i].c_str();
+}
+
+// Diagnosis only (not part of include/mloam_b200.h): the k_match_knn instance this context launches for K = k (MLOAM_KNN_MB):
+// its resident CTAs per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor, 256 threads) and its registers per thread.
+int mloam_debug_knn_residency(mloam_ctx_t *h, int k, int *ctas_per_sm, int *regs) {
+  const Ctx *c = h ? &h->c : nullptr;
+  if (!c || !ctas_per_sm || !regs) return MLOAM_E_INVALID;
+  cudaSetDevice(c->device);
+  return knn_residency(c, k, ctas_per_sm, regs);
 }
 
 // Diagnosis only (not part of include/mloam_b200.h): per-query words of the last traced k_match_knn launch.

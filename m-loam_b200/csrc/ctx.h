@@ -462,7 +462,7 @@ struct Ctx {
   DevBuf stamps;
   int stamp_n = 0;
   std::vector<std::string> stamp_labels;
-  int knn_min_blocks = 2;          // k_match_knn variant: resident CTAs per SM it is compiled for (MLOAM_KNN_MB = 2 | 3 | 4); 2 is fastest on the H100
+  int knn_min_blocks = 3;          // k_match_knn instance: resident CTAs per SM it is compiled for (MLOAM_KNN_MB = 2 | 3, match_kernels.cu)
   // MLOAM_KNN_SCHEDULE=0: k_match_knn as before the shortened queries — every ball and blind search listed for the next launch
   // (HeavyQ) and the selection unpruned by the search bound (scan_runs).  Same results; kept to compare the two
   bool knn_all_searches = false;
@@ -589,6 +589,8 @@ struct MatchJob {
 // pdl: the kNN launch is a link of scan2map's GN chain (launch_chain)
 int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_pose7, const MatchCfg &cfg, int buf_base = 0,
                       PendingFit *defer = nullptr, const int *d_sel = nullptr, bool pdl = false);
+// the k_match_knn instance this context launches for K (non-instrumented): resident CTAs per SM by the occupancy calculator, registers
+int knn_residency(const Ctx *c, int K, int *ctas_per_sm, int *regs);
 
 // track_kernels.cu
 int match_from_scan_device(Ctx *c, int slot, int type, const float4 *d_pts, int n, const double *d_pose7, unsigned char *d_valid,

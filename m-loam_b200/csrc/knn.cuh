@@ -45,7 +45,7 @@ struct __align__(16) KnnSmem {
   float4 pts[KNN_TILE];
   unsigned long long mbar;
   unsigned phase;  // parity of the next wait (kept by lane 0, broadcast)
-  unsigned pad;
+  int slot, first;  // the caller's (k_match_knn: the warp's place in its schedule, its first listed feature)
 };
 
 // Optional per-query instrumentation of the blind search (stage profiling only).
@@ -53,6 +53,13 @@ struct KnnDbg {
   long long t_ring1, t_ball;  // SM cycles per phase
   int ring1_pts, ball_pts, ball_rows, ball_steps;
 };
+
+// %laneid read where it is used (volatile: not held in a register across a search)
+__device__ __forceinline__ unsigned lane_id() {
+  unsigned l;
+  asm volatile("mov.u32 %0, %%laneid;" : "=r"(l));
+  return l;
+}
 
 __device__ __forceinline__ unsigned long long warp_min_u64(unsigned long long v) {
   unsigned hi = (unsigned)(v >> 32);
@@ -122,9 +129,10 @@ __device__ __forceinline__ bool key_less(unsigned da, unsigned ia, unsigned db, 
 // beats min(N-th, bound) — with an empty list too, so the points of a row that lie outside the caller's ball (rows are
 // clipped at cell granularity) cost one compare and no selection round.  Entries <= bound are those of the unbounded
 // list; the callers only look beyond the bound through min(explored, d) with explored below the bound (warp_knn).
-// Out of line on purpose: it is used from several places and every launch starts with a cold instruction cache.
+// Inlined: out of line, the call ABI saved the caller's live registers around each of its call sites, which alone kept
+// k_match_knn above its 72-register budget (match_kernels.cu).
 template <int N>
-__device__ __noinline__ Best scan_runs(const float4 *__restrict__ sorted, KnnSmem *ks, int start, int count, float qx, float qy, float qz,
+__device__ __forceinline__ Best scan_runs(const float4 *__restrict__ sorted, KnnSmem *ks, int start, int count, float qx, float qy, float qz,
                                        Best best, int *n_points, unsigned bound) {
   constexpr int U = 2;  // candidates per lane and selection step
   const int lane = threadIdx.x & 31;
@@ -149,16 +157,17 @@ __device__ __noinline__ Best scan_runs(const float4 *__restrict__ sorted, KnnSme
 #pragma unroll 1
     for (int c0 = 0; c0 < chunk; c0 += 32 * U) {
       unsigned cd[U], ci[U];
-      int cp[U];
+      // candidate u's encoded position, formed where it is taken rather than held in registers through the rounds
+      auto cp = [&](int u) { return -(base + c0 + u * 32 + lane) - 2; };
 #pragma unroll
       for (int u = 0; u < U; u++) {
         const int t = c0 + u * 32 + lane;
-        cd[u] = MLOAM_D_NONE, ci[u] = 0xffffffffu, cp[u] = -1;
+        cd[u] = MLOAM_D_NONE, ci[u] = 0xffffffffu;
         if (t < chunk) {
           const float4 v = ks->pts[t];
           const float ex = v.x - qx, ey = v.y - qy, ez = v.z - qz;
           const float d2 = ex * ex + ey * ey + ez * ez;
-          cd[u] = __float_as_uint(d2), ci[u] = (unsigned)__float_as_int(v.w), cp[u] = -(base + t) - 2;
+          cd[u] = __float_as_uint(d2), ci[u] = (unsigned)__float_as_int(v.w);
         }
       }
       // how many candidates beat min(N-th, bound)?  The bound as a key is (bound, 0xffffffff): d2 == bound still enters.
@@ -185,7 +194,7 @@ __device__ __noinline__ Best scan_runs(const float4 *__restrict__ sorted, KnnSme
             const int src = __ffs(mk) - 1;
             mk &= mk - 1;
             const unsigned xd = __shfl_sync(MLOAM_FULL_MASK, cd[u], src), xi = __shfl_sync(MLOAM_FULL_MASK, ci[u], src);
-            const int xp = __shfl_sync(MLOAM_FULL_MASK, cp[u], src);
+            const int xp = -(base + c0 + u * 32 + src) - 2;
             const int slot = __popc(__ballot_sync(MLOAM_FULL_MASK, lane < N && key_less(e.d, e.i, xd, xi)));
             const unsigned ud = __shfl_up_sync(MLOAM_FULL_MASK, e.d, 1), ui = __shfl_up_sync(MLOAM_FULL_MASK, e.i, 1);
             const int up = __shfl_up_sync(MLOAM_FULL_MASK, e.p, 1);
@@ -205,7 +214,7 @@ __device__ __noinline__ Best scan_runs(const float4 *__restrict__ sorted, KnnSme
         int lp = o.p, which = U;
 #pragma unroll
         for (int u = 0; u < U; u++)
-          if (key_less(cd[u], ci[u], ld, li)) ld = cd[u], li = ci[u], lp = cp[u], which = u;
+          if (key_less(cd[u], ci[u], ld, li)) ld = cd[u], li = ci[u], lp = cp(u), which = u;
         const unsigned md = __reduce_min_sync(MLOAM_FULL_MASK, ld);
         if (md == MLOAM_D_NONE) break;  // fewer than N points so far
         unsigned owners = __ballot_sync(MLOAM_FULL_MASK, ld == md);
@@ -403,7 +412,7 @@ __device__ __forceinline__ void warp_knn(const MapView &map, const GridP &g, Knn
   {
     int start = 0, count = 0;
     if (lane < 9) {
-      const int y = cy + lane % 3 - 1, z = cz + lane / 3 - 1;
+      const int y = cy + (int)(lane_id() % 3u) - 1, z = cz + (int)(lane_id() / 3u) - 1;
       const int xl = max(cx - 1, 0), xh = min(cx + 1, g.nx - 1);
       if (y >= 0 && y < g.ny && z >= 0 && z < g.nz && xl <= xh) row_run(map, g, y, z, xl, xh, &start, &count);
     }

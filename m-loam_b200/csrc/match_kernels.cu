@@ -12,6 +12,7 @@
 //                register footprint.  The per-feature routine lives in match_fit.cuh; scan2map without good-feature
 //                selection defers it into the first evaluation of the solve (k_linearize), so that a GN iteration is
 //                two launches.
+#include <climits>
 #include <cstdlib>
 
 #include "ctx.h"
@@ -55,18 +56,36 @@ struct HeavyQ {
   int all_searches;
 };
 
-// MB: resident CTAs per SM the kernel is compiled for (register budget 65536 / (256 * MB)).  The search is a chain of
-// dependent warp-wide operations (prefix loads -> point loads -> REDUX / ballot / shuffle rounds).  MB = 3 and 4 buy more
-// resident warps with spilled registers (local-memory round trips inside that chain); on the H100 the spill-free MB = 2
-// variant (104 registers, no spills; MB = 3 still spills) runs the C2 frame about 9 % faster than MB = 4, so it is the default (Ctx::knn_min_blocks).
-// STATS: the instance for stage profiling and MLOAM_KNN_TRACE=1, with the per-path counters (path_stats: the KnnPathStats
-// of ctx.h addressed as 32-bit words; KPS_WORD(field) is a field's word index) and the per-query trace; the production
-// instance is compiled without them.  sel_prune: bound-pruned selection (scan_runs), 0 under MLOAM_KNN_SCHEDULE=0.
+// Instances.  The search is a chain of dependent warp-wide operations (prefix loads -> TMA -> REDUX / ballot / shuffle rounds),
+// so more resident warps hide more of it, but only without spills (a local-memory round trip inside that chain) and only if one
+// k_eval_candidate block (64 threads x 128 registers = 8192) still fits beside the matcher on each SM: the speculative schedule
+// runs it next to the matcher, and where it does not fit it lands on the path to the next k_linearize.
+//   k_match_knn      the default: at most KNN_LEAN_REGS registers, so three CTAs (3 x 256 x 72 = 55296 of the SM's 65536
+//                    registers) sit beside one k_eval_candidate block.  Spill-free with no stack frame: the sets, the schedule's
+//                    values and the warp's place in it are read from shared memory where they are used, scan_runs is inlined.
+//   k_match_knn_mb2  __launch_bounds__(256, 2), MLOAM_KNN_MB=2: launched with two CTAs per SM, the earlier residency, kept to
+//                    compare against;
+//                    its STATS = true instance is the one for stage profiling and MLOAM_KNN_TRACE=1, with the per-path counters
+//                    (path_stats: the KnnPathStats of ctx.h addressed as 32-bit words; KPS_WORD(field) is a field's word index) and
+//                    the per-query trace.
+// Both run the same body, so a query does the same operations in the same order in either.  sel_prune: bound-pruned selection
+// (scan_runs), 0 under MLOAM_KNN_SCHEDULE=0.
 #define KPS_WORD(field) (offsetof(KnnPathStats, field) / sizeof(unsigned))
-template <int K, int MB, bool STATS>
-__global__ void __launch_bounds__(MWARPS * 32, MB)
-    k_match_knn(KnnSet a, KnnSet b, const double *__restrict__ pose7, float min_match_sq_dis, HeavyQ hq, const int *__restrict__ d_sel,
-                unsigned *__restrict__ path_stats, unsigned tma_min, unsigned *__restrict__ trace, int sel_prune) {
+constexpr int KNN_LEAN_REGS = 72;
+
+// This warp's index in the grid, read afresh from the special registers at every use (volatile: not kept in a register
+// across the search).
+__device__ __forceinline__ int global_warp() {
+  unsigned tid, cta;
+  asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
+  asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(cta));
+  return (int)(cta * MWARPS + (tid >> 5));
+}
+
+template <int K, bool STATS>
+__device__ __forceinline__ void match_knn(const KnnSet &a, const KnnSet &b, const double *__restrict__ pose7, float min_match_sq_dis,
+                                          const HeavyQ &hq, const int *__restrict__ d_sel, unsigned *__restrict__ path_stats, unsigned tma_min,
+                                          unsigned *__restrict__ trace, int sel_prune) {
   if (!STATS) path_stats = nullptr, trace = nullptr;
   __shared__ KnnSmem ksm[MWARPS];
   const int lane = threadIdx.x & 31;
@@ -75,59 +94,73 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
   // feature counts were built before the solve; the heavy list and its count were written by the previous matcher, which is two
   // launches back and complete (no kernel of the chain triggers its dependents before its own grid-dependency wait).
   knn_smem_init(ks, lane, tma_min);
+  // The two sets live in shared memory: a query reads its set's pointers where it uses them instead of holding them in
+  // registers across the search (and a set picked by a runtime index is not copied to local memory).
+  __shared__ KnnSet s_set[2];
   __shared__ GridP s_grid[2];
   __shared__ PoseD s_pose;
-  if (threadIdx.x == 0) s_grid[0] = load_grid(a.map), s_grid[1] = load_grid(b.map);
-  const int na = a.d_n ? min(a.n, *a.d_n) : a.n;
-  const int nb = b.d_n ? min(b.n, *b.d_n) : b.n;
-  const int n = na + nb;
+  if (threadIdx.x == 0) s_set[0] = a, s_set[1] = b, s_grid[0] = load_grid(a.map), s_grid[1] = load_grid(b.map);
   // Schedule: first the listed heavy features of the previous launch (one per warp), then a static stride over the rest.
-  const int gw = blockIdx.x * MWARPS + (threadIdx.x >> 5), n_warps = gridDim.x * MWARPS;
-  const bool listed = hq.list_in != nullptr;
-  const int n_heavy = listed ? min(__ldg(hq.cnt_in), n) : 0;
-  const int it_a = n_heavy > gw ? (n_heavy - gw + n_warps - 1) / n_warps : 0;
-  const int it_b = n > gw ? (n - gw + n_warps - 1) / n_warps : 0;
-  const int first_listed = it_a > 0 ? __ldg(hq.list_in + gw) : 0;
-  const int listed_lane = n_heavy <= 32 && lane < n_heavy ? __ldg(hq.list_in + lane) : -1;  // short list: in registers
+  // Its CTA-wide values are kept in shared memory too and read where they are used.
+  __shared__ int s_na, s_n, s_n_heavy, s_h_in;
+  __shared__ int s_listed[32];  // a short heavy list (n_heavy <= 32): the stride skips these
+  {
+    const int na = a.d_n ? min(a.n, *a.d_n) : a.n;
+    const int n = na + (b.d_n ? min(b.n, *b.d_n) : b.n);
+    const int n_heavy = hq.list_in ? min(__ldg(hq.cnt_in), n) : 0;
+    const int gw = blockIdx.x * MWARPS + (threadIdx.x >> 5);
+    if (threadIdx.x == 0) s_na = na, s_n = n, s_n_heavy = n_heavy;
+    if (threadIdx.x < 32) s_listed[lane] = n_heavy <= 32 && lane < n_heavy ? __ldg(hq.list_in + lane) : -1;
+    if (lane == 0 && gw < n_heavy) ks.first = __ldg(hq.list_in + gw);  // the warp's first listed feature
+  }
   // Programmatic dependent launch: the pose searched at (SpecState::xc, published by k_linearize's tail), d_sel (committed there)
   // and the lists, anchors, changed flags and fit inputs k_linearize reads are only touched after the previous kernel completed
   cudaGridDependencySynchronize();
   cudaTriggerProgrammaticLaunchCompletion();
   unsigned long long t_enter = 0ull;
   if (trace) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_enter));
-  if (threadIdx.x == 0) s_pose = pose_from_param(pose7);
+  if (threadIdx.x == 0) s_pose = pose_from_param(pose7), s_h_in = d_sel ? (*d_sel & 1) : 0;  // double-buffered sets: read half s_h_in, write the other
   __syncthreads();
-  const int h_in = d_sel ? (*d_sel & 1) : 0;  // double-buffered sets: read half h_in, write the other
-  if (hq.cnt_zero && gw == 0 && lane == 0) *hq.cnt_zero = 0;
+  const int n_warps = gridDim.x * MWARPS;
+  if (hq.cnt_zero && global_warp() == 0 && lane == 0) *hq.cnt_zero = 0;
+  // The warp's place in the schedule is kept in its shared-memory words too (written by lane 0, read after a __syncwarp):
+  // slot < 0 walks the heavy list at slot - INT_MIN, slot >= 0 strides over the features.
+  if (lane == 0) ks.slot = global_warp() < s_n_heavy ? INT_MIN + global_warp() : global_warp();
 #pragma unroll 1
-  for (int it = 0; it < it_a + it_b; it++) {
-    int i;
-    if (it < it_a) {
-      i = it == 0 ? first_listed : __ldg(hq.list_in + gw + it * n_warps);
-    } else {
-      i = gw + (it - it_a) * n_warps;
-      if (n_heavy > 32) {  // listed ones have been done above
-        const unsigned char *hin = i < na ? a.heavy_in : b.heavy_in;
-        if (hin && hin[i < na ? i : i - na]) continue;
-      } else if (n_heavy > 0 && __any_sync(MLOAM_FULL_MASK, listed_lane == i)) {
-        continue;
-      }
+  for (;; ) {
+    __syncwarp();
+    int t = ks.slot;
+    __syncwarp();  // every lane has read it before lane 0 advances it
+    bool from_list = t < 0;
+    if (from_list) {
+      t -= INT_MIN;
+      if (t >= s_n_heavy) t = global_warp(), from_list = false;
     }
-    const float4 p = __ldg(i < na ? a.pts + i : b.pts + (i - na));
+    if (!from_list && t >= s_n) break;
+    const int na = s_na;
+    int i = t;
+    if (lane == 0) ks.slot = from_list ? INT_MIN + (t + n_warps) : t + n_warps;
+    if (from_list) {
+      i = t == global_warp() ? ks.first : __ldg(hq.list_in + t);
+    } else if (s_n_heavy > 32) {  // listed ones have been done above
+      const unsigned char *hin = s_set[i < na ? 0 : 1].heavy_in;
+      if (hin && hin[i < na ? i : i - na]) continue;
+    } else if (s_n_heavy > 0 && __any_sync(MLOAM_FULL_MASK, s_listed[lane] == i)) {
+      continue;
+    }
     const bool in_a = i < na;
     const int j = in_a ? i : i - na;
+    const KnnSet &S = s_set[in_a ? 0 : 1];
+    const float4 p = __ldg(S.pts + j);
     const long long t_query = (path_stats || trace) ? clock64() : 0ll;
     int path = 3;  // 0 keep (matched), 1 keep (rejected), 2 ball, 3 blind
     const float3 sel = associate(s_pose, p.x, p.y, p.z);  // pointAssociateToMap, utility.h:103-117
     const GridP &g = s_grid[in_a ? 0 : 1];
     Best best;  // selection width K + 1: lane K holds the nearest scanned point outside the K-set (feeds the anchor's slack)
-    const int hs = in_a ? a.half : b.half, o_in = h_in ? hs : 0, o_out = hs - o_in;
-    const int *const pos_in = (in_a ? a.pos : b.pos) + (size_t)(j + o_in) * K;
-    int *const pos_out = (in_a ? a.pos : b.pos) + (size_t)(j + o_out) * K;
-    const int seeded = in_a ? a.seeded : b.seeded;
-    unsigned char *const changed = in_a ? a.changed : b.changed;
-    const float4 *const anchor_in = (in_a ? a.anchor : b.anchor) + j + o_in;
-    float4 *const anchor = (in_a ? a.anchor : b.anchor) + j + o_out;  // every query writes its complete state to the out half
+    // read half o_in, write half o_out: every query writes its complete state (list, anchor) to the out half.  The addresses
+    // are formed from S where they are used.
+    const int o_in = s_h_in ? S.half : 0, o_out = S.half - o_in;
+    const int seeded = S.seeded;
     // Temporal coherence between re-association iterations (all three shortcuts are exact, see knn.cuh):
     //   keep    the query moved less than the anchor's slack since its last real search: the K-set cannot have
     //           changed, only its order — recompute the K distances and re-rank (no cell probes, no scan)
@@ -137,8 +170,8 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
     bool done = false;
     float r2 = 3.0e38f;
     if (seeded) {
-      if (lane < K) prev = pos_in[lane];
-      const float4 an = *anchor_in;
+      if (lane < K) prev = S.pos[(size_t)(j + o_in) * K + lane];
+      const float4 an = S.anchor[j + o_in];
       const float mx = sel.x - an.x, my = sel.y - an.y, mz = sel.z - an.z;
       const float moved = sqrtf(mx * mx + my * my + mz * mz);
       const bool within = an.w > 0.0f && moved + 2e-5f < an.w;
@@ -147,13 +180,13 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
         if (within) {
           done = true;
           path = 1;
-          if (lane == 0 && o_out != o_in) *anchor = an;
+          if (lane == 0 && o_out != o_in) S.anchor[j + o_out] = an;
         }
       } else {
         unsigned long long key = MLOAM_KEY_NONE;
         unsigned d2b = 0u;
         if (lane < K) {
-          const float4 v = __ldg((in_a ? a.map.sorted : b.map.sorted) + prev);
+          const float4 v = __ldg(S.map.sorted + prev);
           const float ex = v.x - sel.x, ey = v.y - sel.y, ez = v.z - sel.z;
           d2b = __float_as_uint(ex * ex + ey * ey + ez * ez);  // non-negative floats order like their bit patterns
           key = ((unsigned long long)d2b << 32) | (unsigned)__float_as_int(v.w);
@@ -173,9 +206,9 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
           }
           if (!(r2 < min_match_sq_dis)) {  // :407,571,667,814 — the slack of a match says nothing about a rejection
             newpos = -1;
-            if (lane == 0) *anchor = make_float4(sel.x, sel.y, sel.z, 0.0f);
+            if (lane == 0) S.anchor[j + o_out] = make_float4(sel.x, sel.y, sel.z, 0.0f);
           } else if (lane == 0 && o_out != o_in) {
-            *anchor = an;
+            S.anchor[j + o_out] = an;
           }
           done = true;
           path = 0;
@@ -186,12 +219,12 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
       float explored = 0.0f;
       bool found = false;
       if (r2 < min_match_sq_dis)
-        found = warp_knn_seeded<K, K + 1>(in_a ? a.map : b.map, g, ks, sel.x, sel.y, sel.z, r2, 0.1f * g.cell,
+        found = warp_knn_seeded<K, K + 1>(S.map, g, ks, sel.x, sel.y, sel.z, r2, 0.1f * g.cell,
                                              lane, best, &explored, sel_prune != 0);
       if (!found) {
         KnnDbg dbg = {0, 0, 0, 0, 0, 0};
         const long long t_blind = (path_stats || trace) ? clock64() : 0ll;
-        warp_knn<K, true, K + 1>(in_a ? a.map : b.map, g, ks, sel.x, sel.y, sel.z, min_match_sq_dis, lane, best, &explored, 0.05f,
+        warp_knn<K, true, K + 1>(S.map, g, ks, sel.x, sel.y, sel.z, min_match_sq_dis, lane, best, &explored, 0.05f,
                                  (path_stats || trace) ? &dbg : nullptr, sel_prune != 0);
         if (trace && lane == 0) {
           unsigned *tr = trace + 4 * (size_t)((in_a ? 0 : na) + j);
@@ -230,12 +263,12 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
         if (kK != MLOAM_KEY_NONE) lbK = fminf(lbK, sqrtf(key_d2(kK)));
         slack = lbK - sqrtf(min_match_sq_dis) - 2e-5f;
       }
-      if (lane == 0) *anchor = make_float4(sel.x, sel.y, sel.z, slack);
+      if (lane == 0) S.anchor[j + o_out] = make_float4(sel.x, sel.y, sel.z, slack);
     }
-    if (lane < K) pos_out[lane] = newpos;
-    if (changed) {
+    if (lane < K) S.pos[(size_t)(j + o_out) * K + lane] = newpos;
+    if (S.changed) {
       const bool diff = __any_sync(MLOAM_FULL_MASK, lane < K && (!seeded || newpos != prev));
-      if (lane == 0) changed[j] = diff ? 1 : 0;
+      if (lane == 0) S.changed[j] = diff ? 1 : 0;
     }
     if (path_stats && lane == 0) {  // stage profiling: queries and SM cycles per search path, slowest single query
       const unsigned long long dt = (unsigned long long)(clock64() - t_query);
@@ -249,11 +282,11 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
                 (dt << 32) | ((unsigned long long)path << 30) | ((unsigned long long)(in_a ? 0 : 1) << 29) | (unsigned)(j & 0x1fffffff));
     }
     if (trace && lane == 0) trace[4 * (size_t)((in_a ? 0 : na) + j)] = (unsigned)(clock64() - t_query) | ((unsigned)path << 30);
-    unsigned char *const hout = in_a ? a.heavy_out : b.heavy_out;
+    unsigned char *const hout = S.heavy_out;
     if (hout && lane == 0) {
       const bool heavy = hq.all_searches ? path >= 2 : (path == 3 && seeded);
       hout[j] = heavy ? 1 : 0;
-      if (heavy && hq.list_out) hq.list_out[atomicAdd(hq.cnt_out, 1)] = i;
+      if (heavy && hq.list_out) hq.list_out[atomicAdd(hq.cnt_out, 1)] = in_a ? j : j + s_na;
     }
   }
   if (trace && lane == 0) {  // per-warp timeline after the per-query words: [enter, first query, exit] in ns
@@ -263,6 +296,19 @@ __global__ void __launch_bounds__(MWARPS * 32, MB)
     w[0] = t_enter, w[1] = t_exit;
   }
 }
+
+#define KNN_PARAMS                                                                                                                  \
+  KnnSet a, KnnSet b, const double *__restrict__ pose7, float min_match_sq_dis, HeavyQ hq, const int *__restrict__ d_sel,           \
+      unsigned *__restrict__ path_stats, unsigned tma_min, unsigned *__restrict__ trace, int sel_prune
+template <int K>
+__global__ void __maxnreg__(KNN_LEAN_REGS) k_match_knn(KNN_PARAMS) {
+  match_knn<K, false>(a, b, pose7, min_match_sq_dis, hq, d_sel, path_stats, tma_min, trace, sel_prune);
+}
+template <int K, bool STATS>
+__global__ void __launch_bounds__(MWARPS * 32, 2) k_match_knn_mb2(KNN_PARAMS) {
+  match_knn<K, STATS>(a, b, pose7, min_match_sq_dis, hq, d_sel, path_stats, tma_min, trace, sel_prune);
+}
+#undef KNN_PARAMS
 
 template <int K>
 __global__ void __launch_bounds__(128) k_match_fit(FitSet a, FitSet b, const double *__restrict__ pose7, float min_plane_dis, int check_fov) {
@@ -379,17 +425,16 @@ int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_
       const int s = c->knn_trace_n < KNN_TRACE_SLOTS ? c->knn_trace_n++ : KNN_TRACE_SLOTS - 1;
       trace = reinterpret_cast<unsigned *>(c->knn_trace.as<unsigned char>() + slot * (size_t)s);
     }
-    const int mb = c->knn_min_blocks;
+    // the instrumented instance is compiled for two CTAs per SM; the grid never asks for more CTAs than can be resident:
+    // warps stride over the features
+    const bool stats = path_stats || trace;
+    const int mb = stats ? 2 : c->knn_min_blocks;
     int nb = (n_upper + MWARPS - 1) / MWARPS;
-    if (nb > mb * c->sm_count) nb = mb * c->sm_count;  // all CTAs resident; warps pull / stride over the features
+    if (nb > mb * c->sm_count) nb = mb * c->sm_count;
     void (*k)(KnnSet, KnnSet, const double *, float, HeavyQ, const int *, unsigned *, unsigned, unsigned *, int);
-    if (path_stats || trace) {
-      if (K == 5) k = mb == 2 ? k_match_knn<5, 2, true> : (mb == 3 ? k_match_knn<5, 3, true> : k_match_knn<5, 4, true>);
-      else k = mb == 2 ? k_match_knn<10, 2, true> : (mb == 3 ? k_match_knn<10, 3, true> : k_match_knn<10, 4, true>);
-    } else {
-      if (K == 5) k = mb == 2 ? k_match_knn<5, 2, false> : (mb == 3 ? k_match_knn<5, 3, false> : k_match_knn<5, 4, false>);
-      else k = mb == 2 ? k_match_knn<10, 2, false> : (mb == 3 ? k_match_knn<10, 3, false> : k_match_knn<10, 4, false>);
-    }
+    if (stats) k = K == 5 ? k_match_knn_mb2<5, true> : k_match_knn_mb2<10, true>;
+    else if (mb == 2) k = K == 5 ? k_match_knn_mb2<5, false> : k_match_knn_mb2<10, false>;
+    else k = K == 5 ? k_match_knn<5> : k_match_knn<10>;
     MLOAM_CUDA_OK(c, launch_chain(pdl, k, nb, MWARPS * 32, st, ks[0], ks[1], d_pose7, cfg.min_match_sq_dis, hq, d_sel, path_stats,
                                   c->knn_tma_min, trace, c->knn_all_searches ? 0 : 1));
     c->launches++;
@@ -406,6 +451,17 @@ int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_
     c->launches++;
   }
   MLOAM_CUDA_OK(c, cudaGetLastError());
+  return MLOAM_OK;
+}
+
+int knn_residency(const Ctx *c, int K, int *ctas_per_sm, int *regs) {
+  if (K != 5 && K != 10) return MLOAM_E_INVALID;
+  const void *k = c->knn_min_blocks == 2 ? (K == 5 ? (const void *)k_match_knn_mb2<5, false> : (const void *)k_match_knn_mb2<10, false>)
+                                         : (K == 5 ? (const void *)k_match_knn<5> : (const void *)k_match_knn<10>);
+  cudaFuncAttributes fa;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k, MWARPS * 32, 0) != cudaSuccess || cudaFuncGetAttributes(&fa, k) != cudaSuccess)
+    return MLOAM_E_CUDA;
+  *regs = fa.numRegs;
   return MLOAM_OK;
 }
 

@@ -1058,8 +1058,8 @@ __global__ void __launch_bounds__(LM_THREADS) k_lm(const double *__restrict__ pa
 
 // ---------------------------------------------------------------------------------------- candidate evaluation
 // k_eval_candidate: pass 1 of k_linearize (evaluation at xc + mode-2 tail) for a solve with max_inner == 1, in blocks small
-// enough to run beside the speculative matcher: two k_match_knn CTAs (2 x 256 threads x 112 allocated registers = 57344)
-// leave 8192 registers of an SM, i.e. one block of 64 threads at <= 128 registers.  H at xc is never read with one LM
+// enough to run beside the speculative matcher: three k_match_knn CTAs (3 x 256 threads x 72 registers = 55296) leave 10240
+// registers of an SM, enough for one block of 64 threads at <= 128 registers (8192).  H at xc is never read with one LM
 // iteration (the next Solve's mode 1 overwrites LMState::H, the stats report H0), so only g, cost and the row counts are
 // accumulated.  Bit-identical to k_linearize: a thread evaluates the same features (blocks of 64 tile k_linearize's blocks of
 // 256), the per-component warp butterfly is the same addition tree as k_linearize's packed one, and the tail adds the warp
