@@ -137,6 +137,36 @@ struct FrontEnd {
 };
 static_assert(sizeof(FrontEnd) == 24 && sizeof(RigLayout) == 4 * (MLOAM_MAX_LIDARS + 2), "hashed whole: no padding");
 
+// The frame path's configuration as the mloam_set_* calls leave it.  The frame graph key (pipeline.cu frame_key) and the staged inputs
+// (pipeline.cu stage_frame_inputs) derive from it; a value that is staged (the with_ua covariances and threshold, the outlier leaf, the
+// scan period, MAP_DEG_THRE) never enters the key.
+struct FrameCfg {
+  int n_lidars = 1;                         // mloam_set_lidars: LiDARs batched into one frame
+  bool lidar_merge = false;                 // ... was given extrinsics: features go through the rig merge (also for one LiDAR)
+  double lidar_ext[MLOAM_MAX_LIDARS][7];    // ... their sensor -> base extrinsics
+  bool has_ext = false;                     // mloam_set_extrinsic: the sensor -> base extrinsic applied to extracted features
+  double ext[7] = {0, 0, 0, 0, 0, 0, 1};
+  FrontEnd front{};                         // mloam_set_front_end: the front end of raw frames
+  bool front_set = false;
+  int with_ua = 0;                          // mloam_set_uncertainty
+  double ua_ext_cov[MLOAM_MAX_LIDARS][36];  // per LiDAR: pose_ext[l].cov_, row-major [translation | rotation]
+  double ua_cov_meas[9];                    // COV_MEASUREMENT
+  double ua_trace_threshold = 0.0;          // TRACE_THRESHOLD_MAPPING
+  bool outlier_on = false;                  // mloam_set_outlier, with MAP_OUTLIER_RES
+  float outlier_leaf = 0.f;
+  bool undist_on = false;                   // mloam_set_distortion, with SCAN_PERIOD
+  float undist_scan_period = 0.1f;
+  bool reg_on = false;                      // mloam_set_registered
+  bool gf_float_on = false;                 // mloam_set_gf_float, with MAP_DEG_THRE
+  float gf_float_thre = 0.f;
+
+  // The rig decision: with the merge the frame has n_lidars parts and part l goes to the base frame with lidar_ext[l]; without it, one
+  // part with ext (the identity without mloam_set_extrinsic).  part_ext(0) begins the n_parts() poses, 7 doubles each.
+  bool rig_merge() const { return n_lidars > 1 || lidar_merge; }
+  int n_parts() const { return rig_merge() ? n_lidars : 1; }
+  const double *part_ext(int l) const { return rig_merge() ? lidar_ext[l] : ext; }
+};
+
 // One sweep of a frame (mloam_frame*) or announced for the next one (mloam_frame_set_next*)
 struct Sweep {
   const void *key = nullptr;             // the caller's cloud pointer (host or device): the look-ahead matches on it
@@ -209,8 +239,8 @@ struct GfFloatDev {
 // The context's pinned host block (Ctx::pinned): staging of small host-to-device copies and landing of small read-backs, so that
 // they are truly asynchronous.
 struct PinnedBlock {
-  // Read by captured copies: a frame graph copies these to the device at execution time, so every replay writes them again first
-  // (pipeline.cu stage_frame_inputs).
+  // Read by captured copies: a frame graph copies these to the device at execution time.  pipeline.cu stage_frame_inputs writes them
+  // from FrameCfg before a frame is enqueued and before every replay; the stages below only copy them.
   double pose[7];                   // lm_init_state: the initial pose of a solve
   double ext[7];                    // features_enqueue: the single sensor -> base extrinsic
   float rig[MLOAM_MAX_LIDARS][12];  // features_enqueue: the rig's float 3x4 extrinsics of the merge
@@ -416,11 +446,18 @@ struct Ctx {
     bool set = false;
     Sweep sw;                   // a host sweep's device buffers are set when its copy is enqueued (pipeline.cu stage_next_sweep)
   };
+  // A frame's results on the host, applied by pipeline.cu frame_commit on the stream, capture and replay paths alike
+  struct FrameOutcome {
+    ScanRef S{};                   // the scan the solve took (Ctx::last_scan)
+    int ran = 0;                   // the map gate passed and the solve ran
+    Features next{};               // the announced sweep's features, valid when the frame ran the look-ahead (Ctx::prefetched)
+    RegOut reg{};                  // where the registered clouds went (Ctx::reg_last)
+    bool gf_evaluated = false;     // gd_float evaluated the full Hessian (Ctx::gf_float_evaluated)
+  };
+  FrameCfg cfg;                    // what the mloam_set_* calls configured for the frame path
   // raw frames (mloam_set_front_end, mloam_frame_raw*): the front end runs inside features_enqueue, on the main stream and in the look-ahead
   // branch.  Its work (winner images, sort) and output (projected cloud + ScanInfo) have buffers of their own: the look-ahead reuses them
   // after the main stream's front end, while the main stream runs the with_ua stage and the solve.
-  FrontEnd front{};
-  bool front_set = false;
   DevBuf front_work, front_out;
   Features prefetched;             // features of the sweep announced with the previous frame, ready when that frame returned
   NextSweep next;                  // announced for the frame being enqueued (consumed by it)
@@ -433,10 +470,8 @@ struct Ctx {
   struct GraphEntry {
     unsigned long long key = 0, epoch = 0;
     cudaGraphExec_t exec = nullptr;
-    int launches = 0, seen = 0, s2m_ran = 0;
-    ScanRef S{};
-    Features prefetched_out{};     // what the frame leaves in Ctx::prefetched
-    RegOut reg{};                  // where its registered clouds go (Ctx::reg_last)
+    int launches = 0, seen = 0;
+    FrameOutcome out{};            // what every replay of the graph leaves
   };
   std::vector<GraphEntry> graphs;
   bool smem_opt_in_gf = false;     // k_gf_select's 200 KB pool
@@ -474,11 +509,6 @@ struct Ctx {
                                    // the reference the tests compare against
   int graph_pdl_edges = 0;         // programmatic edges of the last instantiated frame graph (mloam_debug_pdl)
   bool frame_from_graph = false;   // the last frame ran from a frame graph
-  bool lidar_merge = false;        // mloam_set_lidars was given extrinsics: features go through the rig merge (also for one LiDAR)
-  int n_lidars = 1;                // LiDARs batched into one frame of this context (mloam_set_lidars)
-  double lidar_ext[MLOAM_MAX_LIDARS][7];  // their sensor -> base extrinsics
-  bool has_ext = false;            // sensor -> base extrinsic applied to extracted features (frame path)
-  double ext[7] = {0, 0, 0, 0, 0, 0, 1};
   void *nccl_comm = nullptr;
   int nranks = 1, rank = 0;
   // peer-memory exchange of the packed normal equations (comm.cu, solve_kernels.cu lm_tail): every rank's exchange
@@ -488,46 +518,33 @@ struct Ctx {
   void *p2p_peer[MLOAM_P2P_MAX_RANKS] = {nullptr};
   void *p2p_view = nullptr;        // device copy of the P2PView the kernels read
   bool p2p_on = false;
-  // uncertainty-aware mapping in the frame path (mloam_set_uncertainty): the per-point uncertainty + trace gate of
-  // downsampleCurrentScan (lidar_mapper_keyframe.cpp:356-421) between the scan filters and the solve, and the pose covariance
-  // H^-1 at the returned pose (:600-610).  The covariances reach the device through the pinned block (PinnedBlock::ua), so a
-  // captured frame replays with new values.
-  int with_ua = 0;
-  double ua_ext_cov[MLOAM_MAX_LIDARS][36];  // per LiDAR: pose_ext[l].cov_, row-major [translation | rotation]
-  double ua_cov_meas[9];                    // COV_MEASUREMENT
-  double ua_trace_threshold = 0.0;          // TRACE_THRESHOLD_MAPPING
+  // uncertainty-aware mapping in the frame path (FrameCfg::with_ua): the per-point uncertainty + trace gate of downsampleCurrentScan
+  // (lidar_mapper_keyframe.cpp:356-421) between the scan filters and the solve, and the pose covariance H^-1 at the returned pose (:600-610)
   DevBuf ua_scan;                  // gated scans of the last with_ua frame (points, cov6, sqrt_info, counts) + its staged configuration
   DevBuf pose_cov;                 // 36 doubles: H^-1 of the last solve (k_pose_cov), copied back with LMState
-  // the outlier cloud of segment_cloud: 0 (mloam_set_outlier): per LiDAR the first point of its ring-ordered sweep -> base frame ->
+  // the outlier cloud of segment_cloud: 0 (FrameCfg::outlier_on): per LiDAR the first point of its ring-ordered sweep -> base frame ->
   // VoxelGridCovarianceMLOAM<PointI>(MAP_OUTLIER_RES) -> the with_ua gate (lidar_mapper_keyframe.cpp:366-418), one launch next to the
-  // with_ua stage.  The leaf reaches the device through the pinned block (PinnedBlock::outlier), so a captured frame replays with it.
-  bool outlier_on = false;
-  float outlier_leaf = 0.f;
+  // with_ua stage
   DevBuf outlier;                  // the staged configuration, the frame's outlier cloud (points, cov_vec) and its count
-  // DISTORTION (mloam_set_distortion): TransformToEnd of each LiDAR's less-sharp and less-flat features with the pose of
-  // mloam_frame_undistort (estimator.cpp:545-590, :376-408), one launch before the rig merge.  The poses reach the device through the
-  // pinned block (PinnedBlock::undist), so a captured frame replays with new ones.  A pose is consumed by one mloam_frame* call.
-  bool undist_on = false;
-  float undist_scan_period = 0.1f;
+  // DISTORTION (FrameCfg::undist_on): TransformToEnd of each LiDAR's less-sharp and less-flat features with the pose of
+  // mloam_frame_undistort (estimator.cpp:545-590, :376-408), one launch before the rig merge.  The poses are staged like the scan period
+  // (PinnedBlock::undist), so a captured frame replays with new ones.  A pose is consumed by one mloam_frame* call.
   bool undist_set = false;         // a pose was given for the next mloam_frame* call
   int undist_n = 0;
   double undist_pose7[MLOAM_MAX_LIDARS][7];
   DevBuf undist;                   // the staged configuration
-  // gd_float (mloam_set_gf_float): every 10th solve call that passes the map gate evaluates the full information matrix of the scan
+  // gd_float (FrameCfg::gf_float_on): every 10th solve call that passes the map gate evaluates the full information matrix of the scan
   // (evalFullHessian) from the Jacobian rows of outer iteration 0 and sets the ratio k_gf_select reads from GfFloatDev.  Allocated once,
   // outside alloc_epoch(): turning the mode on re-captures nothing.  MAP_DEG_THRE and gf_ratio_ini are staged (PinnedBlock::gf_float_cfg).
-  bool gf_float_on = false;
-  float gf_float_thre = 0.f;
   long long gf_float_frames = 0;   // frame_cnt (:1059): solve calls since the mode was turned on
   bool gf_float_eval = false;      // this call's frame_cnt % 10 == 0
   bool gf_float_evaluated = false; // ... and it passed the map gate: the last call evaluated
   bool gf_float_reported = false;  // a solve call has run since the mode was turned on
   DevBuf gf_float;                 // GfFloatDev
   GfFloatState gf_float_host{};    // the state as the last solve call left it (mloam_gf_float_report)
-  // pubPointCloud (mloam_set_registered; registered.cu): the full-resolution sweep with its outlier points, surf_last and corner_last in
+  // pubPointCloud (FrameCfg::reg_on; registered.cu): the full-resolution sweep with its outlier points, surf_last and corner_last in
   // the map frame, written by one launch at the end of every mloam_frame* call.  The extraction keeps the ring-ordered sweep in the
   // sweep's half of the feature double buffer, because the sweep's own buffers are reused before the frame that registers it ends.
-  bool reg_on = false;
   bool reg_valid = false;          // Ctx::registered holds the clouds of the last mloam_frame* call
   DevBuf registered;               // the three clouds and their device counts (registered_layout)
   RegOut reg_last{};               // where the last frame's clouds are
@@ -549,6 +566,9 @@ struct ProfScope {
   ~ProfScope();
 };
 void prof_collect(Ctx *c);
+
+// A communicator or a peer-memory exchange is attached: the single-GPU features (with_ua frames, outlier, ..., keyframe store) refuse it
+inline bool multi_gpu(const Ctx *c) { return c->nccl_comm != nullptr || c->p2p_on; }
 
 #define MLOAM_CUDA_OK(ctx, expr)                                                                      \
   do {                                                                                                \
@@ -644,14 +664,14 @@ void stage_gf_float(Ctx *c);  // writes PinnedBlock::gf_float_cfg
 int sqrt_info_device(Ctx *c, const float *d_cov6, int n, double *d_sinfo);
 // submap.cu: the with_ua stage of a frame (downsampleCurrentScan, lidar_mapper_keyframe.cpp:356-421) on c->stream.  The scans of *S
 // (device counts) -> per point ext^-1 -> evalPointUncertainty under pose_ext -> trace gate -> stable compaction into Ctx::ua_scan with
-// cov6 and sqrt_info; *S then points at the gated scans.  ua_stage_host writes the staged configuration (PinnedBlock::ua).
+// cov6 and sqrt_info; *S then points at the gated scans.  ua_stage_host stages its configuration (PinnedBlock::ua).
 // d_cfg (nullable): where the staged configuration lies on the device (the outlier stage reads its with_ua part)
 int ua_scan_stage(Ctx *c, Ctx::ScanRef *S, const UaStage **d_cfg = nullptr);
 void ua_stage_host(Ctx *c);
 // submap.cu: the outlier stage of a frame (downsampleCurrentScan, lidar_mapper_keyframe.cpp:366-418) on c->stream, after ua_scan_stage:
 // the first points S->first of the LiDARs' parts of the sweep -> float extrinsic, intensity = laser id -> VoxelGridCovarianceMLOAM<PointI>
 // (MAP_OUTLIER_RES) -> with d_ua (the with_ua stage's configuration) the trace gate, else zero cov_vec -> Ctx::outlier, *S's outlier
-// fields.  One single-CTA launch.  stage_outlier writes the staged configuration (PinnedBlock::outlier).
+// fields.  One single-CTA launch.  stage_outlier stages its configuration (PinnedBlock::outlier).
 int outlier_stage(Ctx *c, Ctx::ScanRef *S, const UaStage *d_ua);
 void stage_outlier(Ctx *c);
 // registered.cu: pubPointCloud (lidar_mapper_keyframe.cpp:690-714) of a frame, one launch on c->stream after the solve.  Per point of the
@@ -678,10 +698,8 @@ struct RegArgs {
 // Ctx::registered for a frame of n_sweep sweep points and the given feature capacities
 int registered_layout(Ctx *c, int n_sweep, int cap_flat, int cap_sharp, RegOut *out);
 int registered_stage(Ctx *c, const RegArgs &a, const RegOut &out);
-// pipeline.cu: writers of the pinned fields a captured frame graph reads (PinnedBlock), shared by the enqueue and the replay paths
+// pipeline.cu: PinnedBlock::pose <- the initial pose of a solve
 void stage_pose(Ctx *c, const double *pose7);
-void stage_ext(Ctx *c);
-void stage_rig(Ctx *c);
 // solve_kernels.cu: Ctx::pose_cov <- LMState::H^-1 (partial-pivot LU), zeros when the last evaluation had no residual rows
 int pose_cov_device(Ctx *c, bool pdl);
 // keyframe.cu: frees the keyframe store (mloam_ctx_destroy)
@@ -704,7 +722,7 @@ int extract_device(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start
                    ExtractOut out, float *d_curv_or_null, int *d_label_or_null);
 // undistort.cu: TransformToEnd in place of the extraction's less-sharp (capacity cap_less, count out.counts[1]) and less-flat (cap_flat,
 // out.counts[3]) features on c->stream, LiDAR l's with the staged pose l; d_off (nullable, the rig's per-LiDAR offsets of the two clouds,
-// 2 x (n_lidars + 1)) finds a point's LiDAR, without it every point is LiDAR 0's.  One launch.  stage_undistort writes PinnedBlock::undist.
+// 2 x (n_lidars + 1)) finds a point's LiDAR, without it every point is LiDAR 0's.  One launch.  stage_undistort stages its configuration.
 int undistort_stage(Ctx *c, ExtractOut out, int cap_less, int cap_flat, const int *d_off, int n_lidars);
 void stage_undistort(Ctx *c);
 // extract_device's work in Ctx::extract_work for n points in n_scans rings

@@ -475,7 +475,7 @@ static int full_hessian_launch(Ctx *c, const FhSet &s0, const FhSet &s1, const d
   return MLOAM_OK;
 }
 
-void stage_gf_float(Ctx *c) { c->pinned->gf_float_cfg[0] = (double)c->gf_float_thre, c->pinned->gf_float_cfg[1] = (double)c->params.gf_ratio; }
+void stage_gf_float(Ctx *c) { c->pinned->gf_float_cfg[0] = (double)c->cfg.gf_float_thre, c->pinned->gf_float_cfg[1] = (double)c->params.gf_ratio; }
 
 int gf_full_hessian_device(Ctx *c, const FeatSet *sets) {
   GfFloatDev *d = c->gf_float.as<GfFloatDev>();

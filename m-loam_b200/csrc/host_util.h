@@ -31,6 +31,15 @@ inline float pick_cell(const Ctx *c, float requested) {
   return cell;
 }
 
+// Pose(q, t).T_.cast<float>() of the pose e7 (pose.cpp:34-41): q normalised, [R | t] row-major as a float 3x4
+inline void pose_mat12(const double *e7, float *m12) {
+  const M33 R = qmat(qnormalized(Q4{e7[3], e7[4], e7[5], e7[6]}));
+  for (int r = 0; r < 3; r++) {
+    for (int k = 0; k < 3; k++) m12[4 * r + k] = (float)R.m[3 * r + k];
+    m12[4 * r + 3] = (float)e7[r];
+  }
+}
+
 inline int upload_pose(Ctx *c, const double *pose7, double **d_pose) {
   double *stage = c->pinned->upload_pose;
   for (int k = 0; k < 7; k++) stage[k] = pose7[k];

@@ -214,8 +214,6 @@ void keyframes_release(Ctx *c) {
 
 namespace {
 
-bool multi_gpu(const Ctx *c) { return c->nccl_comm != nullptr || c->p2p_on; }
-
 // saveKeyframe's test (:649-653): the float distance of the PointI positions, and Eigen's
 // angularDistance(q_cur, q_prev) = 2 atan2(|(q_cur q_prev^-1).vec|, |(q_cur q_prev^-1).w|) in degrees
 bool keyframe_due(const KeyframeStore &S, const double *pose7) {
@@ -390,8 +388,7 @@ int mloam_keyframe_submap(mloam_ctx_t *h, const double *pose_pred7, int *rebuilt
     }
     // per-rebuild device tables: positions in | filter out | GatherEnt | dst offsets | UctLaser of the entering keyframes
     const int n_set = (int)sur.size();
-    const bool merged = c->n_lidars > 1 || c->lidar_merge;
-    const int n_lasers = merged ? c->n_lidars : 1;
+    const int n_lasers = c->cfg.n_parts();
     const size_t n_new = sur.size() - n_surv;
     float4 *d_pos, *d_chosen;
     GatherEnt *d_tab;
@@ -410,15 +407,14 @@ int mloam_keyframe_submap(mloam_ctx_t *h, const double *pose_pred7, int *rebuilt
     // :311-322 cloudUCTAssociateToMap of each entering keyframe with its pose + covariance and the context's current extrinsics and
     // covariances (mloam_set_lidars / mloam_set_uncertainty; the with_ua = false branch without uncertainty)
     S.h_lasers.clear();
-    std::vector<double> ext7(7 * (size_t)n_lasers), pc(7 * (size_t)n_lasers), cc(36 * (size_t)n_lasers);
-    const double zero36[36] = {0};
-    for (int l = 0; l < n_lasers; l++) memcpy(&ext7[7 * l], merged ? c->lidar_ext[l] : c->ext, 7 * sizeof(double));
+    std::vector<double> pc(7 * (size_t)n_lasers), cc(36 * (size_t)n_lasers);
+    const double zero36[36] = {0}, *ext7 = c->cfg.part_ext(0);  // the n_lasers extrinsics
     for (size_t i = n_surv; i < sur.size(); i++) {
       const KeyframeStore::Kf &k = S.kfs[sur[i]];
       for (int l = 0; l < n_lasers; l++)
-        mloam_compound_pose_cov(k.pose, k.cov, &ext7[7 * l], c->with_ua ? c->ua_ext_cov[l] : zero36, &pc[7 * l], &cc[36 * l]);
+        mloam_compound_pose_cov(k.pose, k.cov, ext7 + 7 * l, c->cfg.with_ua ? c->cfg.ua_ext_cov[l] : zero36, &pc[7 * l], &cc[36 * l]);
       std::vector<UctLaser> one;
-      fill_lasers(n_lasers, ext7.data(), pc.data(), cc.data(), one);
+      fill_lasers(n_lasers, ext7, pc.data(), cc.data(), one);
       S.h_lasers.insert(S.h_lasers.end(), one.begin(), one.end());
     }
     if (!S.h_lasers.empty())
@@ -436,8 +432,8 @@ int mloam_keyframe_submap(mloam_ctx_t *h, const double *pose_pred7, int *rebuilt
       char *e = S.cache[S.cur].p + o;
       MLOAM_CUDA_OK(c, cudaMemsetAsync(e, 0, 2 * sizeof(int), st));
       UctFrame f;
-      memcpy(f.pose_global, k.pose, sizeof(f.pose_global)), memcpy(f.cov_meas, c->ua_cov_meas, sizeof(f.cov_meas));
-      f.trace_threshold = S.trace_thr, f.with_ua = c->with_ua ? 1 : 0, f.n_lasers = n_lasers, f.scan_frame = 0;
+      memcpy(f.pose_global, k.pose, sizeof(f.pose_global)), memcpy(f.cov_meas, c->cfg.ua_cov_meas, sizeof(f.cov_meas));
+      f.trace_threshold = S.trace_thr, f.with_ua = c->cfg.with_ua ? 1 : 0, f.n_lasers = n_lasers, f.scan_frame = 0;
       const KfRecord rec = kf_record(S.chunks[k.chunk].p + k.off, k.n);
       for (int t = 0; t < 2; t++) {
         rc = uct_associate_append(c, rec.pts[t], k.n[t], f, d_las + (i - n_surv) * n_lasers, B, reinterpret_cast<float4 *>(e + L.pts[t]),
@@ -635,8 +631,7 @@ int mloam_global_map(mloam_ctx_t *h, int mode, const double *center7, double rad
   if (cand.empty()) return MLOAM_OK;
   cudaStream_t st = c->stream;
   const int n_cand = (int)cand.size();
-  const bool merged = c->n_lidars > 1 || c->lidar_merge;
-  const int n_lasers = merged ? c->n_lidars : 1;
+  const int n_lasers = c->cfg.n_parts();
   // the position filter (down_size_filter_global_map_keyframes, VoxelGridCovarianceMLOAM<PointI>(kf_leaf), :809-810): intensity = id,
   // the last id of a voxel wins; its choice goes to the host, which lays out the association
   float4 *d_pos, *d_ds;
@@ -684,16 +679,15 @@ int mloam_global_map(mloam_ctx_t *h, int mode, const double *center7, double rad
     }
   std::vector<double> h_kpose(7 * (size_t)n_ch);
   std::vector<UctLaser> h_las;
-  std::vector<double> ext7(7 * (size_t)n_lasers), pc(7 * (size_t)n_lasers), cc(36 * (size_t)n_lasers);
-  const double zero36[36] = {0};
-  for (int l = 0; l < n_lasers; l++) memcpy(&ext7[7 * l], merged ? c->lidar_ext[l] : c->ext, 7 * sizeof(double));
+  std::vector<double> pc(7 * (size_t)n_lasers), cc(36 * (size_t)n_lasers);
+  const double zero36[36] = {0}, *ext7 = c->cfg.part_ext(0);  // the n_lasers extrinsics
   for (int i = 0; i < n_ch; i++) {
     const KeyframeStore::Kf &k = S.kfs[chosen[i]];
     memcpy(&h_kpose[7 * (size_t)i], k.pose, sizeof(k.pose));
     for (int l = 0; l < n_lasers; l++)
-      mloam_compound_pose_cov(k.pose, k.cov, &ext7[7 * l], c->with_ua ? c->ua_ext_cov[l] : zero36, &pc[7 * l], &cc[36 * l]);
+      mloam_compound_pose_cov(k.pose, k.cov, ext7 + 7 * l, c->cfg.with_ua ? c->cfg.ua_ext_cov[l] : zero36, &pc[7 * l], &cc[36 * l]);
     std::vector<UctLaser> one;
-    fill_lasers(n_lasers, ext7.data(), pc.data(), cc.data(), one);
+    fill_lasers(n_lasers, ext7, pc.data(), cc.data(), one);
     h_las.insert(h_las.end(), one.begin(), one.end());
   }
   UctSeg *d_seg;
@@ -719,8 +713,8 @@ int mloam_global_map(mloam_ctx_t *h, int mode, const double *center7, double rad
   MLOAM_CUDA_OK(c, carve(G.merged, [&](Carve &cv) { mp = cv.take<float4>(N1), mc6 = cv.take<float>(6 * N1), mtr = cv.take<float>(N1); }));
   UctFrame f;
   memset(&f, 0, sizeof(f));
-  memcpy(f.cov_meas, c->ua_cov_meas, sizeof(f.cov_meas));
-  f.trace_threshold = S.trace_thr, f.with_ua = c->with_ua ? 1 : 0, f.n_lasers = n_lasers, f.scan_frame = 0;
+  memcpy(f.cov_meas, c->cfg.ua_cov_meas, sizeof(f.cov_meas));
+  f.trace_threshold = S.trace_thr, f.with_ua = c->cfg.with_ua ? 1 : 0, f.n_lasers = n_lasers, f.scan_frame = 0;
   int *d_out_n[2] = {nullptr, nullptr};
   int seg0 = 0;
   for (int m = 0; m < n_maps; m++) {

@@ -35,15 +35,15 @@ int on_branch(Ctx *c, const Branch &b, bool fork, Body &&body) {
 }
 
 // Enqueue the whole solve on the context stream (no host synchronisation when max_inner == 1, so the sequence can be
-// captured into a CUDA graph); scan2map_finish() waits and unpacks.  *ran: the map-size gate passed and the solve is enqueued.
-// want_cov: also H^-1 at the returned pose (with_ua frame, mloam_scan2map_ua).
-int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool want_cov, int *ran) {
+// captured into a CUDA graph); scan2map_finish() waits and unpacks.  o->ran: the map-size gate passed and the solve is enqueued;
+// o->gf_evaluated: gd_float evaluates the full Hessian.  want_cov: also H^-1 at the returned pose (with_ua frame, mloam_scan2map_ua).
+int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool want_cov, Ctx::FrameOutcome *o) {
   const mloam_params_t &P = c->params;
-  *ran = 0;
+  o->ran = 0, o->gf_evaluated = false;
   const MapStorage &MS = c->maps[MLOAM_MAP_SURF], &MC = c->maps[MLOAM_MAP_CORNER];
   if (!MS.built || !MC.built) return fail(c, MLOAM_E_STATE, "scan2map: build MLOAM_MAP_SURF and MLOAM_MAP_CORNER first");
   if (!((MS.m > 50) && (MC.m > 10))) return MLOAM_OK;  // lidar_mapper_keyframe.cpp:429 ("Map surf num is not enough")
-  *ran = 1;
+  o->ran = 1;
   // Collective participation: the gate above depends on the replicated maps only, so every rank takes the same branch; from here
   // on every rank enqueues the same number of LM evaluations (max_outer x (1 + max_inner) with max_inner == 1; with max_inner > 1
   // the done flag all ranks poll is the identical, summed state).  Per-rank solves (tracker, odometry) are never collective.
@@ -110,8 +110,8 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool wa
       unsigned char *mask[2] = {nullptr, nullptr};
       // gd_float: the ratio is read on the device; an evaluation frame's first iteration makes both sets' rows, evaluates the full
       // Hessian over them (which sets that ratio, :456-495) and only then selects
-      const double *d_ratio = c->gf_float_on ? &c->gf_float.as<GfFloatDev>()->st.ratio_cur : nullptr;
-      const bool eval = c->gf_float_on && c->gf_float_eval && outer == 0;
+      const double *d_ratio = c->cfg.gf_float_on ? &c->gf_float.as<GfFloatDev>()->st.ratio_cur : nullptr;
+      const bool eval = c->cfg.gf_float_on && c->gf_float_eval && outer == 0;
       auto select = [&](int t, int phase) {
         if (sets[t].n <= 0) return MLOAM_OK;
         return gf_select_set_device(c, t, sets[t], d_pose, sinfo, P.gf_method, (double)P.gf_ratio,
@@ -123,7 +123,7 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool wa
         if (rc == MLOAM_OK) rc = select(1, 1);
         if (rc == MLOAM_OK) rc = gf_full_hessian_device(c, sets);
         if (rc) return rc;
-        c->gf_float_evaluated = true;
+        o->gf_evaluated = true;
       }
       const int phase = eval ? 2 : 3;
       // the two selections are independent single-CTA chains: corner on the side stream next to surf (also inside a captured graph)
@@ -181,7 +181,7 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool wa
     stamp(c, "pose covariance");
   }
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(hs, st, sizeof(LMState), cudaMemcpyDeviceToHost, c->stream));
-  if (c->gf_float_on)  // the report (mloam_gf_float_report) lands with the frame's results
+  if (c->cfg.gf_float_on)  // the report (mloam_gf_float_report) lands with the frame's results
     MLOAM_CUDA_OK(c, cudaMemcpyAsync(&c->pinned->gf_float, &c->gf_float.as<GfFloatDev>()->st, sizeof(GfFloatState), cudaMemcpyDeviceToHost, c->stream));
   if (S.d_n_surf) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_cnt, S.d_n_surf, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   if (S.d_n_corner) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_cnt + 1, S.d_n_corner, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -197,7 +197,7 @@ int scan2map_finish(Ctx *c, const ScanRef &S, const double *pose_init7, bool wan
   const LMState *hs = &c->pinned->lm;
   int *h_cnt = c->pinned->counts;
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
-  if (c->gf_float_on) c->gf_float_host = c->pinned->gf_float;
+  if (c->cfg.gf_float_on) c->gf_float_host = c->pinned->gf_float;
   if (!S.d_n_surf) h_cnt[0] = S.n_surf;
   if (!S.d_n_corner) h_cnt[1] = S.n_corner;
   for (int k = 0; k < 7; k++) pose_out7[k] = hs->x[k];
@@ -243,9 +243,9 @@ int scan2map_finish(Ctx *c, const ScanRef &S, const double *pose_init7, bool wan
 // gd_float: what every solve call does first.  frame_cnt advances before the map gate (lidar_mapper_keyframe.cpp:1059, :429); the 10th,
 // 20th, ... call evaluates if it passes the gate (scan2map_enqueue).
 int gf_float_begin(Ctx *c) {
-  if (!c->gf_float_on) return MLOAM_OK;
+  if (!c->cfg.gf_float_on) return MLOAM_OK;
   if (c->params.gf_method != 3) return fail(c, MLOAM_E_STATE, "gd_float is on (mloam_set_gf_float) and params.gf_method is no longer 3");
-  if (c->nccl_comm || c->p2p_on) return fail(c, MLOAM_E_STATE, "gd_float (mloam_set_gf_float) is single-GPU only; detach the communicator or turn it off");
+  if (multi_gpu(c)) return fail(c, MLOAM_E_STATE, "gd_float (mloam_set_gf_float) is single-GPU only; detach the communicator or turn it off");
   c->gf_float_frames++;
   c->gf_float_eval = c->gf_float_frames % 10 == 0;
   c->gf_float_evaluated = false;
@@ -254,13 +254,14 @@ int gf_float_begin(Ctx *c) {
 }
 
 int scan2map_run(Ctx *c, const ScanRef &S, const double *pose_init7, bool want_cov, double *pose_out7, mloam_solve_stats_t *stats) {
-  int ran = 0;
   c->reg_valid = false;  // a scan has no sweep: nothing to register
   int rc = gf_float_begin(c);
   if (rc) return rc;
-  rc = scan2map_enqueue(c, S, pose_init7, want_cov, &ran);
+  Ctx::FrameOutcome o;
+  rc = scan2map_enqueue(c, S, pose_init7, want_cov, &o);
+  c->gf_float_evaluated = o.gf_evaluated;
   if (rc) return rc;
-  return scan2map_finish(c, S, pose_init7, want_cov, ran, pose_out7, stats);
+  return scan2map_finish(c, S, pose_init7, want_cov, o.ran, pose_out7, stats);
 }
 
 // Device buffers of one frame: feature sets of extractCloud + the down-sampled scans fed to matching.
@@ -307,36 +308,27 @@ int sweep_bufs(Ctx *c, DevBuf &B, int n, int n_scans, SweepIn *S) {
 
 }  // namespace
 
-// Writers of the pinned fields a captured frame graph copies to the device at execution time (PinnedBlock): the enqueue path calls them
-// where it stages each field, stage_frame_inputs before every replay.
 void mloam::stage_pose(Ctx *c, const double *pose7) { memcpy(c->pinned->pose, pose7, sizeof(c->pinned->pose)); }
-void mloam::stage_ext(Ctx *c) { memcpy(c->pinned->ext, c->ext, sizeof(c->pinned->ext)); }
-void mloam::stage_rig(Ctx *c) {
-  for (int l = 0; l < c->n_lidars; l++) {
-    const double *e = c->lidar_ext[l];
-    const M33 R = qmat(qnormalized(Q4{e[3], e[4], e[5], e[6]}));  // Pose(q, t): q normalised, T_ = [R | t] (pose.cpp:34-41), cast<float>
-    for (int r = 0; r < 3; r++) {
-      for (int k = 0; k < 3; k++) c->pinned->rig[l][4 * r + k] = (float)R.m[3 * r + k];
-      c->pinned->rig[l][4 * r + 3] = (float)e[r];
-    }
-  }
-}
 
 namespace {
-
-bool rig_merge(const Ctx *c) { return c->n_lidars > 1 || c->lidar_merge; }
 
 // capacity of a frame's less-sharp features: <= 20 picks x 6 sectors per ring
 int less_sharp_cap(int n, int n_scans) { return n < 120 * n_scans ? n : 120 * n_scans; }
 
+// The pinned inputs of a frame (PinnedBlock), from Ctx::cfg and the pose guess: written once before the frame is enqueued and before
+// every replay of its graph, whose captured copies read them at execution time.  The stages only copy them.
 void stage_frame_inputs(Ctx *c, const double *pose7) {
+  const FrameCfg &f = c->cfg;
   stage_pose(c, pose7);
-  if (rig_merge(c)) stage_rig(c);
-  else if (c->has_ext) stage_ext(c);
-  if (c->with_ua) ua_stage_host(c);
-  if (c->outlier_on) stage_outlier(c);
-  if (c->undist_on) stage_undistort(c);
-  if (c->gf_float_on) stage_gf_float(c);
+  if (f.rig_merge()) {
+    for (int l = 0; l < f.n_lidars; l++) pose_mat12(f.lidar_ext[l], c->pinned->rig[l]);
+  } else if (f.has_ext) {
+    memcpy(c->pinned->ext, f.ext, sizeof(c->pinned->ext));
+  }
+  if (f.with_ua) ua_stage_host(c);
+  if (f.outlier_on) stage_outlier(c);
+  if (f.undist_on) stage_undistort(c);
+  if (f.gf_float_on) stage_gf_float(c);
 }
 
 // Whether the look-ahead of the previous frame made the features of sw: same caller pointer and sizes; a raw sweep's features are taken by
@@ -345,7 +337,7 @@ bool frame_has_prefetched(const Ctx *c, const Sweep &sw) {
   const Ctx::Features &f = c->prefetched;
   const bool same_kind = sw.raw ? (f.sw.raw && std::memcmp(&f.sw.L, &sw.L, sizeof(RigLayout)) == 0) : !f.sw.raw;
   return f.valid && c->use_lookahead && !c->prof_on && f.sw.key == sw.key && f.sw.n == sw.n && f.sw.n_scans == sw.n_scans && same_kind &&
-         (f.sw.host || !sw.host) && f.extract_only == c->undist_on && (f.registered || !c->reg_on);
+         (f.sw.host || !sw.host) && f.extract_only == c->cfg.undist_on && (f.registered || !c->cfg.reg_on);
 }
 
 // extractCloud of sweep sw on c->stream into half `parity` of the feature double buffer (*F), with the LiDARs' first points and, for the
@@ -354,13 +346,14 @@ bool frame_has_prefetched(const Ctx *c, const Sweep &sw) {
 // with the raw size n as capacity (no count comes back to the host).
 int extract_enqueue(Ctx *c, const Sweep &sw, int parity, FrameBufs *F_out) {
   const int n = sw.n, n_scans = sw.n_scans;
+  const FrameCfg &cfg = c->cfg;
   FrameBufs F;
-  int rc = frame_bufs(c, n, &F, parity, c->reg_on ? n_scans : 0);
+  int rc = frame_bufs(c, n, &F, parity, cfg.reg_on ? n_scans : 0);
   if (rc) return rc;
   const float4 *d_cloud = sw.cloud;
   const int *d_scan_start = sw.scan_start, *d_scan_end = sw.scan_end;
   if (sw.raw) {
-    const FrontEnd &fe = c->front;
+    const FrontEnd &fe = cfg.front;
     float4 *proj;
     int *ss, *n_proj;
     MLOAM_CUDA_OK(c, carve(c->front_out, [&](Carve &cv) {
@@ -371,21 +364,21 @@ int extract_enqueue(Ctx *c, const Sweep &sw, int parity, FrameBufs *F_out) {
     if (rc) return rc;
     stamp(c, "front end");
     d_cloud = proj, d_scan_start = ss, d_scan_end = ss + n_scans;
-    if (c->reg_on) MLOAM_CUDA_OK(c, cudaMemcpyAsync(F.reg_meta, n_proj, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
+    if (cfg.reg_on) MLOAM_CUDA_OK(c, cudaMemcpyAsync(F.reg_meta, n_proj, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
   }
-  if (c->reg_on) {  // the registered clouds need the sweep when its frame ends: by then next_in, front_out or the caller's buffer may be reused
+  if (cfg.reg_on) {  // the registered clouds need the sweep when its frame ends: by then next_in, front_out or the caller's buffer may be reused
     MLOAM_CUDA_OK(c, cudaMemcpyAsync(F.reg_sweep, d_cloud, sizeof(float4) * (size_t)n, cudaMemcpyDeviceToDevice, c->stream));
     MLOAM_CUDA_OK(c, cudaMemcpyAsync(F.reg_meta + 16, d_scan_start, sizeof(int) * (size_t)n_scans, cudaMemcpyDeviceToDevice, c->stream));
   }
   // every frame's extraction records each LiDAR's first point, so that features extracted ahead serve a frame with the outlier cloud on
-  const int n_parts = rig_merge(c) ? c->n_lidars : 1;
+  const int n_parts = cfg.n_parts();
   if (n_scans % n_parts == 0) F.ex.first = F.first, F.ex.first_ok = F.first_ok, F.ex.first_rings = n_scans / n_parts;  // else the merge
                                                                                                                        // below rejects it
   rc = extract_device(c, d_cloud, n, d_scan_start, d_scan_end, n_scans, F.ex, nullptr, nullptr);
   if (rc) return rc;
-  if (rig_merge(c)) {  // the merge below may run later (undistortion on): each LiDAR's offsets are kept with the sweep's features
-    if (n_scans % c->n_lidars != 0) return fail(c, MLOAM_E_INVALID, "frame: n_scans must be n_lidars x rings per LiDAR");
-    rc = lidar_offsets_device(c, c->n_lidars, n_scans / c->n_lidars, F.off);
+  if (cfg.rig_merge()) {  // the merge below may run later (undistortion on): each LiDAR's offsets are kept with the sweep's features
+    if (n_scans % n_parts != 0) return fail(c, MLOAM_E_INVALID, "frame: n_scans must be n_lidars x rings per LiDAR");
+    rc = lidar_offsets_device(c, n_parts, n_scans / n_parts, F.off);
     if (rc) return rc;
   }
   stamp(c, "extract");
@@ -397,24 +390,23 @@ int extract_enqueue(Ctx *c, const Sweep &sw, int parity, FrameBufs *F_out) {
 // c->stream; the corner filter forks onto branch `side`.
 int scan_enqueue(Ctx *c, const Sweep &sw, const FrameBufs &F, const Branch &side, ScanRef *S_out) {
   const mloam_params_t &P = c->params;
+  const FrameCfg &cfg = c->cfg;
   const int n = sw.n, n_scans = sw.n_scans;
   int rc;
   const int less_cap = less_sharp_cap(n, n_scans);
   DevCtl *ctl = c->ctl.as<DevCtl>();
-  if (c->undist_on) {  // undistortMeasurements (estimator.cpp:376-408): each LiDAR's less-* features in its own frame, before the merge
-    rc = undistort_stage(c, F.ex, less_cap, n, rig_merge(c) ? F.off : nullptr, rig_merge(c) ? c->n_lidars : 1);
+  if (cfg.undist_on) {  // undistortMeasurements (estimator.cpp:376-408): each LiDAR's less-* features in its own frame, before the merge
+    rc = undistort_stage(c, F.ex, less_cap, n, cfg.rig_merge() ? F.off : nullptr, cfg.n_parts());
     if (rc) return rc;
     stamp(c, "undistort");
   }
-  if (rig_merge(c)) {
+  if (cfg.rig_merge()) {
     // batched sweeps of several LiDARs: features of LiDAR l go to the base frame with its extrinsic, intensity = l
     // (transformCloudFeature, visualization.cpp:40-52), LiDAR after LiDAR as pubPointCloud's `+=` (:93-104)
-    stage_rig(c);
-    MLOAM_CUDA_OK(c, cudaMemcpyAsync(ctl->rig, c->pinned->rig, sizeof(float) * 12 * c->n_lidars, cudaMemcpyHostToDevice, c->stream));
-    rc = merge_lidars_device(c, F.ex, less_cap, n, c->n_lidars, &ctl->rig[0][0], F.off);
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(ctl->rig, c->pinned->rig, sizeof(float) * 12 * cfg.n_lidars, cudaMemcpyHostToDevice, c->stream));
+    rc = merge_lidars_device(c, F.ex, less_cap, n, cfg.n_lidars, &ctl->rig[0][0], F.off);
     if (rc) return rc;
-  } else if (c->has_ext) {  // features are handed to the mapper in the base frame
-    stage_ext(c);
+  } else if (cfg.has_ext) {  // features are handed to the mapper in the base frame
     double *d_ext = ctl->ext;
     MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_ext, c->pinned->ext, 7 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
     rc = transform_points_device(c, F.ex.less_sharp, less_cap, F.ex.counts + 1, d_ext);
@@ -461,16 +453,20 @@ int wait_uploads(Ctx *c, cudaEvent_t ev, bool forked) {
   return MLOAM_OK;
 }
 
-// The look-ahead state a frame leaves, on the stream path and on a replay alike: the next frame extracts into the other half, and nf
-// (valid when this frame ran the look-ahead) describes the announced sweep's features
-void frame_advance(Ctx *c, int parity, const Ctx::Features &nf) {
-  c->frame_parity = parity ^ 1;
-  c->prefetched = nf;
-}
+// One mloam_frame* call as frame_call hands it on.  have: the previous frame's look-ahead made the sweep's features, in half `parity`;
+// else they are extracted now into that half.  The submaps are on the device.
+struct FrameCall {
+  Sweep sw;
+  bool have;
+  int parity;
+  const float4 *surf_map, *corner_map;
+  int n_surf_map, n_corner_map, rebuild_maps;
+  const double *pose_init7;
+};
 
 // pubPointCloud of sweep sw, whose features and copy are in half `parity`, on c->stream after the solve: k_registered at pose_wmap_curr,
-// LMState::x when the solve ran (ran), else the initial pose (the map gate keeps it, lidar_mapper_keyframe.cpp:429, :634-638)
-int registered_enqueue(Ctx *c, const Sweep &sw, int parity, int ran, const double *pose_init7) {
+// LMState::x when the solve ran (ran), else the staged initial pose (the map gate keeps it, lidar_mapper_keyframe.cpp:429, :634-638)
+int registered_enqueue(Ctx *c, const Sweep &sw, int parity, int ran, RegOut *out) {
   FrameBufs F;
   int rc = frame_bufs(c, sw.n, &F, parity, sw.n_scans);  // the layout the extraction carved: nothing moves or grows
   if (rc) return rc;
@@ -479,58 +475,58 @@ int registered_enqueue(Ctx *c, const Sweep &sw, int parity, int ran, const doubl
   if (ran) {
     d_pose = c->lm_state.as<LMState>()->x;
   } else {
-    stage_pose(c, pose_init7);
     MLOAM_CUDA_OK(c, cudaMemcpyAsync(ctl->pose, c->pinned->pose, 7 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
     d_pose = ctl->pose;
   }
-  const bool merge = rig_merge(c);
   const int less_cap = less_sharp_cap(sw.n, sw.n_scans);
   RegArgs a{};
   a.sweep = F.reg_sweep, a.n_sweep = sw.n, a.d_n_sweep = sw.raw ? F.reg_meta : nullptr, a.scan_start = F.reg_meta + 16;
-  a.n_parts = merge ? c->n_lidars : 1, a.rings_per_lidar = sw.n_scans / a.n_parts;
-  a.to_base = merge ? 1 : (c->has_ext ? 2 : 0), a.rig = &ctl->rig[0][0], a.ext = ctl->ext;  // as scan_enqueue staged them
-  a.undist = c->undist_on ? c->undist.as<UndistStage>() : nullptr;                          // undistort_stage's configuration
-  if (c->outlier_on) a.first = F.first, a.first_ok = F.first_ok, a.outlier = c->outlier.as<OutlierStage>();  // outlier_stage's
+  a.n_parts = c->cfg.n_parts(), a.rings_per_lidar = sw.n_scans / a.n_parts;
+  a.to_base = c->cfg.rig_merge() ? 1 : (c->cfg.has_ext ? 2 : 0), a.rig = &ctl->rig[0][0], a.ext = ctl->ext;  // as scan_enqueue copied them
+  a.undist = c->cfg.undist_on ? c->undist.as<UndistStage>() : nullptr;  // undistort_stage's configuration
+  if (c->cfg.outlier_on) a.first = F.first, a.first_ok = F.first_ok, a.outlier = c->outlier.as<OutlierStage>();  // outlier_stage's
   a.less_flat = F.ex.less_flat, a.less_sharp = F.ex.less_sharp, a.cap_flat = sw.n, a.cap_sharp = less_cap;
   a.n_flat = F.ex.counts + 3, a.n_sharp = F.ex.counts + 1, a.pose = d_pose;
-  RegOut o;
-  rc = registered_layout(c, sw.n, sw.n, less_cap, &o);
-  if (rc == MLOAM_OK) rc = registered_stage(c, a, o);
+  rc = registered_layout(c, sw.n, sw.n, less_cap, out);
+  if (rc == MLOAM_OK) rc = registered_stage(c, a, *out);
   if (rc) return rc;
-  c->reg_last = o;
   stamp(c, "registered");
   return MLOAM_OK;
 }
 
-// The features of sw — ready from the look-ahead when `have`, else extracted now into half `parity` — the look-ahead of the announced
-// sweep, the map builds (rebuild_maps) and the solve on c->stream.  *ran: scan2map_enqueue's.
-int frame_enqueue(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_surf_map, int n_surf_map, const float4 *d_corner_map,
-                  int n_corner_map, int rebuild_maps, const double *pose_init7, ScanRef *S_out, int *ran) {
+// The frame's inputs staged, then on c->stream: the features of the sweep — ready from the look-ahead when f.have, else extracted now
+// into half f.parity —, the look-ahead of the announced sweep, the map builds (f.rebuild_maps) and the solve.  Writes nothing of the
+// context's frame state: the host-side results go to *o for frame_commit.
+int frame_enqueue(Ctx *c, const FrameCall &f, Ctx::FrameOutcome *o) {
+  const FrameCfg &cfg = c->cfg;
+  const Sweep &sw = f.sw;
+  *o = Ctx::FrameOutcome{};
+  stage_frame_inputs(c, f.pose_init7);
   // lidar_mapper_keyframe.cpp:433-434 (every frame in the reference).  The two submap builds do not depend on the sweep: they run on a
   // forked side stream, concurrently with extraction + scan down-sampling, and join right before matching (also inside a captured graph).
   // With stage profiling on the branch stays on the main stream so that per-stage event times do not overlap.
-  const bool fork_maps = rebuild_maps && !c->prof_on;
+  const bool fork_maps = f.rebuild_maps && !c->prof_on;
   int rc;
-  if (rebuild_maps) {
+  if (f.rebuild_maps) {
     rc = on_branch(c, c->br_maps, fork_maps, [&] {
       int r = c->maps_pending ? wait_uploads(c, c->ev_maps, fork_maps) : MLOAM_OK;
-      if (r == MLOAM_OK) r = map_build_device(c, MLOAM_MAP_SURF, d_surf_map, n_surf_map, pick_cell(c, 0.f));
-      if (r == MLOAM_OK) r = map_build_device(c, MLOAM_MAP_CORNER, d_corner_map, n_corner_map, pick_cell(c, 0.f));
+      if (r == MLOAM_OK) r = map_build_device(c, MLOAM_MAP_SURF, f.surf_map, f.n_surf_map, pick_cell(c, 0.f));
+      if (r == MLOAM_OK) r = map_build_device(c, MLOAM_MAP_CORNER, f.corner_map, f.n_corner_map, pick_cell(c, 0.f));
       return r;
     });
     if (rc) return rc;
   }
   c->stamp_n = 0;
   stamp(c, "start");
-  ScanRef S{};
-  if (have && !c->prefetched.extract_only) S = c->prefetched.S;
-  c->prefetched.valid = false;  // half `parity` is taken or overwritten here
-  if (!have) {
-    rc = features_enqueue(c, sw, parity, c->br_scan, &S);
+  ScanRef &S = o->S;
+  const Ctx::Features &pf = c->prefetched;  // the look-ahead's features of this sweep, when f.have
+  if (f.have && !pf.extract_only) S = pf.S;
+  if (!f.have) {
+    rc = features_enqueue(c, sw, f.parity, c->br_scan, &S);
     if (rc) return rc;
-  } else if (c->prefetched.extract_only) {  // undistortion on: the look-ahead extracted; this sweep's pose is known now
+  } else if (pf.extract_only) {  // undistortion on: the look-ahead extracted; this sweep's pose is known now
     FrameBufs F;
-    rc = frame_bufs(c, sw.n, &F, parity, c->reg_on ? sw.n_scans : 0);
+    rc = frame_bufs(c, sw.n, &F, f.parity, cfg.reg_on ? sw.n_scans : 0);
     F.ex.first = F.first, F.ex.first_ok = F.first_ok;  // recorded by the look-ahead's extraction (extract_enqueue)
     if (rc == MLOAM_OK) rc = scan_enqueue(c, sw, F, c->br_scan, &S);
     if (rc) return rc;
@@ -539,32 +535,32 @@ int frame_enqueue(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *
   // and solved (it reuses Ctx::extract_work, voxel_corner and voxel_surf of the block above, hence the fork AFTER it).  With the
   // undistortion on, the next sweep's pose comes with the next call: the branch extracts only (extract_work), and that call runs
   // undistortion, merge and the scan filters on the main stream before it forks its own look-ahead.
-  Ctx::Features nf{};
+  Ctx::Features &nf = o->next;
   if (c->next.set && c->use_lookahead && !c->prof_on) {
     const Sweep &nx = c->next.sw;
     c->stamp_mute = true;
     rc = on_branch(c, c->br_ahead, true, [&] {
       int r = c->next_pending ? wait_uploads(c, c->ev_next, true) : MLOAM_OK;  // mloam_frame copied the next sweep on br_ahead
-      if (r == MLOAM_OK && c->undist_on) {
+      if (r == MLOAM_OK && cfg.undist_on) {
         FrameBufs F;
-        r = extract_enqueue(c, nx, parity ^ 1, &F);
+        r = extract_enqueue(c, nx, f.parity ^ 1, &F);
       } else if (r == MLOAM_OK) {
-        r = features_enqueue(c, nx, parity ^ 1, c->br_ahead_scan, &nf.S);
+        r = features_enqueue(c, nx, f.parity ^ 1, c->br_ahead_scan, &nf.S);
       }
       return r;
     });
     c->stamp_mute = false;
     if (rc) return rc;
-    nf.valid = true, nf.parity = parity ^ 1, nf.sw = nx, nf.extract_only = c->undist_on, nf.registered = c->reg_on;
+    nf.valid = true, nf.parity = f.parity ^ 1, nf.sw = nx, nf.extract_only = cfg.undist_on, nf.registered = cfg.reg_on;
   }
-  stamp(c, have ? "features (prefetched)" : "extract + voxel");
+  stamp(c, f.have ? "features (prefetched)" : "extract + voxel");
   const UaStage *d_ua = nullptr;
-  if (c->with_ua) {  // downsampleCurrentScan's per-point uncertainty + trace gate: on the main stream with the covariances of THIS call
+  if (cfg.with_ua) {  // downsampleCurrentScan's per-point uncertainty + trace gate: on the main stream with the covariances of THIS call
     rc = ua_scan_stage(c, &S, &d_ua);
     if (rc) return rc;
     stamp(c, "uncertainty + gate");
   }
-  if (c->outlier_on) {  // the outlier cloud (:366-418): the recorded first points -> base frame -> filter -> the same gate, one launch
+  if (cfg.outlier_on) {  // the outlier cloud (:366-418): the recorded first points -> base frame -> filter -> the same gate, one launch
     rc = outlier_stage(c, &S, d_ua);
     if (rc) return rc;
     stamp(c, "outlier cloud");
@@ -573,19 +569,26 @@ int frame_enqueue(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *
     MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream, c->br_maps.join, 0));
     stamp(c, "map build join");
   }
-  *S_out = S;
-  rc = scan2map_enqueue(c, S, pose_init7, c->with_ua != 0, ran);
+  rc = scan2map_enqueue(c, S, f.pose_init7, cfg.with_ua != 0, o);
   if (rc) return rc;
-  if (c->reg_on) {  // pubPointCloud (:690-714): after the solve, next to the look-ahead's tail
-    rc = registered_enqueue(c, sw, parity, *ran, pose_init7);
+  if (cfg.reg_on) {  // pubPointCloud (:690-714): after the solve, next to the look-ahead's tail
+    rc = registered_enqueue(c, sw, f.parity, o->ran, &o->reg);
     if (rc) return rc;
   }
   if (nf.valid) {  // the frame ends when both branches have: the features of the next sweep are complete when this call returns
     MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream, c->br_ahead.join, 0));
     stamp(c, "look-ahead join");
   }
-  frame_advance(c, parity, nf);
   return MLOAM_OK;
+}
+
+// A frame's outcome applied to the context, on the stream, capture and replay paths alike
+void frame_commit(Ctx *c, int parity, const Ctx::FrameOutcome &o) {
+  c->frame_parity = parity ^ 1;
+  c->prefetched = o.next;
+  c->last_scan = o.S, c->last_scan_valid = true;
+  c->reg_last = o.reg;
+  c->gf_float_evaluated = o.gf_evaluated;
 }
 
 // Point the device side of host sweep *sw into B (the points, then room for its ScanInfo) and, with `upload`, copy the sweep there on st.
@@ -630,138 +633,117 @@ int count_programmatic_edges(cudaGraph_t g) {
   return k;
 }
 
-unsigned long long fnv1a(unsigned long long h, const void *p, size_t n) {
-  const unsigned char *b = static_cast<const unsigned char *>(p);
-  for (size_t i = 0; i < n; i++) h = (h ^ b[i]) * 1099511628211ull;
+// Everything a frame graph depends on besides its staged inputs (stage_frame_inputs), hashed whole into the graph cache's key.  What a
+// frame does not use is zero, so two frames share a key exactly when they enqueue the same graph.
+struct FrameKey {
+  const void *sweep[4];  // the sweep on the device (cloud, scan_start, scan_end) and the caller's pointer
+  const void *maps[2];   // the submaps of an in-frame rebuild
+  const void *next[4];   // the announced sweep (look-ahead): the caller's pointer, cloud, scan_start, scan_end
+  cudaStream_t stream;
+  mloam_params_t params;
+  double ext[7], lidar_ext[MLOAM_MAX_LIDARS][7];  // the rig's first n_lidars
+  FrontEnd front, next_front;  // kernel arguments of the captured front end of a raw sweep / a raw announced sweep
+  RigLayout L, next_L;
+  float cells[2];              // the auto cell edges of an in-frame rebuild: kernel arguments of the captured builds
+  // gate: the map-size gate (scan2map_enqueue) is decided on the host at capture: with maps built outside the frame (mloam_map_build*,
+  // mloam_submap_assemble, mloam_keyframe_submap) a graph captured while it failed must not be replayed once it passes, and back
+  int n, n_scans, raw, n_surf_map, n_corner_map, rebuild_maps, maps_pending, gate, has_ext, n_lidars, lidar_merge;
+  // the stages' launches and the look-ahead's split with the undistortion on (their staged values are not part of the key)
+  int with_ua, outlier_on, undist_on, undist_n, reg_on, gf_float_on, gf_eval;
+  // the look-ahead: which half holds this sweep's features (or that they are extracted now), and the announced next sweep
+  int have, parity, ahead, next_n, next_n_scans, next_host, next_pending, stamp_on;
+};
+static_assert(sizeof(FrameKey) == 11 * sizeof(void *) + sizeof(mloam_params_t) + sizeof(double) * 7 * (1 + MLOAM_MAX_LIDARS) +
+                                      2 * sizeof(FrontEnd) + 2 * sizeof(RigLayout) + 2 * sizeof(float) + 26 * sizeof(int),
+              "hashed whole in 8-byte words: no padding");
+
+unsigned long long frame_key(Ctx *c, const FrameCall &f) {
+  const FrameCfg &cfg = c->cfg;
+  const Sweep &sw = f.sw, &nx = c->next.sw;
+  FrameKey k;
+  memset(&k, 0, sizeof(k));
+  k.sweep[0] = sw.cloud, k.sweep[1] = sw.scan_start, k.sweep[2] = sw.scan_end, k.sweep[3] = sw.key;
+  k.maps[0] = f.surf_map, k.maps[1] = f.corner_map, k.stream = c->stream;
+  memcpy(&k.params, &c->params, sizeof(k.params));
+  memcpy(k.ext, cfg.ext, sizeof(k.ext));
+  memcpy(k.lidar_ext, cfg.lidar_ext, sizeof(double) * 7 * (size_t)cfg.n_lidars);
+  if (sw.raw) k.front = cfg.front, k.L = sw.L;
+  if (f.rebuild_maps && !(c->params.map_cell > 0.f)) {
+    k.cells[0] = c->maps[MLOAM_MAP_SURF].auto_cell_pick(c->pinned, MLOAM_MAP_SURF);
+    k.cells[1] = c->maps[MLOAM_MAP_CORNER].auto_cell_pick(c->pinned, MLOAM_MAP_CORNER);
+  }
+  k.n = sw.n, k.n_scans = sw.n_scans, k.raw = sw.raw, k.n_surf_map = f.n_surf_map, k.n_corner_map = f.n_corner_map;
+  k.rebuild_maps = f.rebuild_maps, k.maps_pending = c->maps_pending;
+  const MapStorage &MS = c->maps[MLOAM_MAP_SURF], &MC = c->maps[MLOAM_MAP_CORNER];
+  k.gate = !f.rebuild_maps && MS.built && MC.built && MS.m > 50 && MC.m > 10;
+  k.has_ext = cfg.has_ext, k.n_lidars = cfg.n_lidars, k.lidar_merge = cfg.lidar_merge;
+  k.with_ua = cfg.with_ua, k.outlier_on = cfg.outlier_on, k.reg_on = cfg.reg_on;
+  k.undist_on = cfg.undist_on, k.undist_n = cfg.undist_on ? c->undist_n : 0;
+  k.gf_float_on = cfg.gf_float_on, k.gf_eval = cfg.gf_float_on && c->gf_float_eval;  // an evaluation frame's extra launch
+  k.have = f.have, k.parity = f.parity, k.stamp_on = c->stamp_on;
+  if (c->next.set && c->use_lookahead) {
+    k.next[0] = nx.key, k.next[1] = nx.cloud, k.next[2] = nx.scan_start, k.next[3] = nx.scan_end;
+    k.ahead = 1, k.next_n = nx.n, k.next_n_scans = nx.n_scans, k.next_host = nx.host, k.next_pending = c->next_pending;
+    if (nx.raw) k.next_front = cfg.front, k.next_L = nx.L;
+  }
+  unsigned long long h = 1469598103934665603ull, w;  // FNV-1a over 8-byte words: the key is built on the frame's host critical path
+  for (size_t i = 0; i < sizeof(k); i += 8) memcpy(&w, reinterpret_cast<const char *>(&k) + i, 8), h = (h ^ w) * 1099511628211ull;
   return h;
 }
 
-// One frame.  With max_inner == 1 the ~60 launches of a frame form a fixed sequence that depends on the host only
-// through the pose guess (staged in pinned memory) — it is captured once per (buffers, sizes, parameters) into a CUDA
-// graph and replayed: the first call with a new key runs on the stream (and performs every allocation), the second
-// captures + instantiates, later ones replay.  Profiling, multi-GPU (NCCL on the stream) and max_inner > 1 (the host
-// polls the LM done flag) use the plain stream path.  have / parity: the look-ahead decision of frame_call, in the key and the
-// same on every path.
-int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_surf_map, int n_surf_map, const float4 *d_corner_map,
-              int n_corner_map, int rebuild_maps, const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
-  ScanRef S{};
-  if (c->with_ua && c->nccl_comm)
-    return fail(c, MLOAM_E_STATE, "frame: uncertainty-aware frames (mloam_set_uncertainty) are single-GPU only; detach the communicator or set with_ua = 0");
-  if (c->outlier_on && c->nccl_comm)  // turned on before the communicator was attached
-    return fail(c, MLOAM_E_STATE, "frame: the outlier cloud (mloam_set_outlier) is single-GPU only; detach the communicator or set it to 0");
-  if (c->undist_on && c->nccl_comm)
-    return fail(c, MLOAM_E_STATE, "frame: the undistortion (mloam_set_distortion) is single-GPU only; detach the communicator or turn it off");
-  if (c->reg_on && c->nccl_comm)
-    return fail(c, MLOAM_E_STATE, "frame: the registered clouds (mloam_set_registered) are single-GPU only; detach the communicator or turn them off");
-  const bool want_cov = c->with_ua != 0;
+// The single-GPU stages at frame time: their setters refuse a multi-GPU context (multi_gpu), and this refuses a communicator attached
+// after them.  raw: the sweep is raw, and the front end is single-GPU too.
+int frame_single_gpu(Ctx *c, bool raw) {
+  if (!c->nccl_comm) return MLOAM_OK;
+  const FrameCfg &f = c->cfg;
+  const char *msg =
+      raw          ? "frame_raw: raw frames are single-GPU only; detach the communicator"
+      : f.with_ua  ? "frame: uncertainty-aware frames (mloam_set_uncertainty) are single-GPU only; detach the communicator or set with_ua = 0"
+      : f.outlier_on ? "frame: the outlier cloud (mloam_set_outlier) is single-GPU only; detach the communicator or set it to 0"
+      : f.undist_on  ? "frame: the undistortion (mloam_set_distortion) is single-GPU only; detach the communicator or turn it off"
+      : f.reg_on     ? "frame: the registered clouds (mloam_set_registered) are single-GPU only; detach the communicator or turn them off"
+                     : nullptr;
+  return msg ? fail(c, MLOAM_E_STATE, msg) : MLOAM_OK;
+}
+
+// One frame.  With max_inner == 1 the ~60 launches of a frame form a fixed sequence that depends on the host only through the staged
+// inputs — it is captured once per frame_key into a CUDA graph and replayed: the first call with a new key runs on the stream (and
+// performs every allocation), the second captures + instantiates, later ones replay.  Profiling, multi-GPU (NCCL on the stream) and
+// max_inner > 1 (the host polls the LM done flag) use the plain stream path.
+int frame_run(Ctx *c, const FrameCall &f, double *pose_out7, mloam_solve_stats_t *stats) {
+  int rc = frame_single_gpu(c, false);
+  if (rc) return rc;
+  const bool want_cov = c->cfg.with_ua != 0;
   c->last_scan_valid = false;
   c->frame_from_graph = false;
-  {
-    const int rc = gf_float_begin(c);
-    if (rc) return rc;
-  }
+  rc = gf_float_begin(c);
+  if (rc) return rc;
+  Ctx::FrameOutcome o;
   const bool can_graph = c->use_graphs && c->params.max_inner == 1 && !c->prof_on && (!c->nccl_comm || c->p2p_on);
   if (can_graph) {
-    unsigned long long key = 1469598103934665603ull;
-    const void *ptrs[5] = {sw.cloud, sw.scan_start, sw.scan_end, d_surf_map, d_corner_map};
-    const int ints[7] = {sw.n, sw.n_scans, n_surf_map, n_corner_map, rebuild_maps, c->has_ext ? 1 : 0, c->maps_pending ? 1 : 0};
-    key = fnv1a(key, ptrs, sizeof(ptrs));
-    key = fnv1a(key, ints, sizeof(ints));
-    if (rebuild_maps && !(c->params.map_cell > 0.f)) {  // the auto cell edges are kernel arguments of the captured build
-      const float cells[2] = {c->maps[MLOAM_MAP_SURF].auto_cell_pick(c->pinned, MLOAM_MAP_SURF),
-                              c->maps[MLOAM_MAP_CORNER].auto_cell_pick(c->pinned, MLOAM_MAP_CORNER)};
-      key = fnv1a(key, cells, sizeof(cells));
-    }
-    key = fnv1a(key, &c->params, sizeof(c->params));
-    key = fnv1a(key, c->ext, sizeof(c->ext));
-    key = fnv1a(key, &c->n_lidars, sizeof(c->n_lidars));
-    key = fnv1a(key, &c->lidar_merge, sizeof(c->lidar_merge));
-    key = fnv1a(key, c->lidar_ext, sizeof(double) * 7 * (size_t)c->n_lidars);
-    key = fnv1a(key, &c->stream, sizeof(c->stream));
-    key = fnv1a(key, &c->with_ua, sizeof(c->with_ua));  // the covariances and the threshold are staged, not part of the key
-    if (c->outlier_on) {  // the outlier stage's launch (its leaf is staged); a context that never turns it on keeps its keys
-      const int on = 1;
-      key = fnv1a(key, &on, sizeof(on));
-    }
-    if (c->undist_on) {  // the undistortion's launch and the look-ahead's split (poses and scan period are staged)
-      const int on[2] = {'u', c->undist_n};
-      key = fnv1a(key, on, sizeof(on));
-    }
-    if (c->reg_on) {  // pubPointCloud's launch and the sweep copies of the extraction; a context that never turns it on keeps its keys
-      const int on = 'r';
-      key = fnv1a(key, &on, sizeof(on));
-    }
-    if (c->gf_float_on) {  // gd_float: the ratio's device read, and an evaluation frame's extra launch (threshold, gf_ratio_ini and the
-      const int on[2] = {'g', c->gf_float_eval ? 1 : 0};  // ratio itself are not in the key: they are staged or stay on the device)
-      key = fnv1a(key, on, sizeof(on));
-    }
-    if (sw.raw) {  // raw frame: the per-LiDAR counts and the front-end parameters are kernel arguments of the captured front end
-      key = fnv1a(key, &sw.L, sizeof(RigLayout));
-      key = fnv1a(key, &c->front, sizeof(c->front));
-    }
-    if (!rebuild_maps) {
-      // the map-size gate (scan2map_enqueue) is decided on the host at capture: with maps built outside the frame (mloam_map_build*,
-      // mloam_submap_assemble, mloam_keyframe_submap) a graph captured while it failed must not be replayed once it passes, and back
-      const MapStorage &MS = c->maps[MLOAM_MAP_SURF], &MC = c->maps[MLOAM_MAP_CORNER];
-      const int gate = (MS.built && MC.built && MS.m > 50 && MC.m > 10) ? 1 : 0;
-      key = fnv1a(key, &gate, sizeof(gate));
-    }
-    {  // look-ahead: which half holds this sweep's features (or that they are extracted now), and the announced next sweep
-      const Sweep &nx = c->next.sw;
-      const bool ahead = c->next.set && c->use_lookahead;
-      const int la[8] = {have ? 1 : 0, parity, ahead ? 1 : 0, ahead ? nx.n : 0, ahead ? nx.n_scans : 0, (ahead && nx.host) ? 1 : 0,
-                         (ahead && c->next_pending) ? 1 : 0, c->stamp_on ? 1 : 0};
-      const void *lp[5] = {sw.key, ahead ? nx.key : nullptr, ahead ? static_cast<const void *>(nx.cloud) : nullptr,
-                           ahead ? static_cast<const void *>(nx.scan_start) : nullptr, ahead ? static_cast<const void *>(nx.scan_end) : nullptr};
-      key = fnv1a(key, la, sizeof(la));
-      key = fnv1a(key, lp, sizeof(lp));
-      if (ahead && nx.raw) key = fnv1a(key, &nx.L, sizeof(RigLayout)), key = fnv1a(key, &c->front, sizeof(c->front));
-    }
+    const unsigned long long key = frame_key(c, f);
     Ctx::GraphEntry *e = nullptr;
     for (auto &g : c->graphs)
       if (g.key == key) e = &g;
-    if (e && e->exec && e->epoch == alloc_epoch()) {
-      stage_frame_inputs(c, pose_init7);  // the captured H2D nodes read them at execution time
-      MLOAM_CUDA_OK(c, cudaGraphLaunch(e->exec, c->stream));
-      c->frame_from_graph = true;
-      c->launches += e->launches;
-      c->gf_float_evaluated = c->gf_float_on && c->gf_float_eval && e->s2m_ran;
-      frame_advance(c, parity, e->prefetched_out);
-      c->last_scan = e->S, c->last_scan_valid = true;
-      c->reg_last = e->reg;
-      return scan2map_finish(c, e->S, pose_init7, want_cov, e->s2m_ran, pose_out7, stats);
-    }
-    if (e && e->seen >= 1) {  // second sighting: capture
+    if (e && e->seen >= 1 && !(e->exec && e->epoch == alloc_epoch())) {  // second sighting: capture, then replay below
       if (e->exec) cudaGraphExecDestroy(e->exec), e->exec = nullptr;
       const long long l0 = c->launches;
       const unsigned long long ep0 = alloc_epoch();
       cudaGraph_t graph = nullptr;
-      const Ctx::Features pf0 = c->prefetched;  // frame_enqueue advances these: put them back when the capture fails
-      const int par0 = c->frame_parity;
-      int ran = 0;
       MLOAM_CUDA_OK(c, cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
-      int rc = frame_enqueue(c, sw, have, parity, d_surf_map, n_surf_map, d_corner_map, n_corner_map, rebuild_maps, pose_init7, &S, &ran);
+      rc = frame_enqueue(c, f, &o);
       cudaError_t ce = cudaStreamEndCapture(c->stream, &graph);
-      if (rc == MLOAM_OK && ce == cudaSuccess && graph && ep0 == alloc_epoch() &&
-          cudaGraphInstantiate(&e->exec, graph, 0) == cudaSuccess) {
-        e->launches = (int)(c->launches - l0), e->epoch = ep0, e->S = S, e->s2m_ran = ran;
-        e->prefetched_out = c->prefetched, e->reg = c->reg_last;
-        c->launches = l0;
-        c->graph_captures++;
-        c->graph_pdl_edges = count_programmatic_edges(graph);
-        cudaGraphDestroy(graph);
-        MLOAM_CUDA_OK(c, cudaGraphLaunch(e->exec, c->stream));
-        c->frame_from_graph = true;
-        c->launches += e->launches;
-        c->last_scan = S, c->last_scan_valid = true;
-        return scan2map_finish(c, S, pose_init7, want_cov, ran, pose_out7, stats);
-      }
+      const bool ok = rc == MLOAM_OK && ce == cudaSuccess && graph && ep0 == alloc_epoch() &&
+                      cudaGraphInstantiate(&e->exec, graph, 0) == cudaSuccess;
+      if (ok) e->launches = (int)(c->launches - l0), e->epoch = ep0, e->out = o, c->graph_captures++;
+      if (ok) c->graph_pdl_edges = count_programmatic_edges(graph);
       if (graph) cudaGraphDestroy(graph);
-      cudaGetLastError();
-      e->exec = nullptr, e->seen = 0;  // capture failed (e.g. a buffer had to grow, which is illegal while capturing): run this frame on
-      c->launches = l0;                // the plain stream path below — it performs the allocation — and capture at a later sighting
-      c->graph_capture_failures++;
-      c->prefetched = pf0, c->frame_parity = par0;
+      c->launches = l0;
+      if (!ok) {
+        cudaGetLastError();
+        e->exec = nullptr, e->seen = 0;  // capture failed (e.g. a buffer had to grow, which is illegal while capturing): run this frame on
+        c->graph_capture_failures++;     // the plain stream path below — it performs the allocation — and capture at a later sighting
+      }
     } else if (!e) {
       if (c->graphs.size() >= 96) {
         if (c->graphs.front().exec) cudaGraphExecDestroy(c->graphs.front().exec);
@@ -771,12 +753,22 @@ int frame_run(Ctx *c, const Sweep &sw, bool have, int parity, const float4 *d_su
       g.key = key, g.seen = 1;
       c->graphs.push_back(g);
     }
+    if (e && e->exec && e->epoch == alloc_epoch()) {
+      stage_frame_inputs(c, f.pose_init7);  // the captured H2D nodes read them at execution time
+      MLOAM_CUDA_OK(c, cudaGraphLaunch(e->exec, c->stream));
+      c->frame_from_graph = true;
+      c->launches += e->launches;
+      frame_commit(c, f.parity, e->out);
+      return scan2map_finish(c, e->out.S, f.pose_init7, want_cov, e->out.ran, pose_out7, stats);
+    }
   }
-  int ran = 0;
-  int rc = frame_enqueue(c, sw, have, parity, d_surf_map, n_surf_map, d_corner_map, n_corner_map, rebuild_maps, pose_init7, &S, &ran);
-  if (rc) return rc;
-  c->last_scan = S, c->last_scan_valid = true;
-  return scan2map_finish(c, S, pose_init7, want_cov, ran, pose_out7, stats);
+  rc = frame_enqueue(c, f, &o);
+  if (rc) {
+    c->prefetched.valid = false;  // half f.parity may be partly overwritten
+    return rc;
+  }
+  frame_commit(c, f.parity, o);
+  return scan2map_finish(c, o.S, f.pose_init7, want_cov, o.ran, pose_out7, stats);
 }
 
 // A ring-ordered sweep (cloud + ScanInfo, in host or in device memory)
@@ -791,25 +783,26 @@ Sweep ring_sweep(const mloam_point_t *cloud, bool host, int n, const int *scan_s
 // The rig's raw sweeps at `raw` (host or device memory; h_counts[l] points of LiDAR l, n_lidars of mloam_set_lidars) after the checks every
 // raw entry point makes
 int raw_sweep(Ctx *c, const mloam_point_t *raw, bool host, const int *h_counts, Sweep *sw) {
-  if (!c->front_set) return fail(c, MLOAM_E_STATE, "frame_raw: call mloam_set_front_end first");
-  if (c->nccl_comm) return fail(c, MLOAM_E_STATE, "frame_raw: raw frames are single-GPU only; detach the communicator");
+  if (!c->cfg.front_set) return fail(c, MLOAM_E_STATE, "frame_raw: call mloam_set_front_end first");
+  const int rc = frame_single_gpu(c, true);
+  if (rc) return rc;
   if (!h_counts) return MLOAM_E_INVALID;
-  const FrontEnd &fe = c->front;
+  const FrontEnd &fe = c->cfg.front;
   if (c->params.max_ring_points > 0 && c->params.max_ring_points < fe.horizon_scans)
     return fail(c, MLOAM_E_INVALID, "frame_raw: params.max_ring_points is below horizon_scans (a projected ring holds up to horizon_scans points)");
   *sw = Sweep{};
   RigLayout &L = sw->L;
-  L.n_lidars = c->n_lidars;
+  L.n_lidars = c->cfg.n_lidars;
   long long total = 0;
-  for (int l = 0; l < c->n_lidars; l++) {
+  for (int l = 0; l < L.n_lidars; l++) {
     if (h_counts[l] <= 0)  // the driver node's empty_check (rosNodeRVOxford.cpp:216-220)
       return fail(c, MLOAM_E_INVALID, "frame_raw: every LiDAR of the rig needs a non-empty sweep");
     L.off[l] = (int)total;
     total += h_counts[l];
     if (total > (1 << 30)) return fail(c, MLOAM_E_INVALID, "frame_raw: sweeps too large");
   }
-  L.off[c->n_lidars] = (int)total;
-  sw->key = raw, sw->host = host, sw->raw = true, sw->n = (int)total, sw->n_scans = c->n_lidars * fe.vertical_scans;
+  L.off[L.n_lidars] = (int)total;
+  sw->key = raw, sw->host = host, sw->raw = true, sw->n = (int)total, sw->n_scans = L.n_lidars * fe.vertical_scans;
   if (!host) sw->cloud = reinterpret_cast<const float4 *>(raw);
   return MLOAM_OK;
 }
@@ -837,26 +830,25 @@ int frame_call(Ctx *c, Sweep sw, const mloam_point_t *surf_map, int n_surf_map, 
                int rebuild_maps, const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
   c->reg_valid = false;
   if (sw.host && rebuild_maps && (!surf_map || !corner_map || n_surf_map < 0 || n_corner_map < 0)) return MLOAM_E_INVALID;
-  if (c->undist_on) {  // the sweep's pose_undist (mloam_frame_undistort), consumed by this call whatever it returns
+  if (c->cfg.undist_on) {  // the sweep's pose_undist (mloam_frame_undistort), consumed by this call whatever it returns
     const bool set = c->undist_set;
     c->undist_set = false;
     if (!set) return fail(c, MLOAM_E_STATE, "frame: the undistortion is on and no pose was given for this sweep (mloam_frame_undistort)");
-    if (c->undist_n != (rig_merge(c) ? c->n_lidars : 1))
+    if (c->undist_n != c->cfg.n_parts())
       return fail(c, MLOAM_E_INVALID, "frame: mloam_frame_undistort gave a pose count other than the frame's LiDARs (1 without the rig merge)");
   }
   cudaSetDevice(c->device);
   // this sweep's features: extracted while the previous frame was solved (look-ahead), or now into the half after the previous frame's
-  const bool have = frame_has_prefetched(c, sw);
-  const int parity = have ? c->prefetched.parity : c->frame_parity;
-  const float4 *d_sm = sw.host ? nullptr : reinterpret_cast<const float4 *>(surf_map);
-  const float4 *d_cm = sw.host ? nullptr : reinterpret_cast<const float4 *>(corner_map);
-  int rc = sw.host ? sweep_to_device(c, c->sweep_in, &sw, !have, c->pinned->scan_info, c->stream) : MLOAM_OK;
+  FrameCall f{sw, frame_has_prefetched(c, sw), 0, nullptr, nullptr, n_surf_map, n_corner_map, rebuild_maps, pose_init7};
+  f.parity = f.have ? c->prefetched.parity : c->frame_parity;
+  if (!sw.host) f.surf_map = reinterpret_cast<const float4 *>(surf_map), f.corner_map = reinterpret_cast<const float4 *>(corner_map);
+  int rc = sw.host ? sweep_to_device(c, c->sweep_in, &f.sw, !f.have, c->pinned->scan_info, c->stream) : MLOAM_OK;
   if (rc == MLOAM_OK) rc = stage_next_sweep(c);
-  if (rc == MLOAM_OK && sw.host && rebuild_maps) rc = upload_submaps(c, surf_map, n_surf_map, corner_map, n_corner_map, &d_sm, &d_cm);
-  if (rc == MLOAM_OK) rc = frame_run(c, sw, have, parity, d_sm, n_surf_map, d_cm, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+  if (rc == MLOAM_OK && sw.host && rebuild_maps) rc = upload_submaps(c, surf_map, n_surf_map, corner_map, n_corner_map, &f.surf_map, &f.corner_map);
+  if (rc == MLOAM_OK) rc = frame_run(c, f, pose_out7, stats);
   c->maps_pending = false, c->next_pending = false, c->next.set = false;
   if (rc == MLOAM_OK) memcpy(c->last_pose7, pose_out7, sizeof(c->last_pose7)), c->frame_since_save = true;  // mloam_keyframe_save
-  c->reg_valid = rc == MLOAM_OK && c->reg_on;  // mloam_frame_registered
+  c->reg_valid = rc == MLOAM_OK && c->cfg.reg_on;  // mloam_frame_registered
   return rc;
 }
 
@@ -1119,8 +1111,8 @@ int mloam_set_front_end(mloam_ctx_t *h, int vertical_scans, int horizon_scans, d
   if (horizon_scans <= 0 || !(scan_period > 0.f)) return fail(c, MLOAM_E_INVALID, "set_front_end: horizon_scans and scan_period must be positive");
   if (c->params.max_ring_points > 0 && c->params.max_ring_points < horizon_scans)
     return fail(c, MLOAM_E_INVALID, "set_front_end: params.max_ring_points is below horizon_scans (a projected ring holds up to horizon_scans points)");
-  c->front = FrontEnd{vertical_scans, horizon_scans, roi_range, scan_period, time_field ? 1 : 0};
-  c->front_set = true;
+  c->cfg.front = FrontEnd{vertical_scans, horizon_scans, roi_range, scan_period, time_field ? 1 : 0};
+  c->cfg.front_set = true;
   c->prefetched.valid = false;  // look-ahead features were made with the previous front end
   return MLOAM_OK;
 }
@@ -1142,7 +1134,7 @@ int mloam_front_end(mloam_ctx_t *h, const mloam_point_t *h_raw, const int *h_cou
   MLOAM_CUDA_OK(c, carve(c->front_out, [&](Carve &cv) { d_out = cv.take<float4>((size_t)n + 1), d_meta = cv.take<int>(4 + 2 * (size_t)n_scans); }));
   cudaStream_t st = c->stream;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->sweep_in.p, h_raw, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, st));
-  const FrontEnd &fe = c->front;
+  const FrontEnd &fe = c->cfg.front;
   rc = project_cloud_device(c, c->sweep_in.as<float4>(), sw.L, fe.vertical_scans, fe.horizon_scans, fe.roi_range, &fe, d_out, d_meta + 4,
                             d_meta + 4 + n_scans, d_meta, c->front_work);
   if (rc) return rc;
@@ -1194,11 +1186,12 @@ int mloam_frame_set_next_raw_device(mloam_ctx_t *h, const mloam_point_t *d_raw, 
 int mloam_set_lidars(mloam_ctx_t *h, int n_lidars, const double *ext7) {
   if (!h || n_lidars < 1 || n_lidars > MLOAM_MAX_LIDARS || (n_lidars > 1 && !ext7)) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
-  c->n_lidars = n_lidars;
+  FrameCfg &f = c->cfg;
+  f.n_lidars = n_lidars;
   c->prefetched.valid = false;  // look-ahead features were merged with the previous extrinsics
-  c->lidar_merge = ext7 != nullptr;  // also for ONE LiDAR with an extrinsic: same float transform + laser id as in a rig
+  f.lidar_merge = ext7 != nullptr;  // also for ONE LiDAR with an extrinsic: same float transform + laser id as in a rig
   for (int l = 0; l < n_lidars; l++)
-    for (int k = 0; k < 7; k++) c->lidar_ext[l][k] = ext7 ? ext7[7 * l + k] : (k == 6 ? 1.0 : 0.0);
+    for (int k = 0; k < 7; k++) f.lidar_ext[l][k] = ext7 ? ext7[7 * l + k] : (k == 6 ? 1.0 : 0.0);
   return MLOAM_OK;
 }
 
@@ -1207,13 +1200,14 @@ int mloam_set_uncertainty(mloam_ctx_t *h, int with_ua, const double *ext_cov36, 
   if (!h) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
   if (with_ua && (!ext_cov36 || !cov_meas9)) return MLOAM_E_INVALID;
-  c->with_ua = with_ua ? 1 : 0;
+  FrameCfg &f = c->cfg;
+  f.with_ua = with_ua ? 1 : 0;
   if (!with_ua) return MLOAM_OK;
-  const int n_lasers = (c->n_lidars > 1 || c->lidar_merge) ? c->n_lidars : 1;
+  const int n_lasers = f.n_parts();
   for (int l = 0; l < MLOAM_MAX_LIDARS; l++)
-    for (int k = 0; k < 36; k++) c->ua_ext_cov[l][k] = l < n_lasers ? ext_cov36[36 * l + k] : 0.0;
-  memcpy(c->ua_cov_meas, cov_meas9, sizeof(c->ua_cov_meas));
-  c->ua_trace_threshold = trace_threshold;
+    for (int k = 0; k < 36; k++) f.ua_ext_cov[l][k] = l < n_lasers ? ext_cov36[36 * l + k] : 0.0;
+  memcpy(f.ua_cov_meas, cov_meas9, sizeof(f.ua_cov_meas));
+  f.ua_trace_threshold = trace_threshold;
   return MLOAM_OK;
 }
 
@@ -1221,10 +1215,10 @@ int mloam_set_uncertainty(mloam_ctx_t *h, int with_ua, const double *ext_cov36, 
 int mloam_set_outlier(mloam_ctx_t *h, float map_outlier_res) {
   if (!h || !(map_outlier_res >= 0.f) || map_outlier_res > 3.0e38f) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
-  if (c->nccl_comm || c->p2p_on)
+  if (multi_gpu(c))
     return fail(c, MLOAM_E_STATE, "set_outlier: the outlier cloud is single-GPU only, like with_ua; detach the communicator");
-  c->outlier_on = map_outlier_res > 0.f;
-  c->outlier_leaf = c->outlier_on ? map_outlier_res : 0.f;
+  c->cfg.outlier_on = map_outlier_res > 0.f;
+  c->cfg.outlier_leaf = c->cfg.outlier_on ? map_outlier_res : 0.f;
   return MLOAM_OK;
 }
 
@@ -1255,11 +1249,11 @@ int mloam_set_gf_float(mloam_ctx_t *h, int on, float map_deg_thre) {
   if (!h || (on && !(map_deg_thre == map_deg_thre))) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
   if (!on) {
-    c->gf_float_on = false;
+    c->cfg.gf_float_on = false;
     return MLOAM_OK;
   }
   if (c->params.gf_method != 3) return fail(c, MLOAM_E_STATE, "set_gf_float: gd_float is gd_fix with an adaptive ratio; set params.gf_method = 3 first");
-  if (c->nccl_comm || c->p2p_on)
+  if (multi_gpu(c))
     return fail(c, MLOAM_E_STATE, "set_gf_float: gd_float is single-GPU only (the 21 sums of sharded features are not exchanged); detach the communicator");
   cudaSetDevice(c->device);
   c->gf_float.in_graphs = false;  // allocated once, so the graphs that hold its address stay valid
@@ -1269,7 +1263,7 @@ int mloam_set_gf_float(mloam_ctx_t *h, int on, float map_deg_thre) {
   c->pinned->gf_float = c->gf_float_host;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(&c->gf_float.as<GfFloatDev>()->st, &c->pinned->gf_float, sizeof(GfFloatState), cudaMemcpyHostToDevice, c->stream));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
-  c->gf_float_on = true, c->gf_float_thre = map_deg_thre;
+  c->cfg.gf_float_on = true, c->cfg.gf_float_thre = map_deg_thre;
   c->gf_float_frames = 0, c->gf_float_eval = c->gf_float_evaluated = c->gf_float_reported = false;
   return MLOAM_OK;
 }
@@ -1277,15 +1271,15 @@ int mloam_set_gf_float(mloam_ctx_t *h, int on, float map_deg_thre) {
 int mloam_set_gf_float_threshold(mloam_ctx_t *h, float map_deg_thre) {
   if (!h || !(map_deg_thre == map_deg_thre)) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
-  if (!c->gf_float_on) return fail(c, MLOAM_E_STATE, "set_gf_float_threshold: gd_float is off (mloam_set_gf_float)");
-  c->gf_float_thre = map_deg_thre;
+  if (!c->cfg.gf_float_on) return fail(c, MLOAM_E_STATE, "set_gf_float_threshold: gd_float is off (mloam_set_gf_float)");
+  c->cfg.gf_float_thre = map_deg_thre;
   return MLOAM_OK;
 }
 
 int mloam_gf_float_report(mloam_ctx_t *h, double *ratio_cur, double *deg_factor, int *total_feat_num, int *evaluated_last_call, long long *frame_cnt) {
   if (!h) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
-  if (!c->gf_float_on) return fail(c, MLOAM_E_STATE, "gf_float_report: gd_float is off (mloam_set_gf_float)");
+  if (!c->cfg.gf_float_on) return fail(c, MLOAM_E_STATE, "gf_float_report: gd_float is off (mloam_set_gf_float)");
   if (!c->gf_float_reported) return fail(c, MLOAM_E_STATE, "gf_float_report: no solve call has run since gd_float was turned on");
   const GfFloatState &g = c->gf_float_host;
   if (ratio_cur) *ratio_cur = g.ratio_cur;
@@ -1340,9 +1334,9 @@ int mloam_frame_scan(mloam_ctx_t *h, mloam_point_t *h_surf, float *h_surf_cov6, 
 int mloam_set_extrinsic(mloam_ctx_t *h, const double *ext7) {
   if (!h) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
-  c->has_ext = ext7 != nullptr;
+  c->cfg.has_ext = ext7 != nullptr;
   c->prefetched.valid = false;
-  for (int k = 0; k < 7; k++) c->ext[k] = ext7 ? ext7[k] : (k == 6 ? 1.0 : 0.0);
+  for (int k = 0; k < 7; k++) c->cfg.ext[k] = ext7 ? ext7[k] : (k == 6 ? 1.0 : 0.0);
   return MLOAM_OK;
 }
 

@@ -114,7 +114,7 @@ int registered_count(Ctx *c, int which, int *m) {
   *m = 0;
   if (which < MLOAM_REGISTERED_FULL_RES || which > MLOAM_REGISTERED_CORNER)
     return fail(c, MLOAM_E_INVALID, "frame_registered: which must be MLOAM_REGISTERED_FULL_RES, _SURF or _CORNER");
-  if (c->nccl_comm || c->p2p_on) return fail(c, MLOAM_E_STATE, "frame_registered: the registered clouds are single-GPU only; detach the communicator");
+  if (multi_gpu(c)) return fail(c, MLOAM_E_STATE, "frame_registered: the registered clouds are single-GPU only; detach the communicator");
   if (!c->reg_valid)
     return fail(c, MLOAM_E_STATE, "frame_registered: the last call was no mloam_frame* call run with the registered clouds on (mloam_set_registered)");
   cudaSetDevice(c->device);
@@ -132,9 +132,9 @@ extern "C" {
 int mloam_set_registered(mloam_ctx_t *h, int on) {
   if (!h || (on != 0 && on != 1)) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
-  if (on && (c->nccl_comm || c->p2p_on))
+  if (on && multi_gpu(c))
     return fail(c, MLOAM_E_STATE, "set_registered: the registered clouds are single-GPU only, like with_ua; detach the communicator");
-  c->reg_on = on != 0;
+  c->cfg.reg_on = on != 0;
   return MLOAM_OK;
 }
 

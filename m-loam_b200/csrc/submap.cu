@@ -237,18 +237,18 @@ void fill_lasers(int n_lasers, const double *ext7, const double *pose_compound7,
 void ua_stage_host(Ctx *c) {
   UctFrame *f = &c->pinned->ua.frame;
   UctLaser *L = c->pinned->ua.lasers;
-  const bool merged = c->n_lidars > 1 || c->lidar_merge;
-  const int n_lasers = merged ? c->n_lidars : 1;
+  const FrameCfg &cfg = c->cfg;
+  const int n_lasers = cfg.n_parts();
   memset(f, 0, sizeof(*f));
   for (int k = 0; k < 7; k++) f->pose_global[k] = k == 6 ? 1.0 : 0.0;
-  memcpy(f->cov_meas, c->ua_cov_meas, sizeof(f->cov_meas));
-  f->trace_threshold = c->ua_trace_threshold, f->with_ua = 1, f->n_lasers = n_lasers, f->scan_frame = 1;
+  memcpy(f->cov_meas, cfg.ua_cov_meas, sizeof(f->cov_meas));
+  f->trace_threshold = cfg.ua_trace_threshold, f->with_ua = 1, f->n_lasers = n_lasers, f->scan_frame = 1;
   for (int l = 0; l < n_lasers; l++) {
     // pose_ext[idx]: the extrinsic the features were moved to the base frame with (identity when there is none)
-    const double *e = merged ? c->lidar_ext[l] : c->ext;
+    const double *e = cfg.part_ext(l);
     pose_inverse(e, L[l].ext_inv);
     for (int k = 0; k < 7; k++) L[l].compound[k] = e[k];
-    for (int k = 0; k < 36; k++) L[l].cov[k] = c->ua_ext_cov[l][k];
+    for (int k = 0; k < 36; k++) L[l].cov[k] = cfg.ua_ext_cov[l][k];
   }
 }
 
@@ -271,7 +271,6 @@ int ua_scan_stage(Ctx *c, Ctx::ScanRef *S, const UaStage **d_cfg_out) {
       out[t] = cv.take<float4>(N1), ocov6[t] = cv.take<float>(6 * N1), otrace[t] = cv.take<float>(N1), osinfo[t] = cv.take<double>(N1);
     }
   }));
-  ua_stage_host(c);
   if (d_cfg_out) *d_cfg_out = d_cfg;
   cudaStream_t st = c->stream;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_cfg, &c->pinned->ua, sizeof(UaStage), cudaMemcpyHostToDevice, st));
@@ -303,17 +302,9 @@ int ua_scan_stage(Ctx *c, Ctx::ScanRef *S, const UaStage **d_cfg_out) {
 void stage_outlier(Ctx *c) {
   OutlierStage *o = &c->pinned->outlier;
   memset(o, 0, sizeof(*o));
-  const bool merged = c->n_lidars > 1 || c->lidar_merge;
-  o->leaf = c->outlier_leaf, o->n_lasers = merged ? c->n_lidars : 1;
-  for (int l = 0; l < o->n_lasers; l++) {
-    // Pose(qbl, tbl).T_.cast<float>() (pose.cpp:34-41); in the single-LiDAR path the extrinsic of mloam_set_extrinsic, identity without one
-    const double *e = merged ? c->lidar_ext[l] : c->ext;
-    const M33 R = qmat(qnormalized(Q4{e[3], e[4], e[5], e[6]}));
-    for (int r = 0; r < 3; r++) {
-      for (int k = 0; k < 3; k++) o->mat[l][4 * r + k] = (float)R.m[3 * r + k];
-      o->mat[l][4 * r + 3] = (float)e[r];
-    }
-  }
+  o->leaf = c->cfg.outlier_leaf, o->n_lasers = c->cfg.n_parts();
+  // Pose(qbl, tbl).T_.cast<float>(); in the single-LiDAR path the extrinsic of mloam_set_extrinsic, identity without one
+  for (int l = 0; l < o->n_lasers; l++) pose_mat12(c->cfg.part_ext(l), o->mat[l]);
 }
 
 namespace {
@@ -418,7 +409,6 @@ int outlier_stage(Ctx *c, Ctx::ScanRef *S, const UaStage *d_ua) {
   MLOAM_CUDA_OK(c, carve(c->outlier, [&](Carve &cv) {
     d_cfg = cv.take<OutlierStage>(1), out = cv.take<float4>(MLOAM_MAX_LIDARS), cov6 = cv.take<float>(6 * MLOAM_MAX_LIDARS), cnt = cv.take<int>(16);
   }));
-  stage_outlier(c);
   cudaStream_t st = c->stream;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_cfg, &c->pinned->outlier, sizeof(OutlierStage), cudaMemcpyHostToDevice, st));
   k_outlier_scan<<<1, 32, 0, st>>>(S->first, S->first_ok, d_cfg, d_ua, out, cov6, cnt);
@@ -636,14 +626,7 @@ int mloam_local_map_build(mloam_ctx_t *h, int slot, int n_frames, const mloam_po
   if (n > 0 && !h_pts) return MLOAM_E_INVALID;
   cudaStream_t st = c->stream;
   std::vector<float> mats(12 * (size_t)(n_frames + 1), 0.f);
-  for (int k = 0; k < n_frames; k++) {  // Pose(Matrix4d) normalises the quaternion; T_.cast<float>()
-    const double *e = pose_local7 + 7 * (size_t)k;
-    const M33 R = qmat(qnormalized(Q4{e[3], e[4], e[5], e[6]}));
-    for (int r = 0; r < 3; r++) {
-      for (int q = 0; q < 3; q++) mats[12 * k + 4 * r + q] = (float)R.m[3 * r + q];
-      mats[12 * k + 4 * r + 3] = (float)e[r];
-    }
-  }
+  for (int k = 0; k < n_frames; k++) pose_mat12(pose_local7 + 7 * (size_t)k, &mats[12 * (size_t)k]);  // Pose(Matrix4d) normalises q
   const size_t N1 = (size_t)n + 16;
   float4 *d_in, *d_out;
   int *d_off, *d_cnt;

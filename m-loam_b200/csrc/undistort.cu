@@ -52,14 +52,13 @@ PoseD pose_mul(const PoseD &a, const PoseD &b) { return PoseD{qnormalized(qmul(a
 void stage_undistort(Ctx *c) {
   UndistStage *u = &c->pinned->undist;
   memset(u, 0, sizeof(*u));
-  u->scan_period = c->undist_scan_period, u->n_lidars = c->undist_n;
+  u->scan_period = c->cfg.undist_scan_period, u->n_lidars = c->undist_n;
   for (int l = 0; l < c->undist_n; l++) ud::undist_pose_make(c->undist_pose7[l], &u->pose[l]);
 }
 
 int undistort_stage(Ctx *c, ExtractOut out, int cap_less, int cap_flat, const int *d_off, int n_lidars) {
   UndistStage *d_cfg = nullptr;
   MLOAM_CUDA_OK(c, carve(c->undist, [&](Carve &cv) { d_cfg = cv.take<UndistStage>(1); }));
-  stage_undistort(c);
   ProfScope ps(c, "undistort");
   cudaStream_t st = c->stream;
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_cfg, &c->pinned->undist, sizeof(UndistStage), cudaMemcpyHostToDevice, st));
@@ -99,10 +98,10 @@ int mloam_undistort_poses(const double *pose_rlt7, int idx_ref, int n_lidars, co
 int mloam_set_distortion(mloam_ctx_t *h, int on, float scan_period) {
   if (!h || (on != 0 && on != 1) || (on && !(scan_period > 0.f && scan_period <= 3.0e38f))) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
-  if (c->nccl_comm || c->p2p_on)
+  if (multi_gpu(c))
     return fail(c, MLOAM_E_STATE, "set_distortion: the undistortion is single-GPU only, like with_ua; detach the communicator");
-  c->undist_on = on != 0;
-  if (on) c->undist_scan_period = scan_period;
+  c->cfg.undist_on = on != 0;
+  if (on) c->cfg.undist_scan_period = scan_period;
   c->undist_set = false;
   return MLOAM_OK;
 }
@@ -110,7 +109,7 @@ int mloam_set_distortion(mloam_ctx_t *h, int on, float scan_period) {
 int mloam_frame_undistort(mloam_ctx_t *h, int n_lidars, const double *pose7) {
   if (!h || !pose7 || n_lidars < 1 || n_lidars > MLOAM_MAX_LIDARS) return MLOAM_E_INVALID;
   Ctx *c = &h->c;
-  if (!c->undist_on) return fail(c, MLOAM_E_STATE, "frame_undistort: turn the undistortion on first (mloam_set_distortion)");
+  if (!c->cfg.undist_on) return fail(c, MLOAM_E_STATE, "frame_undistort: turn the undistortion on first (mloam_set_distortion)");
   for (int k = 0; k < 7 * n_lidars; k++)
     if (!std::isfinite(pose7[k])) return fail(c, MLOAM_E_INVALID, "frame_undistort: non-finite pose");
   memcpy(c->undist_pose7, pose7, sizeof(double) * 7 * (size_t)n_lidars);
