@@ -395,10 +395,25 @@ int mloam_frame_registered_device(mloam_ctx_t *ctx, int which, const mloam_point
  *   TransformToEnd(p, pose[n], true, SCAN_PERIOD) — s = (intensity - int(intensity)) / SCAN_PERIOD in float, Eigen's slerp from the
  *   identity, float stores — before the rig merge (or mloam_set_extrinsic's transform) and the scan filters: one more launch.  The sharp
  *   and flat clouds and the outlier cloud (mloam_set_outlier) are not moved.  With the look-ahead the announced sweep is extracted ahead
- *   and the rest runs at its call.  The poses are staged: a captured frame replays with new ones. */
+ *   and the rest runs at its call, unless its poses are announced with it (mloam_frame_set_next_undistort).  The poses are staged: a
+ *   captured frame replays with new ones.
+ * mloam_frame_set_next_undistort: the poses of the sweep announced by the last mloam_frame_set_next* call (any of the four), n_lidars x
+ *   [t q] as mloam_frame_undistort takes them for that sweep.  The look-ahead branch then runs the sweep's whole feature chain while the
+ *   coming frame is solved: front end, extraction, undistortion with these poses, rig merge or base-frame transform and both scan filters
+ *   (the with_ua gate and the outlier cloud stay with the call that takes the sweep).  Results do not change, only where the work runs.
+ *   - MLOAM_E_STATE: the undistortion is off, no sweep is announced, the announcement's poses were withdrawn (below), or a communicator
+ *     is attached.  MLOAM_E_INVALID: n_lidars is not the frame's LiDAR count (1 without the rig merge), or a value is not finite.
+ *   - Withdrawn with the sweep by a new mloam_frame_set_next*, and by mloam_set_lidars, mloam_set_params, mloam_set_front_end and
+ *     mloam_set_distortion (which also drop the features undistorted with them); after one of these, announce the sweep again.
+ *   - The mloam_frame* call that takes the announced sweep (the same pointer and sizes, as the look-ahead matches it) undistorts it with
+ *     these poses: it needs no mloam_frame_undistort.  Given one anyway, with the same bits the look-ahead's work is taken; with other bits
+ *     the sweep is extracted again at the call and undistorted with the call's poses, as after an announcement of the wrong sweep.
+ *   - A caller that never calls it sees no change.  mloam_profile_get(ctx, "undistort_ahead", ...) counts in `launches` the sweeps
+ *     undistorted by the look-ahead that a frame call then took. */
 int mloam_undistort_poses(const double *pose_rlt7, int idx_ref, int n_lidars, const double *ext7s, int estimate_extrinsic, double *out7s);
 int mloam_set_distortion(mloam_ctx_t *ctx, int on, float scan_period);
 int mloam_frame_undistort(mloam_ctx_t *ctx, int n_lidars, const double *pose7);
+int mloam_frame_set_next_undistort(mloam_ctx_t *ctx, int n_lidars, const double *pose7);
 
 /* ---- the mapper's keyframe store, kept on the device: saveKeyframe -> clearCloud -> extractSurroundingKeyFrames
  *      (lidar_mapper_keyframe.cpp:641-683, :921-927 at :1101, :254-354).  The mapper loop of process() (:1062-1101) becomes

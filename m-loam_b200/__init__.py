@@ -37,7 +37,7 @@ ABI_SYMBOLS = [
     "mloam_global_map", "mloam_global_map_read", "mloam_global_map_chosen",
     "mloam_cal_timestamp", "mloam_set_front_end", "mloam_front_end", "mloam_frame_raw", "mloam_frame_raw_device", "mloam_frame_set_next_raw",
     "mloam_frame_set_next_raw_device", "mloam_set_outlier", "mloam_frame_outlier", "mloam_keyframe_outlier",
-    "mloam_undistort_poses", "mloam_set_distortion", "mloam_frame_undistort",
+    "mloam_undistort_poses", "mloam_set_distortion", "mloam_frame_undistort", "mloam_frame_set_next_undistort",
     "mloam_full_hessian", "mloam_set_gf_float", "mloam_set_gf_float_threshold", "mloam_gf_float_report",
     "mloam_set_registered", "mloam_frame_registered", "mloam_frame_registered_device",
 ]
@@ -649,6 +649,12 @@ class Context:
         """The per-LiDAR pose_undist [n_lidars, 7] ([t q], as undistort_poses returns it) of the sweep of the next frame call."""
         p = np.ascontiguousarray(pose7s, np.float64).reshape(-1, 7)
         self._ck(lib().mloam_frame_undistort(self._h, p.shape[0], _p(p)))
+
+    def frame_set_next_undistort(self, pose7s):
+        """The per-LiDAR pose_undist [n_lidars, 7] of the sweep announced by the last frame_set_next* call: the look-ahead then undistorts,
+        merges and down-samples it while the coming frame is solved, and the call that takes it needs no frame_undistort."""
+        p = np.ascontiguousarray(pose7s, np.float64).reshape(-1, 7)
+        self._ck(lib().mloam_frame_set_next_undistort(self._h, p.shape[0], _p(p)))
 
     def set_outlier(self, map_outlier_res: float):
         """The outlier cloud of segment_cloud: 0 (mloam_set_outlier): leaf MAP_OUTLIER_RES > 0 turns it on, 0 off.  Call after set_lidars."""

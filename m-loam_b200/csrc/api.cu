@@ -170,6 +170,7 @@ int mloam_set_params(mloam_ctx_t *h, const mloam_params_t *p) {
   if (p->n_neigh != 5 && p->n_neigh != 10) return fail(&h->c, MLOAM_E_INVALID, "n_neigh must be 5 or 10");
   h->c.params = *p;
   h->c.prefetched.valid = false;  // look-ahead features were extracted under the previous parameters
+  undist_withdraw(&h->c);
   return MLOAM_OK;
 }
 
@@ -209,6 +210,11 @@ int mloam_profile_get(mloam_ctx_t *h, const char *name, double *ms_total, long l
   if (!strcmp(name, "graph_captures")) {  // frame graphs captured and instantiated so far
     if (ms_total) *ms_total = 0.0;
     if (launches) *launches = c->graph_captures;
+    return MLOAM_OK;
+  }
+  if (!strcmp(name, "undistort_ahead")) {  // sweeps undistorted in the look-ahead branch and taken by their frame call so far
+    if (ms_total) *ms_total = 0.0;
+    if (launches) *launches = c->undist_ahead_taken;
     return MLOAM_OK;
   }
   // query counts / SM cycles of the matcher's search paths (k_match_knn), reported through `launches`

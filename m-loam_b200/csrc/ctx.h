@@ -1,6 +1,7 @@
 // ctx.h — host-side context behind the C ABI (include/mloam_b200.h) and the kernel launchers.
 #pragma once
 #include <cuda_runtime.h>
+#include <cstring>
 #include <map>
 #include <string>
 #include <vector>
@@ -206,7 +207,14 @@ struct OutlierStage {
   int pad[2];
   float mat[MLOAM_MAX_LIDARS][12];   // per LiDAR the float 3x4 extrinsic of pubPointCloud's transformPointCloud (identity without one)
 };
-// the configuration of a frame's undistortion (mloam_set_distortion / mloam_frame_undistort; undistort.cu), copied to the device as one block
+// The per-LiDAR pose_undist of one sweep as the caller gave it (mloam_frame_undistort, mloam_frame_set_next_undistort); n == 0: none
+struct UndistPoses {
+  int n = 0;
+  double pose7[MLOAM_MAX_LIDARS][7];
+  bool same_bits(const UndistPoses &o) const { return n == o.n && std::memcmp(pose7, o.pose7, sizeof(double) * 7 * (size_t)n) == 0; }
+};
+// the configuration of a sweep's undistortion (mloam_set_distortion / mloam_frame_undistort; undistort.cu), copied to the device as one block
+// per half of the feature double buffer
 struct UndistStage {
   float scan_period;                       // SCAN_PERIOD
   int n_lidars;                            // staged poses (the frame's LiDARs; 1 in the single-LiDAR path)
@@ -246,7 +254,7 @@ struct PinnedBlock {
   float rig[MLOAM_MAX_LIDARS][12];  // features_enqueue: the rig's float 3x4 extrinsics of the merge
   UaStage ua;                       // ua_scan_stage: the with_ua configuration
   OutlierStage outlier;             // outlier_stage: the outlier cloud's configuration
-  UndistStage undist;               // undistort_stage: the sweep's poses
+  UndistStage undist[2];            // undistort_stage: per half of the feature double buffer, the poses of the sweep in that half
   // Written by captured copies (landing of a frame's results) and by the host-buffer entry points, one call at a time
   LMState lm;                       // LMState mirror
   int counts[192];                  // count read-backs; mloam_project_cloud: [0] count, [64..] scan starts, [128..] scan ends
@@ -441,10 +449,20 @@ struct Ctx {
     bool extract_only = false;  // the undistortion was on: the half holds the extraction only (undistortion, merge and the scan
                                 // filters run at the frame call, which knows the sweep's pose)
     bool registered = false;    // the registered clouds were on: the half also holds the sweep itself (FrameBufs::reg_sweep)
+    UndistPoses undist;         // n > 0: the undistortion was on and the look-ahead ran it too, with these poses (the sweep's announced
+                                // ones); a call takes the half only with the same bits
   };
   struct NextSweep {
     bool set = false;
     Sweep sw;                   // a host sweep's device buffers are set when its copy is enqueued (pipeline.cu stage_next_sweep)
+    bool undist_open = false;   // mloam_frame_set_next_undistort may still give its poses: no setter has withdrawn them since
+    UndistPoses undist;         // ... and the poses it gave
+  };
+  // The sweep announced with the last mloam_frame* call and its poses (mloam_frame_set_next_undistort): the call that takes that sweep
+  // undistorts it with them unless it gives its own (mloam_frame_undistort).  Consumed by the next mloam_frame* call.
+  struct AnnouncedPoses {
+    Sweep sw;
+    UndistPoses undist;
   };
   // A frame's results on the host, applied by pipeline.cu frame_commit on the stream, capture and replay paths alike
   struct FrameOutcome {
@@ -532,7 +550,9 @@ struct Ctx {
   bool undist_set = false;         // a pose was given for the next mloam_frame* call
   int undist_n = 0;
   double undist_pose7[MLOAM_MAX_LIDARS][7];
-  DevBuf undist;                   // the staged configuration
+  DevBuf undist;                   // the staged configuration, one UndistStage per half of the feature double buffer
+  AnnouncedPoses undist_announced;  // the poses announced with the sweep of the last call's look-ahead, for the call that takes it
+  long long undist_ahead_taken = 0;  // sweeps undistorted by the look-ahead and taken by their frame call (mloam_profile_get "undistort_ahead")
   // gd_float (FrameCfg::gf_float_on): every 10th solve call that passes the map gate evaluates the full information matrix of the scan
   // (evalFullHessian) from the Jacobian rows of outer iteration 0 and sets the ratio k_gf_select reads from GfFloatDev.  Allocated once,
   // outside alloc_epoch(): turning the mode on re-captures nothing.  MAP_DEG_THRE and gf_ratio_ini are staged (PinnedBlock::gf_float_cfg).
@@ -723,8 +743,13 @@ int extract_device(Ctx *c, const float4 *d_cloud, int n, const int *d_scan_start
 // undistort.cu: TransformToEnd in place of the extraction's less-sharp (capacity cap_less, count out.counts[1]) and less-flat (cap_flat,
 // out.counts[3]) features on c->stream, LiDAR l's with the staged pose l; d_off (nullable, the rig's per-LiDAR offsets of the two clouds,
 // 2 x (n_lidars + 1)) finds a point's LiDAR, without it every point is LiDAR 0's.  One launch.  stage_undistort stages its configuration.
-int undistort_stage(Ctx *c, ExtractOut out, int cap_less, int cap_flat, const int *d_off, int n_lidars);
-void stage_undistort(Ctx *c);
+// parity: the half of the feature double buffer the features are in; its UndistStage is copied and read.
+int undistort_stage(Ctx *c, int parity, ExtractOut out, int cap_less, int cap_flat, const int *d_off, int n_lidars);
+// PinnedBlock::undist[parity] <- the poses of this call (Ctx::undist_pose7); with `ahead`, undist[parity ^ 1] <- the announced sweep's
+void stage_undistort(Ctx *c, int parity, const UndistPoses *ahead);
+// mloam_set_lidars / _params / _front_end / _distortion: the announced sweep's poses are withdrawn, and so are the features the
+// look-ahead undistorted with them
+void undist_withdraw(Ctx *c);
 // extract_device's work in Ctx::extract_work for n points in n_scans rings
 struct RingStage;
 struct ExtractWork {

@@ -315,11 +315,31 @@ namespace {
 // capacity of a frame's less-sharp features: <= 20 picks x 6 sectors per ring
 int less_sharp_cap(int n, int n_scans) { return n < 120 * n_scans ? n : 120 * n_scans; }
 
+// The poses the look-ahead branch undistorts the announced sweep with (mloam_frame_set_next_undistort), or nullptr: the branch does not
+// run, or it extracts only and the undistortion, merge and scan filters wait for the call that takes the sweep
+const UndistPoses *undist_ahead(const Ctx *c) {
+  return c->cfg.undist_on && c->next.set && c->next.undist.n > 0 && c->use_lookahead && !c->prof_on ? &c->next.undist : nullptr;
+}
+
+// One mloam_frame* call as frame_call hands it on.  have: the previous frame's look-ahead made the sweep's features, in half `parity`;
+// else they are extracted now into that half.  take_undist: they are complete although the undistortion is on (the look-ahead ran it
+// with the poses of mloam_frame_set_next_undistort).  The submaps are on the device.
+struct FrameCall {
+  Sweep sw;
+  bool have;
+  int parity;
+  const float4 *surf_map, *corner_map;
+  int n_surf_map, n_corner_map, rebuild_maps;
+  const double *pose_init7;
+  bool take_undist;
+};
+
 // The pinned inputs of a frame (PinnedBlock), from Ctx::cfg and the pose guess: written once before the frame is enqueued and before
-// every replay of its graph, whose captured copies read them at execution time.  The stages only copy them.
-void stage_frame_inputs(Ctx *c, const double *pose7) {
+// every replay of its graph, whose captured copies read them at execution time.  The stages only copy them.  The undistortion's poses
+// are staged per half: this sweep's into its half, the announced sweep's into the other one when the look-ahead undistorts it.
+void stage_frame_inputs(Ctx *c, const FrameCall &fc) {
   const FrameCfg &f = c->cfg;
-  stage_pose(c, pose7);
+  stage_pose(c, fc.pose_init7);
   if (f.rig_merge()) {
     for (int l = 0; l < f.n_lidars; l++) pose_mat12(f.lidar_ext[l], c->pinned->rig[l]);
   } else if (f.has_ext) {
@@ -327,17 +347,25 @@ void stage_frame_inputs(Ctx *c, const double *pose7) {
   }
   if (f.with_ua) ua_stage_host(c);
   if (f.outlier_on) stage_outlier(c);
-  if (f.undist_on) stage_undistort(c);
+  if (f.undist_on) stage_undistort(c, fc.parity, undist_ahead(c));
   if (f.gf_float_on) stage_gf_float(c);
 }
 
-// Whether the look-ahead of the previous frame made the features of sw: same caller pointer and sizes; a raw sweep's features are taken by
-// a raw frame with the same per-LiDAR counts only, a ring-ordered sweep's by a ring-ordered frame, and a host frame takes a host announcement
+// Whether sweep sw is the announced sweep a: same caller pointer and sizes; a raw sweep is taken by a raw frame with the same per-LiDAR
+// counts only, a ring-ordered sweep by a ring-ordered frame, and a host frame takes a host announcement
+bool same_sweep(const Sweep &a, const Sweep &sw) {
+  const bool same_kind = sw.raw ? (a.raw && std::memcmp(&a.L, &sw.L, sizeof(RigLayout)) == 0) : !a.raw;
+  return a.key == sw.key && a.n == sw.n && a.n_scans == sw.n_scans && same_kind && (a.host || !sw.host);
+}
+
+// Whether the look-ahead of the previous frame made the features of sw.  With the undistortion on they are the extraction only, or
+// complete when the look-ahead undistorted with the very bits this call undistorts with (Ctx::undist_pose7, set by frame_call).
 bool frame_has_prefetched(const Ctx *c, const Sweep &sw) {
   const Ctx::Features &f = c->prefetched;
-  const bool same_kind = sw.raw ? (f.sw.raw && std::memcmp(&f.sw.L, &sw.L, sizeof(RigLayout)) == 0) : !f.sw.raw;
-  return f.valid && c->use_lookahead && !c->prof_on && f.sw.key == sw.key && f.sw.n == sw.n && f.sw.n_scans == sw.n_scans && same_kind &&
-         (f.sw.host || !sw.host) && f.extract_only == c->cfg.undist_on && (f.registered || !c->cfg.reg_on);
+  UndistPoses call;
+  if (c->cfg.undist_on && f.undist.n > 0) call.n = c->undist_n, std::memcpy(call.pose7, c->undist_pose7, sizeof(double) * 7 * (size_t)call.n);
+  const bool undist_ok = !c->cfg.undist_on ? !f.extract_only && f.undist.n == 0 : f.extract_only || (f.undist.n > 0 && f.undist.same_bits(call));
+  return f.valid && c->use_lookahead && !c->prof_on && same_sweep(f.sw, sw) && undist_ok && (f.registered || !c->cfg.reg_on);
 }
 
 // extractCloud of sweep sw on c->stream into half `parity` of the feature double buffer (*F), with the LiDARs' first points and, for the
@@ -386,9 +414,9 @@ int extract_enqueue(Ctx *c, const Sweep &sw, int parity, FrameBufs *F_out) {
   return MLOAM_OK;
 }
 
-// [undistortion] + (multi-LiDAR merge | base-frame transform) + downsampleCurrentScan of the features extract_enqueue left in F, on
-// c->stream; the corner filter forks onto branch `side`.
-int scan_enqueue(Ctx *c, const Sweep &sw, const FrameBufs &F, const Branch &side, ScanRef *S_out) {
+// [undistortion] + (multi-LiDAR merge | base-frame transform) + downsampleCurrentScan of the features extract_enqueue left in F (half
+// `parity`), on c->stream; the corner filter forks onto branch `side`.
+int scan_enqueue(Ctx *c, const Sweep &sw, const FrameBufs &F, int parity, const Branch &side, ScanRef *S_out) {
   const mloam_params_t &P = c->params;
   const FrameCfg &cfg = c->cfg;
   const int n = sw.n, n_scans = sw.n_scans;
@@ -396,7 +424,7 @@ int scan_enqueue(Ctx *c, const Sweep &sw, const FrameBufs &F, const Branch &side
   const int less_cap = less_sharp_cap(n, n_scans);
   DevCtl *ctl = c->ctl.as<DevCtl>();
   if (cfg.undist_on) {  // undistortMeasurements (estimator.cpp:376-408): each LiDAR's less-* features in its own frame, before the merge
-    rc = undistort_stage(c, F.ex, less_cap, n, cfg.rig_merge() ? F.off : nullptr, cfg.n_parts());
+    rc = undistort_stage(c, parity, F.ex, less_cap, n, cfg.rig_merge() ? F.off : nullptr, cfg.n_parts());
     if (rc) return rc;
     stamp(c, "undistort");
   }
@@ -437,7 +465,7 @@ int features_enqueue(Ctx *c, const Sweep &sw, int parity, const Branch &side, Sc
   FrameBufs F;
   int rc = extract_enqueue(c, sw, parity, &F);
   if (rc) return rc;
-  return scan_enqueue(c, sw, F, side, S_out);
+  return scan_enqueue(c, sw, F, parity, side, S_out);
 }
 
 // mloam_frame copied inputs on a branch's stream outside of any capture, recorded in ev.  Run on that branch (forked), the stream path is
@@ -452,17 +480,6 @@ int wait_uploads(Ctx *c, cudaEvent_t ev, bool forked) {
   if (cs == cudaStreamCaptureStatusActive) MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream, ev, cudaEventWaitExternal));
   return MLOAM_OK;
 }
-
-// One mloam_frame* call as frame_call hands it on.  have: the previous frame's look-ahead made the sweep's features, in half `parity`;
-// else they are extracted now into that half.  The submaps are on the device.
-struct FrameCall {
-  Sweep sw;
-  bool have;
-  int parity;
-  const float4 *surf_map, *corner_map;
-  int n_surf_map, n_corner_map, rebuild_maps;
-  const double *pose_init7;
-};
 
 // pubPointCloud of sweep sw, whose features and copy are in half `parity`, on c->stream after the solve: k_registered at pose_wmap_curr,
 // LMState::x when the solve ran (ran), else the staged initial pose (the map gate keeps it, lidar_mapper_keyframe.cpp:429, :634-638)
@@ -483,7 +500,7 @@ int registered_enqueue(Ctx *c, const Sweep &sw, int parity, int ran, RegOut *out
   a.sweep = F.reg_sweep, a.n_sweep = sw.n, a.d_n_sweep = sw.raw ? F.reg_meta : nullptr, a.scan_start = F.reg_meta + 16;
   a.n_parts = c->cfg.n_parts(), a.rings_per_lidar = sw.n_scans / a.n_parts;
   a.to_base = c->cfg.rig_merge() ? 1 : (c->cfg.has_ext ? 2 : 0), a.rig = &ctl->rig[0][0], a.ext = ctl->ext;  // as scan_enqueue copied them
-  a.undist = c->cfg.undist_on ? c->undist.as<UndistStage>() : nullptr;  // undistort_stage's configuration
+  a.undist = c->cfg.undist_on ? c->undist.as<UndistStage>() + parity : nullptr;  // undistort_stage's configuration of this sweep's half
   if (c->cfg.outlier_on) a.first = F.first, a.first_ok = F.first_ok, a.outlier = c->outlier.as<OutlierStage>();  // outlier_stage's
   a.less_flat = F.ex.less_flat, a.less_sharp = F.ex.less_sharp, a.cap_flat = sw.n, a.cap_sharp = less_cap;
   a.n_flat = F.ex.counts + 3, a.n_sharp = F.ex.counts + 1, a.pose = d_pose;
@@ -501,7 +518,7 @@ int frame_enqueue(Ctx *c, const FrameCall &f, Ctx::FrameOutcome *o) {
   const FrameCfg &cfg = c->cfg;
   const Sweep &sw = f.sw;
   *o = Ctx::FrameOutcome{};
-  stage_frame_inputs(c, f.pose_init7);
+  stage_frame_inputs(c, f);
   // lidar_mapper_keyframe.cpp:433-434 (every frame in the reference).  The two submap builds do not depend on the sweep: they run on a
   // forked side stream, concurrently with extraction + scan down-sampling, and join right before matching (also inside a captured graph).
   // With stage profiling on the branch stays on the main stream so that per-stage event times do not overlap.
@@ -528,20 +545,23 @@ int frame_enqueue(Ctx *c, const FrameCall &f, Ctx::FrameOutcome *o) {
     FrameBufs F;
     rc = frame_bufs(c, sw.n, &F, f.parity, cfg.reg_on ? sw.n_scans : 0);
     F.ex.first = F.first, F.ex.first_ok = F.first_ok;  // recorded by the look-ahead's extraction (extract_enqueue)
-    if (rc == MLOAM_OK) rc = scan_enqueue(c, sw, F, c->br_scan, &S);
+    if (rc == MLOAM_OK) rc = scan_enqueue(c, sw, F, f.parity, c->br_scan, &S);
     if (rc) return rc;
   }
   // look-ahead: the announced next sweep goes through the same steps on br_ahead into the other half while this frame is matched
   // and solved (it reuses Ctx::extract_work, voxel_corner and voxel_surf of the block above, hence the fork AFTER it).  With the
-  // undistortion on, the next sweep's pose comes with the next call: the branch extracts only (extract_work), and that call runs
-  // undistortion, merge and the scan filters on the main stream before it forks its own look-ahead.
+  // undistortion on, the branch needs the next sweep's poses: announced with it (mloam_frame_set_next_undistort), it runs every step
+  // with them, staged in the other half's UndistStage; else they come with the next call, the branch extracts only (extract_work),
+  // and that call runs undistortion, merge and the scan filters on the main stream before it forks its own look-ahead.
   Ctx::Features &nf = o->next;
   if (c->next.set && c->use_lookahead && !c->prof_on) {
     const Sweep &nx = c->next.sw;
+    const UndistPoses *nx_undist = undist_ahead(c);
+    const bool extract_only = cfg.undist_on && !nx_undist;
     c->stamp_mute = true;
     rc = on_branch(c, c->br_ahead, true, [&] {
       int r = c->next_pending ? wait_uploads(c, c->ev_next, true) : MLOAM_OK;  // mloam_frame copied the next sweep on br_ahead
-      if (r == MLOAM_OK && cfg.undist_on) {
+      if (r == MLOAM_OK && extract_only) {
         FrameBufs F;
         r = extract_enqueue(c, nx, f.parity ^ 1, &F);
       } else if (r == MLOAM_OK) {
@@ -551,7 +571,8 @@ int frame_enqueue(Ctx *c, const FrameCall &f, Ctx::FrameOutcome *o) {
     });
     c->stamp_mute = false;
     if (rc) return rc;
-    nf.valid = true, nf.parity = f.parity ^ 1, nf.sw = nx, nf.extract_only = cfg.undist_on, nf.registered = cfg.reg_on;
+    nf.valid = true, nf.parity = f.parity ^ 1, nf.sw = nx, nf.extract_only = extract_only, nf.registered = cfg.reg_on;
+    if (nx_undist) nf.undist = *nx_undist;
   }
   stamp(c, f.have ? "features (prefetched)" : "extract + voxel");
   const UaStage *d_ua = nullptr;
@@ -586,6 +607,8 @@ int frame_enqueue(Ctx *c, const FrameCall &f, Ctx::FrameOutcome *o) {
 void frame_commit(Ctx *c, int parity, const Ctx::FrameOutcome &o) {
   c->frame_parity = parity ^ 1;
   c->prefetched = o.next;
+  // the poses the look-ahead undistorted with are staged, not captured: a replay's are the ones announced for it (same key: announced)
+  if (c->prefetched.undist.n > 0) c->prefetched.undist = c->next.undist;
   c->last_scan = o.S, c->last_scan_valid = true;
   c->reg_last = o.reg;
   c->gf_float_evaluated = o.gf_evaluated;
@@ -688,6 +711,10 @@ unsigned long long frame_key(Ctx *c, const FrameCall &f) {
   }
   unsigned long long h = 1469598103934665603ull, w;  // FNV-1a over 8-byte words: the key is built on the frame's host critical path
   for (size_t i = 0; i < sizeof(k); i += 8) memcpy(&w, reinterpret_cast<const char *>(&k) + i, 8), h = (h ^ w) * 1099511628211ull;
+  // the undistortion in the look-ahead branch, and a call that takes a sweep undistorted there (mloam_frame_set_next_undistort): one
+  // more word, only when either is on, so that the keys of a context that never announces poses are the ones it had without them
+  w = (undist_ahead(c) ? 1ull : 0ull) | (f.take_undist ? 2ull : 0ull);
+  if (w) h = (h ^ w) * 1099511628211ull;
   return h;
 }
 
@@ -754,7 +781,7 @@ int frame_run(Ctx *c, const FrameCall &f, double *pose_out7, mloam_solve_stats_t
       c->graphs.push_back(g);
     }
     if (e && e->exec && e->epoch == alloc_epoch()) {
-      stage_frame_inputs(c, f.pose_init7);  // the captured H2D nodes read them at execution time
+      stage_frame_inputs(c, f);  // the captured H2D nodes read them at execution time
       MLOAM_CUDA_OK(c, cudaGraphLaunch(e->exec, c->stream));
       c->frame_from_graph = true;
       c->launches += e->launches;
@@ -830,22 +857,32 @@ int frame_call(Ctx *c, Sweep sw, const mloam_point_t *surf_map, int n_surf_map, 
                int rebuild_maps, const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
   c->reg_valid = false;
   if (sw.host && rebuild_maps && (!surf_map || !corner_map || n_surf_map < 0 || n_corner_map < 0)) return MLOAM_E_INVALID;
-  if (c->cfg.undist_on) {  // the sweep's pose_undist (mloam_frame_undistort), consumed by this call whatever it returns
-    const bool set = c->undist_set;
+  // the poses announced with this sweep (mloam_frame_set_next_undistort), consumed by this call whatever it returns
+  const Ctx::AnnouncedPoses ann = c->undist_announced;
+  c->undist_announced.undist.n = 0;
+  if (c->cfg.undist_on) {  // the sweep's pose_undist (mloam_frame_undistort, else the announced one), consumed by this call whatever it returns
+    bool set = c->undist_set;
     c->undist_set = false;
+    if (!set && ann.undist.n > 0 && same_sweep(ann.sw, sw)) {
+      std::memcpy(c->undist_pose7, ann.undist.pose7, sizeof(double) * 7 * (size_t)ann.undist.n);
+      c->undist_n = ann.undist.n, set = true;
+    }
     if (!set) return fail(c, MLOAM_E_STATE, "frame: the undistortion is on and no pose was given for this sweep (mloam_frame_undistort)");
     if (c->undist_n != c->cfg.n_parts())
       return fail(c, MLOAM_E_INVALID, "frame: mloam_frame_undistort gave a pose count other than the frame's LiDARs (1 without the rig merge)");
   }
   cudaSetDevice(c->device);
   // this sweep's features: extracted while the previous frame was solved (look-ahead), or now into the half after the previous frame's
-  FrameCall f{sw, frame_has_prefetched(c, sw), 0, nullptr, nullptr, n_surf_map, n_corner_map, rebuild_maps, pose_init7};
+  FrameCall f{sw, frame_has_prefetched(c, sw), 0, nullptr, nullptr, n_surf_map, n_corner_map, rebuild_maps, pose_init7, false};
   f.parity = f.have ? c->prefetched.parity : c->frame_parity;
+  f.take_undist = f.have && c->cfg.undist_on && !c->prefetched.extract_only;
   if (!sw.host) f.surf_map = reinterpret_cast<const float4 *>(surf_map), f.corner_map = reinterpret_cast<const float4 *>(corner_map);
   int rc = sw.host ? sweep_to_device(c, c->sweep_in, &f.sw, !f.have, c->pinned->scan_info, c->stream) : MLOAM_OK;
   if (rc == MLOAM_OK) rc = stage_next_sweep(c);
   if (rc == MLOAM_OK && sw.host && rebuild_maps) rc = upload_submaps(c, surf_map, n_surf_map, corner_map, n_corner_map, &f.surf_map, &f.corner_map);
   if (rc == MLOAM_OK) rc = frame_run(c, f, pose_out7, stats);
+  if (rc == MLOAM_OK && f.take_undist) c->undist_ahead_taken++;
+  if (c->next.set && c->next.undist.n > 0) c->undist_announced = Ctx::AnnouncedPoses{c->next.sw, c->next.undist};
   c->maps_pending = false, c->next_pending = false, c->next.set = false;
   if (rc == MLOAM_OK) memcpy(c->last_pose7, pose_out7, sizeof(c->last_pose7)), c->frame_since_save = true;  // mloam_keyframe_save
   c->reg_valid = rc == MLOAM_OK && c->cfg.reg_on;  // mloam_frame_registered
@@ -856,7 +893,7 @@ int frame_call(Ctx *c, Sweep sw, const mloam_point_t *surf_map, int n_surf_map, 
 // failed or sw is empty (a withdrawal) — is announced for the next frame
 int announce(Ctx *c, const Sweep &sw, int rc) {
   c->next = Ctx::NextSweep{};
-  if (rc == MLOAM_OK && sw.key) c->next.set = true, c->next.sw = sw;
+  if (rc == MLOAM_OK && sw.key) c->next.set = true, c->next.sw = sw, c->next.undist_open = true;
   return rc;
 }
 
@@ -1114,6 +1151,7 @@ int mloam_set_front_end(mloam_ctx_t *h, int vertical_scans, int horizon_scans, d
   c->cfg.front = FrontEnd{vertical_scans, horizon_scans, roi_range, scan_period, time_field ? 1 : 0};
   c->cfg.front_set = true;
   c->prefetched.valid = false;  // look-ahead features were made with the previous front end
+  undist_withdraw(c);
   return MLOAM_OK;
 }
 
@@ -1189,6 +1227,7 @@ int mloam_set_lidars(mloam_ctx_t *h, int n_lidars, const double *ext7) {
   FrameCfg &f = c->cfg;
   f.n_lidars = n_lidars;
   c->prefetched.valid = false;  // look-ahead features were merged with the previous extrinsics
+  undist_withdraw(c);           // ... and the announced poses may be of another count
   f.lidar_merge = ext7 != nullptr;  // also for ONE LiDAR with an extrinsic: same float transform + laser id as in a rig
   for (int l = 0; l < n_lidars; l++)
     for (int k = 0; k < 7; k++) f.lidar_ext[l][k] = ext7 ? ext7[7 * l + k] : (k == 6 ? 1.0 : 0.0);

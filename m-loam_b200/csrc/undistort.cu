@@ -4,6 +4,8 @@
 //                           LiDAR's features move with (ESTIMATE_EXTRINSIC == 2: its own; otherwise IDX_REF's, :403-405) — host only
 //   mloam_set_distortion    on / off and SCAN_PERIOD
 //   mloam_frame_undistort   the per-LiDAR poses of the sweep of the next mloam_frame* call
+//   mloam_frame_set_next_undistort   the poses of the sweep announced for the look-ahead (mloam_frame_set_next*), so that the branch
+//                           undistorts, merges and down-samples it too
 //   k_undistort             TransformToEnd of the less-sharp and less-flat features of every LiDAR, in the LiDAR's frame, between the
 //                           extraction and the rig merge (the reference undistorts cur_feature_ before the mapper sees it; the sharp and
 //                           flat clouds and the outlier cloud are left as they are, and so is what the tracker kept in prev_feature_)
@@ -49,19 +51,31 @@ PoseD pose_mul(const PoseD &a, const PoseD &b) { return PoseD{qnormalized(qmul(a
 
 }  // namespace
 
-void stage_undistort(Ctx *c) {
-  UndistStage *u = &c->pinned->undist;
+namespace {
+void stage_poses(Ctx *c, int n, const double (*pose7)[7], UndistStage *u) {
   memset(u, 0, sizeof(*u));
-  u->scan_period = c->cfg.undist_scan_period, u->n_lidars = c->undist_n;
-  for (int l = 0; l < c->undist_n; l++) ud::undist_pose_make(c->undist_pose7[l], &u->pose[l]);
+  u->scan_period = c->cfg.undist_scan_period, u->n_lidars = n;
+  for (int l = 0; l < n; l++) ud::undist_pose_make(pose7[l], &u->pose[l]);
+}
+}  // namespace
+
+void stage_undistort(Ctx *c, int parity, const UndistPoses *ahead) {
+  stage_poses(c, c->undist_n, c->undist_pose7, &c->pinned->undist[parity]);
+  if (ahead) stage_poses(c, ahead->n, ahead->pose7, &c->pinned->undist[parity ^ 1]);
 }
 
-int undistort_stage(Ctx *c, ExtractOut out, int cap_less, int cap_flat, const int *d_off, int n_lidars) {
+void undist_withdraw(Ctx *c) {
+  c->next.undist_open = false, c->next.undist.n = 0;
+  c->undist_announced.undist.n = 0;
+  if (c->prefetched.undist.n) c->prefetched.valid = false;
+}
+
+int undistort_stage(Ctx *c, int parity, ExtractOut out, int cap_less, int cap_flat, const int *d_off, int n_lidars) {
   UndistStage *d_cfg = nullptr;
-  MLOAM_CUDA_OK(c, carve(c->undist, [&](Carve &cv) { d_cfg = cv.take<UndistStage>(1); }));
+  MLOAM_CUDA_OK(c, carve(c->undist, [&](Carve &cv) { d_cfg = cv.take<UndistStage>(2) + parity; }));
   ProfScope ps(c, "undistort");
   cudaStream_t st = c->stream;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_cfg, &c->pinned->undist, sizeof(UndistStage), cudaMemcpyHostToDevice, st));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_cfg, &c->pinned->undist[parity], sizeof(UndistStage), cudaMemcpyHostToDevice, st));
   const long long total = (long long)cap_less + cap_flat;
   if (total <= 0) return MLOAM_OK;
   k_undistort<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(out.less_sharp, cap_less, out.counts + 1, out.less_flat, cap_flat, out.counts + 3,
@@ -103,6 +117,7 @@ int mloam_set_distortion(mloam_ctx_t *h, int on, float scan_period) {
   c->cfg.undist_on = on != 0;
   if (on) c->cfg.undist_scan_period = scan_period;
   c->undist_set = false;
+  undist_withdraw(c);
   return MLOAM_OK;
 }
 
@@ -114,6 +129,25 @@ int mloam_frame_undistort(mloam_ctx_t *h, int n_lidars, const double *pose7) {
     if (!std::isfinite(pose7[k])) return fail(c, MLOAM_E_INVALID, "frame_undistort: non-finite pose");
   memcpy(c->undist_pose7, pose7, sizeof(double) * 7 * (size_t)n_lidars);
   c->undist_n = n_lidars, c->undist_set = true;
+  return MLOAM_OK;
+}
+
+int mloam_frame_set_next_undistort(mloam_ctx_t *h, int n_lidars, const double *pose7) {
+  if (!h || !pose7) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (!c->cfg.undist_on) return fail(c, MLOAM_E_STATE, "frame_set_next_undistort: turn the undistortion on first (mloam_set_distortion)");
+  if (!c->next.set) return fail(c, MLOAM_E_STATE, "frame_set_next_undistort: no sweep is announced (mloam_frame_set_next*)");
+  if (!c->next.undist_open)
+    return fail(c, MLOAM_E_STATE, "frame_set_next_undistort: a setter withdrew the announcement's poses since the sweep was announced; "
+                                  "announce it again (mloam_frame_set_next*)");
+  if (multi_gpu(c))
+    return fail(c, MLOAM_E_STATE, "frame_set_next_undistort: the undistortion is single-GPU only; detach the communicator");
+  if (n_lidars != c->cfg.n_parts())
+    return fail(c, MLOAM_E_INVALID, "frame_set_next_undistort: a pose count other than the frame's LiDARs (1 without the rig merge)");
+  for (int k = 0; k < 7 * n_lidars; k++)
+    if (!std::isfinite(pose7[k])) return fail(c, MLOAM_E_INVALID, "frame_set_next_undistort: non-finite pose");
+  memcpy(c->next.undist.pose7, pose7, sizeof(double) * 7 * (size_t)n_lidars);
+  c->next.undist.n = n_lidars;
   return MLOAM_OK;
 }
 

@@ -452,6 +452,10 @@ class ActiveFeatureSelection {
 //   mloam::setDistortion(ctx, DISTORTION, SCAN_PERIOD);                                    once, after mloam_set_lidars
 //   pose_undist = mloam::undistortPoses(pose_rlt_[IDX_REF], qbl_, tbl_);                    estimator.cpp:575-579
 //   mloam::undistortMeasurements(ctx, pose_undist, IDX_REF, ESTIMATE_EXTRINSIC);           in place of Estimator::undistortMeasurements
+// or, when the odometry has sweep k+1's pose_undist before the mapper takes it (the node split: the odometry undistorts sweep k+1 while
+// the mapper solves sweep k), with that sweep's announcement:
+//   mloam_frame_set_next(ctx, ...sweep k+1...);
+//   mloam::undistortMeasurementsNext(ctx, pose_undist_next, IDX_REF, ESTIMATE_EXTRINSIC);  the look-ahead undistorts it too
 namespace mloam {
 inline void setDistortion(mloam_ctx_t *ctx, bool on, float scan_period) {
   check(ctx, mloam_set_distortion(ctx, on ? 1 : 0, scan_period), "mloam_set_distortion");
@@ -481,6 +485,13 @@ inline void undistortMeasurements(mloam_ctx_t *ctx, const std::vector<Pose> &pos
   std::vector<double> x(7 * pose_undist.size());
   for (size_t l = 0; l < pose_undist.size(); l++) poseToParam(pose_undist[estimate_extrinsic == 2 ? l : idx_ref], &x[7 * l]);
   check(ctx, mloam_frame_undistort(ctx, (int)pose_undist.size(), x.data()), "mloam_frame_undistort");
+}
+// the same poses for the sweep announced by the last mloam_frame_set_next* call of ctx: the call that takes that sweep needs no
+// undistortMeasurements
+inline void undistortMeasurementsNext(mloam_ctx_t *ctx, const std::vector<Pose> &pose_undist, size_t idx_ref, int estimate_extrinsic) {
+  std::vector<double> x(7 * pose_undist.size());
+  for (size_t l = 0; l < pose_undist.size(); l++) poseToParam(pose_undist[estimate_extrinsic == 2 ? l : idx_ref], &x[7 * l]);
+  check(ctx, mloam_frame_set_next_undistort(ctx, (int)pose_undist.size(), x.data()), "mloam_frame_set_next_undistort");
 }
 }  // namespace mloam
 

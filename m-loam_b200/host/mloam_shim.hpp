@@ -480,7 +480,8 @@ inline std::vector<Pose> undistortPoses(const Pose &pose_rlt, int idx_ref, const
   }
   return res;
 }
-// mloam_set_distortion / mloam_frame_undistort on ctx, the context that runs the frames (the poses as undistortPoses returns them)
+// mloam_set_distortion / mloam_frame_undistort / mloam_frame_set_next_undistort on ctx, the context that runs the frames (the poses as
+// undistortPoses returns them)
 inline void setDistortion(mloam_ctx_t *ctx, bool on, float scan_period) {
   check(ctx, mloam_set_distortion(ctx, on ? 1 : 0, scan_period), "mloam_set_distortion");
 }
@@ -488,6 +489,12 @@ inline void undistortMeasurements(mloam_ctx_t *ctx, const std::vector<Pose> &pos
   std::vector<double> x(7 * pose_undist.size());
   for (size_t l = 0; l < pose_undist.size(); l++) pose_undist[l].toParam(&x[7 * l]);
   check(ctx, mloam_frame_undistort(ctx, (int)pose_undist.size(), x.data()), "mloam_frame_undistort");
+}
+// the poses of the sweep announced by the last mloam_frame_set_next* call: the look-ahead undistorts it too
+inline void undistortMeasurementsNext(mloam_ctx_t *ctx, const std::vector<Pose> &pose_undist) {
+  std::vector<double> x(7 * pose_undist.size());
+  for (size_t l = 0; l < pose_undist.size(); l++) pose_undist[l].toParam(&x[7 * l]);
+  check(ctx, mloam_frame_set_next_undistort(ctx, (int)pose_undist.size(), x.data()), "mloam_frame_set_next_undistort");
 }
 }  // namespace mloam
 
