@@ -167,6 +167,54 @@ int mloam_frame_raw_device(mloam_ctx_t *ctx, const mloam_point_t *d_raw, const i
 int mloam_frame_set_next_raw(mloam_ctx_t *ctx, const mloam_point_t *h_raw, const int *h_counts);
 int mloam_frame_set_next_raw_device(mloam_ctx_t *ctx, const mloam_point_t *d_raw, const int *h_counts);
 
+/* ---- the rig's sensor_msgs/PointCloud2 messages: what each driver node receives and turns into a cloud with pcl::fromROSMsg
+ *      (rosNodeRVHercules.cpp:169, rosNodeRVKITTI.cpp:157, rosNodeRVOxford.cpp:173), unpacked on the device in front of the raw front end.
+ * mloam_pc2_layout_t: one driver's point layout, as host/mloam_io.hpp resolvePointCloud2Layout finds it by field name.  point_step
+ *   (1 .. 1024 bytes); per lane (x, y, z, lane 3) the field's byte offset and datatype, 7 FLOAT32 or 8 FLOAT64 (rounded to float as
+ *   (float)d does), offset + size <= point_step; is_bigendian != 0: the data is byte-swapped on a little-endian device.  Lane 3 is the
+ *   `timestamp` field [us] with time_field 1 (calTimestamp(PointITimeCloud)); datatype[3] = 0: none, the lane is 0 — calTimestamp
+ *   discards the sweep's intensity either way, so time_field 0 needs no fourth field.
+ * mloam_pc2_msg_t: one LiDAR's message: data (host or device bytes, by entry point), size = bytes at data, width x height points
+ *   (organised clouds row-major), rows row_step >= width x point_step bytes apart; size >= height x row_step.
+ * mloam_set_front_end_layout: the layouts of the n_lidars LiDARs of mloam_set_lidars (one without it), in that order; the LiDARs of a rig
+ *   may use different drivers.  MLOAM_E_INVALID for a bad layout.  Like mloam_set_front_end it withdraws the features and poses announced
+ *   for the next sweep.
+ * mloam_front_end_msg / mloam_frame_msg / mloam_frame_msg_device / mloam_frame_set_next_msg / mloam_frame_set_next_msg_device: as
+ *   mloam_front_end / mloam_frame_raw / mloam_frame_raw_device / mloam_frame_set_next_raw / mloam_frame_set_next_raw_device, with msgs[l]
+ *   the message of LiDAR l in place of its part of the concatenated raw sweeps.  One launch unpacks the whole rig's messages into the float4
+ *   raw sweep (lane 3 in the intensity lane), which then goes through the raw front end; results are bit-identical to the raw entry points
+ *   on the sweep host/mloam_io.hpp unpackPointCloud2 gives (lane 3 = `timestamp` with time_field 1).  Non-finite points are passed on:
+ *   the front end's removeNaN drops them.  The host entry points copy height x row_step bytes per LiDAR to the device as mloam_frame_raw
+ *   copies its sweep, 16 B per point: a message of point_step bytes per point moves point_step / 16 times as many bytes over PCIe.  The
+ *   look-ahead (mloam_frame_set_next_msg*) is taken by the next mloam_frame_msg* call with the same data pointers and shapes; it unpacks
+ *   the sweep in the look-ahead branch, and its host variant starts the copy at the frame call that runs the look-ahead.
+ *   MLOAM_E_INVALID: a message without points (the node's empty_check), row_step < width x point_step, size < height x row_step, more
+ *   than 2^30 points, a NULL data pointer, and time_field 1 (mloam_set_front_end) with a layout that has no lane 3.  MLOAM_E_STATE:
+ *   without mloam_set_front_end or mloam_set_front_end_layout, when the layouts were given for another LiDAR count, and on a context with
+ *   a communicator. */
+typedef struct {
+  int point_step;
+  int offset[4];   /* x, y, z, lane 3 */
+  int datatype[4]; /* 7 FLOAT32 | 8 FLOAT64; datatype[3] = 0: no lane 3 */
+  int is_bigendian;
+} mloam_pc2_layout_t;
+typedef struct {
+  const void *data;
+  size_t size;
+  int width, height;
+  size_t row_step;
+} mloam_pc2_msg_t;
+int mloam_set_front_end_layout(mloam_ctx_t *ctx, int n_lidars, const mloam_pc2_layout_t *layouts);
+int mloam_front_end_msg(mloam_ctx_t *ctx, const mloam_pc2_msg_t *msgs, mloam_point_t *h_out, int *n_out, int *h_scan_start, int *h_scan_end);
+int mloam_frame_msg(mloam_ctx_t *ctx, const mloam_pc2_msg_t *msgs, const mloam_point_t *h_surf_map, int n_surf_map,
+                    const mloam_point_t *h_corner_map, int n_corner_map, int rebuild_maps, const double *pose_init7, double *pose_out7,
+                    mloam_solve_stats_t *stats);
+int mloam_frame_msg_device(mloam_ctx_t *ctx, const mloam_pc2_msg_t *msgs, const mloam_point_t *d_surf_map, int n_surf_map,
+                           const mloam_point_t *d_corner_map, int n_corner_map, int rebuild_maps, const double *pose_init7,
+                           double *pose_out7, mloam_solve_stats_t *stats);
+int mloam_frame_set_next_msg(mloam_ctx_t *ctx, const mloam_pc2_msg_t *msgs);
+int mloam_frame_set_next_msg_device(mloam_ctx_t *ctx, const mloam_pc2_msg_t *msgs);
+
 /* ---- FeatureExtract::extractCloud (feature_extract.cpp:118-297) -------------------------------- */
 int mloam_extract_features(mloam_ctx_t *ctx, const mloam_point_t *h_cloud, int n, const int *h_scan_start,
                            const int *h_scan_end, int n_scans, mloam_features_t *out);

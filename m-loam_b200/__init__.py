@@ -40,6 +40,8 @@ ABI_SYMBOLS = [
     "mloam_undistort_poses", "mloam_set_distortion", "mloam_frame_undistort", "mloam_frame_set_next_undistort",
     "mloam_full_hessian", "mloam_set_gf_float", "mloam_set_gf_float_threshold", "mloam_gf_float_report",
     "mloam_set_registered", "mloam_frame_registered", "mloam_frame_registered_device",
+    "mloam_set_front_end_layout", "mloam_front_end_msg", "mloam_frame_msg", "mloam_frame_msg_device", "mloam_frame_set_next_msg",
+    "mloam_frame_set_next_msg_device",
 ]
 
 
@@ -94,6 +96,40 @@ class Features(C.Structure):
         ("surf_points_less_flat", C.c_void_p), ("n_sharp", C.c_int), ("n_less_sharp", C.c_int), ("n_flat", C.c_int),
         ("n_less_flat", C.c_int), ("cap", C.c_int),
     ]
+
+
+class Pc2Layout(C.Structure):
+    """mloam_pc2_layout_t: one driver's PointCloud2 point layout (offset / datatype per lane x, y, z, lane 3; datatype 0: no lane 3)."""
+    _fields_ = [("point_step", C.c_int), ("offset", C.c_int * 4), ("datatype", C.c_int * 4), ("is_bigendian", C.c_int)]
+
+
+class Pc2Msg(C.Structure):
+    """mloam_pc2_msg_t: one LiDAR's message (data: host or device bytes)."""
+    _fields_ = [("data", C.c_void_p), ("size", C.c_size_t), ("width", C.c_int), ("height", C.c_int), ("row_step", C.c_size_t)]
+
+
+def pc2_layout(point_step: int, fields, is_bigendian: bool = False) -> Pc2Layout:
+    """fields: [(offset, datatype)] of x, y, z and optionally lane 3 (datatype 7 FLOAT32, 8 FLOAT64)."""
+    lay = Pc2Layout()
+    lay.point_step, lay.is_bigendian = int(point_step), int(bool(is_bigendian))
+    for k, (off, dt) in enumerate(fields):
+        lay.offset[k], lay.datatype[k] = int(off), int(dt)
+    return lay
+
+
+def _msgs(msgs):
+    """msgs: per LiDAR (data, width, height, row_step) with data a host uint8 array, or (ptr, size, width, height, row_step) with a
+    device pointer -> a Pc2Msg array."""
+    arr = (Pc2Msg * len(msgs))()
+    for l, m in enumerate(msgs):
+        if len(m) == 4:
+            data, width, height, row_step = m
+            arr[l].data, arr[l].size = data.__array_interface__["data"][0], data.nbytes
+        else:
+            ptr, size, width, height, row_step = m
+            arr[l].data, arr[l].size = ptr, size
+        arr[l].width, arr[l].height, arr[l].row_step = int(width), int(height), int(row_step)
+    return arr
 
 
 def build(force: bool = False) -> str:
@@ -384,6 +420,50 @@ class Context:
     def frame_set_next_raw_device(self, d_raw: int, counts):
         cnt = None if d_raw is None else np.ascontiguousarray(counts, np.int32)
         self._ck(lib().mloam_frame_set_next_raw_device(self._h, None if d_raw is None else C.c_void_p(d_raw), _p(cnt)))
+
+    # ---- PointCloud2 messages (unpacked on the device, then the raw front end)
+    def set_front_end_layout(self, layouts):
+        """One Pc2Layout (pc2_layout) per LiDAR of set_lidars."""
+        arr = (Pc2Layout * len(layouts))(*layouts)
+        self._ck(lib().mloam_set_front_end_layout(self._h, len(layouts), arr))
+
+    def front_end_msg(self, msgs):
+        """front_end() on the rig's messages (host bytes, see _msgs) -> (ring-ordered sweep, scan_start, scan_end)."""
+        arr = _msgs(msgs)
+        n_pts = sum(int(m.width) * int(m.height) for m in arr)
+        out = np.empty((max(n_pts, 1), 4), np.float32)
+        ss, se = np.zeros(1024, np.int32), np.zeros(1024, np.int32)
+        n = C.c_int(0)
+        self._ck(lib().mloam_front_end_msg(self._h, arr, _p(out), C.byref(n), _p(ss), _p(se)))
+        return out[: n.value].copy(), ss, se
+
+    def frame_msg(self, msgs, surf_map, corner_map, pose_init7, rebuild_maps: bool = True):
+        """frame_raw() on the rig's messages in host memory (see _msgs)."""
+        sm = None if surf_map is None else _cloud(surf_map)
+        cm = None if corner_map is None else _cloud(corner_map)
+        pi = np.ascontiguousarray(pose_init7, np.float64)
+        out = np.zeros(7)
+        st = SolveStats()
+        self._ck(lib().mloam_frame_msg(self._h, _msgs(msgs), _p(sm), 0 if sm is None else sm.shape[0], _p(cm), 0 if cm is None else cm.shape[0],
+                                       int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
+        return out, st.as_dict()
+
+    def frame_msg_device(self, msgs, d_surf_map: int, n_surf_map: int, d_corner_map: int, n_corner_map: int, pose_init7, rebuild_maps: bool = True):
+        """frame_raw_device() on the rig's messages in device memory: msgs per LiDAR (ptr, size, width, height, row_step)."""
+        pi = np.ascontiguousarray(pose_init7, np.float64)
+        out = np.zeros(7)
+        st = SolveStats()
+        self._ck(lib().mloam_frame_msg_device(self._h, _msgs(msgs), C.c_void_p(d_surf_map), n_surf_map, C.c_void_p(d_corner_map), n_corner_map,
+                                              int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
+        return out, st.as_dict()
+
+    def frame_set_next_msg(self, msgs):
+        """Announce the messages of the next frame_msg() call (pass the SAME arrays to it).  None withdraws."""
+        self._next_keep = msgs  # must outlive the coming frame call
+        self._ck(lib().mloam_frame_set_next_msg(self._h, None if msgs is None else _msgs(msgs)))
+
+    def frame_set_next_msg_device(self, msgs):
+        self._ck(lib().mloam_frame_set_next_msg_device(self._h, None if msgs is None else _msgs(msgs)))
 
     # ---- orchestrators
     def scan2map(self, surf_scan, corner_scan, pose_init7):

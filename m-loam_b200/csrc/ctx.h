@@ -137,6 +137,13 @@ struct FrontEnd {
   int time_field;  // 0: time from the azimuth; 1: from the point's timestamp [us] in the w lane (PointITimeCloud overload)
 };
 static_assert(sizeof(FrontEnd) == 24 && sizeof(RigLayout) == 4 * (MLOAM_MAX_LIDARS + 2), "hashed whole: no padding");
+// A rig's PointCloud2 messages (mloam_frame_msg*): per LiDAR the caller's message and the layout it was checked against; zero past the
+// rig's LiDARs.  Compared whole by the look-ahead and hashed whole into the frame graph key.
+struct WireMsgs {
+  mloam_pc2_msg_t msg[MLOAM_MAX_LIDARS];
+  mloam_pc2_layout_t layout[MLOAM_MAX_LIDARS];
+};
+static_assert(sizeof(mloam_pc2_msg_t) == 32 && sizeof(mloam_pc2_layout_t) == 40 && sizeof(WireMsgs) % 8 == 0, "hashed whole: no padding");
 
 // The frame path's configuration as the mloam_set_* calls leave it.  The frame graph key (pipeline.cu frame_key) and the staged inputs
 // (pipeline.cu stage_frame_inputs) derive from it; a value that is staged (the with_ua covariances and threshold, the outlier leaf, the
@@ -149,6 +156,8 @@ struct FrameCfg {
   double ext[7] = {0, 0, 0, 0, 0, 0, 1};
   FrontEnd front{};                         // mloam_set_front_end: the front end of raw frames
   bool front_set = false;
+  int n_layouts = 0;                        // mloam_set_front_end_layout: the PointCloud2 layouts of the rig's LiDARs (0: none given)
+  mloam_pc2_layout_t layouts[MLOAM_MAX_LIDARS];
   int with_ua = 0;                          // mloam_set_uncertainty
   double ua_ext_cov[MLOAM_MAX_LIDARS][36];  // per LiDAR: pose_ext[l].cov_, row-major [translation | rotation]
   double ua_cov_meas[9];                    // COV_MEASUREMENT
@@ -178,6 +187,9 @@ struct Sweep {
   bool host = false;                     // key is a host pointer
   bool raw = false;                      // the rig's raw sweeps with layout L: the front end runs before extraction
   RigLayout L{};
+  bool msg = false;                      // raw sweeps as PointCloud2 messages (wire): unpacked on the device before the front end
+  WireMsgs wire{};
+  const unsigned char *bytes = nullptr;  // a host message sweep: where its bytes are copied (wire_stage_offset per LiDAR)
 };
 
 // the per-point association with uncertainty (uct.h): per LiDAR of the rig, and per run
@@ -477,6 +489,7 @@ struct Ctx {
   // branch.  Its work (winner images, sort) and output (projected cloud + ScanInfo) have buffers of their own: the look-ahead reuses them
   // after the main stream's front end, while the main stream runs the with_ua stage and the solve.
   DevBuf front_work, front_out;
+  DevBuf wire_out;                 // message frames (mloam_frame_msg*): the unpacked raw sweep the front end reads, on either stream like front_out
   Features prefetched;             // features of the sweep announced with the previous frame, ready when that frame returned
   NextSweep next;                  // announced for the frame being enqueued (consumed by it)
   bool next_pending = false;       // its H2D copy was enqueued on br_ahead outside of any capture (ev_next)
@@ -773,6 +786,10 @@ int project_cloud_device(Ctx *c, const float4 *d_in, const RigLayout &L, int ver
 // *d_n_out their count.
 int front_times_device(Ctx *c, const float4 *d_in, const RigLayout &L, int time_field, float scan_period, float4 *d_out, int *d_n_out,
                        DevBuf &work);
+// wire.cu: the PointCloud2 messages of sweep sw (sw.msg) -> the float4 raw sweep out (sw.L's offsets), one launch on c->stream
+int wire_unpack_device(Ctx *c, const Sweep &sw, float4 *out);
+// where LiDAR l's bytes lie in a host message sweep's device staging (256-byte aligned), and l = n_lidars: the staging's size
+size_t wire_stage_offset(const WireMsgs &w, int l);
 int transform_segments_device(Ctx *c, float4 *d_pts, int n, const int *d_off, int n_seg, const float *d_mat12);
 // VoxelGridCovarianceMLOAM<PointIWithCov>::filter: covariance-weighted merge per voxel (cov6 + trace per point in and out)
 int voxel_downsample_cov_device(Ctx *c, const float4 *d_in, const float *d_cov6, const float *d_trace, int n, const int *d_n_in, float leaf,

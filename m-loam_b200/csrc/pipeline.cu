@@ -352,9 +352,11 @@ void stage_frame_inputs(Ctx *c, const FrameCall &fc) {
 }
 
 // Whether sweep sw is the announced sweep a: same caller pointer and sizes; a raw sweep is taken by a raw frame with the same per-LiDAR
-// counts only, a ring-ordered sweep by a ring-ordered frame, and a host frame takes a host announcement
+// counts only, a ring-ordered sweep by a ring-ordered frame, and a host frame takes a host announcement.  Messages: the same messages
+// (pointers and shapes) with the same layouts.
 bool same_sweep(const Sweep &a, const Sweep &sw) {
-  const bool same_kind = sw.raw ? (a.raw && std::memcmp(&a.L, &sw.L, sizeof(RigLayout)) == 0) : !a.raw;
+  const bool same_kind = (sw.raw ? (a.raw && std::memcmp(&a.L, &sw.L, sizeof(RigLayout)) == 0) : !a.raw) && a.msg == sw.msg &&
+                         (!sw.msg || std::memcmp(&a.wire, &sw.wire, sizeof(WireMsgs)) == 0);
   return a.key == sw.key && a.n == sw.n && a.n_scans == sw.n_scans && same_kind && (a.host || !sw.host);
 }
 
@@ -380,6 +382,12 @@ int extract_enqueue(Ctx *c, const Sweep &sw, int parity, FrameBufs *F_out) {
   if (rc) return rc;
   const float4 *d_cloud = sw.cloud;
   const int *d_scan_start = sw.scan_start, *d_scan_end = sw.scan_end;
+  if (sw.msg) {  // PointCloud2 messages: unpacked into the raw sweep the front end reads
+    MLOAM_CUDA_OK(c, c->wire_out.reserve(sizeof(float4) * ((size_t)n + 1)));
+    rc = wire_unpack_device(c, sw, c->wire_out.as<float4>());
+    if (rc) return rc;
+    d_cloud = c->wire_out.as<float4>();
+  }
   if (sw.raw) {
     const FrontEnd &fe = cfg.front;
     float4 *proj;
@@ -617,6 +625,15 @@ void frame_commit(Ctx *c, int parity, const Ctx::FrameOutcome &o) {
 // Point the device side of host sweep *sw into B (the points, then room for its ScanInfo) and, with `upload`, copy the sweep there on st.
 // The ScanInfo goes through the pinned rows pin: an async copy from pageable memory would block the host behind the sweep's copy.
 int sweep_to_device(Ctx *c, DevBuf &B, Sweep *sw, bool upload, int (*pin)[MLOAM_MAX_RINGS], cudaStream_t st) {
+  if (sw->msg) {  // each LiDAR's message bytes, at wire_stage_offset
+    const WireMsgs &w = sw->wire;
+    MLOAM_CUDA_OK(c, B.reserve(wire_stage_offset(w, sw->L.n_lidars)));
+    sw->bytes = B.as<unsigned char>();
+    for (int l = 0; upload && l < sw->L.n_lidars; l++)
+      MLOAM_CUDA_OK(c, cudaMemcpyAsync(B.as<unsigned char>() + wire_stage_offset(w, l), w.msg[l].data, (size_t)w.msg[l].height * w.msg[l].row_step,
+                                       cudaMemcpyHostToDevice, st));
+    return MLOAM_OK;
+  }
   SweepIn D;
   int rc = sweep_bufs(c, B, sw->n, sw->n_scans, &D);
   if (rc) return rc;
@@ -715,6 +732,15 @@ unsigned long long frame_key(Ctx *c, const FrameCall &f) {
   // more word, only when either is on, so that the keys of a context that never announces poses are the ones it had without them
   w = (undist_ahead(c) ? 1ull : 0ull) | (f.take_undist ? 2ull : 0ull);
   if (w) h = (h ^ w) * 1099511628211ull;
+  // message sweeps: their messages, layouts and staging are kernel arguments of the captured unpack — hashed only for them, so that a
+  // context that never takes a message keeps the keys it had without them
+  auto hash_wire = [&](const Sweep &x, unsigned long long tag) {
+    h = (h ^ tag) * 1099511628211ull;
+    h = (h ^ (unsigned long long)reinterpret_cast<uintptr_t>(x.bytes)) * 1099511628211ull;
+    for (size_t i = 0; i < sizeof(WireMsgs); i += 8) memcpy(&w, reinterpret_cast<const char *>(&x.wire) + i, 8), h = (h ^ w) * 1099511628211ull;
+  };
+  if (sw.msg) hash_wire(sw, 4ull);
+  if (c->next.set && c->use_lookahead && nx.msg) hash_wire(nx, 8ull);
   return h;
 }
 
@@ -831,6 +857,40 @@ int raw_sweep(Ctx *c, const mloam_point_t *raw, bool host, const int *h_counts, 
   L.off[L.n_lidars] = (int)total;
   sw->key = raw, sw->host = host, sw->raw = true, sw->n = (int)total, sw->n_scans = L.n_lidars * fe.vertical_scans;
   if (!host) sw->cloud = reinterpret_cast<const float4 *>(raw);
+  return MLOAM_OK;
+}
+
+// The rig's PointCloud2 messages msgs (n_lidars of mloam_set_lidars; data in host or device memory) after the checks every message entry
+// point makes: a raw sweep whose points the unpack launch writes
+int msg_sweep(Ctx *c, const mloam_pc2_msg_t *msgs, bool host, Sweep *sw) {
+  const FrameCfg &cfg = c->cfg;
+  if (!cfg.front_set) return fail(c, MLOAM_E_STATE, "frame_msg: call mloam_set_front_end first");
+  if (cfg.n_layouts == 0) return fail(c, MLOAM_E_STATE, "frame_msg: call mloam_set_front_end_layout first");
+  if (cfg.n_layouts != cfg.n_lidars)
+    return fail(c, MLOAM_E_STATE, "frame_msg: mloam_set_front_end_layout gave another LiDAR count than mloam_set_lidars; give the layouts again");
+  int rc = frame_single_gpu(c, true);
+  if (rc) return rc;
+  if (!msgs) return MLOAM_E_INVALID;
+  if (cfg.front.time_field)
+    for (int l = 0; l < cfg.n_lidars; l++)
+      if (!cfg.layouts[l].datatype[3]) return fail(c, MLOAM_E_INVALID, "frame_msg: time_field 1 needs the timestamp field as lane 3 of every layout");
+  std::vector<int> counts(cfg.n_lidars);
+  for (int l = 0; l < cfg.n_lidars; l++) {
+    const mloam_pc2_msg_t &m = msgs[l];
+    const mloam_pc2_layout_t &F = cfg.layouts[l];
+    if (!m.data) return fail(c, MLOAM_E_INVALID, "frame_msg: a message without data");
+    if (m.width <= 0 || m.height <= 0)  // the driver node's empty_check (rosNodeRVOxford.cpp:216-220)
+      return fail(c, MLOAM_E_INVALID, "frame_msg: every LiDAR of the rig needs a non-empty message");
+    if ((long long)m.width * m.height > (1 << 30)) return fail(c, MLOAM_E_INVALID, "frame_msg: sweeps too large");
+    if (m.row_step < (size_t)m.width * (size_t)F.point_step) return fail(c, MLOAM_E_INVALID, "frame_msg: row_step < width x point_step");
+    if (m.row_step > m.size / (size_t)m.height)  // size < height x row_step, without the product's overflow
+      return fail(c, MLOAM_E_INVALID, "frame_msg: a message is shorter than height x row_step");
+    counts[l] = m.width * m.height;
+  }
+  rc = raw_sweep(c, nullptr, host, counts.data(), sw);
+  if (rc) return rc;
+  sw->key = msgs[0].data, sw->cloud = nullptr, sw->msg = true;
+  for (int l = 0; l < cfg.n_lidars; l++) sw->wire.msg[l] = msgs[l], sw->wire.layout[l] = cfg.layouts[l];
   return MLOAM_OK;
 }
 
@@ -1218,6 +1278,99 @@ int mloam_frame_set_next_raw_device(mloam_ctx_t *h, const mloam_point_t *d_raw, 
   if (!h) return MLOAM_E_INVALID;
   Sweep sw;
   const int rc = d_raw ? raw_sweep(&h->c, d_raw, false, h_counts, &sw) : MLOAM_OK;  // nullptr: withdraw
+  return announce(&h->c, sw, rc);
+}
+
+// ------------------------------------------------------------------------------------------ PointCloud2 messages
+int mloam_set_front_end_layout(mloam_ctx_t *h, int n_lidars, const mloam_pc2_layout_t *layouts) {
+  if (!h) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  if (n_lidars < 1 || n_lidars > MLOAM_MAX_LIDARS || !layouts) return fail(c, MLOAM_E_INVALID, "set_front_end_layout: 1 to 16 layouts");
+  for (int l = 0; l < n_lidars; l++) {
+    const mloam_pc2_layout_t &F = layouts[l];
+    if (F.point_step < 1 || F.point_step > 1024) return fail(c, MLOAM_E_INVALID, "set_front_end_layout: point_step must be 1 .. 1024 bytes");
+    for (int k = 0; k < 4; k++) {
+      const int dt = F.datatype[k];
+      if (k == 3 && dt == 0) continue;  // no lane 3
+      if (dt != 7 && dt != 8) return fail(c, MLOAM_E_INVALID, "set_front_end_layout: fields must be FLOAT32 (7) or FLOAT64 (8)");
+      if (F.offset[k] < 0 || F.offset[k] > F.point_step - (dt == 8 ? 8 : 4))
+        return fail(c, MLOAM_E_INVALID, "set_front_end_layout: a field does not lie inside the point (offset + size > point_step)");
+    }
+  }
+  FrameCfg &f = c->cfg;
+  f.n_layouts = n_lidars;
+  memset(f.layouts, 0, sizeof(f.layouts));
+  memcpy(f.layouts, layouts, sizeof(mloam_pc2_layout_t) * (size_t)n_lidars);
+  c->prefetched.valid = false;  // as mloam_set_front_end
+  undist_withdraw(c);
+  return MLOAM_OK;
+}
+
+int mloam_front_end_msg(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs, mloam_point_t *h_out, int *n_out, int *h_scan_start, int *h_scan_end) {
+  if (!h || !h_out || !n_out || !h_scan_start || !h_scan_end) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  *n_out = 0;
+  Sweep sw;
+  int rc = msg_sweep(c, msgs, true, &sw);
+  if (rc) return rc;
+  cudaSetDevice(c->device);
+  const int n = sw.n, n_scans = sw.n_scans;
+  c->prefetched.valid = false;  // the front end's output buffer is the frame's
+  rc = sweep_to_device(c, c->sweep_in, &sw, true, nullptr, c->stream);
+  if (rc) return rc;
+  MLOAM_CUDA_OK(c, c->wire_out.reserve(sizeof(float4) * ((size_t)n + 1)));
+  rc = wire_unpack_device(c, sw, c->wire_out.as<float4>());
+  if (rc) return rc;
+  float4 *d_out;
+  int *d_meta;  // [0] count, then scan starts, scan ends
+  MLOAM_CUDA_OK(c, carve(c->front_out, [&](Carve &cv) { d_out = cv.take<float4>((size_t)n + 1), d_meta = cv.take<int>(4 + 2 * (size_t)n_scans); }));
+  cudaStream_t st = c->stream;
+  const FrontEnd &fe = c->cfg.front;
+  rc = project_cloud_device(c, c->wire_out.as<float4>(), sw.L, fe.vertical_scans, fe.horizon_scans, fe.roi_range, &fe, d_out, d_meta + 4,
+                            d_meta + 4 + n_scans, d_meta, c->front_work);
+  if (rc) return rc;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_start, d_meta + 4, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_end, d_meta + 4 + n_scans, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
+  int *hc = c->pinned->counts;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_meta, sizeof(int), cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  *n_out = hc[0];
+  if (hc[0] > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_out, d_out, sizeof(float4) * (size_t)hc[0], cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  return MLOAM_OK;
+}
+
+int mloam_frame_msg(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs, const mloam_point_t *h_surf_map, int n_surf_map,
+                    const mloam_point_t *h_corner_map, int n_corner_map, int rebuild_maps, const double *pose_init7, double *pose_out7,
+                    mloam_solve_stats_t *stats) {
+  if (!h || !pose_init7 || !pose_out7) return MLOAM_E_INVALID;
+  Sweep sw;
+  const int rc = msg_sweep(&h->c, msgs, true, &sw);
+  if (rc) return rc;
+  return frame_call(&h->c, sw, h_surf_map, n_surf_map, h_corner_map, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+}
+
+int mloam_frame_msg_device(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs, const mloam_point_t *d_surf_map, int n_surf_map,
+                           const mloam_point_t *d_corner_map, int n_corner_map, int rebuild_maps, const double *pose_init7,
+                           double *pose_out7, mloam_solve_stats_t *stats) {
+  if (!h || !pose_init7 || !pose_out7) return MLOAM_E_INVALID;
+  Sweep sw;
+  const int rc = msg_sweep(&h->c, msgs, false, &sw);
+  if (rc) return rc;
+  return frame_call(&h->c, sw, d_surf_map, n_surf_map, d_corner_map, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+}
+
+// Look-ahead for message frames: as mloam_frame_set_next_raw*, picked up by the next mloam_frame_msg* call with the same messages
+int mloam_frame_set_next_msg(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs) {
+  if (!h) return MLOAM_E_INVALID;
+  Sweep sw;
+  const int rc = msgs ? msg_sweep(&h->c, msgs, true, &sw) : MLOAM_OK;  // nullptr: withdraw
+  return announce(&h->c, sw, rc);
+}
+int mloam_frame_set_next_msg_device(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs) {
+  if (!h) return MLOAM_E_INVALID;
+  Sweep sw;
+  const int rc = msgs ? msg_sweep(&h->c, msgs, false, &sw) : MLOAM_OK;  // nullptr: withdraw
   return announce(&h->c, sw, rc);
 }
 

@@ -7,9 +7,11 @@
 //                                                digits, the rest with 8 (std::ostream::precision semantics, not fixed notation)
 //
 // PointCloud2 layout rules implemented (sensor_msgs/PointCloud2 definition): fields are located by NAME ("x", "y", "z",
-// "intensity"), each with its byte offset and datatype (FLOAT32 = 7; FLOAT64 = 8 is converted); points are `point_step` bytes apart,
-// rows `row_step` apart; is_bigendian data is byte-swapped; a missing "intensity" field gives 0 — the reference exits in that case
-// (feature_extract.hpp:138-142), which callers can reproduce by checking PointCloud2View::has_intensity.
+// "intensity"), each with its byte offset and datatype (FLOAT32 = 7; FLOAT64 = 8 is converted); a field lies inside the point (offset +
+// size <= point_step); points are `point_step` bytes apart, rows `row_step` apart; is_bigendian data is byte-swapped; a missing
+// "intensity" field gives 0 — the reference exits in that case (feature_extract.hpp:138-142), which callers can reproduce by checking
+// PointCloud2View::has_intensity.  The fourth lane may name another field: "timestamp" for calTimestamp's PointITimeCloud overload.
+// The device unpack of mloam_frame_msg* follows the same rules (resolvePointCloud2Layout).
 #pragma once
 #include <cstdint>
 #include <cstring>
@@ -60,23 +62,30 @@ inline bool host_is_bigendian() {
   const uint16_t one = 1;
   return *reinterpret_cast<const uint8_t *>(&one) == 0;
 }
+inline const PointField *find_field(const PointCloud2View &msg, const char *name) {
+  if (!name) return nullptr;
+  for (const PointField &f : msg.fields)
+    if (f.name == name) return &f;
+  return nullptr;
+}
+// FLOAT32 or FLOAT64, inside the point
+inline bool field_ok(const PointField &f, uint32_t point_step) {
+  if (f.datatype != FLOAT32 && f.datatype != FLOAT64) return false;
+  return (uint64_t)f.offset + (f.datatype == FLOAT64 ? 8u : 4u) <= point_step;
+}
 }  // namespace detail
 
-// PointCloud2 -> float4 points (x, y, z, intensity).  Returns false when x / y / z are missing, a field is not FLOAT32 / FLOAT64, or
-// the buffer is shorter than height * row_step.
-inline bool unpackPointCloud2(PointCloud2View &msg, std::vector<mloam_point_t> &out) {
-  const PointField *fx = nullptr, *fy = nullptr, *fz = nullptr, *fi = nullptr;
-  for (const PointField &f : msg.fields) {
-    if (f.name == "x") fx = &f;
-    else if (f.name == "y") fy = &f;
-    else if (f.name == "z") fz = &f;
-    else if (f.name == "intensity") fi = &f;
-  }
-  msg.has_intensity = fi != nullptr;
+// PointCloud2 -> float4 points (x, y, z, lane 3); lane 3 is the field named lane3 ("intensity" by default, nullptr: none), 0 when the
+// message has no such field.  Returns false when x / y / z are missing, a field is not FLOAT32 / FLOAT64 or does not lie inside the point
+// (offset + size > point_step), or the buffer is shorter than height * row_step.
+inline bool unpackPointCloud2(PointCloud2View &msg, std::vector<mloam_point_t> &out, const char *lane3 = "intensity") {
+  const PointField *fx = detail::find_field(msg, "x"), *fy = detail::find_field(msg, "y"), *fz = detail::find_field(msg, "z");
+  const PointField *fi = detail::find_field(msg, lane3);
+  msg.has_intensity = detail::find_field(msg, "intensity") != nullptr;
   out.clear();
   if (!fx || !fy || !fz) return false;
   for (const PointField *f : {fx, fy, fz, fi})
-    if (f && f->datatype != FLOAT32 && f->datatype != FLOAT64) return false;
+    if (f && !detail::field_ok(*f, msg.point_step)) return false;
   const uint32_t row_step = msg.row_step ? msg.row_step : msg.width * msg.point_step;
   if (!msg.data || msg.data_size < (size_t)msg.height * row_step) return false;
   const bool swap = msg.is_bigendian != detail::host_is_bigendian();
@@ -91,6 +100,34 @@ inline bool unpackPointCloud2(PointCloud2View &msg, std::vector<mloam_point_t> &
       out[k].intensity = fi ? detail::load_scalar(p + fi->offset, fi->datatype, swap) : 0.0f;
     }
   return true;
+}
+
+// The layout of msg's points for mloam_set_front_end_layout, found by field name once per driver: x, y, z and, with lane3 (e.g.
+// "timestamp" for time_field 1), that field as lane 3; lane3 nullptr: no lane 3.  Returns false when x / y / z or the lane-3 field asked
+// for are missing, a field is not FLOAT32 / FLOAT64, or a field does not lie inside the point (offset + size > point_step).
+inline bool resolvePointCloud2Layout(const PointCloud2View &msg, const char *lane3, mloam_pc2_layout_t &layout) {
+  const PointField *f[4] = {detail::find_field(msg, "x"), detail::find_field(msg, "y"), detail::find_field(msg, "z"),
+                            detail::find_field(msg, lane3)};
+  std::memset(&layout, 0, sizeof(layout));
+  if (msg.point_step > 1024) return false;  // mloam_set_front_end_layout's bound
+  for (int k = 0; k < 4; k++) {
+    if (!f[k]) {
+      if (k < 3 || lane3) return false;
+      continue;
+    }
+    if (!detail::field_ok(*f[k], msg.point_step)) return false;
+    layout.offset[k] = (int)f[k]->offset, layout.datatype[k] = f[k]->datatype;
+  }
+  layout.point_step = (int)msg.point_step, layout.is_bigendian = msg.is_bigendian ? 1 : 0;
+  return true;
+}
+
+// One LiDAR's message for mloam_frame_msg* (the bytes stay the caller's)
+inline mloam_pc2_msg_t pointCloud2Msg(const PointCloud2View &msg) {
+  mloam_pc2_msg_t m;
+  m.data = msg.data, m.size = msg.data_size, m.width = (int)msg.width, m.height = (int)msg.height;
+  m.row_step = msg.row_step ? msg.row_step : (size_t)msg.width * msg.point_step;
+  return m;
 }
 
 // float4 points -> the PointCloud2 layout pcl::toROSMsg gives a pcl::PointXYZI cloud: point_step 32, x/y/z at 0/4/8, intensity at 16,

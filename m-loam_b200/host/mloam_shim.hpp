@@ -33,6 +33,7 @@
 
 #include "../../include/mloam_b200.h"
 #include "mloam_context.hpp"
+#include "mloam_io.hpp"
 
 // ----------------------------------------------------------------------------------------------- point types
 namespace common {
@@ -515,5 +516,35 @@ inline void frameRegistered(mloam_ctx_t *ctx, common::PointICloud &full_res, com
   frameRegistered(ctx, MLOAM_REGISTERED_FULL_RES, full_res);
   frameRegistered(ctx, MLOAM_REGISTERED_SURF, surf_last);
   frameRegistered(ctx, MLOAM_REGISTERED_CORNER, corner_last);
+}
+}  // namespace mloam
+
+// ----------------------------------------------------------------------------------------------- PointCloud2 messages
+namespace mloam {
+// laserCloudHandler -> mloam_frame_msg: the rig's messages as the driver nodes receive them (one per LiDAR, the order of mloam_set_lidars).
+// setFrontEndLayout resolves each driver's layout once (lane 3: "timestamp" with time_field 1, none otherwise); frameMsg runs the frame on
+// the messages' bytes, which the library unpacks on the device (the maps are the frame's submaps, rebuilt as mloam_frame_raw does).
+inline void setFrontEndLayout(mloam_ctx_t *ctx, const std::vector<io::PointCloud2View> &msgs, bool time_field) {
+  std::vector<mloam_pc2_layout_t> layouts(msgs.size());
+  for (size_t l = 0; l < msgs.size(); l++)
+    if (!io::resolvePointCloud2Layout(msgs[l], time_field ? "timestamp" : nullptr, layouts[l]))
+      throw std::runtime_error("setFrontEndLayout: a message lacks x / y / z (or timestamp) as FLOAT32 / FLOAT64 fields inside the point");
+  check(ctx, mloam_set_front_end_layout(ctx, (int)layouts.size(), layouts.data()), "mloam_set_front_end_layout");
+}
+inline bool frameMsg(mloam_ctx_t *ctx, const std::vector<io::PointCloud2View> &msgs, const common::PointICloud &laser_cloud_surf_from_map,
+                     const common::PointICloud &laser_cloud_corner_from_map, Pose &pose_wmap_curr, mloam_solve_stats_t *stats = nullptr) {
+  std::vector<mloam_pc2_msg_t> m(msgs.size());
+  for (size_t l = 0; l < msgs.size(); l++) m[l] = io::pointCloud2Msg(msgs[l]);
+  std::vector<mloam_point_t> sm = pack(laser_cloud_surf_from_map), cm = pack(laser_cloud_corner_from_map);
+  double x[7], y[7];
+  pose_wmap_curr.toParam(x);
+  mloam_solve_stats_t st;
+  check(ctx, mloam_frame_msg(ctx, m.data(), sm.data(), (int)sm.size(), cm.data(), (int)cm.size(), 1, x, y, &st), "mloam_frame_msg");
+  if (stats) *stats = st;
+  if (st.ran) {
+    pose_wmap_curr.t_ = {{y[0], y[1], y[2]}};
+    pose_wmap_curr.q_ = {{y[3], y[4], y[5], y[6]}};
+  }
+  return st.ran != 0;
 }
 }  // namespace mloam
