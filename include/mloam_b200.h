@@ -13,7 +13,8 @@
  * device.  Points are float4 (x, y, z, intensity) == the payload of pcl::PointXYZI
  * (common::PointI, mloam_common/libs/include/common/types/type.h:20); intensity = ring id + relative
  * time (image_segmenter.hpp:128).  Poses are 7 doubles [tx ty tz qx qy qz qw]
- * (pose_local_parameterization.h:20).
+ * (pose_local_parameterization.h:20).  PointCloud2 bytes cross the ABI both ways: the driver messages
+ * of mloam_frame_msg* in, the published clouds of mloam_cloud_msgs* (pcl::toROSMsg's layouts) out.
  */
 #ifndef MLOAM_B200_H_
 #define MLOAM_B200_H_
@@ -532,6 +533,43 @@ int mloam_global_map(mloam_ctx_t *ctx, int mode, const double *center7, double r
                      int *n_map1);
 int mloam_global_map_read(mloam_ctx_t *ctx, int which, mloam_point_t *h_pts, float *h_cov6, int cap, int *n);
 int mloam_global_map_chosen(mloam_ctx_t *ctx, int *h_ids, int cap, int *n);
+
+/* ---- the mapper's published clouds as sensor_msgs/PointCloud2: pcl::toROSMsg of pubPointCloud (lidar_mapper_keyframe.cpp:690-714) and
+ *      pubGlobalMap (:780-851), packed on the device.  Every message is little-endian, unorganised (height 1), row_step = width x
+ *      point_step, in one of the two layouts toROSMsg gives the reference's point types; padding bytes are zero (the reference leaves them
+ *      indeterminate), so messages compare byte for byte:
+ *   PointXYZI         point_step 32: x 0, y 4, z 8, intensity 16, FLOAT32, count 1 (host/mloam_io.hpp packPointCloud2)
+ *   PointXYZIWithCov  point_step 48: x 0, y 4, z 8, intensity 16, cov_xx 20, cov_xy 24, cov_xz 28, cov_yy 32, cov_yz 36, cov_zz 40,
+ *                     cov_trace 44 (mloam_pcl/point_with_cov.hpp; host/mloam_io.hpp packPointCloud2Cov)
+ * The sources:
+ *   MLOAM_MSG_FULL_RES / _SURF_LAST / _CORNER_LAST  (PointXYZI) the registered clouds of the last mloam_frame* call, exactly as
+ *     mloam_frame_registered returns MLOAM_REGISTERED_FULL_RES / _SURF / _CORNER; non-finite points keep their bits.
+ *   MLOAM_MSG_SURROUND  (PointXYZIWithCov) laser_cloud_surround (:789): the keyframe store's filtered surf map followed by its filtered
+ *     corner map (mloam_keyframe_submap's outputs), with cov_vec and cov_trace; empty after mloam_keyframe_save until the next rebuild
+ *     (clearCloud, :921-927).
+ *   MLOAM_MSG_GLOBAL_MAP0 / _GLOBAL_MAP1  (PointXYZIWithCov) maps 0 and 1 of the last mloam_global_map (laser_cloud_map, :845), with
+ *     cov_vec and cov_trace.
+ *   cov_trace is the value the device filter stored: (cov_xx + cov_yy) + cov_zz in float, except where the filter's voxel index
+ *   overflows int32 and it passes its input through, with the association's trace.
+ * mloam_cloud_msgs: the messages of n (1 .. 6) distinct sources, packed by ONE launch on the context stream (outside every frame graph:
+ *   frames run, capture and replay as without it).  width[k] = source k's point count, always set; msg k is width[k] x point_step bytes.
+ *   h_data[k] NULL: a size query for source k; otherwise its bytes are copied there, when cap_bytes[k] holds them; if any does not,
+ *   MLOAM_E_INVALID and nothing is copied.  Pageable memory works; a pinned destination (cudaMallocHost / cudaHostRegister) is what
+ *   makes the copy run at PCIe speed.  An empty cloud gives width 0 and is a success.
+ * mloam_cloud_msgs_device: the same messages left in context memory, d_data[k] 256-byte aligned; valid until the next mloam_cloud_msgs*
+ *   call, or the next call that replaces a source (mloam_frame*, mloam_keyframe_submap, mloam_keyframe_save, mloam_global_map,
+ *   mloam_keyframes_init).
+ *   Both synchronise the context stream.  MLOAM_E_INVALID: n out of range, a NULL array, a source that is not one of the six or given
+ *   twice.  MLOAM_E_STATE: a registered source when the last mloam_frame* call ran without mloam_set_registered or failed (as
+ *   mloam_frame_registered), a keyframe-store source without mloam_keyframes_init, and on a context with a communicator. */
+#define MLOAM_MSG_FULL_RES 0 /* PointXYZI */
+#define MLOAM_MSG_SURF_LAST 1
+#define MLOAM_MSG_CORNER_LAST 2
+#define MLOAM_MSG_SURROUND 3 /* PointXYZIWithCov */
+#define MLOAM_MSG_GLOBAL_MAP0 4
+#define MLOAM_MSG_GLOBAL_MAP1 5
+int mloam_cloud_msgs(mloam_ctx_t *ctx, int n, const int *sources, void *const *h_data, const size_t *cap_bytes, int *width);
+int mloam_cloud_msgs_device(mloam_ctx_t *ctx, int n, const int *sources, const void **d_data, int *width);
 
 /* ---- FeatureExtract::matchCornerFromScan / matchSurfFromScan (feature_extract.hpp:131-376) against the map slot
  * built (mloam_map_build, cell ~1.3 m) from the previous sweep's less-sharp / less-flat features, which must be in

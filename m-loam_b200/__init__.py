@@ -22,6 +22,8 @@ LIB_PATH = os.environ.get("MLOAM_LIB", os.path.join(HERE, "libmloam_b200.so"))
 MAP_CORNER, MAP_SURF, MAP_SCAN_CORNER, MAP_SCAN_SURF = 0, 1, 2, 3
 GLOBAL_MAP_SURROUND, GLOBAL_MAP_SAVE = 0, 1  # mloam_global_map modes: pubGlobalMap, saveGlobalMap
 REGISTERED_FULL_RES, REGISTERED_SURF, REGISTERED_CORNER = 0, 1, 2  # mloam_frame_registered clouds (pubPointCloud)
+# mloam_cloud_msgs sources: PointXYZI messages (32 B per point), then PointXYZIWithCov messages (48 B per point)
+MSG_FULL_RES, MSG_SURF_LAST, MSG_CORNER_LAST, MSG_SURROUND, MSG_GLOBAL_MAP0, MSG_GLOBAL_MAP1 = 0, 1, 2, 3, 4, 5
 E_NO_DEVICE = -2
 
 # every entry point include/mloam_b200.h declares
@@ -41,7 +43,7 @@ ABI_SYMBOLS = [
     "mloam_full_hessian", "mloam_set_gf_float", "mloam_set_gf_float_threshold", "mloam_gf_float_report",
     "mloam_set_registered", "mloam_frame_registered", "mloam_frame_registered_device",
     "mloam_set_front_end_layout", "mloam_front_end_msg", "mloam_frame_msg", "mloam_frame_msg_device", "mloam_frame_set_next_msg",
-    "mloam_frame_set_next_msg_device",
+    "mloam_frame_set_next_msg_device", "mloam_cloud_msgs", "mloam_cloud_msgs_device",
 ]
 
 
@@ -130,6 +132,11 @@ def _msgs(msgs):
             arr[l].data, arr[l].size = ptr, size
         arr[l].width, arr[l].height, arr[l].row_step = int(width), int(height), int(row_step)
     return arr
+
+
+def msg_step(source: int) -> int:
+    """point_step of a cloud_msgs source: 32 (PointXYZI) or 48 (PointXYZIWithCov)."""
+    return 32 if source <= MSG_CORNER_LAST else 48
 
 
 def build(force: bool = False) -> str:
@@ -781,6 +788,46 @@ class Context:
             __cuda_array_interface__ = {"shape": (n.value, 4), "typestr": "<f4", "data": (ptr.value, False), "version": 3, "strides": None}
 
         return torch.as_tensor(_View(), device=f"cuda:{self.device}").clone()
+
+    # ---- the published clouds as sensor_msgs/PointCloud2 data (pcl::toROSMsg on the device)
+    @staticmethod
+    def _sources(sources):
+        src = (C.c_int * len(sources))(*[int(s) for s in sources])
+        return src, (C.c_int * len(sources))()
+
+    def cloud_msgs(self, sources, out=None):
+        """The PointCloud2 data of each source (MSG_*) as bytes, packed by one launch per call: width x 32 bytes (PointXYZI) or
+        width x 48 (PointXYZIWithCov).  out (optional): per source a writable uint8 array (pageable or pinned) the library copies into;
+        without it a size query runs first."""
+        src, width = self._sources(sources)
+        n = len(sources)
+        if out is None:
+            self._ck(lib().mloam_cloud_msgs(self._h, n, src, (C.c_void_p * n)(), (C.c_size_t * n)(), width))
+            out = [np.empty(width[k] * msg_step(s), np.uint8) for k, s in enumerate(sources)]
+        ptrs = (C.c_void_p * n)(*[a.__array_interface__["data"][0] if a.nbytes else None for a in out])
+        self._ck(lib().mloam_cloud_msgs(self._h, n, src, ptrs, (C.c_size_t * n)(*[a.nbytes for a in out]), width))
+        return [out[k][: width[k] * msg_step(s)].tobytes() for k, s in enumerate(sources)]
+
+    def cloud_msgs_device(self, sources):
+        """The same messages as CUDA uint8 tensors, cloned from the context's buffer (which the next cloud_msgs* call reuses)."""
+        import torch
+
+        src, width = self._sources(sources)
+        n = len(sources)
+        ptrs = (C.c_void_p * n)()
+        self._ck(lib().mloam_cloud_msgs_device(self._h, n, src, ptrs, width))
+        res = []
+        for k, s in enumerate(sources):
+            nb = width[k] * msg_step(s)
+            if nb == 0:
+                res.append(torch.zeros(0, dtype=torch.uint8, device=f"cuda:{self.device}"))
+                continue
+
+            class _View:  # the context's buffer as a CUDA array, viewed without a copy
+                __cuda_array_interface__ = {"shape": (nb,), "typestr": "|u1", "data": (ptrs[k], False), "version": 3, "strides": None}
+
+            res.append(torch.as_tensor(_View(), device=f"cuda:{self.device}").clone())
+        return res
 
     # ---- keyframe store (saveKeyframe / extractSurroundingKeyFrames on the device)
     def keyframes_init(self, distance_keyframes: float, orientation_keyframes_deg: float, surrounding_kf_radius: float, map_sur_kf_res: float,

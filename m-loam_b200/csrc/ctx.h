@@ -490,6 +490,9 @@ struct Ctx {
   // after the main stream's front end, while the main stream runs the with_ua stage and the solve.
   DevBuf front_work, front_out;
   DevBuf wire_out;                 // message frames (mloam_frame_msg*): the unpacked raw sweep the front end reads, on either stream like front_out
+  // mloam_cloud_msgs* (wire.cu): the packed PointCloud2 bytes of the last call, each message 256-byte aligned, then the widths.  No frame
+  // graph references it, so its growth re-captures nothing.
+  DevBuf cloud_msgs{nullptr, 0, false};
   Features prefetched;             // features of the sweep announced with the previous frame, ready when that frame returned
   NextSweep next;                  // announced for the frame being enqueued (consumed by it)
   bool next_pending = false;       // its H2D copy was enqueued on br_ahead outside of any capture (ev_next)
@@ -737,6 +740,18 @@ void stage_pose(Ctx *c, const double *pose7);
 int pose_cov_device(Ctx *c, bool pdl);
 // keyframe.cu: frees the keyframe store (mloam_ctx_destroy)
 void keyframes_release(Ctx *c);
+// One run of points a PointCloud2 message is packed from (wire.cu k_wire_pack): points, and for the 48-byte layout cov_vec and
+// cov_trace; n points, or min(n, *d_n) when the count lives on the device
+struct PackSeg {
+  const float4 *pts;
+  const float *cov6, *trace;
+  const int *d_n;
+  int n;
+  int cloud;  // the message it belongs to (set by the packer)
+};
+// keyframe.cu: the segments of source MLOAM_MSG_SURROUND (the filtered surf map, then the filtered corner map) or MLOAM_MSG_GLOBAL_MAP0 / 1
+// into seg[0..]; returns their count (1 or 2).  The caller has checked that the store exists.
+int keyframe_msg_segments(const Ctx *c, int source, PackSeg *seg);
 
 // comm.cu: in-place sum over ranks on the context stream (no-op without a communicator)
 int comm_allreduce_doubles(Ctx *c, double *d_buf, int count);

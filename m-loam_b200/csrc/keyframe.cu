@@ -179,6 +179,7 @@ struct KeyframeStore {
     int n[2] = {0, 0};                    // filtered sizes
     const float4 *pts[2] = {nullptr, nullptr};
     const float *cov6[2] = {nullptr, nullptr};
+    const float *trace[2] = {nullptr, nullptr};  // cov_trace as the filter stored it (mloam_cloud_msgs)
     std::vector<int> chosen;              // keyframe ids the position filter chose, in filter order
   } gm;
   void release() {
@@ -210,6 +211,21 @@ void keyframes_release(Ctx *c) {
   c->kf->release();
   delete c->kf;
   c->kf = nullptr;
+}
+
+int keyframe_msg_segments(const Ctx *c, int source, PackSeg *seg) {
+  const KeyframeStore &S = *c->kf;
+  if (source == MLOAM_MSG_SURROUND) {  // laser_cloud_surf_from_map_cov_ds + laser_cloud_corner_from_map_cov_ds (:789)
+    for (int t = 0; t < 2; t++) {
+      const int m = S.map_n[t];
+      const KeyframeStore::Filt F = m > 0 ? S.filt_layout(t) : KeyframeStore::Filt{nullptr, nullptr, nullptr, 0};
+      seg[t] = PackSeg{F.pts, F.cov6, F.trace, nullptr, m, 0};
+    }
+    return 2;
+  }
+  const int m = source - MLOAM_MSG_GLOBAL_MAP0, n = S.gm.n[m];
+  seg[0] = n > 0 ? PackSeg{S.gm.pts[m], S.gm.cov6[m], S.gm.trace[m], nullptr, n, 0} : PackSeg{nullptr, nullptr, nullptr, nullptr, 0, 0};
+  return 1;
 }
 
 namespace {
@@ -724,7 +740,7 @@ int mloam_global_map(mloam_ctx_t *h, int mode, const double *center7, double rad
     MLOAM_CUDA_OK(c, carve(G.out[m], [&](Carve &cv) {
       op = cv.take<float4>(M1), oc6 = cv.take<float>(6 * M1), otr = cv.take<float>(M1), d_out_n[m] = cv.take<int>(16);
     }));
-    G.pts[m] = op, G.cov6[m] = oc6;
+    G.pts[m] = op, G.cov6[m] = oc6, G.trace[m] = otr;
     if (tot[m] == 0) {
       MLOAM_CUDA_OK(c, cudaMemsetAsync(d_out_n[m], 0, sizeof(int), st));
     } else {

@@ -17,6 +17,7 @@
 #pragma once
 #include <cmath>
 #include <cstring>
+#include <initializer_list>
 #include <limits>
 #include <memory>
 #include <stdexcept>
@@ -25,6 +26,7 @@
 
 #include "../../include/mloam_b200.h"
 #include "mloam_context.hpp"
+#include "mloam_io.hpp"
 
 namespace mloam {
 
@@ -512,5 +514,38 @@ inline void frameRegistered(mloam_ctx_t *ctx, common::PointICloud &full_res, com
   frameRegistered(ctx, MLOAM_REGISTERED_FULL_RES, full_res);
   frameRegistered(ctx, MLOAM_REGISTERED_SURF, surf_last);
   frameRegistered(ctx, MLOAM_REGISTERED_CORNER, corner_last);
+}
+}  // namespace mloam
+
+// ---- pcl::toROSMsg of the published clouds (pubPointCloud :690-714, pubGlobalMap :780-851), packed on the device by one launch:
+//   mloam::toROSMsg(ctx, {MLOAM_MSG_FULL_RES, MLOAM_MSG_SURF_LAST, MLOAM_MSG_CORNER_LAST},
+//                   {&laser_cloud_full_res_msg, &laser_cloud_surf_last_msg, &laser_cloud_corner_last_msg});
+//   mloam::toROSMsg(ctx, MLOAM_MSG_GLOBAL_MAP0, laser_cloud_map_msg);
+// in place of the pointAssociateToMap loops and pcl::toROSMsg; setting header.stamp / frame_id and publishing stay the caller's.  Each
+// message's data buffer is reused, so publishers that keep their messages pay one launch a call.  A template on the message type
+// (sensor_msgs::PointCloud2), so that this header still compiles in a tree without ROS.
+namespace mloam {
+template <typename PointCloud2>
+inline void toROSMsg(mloam_ctx_t *ctx, const std::vector<int> &sources, std::initializer_list<PointCloud2 *> msgs) {
+  const std::vector<PointCloud2 *> out(msgs);
+  if (out.size() != sources.size()) throw std::invalid_argument("toROSMsg: one message per source");
+  std::vector<std::vector<uint8_t> *> data;
+  for (PointCloud2 *m : out) data.push_back(&m->data);
+  std::vector<int> width;
+  check(ctx, io::cloudMsgs(ctx, sources, data, width), "mloam_cloud_msgs");
+  for (size_t k = 0; k < out.size(); k++) {
+    const io::PointCloud2View v = io::cloudMsgView(sources[k], (size_t)width[k], data[k]->data());
+    PointCloud2 &m = *out[k];
+    m.height = v.height, m.width = v.width, m.is_bigendian = v.is_bigendian, m.point_step = v.point_step, m.row_step = v.row_step;
+    m.is_dense = v.is_dense;
+    m.fields.resize(v.fields.size());
+    for (size_t f = 0; f < v.fields.size(); f++)
+      m.fields[f].name = v.fields[f].name, m.fields[f].offset = v.fields[f].offset, m.fields[f].datatype = v.fields[f].datatype,
+      m.fields[f].count = v.fields[f].count;
+  }
+}
+template <typename PointCloud2>
+inline void toROSMsg(mloam_ctx_t *ctx, int source, PointCloud2 &msg) {
+  toROSMsg(ctx, {source}, {&msg});
 }
 }  // namespace mloam

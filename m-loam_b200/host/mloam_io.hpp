@@ -42,6 +42,7 @@ struct PointCloud2View {  // the members of sensor_msgs/PointCloud2 the packing 
   const uint8_t *data = nullptr;
   size_t data_size = 0;
   bool has_intensity = false;  // set by unpack
+  bool is_dense = false;       // no point is invalid (sensor_msgs/PointCloud2::is_dense); set by cloudMsgView
 };
 
 namespace detail {
@@ -130,18 +131,23 @@ inline mloam_pc2_msg_t pointCloud2Msg(const PointCloud2View &msg) {
   return m;
 }
 
+namespace detail {
+// the fields pcl::toROSMsg lists for pcl::PointXYZI (n = 4) and mloam_pcl::PointXYZIWithCov (n = 11, point_with_cov.hpp:113-125)
+inline std::vector<PointField> cloud_fields(int n) {
+  static const char *const names[11] = {"x", "y", "z", "intensity", "cov_xx", "cov_xy", "cov_xz", "cov_yy", "cov_yz", "cov_zz", "cov_trace"};
+  static const uint32_t offs[11] = {0, 4, 8, 16, 20, 24, 28, 32, 36, 40, 44};
+  std::vector<PointField> fields(n);
+  for (int i = 0; i < n; i++) fields[i].name = names[i], fields[i].offset = offs[i], fields[i].datatype = FLOAT32, fields[i].count = 1;
+  return fields;
+}
+}  // namespace detail
+
 // float4 points -> the PointCloud2 layout pcl::toROSMsg gives a pcl::PointXYZI cloud: point_step 32, x/y/z at 0/4/8, intensity at 16,
 // unorganised (height 1), little endian.  `storage` receives the bytes the returned view points at.
 inline PointCloud2View packPointCloud2(const mloam_point_t *pts, size_t n, std::vector<uint8_t> &storage) {
   PointCloud2View msg;
   msg.height = 1, msg.width = (uint32_t)n, msg.point_step = 32, msg.row_step = (uint32_t)(32 * n), msg.is_bigendian = false;
-  const char *names[4] = {"x", "y", "z", "intensity"};
-  const uint32_t offs[4] = {0, 4, 8, 16};
-  for (int i = 0; i < 4; i++) {
-    PointField f;
-    f.name = names[i], f.offset = offs[i], f.datatype = FLOAT32, f.count = 1;
-    msg.fields.push_back(f);
-  }
+  msg.fields = detail::cloud_fields(4);
   storage.assign(32 * n, 0);
   for (size_t i = 0; i < n; i++) {
     std::memcpy(&storage[32 * i], &pts[i].x, 12);
@@ -149,6 +155,64 @@ inline PointCloud2View packPointCloud2(const mloam_point_t *pts, size_t n, std::
   }
   msg.data = storage.data(), msg.data_size = storage.size(), msg.has_intensity = true;
   return msg;
+}
+
+// float4 points with cov_vec (6 floats per point: xx xy xz yy yz zz) and cov_trace -> the PointCloud2 layout pcl::toROSMsg gives a
+// mloam_pcl::PointXYZIWithCov cloud: point_step 48, x/y/z at 0/4/8, intensity at 16, cov_xx .. cov_zz at 20 .. 40, cov_trace at 44,
+// unorganised, little endian; bytes 12-15 are zero.  `storage` receives the bytes the returned view points at.
+inline PointCloud2View packPointCloud2Cov(const mloam_point_t *pts, const float *cov6, const float *trace, size_t n,
+                                          std::vector<uint8_t> &storage) {
+  PointCloud2View msg;
+  msg.height = 1, msg.width = (uint32_t)n, msg.point_step = 48, msg.row_step = (uint32_t)(48 * n), msg.is_bigendian = false;
+  msg.fields = detail::cloud_fields(11);
+  storage.assign(48 * n, 0);
+  for (size_t i = 0; i < n; i++) {
+    std::memcpy(&storage[48 * i], &pts[i].x, 12);
+    std::memcpy(&storage[48 * i + 16], &pts[i].intensity, 4);
+    std::memcpy(&storage[48 * i + 20], cov6 + 6 * i, 24);
+    std::memcpy(&storage[48 * i + 44], trace + i, 4);
+  }
+  msg.data = storage.data(), msg.data_size = storage.size(), msg.has_intensity = true;
+  return msg;
+}
+
+// point_step of a mloam_cloud_msgs* source: 32 (PointXYZI) or 48 (PointXYZIWithCov)
+inline uint32_t cloudMsgStep(int source) { return source >= MLOAM_MSG_SURROUND ? 48u : 32u; }
+
+// The PointCloud2 a message of mloam_cloud_msgs* is: `width` points of `source` (MLOAM_MSG_*) at data, its fields, steps and is_dense —
+// false for MLOAM_MSG_FULL_RES, which holds the sweep's non-finite points, true for the others.  The bytes stay the caller's.
+inline PointCloud2View cloudMsgView(int source, size_t width, const uint8_t *data) {
+  PointCloud2View msg;
+  msg.height = 1, msg.width = (uint32_t)width, msg.point_step = cloudMsgStep(source), msg.row_step = (uint32_t)(msg.point_step * width);
+  msg.is_bigendian = false, msg.is_dense = source != MLOAM_MSG_FULL_RES;
+  msg.fields = detail::cloud_fields(msg.point_step == 48 ? 11 : 4);
+  msg.data = data, msg.data_size = (size_t)msg.point_step * width, msg.has_intensity = true;
+  return msg;
+}
+
+// mloam_cloud_msgs of `sources` into data[k], each resized to its message (width[k] x cloudMsgStep bytes).  The buffers' capacities are
+// offered first, so a caller that keeps its buffers from frame to frame pays one launch per call; a message that outgrew its buffer
+// costs a second call.  Returns the library's code.
+inline int cloudMsgs(mloam_ctx_t *ctx, const std::vector<int> &sources, std::vector<std::vector<uint8_t> *> &data, std::vector<int> &width) {
+  const size_t n = sources.size();
+  std::vector<void *> dst(n);
+  std::vector<size_t> cap(n);
+  width.assign(n, 0);
+  int rc = MLOAM_OK;
+  for (int pass = 0; pass < 2; pass++) {
+    for (size_t k = 0; k < n; k++) {
+      std::vector<uint8_t> &d = *data[k];
+      d.resize(pass == 0 ? d.capacity() : (size_t)width[k] * cloudMsgStep(sources[k]));
+      dst[k] = d.empty() ? nullptr : d.data(), cap[k] = d.size();
+    }
+    rc = mloam_cloud_msgs(ctx, (int)n, sources.data(), dst.data(), cap.data(), width.data());
+    bool fit = true;
+    for (size_t k = 0; k < n; k++) fit = fit && (size_t)width[k] * cloudMsgStep(sources[k]) <= cap[k];
+    if (!fit && pass == 0) continue;  // too small (MLOAM_E_INVALID), or an empty buffer taken as a size query
+    break;
+  }
+  for (size_t k = 0; k < n && rc == MLOAM_OK; k++) data[k]->resize((size_t)width[k] * cloudMsgStep(sources[k]));
+  return rc;
 }
 
 // ---- mloam_msgs (header reduced to stamp + frame_id; nav_msgs/Odometry and PoseWithCovarianceStamped to what the nodes fill)

@@ -548,3 +548,20 @@ inline bool frameMsg(mloam_ctx_t *ctx, const std::vector<io::PointCloud2View> &m
   return st.ran != 0;
 }
 }  // namespace mloam
+
+// ----------------------------------------------------------------------------------------------- published clouds as PointCloud2
+namespace mloam {
+// pcl::toROSMsg of the clouds pubPointCloud (lidar_mapper_keyframe.cpp:690-714) and pubGlobalMap (:780-851) publish, packed on the
+// device by one launch: sources[k] (MLOAM_MSG_*) into storage[k], which the returned views point at.  Keep the storage from call to
+// call, so that its capacity is reused.
+inline std::vector<io::PointCloud2View> cloudMsgs(mloam_ctx_t *ctx, const std::vector<int> &sources, std::vector<std::vector<uint8_t>> &storage) {
+  storage.resize(sources.size());
+  std::vector<std::vector<uint8_t> *> data;
+  for (auto &s : storage) data.push_back(&s);
+  std::vector<int> width;
+  check(ctx, io::cloudMsgs(ctx, sources, data, width), "mloam_cloud_msgs");
+  std::vector<io::PointCloud2View> views;
+  for (size_t k = 0; k < sources.size(); k++) views.push_back(io::cloudMsgView(sources[k], (size_t)width[k], storage[k].data()));
+  return views;
+}
+}  // namespace mloam
