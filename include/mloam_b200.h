@@ -613,6 +613,27 @@ int mloam_calib_frame(mloam_ctx_t *ctx, const mloam_point_t *h_surf_ref, int n_s
                       int n_corner_cal, const double *pose_pivot7, double *pose_i7, const double *ext_ref7, double *ext_cal7,
                       int max_outer, int max_inner, double huber_a, int own_cal_maps, mloam_solve_stats_t *stats);
 
+/* ---- the same step over the whole rig (estimator.cpp:633-642, 670-787, ESTIMATE_EXTRINSIC == 1 with NUM_OF_LASER = n_lidars): every
+ * non-reference extrinsic is free in one problem, with one trust region.  h_surf / h_corner hold n_lidars clouds (sensor frame),
+ * concatenated in LiDAR order, surf_counts[n] / corner_counts[n] points each.
+ *   cloud idx_ref: frame i's features, matched at pivot^-1 * pose_i * ext_ref against MLOAM_MAP_CORNER / _SURF with n_neigh 5 ->
+ *     LidarPureOdom* rows on pose_i; ext7s[idx_ref] is a constant block (:642);
+ *   cloud n != idx_ref: the calibrated LiDAR's pivot-frame (or accumulated) features, matched at ext7s[n] against
+ *     MLOAM_MAP_SCAN_CORNER / _SCAN_SURF (own_cal_maps != 0) or the same maps, n_neigh 10 -> LidarOnlineCalib* rows on ext7s[n].
+ * CHECK_FOV is true throughout; the association is redone at every outer iteration, as in mloam_calib_frame.
+ * prior_pos / prior_rot != 0 (prior_factor: 1, :675-685): PriorFactor(prior7s[n], PRIOR_FACTOR_POS, PRIOR_FACTOR_ROT) without loss on
+ * every extrinsic (prior_factor.hpp:27-72, its rotation Jacobian as written); the constant ext_ref's prior adds to the cost only.
+ * prior_pos = prior_rot = 0: no prior blocks (prior7s may be NULL).  HuberLoss(huber_a) on the features, max_outer x (re-association
+ * + <= max_inner LM iterations).  With n_lidars = 2 and no prior the result equals mloam_calib_frame's bit for bit.
+ * pose_i7 and ext7s are in/out.  stats->n_surf = feature rows of the last evaluation, stats->H = the pose_i block; h_rows (nullable,
+ * n_lidars) = each LiDAR's feature rows of the last evaluation.  The launches per call do not depend on n_lidars.  Single GPU:
+ * MLOAM_E_STATE with a communicator attached (the two-rank calibration is mloam_calib_frame).  MLOAM_E_INVALID: n_lidars outside
+ * 2..16, a bad idx_ref, a negative count, a non-finite pose, extrinsic, prior or scale.  The frame path's state is left alone. */
+int mloam_calib_rig(mloam_ctx_t *ctx, int n_lidars, int idx_ref, const mloam_point_t *h_surf, const int *surf_counts,
+                    const mloam_point_t *h_corner, const int *corner_counts, const double *pose_pivot7, double *pose_i7, double *ext7s,
+                    const double *prior7s, double prior_pos, double prior_rot, int max_outer, int max_inner, double huber_a,
+                    int own_cal_maps, mloam_solve_stats_t *stats, int *h_rows);
+
 /* ---- ActiveFeatureSelection::goodFeatureMatching for one feature set (lidar_mapper.h:229-573; Estimator::goodFeatureMatching,
  * estimator.cpp:1347-1517): match every feature of `h_pts` against map `slot` at pose7, evaluate its 1x6 Jacobian row
  * (evaluateFeatJacobianMatching, lidar_mapper.h:130-174; sqrt_info from the point's covariance h_cov6[n*6] — PointIWithCov::cov_vec —

@@ -33,7 +33,7 @@ ABI_SYMBOLS = [
     "mloam_profile_reset", "mloam_project_cloud", "mloam_frame_set_next", "mloam_frame_set_next_device", "mloam_extract_features", "mloam_extract_debug", "mloam_voxel_downsample", "mloam_map_build",
     "mloam_map_build_device", "mloam_map_size", "mloam_knn", "mloam_match_from_map", "mloam_factor_evaluate",
     "mloam_normal_equations", "mloam_pose_plus", "mloam_scan2map", "mloam_scan2map_device", "mloam_frame",
-    "mloam_frame_device", "mloam_set_extrinsic", "mloam_set_lidars", "mloam_calib_frame", "mloam_compound_pose_cov", "mloam_cloud_uct_associate", "mloam_voxel_downsample_cov", "mloam_submap_assemble", "mloam_good_features_odom", "mloam_local_map_build", "mloam_match_from_scan", "mloam_track_cloud", "mloam_odom_solve", "mloam_point_uncertainty", "mloam_scan2map_ua", "mloam_good_features", "mloam_comm_unique_id", "mloam_comm_init", "mloam_comm_destroy", "mloam_comm_p2p_export", "mloam_comm_p2p_init", "mloam_comm_p2p_reset",
+    "mloam_frame_device", "mloam_set_extrinsic", "mloam_set_lidars", "mloam_calib_frame", "mloam_calib_rig", "mloam_compound_pose_cov", "mloam_cloud_uct_associate", "mloam_voxel_downsample_cov", "mloam_submap_assemble", "mloam_good_features_odom", "mloam_local_map_build", "mloam_match_from_scan", "mloam_track_cloud", "mloam_odom_solve", "mloam_point_uncertainty", "mloam_scan2map_ua", "mloam_good_features", "mloam_comm_unique_id", "mloam_comm_init", "mloam_comm_destroy", "mloam_comm_p2p_export", "mloam_comm_p2p_init", "mloam_comm_p2p_reset",
     "mloam_set_uncertainty", "mloam_pose_covariance", "mloam_frame_scan",
     "mloam_keyframes_init", "mloam_keyframe_save", "mloam_keyframe_submap", "mloam_keyframe_query", "mloam_keyframe_scan",
     "mloam_global_map", "mloam_global_map_read", "mloam_global_map_chosen",
@@ -579,6 +579,30 @@ class Context:
         self._ck(lib().mloam_calib_frame(self._h, _p(sr), n[0], _p(cr), n[1], _p(sc), n[2], _p(cc), n[3], _p(pv), _p(pi), _p(er), _p(ec),
                                          max_outer, max_inner, C.c_double(huber_a), int(own_cal_maps), C.byref(st)))
         return pi, ec, st.as_dict()
+
+    def calib_rig(self, surf, corner, pivot7, pose_i7, ext7s, idx_ref: int = 0, prior7s=None, prior_pos: float = 0.0, prior_rot: float = 0.0,
+                  max_outer: int = 2, max_inner: int = 4, huber_a: float = 1.0, own_cal_maps: bool = False):
+        """mloam_calib_rig: surf / corner are per-LiDAR clouds (None or empty: no features).  Returns (pose_i, ext7s [L, 7], stats, rows [L])."""
+        L = len(surf)
+        if len(corner) != L:
+            raise ValueError(f"calib_rig: {L} surf clouds but {len(corner)} corner clouds")
+        sc = [np.zeros((0, 4), np.float32) if x is None or len(x) == 0 else _cloud(x) for x in surf]
+        cc = [np.zeros((0, 4), np.float32) if x is None or len(x) == 0 else _cloud(x) for x in corner]
+        ns = np.array([x.shape[0] for x in sc], np.int32)
+        nc = np.array([x.shape[0] for x in cc], np.int32)
+        hs = np.ascontiguousarray(np.concatenate(sc), np.float32) if ns.sum() else None
+        hc = np.ascontiguousarray(np.concatenate(cc), np.float32) if nc.sum() else None
+        pv = np.ascontiguousarray(pivot7, np.float64)
+        pi = np.array(pose_i7, np.float64)
+        ex = np.array(ext7s, np.float64)
+        pr = None if prior7s is None else np.ascontiguousarray(prior7s, np.float64)
+        if ex.shape != (L, 7) or (pr is not None and pr.shape != (L, 7)) or pv.shape != (7,) or pi.shape != (7,):
+            raise ValueError(f"calib_rig: {L} LiDARs need ext7s / prior7s of shape ({L}, 7) and 7-vector poses")
+        rows = np.zeros(L, np.int32)
+        st = SolveStats()
+        self._ck(lib().mloam_calib_rig(self._h, L, idx_ref, _p(hs), _p(ns), _p(hc), _p(nc), _p(pv), _p(pi), _p(ex), _p(pr), C.c_double(prior_pos),
+                                       C.c_double(prior_rot), max_outer, max_inner, C.c_double(huber_a), int(own_cal_maps), C.byref(st), _p(rows)))
+        return pi, ex, st.as_dict(), rows
 
     def local_map_build(self, slot: int, clouds, pose_local7, leaf: float, map_cell: float = 0.0):
         clouds = [_cloud(x) for x in clouds]

@@ -411,6 +411,7 @@ struct Ctx {
   DevBuf voxel_corner, voxel_surf;  // the frame's two scan filters, on two streams at once; the look-ahead branch forks after them
   DevBuf host_work;               // host entry points: work and output staging (good features, kNN, factors, scan2map_ua, ...)
   DevBuf odom_work;               // OdomState + partials of mloam_odom_solve / mloam_calib_frame
+  DevBuf rig_work;                // mloam_calib_rig: the rig's features, their matches and fits, RigState, partials (calib_rig.cu)
   // association work (uct.h uct_bufs) of the keyframe submap and the host entry points: never inside a frame, so it shares the
   // corner submap upload's allocation
   DevBuf &assoc_work() { return map_in[1]; }

@@ -1,6 +1,6 @@
 // mloam_adapter.hpp — the hot-path classes with the REFERENCE'S OWN types (PCL clouds, Eigen vectors, Ceres bases), for a tree that
 // has PCL / Eigen / Ceres: include it INSTEAD of estimator/src/imageSegmenter/image_segmenter.hpp, featureExtract/feature_extract.hpp, lidarTracker/lidar_tracker.h,
-// factor/pose_local_parameterization.h and factor/lidar_{map,scan,pure_odom,online_calib}_factor.hpp, AFTER the reference's
+// factor/pose_local_parameterization.h, factor/lidar_{map,scan,pure_odom,online_calib}_factor.hpp and factor/prior_factor.hpp, AFTER the reference's
 // parameters.h (ScanInfo, cloudFeature, PointPlaneFeature), pose.h (Pose) and <pcl/point_cloud.h>, <Eigen/Dense>, <ceres/ceres.h>.
 //
 // What keeps compiling unchanged: every call of FeatureExtract::extractCloud / match*FromMap / match*FromScan / match*PointFromMap
@@ -359,6 +359,47 @@ MLOAM_FACTOR(LidarOnlineCalibEdgeFactor, 1, 1, 1, Eigen::VectorXd, 6, double, 1.
 MLOAM_ODOM_FACTOR(LidarPureOdomPlaneNormFactor, 3, Eigen::Vector4d, 4);
 MLOAM_ODOM_FACTOR(LidarPureOdomEdgeFactor, 4, Eigen::VectorXd, 6);
 #undef MLOAM_ODOM_FACTOR
+// prior_factor.hpp:27-72 — PriorFactor(pos, rot, pos_scale, rot_scale) on one pose block, evaluated on the host (6 residuals):
+// residual = diag(pos_scale I3, rot_scale I3) [P - pos ; 2 (rot^-1 Q).vec], jacobian = the same scales times diag(I3,
+// LeftQuatMatrix(Q^-1 rot).topLeftCorner<3,3>()) with a zero 7th column — as the reference writes it (its comment: "seem to be
+// wrong"), so that a problem built with it is the one the reference solves.  Eigen's inverse() is conjugate / squaredNorm.  The same
+// statement is what mloam_calib_rig adds on the device.
+class PriorFactor : public ceres::SizedCostFunction<6, 7> {
+ public:
+  PriorFactor(const Eigen::Vector3d &pos, const Eigen::Quaterniond &rot, const double &pos_scale, const double &rot_scale)
+      : pos_scale_(pos_scale), rot_scale_(rot_scale) {
+    x0_[0] = pos(0), x0_[1] = pos(1), x0_[2] = pos(2), x0_[3] = rot.x(), x0_[4] = rot.y(), x0_[5] = rot.z(), x0_[6] = rot.w();
+  }
+  bool Evaluate(double const *const *param, double *residuals, double **jacobians) const {
+    const double *x = param[0];
+    const double q[4] = {x[3], x[4], x[5], x[6]}, r0[4] = {x0_[3], x0_[4], x0_[5], x0_[6]};
+    double qi[4], e[4];
+    inv(r0, qi), mul(qi, q, e);
+    for (int k = 0; k < 3; k++) residuals[k] = pos_scale_ * (x[k] - x0_[k]), residuals[3 + k] = rot_scale_ * (2 * e[k]);
+    if (jacobians && jacobians[0]) {
+      double m[4];
+      inv(q, qi), mul(qi, r0, m);
+      const double L[9] = {m[3], -m[2], m[1], m[2], m[3], -m[0], -m[1], m[0], m[3]};  // w I + [v]x
+      double *J = jacobians[0];
+      for (int k = 0; k < 42; k++) J[k] = 0.0;
+      for (int k = 0; k < 3; k++) J[k * 7 + k] = pos_scale_;
+      for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) J[(3 + i) * 7 + 3 + j] = rot_scale_ * L[i * 3 + j];
+    }
+    return true;
+  }
+
+ private:
+  static void inv(const double *q, double *o) {  // [x y z w]
+    const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+    o[0] = -q[0] / n2, o[1] = -q[1] / n2, o[2] = -q[2] / n2, o[3] = q[3] / n2;
+  }
+  static void mul(const double *a, const double *b, double *o) {
+    o[0] = a[3] * b[0] + a[0] * b[3] + a[1] * b[2] - a[2] * b[1], o[1] = a[3] * b[1] + a[1] * b[3] + a[2] * b[0] - a[0] * b[2];
+    o[2] = a[3] * b[2] + a[2] * b[3] + a[0] * b[1] - a[1] * b[0], o[3] = a[3] * b[3] - a[0] * b[0] - a[1] * b[1] - a[2] * b[2];
+  }
+  double x0_[7], pos_scale_, rot_scale_;
+};
 
 // ----------------------------------------------------------------------------------------------- LidarTracker
 class LidarTracker {
@@ -547,5 +588,48 @@ inline void toROSMsg(mloam_ctx_t *ctx, const std::vector<int> &sources, std::ini
 template <typename PointCloud2>
 inline void toROSMsg(mloam_ctx_t *ctx, int source, PointCloud2 &msg) {
   toROSMsg(ctx, {source}, {&msg});
+}
+}  // namespace mloam
+
+// ---- Estimator::optimizeMap with ESTIMATE_EXTRINSIC == 1 over the whole rig (estimator.cpp:633-642, 670-787): one call in place of the
+// problem assembly (PriorFactor on every extrinsic when PRIOR_FACTOR, LidarPureOdom* of IDX_REF's frame-i features on pose_i,
+// LidarOnlineCalib* of every other LiDAR's features on its extrinsic) and ceres::Solve:
+//   mloam::calibRig(ctx, IDX_REF, surf, corner, pose_pivot, pose_i, pose_ext, PRIOR_FACTOR ? &pose_ext : nullptr, PRIOR_FACTOR_POS,
+//                   PRIOR_FACTOR_ROT, max_outer, NUM_ITERATIONS);
+// surf[n] / corner[n]: LiDAR n's features in its sensor frame (frame i for IDX_REF, the pivot or the accumulation for the others).
+// pose_i and pose_ext (one Pose per LiDAR, pose_ext[IDX_REF] constant) are in/out; prior: the PriorFactor targets (tbl_ / qbl_), copied
+// before the call, so the extrinsics themselves may be passed.  rows (nullable): each LiDAR's feature rows of the last evaluation.
+namespace mloam {
+inline mloam_solve_stats_t calibRig(mloam_ctx_t *ctx, size_t idx_ref, const std::vector<common::PointICloud> &surf,
+                                    const std::vector<common::PointICloud> &corner, const Pose &pose_pivot, Pose &pose_i, std::vector<Pose> &pose_ext,
+                                    const std::vector<Pose> *prior, double prior_pos, double prior_rot, int max_outer, int max_inner,
+                                    bool own_cal_maps = false, std::vector<int> *rows = nullptr, double huber_a = 1.0) {
+  const size_t L = pose_ext.size();
+  if (surf.size() != L || corner.size() != L || (prior && prior->size() != L)) throw std::invalid_argument("calibRig: one cloud / prior per LiDAR");
+  std::vector<mloam_point_t> s, c;
+  std::vector<int> ns(L), nc(L), r(L);
+  for (size_t n = 0; n < L; n++) {
+    const std::vector<mloam_point_t> a = packCloud(surf[n]), b = packCloud(corner[n]);
+    s.insert(s.end(), a.begin(), a.end()), c.insert(c.end(), b.begin(), b.end());
+    ns[n] = (int)a.size(), nc[n] = (int)b.size();
+  }
+  std::vector<double> ext(7 * L), pr(prior ? 7 * L : 0);
+  for (size_t n = 0; n < L; n++) {
+    poseToParam(pose_ext[n], &ext[7 * n]);
+    if (prior) poseToParam((*prior)[n], &pr[7 * n]);
+  }
+  double pv[7], pi[7];
+  poseToParam(pose_pivot, pv), poseToParam(pose_i, pi);
+  mloam_solve_stats_t st;
+  check(ctx, mloam_calib_rig(ctx, (int)L, (int)idx_ref, s.data(), ns.data(), c.data(), nc.data(), pv, pi, ext.data(), prior ? pr.data() : nullptr,
+                             prior ? prior_pos : 0.0, prior ? prior_rot : 0.0, max_outer, max_inner, huber_a, own_cal_maps ? 1 : 0, &st, r.data()),
+        "mloam_calib_rig");
+  pose_i.q_ = Eigen::Quaterniond(pi[6], pi[3], pi[4], pi[5]), pose_i.t_ = Eigen::Vector3d(pi[0], pi[1], pi[2]);
+  for (size_t n = 0; n < L; n++) {
+    const double *x = &ext[7 * n];
+    pose_ext[n].q_ = Eigen::Quaterniond(x[6], x[3], x[4], x[5]), pose_ext[n].t_ = Eigen::Vector3d(x[0], x[1], x[2]);
+  }
+  if (rows) *rows = r;
+  return st;
 }
 }  // namespace mloam

@@ -565,3 +565,42 @@ inline std::vector<io::PointCloud2View> cloudMsgs(mloam_ctx_t *ctx, const std::v
   return views;
 }
 }  // namespace mloam
+
+// ---- Estimator::optimizeMap with ESTIMATE_EXTRINSIC == 1 over the whole rig (estimator.cpp:633-642, 670-787): mloam_calib_rig on ctx.
+// surf[n] / corner[n]: LiDAR n's features (sensor frame); pose_i and pose_ext (one per LiDAR, pose_ext[idx_ref] constant) in/out; prior
+// (nullable): the PriorFactor targets tbl_ / qbl_ with prior_pos / prior_rot (prior_factor.hpp:27-72).  rows (nullable): each LiDAR's
+// feature rows of the last evaluation.
+namespace mloam {
+inline mloam_solve_stats_t calibRig(mloam_ctx_t *ctx, int idx_ref, const std::vector<common::PointICloud> &surf, const std::vector<common::PointICloud> &corner,
+                                    const Pose &pose_pivot, Pose &pose_i, std::vector<Pose> &pose_ext, const std::vector<Pose> *prior, double prior_pos,
+                                    double prior_rot, int max_outer, int max_inner, bool own_cal_maps = false, std::vector<int> *rows = nullptr,
+                                    double huber_a = 1.0) {
+  const size_t L = pose_ext.size();
+  if (surf.size() != L || corner.size() != L || (prior && prior->size() != L)) throw std::invalid_argument("calibRig: one cloud / prior per LiDAR");
+  std::vector<mloam_point_t> s, c;
+  std::vector<int> ns(L), nc(L), r(L);
+  for (size_t n = 0; n < L; n++) {
+    const std::vector<mloam_point_t> a = pack(surf[n]), b = pack(corner[n]);
+    s.insert(s.end(), a.begin(), a.end()), c.insert(c.end(), b.begin(), b.end());
+    ns[n] = (int)a.size(), nc[n] = (int)b.size();
+  }
+  std::vector<double> ext(7 * L), pr(prior ? 7 * L : 0);
+  for (size_t n = 0; n < L; n++) {
+    pose_ext[n].toParam(&ext[7 * n]);
+    if (prior) (*prior)[n].toParam(&pr[7 * n]);
+  }
+  double pv[7], pi[7];
+  pose_pivot.toParam(pv), pose_i.toParam(pi);
+  mloam_solve_stats_t st;
+  check(ctx, mloam_calib_rig(ctx, (int)L, idx_ref, s.data(), ns.data(), c.data(), nc.data(), pv, pi, ext.data(), prior ? pr.data() : nullptr,
+                             prior ? prior_pos : 0.0, prior ? prior_rot : 0.0, max_outer, max_inner, huber_a, own_cal_maps ? 1 : 0, &st, r.data()),
+        "mloam_calib_rig");
+  pose_i.t_ = {{pi[0], pi[1], pi[2]}}, pose_i.q_ = {{pi[3], pi[4], pi[5], pi[6]}};  // as solved: PoseLocalParameterization normalised it
+  for (size_t n = 0; n < L; n++) {
+    const double *x = &ext[7 * n];
+    pose_ext[n].t_ = {{x[0], x[1], x[2]}}, pose_ext[n].q_ = {{x[3], x[4], x[5], x[6]}};
+  }
+  if (rows) *rows = r;
+  return st;
+}
+}  // namespace mloam
