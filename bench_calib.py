@@ -1,9 +1,9 @@
 """bench_calib.py — the C3 workload of bench.py (BASELINE.json configs[2]): 2 LiDARs, 64 x 2048 sweeps, 2M-point local map,
 12-DoF online extrinsic calibration.  A step is one calibration step of Estimator::optimizeMap with ESTIMATE_EXTRINSIC == 1
-(mloam_calib_frame): upload of the two LiDARs' window-level features, GN_ITERS x (buildCalibMap association of both groups +
-residuals / Jacobians + 12x12 normal equations + LM step), local maps uploaded + rebuilt on keyframe steps.
---gpus 2: rank 0 holds the reference LiDAR's features, rank 1 the calibrated LiDAR's; one ncclAllReduce of the packed 12x12 normal
-equations (92 doubles) per LM evaluation.  --gpus 1: both groups in one context."""
+(mloam_calib_frame, the two-LiDAR case of mloam_calib_rig): upload of the two LiDARs' window-level features, GN_ITERS x (buildCalibMap
+association of both groups + residuals / Jacobians + the per-block 6x6 normal equations + LM step), local maps uploaded + rebuilt on
+keyframe steps.  --gpus 2: rank 0 holds the reference LiDAR's features, rank 1 the calibrated LiDAR's; one ncclAllReduce of both
+blocks' packed normal equations and the cost (57 doubles) per LM evaluation.  --gpus 1: both groups in one context."""
 from __future__ import annotations
 
 import os
@@ -56,7 +56,7 @@ def gpu_measure_calib(m, syn, torch, dist, cfg_name, cfg, args, rank, local_rank
         uid = [m.Context.comm_unique_id() if rank == 0 else None]
         dist.broadcast_object_list(uid, src=0)
         ctx.comm_init(world, rank, uid[0])
-        exchange = "ncclAllReduce of the packed 12x12 normal equations (92 doubles) per LM evaluation"
+        exchange = "ncclAllReduce of the two blocks' packed normal equations and the cost (57 doubles) per LM evaluation"
         dist.barrier()
     cases, map_info = make_calib_workload(syn, cfg, n_frames, args.map)
     KF = max(1, args.keyframe_every)

@@ -604,10 +604,12 @@ int mloam_odom_solve(mloam_ctx_t *ctx, int n, const unsigned char *h_types, cons
  *   calibrated LiDAR, pivot frame : features are matched at ext_cal (n_neigh = 10, CHECK_FOV = true) against slots
  *     MLOAM_MAP_SCAN_CORNER / MLOAM_MAP_SCAN_SURF when own_cal_maps != 0 (its own local map, leaf 0.2, :1103-1109), else the same maps,
  *     and enter as LidarOnlineCalib{PlaneNorm,Edge}Factor on ext_cal (lidar_online_calib_factor.hpp:24-227) — 1x6 rows on ext_cal.
+ * This is the two-LiDAR case of mloam_calib_rig (idx_ref 0, no prior), which also leaves the frame path's state alone.
  * Either group may be empty: with a communicator (mloam_comm_init) rank 0 passes the reference LiDAR's features, rank 1 the
- * calibrated LiDAR's, and the packed 12x12 normal equations (92 doubles) are summed with one ncclAllReduce per LM evaluation
- * (SURVEY.md 8e); every rank applies the identical step.  ceres::Solve: max_outer x (re-association + <= max_inner LM iterations),
- * HuberLoss(huber_a = 1.0, :602).  stats->n_surf = residual rows of the last evaluation (all ranks), stats->H = the pose block. */
+ * calibrated LiDAR's, and each block's packed normal equations and the cost (57 doubles) are summed with one ncclAllReduce per LM
+ * evaluation (SURVEY.md 8e); every rank applies the identical step.  ceres::Solve: max_outer x (re-association + <= max_inner LM
+ * iterations), HuberLoss(huber_a = 1.0, :602).  stats->n_surf = residual rows of the last evaluation (all ranks), stats->H = the pose
+ * block. */
 int mloam_calib_frame(mloam_ctx_t *ctx, const mloam_point_t *h_surf_ref, int n_surf_ref, const mloam_point_t *h_corner_ref,
                       int n_corner_ref, const mloam_point_t *h_surf_cal, int n_surf_cal, const mloam_point_t *h_corner_cal,
                       int n_corner_cal, const double *pose_pivot7, double *pose_i7, const double *ext_ref7, double *ext_cal7,
@@ -624,7 +626,7 @@ int mloam_calib_frame(mloam_ctx_t *ctx, const mloam_point_t *h_surf_ref, int n_s
  * prior_pos / prior_rot != 0 (prior_factor: 1, :675-685): PriorFactor(prior7s[n], PRIOR_FACTOR_POS, PRIOR_FACTOR_ROT) without loss on
  * every extrinsic (prior_factor.hpp:27-72, its rotation Jacobian as written); the constant ext_ref's prior adds to the cost only.
  * prior_pos = prior_rot = 0: no prior blocks (prior7s may be NULL).  HuberLoss(huber_a) on the features, max_outer x (re-association
- * + <= max_inner LM iterations).  With n_lidars = 2 and no prior the result equals mloam_calib_frame's bit for bit.
+ * + <= max_inner LM iterations).  mloam_calib_frame is the two-LiDAR case of this call.
  * pose_i7 and ext7s are in/out.  stats->n_surf = feature rows of the last evaluation, stats->H = the pose_i block; h_rows (nullable,
  * n_lidars) = each LiDAR's feature rows of the last evaluation.  The launches per call do not depend on n_lidars.  Single GPU:
  * MLOAM_E_STATE with a communicator attached (the two-rank calibration is mloam_calib_frame).  MLOAM_E_INVALID: n_lidars outside

@@ -144,8 +144,7 @@ void mloam_ctx_destroy(mloam_ctx_t *h) {
   for (auto &m : c->maps) {
     m.sorted.release(), m.orig.release(), m.cells.release(), m.rank_of.release(), m.tile_sums.release(), m.hdr.release();
   }
-  for (int i = 0; i < 4; i++) c->scan_pts[i].release(), c->feat_valid[i].release(), c->feat_coeff[i].release(), c->feat_nn[i].release(), c->knn_pos[i].release(), c->knn_changed[i].release(), c->knn_anchor[i].release(), c->knn_heavy[i].release();
-  for (int i = 0; i < 2; i++) c->gf_work[i].release();
+  for (int i = 0; i < 2; i++) c->scan_pts[i].release(), c->feat_valid[i].release(), c->feat_coeff[i].release(), c->feat_nn[i].release(), c->knn_pos[i].release(), c->knn_changed[i].release(), c->knn_anchor[i].release(), c->knn_heavy[i].release(), c->gf_work[i].release();
   c->knn_heavy_list.release(), c->knn_trace.release(), c->lin_trace.release(), c->knn_spec.release();
   c->partials.release(), c->lm_state.release();
   for (DevBuf *b : {&c->sweep_in, &c->map_in[0], &c->map_in[1], &c->extract_work, &c->voxel_work, &c->voxel_corner, &c->voxel_surf,
@@ -330,7 +329,7 @@ int mloam_debug_knn_trace(mloam_ctx_t *h, unsigned *out, int n_queries) {
 // that is not double-buffered repeats its one half.  *k: K.
 int mloam_debug_knn_lists(mloam_ctx_t *h, int set, int n, int *pos, float *anchor, unsigned char *changed, int *k) {
   const Ctx *c = h ? &h->c : nullptr;
-  if (!c || set < 0 || set > 3 || n <= 0 || !pos || !anchor || !changed || !k || c->knn_k <= 0) return MLOAM_E_INVALID;
+  if (!c || set < 0 || set > 1 || n <= 0 || !pos || !anchor || !changed || !k || c->knn_k <= 0) return MLOAM_E_INVALID;
   const int K = c->knn_k, half = c->knn_half[set];
   if (c->knn_pos[set].cap < sizeof(int) * (size_t)K * (size_t)(half + n) || c->knn_anchor[set].cap < sizeof(float4) * (size_t)(half + n) ||
       c->knn_changed[set].cap < (size_t)n)

@@ -13,8 +13,9 @@
 //                    cost, reduced in a fixed order without atomics (as k_odom_linearize)
 //   k_rig_lm         the k_odom_lm state machine with one trust region over B blocks, on one warp: lane b scales, damps, factors and
 //                    solves block b; step norm, x_norm and model cost change are summed across blocks in column order, so that a
-//                    two-LiDAR rig without priors repeats mloam_calib_frame's 12-dof arithmetic bit for bit
-// then max_inner x (k_rig_linearize + k_rig_lm) at the candidate.
+//                    two-LiDAR rig without priors repeats the arithmetic of the coupled 12-dof [pose_i | ext_cal] solve bit for bit
+// then max_inner x (k_rig_linearize + k_rig_lm) at the candidate.  mloam_calib_frame is the two-LiDAR case; with its communicator
+// each evaluation adds k_rig_sum_partials and one all-reduce of B * 28 + 1 doubles before k_rig_lm.
 #include <algorithm>
 #include <climits>
 #include <cmath>
@@ -84,7 +85,7 @@ __global__ void k_rig_poses(RigState *st) {
     for (int k = 0; k < 7; k++) o[k] = st->x[b][k];
     return;
   }
-  // pivot^-1 * (pose_i * ext_ref), as k_calib_poses
+  // pivot^-1 * (pose_i * ext_ref)
   const PoseD P = pose_from_param(st->xp), I = pose_from_param(st->x[0]), R = pose_from_param(st->xr);
   const Q4 qpi = qconj(qnormalized(P.q));
   const Q4 q_ir = qmul(I.q, R.q);
@@ -410,15 +411,25 @@ __device__ double rig_gather(RigState *st, const double *ne, const double (*x)[7
   return cost;
 }
 
-__global__ void __launch_bounds__(RIG_THREADS) k_rig_lm(const double *__restrict__ partials, int n_blocks, RigState *st, int mode) {
-  __shared__ double ne[RIG_N];
-  __shared__ double cH[RIG_L][36], cg[RIG_L][6];
-  const int B = st->B, N = B * RIG_PB + 1;
-  for (int k = threadIdx.x; k < N; k += RIG_THREADS) {
+// The N packed sums of one evaluation over the CTAs' partials, CTA after CTA
+__device__ __forceinline__ void rig_sum_partials(const double *__restrict__ partials, int n_blocks, int N, double *ne) {
+  for (int k = threadIdx.x; k < N; k += blockDim.x) {
     double v = 0.0;
     for (int b = 0; b < n_blocks; b++) v += partials[(size_t)b * N + k];
     ne[k] = v;
   }
+}
+
+// The sums a rank contributes to the all-reduce of a collective evaluation
+__global__ void k_rig_sum_partials(const double *__restrict__ partials, int n_blocks, int N, double *__restrict__ ne) {
+  rig_sum_partials(partials, n_blocks, N, ne);
+}
+
+__global__ void __launch_bounds__(RIG_THREADS) k_rig_lm(const double *__restrict__ partials, int n_blocks, RigState *st, int mode) {
+  __shared__ double ne[RIG_N];
+  __shared__ double cH[RIG_L][36], cg[RIG_L][6];
+  const int B = st->B;
+  rig_sum_partials(partials, n_blocks, B * RIG_PB + 1, ne);
   __syncthreads();
   if (threadIdx.x >= 32) return;
   const int lane = threadIdx.x;
@@ -504,6 +515,141 @@ static bool finite_n(const double *v, int n) {
   return true;
 }
 
+// The rig problem after the callers' checks: per-LiDAR clouds and counts, the maps built.  prior7s nullable: no prior.  With a
+// communicator (mloam_calib_frame's two ranks, each holding some LiDARs' features), every evaluation's packed sums and cost are
+// all-reduced before the LM step, so that every rank takes the same step.
+static int calib_rig_solve(Ctx *c, int n_lidars, int idx_ref, const mloam_point_t *const *surf, const int *surf_counts,
+                           const mloam_point_t *const *corner, const int *corner_counts, const double *pose_pivot7, double *pose_i7,
+                           double *ext7s, const double *prior7s, double prior_pos, double prior_rot, int max_outer, int max_inner,
+                           double huber_a, int own_cal_maps, mloam_solve_stats_t *stats, int *h_rows) {
+  const MapStorage *M = c->maps;
+  const bool has_prior = prior7s != nullptr;
+  long long n_surf = 0, n_corner = 0;
+  for (int n = 0; n < n_lidars; n++) n_surf += surf_counts[n], n_corner += corner_counts[n];
+  // blocks: 0 = pose_i (the reference LiDAR's rows), then the calibrated LiDARs in index order
+  int blk_of[RIG_L], lidar_of[RIG_L];
+  for (int n = 0, b = 1; n < n_lidars; n++) {
+    const int bb = n == idx_ref ? 0 : b++;
+    blk_of[n] = bb, lidar_of[bb] = n;
+  }
+  // segments: the reference LiDAR's corner and surf features, then each calibrated LiDAR's
+  RigSegs sets;
+  memset(&sets, 0, sizeof(sets));
+  const int n_total = (int)(n_surf + n_corner);
+  DevBuf &wb = c->rig_work;
+  wb.in_graphs = false;  // no frame graph holds it
+  int nb = 1;
+  {
+    int n_max = 1;
+    for (int n = 0; n < n_lidars; n++) n_max = std::max(n_max, std::max(surf_counts[n], corner_counts[n]));
+    nb = (n_max + RIG_THREADS - 1) / RIG_THREADS;
+    nb = nb < 1 ? 1 : (nb > c->sm_count ? c->sm_count : nb);
+  }
+  float4 *d_pts;
+  RigState *st;
+  double *partials;
+  MLOAM_CUDA_OK(c, carve(wb, [&](Carve &cv) {
+    d_pts = cv.take<float4>((size_t)n_total + 1);
+    sets.pos = cv.take<int>(RIG_KMAX * ((size_t)n_total + 1));
+    sets.valid = cv.take<unsigned char>((size_t)n_total + 1);
+    sets.coeff = cv.take<float>(6 * ((size_t)n_total + 1));
+    st = cv.take<RigState>(1);
+    partials = cv.take<double>((size_t)RIG_N * (nb + 1));  // + the all-reduced sums of a collective evaluation
+  }));
+  sets.pts = d_pts;
+  int off = 0;
+  for (int b = 0; b < n_lidars; b++) {
+    const int n = lidar_of[b];
+    for (int t = 0; t < 2; t++) {  // 0 corner, 1 surf
+      RigSeg &S = sets.s[sets.n_seg++];
+      S.off = off, S.n = t ? surf_counts[n] : corner_counts[n], S.blk = b, S.plane = t, S.kind = b == 0 ? 1 : 2;
+      S.map = (b == 0 ? 0 : 2) + t;
+      const mloam_point_t *src = t ? surf[n] : corner[n];
+      if (S.n > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_pts + off, src, sizeof(float4) * (size_t)S.n, cudaMemcpyHostToDevice, c->stream));
+      off += S.n;
+    }
+  }
+  sets.map[0] = M[MLOAM_MAP_CORNER].view(), sets.map[1] = M[MLOAM_MAP_SURF].view();
+  sets.map[2] = M[own_cal_maps ? MLOAM_MAP_SCAN_CORNER : MLOAM_MAP_CORNER].view();
+  sets.map[3] = M[own_cal_maps ? MLOAM_MAP_SCAN_SURF : MLOAM_MAP_SURF].view();
+  sets.n_total = n_total, sets.B = n_lidars, sets.sel_prune = c->knn_all_searches ? 0 : 1;
+  sets.min_match_sq_dis = c->params.min_match_sq_dis, sets.min_plane_dis = c->params.min_plane_dis, sets.huber_a = huber_a;
+
+  // the initial state goes up whole (the scratch and the LM fields are set by the first evaluation)
+  std::vector<RigState> init(1);
+  RigState &s0 = init[0];
+  memset(&s0, 0, sizeof(s0));
+  for (int k = 0; k < 7; k++) {
+    s0.xp[k] = pose_pivot7[k], s0.xr[k] = ext7s[7 * idx_ref + k], s0.x[0][k] = pose_i7[k];
+    for (int b = 1; b < n_lidars; b++) s0.x[b][k] = ext7s[7 * lidar_of[b] + k];
+    if (has_prior) {
+      s0.prior_ref[k] = prior7s[7 * idx_ref + k];
+      for (int b = 1; b < n_lidars; b++) s0.prior[b][k] = prior7s[7 * lidar_of[b] + k];
+    }
+  }
+  s0.prior_pos = prior_pos, s0.prior_rot = prior_rot, s0.has_prior = has_prior ? 1 : 0, s0.B = n_lidars, s0.max_inner = max_inner;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(st, &s0, sizeof(RigState), cudaMemcpyHostToDevice, c->stream));
+  int *h_done = &c->pinned->done;
+  int nbk = (n_total + RIG_WARPS - 1) / RIG_WARPS, nbf = (n_total + 127) / 128;
+  nbk = nbk > 4 * c->sm_count ? 4 * c->sm_count : nbk;
+  nbf = nbf > 4 * c->sm_count ? 4 * c->sm_count : nbf;
+  const int N = n_lidars * RIG_PB + 1;
+  // one LM evaluation: the per-feature sums at x (use_candidate 0) or at the candidate, then the LM step
+  auto evaluate = [&](int use_candidate, int mode) -> int {
+    k_rig_linearize<<<nb, RIG_THREADS, 0, c->stream>>>(sets, st, use_candidate, partials);
+    c->launches += 2;
+    if (!c->nccl_comm) {
+      k_rig_lm<<<1, RIG_THREADS, 0, c->stream>>>(partials, nb, st, mode);
+      return MLOAM_OK;
+    }
+    double *ne = partials + (size_t)RIG_N * nb;
+    k_rig_sum_partials<<<1, 128, 0, c->stream>>>(partials, nb, N, ne);
+    c->launches++;
+    const int rc = comm_allreduce_doubles(c, ne, N);
+    if (rc) return rc;
+    k_rig_lm<<<1, RIG_THREADS, 0, c->stream>>>(ne, 1, st, mode);
+    return MLOAM_OK;
+  };
+  for (int outer = 0; outer < max_outer; outer++) {
+    k_rig_poses<<<1, 32, 0, c->stream>>>(st);
+    c->launches++;
+    if (n_total > 0) {
+      k_rig_knn<<<nbk, RIG_THREADS, 0, c->stream>>>(sets, st);
+      k_rig_fit<<<nbf, 128, 0, c->stream>>>(sets, st);
+      c->launches += 2;
+    }
+    int rc = evaluate(0, 1);
+    if (rc) return rc;
+    for (int it = 0; it < max_inner; it++) {
+      rc = evaluate(1, 2);
+      if (rc) return rc;
+      if (max_inner > 1) {
+        MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_done, &st->done, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+        MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
+        if (*h_done) break;
+      }
+    }
+  }
+  MLOAM_CUDA_OK(c, cudaGetLastError());
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(&s0, st, sizeof(RigState), cudaMemcpyDeviceToHost, c->stream));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
+  for (int k = 0; k < 7; k++) {
+    pose_i7[k] = s0.x[0][k];
+    for (int b = 1; b < n_lidars; b++) ext7s[7 * lidar_of[b] + k] = s0.x[b][k];
+  }
+  int rows = 0;
+  for (int b = 0; b < n_lidars; b++) rows += s0.rows[b];
+  if (h_rows)
+    for (int n = 0; n < n_lidars; n++) h_rows[n] = s0.rows[blk_of[n]];
+  if (stats) {
+    stats->ran = 1, stats->lm_iterations = s0.total_iterations, stats->termination = s0.termination, stats->final_cost = s0.cost;
+    stats->n_surf = rows;  // feature rows of the last evaluation, all ranks
+    stats->n_surf_in = (int)n_surf, stats->n_corner_in = (int)n_corner;
+    for (int i = 0; i < 36; i++) stats->H[i] = s0.H[0][i];  // pose_i block
+  }
+  return MLOAM_OK;
+}
+
 // Estimator::optimizeMap with ESTIMATE_EXTRINSIC == 1 for one frame i and the whole rig: see include/mloam_b200.h.
 extern "C" int mloam_calib_rig(mloam_ctx_t *h, int n_lidars, int idx_ref, const mloam_point_t *h_surf, const int *surf_counts,
                                const mloam_point_t *h_corner, const int *corner_counts, const double *pose_pivot7, double *pose_i7,
@@ -536,114 +682,42 @@ extern "C" int mloam_calib_rig(mloam_ctx_t *h, int n_lidars, int idx_ref, const 
   if (!M[MLOAM_MAP_SURF].built || !M[MLOAM_MAP_CORNER].built) return fail(c, MLOAM_E_STATE, "calib_rig: build the local maps first");
   if (own_cal_maps && !(M[MLOAM_MAP_SCAN_SURF].built && M[MLOAM_MAP_SCAN_CORNER].built))
     return fail(c, MLOAM_E_STATE, "calib_rig: own_cal_maps needs MLOAM_MAP_SCAN_SURF / MLOAM_MAP_SCAN_CORNER built");
+  const mloam_point_t *surf[RIG_L], *corner[RIG_L];
+  long long so = 0, co = 0;
+  for (int n = 0; n < n_lidars; n++) {
+    surf[n] = h_surf ? h_surf + so : nullptr, corner[n] = h_corner ? h_corner + co : nullptr;
+    so += surf_counts[n], co += corner_counts[n];
+  }
+  return calib_rig_solve(c, n_lidars, idx_ref, surf, surf_counts, corner, corner_counts, pose_pivot7, pose_i7, ext7s, has_prior ? prior7s : nullptr,
+                         prior_pos, prior_rot, max_outer, max_inner, huber_a, own_cal_maps, stats, h_rows);
+}
 
-  // blocks: 0 = pose_i (the reference LiDAR's rows), then the calibrated LiDARs in index order
-  int blk_of[RIG_L], lidar_of[RIG_L];
-  for (int n = 0, b = 1; n < n_lidars; n++) {
-    const int bb = n == idx_ref ? 0 : b++;
-    blk_of[n] = bb, lidar_of[bb] = n;
-  }
-  // segments: the reference LiDAR's corner and surf features, then each calibrated LiDAR's (mloam_calib_frame's set order)
-  RigSegs sets;
-  memset(&sets, 0, sizeof(sets));
-  long long soff[RIG_L + 1] = {0}, coff[RIG_L + 1] = {0};
-  for (int n = 0; n < n_lidars; n++) soff[n + 1] = soff[n] + surf_counts[n], coff[n + 1] = coff[n] + corner_counts[n];
-  const int n_total = (int)(n_surf + n_corner);
-  DevBuf &wb = c->rig_work;
-  wb.in_graphs = false;  // no frame graph holds it
-  int nb = 1;
-  {
-    int n_max = 1;
-    for (int n = 0; n < n_lidars; n++) n_max = std::max(n_max, std::max(surf_counts[n], corner_counts[n]));
-    nb = (n_max + RIG_THREADS - 1) / RIG_THREADS;
-    nb = nb < 1 ? 1 : (nb > c->sm_count ? c->sm_count : nb);
-  }
-  float4 *d_pts;
-  RigState *st;
-  double *partials;
-  MLOAM_CUDA_OK(c, carve(wb, [&](Carve &cv) {
-    d_pts = cv.take<float4>((size_t)n_total + 1);
-    sets.pos = cv.take<int>(RIG_KMAX * ((size_t)n_total + 1));
-    sets.valid = cv.take<unsigned char>((size_t)n_total + 1);
-    sets.coeff = cv.take<float>(6 * ((size_t)n_total + 1));
-    st = cv.take<RigState>(1);
-    partials = cv.take<double>((size_t)RIG_N * nb);
-  }));
-  sets.pts = d_pts;
-  int off = 0;
-  for (int b = 0; b < n_lidars; b++) {
-    const int n = lidar_of[b];
-    for (int t = 0; t < 2; t++) {  // 0 corner, 1 surf
-      RigSeg &S = sets.s[sets.n_seg++];
-      S.off = off, S.n = t ? surf_counts[n] : corner_counts[n], S.blk = b, S.plane = t, S.kind = b == 0 ? 1 : 2;
-      S.map = (b == 0 ? 0 : 2) + t;
-      const mloam_point_t *src = t ? h_surf + soff[n] : h_corner + coff[n];
-      if (S.n > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_pts + off, src, sizeof(float4) * (size_t)S.n, cudaMemcpyHostToDevice, c->stream));
-      off += S.n;
-    }
-  }
-  sets.map[0] = M[MLOAM_MAP_CORNER].view(), sets.map[1] = M[MLOAM_MAP_SURF].view();
-  sets.map[2] = M[own_cal_maps ? MLOAM_MAP_SCAN_CORNER : MLOAM_MAP_CORNER].view();
-  sets.map[3] = M[own_cal_maps ? MLOAM_MAP_SCAN_SURF : MLOAM_MAP_SURF].view();
-  sets.n_total = n_total, sets.B = n_lidars, sets.sel_prune = c->knn_all_searches ? 0 : 1;
-  sets.min_match_sq_dis = c->params.min_match_sq_dis, sets.min_plane_dis = c->params.min_plane_dis, sets.huber_a = huber_a;
-
-  // the initial state goes up whole (the scratch and the LM fields are set by the first evaluation)
-  std::vector<RigState> init(1);
-  RigState &s0 = init[0];
-  memset(&s0, 0, sizeof(s0));
-  for (int k = 0; k < 7; k++) {
-    s0.xp[k] = pose_pivot7[k], s0.xr[k] = ext7s[7 * idx_ref + k], s0.x[0][k] = pose_i7[k];
-    for (int b = 1; b < n_lidars; b++) s0.x[b][k] = ext7s[7 * lidar_of[b] + k];
-    if (has_prior) {
-      s0.prior_ref[k] = prior7s[7 * idx_ref + k];
-      for (int b = 1; b < n_lidars; b++) s0.prior[b][k] = prior7s[7 * lidar_of[b] + k];
-    }
-  }
-  s0.prior_pos = prior_pos, s0.prior_rot = prior_rot, s0.has_prior = has_prior ? 1 : 0, s0.B = n_lidars, s0.max_inner = max_inner;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(st, &s0, sizeof(RigState), cudaMemcpyHostToDevice, c->stream));
-  int *h_done = &c->pinned->done;
-  int nbk = (n_total + RIG_WARPS - 1) / RIG_WARPS, nbf = (n_total + 127) / 128;
-  nbk = nbk > 4 * c->sm_count ? 4 * c->sm_count : nbk;
-  nbf = nbf > 4 * c->sm_count ? 4 * c->sm_count : nbf;
-  for (int outer = 0; outer < max_outer; outer++) {
-    k_rig_poses<<<1, 32, 0, c->stream>>>(st);
-    c->launches++;
-    if (n_total > 0) {
-      k_rig_knn<<<nbk, RIG_THREADS, 0, c->stream>>>(sets, st);
-      k_rig_fit<<<nbf, 128, 0, c->stream>>>(sets, st);
-      c->launches += 2;
-    }
-    k_rig_linearize<<<nb, RIG_THREADS, 0, c->stream>>>(sets, st, 0, partials);
-    k_rig_lm<<<1, RIG_THREADS, 0, c->stream>>>(partials, nb, st, 1);
-    c->launches += 2;
-    for (int it = 0; it < max_inner; it++) {
-      k_rig_linearize<<<nb, RIG_THREADS, 0, c->stream>>>(sets, st, 1, partials);
-      k_rig_lm<<<1, RIG_THREADS, 0, c->stream>>>(partials, nb, st, 2);
-      c->launches += 2;
-      if (max_inner > 1) {
-        MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_done, &st->done, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
-        if (*h_done) break;
-      }
-    }
-  }
-  MLOAM_CUDA_OK(c, cudaGetLastError());
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(&s0, st, sizeof(RigState), cudaMemcpyDeviceToHost, c->stream));
-  MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
-  for (int k = 0; k < 7; k++) {
-    pose_i7[k] = s0.x[0][k];
-    for (int b = 1; b < n_lidars; b++) ext7s[7 * lidar_of[b] + k] = s0.x[b][k];
-  }
-  int rows = 0;
-  for (int b = 0; b < n_lidars; b++) rows += s0.rows[b];
-  if (h_rows)
-    for (int n = 0; n < n_lidars; n++) h_rows[n] = s0.rows[blk_of[n]];
-  if (stats) {
-    stats->ran = 1, stats->lm_iterations = s0.total_iterations, stats->termination = s0.termination, stats->final_cost = s0.cost;
-    stats->n_surf = rows;  // feature rows of the last evaluation
-    stats->n_surf_in = (int)n_surf, stats->n_corner_in = (int)n_corner;
-    for (int i = 0; i < 36; i++) stats->H[i] = s0.H[0][i];  // pose_i block
-  }
+// Estimator::optimizeMap with ESTIMATE_EXTRINSIC == 1 for one frame i and one calibrated LiDAR: the rig problem of two LiDARs, the
+// reference first (see include/mloam_b200.h).
+extern "C" int mloam_calib_frame(mloam_ctx_t *h, const mloam_point_t *h_surf_ref, int n_surf_ref, const mloam_point_t *h_corner_ref,
+                                 int n_corner_ref, const mloam_point_t *h_surf_cal, int n_surf_cal, const mloam_point_t *h_corner_cal,
+                                 int n_corner_cal, const double *pose_pivot7, double *pose_i7, const double *ext_ref7, double *ext_cal7,
+                                 int max_outer, int max_inner, double huber_a, int own_cal_maps, mloam_solve_stats_t *stats) {
+  if (!h || !pose_pivot7 || !pose_i7 || !ext_ref7 || !ext_cal7 || n_surf_ref < 0 || n_corner_ref < 0 || n_surf_cal < 0 || n_corner_cal < 0 ||
+      max_outer < 1 || max_inner < 1)
+    return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  cudaSetDevice(c->device);
+  if (stats) memset(stats, 0, sizeof(*stats));
+  const MapStorage *M = c->maps;
+  if (!M[MLOAM_MAP_SURF].built || !M[MLOAM_MAP_CORNER].built) return fail(c, MLOAM_E_STATE, "calib_frame: build the local maps first");
+  if (own_cal_maps && !(M[MLOAM_MAP_SCAN_SURF].built && M[MLOAM_MAP_SCAN_CORNER].built))
+    return fail(c, MLOAM_E_STATE, "calib_frame: own_cal_maps needs MLOAM_MAP_SCAN_SURF / MLOAM_MAP_SCAN_CORNER built");
+  const mloam_point_t *surf[2] = {h_surf_ref, h_surf_cal}, *corner[2] = {h_corner_ref, h_corner_cal};
+  const int surf_counts[2] = {n_surf_ref, n_surf_cal}, corner_counts[2] = {n_corner_ref, n_corner_cal};
+  for (int n = 0; n < 2; n++)
+    if ((surf_counts[n] > 0 && !surf[n]) || (corner_counts[n] > 0 && !corner[n])) return MLOAM_E_INVALID;
+  if ((long long)n_surf_ref + n_corner_ref + n_surf_cal + n_corner_cal > INT_MAX / RIG_KMAX) return MLOAM_E_INVALID;
+  double ext7s[14];
+  for (int k = 0; k < 7; k++) ext7s[k] = ext_ref7[k], ext7s[7 + k] = ext_cal7[k];
+  const int rc = calib_rig_solve(c, 2, 0, surf, surf_counts, corner, corner_counts, pose_pivot7, pose_i7, ext7s, nullptr, 0.0, 0.0, max_outer,
+                                 max_inner, huber_a, own_cal_maps, stats, nullptr);
+  if (rc) return rc;
+  for (int k = 0; k < 7; k++) ext_cal7[k] = ext7s[7 + k];
   return MLOAM_OK;
 }

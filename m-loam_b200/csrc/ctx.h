@@ -274,7 +274,7 @@ struct PinnedBlock {
   GridHdr map_hdr[MLOAM_NUM_MAPS];  // map_build_device: the GridHdr head of each slot's last build (auto cell)
   int done;                         // LM done-flag poll of the solves with max_inner > 1
   double upload_pose[7];            // upload_pose
-  double odom_x[28];                // odometry / calibration / good-feature poses (DevCtl::odom_x)
+  double odom_x[21];                // odometry / good-feature poses: pivot | pose_i | ext (DevCtl::odom_x)
   alignas(16) unsigned char odom[4096];  // OdomState mirror (odom_kernels.cu)
   double normal_eq[30];             // mloam_normal_equations read-back
   double pose_plus[64];             // mloam_pose_plus: x | delta | V in, result at [56]
@@ -306,8 +306,7 @@ struct DevCtl {
   double pose[8];                       // PinnedBlock::pose
   double upload_pose[8];                // PinnedBlock::upload_pose
   double ext[8];                        // PinnedBlock::ext
-  double odom_x[32];                    // PinnedBlock::odom_x: 21 (odometry, good features) or 28 (calibration) doubles
-  double match_pose[2][8];              // calibration: the poses its two feature groups are matched at
+  double odom_x[24];                    // PinnedBlock::odom_x
   double normal_eq[32];                 // mloam_normal_equations
   double pose_plus[64];                 // mloam_pose_plus
   float rig[MLOAM_MAX_LIDARS][12];      // PinnedBlock::rig
@@ -384,22 +383,22 @@ struct Ctx {
   MapStorage maps[MLOAM_NUM_MAPS];
 
   // scan features (device copies when the caller passes host buffers)
-  DevBuf scan_pts[4];             // [0] corner, [1] surf
-  DevBuf feat_valid[4];           // unsigned char per query
-  DevBuf feat_coeff[4];           // float[6] per query
-  DevBuf feat_nn[4];              // int[n_neigh] per query (optional)
-  DevBuf knn_pos[4];              // int[n_neigh] per query: neighbour positions handed from k_match_knn to k_match_fit
-  DevBuf knn_changed[4];          // unsigned char per query: neighbour list differs from the previous iteration's
-  DevBuf knn_anchor[4];           // float4 per query: position of its last real search + tolerated displacement
+  DevBuf scan_pts[2];             // [0] corner, [1] surf
+  DevBuf feat_valid[2];           // unsigned char per query
+  DevBuf feat_coeff[2];           // float[6] per query
+  DevBuf feat_nn[2];              // int[n_neigh] per query (optional)
+  DevBuf knn_pos[2];              // int[n_neigh] per query: neighbour positions handed from k_match_knn to k_match_fit
+  DevBuf knn_changed[2];          // unsigned char per query: neighbour list differs from the previous iteration's
+  DevBuf knn_anchor[2];           // float4 per query: position of its last real search + tolerated displacement
   DevBuf knn_spec;                // SpecState of the speculative scan2map schedule
   DevBuf gf_work[2];              // good-feature selection scratch per set (Jacobian rows, pool tree, mask, ...)
-  DevBuf knn_heavy[4];            // 2 x unsigned char per query: "needed a real search" verdicts of the last two launches
+  DevBuf knn_heavy[2];            // 2 x unsigned char per query: "needed a real search" verdicts of the last two launches
   DevBuf knn_heavy_list;          // 3 rotating counters + 2 lists of feature indices that needed a real search (match_kernels.cu HeavyQ)
   int knn_rot = 0;                // launch ordinal inside the current solve (rotation of the heavy lists / counters)
   int knn_parity = 0;             // which half of knn_heavy the next seeded launch reads
-  int knn_half[4] = {0, 0, 0, 0}; // per set: features per half of knn_pos / knn_anchor in its last launch (0: one half)
+  int knn_half[2] = {0, 0};       // per set: features per half of knn_pos / knn_anchor in its last launch (0: one half)
   int knn_k = 0;                  // neighbours per feature of the last launch
-  MapView knn_map[4] = {};        // per set: the map its last launch searched (mloam_debug_knn_lists)
+  MapView knn_map[2] = {};        // per set: the map its last launch searched (mloam_debug_knn_lists)
   DevBuf partials;                // per-block packed normal equations
   DevBuf lm_state;                // LMState
   void *ticket_zeroed_for = nullptr;  // partials allocation whose last-block ticket has been zeroed
@@ -410,8 +409,8 @@ struct Ctx {
   DevBuf voxel_work;              // voxel filters of the host entry points and of the keyframe submap
   DevBuf voxel_corner, voxel_surf;  // the frame's two scan filters, on two streams at once; the look-ahead branch forks after them
   DevBuf host_work;               // host entry points: work and output staging (good features, kNN, factors, scan2map_ua, ...)
-  DevBuf odom_work;               // OdomState + partials of mloam_odom_solve / mloam_calib_frame
-  DevBuf rig_work;                // mloam_calib_rig: the rig's features, their matches and fits, RigState, partials (calib_rig.cu)
+  DevBuf odom_work;               // OdomState + partials of mloam_odom_solve
+  DevBuf rig_work;                // mloam_calib_rig / mloam_calib_frame: the rig's features, their matches and fits, RigState, partials (calib_rig.cu)
   // association work (uct.h uct_bufs) of the keyframe submap and the host entry points: never inside a frame, so it shares the
   // corner submap upload's allocation
   DevBuf &assoc_work() { return map_in[1]; }
@@ -639,13 +638,12 @@ struct MatchJob {
   int seeded;               // 1: same features against the same map as the previous call with this job index — its neighbour
                             // lists (Ctx::knn_pos) seed the search and unchanged lists keep their fit
 };
-// buf_base: which pair of the context's per-set buffers (knn_pos / knn_anchor / ...) the jobs use: 0 (sets 0, 1) or 2 (sets 2, 3)
 // defer (nullable): skip the fit launch and write the fit into *defer for the caller's next linearize_device(lm_mode 1) (LinOpts::fit);
 // defer->K == 0 when the fit was launched here (a job wants neighbour indices) or nothing was matched.  nullptr: fit now.
 // d_sel (speculative schedule, with defer): double-buffered lists, read half *d_sel and write the other (SpecState::sel)
 // pdl: the kNN launch is a link of scan2map's GN chain (launch_chain)
-int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_pose7, const MatchCfg &cfg, int buf_base = 0,
-                      PendingFit *defer = nullptr, const int *d_sel = nullptr, bool pdl = false);
+int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_pose7, const MatchCfg &cfg, PendingFit *defer = nullptr,
+                      const int *d_sel = nullptr, bool pdl = false);
 // the k_match_knn instance this context launches for K (non-instrumented): resident CTAs per SM by the occupancy calculator, registers
 int knn_residency(const Ctx *c, int K, int *ctas_per_sm, int *regs);
 

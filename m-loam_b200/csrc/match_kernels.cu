@@ -324,10 +324,10 @@ __global__ void __launch_bounds__(128) k_match_fit(FitSet a, FitSet b, const dou
 // ------------------------------------------------------------------------------------------------ launchers
 // Match up to two feature sets (corner against MLOAM_MAP_CORNER-like slot, surf against a surf slot) in one
 // kNN launch + one fit launch.  Sets with n == 0 are skipped.
-int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_pose7, const MatchCfg &cfg, int buf_base, PendingFit *defer,
-                      const int *d_sel, bool pdl) {
+int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_pose7, const MatchCfg &cfg, PendingFit *defer, const int *d_sel,
+                      bool pdl) {
   if (defer) defer->K = 0;
-  if (n_jobs < 1 || n_jobs > 2 || (buf_base != 0 && buf_base != 2)) {
+  if (n_jobs < 1 || n_jobs > 2) {
     c->err = "match: 1 or 2 jobs";
     return MLOAM_E_INVALID;
   }
@@ -355,20 +355,20 @@ int match_pair_device(Ctx *c, const MatchJob *jobs, int n_jobs, const double *d_
       c->err = "match_from_map: type must be 'c' or 's'";
       return MLOAM_E_INVALID;
     }
-    DevBuf &pb = c->knn_pos[buf_base + t];
+    DevBuf &pb = c->knn_pos[t];
     const int halves = d_sel ? 2 : 1;  // double-buffered (speculative schedule): half 1 follows half 0
     MLOAM_CUDA_OK(c, pb.reserve(sizeof(int) * (size_t)K * (size_t)(J.n + 1) * halves));
     k.map = c->maps[J.slot].view();
-    DevBuf &cb = c->knn_changed[buf_base + t];
+    DevBuf &cb = c->knn_changed[t];
     MLOAM_CUDA_OK(c, cb.reserve((size_t)(J.n + 1)));
     k.pts = J.pts, k.n = J.n, k.d_n = J.d_n, k.pos = pb.as<int>();
-    DevBuf &ab = c->knn_anchor[buf_base + t];
+    DevBuf &ab = c->knn_anchor[t];
     MLOAM_CUDA_OK(c, ab.reserve(sizeof(float4) * (size_t)(J.n + 1) * halves));
     k.seeded = J.seeded, k.changed = cb.as<unsigned char>(), k.anchor = ab.as<float4>();
     k.half = d_sel ? J.n + 1 : 0;
-    c->knn_half[buf_base + t] = k.half, c->knn_k = K, c->knn_map[buf_base + t] = k.map;
+    c->knn_half[t] = k.half, c->knn_k = K, c->knn_map[t] = k.map;
     // search verdicts ("had to search") alternate between two halves from launch to launch: read the previous, write the next
-    DevBuf &hb = c->knn_heavy[buf_base + t];
+    DevBuf &hb = c->knn_heavy[t];
     const size_t half = ((size_t)J.n + 256) & ~(size_t)255;
     MLOAM_CUDA_OK(c, hb.reserve(2 * half));
     k.heavy_in = J.seeded ? hb.as<unsigned char>() + half * (size_t)c->knn_parity : nullptr;

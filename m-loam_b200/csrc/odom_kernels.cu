@@ -3,7 +3,7 @@
 // ceres::Solve(DENSE_SCHUR, NUM_ITERATIONS).  Each feature emits one row over the FREE blocks:
 //   1x6  (pose_i free, ext constant: ESTIMATE_EXTRINSIC == 0, estimator.cpp:640,794-848)
 //   1x6  (ext free only)
-//   1x12 [J_pose_i | J_ext]  (both free: the calibration row of BASELINE.json's north star)
+//   1x12 [J_pose_i | J_ext]  (both free)
 // k_odom_linearize<D>: one thread per feature computes (r, row); the D(D+1)/2 + D + 2 packed sums are reduced
 // element by element with warp shuffles into a per-warp shared-memory accumulator (a 1x12 row would need 92 fp64
 // accumulators per thread otherwise), summed across warps in fixed order, one partial per CTA — no atomics.
@@ -24,7 +24,6 @@ struct OdPack {
 };
 
 struct OdomState {
-  double xr[7];                // calibration frame: extrinsic of the reference LiDAR (constant, estimator.cpp:642)
   double xp[7], xi[7], xe[7];  // pivot (constant), pose_i, ext: accepted
   double xic[7], xec[7];       // candidates
   double H[144], g[12], cost;
@@ -34,18 +33,13 @@ struct OdomState {
   int reuse_diagonal, iteration, num_invalid, done, termination, total_iterations, rows, max_inner, pad;
 };
 
-// Row kinds.  0: LidarPureOdom* on (pivot, pose_i, ext) with the free blocks of OdomState::free_mask (mloam_odom_solve).
-// Calibration frame (D = 12, state [pose_i | ext_cal]; Estimator::optimizeMap with ESTIMATE_EXTRINSIC == 1, estimator.cpp:687-787):
-// 1: LidarPureOdom* of the REFERENCE LiDAR on (pivot, pose_i, ext_ref constant) -> columns 0..5;
-// 2: LidarOnlineCalib* of the calibrated LiDAR on ext_cal (lidar_online_calib_factor.hpp:24-227) -> columns 6..11.
-constexpr int OD_SETS = 4;
+// Rows: LidarPureOdom* on (pivot, pose_i, ext) with the free blocks of OdomState::free_mask; set 0 corner, 1 surf.
+constexpr int OD_SETS = 2;
 struct OdomSets {
   const float4 *pts[OD_SETS];
   const float *coeff[OD_SETS];
-  const unsigned char *valid[OD_SETS];  // nullable: all valid
   int n[OD_SETS];
   int is_plane[OD_SETS];
-  int kind[OD_SETS];
   double sqrt_info, huber_a;
 };
 
@@ -58,13 +52,10 @@ __global__ void __launch_bounds__(OD_THREADS) k_odom_linearize(OdomSets a, const
   for (int k = lane; k < N; k += 32) acc[wid][k] = 0.0;
   __syncwarp();
   const Chain ch = make_chain(st->xp, use_candidate ? st->xic : st->xi, use_candidate ? st->xec : st->xe);
-  const Chain ch_ref = make_chain(st->xp, use_candidate ? st->xic : st->xi, st->xr);
-  const PoseR p_cal = make_poser(use_candidate ? st->xec : st->xe);
   const int fm = st->free_mask;
   for (int s = 0; s < OD_SETS; s++) {
     const int n = a.n[s];
     if (n <= 0) continue;
-    const int kind = a.kind[s];
     // all lanes of a warp iterate together (the shuffles below need them); out-of-range lanes contribute zeros
     for (int base = (blockIdx.x * (OD_THREADS / 32) + wid) * 32; base < n; base += gridDim.x * OD_THREADS) {
       const int i = base + lane;
@@ -72,25 +63,14 @@ __global__ void __launch_bounds__(OD_THREADS) k_odom_linearize(OdomSets a, const
 #pragma unroll
       for (int k = 0; k < D; k++) row[k] = 0.0;
       double r = 0.0, rho = 0.0, one = 0.0;
-      if (i < n && (!a.valid[s] || a.valid[s][i])) {
+      if (i < n) {
         const float4 pf = __ldg(a.pts[s] + i);
         const D3 p{(double)pf.x, (double)pf.y, (double)pf.z};
         const float *cf = a.coeff[s] + (size_t)i * 6;
         double Ji[6], Je[6];
         const D3 c0{(double)cf[0], (double)cf[1], (double)cf[2]}, c1{(double)cf[3], (double)cf[4], (double)cf[5]};
-        if (kind == 2) {  // LidarOnlineCalib*: the map factor with T = ext_cal, sqrt_info as given
-#pragma unroll
-          for (int k = 0; k < 6; k++) Ji[k] = 0.0;
-          r = a.is_plane[s] ? plane_factor(p_cal, p, c0, (double)cf[3], a.sqrt_info, Je, true) : edge_factor(p_cal, p, c0, c1, a.sqrt_info, Je, true);
-        } else {
-          const Chain &cc = kind == 1 ? ch_ref : ch;
-          if (a.is_plane[s]) r = odom_plane_factor(cc, p, c0, (double)cf[3], a.sqrt_info, nullptr, Ji, Je);
-          else r = odom_edge_factor(cc, p, c0, c1, a.sqrt_info, nullptr, Ji, Je);
-          if (kind == 1) {
-#pragma unroll
-            for (int k = 0; k < 6; k++) Je[k] = 0.0;  // the reference LiDAR's extrinsic is a constant block
-          }
-        }
+        if (a.is_plane[s]) r = odom_plane_factor(ch, p, c0, (double)cf[3], a.sqrt_info, nullptr, Ji, Je);
+        else r = odom_edge_factor(ch, p, c0, c1, a.sqrt_info, nullptr, Ji, Je);
         double rho1;
         huber(a.huber_a, r * r, &rho, &rho1);
         const double sc = sqrt(rho1);
@@ -333,10 +313,9 @@ __global__ void __launch_bounds__(OD_THREADS) k_odom_lm(const double *__restrict
   od_compute_step<D>(st);
 }
 
-__global__ void k_odom_init(OdomState *st, const double *x21, int free_mask, int max_inner, const double *xr7 = nullptr) {
+__global__ void k_odom_init(OdomState *st, const double *x21, int free_mask, int max_inner) {
   if (threadIdx.x == 0) {
     for (int k = 0; k < 7; k++) st->xp[k] = x21[k], st->xi[k] = st->xic[k] = x21[7 + k], st->xe[k] = st->xec[k] = x21[14 + k];
-    for (int k = 0; k < 7; k++) st->xr[k] = xr7 ? xr7[k] : (k == 6 ? 1.0 : 0.0);
     st->free_mask = free_mask, st->max_inner = max_inner;
     st->done = 0, st->termination = 0, st->total_iterations = 0, st->iteration = 0, st->rows = 0, st->cost = st->initial_cost = 0;
   }
@@ -360,62 +339,14 @@ static int odom_solve_run(Ctx *c, const OdomSets &sets, OdomState *st, int max_i
   return MLOAM_OK;
 }
 
-// ------------------------------------------------------------------------------------------ calibration frame
-// poses the two feature groups are matched at (buildCalibMap, estimator.cpp:1086-1090,1135-1149):
-//   reference LiDAR, frame i:   pose_local = pivot^-1 * pose_i * ext_ref
-//   calibrated LiDAR, pivot:    pose_local = pivot^-1 * pivot * ext_cal = ext_cal
-__global__ void k_calib_poses(const OdomState *st, double *pose_a7, double *pose_b7) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  const PoseD P = pose_from_param(st->xp), I = pose_from_param(st->xi), R = pose_from_param(st->xr);
-  const Q4 qpi = qconj(qnormalized(P.q));
-  // pivot^-1 * (pose_i * ext_ref)
-  const Q4 q_ir = qmul(I.q, R.q);
-  const D3 t_ir = qrot(I.q, R.t) + I.t;
-  const Q4 q = qnormalized(qmul(qpi, q_ir));
-  const D3 t = qrot(qpi, t_ir - P.t);
-  pose_a7[0] = t.x, pose_a7[1] = t.y, pose_a7[2] = t.z, pose_a7[3] = q.x, pose_a7[4] = q.y, pose_a7[5] = q.z, pose_a7[6] = q.w;
-  for (int k = 0; k < 7; k++) pose_b7[k] = st->xe[k];
-}
-
-template <int D>
-__global__ void k_odom_sum_partials(const double *__restrict__ partials, int n_blocks, double *__restrict__ out) {
-  constexpr int N = OdPack<D>::N;
-  for (int k = threadIdx.x; k < N; k += blockDim.x) {
-    double v = 0.0;
-    for (int b = 0; b < n_blocks; b++) v += partials[(size_t)b * N + k];
-    out[k] = v;
-  }
-}
-
-// One evaluation of the 12-dof calibration problem + LM state machine step; with a communicator the packed normal
-// equations (78 + 12 + 2 doubles) are summed over the ranks first — the path's one collective (SURVEY.md 8e).
-static int calib_eval(Ctx *c, const OdomSets &sets, OdomState *st, int nb, double *partials, int use_candidate, int lm_mode) {
-  constexpr int N = OdPack<12>::N;
-  k_odom_linearize<12><<<nb, OD_THREADS, 0, c->stream>>>(sets, st, use_candidate, partials);
-  c->launches++;
-  if (c->nccl_comm) {
-    double *ne = partials + (size_t)N * (nb + 1);
-    k_odom_sum_partials<12><<<1, 128, 0, c->stream>>>(partials, nb, ne);
-    c->launches++;
-    int rc = comm_allreduce_doubles(c, ne, N);
-    if (rc) return rc;
-    k_odom_lm<12><<<1, OD_THREADS, 0, c->stream>>>(ne, 1, st, lm_mode);
-  } else {
-    k_odom_lm<12><<<1, OD_THREADS, 0, c->stream>>>(partials, nb, st, lm_mode);
-  }
-  c->launches++;
-  MLOAM_CUDA_OK(c, cudaGetLastError());
-  return MLOAM_OK;
-}
-
 static_assert(sizeof(OdomState) <= sizeof(PinnedBlock::odom), "OdomState mirror in the pinned block");
 static OdomState *odom_mirror(Ctx *c) { return reinterpret_cast<OdomState *>(c->pinned->odom); }
 
-// Ctx::odom_work: OdomState, then the packed equations of nb blocks and spare rows (calib_eval sums the blocks into one of them)
+// Ctx::odom_work: OdomState, then the packed equations of nb blocks
 static int odom_work(Ctx *c, int nb, OdomState **st, double **partials) {
   MLOAM_CUDA_OK(c, carve(c->odom_work, [&](Carve &cv) {
     *st = cv.take<OdomState>(1);
-    *partials = cv.take<double>(96 * (size_t)(nb + 3));
+    *partials = cv.take<double>(OdPack<12>::N * (size_t)nb);
   }));
   return MLOAM_OK;
 }
@@ -423,98 +354,6 @@ static int odom_work(Ctx *c, int nb, OdomState **st, double **partials) {
 }  // namespace mloam
 
 using namespace mloam;
-
-// Estimator::optimizeMap with ESTIMATE_EXTRINSIC == 1 for one frame i and one calibrated LiDAR (estimator.cpp:687-787), the
-// matching of buildCalibMap (:1135-1149) redone at every outer iteration: see include/mloam_b200.h.
-extern "C" int mloam_calib_frame(mloam_ctx_t *h, const mloam_point_t *h_surf_ref, int n_surf_ref, const mloam_point_t *h_corner_ref,
-                                 int n_corner_ref, const mloam_point_t *h_surf_cal, int n_surf_cal, const mloam_point_t *h_corner_cal,
-                                 int n_corner_cal, const double *pose_pivot7, double *pose_i7, const double *ext_ref7, double *ext_cal7,
-                                 int max_outer, int max_inner, double huber_a, int own_cal_maps, mloam_solve_stats_t *stats) {
-  if (!h || !pose_pivot7 || !pose_i7 || !ext_ref7 || !ext_cal7 || n_surf_ref < 0 || n_corner_ref < 0 || n_surf_cal < 0 || n_corner_cal < 0 ||
-      max_outer < 1 || max_inner < 1)
-    return MLOAM_E_INVALID;
-  Ctx *c = &h->c;
-  cudaSetDevice(c->device);
-  if (stats) memset(stats, 0, sizeof(*stats));
-  const MapStorage *M = c->maps;
-  if (!M[MLOAM_MAP_SURF].built || !M[MLOAM_MAP_CORNER].built) return fail(c, MLOAM_E_STATE, "calib_frame: build the local maps first");
-  if (own_cal_maps && !(M[MLOAM_MAP_SCAN_SURF].built && M[MLOAM_MAP_SCAN_CORNER].built))
-    return fail(c, MLOAM_E_STATE, "calib_frame: own_cal_maps needs MLOAM_MAP_SCAN_SURF / MLOAM_MAP_SCAN_CORNER built");
-  const int cal_surf = own_cal_maps ? MLOAM_MAP_SCAN_SURF : MLOAM_MAP_SURF, cal_corner = own_cal_maps ? MLOAM_MAP_SCAN_CORNER : MLOAM_MAP_CORNER;
-  // sets: 0 corner_ref, 1 surf_ref, 2 corner_cal, 3 surf_cal
-  const mloam_point_t *hp[4] = {h_corner_ref, h_surf_ref, h_corner_cal, h_surf_cal};
-  const int ns[4] = {n_corner_ref, n_surf_ref, n_corner_cal, n_surf_cal};
-  int n_max = 1;
-  for (int t = 0; t < 4; t++) {
-    if (ns[t] > 0 && !hp[t]) return MLOAM_E_INVALID;
-    MLOAM_CUDA_OK(c, c->scan_pts[t].reserve(sizeof(float4) * (size_t)(ns[t] + 1)));
-    int rc = reserve_feat(c, t, ns[t]);
-    if (rc) return rc;
-    if (ns[t] > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->scan_pts[t].p, hp[t], sizeof(float4) * (size_t)ns[t], cudaMemcpyHostToDevice, c->stream));
-    n_max = ns[t] > n_max ? ns[t] : n_max;
-  }
-  int nb = (n_max + OD_THREADS - 1) / OD_THREADS;
-  nb = nb < 1 ? 1 : (nb > c->sm_count ? c->sm_count : nb);
-  OdomState *st;
-  double *partials;
-  int rc = odom_work(c, nb, &st, &partials);
-  if (rc) return rc;
-  double *stage = c->pinned->odom_x;
-  for (int k = 0; k < 7; k++) stage[k] = pose_pivot7[k], stage[7 + k] = pose_i7[k], stage[14 + k] = ext_cal7[k], stage[21 + k] = ext_ref7[k];
-  DevCtl *ctl = c->ctl.as<DevCtl>();
-  double *d_x = ctl->odom_x, *d_pose_a = ctl->match_pose[0], *d_pose_b = ctl->match_pose[1];
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(d_x, stage, 28 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  k_odom_init<<<1, 32, 0, c->stream>>>(st, d_x, 3, max_inner, d_x + 21);
-  c->launches++;
-  OdomSets sets;
-  memset(&sets, 0, sizeof(sets));
-  for (int t = 0; t < 4; t++) {
-    sets.pts[t] = c->scan_pts[t].as<float4>(), sets.coeff[t] = c->feat_coeff[t].as<float>(), sets.valid[t] = c->feat_valid[t].as<unsigned char>();
-    sets.n[t] = ns[t], sets.is_plane[t] = t & 1, sets.kind[t] = t < 2 ? 1 : 2;
-  }
-  sets.sqrt_info = 1.0, sets.huber_a = huber_a;  // factors are built with s = 1.0 (estimator.cpp:696,733); Huber(1.0) (:602)
-  MatchCfg cfg_ref{c->params.min_match_sq_dis, c->params.min_plane_dis, 5, 1};   // n_neigh 5, CHECK_FOV true (estimator.cpp:1135-1142)
-  MatchCfg cfg_cal{c->params.min_match_sq_dis, c->params.min_plane_dis, 10, 1};  // n_neigh 10 for the other LiDARs
-  int *h_done = &c->pinned->done;
-  for (int outer = 0; outer < max_outer && rc == MLOAM_OK; outer++) {
-    k_calib_poses<<<1, 32, 0, c->stream>>>(st, d_pose_a, d_pose_b);
-    c->launches++;
-    if (n_corner_ref + n_surf_ref > 0) {
-      MatchJob jobs[2] = {MatchJob{MLOAM_MAP_CORNER, 'c', sets.pts[0], ns[0], nullptr, c->feat_valid[0].as<unsigned char>(), c->feat_coeff[0].as<float>(), nullptr, 0},
-                          MatchJob{MLOAM_MAP_SURF, 's', sets.pts[1], ns[1], nullptr, c->feat_valid[1].as<unsigned char>(), c->feat_coeff[1].as<float>(), nullptr, 0}};
-      rc = match_pair_device(c, jobs, 2, d_pose_a, cfg_ref, 0);
-      if (rc) break;
-    }
-    if (n_corner_cal + n_surf_cal > 0) {
-      MatchJob jobs[2] = {MatchJob{cal_corner, 'c', sets.pts[2], ns[2], nullptr, c->feat_valid[2].as<unsigned char>(), c->feat_coeff[2].as<float>(), nullptr, 0},
-                          MatchJob{cal_surf, 's', sets.pts[3], ns[3], nullptr, c->feat_valid[3].as<unsigned char>(), c->feat_coeff[3].as<float>(), nullptr, 0}};
-      rc = match_pair_device(c, jobs, 2, d_pose_b, cfg_cal, 2);
-      if (rc) break;
-    }
-    rc = calib_eval(c, sets, st, nb, partials, 0, 1);
-    for (int it = 0; it < max_inner && rc == MLOAM_OK; it++) {
-      rc = calib_eval(c, sets, st, nb, partials, 1, 2);
-      if (rc == MLOAM_OK && max_inner > 1) {
-        MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_done, &st->done, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
-        if (*h_done) break;
-      }
-    }
-  }
-  if (rc) return rc;
-  OdomState *hs = odom_mirror(c);
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(hs, st, sizeof(OdomState), cudaMemcpyDeviceToHost, c->stream));
-  MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
-  for (int k = 0; k < 7; k++) pose_i7[k] = hs->xi[k], ext_cal7[k] = hs->xe[k];
-  if (stats) {
-    stats->ran = 1, stats->lm_iterations = hs->total_iterations, stats->termination = hs->termination, stats->final_cost = hs->cost;
-    stats->n_surf = hs->rows;  // residual rows of the last evaluation, all ranks
-    stats->n_surf_in = n_surf_ref + n_surf_cal, stats->n_corner_in = n_corner_ref + n_corner_cal;
-    for (int i = 0; i < 6; i++)
-      for (int j = 0; j < 6; j++) stats->H[i * 6 + j] = hs->H[i * 12 + j];  // pose block
-  }
-  return MLOAM_OK;
-}
 
 extern "C" int mloam_odom_solve(mloam_ctx_t *h, int n, const unsigned char *h_types, const double *h_points, const double *h_coeffs,
                                 const double *pose_pivot7, double *pose_i7, double *ext7, int free_mask, int max_iterations,

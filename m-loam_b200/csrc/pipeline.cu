@@ -95,7 +95,7 @@ int scan2map_enqueue(Ctx *c, const ScanRef &S, const double *pose_init7, bool wa
                  c->feat_coeff[0].as<float>(), nullptr, seeded},
         MatchJob{MLOAM_MAP_SURF, 's', S.surf, ns_use, S.d_n_surf, c->feat_valid[1].as<unsigned char>(),
                  c->feat_coeff[1].as<float>(), nullptr, seeded}};
-    return match_pair_device(c, jobs, 2, d_pose, cfg, 0, defer_fit ? &pending : nullptr, spec ? &d_spec->sel : nullptr, pdl);
+    return match_pair_device(c, jobs, 2, d_pose, cfg, defer_fit ? &pending : nullptr, spec ? &d_spec->sel : nullptr, pdl);
   };
   for (int outer = 0; outer < P.max_outer; outer++) {
     if (!spec || outer == 0) {  // speculative: the previous iteration enqueued this one's matcher

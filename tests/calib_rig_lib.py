@@ -1,9 +1,10 @@
 """Test infrastructure of the rig calibration (mloam_calib_rig): the binding of the oracle's restatement (oracle/orc_calib_rig.cpp, built by
-oracle/calib_rig.mk), a numpy restatement of PriorFactor (prior_factor.hpp), and the synthetic rig case the tests and
-tools/bench_calib_rig.py solve."""
+oracle/calib_rig.mk), a numpy restatement of PriorFactor (prior_factor.hpp), the synthetic rig case the tests and
+tools/bench_calib_rig.py solve, and the cases of tests/golden/calib_frame_12dof.npz."""
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
 import math
 import os
 import subprocess
@@ -115,3 +116,46 @@ def make_rig_case(scene, n_lidars, n_rings, horizon, map_points, idx_ref=0, seed
     ext_init = np.array([ext[n] if n == idx_ref else perturb_ext(ext[n], n) for n in range(n_lidars)])
     return dict(surf_map=surf_map, corner_map=corner_map, surf=surf, corner=corner, pivot=pivot, pose_i=pose_i, ext=ext,
                 pose_i_init=syn.perturb_pose(pose_i, rng), ext_init=ext_init, idx_ref=idx_ref)
+
+
+# tests/golden/calib_frame_12dof.npz holds mloam_calib_frame's outputs as its 12-DoF solver computed them, on these cases
+# (name: inputs, max_outer, max_inner, feature groups given, the calibrated LiDAR matched against its own maps)
+CALIB_GOLDEN = {"case2_10x1": ("case2", 10, 1, "both", False), "case2_2x4": ("case2", 2, 4, "both", False),
+                "own_cal_maps": ("case2", 10, 1, "both", True), "ref_only": ("case2", 10, 1, "ref", False),
+                "cal_only": ("case2", 10, 1, "cal", False), "c3": ("c3", 10, 1, "both", False)}
+CALIB_GOLDEN_STATS = ("termination", "lm_iterations", "n_surf", "final_cost", "n_surf_in", "n_corner_in")
+_GOLDEN_INPUTS = {}
+
+
+def calib_golden_inputs(kind):
+    """The seeded inputs of a golden case ("case2": 16 x 1024 sweeps and a 100k-point map; "c3": bench.py C3's 64 x 2048 sweeps and a 2M-point
+    map), with the calibration maps of own_cal_maps (leaf 0.2) for case2 and a sha256 over every array."""
+    if kind not in _GOLDEN_INPUTS:
+        rings, horizon, pts = (16, 1024, 100_000) if kind == "case2" else (64, 2048, 2_000_000)
+        cs = syn.make_calib_case(syn.make_scene(), orc.extract_cloud, orc.voxel_grid, rings, horizon, pts)
+        if kind == "case2":
+            cs["surf_map_cal"] = orc.voxel_grid(cs["surf_map"], 0.2, False)[0]
+            cs["corner_map_cal"] = orc.voxel_grid(cs["corner_map"], 0.2, False)[0]
+        h = hashlib.sha256()
+        for k in sorted(cs):
+            a = np.ascontiguousarray(cs[k])
+            h.update(f"{k} {a.dtype} {a.shape}".encode())
+            h.update(a.tobytes())
+        cs["sha256"] = h.hexdigest()
+        _GOLDEN_INPUTS[kind] = cs
+    return _GOLDEN_INPUTS[kind]
+
+
+def calib_golden_maps(ctx, cs, own):
+    ctx.map_build(0, cs["corner_map"], 0.25)
+    ctx.map_build(1, cs["surf_map"], 0.25)
+    if own:
+        ctx.map_build(2, cs["corner_map_cal"], 0.25)
+        ctx.map_build(3, cs["surf_map_cal"], 0.25)
+
+
+def calib_golden_groups(cs, groups):
+    """(surf_ref, corner_ref, surf_cal, corner_cal), None for a group not given."""
+    ref = (cs["surf_ref"], cs["corner_ref"]) if groups != "cal" else (None, None)
+    cal = (cs["surf_cal"], cs["corner_cal"]) if groups != "ref" else (None, None)
+    return ref + cal

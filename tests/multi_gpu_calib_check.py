@@ -2,8 +2,8 @@
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29541 tests/multi_gpu_calib_check.py
 
-Rank 0 holds the reference LiDAR's features (1x6 rows on pose_i), rank 1 the second LiDAR's (1x6 rows on its extrinsic); the
-packed 12x12 normal equations are summed with one ncclAllReduce per LM evaluation inside mloam_calib_frame.  Both ranks must end
+Rank 0 holds the reference LiDAR's features (1x6 rows on pose_i), rank 1 the second LiDAR's (1x6 rows on its extrinsic); both
+blocks' packed normal equations and the cost (57 doubles) are summed with one ncclAllReduce per LM evaluation inside mloam_calib_frame.  Both ranks must end
 with the same [pose_i | ext_cal], equal (<= 1e-4 m / rad) to the oracle's joint solve."""
 import os
 import sys

@@ -1,7 +1,9 @@
-"""GPU tests of mloam_calib_rig, the online-calibration step over the whole rig: bit for bit against mloam_calib_frame on two LiDARs,
-against the oracle's rig restatement (oracle/orc_calib_rig.cpp) on 2, 3, 4 and 16 LiDARs with and without priors, the edges, every error
-path, launches that do not depend on the rig size, and a frame path the call leaves alone."""
+"""GPU tests of mloam_calib_rig, the online-calibration step over the whole rig, and of mloam_calib_frame, its two-LiDAR case: both bit
+for bit against the outputs of the former 12-DoF mloam_calib_frame (tests/golden/calib_frame_12dof.npz), mloam_calib_frame's collective
+branch on a one-rank communicator, the rig against the oracle's rig restatement (oracle/orc_calib_rig.cpp) on 2, 3, 4 and 16 LiDARs with
+and without priors, the edges, every error path, launches that do not depend on the rig size, and a frame path both calls leave alone."""
 import ctypes as C
+import os
 
 import numpy as np
 import pytest
@@ -51,27 +53,40 @@ def _maps(ctx, surf_map, corner_map, own=False):
     return None, None
 
 
-@pytest.mark.parametrize("outer,inner", [(10, 1), (2, 4)])
-def test_two_lidars_equal_calib_frame_bit_for_bit(rctx, case2, outer, inner):
-    cs = case2
-    _maps(rctx, cs["surf_map"], cs["corner_map"])
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "calib_frame_12dof.npz")
+
+
+def _equal_golden(g, name, pi, ec, st):
+    assert np.array_equal(pi, g[f"{name}.pose_i"]) and np.array_equal(ec, g[f"{name}.ext_cal"])
+    for k in crl.CALIB_GOLDEN_STATS:
+        assert st[k] == g[f"{name}.{k}"], (k, st[k], g[f"{name}.{k}"])
+    assert np.array_equal(np.asarray(st["H"]), g[f"{name}.H"])
+
+
+@pytest.mark.parametrize("name", list(crl.CALIB_GOLDEN))
+def test_calib_frame_and_two_lidar_rig_equal_the_12dof_golden(rctx, name):
+    """mloam_calib_frame, and mloam_calib_rig on the same two LiDARs (both idx_ref), give bit for bit what the 12-DoF implementation of
+    mloam_calib_frame gave (tests/golden/make_calib_golden.py), with the same launches."""
+    g = np.load(GOLDEN)
+    kind, outer, inner, groups, own = crl.CALIB_GOLDEN[name]
+    cs = crl.calib_golden_inputs(kind)
+    assert cs["sha256"] == str(g[f"{name}.inputs_sha256"]), "the seeded inputs changed"
+    crl.calib_golden_maps(rctx, cs, own)
+    sr, cr, sc, cc = crl.calib_golden_groups(cs, groups)
     l0 = rctx.launch_count()
-    pi, ec, st = rctx.calib_frame(cs["surf_ref"], cs["corner_ref"], cs["surf_cal"], cs["corner_cal"], cs["pivot"], cs["pose_i_init"], cs["ext_ref"],
-                                  cs["ext_cal_init"], outer, inner)
-    l1 = rctx.launch_count()
+    pi, ec, st = rctx.calib_frame(sr, cr, sc, cc, cs["pivot"], cs["pose_i_init"], cs["ext_ref"], cs["ext_cal_init"], outer, inner, own_cal_maps=own)
+    launches = rctx.launch_count() - l0
+    _equal_golden(g, name, pi, ec, st)
     for idx_ref in (0, 1):
         order = [0, 1] if idx_ref == 0 else [1, 0]
-        s = [[cs["surf_ref"], cs["surf_cal"]][k] for k in order]
-        c = [[cs["corner_ref"], cs["corner_cal"]][k] for k in order]
+        s = [[sr, sc][k] for k in order]
+        c = [[cr, cc][k] for k in order]
         e = [[cs["ext_ref"], cs["ext_cal_init"]][k] for k in order]
-        l2 = rctx.launch_count()
-        rpi, rex, rst, rows = rctx.calib_rig(s, c, cs["pivot"], cs["pose_i_init"], e, idx_ref, max_outer=outer, max_inner=inner)
-        assert np.array_equal(rpi, pi) and np.array_equal(rex[1 - idx_ref], ec) and np.array_equal(rex[idx_ref], cs["ext_ref"])
-        for k in ("termination", "lm_iterations", "n_surf", "final_cost", "n_surf_in", "n_corner_in"):
-            assert rst[k] == st[k], (k, rst[k], st[k])
-        assert np.array_equal(np.asarray(rst["H"]), np.asarray(st["H"])) and rows.sum() == st["n_surf"]
-        # calib_frame launches k_odom_init and two matcher launches per group; the rig call none, and one matcher pass for the rig
-        assert rctx.launch_count() - l2 == (l1 - l0) - 1 - 2 * outer
+        l0 = rctx.launch_count()
+        rpi, rex, rst, rows = rctx.calib_rig(s, c, cs["pivot"], cs["pose_i_init"], e, idx_ref, max_outer=outer, max_inner=inner, own_cal_maps=own)
+        n = rctx.launch_count() - l0
+        _equal_golden(g, name, rpi, rex[1 - idx_ref], rst)
+        assert np.array_equal(rex[idx_ref], cs["ext_ref"]) and rows.sum() == st["n_surf"] and n == launches
 
 
 CASES = [  # L, idx_ref, prior (0 off, 1 at the true extrinsics, 2 with ext_ref's target offset too), own maps, outer, inner
@@ -214,6 +229,36 @@ def test_rig_with_a_communicator_is_refused(mloam, case2):
         c.close()
 
 
+def test_calib_frame_with_a_one_rank_communicator(mloam, case2):
+    """With a communicator attached (one rank), mloam_calib_frame all-reduces each evaluation's sums: the results are those without one, at one
+    more launch per evaluation (2 per outer iteration at max_inner 1)."""
+    import torch  # noqa: F401  (loads the libnccl.so.2 the library resolves)
+    cs = case2
+    out = []
+    for with_comm in (False, True):
+        c = mloam.Context(0)
+        try:
+            if with_comm:
+                lib = mloam.lib()
+                uid = C.create_string_buffer(128)
+                if lib.mloam_comm_unique_id(uid) != 0 or lib.mloam_comm_init(c._h, 1, 0, uid) != 0:
+                    pytest.fail("mloam_comm_init with one rank: " + str(lib.mloam_last_error(c._h)))
+            _maps(c, cs["surf_map"], cs["corner_map"])
+            l0 = c.launch_count()
+            pi, ec, st = c.calib_frame(cs["surf_ref"], cs["corner_ref"], cs["surf_cal"], cs["corner_cal"], cs["pivot"], cs["pose_i_init"],
+                                       cs["ext_ref"], cs["ext_cal_init"], 10, 1)
+            out.append((pi, ec, st, c.launch_count() - l0))
+            if with_comm:
+                lib.mloam_comm_destroy(c._h)
+        finally:
+            c.close()
+    (pi, ec, st, n), (pi1, ec1, st1, n1) = out
+    assert np.array_equal(pi, pi1) and np.array_equal(ec, ec1) and n1 == n + 2 * 10
+    for k in crl.CALIB_GOLDEN_STATS:
+        assert st[k] == st1[k], k
+    assert np.array_equal(np.asarray(st["H"]), np.asarray(st1["H"]))
+
+
 def test_rig_launches_do_not_depend_on_the_rig_size(rctx):
     counts = []
     for L in (2, 4):
@@ -226,6 +271,7 @@ def test_rig_launches_do_not_depend_on_the_rig_size(rctx):
 
 
 def test_rig_call_leaves_the_frame_path_alone(mloam, case2):
+    """A frame after a calibration call (mloam_calib_rig or mloam_calib_frame) computes and launches what it would without one."""
     cs = case2
     scene = syn.make_scene()
     traj = syn.trajectory(3)
@@ -235,20 +281,25 @@ def test_rig_call_leaves_the_frame_path_alone(mloam, case2):
     p = mloam.default_params()
     p.n_scans = 16
     out = []
-    for with_rig in (False, True):
+    for call in (None, "calib_rig", "calib_frame"):
         c = mloam.Context(0, p)
         try:
             _maps(c, cs["surf_map"], cs["corner_map"])
             c.frame(cloud, ss, se, surf_map, corner_map, init)
-            if with_rig:
+            if call:
                 _maps(c, cs["surf_map"], cs["corner_map"])
+            if call == "calib_rig":
                 c.calib_rig([cs["surf_ref"], cs["surf_cal"]], [cs["corner_ref"], cs["corner_cal"]], cs["pivot"], cs["pose_i_init"],
                             [cs["ext_ref"], cs["ext_cal_init"]])
+            elif call == "calib_frame":
+                c.calib_frame(cs["surf_ref"], cs["corner_ref"], cs["surf_cal"], cs["corner_cal"], cs["pivot"], cs["pose_i_init"], cs["ext_ref"],
+                              cs["ext_cal_init"])
             l0 = c.launch_count()
             pose, st = c.frame(cloud, ss, se, surf_map, corner_map, init)
             out.append((pose, st, c.launch_count() - l0))
         finally:
             c.close()
-    assert np.array_equal(out[0][0], out[1][0]) and out[0][2] == out[1][2]
-    for k, v in out[0][1].items():
-        assert np.array_equal(np.asarray(v), np.asarray(out[1][1][k])), k
+    for o in out[1:]:
+        assert np.array_equal(out[0][0], o[0]) and out[0][2] == o[2]
+        for k, v in out[0][1].items():
+            assert np.array_equal(np.asarray(v), np.asarray(o[1][k])), k

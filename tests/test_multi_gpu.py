@@ -94,7 +94,7 @@ def test_two_gpu_frame_parity(exchange):
 
 @pytest.mark.gpu
 def test_two_gpu_calibration_parity():
-    """12-DoF online calibration sharded over two GPUs (one LiDAR each) with the NCCL all-reduce of the 12x12 normal equations."""
+    """12-DoF online calibration sharded over two GPUs (one LiDAR each) with the NCCL all-reduce of both blocks' normal equations."""
     import torch
 
     if torch.cuda.device_count() < 2:
