@@ -67,7 +67,9 @@ typedef struct {
   float surf_leaf;             /* MAP_SURF_RES */
   int gf_method;               /* FLAGS_gf_method in scan2MapOptimization (:474-532): 0 wo_gf, 1 rnd, 2 fps, 3 gd_fix
                                   (gd_float: 3 and mloam_set_gf_float) */
-  float gf_ratio;              /* FLAGS_gf_ratio_ini */
+  float gf_ratio;              /* FLAGS_gf_ratio_ini, in [0, 1]: mloam_set_params refuses a non-finite, negative or larger value
+                                  (MLOAM_E_INVALID, parameters unchanged) instead of restating the reference, whose gd then
+                                  selects every matched feature in random order */
   unsigned gf_seed;            /* selection seed; outer iteration i, set s (0 corner, 1 surf) uses gf_seed + 2 i + s */
   int max_ring_points;         /* upper bound of the points of one ring (0: up to 12288); sizes the in-CTA sort of extractCloud so that
                                   several rings share an SM — set it to the sensor's horizontal resolution */

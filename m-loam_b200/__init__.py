@@ -228,9 +228,14 @@ class Context:
             raise MloamError(f"mloam error {rc}: {lib().mloam_last_error(self._h).decode()}")
 
     def set_params(self, **kw):
+        old = {k: getattr(self.params, k) for k in kw}
         for k, v in kw.items():
             setattr(self.params, k, v)
-        self._ck(lib().mloam_set_params(self._h, C.byref(self.params)))
+        rc = lib().mloam_set_params(self._h, C.byref(self.params))
+        if rc != 0:  # refused: the context keeps its parameters, and so does this copy of them
+            for k, v in old.items():
+                setattr(self.params, k, v)
+        self._ck(rc)
 
     def set_stream(self, cuda_stream_ptr: int):
         self._ck(lib().mloam_set_stream(self._h, C.c_void_p(cuda_stream_ptr)))

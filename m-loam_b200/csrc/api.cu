@@ -167,6 +167,7 @@ void mloam_ctx_destroy(mloam_ctx_t *h) {
 int mloam_set_params(mloam_ctx_t *h, const mloam_params_t *p) {
   if (!h || !p) return MLOAM_E_INVALID;
   if (p->n_neigh != 5 && p->n_neigh != 10) return fail(&h->c, MLOAM_E_INVALID, "n_neigh must be 5 or 10");
+  if (!(p->gf_ratio >= 0.0f) || p->gf_ratio > 1.0f) return fail(&h->c, MLOAM_E_INVALID, "gf_ratio must be a number in [0, 1]");
   h->c.params = *p;
   h->c.prefetched.valid = false;  // look-ahead features were extracted under the previous parameters
   undist_withdraw(&h->c);

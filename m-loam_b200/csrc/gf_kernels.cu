@@ -296,13 +296,14 @@ __global__ void __launch_bounds__(GF_THREADS) k_gf_select(GfArgs a) {
         if (s_num_sel >= num_use || cnt_visited >= n) break;  // uniform: s_num_sel is only written between barriers
         const float4 po = a.pts[old];
         float best_d = -1.0f;
-        int best_j = 0x7fffffff;
+        int best_j = 0x7fffffff;  // none: no d2 > -1 on this thread
         for (int j = tid; j < n; j += GF_THREADS) {
           if (visited[j]) continue;
           const float4 pn = a.pts[j];
           const float dx = po.x - pn.x, dy = po.y - pn.y, dz = po.z - pn.z;
           const float d = sqrtf(dx * dx + dy * dy + dz * dz);
-          const float d2 = fminf(d, a.dist[j]);
+          const float dj = a.dist[j];
+          const float d2 = dj < d ? dj : d;  // std::min(d, dist[j]) (:410): a NaN d stays NaN, so a non-finite point is never the arg-max
           a.dist[j] = d2;
           if (d2 > best_d) best_d = d2, best_j = j;  // ascending j per thread: the first maximum wins, as in the reference
         }
@@ -320,7 +321,8 @@ __global__ void __launch_bounds__(GF_THREADS) k_gf_select(GfArgs a) {
           int bj = red_j[0];
           for (int w = 1; w < GF_THREADS / 32; w++)
             if (red_d[w] > bd || (red_d[w] == bd && red_j[w] < bj)) bd = red_d[w], bj = red_j[w];
-          const int q = bj;
+          // no unvisited point with d2 > -1 (all that remain are non-finite): best_j keeps its initial 1 (:402), visited or not
+          const int q = bj == 0x7fffffff ? 1 : bj;
           visited[q] = 1;
           if (matched[q]) gf_add_outer(H, a.jaco + (size_t)q * 6), a.sel[s_num_sel] = q, s_num_sel = s_num_sel + 1;
           s_pick = q;
@@ -332,7 +334,8 @@ __global__ void __launch_bounds__(GF_THREADS) k_gf_select(GfArgs a) {
     }
   } else if (tid < 32) {  // gd_fix / gd_float (:450-556), warp 0
     int size = n, num_sel = 0, num_rnd_que = 0;
-    const int size_rnd_subset = num_use > 0 ? (int)(1.0 * n / num_use) : 0;
+    // at least 1: the reference's subset of 0 (num_use > n) pops its first candidate at once (heap.size() >= 0), as a subset of 1 does
+    const int size_rnd_subset = num_use > 0 ? max(1, (int)(1.0 * n / num_use)) : 0;
     while (true) {
       if (num_sel >= num_use || size == 0) break;
       int heap_n = 0, best_idx = -1;
@@ -389,9 +392,10 @@ __global__ void __launch_bounds__(GF_THREADS) k_gf_select(GfArgs a) {
         heap_n += n_cand;
         __syncwarp();
         if (heap_n >= size_rnd_subset && heap_n > 0) {  // pop the heap's top: the round's pick
-          {  // sub_mat_H += J^T J: one element per lane (the same single addition per element as the sequential loop)
+          if (lane < 6) {  // sub_mat_H += J^T J: one row per lane (the same single addition per element as the sequential loop)
             const double *jb = a.jaco + (size_t)best_idx * 6;
-            for (int e = lane; e < 36; e += 32) H[e] += jb[e / 6] * jb[e % 6];
+            const double ja = jb[lane];
+            for (int b = 0; b < 6; b++) H[lane * 6 + b] += ja * jb[b];
           }
           if (lane == 0) {
             fen_remove(fen, n, best_idx);
