@@ -218,6 +218,60 @@ int mloam_frame_msg_device(mloam_ctx_t *ctx, const mloam_pc2_msg_t *msgs, const 
 int mloam_frame_set_next_msg(mloam_ctx_t *ctx, const mloam_pc2_msg_t *msgs);
 int mloam_frame_set_next_msg_device(mloam_ctx_t *ctx, const mloam_pc2_msg_t *msgs);
 
+/* ---- the dataset nodes' PCD files: pcl::io::loadPCDFile<pcl::PointXYZ>(cloud_<j>/data/<idx>.pcd) per frame and LiDAR
+ *      (rosNodeRVOxford.cpp:355-370,466, rosNodeRVHercules.cpp:354-368,478), ASCII as pcl::io::savePCDFileASCII writes them
+ *      (test_parse_bag.cpp:47-72), decoded on the device.
+ * mloam_pcd_t: one file's ASCII body: data (host or device bytes, by entry point) = the bytes after the header's DATA line, size bytes,
+ *   points = POINTS, tokens = tokens per line (the header's COUNTs summed), index = the token index of x, y and z in a line.
+ *   host/mloam_io.hpp resolvePCDHeader reads them from the header, pcdBody makes the struct.  DATA binary files need no decode: pcdBinaryMsg
+ *   gives their mloam_pc2_layout_t / mloam_pc2_msg_t for mloam_frame_msg*.
+ * mloam_pcd_decode / mloam_pcd_decode_device: the n files' points (x, y, z, 0) in file order, file after file, into out (sum of points
+ *   float4s; host or device memory, by entry point) — the device counterpart of loadPCDFile<PointXYZ>, before removeNaN: non-finite
+ *   coordinates are passed on.  Two launches decode all n files.  Values are bit-identical to host/mloam_io.hpp decodePCDASCII, which
+ *   restates PCL's reader with std::istringstream and atof as PCL calls them: a token is "nan" (quiet NaN), or the correctly rounded float
+ *   of its decimal (ties to even, subnormals included), +-inf past FLT_MAX's rounding boundary.  Lines end at '\n'; tokens are split on
+ *   runs of space, tab and '\r'; point i is the i-th line that holds a token; lines after POINTS and tokens after `tokens` are ignored.
+ *   Unlike PCL, a line of only spaces, tabs or '\r' is skipped (PCL throws on it), and these bodies are refused where PCL throws or stores
+ *   a prefix parse or atof's reading: a line with fewer than `tokens` tokens, fewer lines than points, an x / y / z token outside
+ *   [+-]?(d+(.d*)?|.d+)([eE][+-]?d+)? | nan | inf | +inf | -inf, or with more than 19 significant digits (digits without leading and
+ *   trailing zeros).  The calls return when the points are written.
+ *   MLOAM_E_INVALID: n outside 1..MLOAM_MAX_LIDARS, a NULL pointer, points < 1, more than 2^30 points in all, index outside
+ *   [0, tokens), and a refused body (mloam_last_error names the reason).
+ * mloam_front_end_pcd: as mloam_front_end_msg, with pcds[l] the ASCII body of LiDAR l (n_lidars of mloam_set_lidars, host bytes): the
+ *   decode, then the raw front end; bit-identical to mloam_front_end on the sweep decodePCDASCII gives.  PointXYZ has no intensity, so
+ *   lane 3 is 0 and time_field 1 (mloam_set_front_end) is refused with MLOAM_E_INVALID.  The dataset branch of rosNodeRVOxford.cpp runs
+ *   no removeNaN; the front end's removeNaN (as rosNodeRVHercules.cpp:367) drops non-finite points, which differs only for files that
+ *   hold them.  Errors as mloam_front_end_msg's and mloam_pcd_decode's.
+ * mloam_frame_pcd / mloam_frame_pcd_device / mloam_frame_set_next_pcd / mloam_frame_set_next_pcd_device: as mloam_frame_msg* with
+ *   pcds[l] the ASCII body of LiDAR l: the decode (two launches for the rig, in the frame or in the look-ahead branch), then the raw front
+ *   end; results are bit-identical to mloam_frame_raw* on the sweep decodePCDASCII gives.  The bodies' byte sizes are staged, not part of
+ *   the frame graph key, so files of other sizes with the same POINTS replay the same graph; the host entry points copy only the body
+ *   bytes, into a staging with room for bodies half as large again (a larger body grows it, which re-captures the graphs once), and the
+ *   caller's host pointer is not part of the key either.  The look-ahead is taken by the next mloam_frame_pcd* call with the same bodies
+ *   (pointers, sizes, counts).  A refused body — found on the device, in the frame or in the look-ahead that decoded it — makes the call
+ *   that takes the sweep return MLOAM_E_INVALID with the initial pose and commit nothing (the announced sweep's features are dropped; the
+ *   next frame extracts its sweep again), as a failed exchange returns MLOAM_E_NCCL; the refusal bits land with the frame's results.
+ *   MLOAM_E_INVALID also for the checks of mloam_pcd_decode and for time_field 1; MLOAM_E_STATE without mloam_set_front_end and on a
+ *   context with a communicator. */
+typedef struct {
+  const void *data;
+  size_t size;
+  int points, tokens;
+  int index[3];
+  int reserved;
+} mloam_pcd_t;
+int mloam_pcd_decode(mloam_ctx_t *ctx, int n, const mloam_pcd_t *pcds, mloam_point_t *h_out);
+int mloam_pcd_decode_device(mloam_ctx_t *ctx, int n, const mloam_pcd_t *pcds, mloam_point_t *d_out);
+int mloam_front_end_pcd(mloam_ctx_t *ctx, const mloam_pcd_t *pcds, mloam_point_t *h_out, int *n_out, int *h_scan_start, int *h_scan_end);
+int mloam_frame_pcd(mloam_ctx_t *ctx, const mloam_pcd_t *pcds, const mloam_point_t *h_surf_map, int n_surf_map,
+                    const mloam_point_t *h_corner_map, int n_corner_map, int rebuild_maps, const double *pose_init7, double *pose_out7,
+                    mloam_solve_stats_t *stats);
+int mloam_frame_pcd_device(mloam_ctx_t *ctx, const mloam_pcd_t *pcds, const mloam_point_t *d_surf_map, int n_surf_map,
+                           const mloam_point_t *d_corner_map, int n_corner_map, int rebuild_maps, const double *pose_init7,
+                           double *pose_out7, mloam_solve_stats_t *stats);
+int mloam_frame_set_next_pcd(mloam_ctx_t *ctx, const mloam_pcd_t *pcds);
+int mloam_frame_set_next_pcd_device(mloam_ctx_t *ctx, const mloam_pcd_t *pcds);
+
 /* ---- FeatureExtract::extractCloud (feature_extract.cpp:118-297) -------------------------------- */
 int mloam_extract_features(mloam_ctx_t *ctx, const mloam_point_t *h_cloud, int n, const int *h_scan_start,
                            const int *h_scan_end, int n_scans, mloam_features_t *out);

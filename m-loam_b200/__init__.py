@@ -44,6 +44,8 @@ ABI_SYMBOLS = [
     "mloam_set_registered", "mloam_frame_registered", "mloam_frame_registered_device",
     "mloam_set_front_end_layout", "mloam_front_end_msg", "mloam_frame_msg", "mloam_frame_msg_device", "mloam_frame_set_next_msg",
     "mloam_frame_set_next_msg_device", "mloam_cloud_msgs", "mloam_cloud_msgs_device",
+    "mloam_pcd_decode", "mloam_pcd_decode_device", "mloam_front_end_pcd", "mloam_frame_pcd", "mloam_frame_pcd_device",
+    "mloam_frame_set_next_pcd", "mloam_frame_set_next_pcd_device",
 ]
 
 
@@ -131,6 +133,31 @@ def _msgs(msgs):
             ptr, size, width, height, row_step = m
             arr[l].data, arr[l].size = ptr, size
         arr[l].width, arr[l].height, arr[l].row_step = int(width), int(height), int(row_step)
+    return arr
+
+
+class PcdBody(C.Structure):
+    """mloam_pcd_t: one PCD file's ASCII body (data: host or device bytes after the DATA line), POINTS, tokens per line, x / y / z token index."""
+    _fields_ = [("data", C.c_void_p), ("size", C.c_size_t), ("points", C.c_int), ("tokens", C.c_int), ("index", C.c_int * 3),
+                ("reserved", C.c_int)]
+
+
+def _pcds(bodies):
+    """bodies: per file (data, points, tokens, (ix, iy, iz)) with data a host uint8 array or bytes, or (ptr, size, points, tokens, index)
+    with a device pointer -> a PcdBody array (host data must outlive the call)."""
+    arr = (PcdBody * len(bodies))()
+    for f, b in enumerate(bodies):
+        if len(b) == 4:
+            data, points, tokens, index = b
+            if isinstance(data, (bytes, bytearray)):
+                data = np.frombuffer(data, np.uint8)
+            arr[f].data, arr[f].size = (data.__array_interface__["data"][0] if data.nbytes else None), data.nbytes
+        else:
+            ptr, size, points, tokens, index = b
+            arr[f].data, arr[f].size = ptr, size
+        arr[f].points, arr[f].tokens = int(points), int(tokens)
+        for k in range(3):
+            arr[f].index[k] = int(index[k])
     return arr
 
 
@@ -448,6 +475,55 @@ class Context:
         n = C.c_int(0)
         self._ck(lib().mloam_front_end_msg(self._h, arr, _p(out), C.byref(n), _p(ss), _p(se)))
         return out[: n.value].copy(), ss, se
+
+    # ---- PCD files (ASCII bodies decoded on the device)
+    def pcd_decode(self, bodies) -> np.ndarray:
+        """mloam_pcd_decode: the files' points (x, y, z, 0) in file order, file after file (bodies: host bytes, see _pcds)."""
+        arr = _pcds(bodies)
+        out = np.empty((max(sum(max(0, b.points) for b in arr), 1), 4), np.float32)
+        self._ck(lib().mloam_pcd_decode(self._h, len(arr), arr, _p(out)))
+        return out[: sum(b.points for b in arr)]
+
+    def pcd_decode_device(self, bodies, d_out: int):
+        """mloam_pcd_decode_device: bodies in device memory (ptr, size, points, tokens, index) -> d_out (device float4s)."""
+        arr = _pcds(bodies)
+        self._ck(lib().mloam_pcd_decode_device(self._h, len(arr), arr, C.c_void_p(d_out)))
+
+    def front_end_pcd(self, bodies):
+        """front_end() on the rig's ASCII PCD bodies (host bytes, see _pcds) -> (ring-ordered sweep, scan_start, scan_end)."""
+        arr = _pcds(bodies)
+        out = np.empty((max(sum(max(0, b.points) for b in arr), 1), 4), np.float32)
+        ss, se = np.zeros(1024, np.int32), np.zeros(1024, np.int32)
+        n = C.c_int(0)
+        self._ck(lib().mloam_front_end_pcd(self._h, arr, _p(out), C.byref(n), _p(ss), _p(se)))
+        return out[: n.value].copy(), ss, se
+
+    def frame_pcd(self, bodies, surf_map, corner_map, pose_init7, rebuild_maps: bool = True):
+        """frame_raw() on the rig's ASCII PCD bodies in host memory (see _pcds)."""
+        sm = None if surf_map is None else _cloud(surf_map)
+        cm = None if corner_map is None else _cloud(corner_map)
+        pi = np.ascontiguousarray(pose_init7, np.float64)
+        out = np.zeros(7)
+        st = SolveStats()
+        self._ck(lib().mloam_frame_pcd(self._h, _pcds(bodies), _p(sm), 0 if sm is None else sm.shape[0], _p(cm), 0 if cm is None else cm.shape[0],
+                                       int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
+        return out, st.as_dict()
+
+    def frame_pcd_device(self, bodies, d_surf_map: int, n_surf_map: int, d_corner_map: int, n_corner_map: int, pose_init7, rebuild_maps: bool = True):
+        """frame_raw_device() on the rig's bodies in device memory: per LiDAR (ptr, size, points, tokens, index)."""
+        pi = np.ascontiguousarray(pose_init7, np.float64)
+        out = np.zeros(7)
+        st = SolveStats()
+        self._ck(lib().mloam_frame_pcd_device(self._h, _pcds(bodies), C.c_void_p(d_surf_map), n_surf_map, C.c_void_p(d_corner_map), n_corner_map,
+                                              int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
+        return out, st.as_dict()
+
+    def frame_set_next_pcd(self, bodies):
+        """Announce the bodies of the next frame_pcd() call (pass the SAME arrays to it).  None withdraws."""
+        self._ck(lib().mloam_frame_set_next_pcd(self._h, None if bodies is None else _pcds(bodies)))
+
+    def frame_set_next_pcd_device(self, bodies):
+        self._ck(lib().mloam_frame_set_next_pcd_device(self._h, None if bodies is None else _pcds(bodies)))
 
     def frame_msg(self, msgs, surf_map, corner_map, pose_init7, rebuild_maps: bool = True):
         """frame_raw() on the rig's messages in host memory (see _msgs)."""

@@ -143,6 +143,11 @@ struct WireMsgs {
   mloam_pc2_msg_t msg[MLOAM_MAX_LIDARS];
   mloam_pc2_layout_t layout[MLOAM_MAX_LIDARS];
 };
+// The rig's ASCII PCD bodies of a PCD sweep (mloam_frame_pcd*), one per LiDAR
+struct PcdFiles {
+  mloam_pcd_t body[MLOAM_MAX_LIDARS];
+};
+static_assert(sizeof(mloam_pcd_t) == 40 && sizeof(PcdFiles) % 8 == 0, "compared whole: no padding");
 static_assert(sizeof(mloam_pc2_msg_t) == 32 && sizeof(mloam_pc2_layout_t) == 40 && sizeof(WireMsgs) % 8 == 0, "hashed whole: no padding");
 
 // The frame path's configuration as the mloam_set_* calls leave it.  The frame graph key (pipeline.cu frame_key) and the staged inputs
@@ -189,7 +194,9 @@ struct Sweep {
   RigLayout L{};
   bool msg = false;                      // raw sweeps as PointCloud2 messages (wire): unpacked on the device before the front end
   WireMsgs wire{};
-  const unsigned char *bytes = nullptr;  // a host message sweep: where its bytes are copied (wire_stage_offset per LiDAR)
+  const unsigned char *bytes = nullptr;  // a host message or PCD sweep: where its bytes are copied (wire_stage_offset / pcd_stage per LiDAR)
+  bool pcd = false;                      // raw sweeps as ASCII PCD bodies: decoded on the device before the front end
+  PcdFiles pcdf{};
 };
 
 // the per-point association with uncertainty (uct.h): per LiDAR of the rig, and per run
@@ -256,6 +263,13 @@ struct GfFloatDev {
   double cfg[2];
 };
 
+// The byte sizes of the ASCII PCD bodies a decode reads (pcd.cu), and where a host body lies in the staging: read on the device, so that
+// the launches depend on the bodies' point counts only
+struct PcdStage {
+  long long size[MLOAM_MAX_LIDARS];
+  long long off[MLOAM_MAX_LIDARS];
+};
+
 // The context's pinned host block (Ctx::pinned): staging of small host-to-device copies and landing of small read-backs, so that
 // they are truly asynchronous.
 struct PinnedBlock {
@@ -282,6 +296,10 @@ struct PinnedBlock {
   GfFloatState gf_float;            // GfFloatState mirror, landed with LMState
   int scan_info[2][MLOAM_MAX_RINGS];       // mloam_frame: ScanInfo of the sweep (start | end)
   int scan_info_next[2][MLOAM_MAX_RINGS];  // ... and of the announced next sweep, copied on Ctx::br_ahead
+  PcdStage pcd;                            // pcd.cu: the ASCII bodies' sizes and staging offsets, copied to the device by the decode
+  unsigned pcd_status;                     // ... and the PCD_E_* bits of the bodies it refused
+  PcdStage pcd_half[2];                    // PCD frames: per half of the feature double buffer, the staged bodies of the sweep decoded into it
+  unsigned pcd_half_status[2];             // ... and their refusal bits, landed with the frame's results
 };
 
 // Matcher counters of k_match_knn with stage profiling on (mloam_profile_get "knn_*"); zeroed at creation and by mloam_profile_reset
@@ -493,6 +511,10 @@ struct Ctx {
   // mloam_cloud_msgs* (wire.cu): the packed PointCloud2 bytes of the last call, each message 256-byte aligned, then the widths.  No frame
   // graph references it, so its growth re-captures nothing.
   DevBuf cloud_msgs{nullptr, 0, false};
+  // mloam_pcd_decode* / mloam_front_end_pcd (pcd.cu): the host bodies' staging, and the PcdStage, per-CTA line counts and status word
+  DevBuf pcd_in{nullptr, 0, false}, pcd_work{nullptr, 0, false};
+  // PCD frames (pcd.cu pcd_decode_half): per half of the feature double buffer, the PcdStage, status word and per-CTA line counts
+  DevBuf pcd_frame;
   Features prefetched;             // features of the sweep announced with the previous frame, ready when that frame returned
   NextSweep next;                  // announced for the frame being enqueued (consumed by it)
   bool next_pending = false;       // its H2D copy was enqueued on br_ahead outside of any capture (ev_next)
@@ -804,6 +826,20 @@ int front_times_device(Ctx *c, const float4 *d_in, const RigLayout &L, int time_
 int wire_unpack_device(Ctx *c, const Sweep &sw, float4 *out);
 // where LiDAR l's bytes lie in a host message sweep's device staging (256-byte aligned), and l = n_lidars: the staging's size
 size_t wire_stage_offset(const WireMsgs &w, int l);
+// The n ASCII PCD bodies (host bytes: staged through Ctx::pcd_in) -> their points, file after file, at out on c->stream; waits for the
+// stream and returns MLOAM_E_INVALID for a refused body
+int pcd_decode_device(Ctx *c, int n, const mloam_pcd_t *pcds, bool host, float4 *out);
+// The checks of n ASCII PCD bodies every PCD entry point makes (MLOAM_E_INVALID), and the message of refusal bits (MLOAM_OK for none)
+int pcd_check(Ctx *c, int n, const mloam_pcd_t *pcds);
+int pcd_refusal(Ctx *c, unsigned bits);
+// The PcdStage of a PCD sweep: each body's size and, for host bytes, its offset in the device staging (256-byte aligned) — staged per
+// frame, never part of a graph key
+void pcd_stage(const Sweep &sw, PcdStage *st);
+// The decode of PCD sweep sw in a frame, on c->stream (also while capturing): its PcdStage copied from PinnedBlock::pcd_half[half]
+// (staged by the frame), the refusal bits into the half's status word, the points to out
+int pcd_decode_half(Ctx *c, const Sweep &sw, int half, float4 *out);
+// The half's device status word (the frame lands it in PinnedBlock::pcd_half_status)
+unsigned *pcd_half_status(Ctx *c);
 int transform_segments_device(Ctx *c, float4 *d_pts, int n, const int *d_off, int n_seg, const float *d_mat12);
 // VoxelGridCovarianceMLOAM<PointIWithCov>::filter: covariance-weighted merge per voxel (cov6 + trace per point in and out)
 int voxel_downsample_cov_device(Ctx *c, const float4 *d_in, const float *d_cov6, const float *d_trace, int n, const int *d_n_in, float leaf,

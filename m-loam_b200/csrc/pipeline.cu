@@ -349,6 +349,9 @@ void stage_frame_inputs(Ctx *c, const FrameCall &fc) {
   if (f.outlier_on) stage_outlier(c);
   if (f.undist_on) stage_undistort(c, fc.parity, undist_ahead(c));
   if (f.gf_float_on) stage_gf_float(c);
+  // PCD sweeps: the bodies' byte sizes (and staging offsets) change from file to file; the captured decode reads them at execution time
+  if (fc.sw.pcd && !fc.have) pcd_stage(fc.sw, &c->pinned->pcd_half[fc.parity]);
+  if (c->next.set && c->use_lookahead && !c->prof_on && c->next.sw.pcd) pcd_stage(c->next.sw, &c->pinned->pcd_half[fc.parity ^ 1]);
 }
 
 // Whether sweep sw is the announced sweep a: same caller pointer and sizes; a raw sweep is taken by a raw frame with the same per-LiDAR
@@ -356,7 +359,8 @@ void stage_frame_inputs(Ctx *c, const FrameCall &fc) {
 // (pointers and shapes) with the same layouts.
 bool same_sweep(const Sweep &a, const Sweep &sw) {
   const bool same_kind = (sw.raw ? (a.raw && std::memcmp(&a.L, &sw.L, sizeof(RigLayout)) == 0) : !a.raw) && a.msg == sw.msg &&
-                         (!sw.msg || std::memcmp(&a.wire, &sw.wire, sizeof(WireMsgs)) == 0);
+                         (!sw.msg || std::memcmp(&a.wire, &sw.wire, sizeof(WireMsgs)) == 0) && a.pcd == sw.pcd &&
+                         (!sw.pcd || std::memcmp(&a.pcdf, &sw.pcdf, sizeof(PcdFiles)) == 0);
   return a.key == sw.key && a.n == sw.n && a.n_scans == sw.n_scans && same_kind && (a.host || !sw.host);
 }
 
@@ -385,6 +389,12 @@ int extract_enqueue(Ctx *c, const Sweep &sw, int parity, FrameBufs *F_out) {
   if (sw.msg) {  // PointCloud2 messages: unpacked into the raw sweep the front end reads
     MLOAM_CUDA_OK(c, c->wire_out.reserve(sizeof(float4) * ((size_t)n + 1)));
     rc = wire_unpack_device(c, sw, c->wire_out.as<float4>());
+    if (rc) return rc;
+    d_cloud = c->wire_out.as<float4>();
+  }
+  if (sw.pcd) {  // ASCII PCD bodies: decoded into the raw sweep the front end reads, their sizes staged for half `parity`
+    MLOAM_CUDA_OK(c, c->wire_out.reserve(sizeof(float4) * ((size_t)n + 1)));
+    rc = pcd_decode_half(c, sw, parity, c->wire_out.as<float4>());
     if (rc) return rc;
     d_cloud = c->wire_out.as<float4>();
   }
@@ -608,6 +618,11 @@ int frame_enqueue(Ctx *c, const FrameCall &f, Ctx::FrameOutcome *o) {
     MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream, c->br_ahead.join, 0));
     stamp(c, "look-ahead join");
   }
+  if (sw.pcd) {  // the refusal bits of both halves land with the frame's results (frame_pcd_status reads this sweep's half)
+    unsigned *d_status = pcd_half_status(c);
+    if (!d_status) return MLOAM_E_CUDA;
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->pinned->pcd_half_status, d_status, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
+  }
   return MLOAM_OK;
 }
 
@@ -632,6 +647,18 @@ int sweep_to_device(Ctx *c, DevBuf &B, Sweep *sw, bool upload, int (*pin)[MLOAM_
     for (int l = 0; upload && l < sw->L.n_lidars; l++)
       MLOAM_CUDA_OK(c, cudaMemcpyAsync(B.as<unsigned char>() + wire_stage_offset(w, l), w.msg[l].data, (size_t)w.msg[l].height * w.msg[l].row_step,
                                        cudaMemcpyHostToDevice, st));
+    return MLOAM_OK;
+  }
+  if (sw->pcd) {  // each LiDAR's body at its pcd_stage offset; room for bodies half as large again, so that a replay of other files
+                  // rarely grows the staging (a growth re-captures the frame graphs)
+    PcdStage ps;
+    pcd_stage(*sw, &ps);
+    const int nl = sw->L.n_lidars;
+    const size_t need = (size_t)(ps.off[nl - 1] + ps.size[nl - 1]) + 16;
+    if (need > B.cap) MLOAM_CUDA_OK(c, B.reserve(need + need / 2));
+    sw->bytes = B.as<unsigned char>();
+    for (int l = 0; upload && l < nl; l++)
+      if (ps.size[l]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(B.as<unsigned char>() + ps.off[l], sw->pcdf.body[l].data, (size_t)ps.size[l], cudaMemcpyHostToDevice, st));
     return MLOAM_OK;
   }
   SweepIn D;
@@ -702,7 +729,9 @@ unsigned long long frame_key(Ctx *c, const FrameCall &f) {
   const Sweep &sw = f.sw, &nx = c->next.sw;
   FrameKey k;
   memset(&k, 0, sizeof(k));
-  k.sweep[0] = sw.cloud, k.sweep[1] = sw.scan_start, k.sweep[2] = sw.scan_end, k.sweep[3] = sw.key;
+  // a host PCD sweep is copied into the staging whatever the caller's buffer: its pointer is no kernel argument (a dataset replay reads
+  // every file into a new place)
+  k.sweep[0] = sw.cloud, k.sweep[1] = sw.scan_start, k.sweep[2] = sw.scan_end, k.sweep[3] = sw.pcd && sw.host ? nullptr : sw.key;
   k.maps[0] = f.surf_map, k.maps[1] = f.corner_map, k.stream = c->stream;
   memcpy(&k.params, &c->params, sizeof(k.params));
   memcpy(k.ext, cfg.ext, sizeof(k.ext));
@@ -722,7 +751,7 @@ unsigned long long frame_key(Ctx *c, const FrameCall &f) {
   k.gf_float_on = cfg.gf_float_on, k.gf_eval = cfg.gf_float_on && c->gf_float_eval;  // an evaluation frame's extra launch
   k.have = f.have, k.parity = f.parity, k.stamp_on = c->stamp_on;
   if (c->next.set && c->use_lookahead) {
-    k.next[0] = nx.key, k.next[1] = nx.cloud, k.next[2] = nx.scan_start, k.next[3] = nx.scan_end;
+    k.next[0] = nx.pcd && nx.host ? nullptr : nx.key, k.next[1] = nx.cloud, k.next[2] = nx.scan_start, k.next[3] = nx.scan_end;
     k.ahead = 1, k.next_n = nx.n, k.next_n_scans = nx.n_scans, k.next_host = nx.host, k.next_pending = c->next_pending;
     if (nx.raw) k.next_front = cfg.front, k.next_L = nx.L;
   }
@@ -741,6 +770,20 @@ unsigned long long frame_key(Ctx *c, const FrameCall &f) {
   };
   if (sw.msg) hash_wire(sw, 4ull);
   if (c->next.set && c->use_lookahead && nx.msg) hash_wire(nx, 8ull);
+  // PCD sweeps: the decode's kernel arguments — the staging or the device bodies, POINTS, tokens and token indices — but not the byte
+  // sizes, which are staged (stage_frame_inputs), so that files of other sizes replay the same graph
+  auto hash_pcd = [&](const Sweep &x, unsigned long long tag) {
+    h = (h ^ tag) * 1099511628211ull;
+    h = (h ^ (unsigned long long)reinterpret_cast<uintptr_t>(x.host ? x.bytes : nullptr)) * 1099511628211ull;
+    for (int l = 0; l < x.L.n_lidars; l++) {
+      const mloam_pcd_t &p = x.pcdf.body[l];
+      h = (h ^ (unsigned long long)reinterpret_cast<uintptr_t>(x.host ? nullptr : p.data)) * 1099511628211ull;
+      h = (h ^ ((unsigned long long)(unsigned)p.points << 32 | (unsigned)p.tokens)) * 1099511628211ull;
+      h = (h ^ ((unsigned long long)(unsigned)p.index[0] << 40 ^ (unsigned long long)(unsigned)p.index[1] << 20 ^ (unsigned)p.index[2])) * 1099511628211ull;
+    }
+  };
+  if (sw.pcd) hash_pcd(sw, 16ull);
+  if (c->next.set && c->use_lookahead && nx.pcd) hash_pcd(nx, 32ull);
   return h;
 }
 
@@ -763,6 +806,19 @@ int frame_single_gpu(Ctx *c, bool raw) {
 // inputs — it is captured once per frame_key into a CUDA graph and replayed: the first call with a new key runs on the stream (and
 // performs every allocation), the second captures + instantiates, later ones replay.  Profiling, multi-GPU (NCCL on the stream) and
 // max_inner > 1 (the host polls the LM done flag) use the plain stream path.
+// A PCD sweep's refusal bits, landed by the frame: the call returns MLOAM_E_INVALID and commits nothing (the look-ahead's features are
+// dropped; the next frame extracts its sweep again).  Waits for the stream, which the frame's read-back does anyway.
+int frame_pcd_status(Ctx *c, const FrameCall &f, double *pose_out7, mloam_solve_stats_t *stats) {
+  if (!f.sw.pcd) return MLOAM_OK;
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
+  const unsigned bits = c->pinned->pcd_half_status[f.parity];
+  if (!bits) return MLOAM_OK;
+  c->prefetched.valid = false;
+  for (int k = 0; k < 7; k++) pose_out7[k] = f.pose_init7[k];
+  if (stats) memset(stats, 0, sizeof(*stats));
+  return pcd_refusal(c, bits);
+}
+
 int frame_run(Ctx *c, const FrameCall &f, double *pose_out7, mloam_solve_stats_t *stats) {
   int rc = frame_single_gpu(c, false);
   if (rc) return rc;
@@ -811,6 +867,8 @@ int frame_run(Ctx *c, const FrameCall &f, double *pose_out7, mloam_solve_stats_t
       MLOAM_CUDA_OK(c, cudaGraphLaunch(e->exec, c->stream));
       c->frame_from_graph = true;
       c->launches += e->launches;
+      rc = frame_pcd_status(c, f, pose_out7, stats);
+      if (rc) return rc;
       frame_commit(c, f.parity, e->out);
       return scan2map_finish(c, e->out.S, f.pose_init7, want_cov, e->out.ran, pose_out7, stats);
     }
@@ -820,6 +878,8 @@ int frame_run(Ctx *c, const FrameCall &f, double *pose_out7, mloam_solve_stats_t
     c->prefetched.valid = false;  // half f.parity may be partly overwritten
     return rc;
   }
+  rc = frame_pcd_status(c, f, pose_out7, stats);
+  if (rc) return rc;
   frame_commit(c, f.parity, o);
   return scan2map_finish(c, o.S, f.pose_init7, want_cov, o.ran, pose_out7, stats);
 }
@@ -891,6 +951,26 @@ int msg_sweep(Ctx *c, const mloam_pc2_msg_t *msgs, bool host, Sweep *sw) {
   if (rc) return rc;
   sw->key = msgs[0].data, sw->cloud = nullptr, sw->msg = true;
   for (int l = 0; l < cfg.n_lidars; l++) sw->wire.msg[l] = msgs[l], sw->wire.layout[l] = cfg.layouts[l];
+  return MLOAM_OK;
+}
+
+// The rig's ASCII PCD bodies pcds (n_lidars of mloam_set_lidars; data in host or device memory) after the checks every PCD entry point
+// makes: a raw sweep of POINTS points per LiDAR, which the decode writes
+int pcd_sweep(Ctx *c, const mloam_pcd_t *pcds, bool host, Sweep *sw) {
+  const FrameCfg &cfg = c->cfg;
+  if (!cfg.front_set) return fail(c, MLOAM_E_STATE, "frame_pcd: call mloam_set_front_end first");
+  int rc = frame_single_gpu(c, true);
+  if (rc) return rc;
+  if (!pcds) return MLOAM_E_INVALID;
+  if (cfg.front.time_field) return fail(c, MLOAM_E_INVALID, "frame_pcd: a PointXYZ cloud has no timestamp field (time_field 1)");
+  rc = pcd_check(c, cfg.n_lidars, pcds);
+  if (rc) return rc;
+  std::vector<int> counts(cfg.n_lidars);
+  for (int l = 0; l < cfg.n_lidars; l++) counts[l] = pcds[l].points;
+  rc = raw_sweep(c, nullptr, host, counts.data(), sw);
+  if (rc) return rc;
+  sw->key = pcds[0].data, sw->cloud = nullptr, sw->pcd = true;
+  for (int l = 0; l < cfg.n_lidars; l++) sw->pcdf.body[l] = pcds[l];
   return MLOAM_OK;
 }
 
@@ -1340,6 +1420,39 @@ int mloam_front_end_msg(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs, mloam_point
   return MLOAM_OK;
 }
 
+// The decode of the rig's ASCII PCD bodies (pcd.cu), then the raw front end, as mloam_front_end_msg
+int mloam_front_end_pcd(mloam_ctx_t *h, const mloam_pcd_t *pcds, mloam_point_t *h_out, int *n_out, int *h_scan_start, int *h_scan_end) {
+  if (!h || !h_out || !n_out || !h_scan_start || !h_scan_end) return MLOAM_E_INVALID;
+  Ctx *c = &h->c;
+  *n_out = 0;
+  Sweep sw;
+  int rc = pcd_sweep(c, pcds, true, &sw);
+  if (rc) return rc;
+  cudaSetDevice(c->device);
+  const int n = sw.n, n_scans = sw.n_scans;
+  c->prefetched.valid = false;  // the front end's output buffer is the frame's
+  MLOAM_CUDA_OK(c, c->wire_out.reserve(sizeof(float4) * ((size_t)n + 1)));
+  rc = pcd_decode_device(c, sw.L.n_lidars, pcds, true, c->wire_out.as<float4>());
+  if (rc) return rc;
+  float4 *d_out;
+  int *d_meta;  // [0] count, then scan starts, scan ends
+  MLOAM_CUDA_OK(c, carve(c->front_out, [&](Carve &cv) { d_out = cv.take<float4>((size_t)n + 1), d_meta = cv.take<int>(4 + 2 * (size_t)n_scans); }));
+  cudaStream_t st = c->stream;
+  const FrontEnd &fe = c->cfg.front;
+  rc = project_cloud_device(c, c->wire_out.as<float4>(), sw.L, fe.vertical_scans, fe.horizon_scans, fe.roi_range, &fe, d_out, d_meta + 4,
+                            d_meta + 4 + n_scans, d_meta, c->front_work);
+  if (rc) return rc;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_start, d_meta + 4, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_end, d_meta + 4 + n_scans, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
+  int *hc = c->pinned->counts;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_meta, sizeof(int), cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  *n_out = hc[0];
+  if (hc[0] > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_out, d_out, sizeof(float4) * (size_t)hc[0], cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  return MLOAM_OK;
+}
+
 int mloam_frame_msg(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs, const mloam_point_t *h_surf_map, int n_surf_map,
                     const mloam_point_t *h_corner_map, int n_corner_map, int rebuild_maps, const double *pose_init7, double *pose_out7,
                     mloam_solve_stats_t *stats) {
@@ -1371,6 +1484,40 @@ int mloam_frame_set_next_msg_device(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs)
   if (!h) return MLOAM_E_INVALID;
   Sweep sw;
   const int rc = msgs ? msg_sweep(&h->c, msgs, false, &sw) : MLOAM_OK;  // nullptr: withdraw
+  return announce(&h->c, sw, rc);
+}
+
+// PCD frames: as mloam_frame_raw* on the sweep the decode of the rig's bodies gives
+int mloam_frame_pcd(mloam_ctx_t *h, const mloam_pcd_t *pcds, const mloam_point_t *h_surf_map, int n_surf_map, const mloam_point_t *h_corner_map,
+                    int n_corner_map, int rebuild_maps, const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
+  if (!h || !pose_init7 || !pose_out7) return MLOAM_E_INVALID;
+  Sweep sw;
+  const int rc = pcd_sweep(&h->c, pcds, true, &sw);
+  if (rc) return rc;
+  return frame_call(&h->c, sw, h_surf_map, n_surf_map, h_corner_map, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+}
+
+int mloam_frame_pcd_device(mloam_ctx_t *h, const mloam_pcd_t *pcds, const mloam_point_t *d_surf_map, int n_surf_map,
+                           const mloam_point_t *d_corner_map, int n_corner_map, int rebuild_maps, const double *pose_init7,
+                           double *pose_out7, mloam_solve_stats_t *stats) {
+  if (!h || !pose_init7 || !pose_out7) return MLOAM_E_INVALID;
+  Sweep sw;
+  const int rc = pcd_sweep(&h->c, pcds, false, &sw);
+  if (rc) return rc;
+  return frame_call(&h->c, sw, d_surf_map, n_surf_map, d_corner_map, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+}
+
+// Look-ahead for PCD frames: as mloam_frame_set_next_msg*, picked up by the next mloam_frame_pcd* call with the same bodies
+int mloam_frame_set_next_pcd(mloam_ctx_t *h, const mloam_pcd_t *pcds) {
+  if (!h) return MLOAM_E_INVALID;
+  Sweep sw;
+  const int rc = pcds ? pcd_sweep(&h->c, pcds, true, &sw) : MLOAM_OK;  // nullptr: withdraw
+  return announce(&h->c, sw, rc);
+}
+int mloam_frame_set_next_pcd_device(mloam_ctx_t *h, const mloam_pcd_t *pcds) {
+  if (!h) return MLOAM_E_INVALID;
+  Sweep sw;
+  const int rc = pcds ? pcd_sweep(&h->c, pcds, false, &sw) : MLOAM_OK;  // nullptr: withdraw
   return announce(&h->c, sw, rc);
 }
 

@@ -16,6 +16,7 @@
 // (tests/test_abi_cpu.py::test_adapter_compiles_against_stub_headers); with the real headers nothing here changes.
 #pragma once
 #include <cmath>
+#include <cstdio>
 #include <cstring>
 #include <initializer_list>
 #include <limits>
@@ -631,5 +632,17 @@ inline mloam_solve_stats_t calibRig(mloam_ctx_t *ctx, size_t idx_ref, const std:
   }
   if (rows) *rows = r;
   return st;
+}
+
+// ---- pcl::io::loadPCDFile<PointT> (pcl::PointXYZ) of the dataset nodes (rosNodeRVOxford.cpp:355-370, rosNodeRVHercules.cpp:354-368): the file's
+// header read on the host (io::resolvePCDHeader), an ASCII body decoded on the device (mloam_pcd_decode: PCL's values bit for bit, the
+// bodies PCL would misread refused), a binary one copied.  Returns 0, or -1 when the file cannot be read or is refused, as PCL does.
+template <typename PointT>
+int loadPCDFile(mloam_ctx_t *ctx, const std::string &path, pcl::PointCloud<PointT> &cloud) {
+  std::vector<mloam_point_t> pts;
+  if (!io::loadPCDPoints(ctx, path, pts)) return -1;
+  cloud.resize(pts.size());
+  for (size_t i = 0; i < pts.size(); i++) cloud[i].x = pts[i].x, cloud[i].y = pts[i].y, cloud[i].z = pts[i].z;
+  return 0;
 }
 }  // namespace mloam

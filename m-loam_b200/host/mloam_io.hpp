@@ -12,15 +12,22 @@
 // "intensity" field gives 0 — the reference exits in that case (feature_extract.hpp:138-142), which callers can reproduce by checking
 // PointCloud2View::has_intensity.  The fourth lane may name another field: "timestamp" for calTimestamp's PointITimeCloud overload.
 // The device unpack of mloam_frame_msg* follows the same rules (resolvePointCloud2Layout).
+//
+// PCD files (resolvePCDHeader, decodePCDASCII, pcdBinaryMsg): the header and body rules of pcl::io::loadPCDFile<pcl::PointXYZ>, below.
 #pragma once
 #include <cstdint>
+#include <cstdio>
+#include <cstdlib>
 #include <cstring>
+#include <limits>
+#include <locale>
 #include <ostream>
 #include <sstream>
 #include <string>
 #include <vector>
 
 #include "../../include/mloam_b200.h"
+#include "../csrc/pcd_ascii.cuh"
 
 namespace mloam {
 namespace io {
@@ -213,6 +220,205 @@ inline int cloudMsgs(mloam_ctx_t *ctx, const std::vector<int> &sources, std::vec
   }
   for (size_t k = 0; k < n && rc == MLOAM_OK; k++) data[k]->resize((size_t)width[k] * cloudMsgStep(sources[k]));
   return rc;
+}
+
+// ---- PCD files: what the dataset nodes read per frame and LiDAR with pcl::io::loadPCDFile<pcl::PointXYZ>(cloud_<j>/data/<idx>.pcd)
+// (rosNodeRVOxford.cpp:355-370, rosNodeRVHercules.cpp:354-368), written by pcl::io::savePCDFileASCII (test_parse_bag.cpp:47-72).
+// Header: the v0.7 header PCL writes, `#` comment lines, then VERSION, FIELDS, SIZE, TYPE, COUNT (optional: 1 each), WIDTH, HEIGHT,
+// VIEWPOINT, POINTS (optional: WIDTH x HEIGHT), DATA.  x, y and z must be fields of SIZE 4, TYPE F, COUNT 1 (what loadPCDFile<PointXYZ>
+// maps by name); every other field, `_` padding included, only takes its COUNT tokens (ASCII) or SIZE x COUNT bytes (binary).  DATA ascii
+// and binary are taken; binary_compressed and anything else are refused.
+struct PCDLayout {
+  int points = 0;                  // POINTS
+  size_t body = 0;                 // byte offset of the body: the byte after the DATA line
+  int tokens = 0;                  // ASCII: tokens per line (the fields' COUNTs summed)
+  int index[3] = {0, 0, 0};        // ASCII: token index of x, y, z in a line
+  bool binary = false;             // DATA binary
+  int point_step = 0;              // binary: bytes per point (SIZE x COUNT summed)
+  int offset[3] = {0, 0, 0};       // binary: byte offset of x, y, z in a point
+};
+
+namespace detail {
+inline std::vector<std::string> pcd_split(const std::string &line) {
+  std::vector<std::string> t;
+  std::istringstream is(line);
+  std::string w;
+  while (is >> w) t.push_back(w);
+  return t;
+}
+inline bool pcd_int(const std::string &s, long long &v) {
+  if (s.empty()) return false;
+  char *end = nullptr;
+  v = std::strtoll(s.c_str(), &end, 10);
+  return end && *end == '\0';
+}
+}  // namespace detail
+
+// The header of the PCD file bytes[0, size) -> layout.  Returns false for a header this library does not take (see above), a missing
+// or inconsistent FIELDS / SIZE / TYPE / COUNT, POINTS other than WIDTH x HEIGHT, or no DATA line.
+inline bool resolvePCDHeader(const uint8_t *bytes, size_t size, PCDLayout &layout) {
+  layout = PCDLayout{};
+  std::vector<std::string> fields, sizes, types, counts;
+  long long width = -1, height = -1, points = -1;
+  size_t at = 0;
+  while (at < size) {
+    size_t end = at;
+    while (end < size && bytes[end] != '\n') end++;
+    const std::string line(reinterpret_cast<const char *>(bytes) + at, end - at);
+    at = end < size ? end + 1 : end;
+    const std::vector<std::string> t = detail::pcd_split(line);
+    if (t.empty() || t[0][0] == '#') continue;
+    const std::string &key = t[0];
+    const std::vector<std::string> vals(t.begin() + 1, t.end());
+    if (key == "VERSION" || key == "VIEWPOINT") continue;
+    if (key == "FIELDS" || key == "COLUMNS") fields = vals;
+    else if (key == "SIZE") sizes = vals;
+    else if (key == "TYPE") types = vals;
+    else if (key == "COUNT") counts = vals;
+    else if (key == "WIDTH" || key == "HEIGHT" || key == "POINTS") {
+      long long v;
+      if (vals.size() != 1 || !detail::pcd_int(vals[0], v) || v < 0) return false;
+      (key == "WIDTH" ? width : key == "HEIGHT" ? height : points) = v;
+    } else if (key == "DATA") {
+      if (vals.size() != 1 || (vals[0] != "ascii" && vals[0] != "binary")) return false;  // binary_compressed: refused
+      layout.binary = vals[0] == "binary";
+      layout.body = at;
+      break;
+    } else {
+      return false;
+    }
+  }
+  if (layout.body == 0 || fields.empty() || sizes.size() != fields.size() || types.size() != fields.size()) return false;
+  if (counts.empty()) counts.assign(fields.size(), "1");
+  if (counts.size() != fields.size() || width < 0 || height < 0) return false;
+  if (points < 0) points = width * height;
+  if (points != width * height || points > (1ll << 30)) return false;
+  int found = 0;
+  long long tok = 0, off = 0;
+  for (size_t f = 0; f < fields.size(); f++) {
+    long long sz, cnt;
+    if (!detail::pcd_int(sizes[f], sz) || !detail::pcd_int(counts[f], cnt) || sz <= 0 || cnt <= 0 || types[f].size() != 1) return false;
+    const int k = fields[f] == "x" ? 0 : fields[f] == "y" ? 1 : fields[f] == "z" ? 2 : -1;
+    if (k >= 0) {
+      if (sz != 4 || types[f] != "F" || cnt != 1 || (found & (1 << k))) return false;
+      found |= 1 << k;
+      layout.index[k] = (int)tok, layout.offset[k] = (int)off;
+    }
+    tok += cnt, off += sz * cnt;
+    if (tok > (1 << 20) || off > (1 << 20)) return false;
+  }
+  if (found != 7) return false;
+  layout.points = (int)points, layout.tokens = (int)tok, layout.point_step = (int)off;
+  return true;
+}
+
+// A DATA binary body as the PointCloud2 message mloam_frame_msg* take: one row of POINTS points, point_step bytes each, x / y / z
+// FLOAT32 at their offsets, no lane 3, little endian (PCL writes the host's byte order).  The bytes stay the caller's.  Returns false for
+// an ASCII layout or a body shorter than POINTS x point_step.
+inline bool pcdBinaryMsg(const uint8_t *bytes, size_t size, const PCDLayout &h, mloam_pc2_layout_t &layout, mloam_pc2_msg_t &msg) {
+  std::memset(&layout, 0, sizeof(layout));
+  std::memset(&msg, 0, sizeof(msg));
+  if (!h.binary || h.body > size || (size - h.body) / (size_t)h.point_step < (size_t)h.points || h.point_step > 1024) return false;
+  layout.point_step = h.point_step;
+  for (int k = 0; k < 3; k++) layout.offset[k] = h.offset[k], layout.datatype[k] = FLOAT32;
+  msg.data = bytes + h.body, msg.size = (size_t)h.points * h.point_step, msg.width = h.points, msg.height = 1;
+  msg.row_step = (size_t)h.points * h.point_step;
+  return true;
+}
+
+// One LiDAR's ASCII body for mloam_pcd_decode* / mloam_frame_pcd* (the bytes stay the caller's)
+inline mloam_pcd_t pcdBody(const uint8_t *bytes, size_t size, const PCDLayout &h) {
+  mloam_pcd_t p;
+  std::memset(&p, 0, sizeof(p));
+  p.data = bytes + h.body, p.size = size - h.body, p.points = h.points, p.tokens = h.tokens;
+  for (int k = 0; k < 3; k++) p.index[k] = h.index[k];
+  return p;
+}
+
+namespace detail {
+// The bytes of the file at path, or false
+inline bool read_file(const std::string &path, std::vector<uint8_t> &bytes) {
+  std::FILE *f = std::fopen(path.c_str(), "rb");
+  if (!f) return false;
+  bytes.clear();
+  uint8_t buf[1 << 16];
+  size_t n;
+  while ((n = std::fread(buf, 1, sizeof(buf), f)) > 0) bytes.insert(bytes.end(), buf, buf + n);
+  const bool ok = std::ferror(f) == 0;
+  std::fclose(f);
+  return ok;
+}
+}  // namespace detail
+
+// The ASCII body[0, size) -> POINTS float4 points (x, y, z, 0) in file order, as loadPCDFile<PointXYZ> reads them (PCL 1.8
+// PCDReader::read, copyStringValue<float>), with std::istringstream and atof exactly as PCL calls them.  The rules:
+//  - lines end at '\n'; a line that is empty or holds only spaces, tabs and '\r' is skipped (PCL skips only an empty line and throws on
+//    the others);
+//  - tokens are split on runs of space, tab and '\r', the line trimmed first; point i is the i-th line not skipped; lines after POINTS,
+//    and tokens after the header's count on a line, are ignored;
+//  - a token is "nan" (quiet NaN) or the float istringstream >> f reads, (float)atof(tok) when that read fails.
+// Returns 0, or the PCD_E_* bits (csrc/pcd_ascii.cuh) of why the body is refused: a line with fewer tokens than the header's, fewer lines
+// than POINTS, an x / y / z token outside pcd_ascii.cuh's grammar or with more than 19 significant digits.  The first refusal ends the
+// decode.  Non-finite coordinates are passed on.
+inline int decodePCDASCII(const uint8_t *body, size_t size, int points, int tokens, const int index[3], std::vector<mloam_point_t> &out) {
+  out.assign((size_t)(points > 0 ? points : 0), mloam_point_t{0.f, 0.f, 0.f, 0.f});
+  int idx = 0;
+  size_t at = 0;
+  std::vector<std::string> st;
+  while (at < size && idx < points) {
+    size_t end = at;
+    while (end < size && body[end] != '\n') end++;
+    const size_t a = at;
+    at = end < size ? end + 1 : end;
+    st.clear();
+    for (size_t k = a; k < end;) {
+      while (k < end && pcd::is_sep(body[k])) k++;
+      const size_t t0 = k;
+      while (k < end && !pcd::is_sep(body[k])) k++;
+      if (k > t0) st.emplace_back(reinterpret_cast<const char *>(body) + t0, k - t0);
+    }
+    if (st.empty()) continue;
+    if ((int)st.size() < tokens) return pcd::PCD_E_SHORT_LINE;
+    float v[3];
+    for (int c = 0; c < 3; c++) {
+      const std::string &tok = st[(size_t)index[c]];
+      uint32_t bits;
+      const int ts = pcd::parse_float(reinterpret_cast<const unsigned char *>(tok.data()), (long long)tok.size(), &bits);
+      if (ts != pcd::PCD_OK) return ts << 1;
+      if (tok == "nan") {
+        v[c] = std::numeric_limits<float>::quiet_NaN();
+      } else {
+        std::istringstream is(tok);
+        is.imbue(std::locale::classic());
+        if (!(is >> v[c])) v[c] = static_cast<float>(std::atof(tok.c_str()));
+      }
+    }
+    out[(size_t)idx++] = mloam_point_t{v[0], v[1], v[2], 0.f};
+  }
+  return idx < points ? pcd::PCD_E_FEW_LINES : 0;
+}
+
+// The points of the PCD file at path (x, y, z, 0), for the adapter's and the shim's loadPCDFile: the header read here, an ASCII body
+// decoded on the device by mloam_pcd_decode (the one helper of this header that calls the library), a binary one copied from its
+// PointCloud2 layout.  false: the file cannot be read, or is refused.
+inline bool loadPCDPoints(mloam_ctx_t *ctx, const std::string &path, std::vector<mloam_point_t> &pts) {
+  std::vector<uint8_t> bytes;
+  PCDLayout h;
+  if (!detail::read_file(path, bytes) || !resolvePCDHeader(bytes.data(), bytes.size(), h)) return false;
+  pts.assign((size_t)h.points, mloam_point_t{0.f, 0.f, 0.f, 0.f});
+  if (h.binary) {
+    mloam_pc2_layout_t lay;
+    mloam_pc2_msg_t m;
+    if (!pcdBinaryMsg(bytes.data(), bytes.size(), h, lay, m)) return false;
+    for (size_t i = 0; i < pts.size(); i++) {
+      const uint8_t *p = static_cast<const uint8_t *>(m.data) + i * (size_t)lay.point_step;
+      std::memcpy(&pts[i].x, p + lay.offset[0], 4), std::memcpy(&pts[i].y, p + lay.offset[1], 4), std::memcpy(&pts[i].z, p + lay.offset[2], 4);
+    }
+    return true;
+  }
+  if (h.points == 0) return true;
+  const mloam_pcd_t body = pcdBody(bytes.data(), bytes.size(), h);
+  return mloam_pcd_decode(ctx, 1, &body, pts.data()) == MLOAM_OK;
 }
 
 // ---- mloam_msgs (header reduced to stamp + frame_id; nav_msgs/Odometry and PoseWithCovarianceStamped to what the nodes fill)

@@ -24,6 +24,7 @@
 #pragma once
 #include <array>
 #include <cmath>
+#include <cstdio>
 #include <cstring>
 #include <map>
 #include <memory>
@@ -602,5 +603,11 @@ inline mloam_solve_stats_t calibRig(mloam_ctx_t *ctx, int idx_ref, const std::ve
   }
   if (rows) *rows = r;
   return st;
+}
+
+// ---- pcl::io::loadPCDFile<pcl::PointXYZ> of the dataset nodes (rosNodeRVOxford.cpp:355-370): the file's points as float4 (x, y, z, 0),
+// an ASCII body decoded on the device by mloam_pcd_decode.  Returns 0, or -1 when the file cannot be read or is refused, as PCL does.
+inline int loadPCDFile(mloam_ctx_t *ctx, const std::string &path, std::vector<mloam_point_t> &cloud) {
+  return io::loadPCDPoints(ctx, path, cloud) ? 0 : -1;
 }
 }  // namespace mloam
