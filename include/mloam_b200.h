@@ -627,6 +627,51 @@ int mloam_global_map_chosen(mloam_ctx_t *ctx, int *h_ids, int cap, int *n);
 int mloam_cloud_msgs(mloam_ctx_t *ctx, int n, const int *sources, void *const *h_data, const size_t *cap_bytes, int *width);
 int mloam_cloud_msgs_device(mloam_ctx_t *ctx, int n, const int *sources, const void **d_data, int *width);
 
+/* ---- the mapper's clouds as ASCII PCD files: pcl::PCDWriter::write (= writeASCII(file, cloud, precision 8), PCL 1.8.0 pcd_io.hpp) of
+ *      saveGlobalMap (lidar_mapper_keyframe.cpp:853-919) and pcl::io::savePCDFileASCII, formatted on the device.  A file of n >= 1 points:
+ *   header  (generateHeader<PointT>, each line ending in '\n')
+ *             # .PCD v0.7 - Point Cloud Data file format
+ *             VERSION 0.7
+ *             FIELDS <names>        x y z | x y z intensity | x y z intensity cov_xx cov_xy cov_xz cov_yy cov_yz cov_zz cov_trace
+ *             SIZE 4 ... / TYPE F ... / COUNT 1 ...   one per field
+ *             WIDTH n / HEIGHT 1 / VIEWPOINT 0 0 0 1 0 0 0 / POINTS n / DATA ascii
+ *   body    one line per point in cloud order: each field `ostream << float` at precision 8 in the classic locale (%.8g of the float
+ *           widened to double), every NaN written "nan" whatever its sign or payload (PCL tests pcl_isnan first), +-inf "inf" / "-inf",
+ *           -0.0f "-0"; values separated by one space, no trailing space (boost::trim), each line ending in '\n'.
+ * PCL throws IOException on an empty cloud ("Input point cloud has no data!") and writes no file; here an empty cloud gives bytes 0 and
+ * is a success (host/mloam_adapter.hpp turns it into PCL's failure).
+ * The sources of mloam_cloud_pcd*: the six MLOAM_MSG_* clouds of mloam_cloud_msgs, with the same point types (PointXYZI: x y z
+ *   intensity; PointXYZIWithCov: the eleven fields), contents and cov_trace; and MLOAM_PCD_KEYFRAMES, pose_keyframes_3d of the keyframe
+ *   store (PointXYZI: the keyframe's float position, intensity = id, in id order), taken by these calls only.
+ * mloam_cloud_pcd: the files of n (1 .. 7) distinct sources, written by ONE launch on the context stream (outside every frame graph:
+ *   frames run, capture and replay as without it).  bytes[k] = file k's size, always set (also on MLOAM_E_INVALID for a capacity).
+ *   h_data[k] NULL: a size query for source k; otherwise the file is copied there when cap_bytes[k] holds it; if any does not,
+ *   MLOAM_E_INVALID and nothing is copied.
+ * mloam_cloud_pcd_device: the same files left in context memory, d_data[k] 256-byte aligned; valid until the next mloam_cloud_pcd* or
+ *   mloam_pcd_encode call, or the next call that replaces a source (as mloam_cloud_msgs_device; mloam_keyframe_save for the keyframes).
+ * mloam_pcd_encode: the files of n (1 .. 16) clouds the caller holds in host memory (savePCDFileASCII / PCDWriter::write of a
+ *   pcl::PointCloud<PointXYZ | PointXYZI | PointXYZIWithCov>): the clouds are copied up, written by one launch and copied back under
+ *   mloam_cloud_pcd's h_data / cap_bytes / bytes rules.
+ *   All three synchronise the context stream.  MLOAM_E_INVALID: n out of range, a NULL array, a source that is not one of the seven or
+ *   given twice; for mloam_pcd_encode a layout that is not one of the three, a negative count, a cloud of count > 0 with NULL pts (or
+ *   cov6 / trace for MLOAM_PCD_XYZI_COV); and a file that could exceed 2^31 - 1 bytes (its header and 15 bytes per field of every
+ *   point).  MLOAM_E_STATE: a registered source or a keyframe-store source as for mloam_cloud_msgs, and on a context with a
+ *   communicator. */
+#define MLOAM_PCD_KEYFRAMES 6
+#define MLOAM_PCD_XYZ 0      /* x y z */
+#define MLOAM_PCD_XYZI 1     /* x y z intensity */
+#define MLOAM_PCD_XYZI_COV 2 /* x y z intensity cov_xx cov_xy cov_xz cov_yy cov_yz cov_zz cov_trace */
+typedef struct {
+  const mloam_point_t *pts; /* count points: x, y, z, intensity (ignored by MLOAM_PCD_XYZ) */
+  const float *cov6;        /* MLOAM_PCD_XYZI_COV: 6 floats per point, cov_xx cov_xy cov_xz cov_yy cov_yz cov_zz */
+  const float *trace;       /* MLOAM_PCD_XYZI_COV: cov_trace per point */
+  int count;
+  int layout;               /* MLOAM_PCD_XYZ, MLOAM_PCD_XYZI or MLOAM_PCD_XYZI_COV */
+} mloam_pcd_cloud_t;
+int mloam_cloud_pcd(mloam_ctx_t *ctx, int n, const int *sources, void *const *h_data, const size_t *cap_bytes, size_t *bytes);
+int mloam_cloud_pcd_device(mloam_ctx_t *ctx, int n, const int *sources, const void **d_data, size_t *bytes);
+int mloam_pcd_encode(mloam_ctx_t *ctx, int n, const mloam_pcd_cloud_t *clouds, void *const *h_data, const size_t *cap_bytes, size_t *bytes);
+
 /* ---- FeatureExtract::matchCornerFromScan / matchSurfFromScan (feature_extract.hpp:131-376) against the map slot
  * built (mloam_map_build, cell ~1.3 m) from the previous sweep's less-sharp / less-flat features, which must be in
  * the reference's ring-sorted order (int(intensity) = ring).  type 'c': coeffs = [X_closest; X_second];

@@ -24,6 +24,8 @@ GLOBAL_MAP_SURROUND, GLOBAL_MAP_SAVE = 0, 1  # mloam_global_map modes: pubGlobal
 REGISTERED_FULL_RES, REGISTERED_SURF, REGISTERED_CORNER = 0, 1, 2  # mloam_frame_registered clouds (pubPointCloud)
 # mloam_cloud_msgs sources: PointXYZI messages (32 B per point), then PointXYZIWithCov messages (48 B per point)
 MSG_FULL_RES, MSG_SURF_LAST, MSG_CORNER_LAST, MSG_SURROUND, MSG_GLOBAL_MAP0, MSG_GLOBAL_MAP1 = 0, 1, 2, 3, 4, 5
+PCD_KEYFRAMES = 6  # mloam_cloud_pcd's seventh source: pose_keyframes_3d (PointXYZI)
+PCD_XYZ, PCD_XYZI, PCD_XYZI_COV = 0, 1, 2  # mloam_pcd_encode layouts
 E_NO_DEVICE = -2
 
 # every entry point include/mloam_b200.h declares
@@ -45,7 +47,7 @@ ABI_SYMBOLS = [
     "mloam_set_front_end_layout", "mloam_front_end_msg", "mloam_frame_msg", "mloam_frame_msg_device", "mloam_frame_set_next_msg",
     "mloam_frame_set_next_msg_device", "mloam_cloud_msgs", "mloam_cloud_msgs_device",
     "mloam_pcd_decode", "mloam_pcd_decode_device", "mloam_front_end_pcd", "mloam_frame_pcd", "mloam_frame_pcd_device",
-    "mloam_frame_set_next_pcd", "mloam_frame_set_next_pcd_device",
+    "mloam_frame_set_next_pcd", "mloam_frame_set_next_pcd_device", "mloam_cloud_pcd", "mloam_cloud_pcd_device", "mloam_pcd_encode",
 ]
 
 
@@ -159,6 +161,11 @@ def _pcds(bodies):
         for k in range(3):
             arr[f].index[k] = int(index[k])
     return arr
+
+
+class PcdCloud(C.Structure):
+    """mloam_pcd_cloud_t: one host cloud for mloam_pcd_encode (pts [count, 4]; cov6 [count, 6] and trace [count] for PCD_XYZI_COV)."""
+    _fields_ = [("pts", C.c_void_p), ("cov6", C.c_void_p), ("trace", C.c_void_p), ("count", C.c_int), ("layout", C.c_int)]
 
 
 def msg_step(source: int) -> int:
@@ -933,6 +940,56 @@ class Context:
 
             res.append(torch.as_tensor(_View(), device=f"cuda:{self.device}").clone())
         return res
+
+    # ---- the mapper's clouds and caller clouds as ASCII PCD files (PCDWriter::write on the device)
+    def _pcd_host(self, call, n, out):
+        """call(h_data, cap_bytes, bytes) with a size query first unless out (per file a writable uint8 array) is given."""
+        nb = (C.c_size_t * n)()
+        if out is None:
+            self._ck(call((C.c_void_p * n)(), (C.c_size_t * n)(), nb))
+            out = [np.empty(nb[k], np.uint8) for k in range(n)]
+        ptrs = (C.c_void_p * n)(*[a.__array_interface__["data"][0] if a.nbytes else None for a in out])
+        self._ck(call(ptrs, (C.c_size_t * n)(*[a.nbytes for a in out]), nb))
+        return [out[k][:nb[k]].tobytes() for k in range(n)]
+
+    def cloud_pcd(self, sources, out=None):
+        """The ASCII PCD file of each source (MSG_* or PCD_KEYFRAMES) as bytes, written by one launch per call (b"" for an empty
+        cloud).  out (optional): per source a writable uint8 array (pageable or pinned) the library copies into."""
+        src = (C.c_int * len(sources))(*[int(s) for s in sources])
+        return self._pcd_host(lambda h, cap, nb: lib().mloam_cloud_pcd(self._h, len(sources), src, h, cap, nb), len(sources), out)
+
+    def cloud_pcd_device(self, sources):
+        """The same files as CUDA uint8 tensors, cloned from the context's buffer (which the next PCD write reuses)."""
+        import torch
+
+        n = len(sources)
+        src, nb, ptrs = (C.c_int * n)(*[int(s) for s in sources]), (C.c_size_t * n)(), (C.c_void_p * n)()
+        self._ck(lib().mloam_cloud_pcd_device(self._h, n, src, ptrs, nb))
+        res = []
+        for k in range(n):
+            if nb[k] == 0:
+                res.append(torch.zeros(0, dtype=torch.uint8, device=f"cuda:{self.device}"))
+                continue
+
+            class _View:  # the context's buffer as a CUDA array, viewed without a copy
+                __cuda_array_interface__ = {"shape": (nb[k],), "typestr": "|u1", "data": (ptrs[k], False), "version": 3, "strides": None}
+
+            res.append(torch.as_tensor(_View(), device=f"cuda:{self.device}").clone())
+        return res
+
+    def pcd_encode(self, clouds, out=None):
+        """savePCDFileASCII of host clouds: each (layout, pts [n,4]) or (PCD_XYZI_COV, pts, cov6 [n,6], trace [n]) -> the files as bytes."""
+        n = len(clouds)
+        arr, keep = (PcdCloud * n)(), []
+        for k, c in enumerate(clouds):
+            layout, pts = int(c[0]), np.ascontiguousarray(c[1], np.float32).reshape(-1, 4)
+            keep.append(pts)
+            arr[k].pts, arr[k].count, arr[k].layout = _p(pts).value if pts.size else None, pts.shape[0], layout
+            if len(c) > 2:
+                c6, tr = np.ascontiguousarray(c[2], np.float32).reshape(-1, 6), np.ascontiguousarray(c[3], np.float32).reshape(-1)
+                keep += [c6, tr]
+                arr[k].cov6, arr[k].trace = _p(c6).value if c6.size else None, _p(tr).value if tr.size else None
+        return self._pcd_host(lambda h, cap, nb: lib().mloam_pcd_encode(self._h, n, arr, h, cap, nb), n, out)
 
     # ---- keyframe store (saveKeyframe / extractSurroundingKeyFrames on the device)
     def keyframes_init(self, distance_keyframes: float, orientation_keyframes_deg: float, surrounding_kf_radius: float, map_sur_kf_res: float,

@@ -511,6 +511,12 @@ struct Ctx {
   // mloam_cloud_msgs* (wire.cu): the packed PointCloud2 bytes of the last call, each message 256-byte aligned, then the widths.  No frame
   // graph references it, so its growth re-captures nothing.
   DevBuf cloud_msgs{nullptr, 0, false};
+  // mloam_cloud_pcd* / mloam_pcd_encode (pcd_write.cu): the files of the last call, each 256-byte aligned, then their sizes; the points
+  // uploaded for it (caller clouds, keyframe positions); the tile ticket counter and the look-back's tile words.  No frame graph
+  // references them.  The ticket counter is never reset: pcd_tickets is its value, and each call's tile words carry pcd_epoch.
+  DevBuf pcd_files{nullptr, 0, false}, pcd_src{nullptr, 0, false}, pcd_tiles{nullptr, 0, false};
+  unsigned long long pcd_tickets = 0;
+  unsigned pcd_epoch = 0;
   // mloam_pcd_decode* / mloam_front_end_pcd (pcd.cu): the host bodies' staging, and the PcdStage, per-CTA line counts and status word
   DevBuf pcd_in{nullptr, 0, false}, pcd_work{nullptr, 0, false};
   // PCD frames (pcd.cu pcd_decode_half): per half of the feature double buffer, the PcdStage, status word and per-CTA line counts
@@ -773,6 +779,9 @@ struct PackSeg {
 // keyframe.cu: the segments of source MLOAM_MSG_SURROUND (the filtered surf map, then the filtered corner map) or MLOAM_MSG_GLOBAL_MAP0 / 1
 // into seg[0..]; returns their count (1 or 2).  The caller has checked that the store exists.
 int keyframe_msg_segments(const Ctx *c, int source, PackSeg *seg);
+// keyframe.cu: pose_keyframes_3d in id order, x / y / z the keyframe's float position and w its id.  The caller has checked that the store
+// exists.
+void keyframe_positions(const Ctx *c, std::vector<float4> &pos);
 
 // comm.cu: in-place sum over ranks on the context stream (no-op without a communicator)
 int comm_allreduce_doubles(Ctx *c, double *d_buf, int count);

@@ -228,6 +228,12 @@ int keyframe_msg_segments(const Ctx *c, int source, PackSeg *seg) {
   return 1;
 }
 
+void keyframe_positions(const Ctx *c, std::vector<float4> &pos) {
+  const KeyframeStore &S = *c->kf;
+  pos.resize(S.kfs.size());
+  for (size_t i = 0; i < S.kfs.size(); i++) pos[i] = make_float4(S.kfs[i].pos[0], S.kfs[i].pos[1], S.kfs[i].pos[2], (float)i);
+}
+
 namespace {
 
 // saveKeyframe's test (:649-653): the float distance of the PointI positions, and Eigen's

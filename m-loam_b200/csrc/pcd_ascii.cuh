@@ -104,10 +104,10 @@ PCD_HD int big_cmp(const Big &a, const Big &b) {
     if (a.d[k] != b.d[k]) return a.d[k] < b.d[k] ? -1 : 1;
   return 0;
 }
-// sign of w * 10^q - (2m + 1) * 2^e.  Both sides stay below 2^180 for the w, q, m and e decimal_to_float passes.
-PCD_HD int cmp_halfway(uint64_t w, int q, uint32_t m, int e) {
+// sign of w * 10^q - b * 2^e, for callers whose aligned sides stay below 2^256
+PCD_HD int cmp_dec_bin(uint64_t w, int q, uint64_t b, int e) {
   Big x, y;
-  big_set(x, w), big_set(y, 2ull * m + 1ull);
+  big_set(x, w), big_set(y, b);
   if (q >= 0) big_mul_pow5(x, q);
   else big_mul_pow5(y, -q);
   const int s = q - e;  // x * 2^q vs y * 2^e
@@ -115,6 +115,8 @@ PCD_HD int cmp_halfway(uint64_t w, int q, uint32_t m, int e) {
   else big_shl(y, -s);
   return big_cmp(x, y);
 }
+// sign of w * 10^q - (2m + 1) * 2^e.  Both sides stay below 2^180 for the w, q, m and e decimal_to_float passes.
+PCD_HD int cmp_halfway(uint64_t w, int q, uint32_t m, int e) { return cmp_dec_bin(w, q, 2ull * m + 1ull, e); }
 
 // The float bits nearest to w * 10^q (ties to even), +inf past FLT_MAX's rounding boundary; w > 0, w < 10^19
 PCD_HD uint32_t decimal_to_float(uint64_t w, int q) {

@@ -645,4 +645,76 @@ int loadPCDFile(mloam_ctx_t *ctx, const std::string &path, pcl::PointCloud<Point
   for (size_t i = 0; i < pts.size(); i++) cloud[i].x = pts[i].x, cloud[i].y = pts[i].y, cloud[i].z = pts[i].z;
   return 0;
 }
+
+// ---- pcl::io::savePCDFileASCII / pcl::PCDWriter::write (= writeASCII at precision 8) of pcl::PointXYZ, pcl::PointXYZI and
+// pcl::PointXYZIWithCov clouds: the file written on the device by mloam_pcd_encode (the format: include/mloam_b200.h) and saved at path.
+// Returns 0, or -1 where PCL fails: an empty cloud (PCL throws IOException and writes nothing) or a file that cannot be written.
+namespace detail {
+// the point type's fields: cov_vec and cov_trace (PointXYZIWithCov), intensity (PointXYZI), neither (PointXYZ)
+template <typename P>
+auto pcd_point(const P &p, mloam_point_t &q, float *cov6, float *trace, int) -> decltype(p.cov_vec[0], p.cov_trace, int()) {
+  q.intensity = p.intensity;
+  for (int k = 0; k < 6; k++) cov6[k] = p.cov_vec[k];
+  *trace = p.cov_trace;
+  return MLOAM_PCD_XYZI_COV;
+}
+template <typename P>
+auto pcd_point(const P &p, mloam_point_t &q, float *, float *, long) -> decltype(p.intensity, int()) {
+  q.intensity = p.intensity;
+  return MLOAM_PCD_XYZI;
+}
+template <typename P>
+int pcd_point(const P &, mloam_point_t &, float *, float *, ...) {
+  return MLOAM_PCD_XYZ;
+}
+}  // namespace detail
+
+template <typename PointT>
+int savePCDFileASCII(mloam_ctx_t *ctx, const std::string &path, const pcl::PointCloud<PointT> &cloud) {
+  const size_t n = cloud.size();
+  if (n == 0) return -1;
+  std::vector<mloam_point_t> pts(n);
+  std::vector<float> cov6(6 * n), trace(n);
+  int layout = MLOAM_PCD_XYZ;
+  for (size_t i = 0; i < n; i++) {
+    pts[i] = mloam_point_t{cloud[i].x, cloud[i].y, cloud[i].z, 0.f};
+    layout = detail::pcd_point(cloud[i], pts[i], &cov6[6 * i], &trace[i], 0);
+  }
+  const mloam_pcd_cloud_t q = {pts.data(), cov6.data(), trace.data(), (int)n, layout};
+  std::vector<uint8_t> bytes(384 + n * 15 * (size_t)io::pcdFields(layout));  // the bound the library refuses beyond: one call
+  void *dst = bytes.data();
+  const size_t cap = bytes.size();
+  size_t nb = 0;
+  check(ctx, mloam_pcd_encode(ctx, 1, &q, &dst, &cap, &nb), "mloam_pcd_encode");
+  bytes.resize(nb);
+  return io::savePCD(path, bytes) ? 0 : -1;
+}
+
+class PCDWriter {
+ public:
+  explicit PCDWriter(mloam_ctx_t *ctx) : ctx_(ctx) {}
+  template <typename PointT>
+  int write(const std::string &path, const pcl::PointCloud<PointT> &cloud) {
+    return savePCDFileASCII(ctx_, path, cloud);
+  }
+
+ private:
+  mloam_ctx_t *ctx_;
+};
+
+// saveGlobalMap (lidar_mapper_keyframe.cpp:853-919) from the keyframe store: mloam_global_map(SAVE, kf_leaf 10 m, leaf 2 x MAP_SURF_RES),
+// then the three files pcd_writer.write gives, under dir (the reference's "/tmp/"): mloam_mapping_keyframes.pcd (pose_keyframes_3d),
+// mloam_mapping_surf_cloud[_wo_ua].pcd and mloam_mapping_corner_cloud[_wo_ua].pcd (maps 0 and 1), written by one launch.  As in the
+// reference, a file that PCL would refuse (an empty cloud) ends the save: -1, and the later files are not written.  Returns 0 or -1.
+inline int saveGlobalMap(mloam_ctx_t *ctx, const std::string &dir, bool with_ua, float map_surf_res) {
+  check(ctx, mloam_global_map(ctx, MLOAM_GLOBAL_MAP_SAVE, nullptr, 0.0, 10.0, 2.f * map_surf_res, nullptr, nullptr, nullptr), "mloam_global_map");
+  std::vector<uint8_t> files[3];
+  std::vector<std::vector<uint8_t> *> data = {&files[0], &files[1], &files[2]};
+  check(ctx, io::cloudPCD(ctx, {MLOAM_PCD_KEYFRAMES, MLOAM_MSG_GLOBAL_MAP0, MLOAM_MSG_GLOBAL_MAP1}, data), "mloam_cloud_pcd");
+  const std::string sfx = with_ua ? ".pcd" : "_wo_ua.pcd";
+  const std::string names[3] = {"mloam_mapping_keyframes.pcd", "mloam_mapping_surf_cloud" + sfx, "mloam_mapping_corner_cloud" + sfx};
+  for (int k = 0; k < 3; k++)
+    if (files[k].empty() || !io::savePCD(dir + names[k], files[k])) return -1;
+  return 0;
+}
 }  // namespace mloam

@@ -421,6 +421,74 @@ inline bool loadPCDPoints(mloam_ctx_t *ctx, const std::string &path, std::vector
   return mloam_pcd_decode(ctx, 1, &body, pts.data()) == MLOAM_OK;
 }
 
+// ---- PCD files written: pcl::PCDWriter::write(file, cloud) = writeASCII(file, cloud, 8) (PCL 1.8.0 pcd_io.hpp) of saveGlobalMap
+// (lidar_mapper_keyframe.cpp:853-919) and pcl::io::savePCDFileASCII (test_parse_bag.cpp:47-72); the format is stated with
+// mloam_cloud_pcd in include/mloam_b200.h.  The fields of a layout: pcdFields(MLOAM_PCD_*).
+inline int pcdFields(int layout) { return layout == MLOAM_PCD_XYZ ? 3 : layout == MLOAM_PCD_XYZI ? 4 : 11; }
+
+// PCL's writer restated with an ostringstream, precision 8, the classic locale and the pcl_isnan test: the file of n points (pts; cov6 /
+// trace for MLOAM_PCD_XYZI_COV).  An empty cloud gives "" (PCL throws and writes nothing).
+inline std::string writePCDASCII(int layout, const mloam_point_t *pts, const float *cov6, const float *trace, size_t n) {
+  if (n == 0) return std::string();
+  static const char *const names[11] = {"x", "y", "z", "intensity", "cov_xx", "cov_xy", "cov_xz", "cov_yy", "cov_yz", "cov_zz", "cov_trace"};
+  const int nf = pcdFields(layout);
+  std::ostringstream os;
+  os.imbue(std::locale::classic());
+  os << "# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS";
+  for (int f = 0; f < nf; f++) os << " " << names[f];
+  os << "\nSIZE";
+  for (int f = 0; f < nf; f++) os << " 4";
+  os << "\nTYPE";
+  for (int f = 0; f < nf; f++) os << " F";
+  os << "\nCOUNT";
+  for (int f = 0; f < nf; f++) os << " 1";
+  os << "\nWIDTH " << n << "\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS " << n << "\nDATA ascii\n";
+  os.precision(8);
+  for (size_t i = 0; i < n; i++) {
+    const float v[11] = {pts[i].x, pts[i].y, pts[i].z, pts[i].intensity, cov6 ? cov6[6 * i] : 0.f, cov6 ? cov6[6 * i + 1] : 0.f,
+                         cov6 ? cov6[6 * i + 2] : 0.f, cov6 ? cov6[6 * i + 3] : 0.f, cov6 ? cov6[6 * i + 4] : 0.f,
+                         cov6 ? cov6[6 * i + 5] : 0.f, trace ? trace[i] : 0.f};
+    for (int f = 0; f < nf; f++) {
+      if (f) os << " ";
+      if (v[f] != v[f]) os << "nan";
+      else os << v[f];
+    }
+    os << "\n";
+  }
+  return os.str();
+}
+
+// mloam_cloud_pcd of `sources` into data[k], each resized to its file.  The buffers' capacities are offered first, so a caller that keeps
+// its buffers pays one launch per call; a file that outgrew its buffer costs a second call.  Returns the library's code.
+inline int cloudPCD(mloam_ctx_t *ctx, const std::vector<int> &sources, std::vector<std::vector<uint8_t> *> &data) {
+  const size_t n = sources.size();
+  std::vector<void *> dst(n);
+  std::vector<size_t> cap(n), bytes(n, 0);
+  int rc = MLOAM_OK;
+  for (int pass = 0; pass < 2; pass++) {
+    for (size_t k = 0; k < n; k++) {
+      std::vector<uint8_t> &d = *data[k];
+      d.resize(pass == 0 ? d.capacity() : bytes[k]);
+      dst[k] = d.empty() ? nullptr : d.data(), cap[k] = d.size();
+    }
+    rc = mloam_cloud_pcd(ctx, (int)n, sources.data(), dst.data(), cap.data(), bytes.data());
+    bool fit = true;
+    for (size_t k = 0; k < n; k++) fit = fit && bytes[k] <= cap[k];
+    if (!fit && pass == 0) continue;  // too small (MLOAM_E_INVALID), or an empty buffer taken as a size query
+    break;
+  }
+  for (size_t k = 0; k < n && rc == MLOAM_OK; k++) data[k]->resize(bytes[k]);
+  return rc;
+}
+
+// The file bytes at path; false when it cannot be written
+inline bool savePCD(const std::string &path, const std::vector<uint8_t> &bytes) {
+  std::FILE *f = std::fopen(path.c_str(), "wb");
+  if (!f) return false;
+  const bool ok = std::fwrite(bytes.data(), 1, bytes.size(), f) == bytes.size();
+  return std::fclose(f) == 0 && ok;
+}
+
 // ---- mloam_msgs (header reduced to stamp + frame_id; nav_msgs/Odometry and PoseWithCovarianceStamped to what the nodes fill)
 struct Header {
   double stamp = 0.0;
