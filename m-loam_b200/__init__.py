@@ -417,51 +417,62 @@ class Context:
         self._ck(lib().mloam_set_front_end(self._h, int(vertical_scans), int(horizon_scans), C.c_double(roi_range), C.c_float(scan_period),
                                            int(time_field)))
 
+    # ---- the frame entry points: one sweep kind each, from host or device memory
+    def _frame(self, fn, sweep, maps, pose_init7, rebuild_maps):
+        """fn(ctx, *sweep, *maps, rebuild_maps, pose_init7, pose_out7, stats) -> (pose, stats)."""
+        pi = np.ascontiguousarray(pose_init7, np.float64)
+        out = np.zeros(7)
+        st = SolveStats()
+        self._ck(fn(self._h, *sweep, *maps, int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
+        return out, st.as_dict()
+
+    def _frame_host(self, fn, sweep, surf_map, corner_map, pose_init7, rebuild_maps):
+        sm = None if surf_map is None else _cloud(surf_map)
+        cm = None if corner_map is None else _cloud(corner_map)
+        maps = (_p(sm), 0 if sm is None else sm.shape[0], _p(cm), 0 if cm is None else cm.shape[0])
+        return self._frame(fn, sweep, maps, pose_init7, rebuild_maps)
+
+    def _frame_device(self, fn, sweep, d_surf_map, n_surf_map, d_corner_map, n_corner_map, pose_init7, rebuild_maps):
+        return self._frame(fn, sweep, (C.c_void_p(d_surf_map), n_surf_map, C.c_void_p(d_corner_map), n_corner_map), pose_init7, rebuild_maps)
+
+    def _announce(self, fn, keep, *args):
+        """A frame_set_next* call.  keep: its host inputs, which the coming frame call reads; held until the next announcement or
+        withdrawal (None)."""
+        self._next_keep = keep
+        self._ck(fn(self._h, *args))
+
+    def _front_end(self, fn, n_pts, *sweep):
+        """fn(ctx, *sweep, out, n_out, scan_start, scan_end) -> (ring-ordered sweep, scan_start, scan_end)."""
+        out = np.empty((max(n_pts, 1), 4), np.float32)
+        ss, se = np.zeros(1024, np.int32), np.zeros(1024, np.int32)
+        n = C.c_int(0)
+        self._ck(fn(self._h, *sweep, _p(out), C.byref(n), _p(ss), _p(se)))
+        return out[: n.value].copy(), ss, se
+
     def front_end(self, raw, counts):
         """The front end of frame_raw() alone -> (ring-ordered sweep, scan_start, scan_end); the first n_lidars x vertical_scans entries
         of scan_start / scan_end are the sweep's ScanInfo."""
         raw = _cloud(raw)
         cnt = np.ascontiguousarray(counts, np.int32)
-        out = np.empty((max(raw.shape[0], 1), 4), np.float32)
-        n_rings = 1024
-        ss, se = np.zeros(n_rings, np.int32), np.zeros(n_rings, np.int32)
-        n = C.c_int(0)
-        self._ck(lib().mloam_front_end(self._h, _p(raw), _p(cnt), _p(out), C.byref(n), _p(ss), _p(se)))
-        return out[: n.value].copy(), ss, se
+        return self._front_end(lib().mloam_front_end, raw.shape[0], _p(raw), _p(cnt))
 
     def frame_raw(self, raw, counts, surf_map, corner_map, pose_init7, rebuild_maps: bool = True):
         """mloam_frame on the rig's raw sweeps (concatenated LiDAR-major, counts[l] points of LiDAR l)."""
         raw = _cloud(raw)
         cnt = np.ascontiguousarray(counts, np.int32)
-        sm = None if surf_map is None else _cloud(surf_map)
-        cm = None if corner_map is None else _cloud(corner_map)
-        pi = np.ascontiguousarray(pose_init7, np.float64)
-        out = np.zeros(7)
-        st = SolveStats()
-        self._ck(lib().mloam_frame_raw(self._h, _p(raw), _p(cnt), _p(sm), 0 if sm is None else sm.shape[0], _p(cm),
-                                       0 if cm is None else cm.shape[0], int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
-        return out, st.as_dict()
+        return self._frame_host(lib().mloam_frame_raw, (_p(raw), _p(cnt)), surf_map, corner_map, pose_init7, rebuild_maps)
 
     def frame_raw_device(self, d_raw: int, counts, d_surf_map: int, n_surf_map: int, d_corner_map: int, n_corner_map: int, pose_init7,
                          rebuild_maps: bool = True):
         cnt = np.ascontiguousarray(counts, np.int32)
-        pi = np.ascontiguousarray(pose_init7, np.float64)
-        out = np.zeros(7)
-        st = SolveStats()
-        self._ck(lib().mloam_frame_raw_device(self._h, C.c_void_p(d_raw), _p(cnt), C.c_void_p(d_surf_map), n_surf_map, C.c_void_p(d_corner_map),
-                                              n_corner_map, int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
-        return out, st.as_dict()
+        return self._frame_device(lib().mloam_frame_raw_device, (C.c_void_p(d_raw), _p(cnt)), d_surf_map, n_surf_map, d_corner_map,
+                                  n_corner_map, pose_init7, rebuild_maps)
 
     def frame_set_next_raw(self, raw, counts):
         """Announce the raw sweeps of the next frame_raw() call (pass the SAME array to it).  None withdraws."""
-        if raw is None:
-            self._next_keep = None
-            self._ck(lib().mloam_frame_set_next_raw(self._h, None, None))
-            return
-        raw = _cloud(raw)
-        cnt = np.ascontiguousarray(counts, np.int32)
-        self._next_keep = (raw, cnt)  # must outlive the coming frame call
-        self._ck(lib().mloam_frame_set_next_raw(self._h, _p(raw), _p(cnt)))
+        raw = None if raw is None else _cloud(raw)
+        cnt = None if raw is None else np.ascontiguousarray(counts, np.int32)
+        self._announce(lib().mloam_frame_set_next_raw, (raw, cnt), _p(raw), _p(cnt))
 
     def frame_set_next_raw_device(self, d_raw: int, counts):
         cnt = None if d_raw is None else np.ascontiguousarray(counts, np.int32)
@@ -476,12 +487,23 @@ class Context:
     def front_end_msg(self, msgs):
         """front_end() on the rig's messages (host bytes, see _msgs) -> (ring-ordered sweep, scan_start, scan_end)."""
         arr = _msgs(msgs)
-        n_pts = sum(int(m.width) * int(m.height) for m in arr)
-        out = np.empty((max(n_pts, 1), 4), np.float32)
-        ss, se = np.zeros(1024, np.int32), np.zeros(1024, np.int32)
-        n = C.c_int(0)
-        self._ck(lib().mloam_front_end_msg(self._h, arr, _p(out), C.byref(n), _p(ss), _p(se)))
-        return out[: n.value].copy(), ss, se
+        return self._front_end(lib().mloam_front_end_msg, sum(int(m.width) * int(m.height) for m in arr), arr)
+
+    def frame_msg(self, msgs, surf_map, corner_map, pose_init7, rebuild_maps: bool = True):
+        """frame_raw() on the rig's messages in host memory (see _msgs)."""
+        return self._frame_host(lib().mloam_frame_msg, (_msgs(msgs),), surf_map, corner_map, pose_init7, rebuild_maps)
+
+    def frame_msg_device(self, msgs, d_surf_map: int, n_surf_map: int, d_corner_map: int, n_corner_map: int, pose_init7, rebuild_maps: bool = True):
+        """frame_raw_device() on the rig's messages in device memory: msgs per LiDAR (ptr, size, width, height, row_step)."""
+        return self._frame_device(lib().mloam_frame_msg_device, (_msgs(msgs),), d_surf_map, n_surf_map, d_corner_map, n_corner_map, pose_init7,
+                                  rebuild_maps)
+
+    def frame_set_next_msg(self, msgs):
+        """Announce the messages of the next frame_msg() call (pass the SAME arrays to it).  None withdraws."""
+        self._announce(lib().mloam_frame_set_next_msg, msgs, None if msgs is None else _msgs(msgs))
+
+    def frame_set_next_msg_device(self, msgs):
+        self._ck(lib().mloam_frame_set_next_msg_device(self._h, None if msgs is None else _msgs(msgs)))
 
     # ---- PCD files (ASCII bodies decoded on the device)
     def pcd_decode(self, bodies) -> np.ndarray:
@@ -499,66 +521,23 @@ class Context:
     def front_end_pcd(self, bodies):
         """front_end() on the rig's ASCII PCD bodies (host bytes, see _pcds) -> (ring-ordered sweep, scan_start, scan_end)."""
         arr = _pcds(bodies)
-        out = np.empty((max(sum(max(0, b.points) for b in arr), 1), 4), np.float32)
-        ss, se = np.zeros(1024, np.int32), np.zeros(1024, np.int32)
-        n = C.c_int(0)
-        self._ck(lib().mloam_front_end_pcd(self._h, arr, _p(out), C.byref(n), _p(ss), _p(se)))
-        return out[: n.value].copy(), ss, se
+        return self._front_end(lib().mloam_front_end_pcd, sum(max(0, b.points) for b in arr), arr)
 
     def frame_pcd(self, bodies, surf_map, corner_map, pose_init7, rebuild_maps: bool = True):
         """frame_raw() on the rig's ASCII PCD bodies in host memory (see _pcds)."""
-        sm = None if surf_map is None else _cloud(surf_map)
-        cm = None if corner_map is None else _cloud(corner_map)
-        pi = np.ascontiguousarray(pose_init7, np.float64)
-        out = np.zeros(7)
-        st = SolveStats()
-        self._ck(lib().mloam_frame_pcd(self._h, _pcds(bodies), _p(sm), 0 if sm is None else sm.shape[0], _p(cm), 0 if cm is None else cm.shape[0],
-                                       int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
-        return out, st.as_dict()
+        return self._frame_host(lib().mloam_frame_pcd, (_pcds(bodies),), surf_map, corner_map, pose_init7, rebuild_maps)
 
     def frame_pcd_device(self, bodies, d_surf_map: int, n_surf_map: int, d_corner_map: int, n_corner_map: int, pose_init7, rebuild_maps: bool = True):
         """frame_raw_device() on the rig's bodies in device memory: per LiDAR (ptr, size, points, tokens, index)."""
-        pi = np.ascontiguousarray(pose_init7, np.float64)
-        out = np.zeros(7)
-        st = SolveStats()
-        self._ck(lib().mloam_frame_pcd_device(self._h, _pcds(bodies), C.c_void_p(d_surf_map), n_surf_map, C.c_void_p(d_corner_map), n_corner_map,
-                                              int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
-        return out, st.as_dict()
+        return self._frame_device(lib().mloam_frame_pcd_device, (_pcds(bodies),), d_surf_map, n_surf_map, d_corner_map, n_corner_map, pose_init7,
+                                  rebuild_maps)
 
     def frame_set_next_pcd(self, bodies):
         """Announce the bodies of the next frame_pcd() call (pass the SAME arrays to it).  None withdraws."""
-        self._ck(lib().mloam_frame_set_next_pcd(self._h, None if bodies is None else _pcds(bodies)))
+        self._announce(lib().mloam_frame_set_next_pcd, bodies, None if bodies is None else _pcds(bodies))
 
     def frame_set_next_pcd_device(self, bodies):
         self._ck(lib().mloam_frame_set_next_pcd_device(self._h, None if bodies is None else _pcds(bodies)))
-
-    def frame_msg(self, msgs, surf_map, corner_map, pose_init7, rebuild_maps: bool = True):
-        """frame_raw() on the rig's messages in host memory (see _msgs)."""
-        sm = None if surf_map is None else _cloud(surf_map)
-        cm = None if corner_map is None else _cloud(corner_map)
-        pi = np.ascontiguousarray(pose_init7, np.float64)
-        out = np.zeros(7)
-        st = SolveStats()
-        self._ck(lib().mloam_frame_msg(self._h, _msgs(msgs), _p(sm), 0 if sm is None else sm.shape[0], _p(cm), 0 if cm is None else cm.shape[0],
-                                       int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
-        return out, st.as_dict()
-
-    def frame_msg_device(self, msgs, d_surf_map: int, n_surf_map: int, d_corner_map: int, n_corner_map: int, pose_init7, rebuild_maps: bool = True):
-        """frame_raw_device() on the rig's messages in device memory: msgs per LiDAR (ptr, size, width, height, row_step)."""
-        pi = np.ascontiguousarray(pose_init7, np.float64)
-        out = np.zeros(7)
-        st = SolveStats()
-        self._ck(lib().mloam_frame_msg_device(self._h, _msgs(msgs), C.c_void_p(d_surf_map), n_surf_map, C.c_void_p(d_corner_map), n_corner_map,
-                                              int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
-        return out, st.as_dict()
-
-    def frame_set_next_msg(self, msgs):
-        """Announce the messages of the next frame_msg() call (pass the SAME arrays to it).  None withdraws."""
-        self._next_keep = msgs  # must outlive the coming frame call
-        self._ck(lib().mloam_frame_set_next_msg(self._h, None if msgs is None else _msgs(msgs)))
-
-    def frame_set_next_msg_device(self, msgs):
-        self._ck(lib().mloam_frame_set_next_msg_device(self._h, None if msgs is None else _msgs(msgs)))
 
     # ---- orchestrators
     def scan2map(self, surf_scan, corner_scan, pose_init7):
@@ -581,41 +560,27 @@ class Context:
         cloud = _cloud(cloud)
         ss = np.ascontiguousarray(scan_start, np.int32)
         se = np.ascontiguousarray(scan_end, np.int32)
-        sm = None if surf_map is None else _cloud(surf_map)
-        cm = None if corner_map is None else _cloud(corner_map)
-        pi = np.ascontiguousarray(pose_init7, np.float64)
-        out = np.zeros(7)
-        st = SolveStats()
-        self._ck(lib().mloam_frame(self._h, _p(cloud), cloud.shape[0], _p(ss), _p(se), ss.shape[0], _p(sm),
-                                   0 if sm is None else sm.shape[0], _p(cm), 0 if cm is None else cm.shape[0], int(rebuild_maps),
-                                   _p(pi), _p(out), C.byref(st)))
-        return out, st.as_dict()
+        return self._frame_host(lib().mloam_frame, (_p(cloud), cloud.shape[0], _p(ss), _p(se), ss.shape[0]), surf_map, corner_map, pose_init7,
+                                rebuild_maps)
 
     def frame_set_next(self, cloud, scan_start, scan_end):
         """Announce the sweep of the next frame() call (host arrays; pass the SAME arrays to that call): it is extracted on a side
         stream while the coming frame is solved.  None withdraws."""
         if cloud is None:
-            self._next_keep = None
-            self._ck(lib().mloam_frame_set_next(self._h, None, 0, None, None, 0))
+            self._announce(lib().mloam_frame_set_next, None, None, 0, None, None, 0)
             return
         cloud = _cloud(cloud)
         ss = np.ascontiguousarray(scan_start, np.int32)
         se = np.ascontiguousarray(scan_end, np.int32)
-        self._next_keep = (cloud, ss, se)  # must outlive the coming frame call
-        self._ck(lib().mloam_frame_set_next(self._h, _p(cloud), cloud.shape[0], _p(ss), _p(se), ss.shape[0]))
+        self._announce(lib().mloam_frame_set_next, (cloud, ss, se), _p(cloud), cloud.shape[0], _p(ss), _p(se), ss.shape[0])
 
     def frame_set_next_device(self, d_cloud: int, n: int, d_scan_start: int, d_scan_end: int, n_scans: int):
         self._ck(lib().mloam_frame_set_next_device(self._h, C.c_void_p(d_cloud), n, C.c_void_p(d_scan_start), C.c_void_p(d_scan_end), n_scans))
 
     def frame_device(self, d_cloud: int, n: int, d_scan_start: int, d_scan_end: int, n_scans: int, d_surf_map: int, n_surf_map: int,
                      d_corner_map: int, n_corner_map: int, pose_init7, rebuild_maps: bool = True):
-        pi = np.ascontiguousarray(pose_init7, np.float64)
-        out = np.zeros(7)
-        st = SolveStats()
-        self._ck(lib().mloam_frame_device(self._h, C.c_void_p(d_cloud), n, C.c_void_p(d_scan_start), C.c_void_p(d_scan_end), n_scans,
-                                          C.c_void_p(d_surf_map), n_surf_map, C.c_void_p(d_corner_map), n_corner_map,
-                                          int(rebuild_maps), _p(pi), _p(out), C.byref(st)))
-        return out, st.as_dict()
+        sweep = (C.c_void_p(d_cloud), n, C.c_void_p(d_scan_start), C.c_void_p(d_scan_end), n_scans)
+        return self._frame_device(lib().mloam_frame_device, sweep, d_surf_map, n_surf_map, d_corner_map, n_corner_map, pose_init7, rebuild_maps)
 
     def match_from_scan(self, slot: int, kind: str, pts, pose7):
         pts = _cloud(pts)

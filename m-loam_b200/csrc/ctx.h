@@ -182,21 +182,26 @@ struct FrameCfg {
   const double *part_ext(int l) const { return rig_merge() ? lidar_ext[l] : ext; }
 };
 
-// One sweep of a frame (mloam_frame*) or announced for the next one (mloam_frame_set_next*)
+// What the caller hands a frame: a ring-ordered cloud with its ScanInfo (mloam_frame*), or the rig's raw sweeps, which the front end
+// turns into one (mloam_frame_raw*) — given as such, as PointCloud2 messages (mloam_frame_msg*, wire.cu) or as ASCII PCD bodies
+// (mloam_frame_pcd*, pcd.cu)
+enum class SweepKind : int { ring, raw, msg, pcd };
+
+// One sweep of a frame (mloam_frame*) or announced for the next one (mloam_frame_set_next*).  What its kind does not use stays zero:
+// the look-ahead compares the payloads (L, wire, pcdf) whole and the frame graph key hashes them whole.
 struct Sweep {
-  const void *key = nullptr;             // the caller's cloud pointer (host or device): the look-ahead matches on it
-  const float4 *cloud = nullptr;         // the sweep on the device (a host sweep: where its copy goes)
-  const int *scan_start = nullptr, *scan_end = nullptr;      // its ScanInfo on the device; none for a raw sweep (the front end makes it)
-  const int *h_scan_start = nullptr, *h_scan_end = nullptr;  // a host sweep's ScanInfo in host memory
-  int n = 0, n_scans = 0;
+  SweepKind kind = SweepKind::ring;
+  const void *key = nullptr;             // the caller's pointer (host or device; the first message's or body's data): the look-ahead matches on it
   bool host = false;                     // key is a host pointer
-  bool raw = false;                      // the rig's raw sweeps with layout L: the front end runs before extraction
-  RigLayout L{};
-  bool msg = false;                      // raw sweeps as PointCloud2 messages (wire): unpacked on the device before the front end
-  WireMsgs wire{};
-  const unsigned char *bytes = nullptr;  // a host message or PCD sweep: where its bytes are copied (wire_stage_offset / pcd_stage per LiDAR)
-  bool pcd = false;                      // raw sweeps as ASCII PCD bodies: decoded on the device before the front end
-  PcdFiles pcdf{};
+  int n = 0, n_scans = 0;                // points (a raw-like sweep: in all of the rig's raw sweeps) and rings
+  const float4 *cloud = nullptr;         // ring, raw: the sweep on the device (a host sweep: where its copy goes)
+  const int *scan_start = nullptr, *scan_end = nullptr;      // ring: its ScanInfo on the device
+  const int *h_scan_start = nullptr, *h_scan_end = nullptr;  // ring, host: its ScanInfo in host memory
+  RigLayout L{};                         // raw, msg, pcd: where each LiDAR's points lie in the raw sweep
+  WireMsgs wire{};                       // msg: the messages and the layouts they were checked against
+  PcdFiles pcdf{};                       // pcd: the bodies
+  const unsigned char *bytes = nullptr;  // msg, pcd from host memory: where the bytes are copied (wire_stage_offset / pcd_stage per LiDAR)
+  bool raw_like() const { return kind != SweepKind::ring; }  // the front end runs before extraction
 };
 
 // the per-point association with uncertainty (uct.h): per LiDAR of the rig, and per run
@@ -831,24 +836,29 @@ int project_cloud_device(Ctx *c, const float4 *d_in, const RigLayout &L, int ver
 // *d_n_out their count.
 int front_times_device(Ctx *c, const float4 *d_in, const RigLayout &L, int time_field, float scan_period, float4 *d_out, int *d_n_out,
                        DevBuf &work);
-// wire.cu: the PointCloud2 messages of sweep sw (sw.msg) -> the float4 raw sweep out (sw.L's offsets), one launch on c->stream
+// wire.cu: the PointCloud2 messages of message sweep sw -> the float4 raw sweep out (sw.L's offsets), one launch on c->stream
 int wire_unpack_device(Ctx *c, const Sweep &sw, float4 *out);
-// where LiDAR l's bytes lie in a host message sweep's device staging (256-byte aligned), and l = n_lidars: the staging's size
-size_t wire_stage_offset(const WireMsgs &w, int l);
+// Host message / PCD sweep *sw: point sw->bytes into B, which grows to hold each LiDAR's bytes, and with `upload` copy them there on st.
+// The PCD staging keeps room for bodies half as large again, so that a replay of other files rarely grows it (a growth re-captures the
+// frame graphs).
+int wire_upload(Ctx *c, DevBuf &B, Sweep *sw, bool upload, cudaStream_t st);
+int pcd_upload(Ctx *c, DevBuf &B, Sweep *sw, bool upload, cudaStream_t st);
 // The n ASCII PCD bodies (host bytes: staged through Ctx::pcd_in) -> their points, file after file, at out on c->stream; waits for the
 // stream and returns MLOAM_E_INVALID for a refused body
 int pcd_decode_device(Ctx *c, int n, const mloam_pcd_t *pcds, bool host, float4 *out);
 // The checks of n ASCII PCD bodies every PCD entry point makes (MLOAM_E_INVALID), and the message of refusal bits (MLOAM_OK for none)
 int pcd_check(Ctx *c, int n, const mloam_pcd_t *pcds);
 int pcd_refusal(Ctx *c, unsigned bits);
-// The PcdStage of a PCD sweep: each body's size and, for host bytes, its offset in the device staging (256-byte aligned) — staged per
-// frame, never part of a graph key
-void pcd_stage(const Sweep &sw, PcdStage *st);
 // The decode of PCD sweep sw in a frame, on c->stream (also while capturing): its PcdStage copied from PinnedBlock::pcd_half[half]
 // (staged by the frame), the refusal bits into the half's status word, the points to out
 int pcd_decode_half(Ctx *c, const Sweep &sw, int half, float4 *out);
-// The half's device status word (the frame lands it in PinnedBlock::pcd_half_status)
-unsigned *pcd_half_status(Ctx *c);
+// What a frame does for sweep sw that only a PCD sweep needs (nothing for the other kinds).  stage: its bodies' byte sizes (and staging
+// offsets) into PinnedBlock::pcd_half[half], before the frame is enqueued and before every replay — they change from file to file and the
+// captured decode reads them at execution time.  land: the refusal bits of both halves into PinnedBlock::pcd_half_status, on c->stream at
+// the frame's end.  refusal: after the frame, MLOAM_E_INVALID for a body the decode in half `half` refused (waits for the stream).
+void pcd_frame_stage(Ctx *c, const Sweep &sw, int half);
+int pcd_frame_land(Ctx *c, const Sweep &sw);
+int pcd_frame_refusal(Ctx *c, const Sweep &sw, int half);
 int transform_segments_device(Ctx *c, float4 *d_pts, int n, const int *d_off, int n_seg, const float *d_mat12);
 // VoxelGridCovarianceMLOAM<PointIWithCov>::filter: covariance-weighted merge per voxel (cov6 + trace per point in and out)
 int voxel_downsample_cov_device(Ctx *c, const float4 *d_in, const float *d_cov6, const float *d_trace, int n, const int *d_n_in, float leaf,

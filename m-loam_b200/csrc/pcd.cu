@@ -202,13 +202,27 @@ int pcd_refusal(Ctx *c, unsigned s) {
   return MLOAM_OK;
 }
 
-void pcd_stage(const Sweep &sw, PcdStage *st) {
+// The PcdStage of a PCD sweep: each body's size and, for host bytes, its offset in the device staging (256-byte aligned) — staged per
+// frame, never part of a graph key
+static void pcd_stage(const Sweep &sw, PcdStage *st) {
   long long off = 0;
   for (int l = 0; l < sw.L.n_lidars; l++) {
     const mloam_pcd_t &p = sw.pcdf.body[l];
     st->size[l] = (long long)p.size, st->off[l] = sw.host ? off : 0;
     off += (long long)((p.size + 255) & ~(size_t)255);
   }
+}
+
+int pcd_upload(Ctx *c, DevBuf &B, Sweep *sw, bool upload, cudaStream_t st) {
+  PcdStage ps;
+  pcd_stage(*sw, &ps);
+  const int nl = sw->L.n_lidars;
+  const size_t need = (size_t)(ps.off[nl - 1] + ps.size[nl - 1]) + 16;
+  if (need > B.cap) MLOAM_CUDA_OK(c, B.reserve(need + need / 2));
+  sw->bytes = B.as<unsigned char>();
+  for (int l = 0; upload && l < nl; l++)
+    if (ps.size[l]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(B.as<unsigned char>() + ps.off[l], sw->pcdf.body[l].data, (size_t)ps.size[l], cudaMemcpyHostToDevice, st));
+  return MLOAM_OK;
 }
 
 int pcd_decode_half(Ctx *c, const Sweep &sw, int half, float4 *out) {
@@ -220,9 +234,23 @@ int pcd_decode_half(Ctx *c, const Sweep &sw, int half, float4 *out) {
   return pcd_launch(c, R, &c->pinned->pcd_half[half], H.stage, H.counts, H.status, out);
 }
 
-unsigned *pcd_half_status(Ctx *c) {
+void pcd_frame_stage(Ctx *c, const Sweep &sw, int half) {
+  if (sw.kind == SweepKind::pcd) pcd_stage(sw, &c->pinned->pcd_half[half]);
+}
+
+int pcd_frame_land(Ctx *c, const Sweep &sw) {
+  if (sw.kind != SweepKind::pcd) return MLOAM_OK;
   PcdHalf H;
-  return pcd_frame_bufs(c, 0, &H) == MLOAM_OK ? H.status : nullptr;
+  const int rc = pcd_frame_bufs(c, 0, &H);
+  if (rc) return rc;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->pinned->pcd_half_status, H.status, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
+  return MLOAM_OK;
+}
+
+int pcd_frame_refusal(Ctx *c, const Sweep &sw, int half) {
+  if (sw.kind != SweepKind::pcd) return MLOAM_OK;
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
+  return pcd_refusal(c, c->pinned->pcd_half_status[half]);
 }
 
 int pcd_decode_device(Ctx *c, int n, const mloam_pcd_t *pcds, bool host, float4 *out) {

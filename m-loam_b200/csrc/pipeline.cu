@@ -321,6 +321,115 @@ const UndistPoses *undist_ahead(const Ctx *c) {
   return c->cfg.undist_on && c->next.set && c->next.undist.n > 0 && c->use_lookahead && !c->prof_on ? &c->next.undist : nullptr;
 }
 
+// ---- what depends on a sweep's kind: one switch per decision (pcd.cu: pcd_frame_stage, pcd_frame_land, pcd_frame_refusal)
+// Whether sweep sw is the announced sweep a: the same kind, caller pointer and sizes, and a host frame takes a host announcement only (a
+// device frame may take either).
+bool same_sweep(const Sweep &a, const Sweep &sw) {
+  if (a.kind != sw.kind || a.key != sw.key || a.n != sw.n || a.n_scans != sw.n_scans || !(a.host || !sw.host)) return false;
+  if (std::memcmp(&a.L, &sw.L, sizeof(RigLayout)) != 0) return false;  // a raw-like sweep: the same per-LiDAR counts
+  switch (sw.kind) {
+    case SweepKind::ring:
+    case SweepKind::raw: return true;
+    case SweepKind::msg: return std::memcmp(&a.wire, &sw.wire, sizeof(WireMsgs)) == 0;  // the same messages (pointers, shapes) and layouts
+    case SweepKind::pcd: return std::memcmp(&a.pcdf, &sw.pcdf, sizeof(PcdFiles)) == 0;  // the same bodies (pointers, sizes, POINTS, tokens)
+  }
+  return false;
+}
+
+// Point the device side of host sweep *sw into B and, with `upload`, copy the sweep there on st.  A ring sweep's ScanInfo goes through
+// the pinned rows pin: an async copy from pageable memory would block the host behind the sweep's copy.
+int sweep_to_device(Ctx *c, DevBuf &B, Sweep *sw, bool upload, int (*pin)[MLOAM_MAX_RINGS], cudaStream_t st) {
+  switch (sw->kind) {
+    case SweepKind::ring:
+    case SweepKind::raw: {  // the points, then room for the ScanInfo, which a raw sweep has not (the front end makes it)
+      SweepIn D;
+      int rc = sweep_bufs(c, B, sw->n, sw->n_scans, &D);
+      if (rc) return rc;
+      sw->cloud = D.cloud;
+      const bool ring = sw->kind == SweepKind::ring;
+      if (ring) sw->scan_start = D.scan_start, sw->scan_end = D.scan_end;
+      if (!upload) return MLOAM_OK;
+      const int ns = sw->n_scans;
+      if (ring) {
+        std::memcpy(pin[0], sw->h_scan_start, sizeof(int) * ns), std::memcpy(pin[1], sw->h_scan_end, sizeof(int) * ns);
+        MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.scan_start, pin[0], sizeof(int) * ns, cudaMemcpyHostToDevice, st));
+        MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.scan_end, pin[1], sizeof(int) * ns, cudaMemcpyHostToDevice, st));
+      }
+      MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.cloud, sw->key, sizeof(float4) * (size_t)sw->n, cudaMemcpyHostToDevice, st));
+      return MLOAM_OK;
+    }
+    case SweepKind::msg: return wire_upload(c, B, sw, upload, st);
+    case SweepKind::pcd: return pcd_upload(c, B, sw, upload, st);
+  }
+  return MLOAM_E_INVALID;
+}
+
+// The points on the device that extraction reads (a ring sweep) or the front end reads (a raw-like one), on c->stream: the caller's or the
+// staged cloud, or the messages unpacked / the PCD bodies decoded into wire_out.  The decode reads the bodies' byte sizes staged for half
+// `parity` (pcd_frame_stage).
+int sweep_points(Ctx *c, const Sweep &sw, int parity, const float4 **out) {
+  switch (sw.kind) {
+    case SweepKind::ring:
+    case SweepKind::raw: *out = sw.cloud; return MLOAM_OK;
+    case SweepKind::msg:
+    case SweepKind::pcd: {
+      MLOAM_CUDA_OK(c, c->wire_out.reserve(sizeof(float4) * ((size_t)sw.n + 1)));
+      float4 *w = c->wire_out.as<float4>();
+      *out = w;
+      return sw.kind == SweepKind::msg ? wire_unpack_device(c, sw, w) : pcd_decode_half(c, sw, parity, w);
+    }
+  }
+  return MLOAM_E_INVALID;
+}
+
+// A sweep's part of the frame graph key (FrameKey)
+struct SweepKey {
+  const void *ptr[4];  // the sweep on the device (cloud, scan_start, scan_end) and the caller's pointer
+  FrontEnd front;      // a raw-like sweep: kernel arguments of the captured front end
+  RigLayout L;
+  int n, n_scans;
+};
+
+// FNV-1a over 8-byte words: the key is built on the frame's host critical path
+inline unsigned long long fnv(unsigned long long h, unsigned long long w) { return (h ^ w) * 1099511628211ull; }
+unsigned long long fnv_words(unsigned long long h, const void *p, size_t bytes) {
+  unsigned long long w;
+  for (size_t i = 0; i < bytes; i += 8) memcpy(&w, static_cast<const char *>(p) + i, 8), h = fnv(h, w);
+  return h;
+}
+
+// Sweep x's part of the frame graph key: *k, and what a message or PCD sweep's capture holds besides, mixed into h before the rest of the
+// key — only for such a sweep, so that a context that never takes one keeps the keys it had without them — tagged by kind and by slot
+// (next: the announced sweep)
+unsigned long long sweep_key(const Sweep &x, const FrontEnd &fe, bool next, SweepKey *k, unsigned long long h) {
+  k->ptr[0] = x.cloud, k->ptr[1] = x.scan_start, k->ptr[2] = x.scan_end, k->ptr[3] = x.key;
+  k->n = x.n, k->n_scans = x.n_scans;
+  if (x.raw_like()) k->front = fe, k->L = x.L;
+  switch (x.kind) {
+    case SweepKind::ring:
+    case SweepKind::raw: return h;
+    case SweepKind::msg:  // the messages, layouts and staging are kernel arguments of the captured unpack
+      h = fnv(h, next ? 8ull : 4ull);
+      h = fnv(h, (unsigned long long)reinterpret_cast<uintptr_t>(x.bytes));
+      return fnv_words(h, &x.wire, sizeof(WireMsgs));
+    case SweepKind::pcd:
+      // the decode's kernel arguments — the staging or the device bodies, POINTS, tokens and token indices — but not the byte sizes, which
+      // are staged (pcd_frame_stage), so that files of other sizes replay the same graph.  A host sweep is copied into the staging whatever
+      // the caller's buffer: its pointer is no kernel argument (a dataset replay reads every file into a new place).
+      if (x.host) k->ptr[3] = nullptr;
+      h = fnv(h, next ? 32ull : 16ull);
+      h = fnv(h, (unsigned long long)reinterpret_cast<uintptr_t>(x.host ? x.bytes : nullptr));
+      for (int l = 0; l < x.L.n_lidars; l++) {
+        const mloam_pcd_t &p = x.pcdf.body[l];
+        h = fnv(h, (unsigned long long)reinterpret_cast<uintptr_t>(x.host ? nullptr : p.data));
+        h = fnv(h, (unsigned long long)(unsigned)p.points << 32 | (unsigned)p.tokens);
+        h = fnv(h, (unsigned long long)(unsigned)p.index[0] << 40 ^ (unsigned long long)(unsigned)p.index[1] << 20 ^ (unsigned)p.index[2]);
+      }
+      return h;
+  }
+  return h;
+}
+
 // One mloam_frame* call as frame_call hands it on.  have: the previous frame's look-ahead made the sweep's features, in half `parity`;
 // else they are extracted now into that half.  take_undist: they are complete although the undistortion is on (the look-ahead ran it
 // with the poses of mloam_frame_set_next_undistort).  The submaps are on the device.
@@ -349,19 +458,8 @@ void stage_frame_inputs(Ctx *c, const FrameCall &fc) {
   if (f.outlier_on) stage_outlier(c);
   if (f.undist_on) stage_undistort(c, fc.parity, undist_ahead(c));
   if (f.gf_float_on) stage_gf_float(c);
-  // PCD sweeps: the bodies' byte sizes (and staging offsets) change from file to file; the captured decode reads them at execution time
-  if (fc.sw.pcd && !fc.have) pcd_stage(fc.sw, &c->pinned->pcd_half[fc.parity]);
-  if (c->next.set && c->use_lookahead && !c->prof_on && c->next.sw.pcd) pcd_stage(c->next.sw, &c->pinned->pcd_half[fc.parity ^ 1]);
-}
-
-// Whether sweep sw is the announced sweep a: same caller pointer and sizes; a raw sweep is taken by a raw frame with the same per-LiDAR
-// counts only, a ring-ordered sweep by a ring-ordered frame, and a host frame takes a host announcement.  Messages: the same messages
-// (pointers and shapes) with the same layouts.
-bool same_sweep(const Sweep &a, const Sweep &sw) {
-  const bool same_kind = (sw.raw ? (a.raw && std::memcmp(&a.L, &sw.L, sizeof(RigLayout)) == 0) : !a.raw) && a.msg == sw.msg &&
-                         (!sw.msg || std::memcmp(&a.wire, &sw.wire, sizeof(WireMsgs)) == 0) && a.pcd == sw.pcd &&
-                         (!sw.pcd || std::memcmp(&a.pcdf, &sw.pcdf, sizeof(PcdFiles)) == 0);
-  return a.key == sw.key && a.n == sw.n && a.n_scans == sw.n_scans && same_kind && (a.host || !sw.host);
+  if (!fc.have) pcd_frame_stage(c, fc.sw, fc.parity);  // a sweep the look-ahead made is not read again
+  if (c->next.set && c->use_lookahead && !c->prof_on) pcd_frame_stage(c, c->next.sw, fc.parity ^ 1);
 }
 
 // Whether the look-ahead of the previous frame made the features of sw.  With the undistortion on they are the extraction only, or
@@ -375,30 +473,20 @@ bool frame_has_prefetched(const Ctx *c, const Sweep &sw) {
 }
 
 // extractCloud of sweep sw on c->stream into half `parity` of the feature double buffer (*F), with the LiDARs' first points and, for the
-// rig merge, each LiDAR's feature offsets — everything that reads Ctx::extract_work.  A raw sweep goes through the front end (removeNaN +
-// calTimestamp + projection, Ctx::front) first, which makes the ring-ordered sweep and its ScanInfo on the device; extraction takes them
-// with the raw size n as capacity (no count comes back to the host).
+// rig merge, each LiDAR's feature offsets — everything that reads Ctx::extract_work.  A raw-like sweep's points (sweep_points) go through
+// the front end (removeNaN + calTimestamp + projection, Ctx::front) first, which makes the ring-ordered sweep and its ScanInfo on the
+// device; extraction takes them with the raw size n as capacity (no count comes back to the host).
 int extract_enqueue(Ctx *c, const Sweep &sw, int parity, FrameBufs *F_out) {
   const int n = sw.n, n_scans = sw.n_scans;
   const FrameCfg &cfg = c->cfg;
   FrameBufs F;
   int rc = frame_bufs(c, n, &F, parity, cfg.reg_on ? n_scans : 0);
   if (rc) return rc;
-  const float4 *d_cloud = sw.cloud;
+  const float4 *d_cloud;
+  rc = sweep_points(c, sw, parity, &d_cloud);
+  if (rc) return rc;
   const int *d_scan_start = sw.scan_start, *d_scan_end = sw.scan_end;
-  if (sw.msg) {  // PointCloud2 messages: unpacked into the raw sweep the front end reads
-    MLOAM_CUDA_OK(c, c->wire_out.reserve(sizeof(float4) * ((size_t)n + 1)));
-    rc = wire_unpack_device(c, sw, c->wire_out.as<float4>());
-    if (rc) return rc;
-    d_cloud = c->wire_out.as<float4>();
-  }
-  if (sw.pcd) {  // ASCII PCD bodies: decoded into the raw sweep the front end reads, their sizes staged for half `parity`
-    MLOAM_CUDA_OK(c, c->wire_out.reserve(sizeof(float4) * ((size_t)n + 1)));
-    rc = pcd_decode_half(c, sw, parity, c->wire_out.as<float4>());
-    if (rc) return rc;
-    d_cloud = c->wire_out.as<float4>();
-  }
-  if (sw.raw) {
+  if (sw.raw_like()) {
     const FrontEnd &fe = cfg.front;
     float4 *proj;
     int *ss, *n_proj;
@@ -515,7 +603,7 @@ int registered_enqueue(Ctx *c, const Sweep &sw, int parity, int ran, RegOut *out
   }
   const int less_cap = less_sharp_cap(sw.n, sw.n_scans);
   RegArgs a{};
-  a.sweep = F.reg_sweep, a.n_sweep = sw.n, a.d_n_sweep = sw.raw ? F.reg_meta : nullptr, a.scan_start = F.reg_meta + 16;
+  a.sweep = F.reg_sweep, a.n_sweep = sw.n, a.d_n_sweep = sw.raw_like() ? F.reg_meta : nullptr, a.scan_start = F.reg_meta + 16;
   a.n_parts = c->cfg.n_parts(), a.rings_per_lidar = sw.n_scans / a.n_parts;
   a.to_base = c->cfg.rig_merge() ? 1 : (c->cfg.has_ext ? 2 : 0), a.rig = &ctl->rig[0][0], a.ext = ctl->ext;  // as scan_enqueue copied them
   a.undist = c->cfg.undist_on ? c->undist.as<UndistStage>() + parity : nullptr;  // undistort_stage's configuration of this sweep's half
@@ -618,12 +706,7 @@ int frame_enqueue(Ctx *c, const FrameCall &f, Ctx::FrameOutcome *o) {
     MLOAM_CUDA_OK(c, cudaStreamWaitEvent(c->stream, c->br_ahead.join, 0));
     stamp(c, "look-ahead join");
   }
-  if (sw.pcd) {  // the refusal bits of both halves land with the frame's results (frame_pcd_status reads this sweep's half)
-    unsigned *d_status = pcd_half_status(c);
-    if (!d_status) return MLOAM_E_CUDA;
-    MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->pinned->pcd_half_status, d_status, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
-  }
-  return MLOAM_OK;
+  return pcd_frame_land(c, sw);
 }
 
 // A frame's outcome applied to the context, on the stream, capture and replay paths alike
@@ -635,46 +718,6 @@ void frame_commit(Ctx *c, int parity, const Ctx::FrameOutcome &o) {
   c->last_scan = o.S, c->last_scan_valid = true;
   c->reg_last = o.reg;
   c->gf_float_evaluated = o.gf_evaluated;
-}
-
-// Point the device side of host sweep *sw into B (the points, then room for its ScanInfo) and, with `upload`, copy the sweep there on st.
-// The ScanInfo goes through the pinned rows pin: an async copy from pageable memory would block the host behind the sweep's copy.
-int sweep_to_device(Ctx *c, DevBuf &B, Sweep *sw, bool upload, int (*pin)[MLOAM_MAX_RINGS], cudaStream_t st) {
-  if (sw->msg) {  // each LiDAR's message bytes, at wire_stage_offset
-    const WireMsgs &w = sw->wire;
-    MLOAM_CUDA_OK(c, B.reserve(wire_stage_offset(w, sw->L.n_lidars)));
-    sw->bytes = B.as<unsigned char>();
-    for (int l = 0; upload && l < sw->L.n_lidars; l++)
-      MLOAM_CUDA_OK(c, cudaMemcpyAsync(B.as<unsigned char>() + wire_stage_offset(w, l), w.msg[l].data, (size_t)w.msg[l].height * w.msg[l].row_step,
-                                       cudaMemcpyHostToDevice, st));
-    return MLOAM_OK;
-  }
-  if (sw->pcd) {  // each LiDAR's body at its pcd_stage offset; room for bodies half as large again, so that a replay of other files
-                  // rarely grows the staging (a growth re-captures the frame graphs)
-    PcdStage ps;
-    pcd_stage(*sw, &ps);
-    const int nl = sw->L.n_lidars;
-    const size_t need = (size_t)(ps.off[nl - 1] + ps.size[nl - 1]) + 16;
-    if (need > B.cap) MLOAM_CUDA_OK(c, B.reserve(need + need / 2));
-    sw->bytes = B.as<unsigned char>();
-    for (int l = 0; upload && l < nl; l++)
-      if (ps.size[l]) MLOAM_CUDA_OK(c, cudaMemcpyAsync(B.as<unsigned char>() + ps.off[l], sw->pcdf.body[l].data, (size_t)ps.size[l], cudaMemcpyHostToDevice, st));
-    return MLOAM_OK;
-  }
-  SweepIn D;
-  int rc = sweep_bufs(c, B, sw->n, sw->n_scans, &D);
-  if (rc) return rc;
-  sw->cloud = D.cloud;
-  if (!sw->raw) sw->scan_start = D.scan_start, sw->scan_end = D.scan_end;  // a raw sweep has no ScanInfo: the front end makes it
-  if (!upload) return MLOAM_OK;
-  const int ns = sw->n_scans;
-  if (!sw->raw) {
-    std::memcpy(pin[0], sw->h_scan_start, sizeof(int) * ns), std::memcpy(pin[1], sw->h_scan_end, sizeof(int) * ns);
-    MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.scan_start, pin[0], sizeof(int) * ns, cudaMemcpyHostToDevice, st));
-    MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.scan_end, pin[1], sizeof(int) * ns, cudaMemcpyHostToDevice, st));
-  }
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(D.cloud, sw->key, sizeof(float4) * (size_t)sw->n, cudaMemcpyHostToDevice, st));
-  return MLOAM_OK;
 }
 
 // A sweep announced from HOST memory goes up on br_ahead right away (outside of any capture); the look-ahead branch of the frame
@@ -703,45 +746,45 @@ int count_programmatic_edges(cudaGraph_t g) {
 // Everything a frame graph depends on besides its staged inputs (stage_frame_inputs), hashed whole into the graph cache's key.  What a
 // frame does not use is zero, so two frames share a key exactly when they enqueue the same graph.
 struct FrameKey {
-  const void *sweep[4];  // the sweep on the device (cloud, scan_start, scan_end) and the caller's pointer
+  SweepKey sweep, next;  // the sweep, and the announced one (look-ahead)
   const void *maps[2];   // the submaps of an in-frame rebuild
-  const void *next[4];   // the announced sweep (look-ahead): the caller's pointer, cloud, scan_start, scan_end
   cudaStream_t stream;
   mloam_params_t params;
   double ext[7], lidar_ext[MLOAM_MAX_LIDARS][7];  // the rig's first n_lidars
-  FrontEnd front, next_front;  // kernel arguments of the captured front end of a raw sweep / a raw announced sweep
-  RigLayout L, next_L;
   float cells[2];              // the auto cell edges of an in-frame rebuild: kernel arguments of the captured builds
   // gate: the map-size gate (scan2map_enqueue) is decided on the host at capture: with maps built outside the frame (mloam_map_build*,
   // mloam_submap_assemble, mloam_keyframe_submap) a graph captured while it failed must not be replayed once it passes, and back
-  int n, n_scans, raw, n_surf_map, n_corner_map, rebuild_maps, maps_pending, gate, has_ext, n_lidars, lidar_merge;
+  int raw, n_surf_map, n_corner_map, rebuild_maps, maps_pending, gate, has_ext, n_lidars, lidar_merge;
   // the stages' launches and the look-ahead's split with the undistortion on (their staged values are not part of the key)
   int with_ua, outlier_on, undist_on, undist_n, reg_on, gf_float_on, gf_eval;
   // the look-ahead: which half holds this sweep's features (or that they are extracted now), and the announced next sweep
-  int have, parity, ahead, next_n, next_n_scans, next_host, next_pending, stamp_on;
+  int have, parity, ahead, next_host, next_pending, stamp_on;
 };
-static_assert(sizeof(FrameKey) == 11 * sizeof(void *) + sizeof(mloam_params_t) + sizeof(double) * 7 * (1 + MLOAM_MAX_LIDARS) +
-                                      2 * sizeof(FrontEnd) + 2 * sizeof(RigLayout) + 2 * sizeof(float) + 26 * sizeof(int),
+static_assert(sizeof(SweepKey) == 4 * sizeof(void *) + sizeof(FrontEnd) + sizeof(RigLayout) + 2 * sizeof(int) &&
+                  sizeof(FrameKey) == 2 * sizeof(SweepKey) + 3 * sizeof(void *) + sizeof(mloam_params_t) +
+                                          sizeof(double) * 7 * (1 + MLOAM_MAX_LIDARS) + 2 * sizeof(float) + 22 * sizeof(int),
               "hashed whole in 8-byte words: no padding");
 
 unsigned long long frame_key(Ctx *c, const FrameCall &f) {
   const FrameCfg &cfg = c->cfg;
-  const Sweep &sw = f.sw, &nx = c->next.sw;
   FrameKey k;
   memset(&k, 0, sizeof(k));
-  // a host PCD sweep is copied into the staging whatever the caller's buffer: its pointer is no kernel argument (a dataset replay reads
-  // every file into a new place)
-  k.sweep[0] = sw.cloud, k.sweep[1] = sw.scan_start, k.sweep[2] = sw.scan_end, k.sweep[3] = sw.pcd && sw.host ? nullptr : sw.key;
+  unsigned long long h = 1469598103934665603ull;
+  h = sweep_key(f.sw, cfg.front, false, &k.sweep, h);
+  if (c->next.set && c->use_lookahead) {
+    const Sweep &nx = c->next.sw;
+    h = sweep_key(nx, cfg.front, true, &k.next, h);
+    k.ahead = 1, k.next_host = nx.host, k.next_pending = c->next_pending;
+  }
   k.maps[0] = f.surf_map, k.maps[1] = f.corner_map, k.stream = c->stream;
   memcpy(&k.params, &c->params, sizeof(k.params));
   memcpy(k.ext, cfg.ext, sizeof(k.ext));
   memcpy(k.lidar_ext, cfg.lidar_ext, sizeof(double) * 7 * (size_t)cfg.n_lidars);
-  if (sw.raw) k.front = cfg.front, k.L = sw.L;
   if (f.rebuild_maps && !(c->params.map_cell > 0.f)) {
     k.cells[0] = c->maps[MLOAM_MAP_SURF].auto_cell_pick(c->pinned, MLOAM_MAP_SURF);
     k.cells[1] = c->maps[MLOAM_MAP_CORNER].auto_cell_pick(c->pinned, MLOAM_MAP_CORNER);
   }
-  k.n = sw.n, k.n_scans = sw.n_scans, k.raw = sw.raw, k.n_surf_map = f.n_surf_map, k.n_corner_map = f.n_corner_map;
+  k.raw = f.sw.raw_like(), k.n_surf_map = f.n_surf_map, k.n_corner_map = f.n_corner_map;
   k.rebuild_maps = f.rebuild_maps, k.maps_pending = c->maps_pending;
   const MapStorage &MS = c->maps[MLOAM_MAP_SURF], &MC = c->maps[MLOAM_MAP_CORNER];
   k.gate = !f.rebuild_maps && MS.built && MC.built && MS.m > 50 && MC.m > 10;
@@ -750,41 +793,11 @@ unsigned long long frame_key(Ctx *c, const FrameCall &f) {
   k.undist_on = cfg.undist_on, k.undist_n = cfg.undist_on ? c->undist_n : 0;
   k.gf_float_on = cfg.gf_float_on, k.gf_eval = cfg.gf_float_on && c->gf_float_eval;  // an evaluation frame's extra launch
   k.have = f.have, k.parity = f.parity, k.stamp_on = c->stamp_on;
-  if (c->next.set && c->use_lookahead) {
-    k.next[0] = nx.pcd && nx.host ? nullptr : nx.key, k.next[1] = nx.cloud, k.next[2] = nx.scan_start, k.next[3] = nx.scan_end;
-    k.ahead = 1, k.next_n = nx.n, k.next_n_scans = nx.n_scans, k.next_host = nx.host, k.next_pending = c->next_pending;
-    if (nx.raw) k.next_front = cfg.front, k.next_L = nx.L;
-  }
-  unsigned long long h = 1469598103934665603ull, w;  // FNV-1a over 8-byte words: the key is built on the frame's host critical path
-  for (size_t i = 0; i < sizeof(k); i += 8) memcpy(&w, reinterpret_cast<const char *>(&k) + i, 8), h = (h ^ w) * 1099511628211ull;
+  h = fnv_words(h, &k, sizeof(k));
   // the undistortion in the look-ahead branch, and a call that takes a sweep undistorted there (mloam_frame_set_next_undistort): one
   // more word, only when either is on, so that the keys of a context that never announces poses are the ones it had without them
-  w = (undist_ahead(c) ? 1ull : 0ull) | (f.take_undist ? 2ull : 0ull);
-  if (w) h = (h ^ w) * 1099511628211ull;
-  // message sweeps: their messages, layouts and staging are kernel arguments of the captured unpack — hashed only for them, so that a
-  // context that never takes a message keeps the keys it had without them
-  auto hash_wire = [&](const Sweep &x, unsigned long long tag) {
-    h = (h ^ tag) * 1099511628211ull;
-    h = (h ^ (unsigned long long)reinterpret_cast<uintptr_t>(x.bytes)) * 1099511628211ull;
-    for (size_t i = 0; i < sizeof(WireMsgs); i += 8) memcpy(&w, reinterpret_cast<const char *>(&x.wire) + i, 8), h = (h ^ w) * 1099511628211ull;
-  };
-  if (sw.msg) hash_wire(sw, 4ull);
-  if (c->next.set && c->use_lookahead && nx.msg) hash_wire(nx, 8ull);
-  // PCD sweeps: the decode's kernel arguments — the staging or the device bodies, POINTS, tokens and token indices — but not the byte
-  // sizes, which are staged (stage_frame_inputs), so that files of other sizes replay the same graph
-  auto hash_pcd = [&](const Sweep &x, unsigned long long tag) {
-    h = (h ^ tag) * 1099511628211ull;
-    h = (h ^ (unsigned long long)reinterpret_cast<uintptr_t>(x.host ? x.bytes : nullptr)) * 1099511628211ull;
-    for (int l = 0; l < x.L.n_lidars; l++) {
-      const mloam_pcd_t &p = x.pcdf.body[l];
-      h = (h ^ (unsigned long long)reinterpret_cast<uintptr_t>(x.host ? nullptr : p.data)) * 1099511628211ull;
-      h = (h ^ ((unsigned long long)(unsigned)p.points << 32 | (unsigned)p.tokens)) * 1099511628211ull;
-      h = (h ^ ((unsigned long long)(unsigned)p.index[0] << 40 ^ (unsigned long long)(unsigned)p.index[1] << 20 ^ (unsigned)p.index[2])) * 1099511628211ull;
-    }
-  };
-  if (sw.pcd) hash_pcd(sw, 16ull);
-  if (c->next.set && c->use_lookahead && nx.pcd) hash_pcd(nx, 32ull);
-  return h;
+  const unsigned long long w = (undist_ahead(c) ? 1ull : 0ull) | (f.take_undist ? 2ull : 0ull);
+  return w ? fnv(h, w) : h;
 }
 
 // The single-GPU stages at frame time: their setters refuse a multi-GPU context (multi_gpu), and this refuses a communicator attached
@@ -806,17 +819,15 @@ int frame_single_gpu(Ctx *c, bool raw) {
 // inputs — it is captured once per frame_key into a CUDA graph and replayed: the first call with a new key runs on the stream (and
 // performs every allocation), the second captures + instantiates, later ones replay.  Profiling, multi-GPU (NCCL on the stream) and
 // max_inner > 1 (the host polls the LM done flag) use the plain stream path.
-// A PCD sweep's refusal bits, landed by the frame: the call returns MLOAM_E_INVALID and commits nothing (the look-ahead's features are
-// dropped; the next frame extracts its sweep again).  Waits for the stream, which the frame's read-back does anyway.
-int frame_pcd_status(Ctx *c, const FrameCall &f, double *pose_out7, mloam_solve_stats_t *stats) {
-  if (!f.sw.pcd) return MLOAM_OK;
-  MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
-  const unsigned bits = c->pinned->pcd_half_status[f.parity];
-  if (!bits) return MLOAM_OK;
+// A sweep the device refused (pcd_frame_refusal): the call returns its error and commits nothing (the look-ahead's features are dropped;
+// the next frame extracts its sweep again)
+int frame_refused(Ctx *c, const FrameCall &f, double *pose_out7, mloam_solve_stats_t *stats) {
+  const int rc = pcd_frame_refusal(c, f.sw, f.parity);
+  if (rc == MLOAM_OK) return rc;
   c->prefetched.valid = false;
   for (int k = 0; k < 7; k++) pose_out7[k] = f.pose_init7[k];
   if (stats) memset(stats, 0, sizeof(*stats));
-  return pcd_refusal(c, bits);
+  return rc;
 }
 
 int frame_run(Ctx *c, const FrameCall &f, double *pose_out7, mloam_solve_stats_t *stats) {
@@ -867,7 +878,7 @@ int frame_run(Ctx *c, const FrameCall &f, double *pose_out7, mloam_solve_stats_t
       MLOAM_CUDA_OK(c, cudaGraphLaunch(e->exec, c->stream));
       c->frame_from_graph = true;
       c->launches += e->launches;
-      rc = frame_pcd_status(c, f, pose_out7, stats);
+      rc = frame_refused(c, f, pose_out7, stats);
       if (rc) return rc;
       frame_commit(c, f.parity, e->out);
       return scan2map_finish(c, e->out.S, f.pose_init7, want_cov, e->out.ran, pose_out7, stats);
@@ -878,11 +889,13 @@ int frame_run(Ctx *c, const FrameCall &f, double *pose_out7, mloam_solve_stats_t
     c->prefetched.valid = false;  // half f.parity may be partly overwritten
     return rc;
   }
-  rc = frame_pcd_status(c, f, pose_out7, stats);
+  rc = frame_refused(c, f, pose_out7, stats);
   if (rc) return rc;
   frame_commit(c, f.parity, o);
   return scan2map_finish(c, o.S, f.pose_init7, want_cov, o.ran, pose_out7, stats);
 }
+
+// ---- one constructor per kind, with the checks of every entry point that takes that kind (raw-like: in this order, rig_sweep's last)
 
 // A ring-ordered sweep (cloud + ScanInfo, in host or in device memory)
 Sweep ring_sweep(const mloam_point_t *cloud, bool host, int n, const int *scan_start, const int *scan_end, int n_scans) {
@@ -893,13 +906,9 @@ Sweep ring_sweep(const mloam_point_t *cloud, bool host, int n, const int *scan_s
   return sw;
 }
 
-// The rig's raw sweeps at `raw` (host or device memory; h_counts[l] points of LiDAR l, n_lidars of mloam_set_lidars) after the checks every
-// raw entry point makes
-int raw_sweep(Ctx *c, const mloam_point_t *raw, bool host, const int *h_counts, Sweep *sw) {
-  if (!c->cfg.front_set) return fail(c, MLOAM_E_STATE, "frame_raw: call mloam_set_front_end first");
-  const int rc = frame_single_gpu(c, true);
-  if (rc) return rc;
-  if (!h_counts) return MLOAM_E_INVALID;
+// A raw-like sweep of kind `kind` at key (host or device memory) whose LiDAR l has counts[l] points (n_lidars of mloam_set_lidars): the
+// checks every raw-like sweep makes last, and its layout
+int rig_sweep(Ctx *c, SweepKind kind, const void *key, bool host, const int *counts, Sweep *sw) {
   const FrontEnd &fe = c->cfg.front;
   if (c->params.max_ring_points > 0 && c->params.max_ring_points < fe.horizon_scans)
     return fail(c, MLOAM_E_INVALID, "frame_raw: params.max_ring_points is below horizon_scans (a projected ring holds up to horizon_scans points)");
@@ -908,20 +917,29 @@ int raw_sweep(Ctx *c, const mloam_point_t *raw, bool host, const int *h_counts, 
   L.n_lidars = c->cfg.n_lidars;
   long long total = 0;
   for (int l = 0; l < L.n_lidars; l++) {
-    if (h_counts[l] <= 0)  // the driver node's empty_check (rosNodeRVOxford.cpp:216-220)
+    if (counts[l] <= 0)  // the driver node's empty_check (rosNodeRVOxford.cpp:216-220)
       return fail(c, MLOAM_E_INVALID, "frame_raw: every LiDAR of the rig needs a non-empty sweep");
     L.off[l] = (int)total;
-    total += h_counts[l];
+    total += counts[l];
     if (total > (1 << 30)) return fail(c, MLOAM_E_INVALID, "frame_raw: sweeps too large");
   }
   L.off[L.n_lidars] = (int)total;
-  sw->key = raw, sw->host = host, sw->raw = true, sw->n = (int)total, sw->n_scans = L.n_lidars * fe.vertical_scans;
-  if (!host) sw->cloud = reinterpret_cast<const float4 *>(raw);
+  sw->kind = kind, sw->key = key, sw->host = host, sw->n = (int)total, sw->n_scans = L.n_lidars * fe.vertical_scans;
   return MLOAM_OK;
 }
 
-// The rig's PointCloud2 messages msgs (n_lidars of mloam_set_lidars; data in host or device memory) after the checks every message entry
-// point makes: a raw sweep whose points the unpack launch writes
+// The rig's raw sweeps at `raw` (host or device memory; h_counts[l] points of LiDAR l)
+int raw_sweep(Ctx *c, const mloam_point_t *raw, bool host, const int *h_counts, Sweep *sw) {
+  if (!c->cfg.front_set) return fail(c, MLOAM_E_STATE, "frame_raw: call mloam_set_front_end first");
+  int rc = frame_single_gpu(c, true);
+  if (rc) return rc;
+  if (!h_counts) return MLOAM_E_INVALID;
+  rc = rig_sweep(c, SweepKind::raw, raw, host, h_counts, sw);
+  if (rc == MLOAM_OK && !host) sw->cloud = reinterpret_cast<const float4 *>(raw);
+  return rc;
+}
+
+// The rig's PointCloud2 messages msgs (data in host or device memory): a raw sweep whose points the unpack launch writes
 int msg_sweep(Ctx *c, const mloam_pc2_msg_t *msgs, bool host, Sweep *sw) {
   const FrameCfg &cfg = c->cfg;
   if (!cfg.front_set) return fail(c, MLOAM_E_STATE, "frame_msg: call mloam_set_front_end first");
@@ -934,7 +952,7 @@ int msg_sweep(Ctx *c, const mloam_pc2_msg_t *msgs, bool host, Sweep *sw) {
   if (cfg.front.time_field)
     for (int l = 0; l < cfg.n_lidars; l++)
       if (!cfg.layouts[l].datatype[3]) return fail(c, MLOAM_E_INVALID, "frame_msg: time_field 1 needs the timestamp field as lane 3 of every layout");
-  std::vector<int> counts(cfg.n_lidars);
+  int counts[MLOAM_MAX_LIDARS];
   for (int l = 0; l < cfg.n_lidars; l++) {
     const mloam_pc2_msg_t &m = msgs[l];
     const mloam_pc2_layout_t &F = cfg.layouts[l];
@@ -947,15 +965,13 @@ int msg_sweep(Ctx *c, const mloam_pc2_msg_t *msgs, bool host, Sweep *sw) {
       return fail(c, MLOAM_E_INVALID, "frame_msg: a message is shorter than height x row_step");
     counts[l] = m.width * m.height;
   }
-  rc = raw_sweep(c, nullptr, host, counts.data(), sw);
+  rc = rig_sweep(c, SweepKind::msg, msgs[0].data, host, counts, sw);
   if (rc) return rc;
-  sw->key = msgs[0].data, sw->cloud = nullptr, sw->msg = true;
   for (int l = 0; l < cfg.n_lidars; l++) sw->wire.msg[l] = msgs[l], sw->wire.layout[l] = cfg.layouts[l];
   return MLOAM_OK;
 }
 
-// The rig's ASCII PCD bodies pcds (n_lidars of mloam_set_lidars; data in host or device memory) after the checks every PCD entry point
-// makes: a raw sweep of POINTS points per LiDAR, which the decode writes
+// The rig's ASCII PCD bodies pcds (data in host or device memory): a raw sweep of POINTS points per LiDAR, which the decode writes
 int pcd_sweep(Ctx *c, const mloam_pcd_t *pcds, bool host, Sweep *sw) {
   const FrameCfg &cfg = c->cfg;
   if (!cfg.front_set) return fail(c, MLOAM_E_STATE, "frame_pcd: call mloam_set_front_end first");
@@ -965,11 +981,10 @@ int pcd_sweep(Ctx *c, const mloam_pcd_t *pcds, bool host, Sweep *sw) {
   if (cfg.front.time_field) return fail(c, MLOAM_E_INVALID, "frame_pcd: a PointXYZ cloud has no timestamp field (time_field 1)");
   rc = pcd_check(c, cfg.n_lidars, pcds);
   if (rc) return rc;
-  std::vector<int> counts(cfg.n_lidars);
+  int counts[MLOAM_MAX_LIDARS];
   for (int l = 0; l < cfg.n_lidars; l++) counts[l] = pcds[l].points;
-  rc = raw_sweep(c, nullptr, host, counts.data(), sw);
+  rc = rig_sweep(c, SweepKind::pcd, pcds[0].data, host, counts, sw);
   if (rc) return rc;
-  sw->key = pcds[0].data, sw->cloud = nullptr, sw->pcd = true;
   for (int l = 0; l < cfg.n_lidars; l++) sw->pcdf.body[l] = pcds[l];
   return MLOAM_OK;
 }
@@ -990,11 +1005,12 @@ int upload_submaps(Ctx *c, const mloam_point_t *h_surf_map, int n_surf_map, cons
   return MLOAM_OK;
 }
 
-// What every mloam_frame* entry point does with its sweep sw and submaps (host buffers for a host sweep, device buffers otherwise): the
-// sweep — unless the look-ahead made its features —, the announced next sweep and the submaps go up, the frame runs, and the call
-// consumes the announcement and the uploads.
-int frame_call(Ctx *c, Sweep sw, const mloam_point_t *surf_map, int n_surf_map, const mloam_point_t *corner_map, int n_corner_map,
-               int rebuild_maps, const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
+// What every mloam_frame* entry point does after its checks and the constructor that made its sweep sw (rc; evaluated with the
+// arguments, before sw is read), with sw and the submaps (host buffers for a host sweep, device buffers otherwise): the sweep — unless the look-ahead made its features —, the announced next sweep and the
+// submaps go up, the frame runs, and the call consumes the announcement and the uploads.
+int frame_call(Ctx *c, int rc, const Sweep &sw, const mloam_point_t *surf_map, int n_surf_map, const mloam_point_t *corner_map,
+               int n_corner_map, int rebuild_maps, const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
+  if (rc) return rc;
   c->reg_valid = false;
   if (sw.host && rebuild_maps && (!surf_map || !corner_map || n_surf_map < 0 || n_corner_map < 0)) return MLOAM_E_INVALID;
   // the poses announced with this sweep (mloam_frame_set_next_undistort), consumed by this call whatever it returns
@@ -1017,7 +1033,7 @@ int frame_call(Ctx *c, Sweep sw, const mloam_point_t *surf_map, int n_surf_map, 
   f.parity = f.have ? c->prefetched.parity : c->frame_parity;
   f.take_undist = f.have && c->cfg.undist_on && !c->prefetched.extract_only;
   if (!sw.host) f.surf_map = reinterpret_cast<const float4 *>(surf_map), f.corner_map = reinterpret_cast<const float4 *>(corner_map);
-  int rc = sw.host ? sweep_to_device(c, c->sweep_in, &f.sw, !f.have, c->pinned->scan_info, c->stream) : MLOAM_OK;
+  rc = sw.host ? sweep_to_device(c, c->sweep_in, &f.sw, !f.have, c->pinned->scan_info, c->stream) : MLOAM_OK;
   if (rc == MLOAM_OK) rc = stage_next_sweep(c);
   if (rc == MLOAM_OK && sw.host && rebuild_maps) rc = upload_submaps(c, surf_map, n_surf_map, corner_map, n_corner_map, &f.surf_map, &f.corner_map);
   if (rc == MLOAM_OK) rc = frame_run(c, f, pose_out7, stats);
@@ -1029,12 +1045,59 @@ int frame_call(Ctx *c, Sweep sw, const mloam_point_t *surf_map, int n_surf_map, 
   return rc;
 }
 
-// What every mloam_frame_set_next* call does after its checks (rc): the previous announcement is withdrawn, and sw — unless the checks
-// failed or sw is empty (a withdrawal) — is announced for the next frame
-int announce(Ctx *c, const Sweep &sw, int rc) {
+// What every mloam_frame_set_next* call does after its checks and its sweep's constructor (rc): the previous announcement is withdrawn,
+// and sw — unless the checks failed or sw is empty (a withdrawal) — is announced for the next frame
+int announce(Ctx *c, int rc, const Sweep &sw) {
   c->next = Ctx::NextSweep{};
   if (rc == MLOAM_OK && sw.key) c->next.set = true, c->next.sw = sw, c->next.undist_open = true;
   return rc;
+}
+
+// The front end alone (mloam_front_end*) of host sweep sw after the constructor that made it (rc, as frame_call's): its raw points on the device, then the projection
+// into front_out and the read-back of the ring-ordered sweep and its ScanInfo
+int front_end_call(Ctx *c, int rc, const Sweep &made, mloam_point_t *h_out, int *n_out, int *h_scan_start, int *h_scan_end) {
+  *n_out = 0;
+  if (rc) return rc;
+  Sweep sw = made;  // a message sweep's staging is set below
+  cudaSetDevice(c->device);
+  const int n = sw.n, n_scans = sw.n_scans;
+  cudaStream_t st = c->stream;
+  c->prefetched.valid = false;  // the front end's output buffer is the frame's
+  const float4 *d_raw = nullptr;
+  switch (sw.kind) {
+    case SweepKind::ring: return MLOAM_E_INVALID;  // the constructors of the front end make raw-like sweeps only
+    case SweepKind::raw:
+      MLOAM_CUDA_OK(c, c->sweep_in.reserve(sizeof(float4) * (size_t)n));
+      MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->sweep_in.p, sw.key, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, st));
+      d_raw = c->sweep_in.as<float4>();
+      break;
+    case SweepKind::msg:  // staged in sweep_in and unpacked into wire_out, as in a frame
+      rc = sweep_to_device(c, c->sweep_in, &sw, true, nullptr, st);
+      if (rc == MLOAM_OK) rc = sweep_points(c, sw, 0, &d_raw);
+      break;
+    case SweepKind::pcd:  // decoded into wire_out by pcd_decode_device, which waits and refuses a malformed body before the projection
+      MLOAM_CUDA_OK(c, c->wire_out.reserve(sizeof(float4) * ((size_t)n + 1)));
+      rc = pcd_decode_device(c, sw.L.n_lidars, sw.pcdf.body, true, c->wire_out.as<float4>());
+      d_raw = c->wire_out.as<float4>();
+      break;
+  }
+  if (rc) return rc;
+  float4 *d_out;
+  int *d_meta;  // [0] count, then scan starts, scan ends
+  MLOAM_CUDA_OK(c, carve(c->front_out, [&](Carve &cv) { d_out = cv.take<float4>((size_t)n + 1), d_meta = cv.take<int>(4 + 2 * (size_t)n_scans); }));
+  const FrontEnd &fe = c->cfg.front;
+  rc = project_cloud_device(c, d_raw, sw.L, fe.vertical_scans, fe.horizon_scans, fe.roi_range, &fe, d_out, d_meta + 4, d_meta + 4 + n_scans,
+                            d_meta, c->front_work);
+  if (rc) return rc;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_start, d_meta + 4, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_end, d_meta + 4 + n_scans, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
+  int *hc = c->pinned->counts;
+  MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_meta, sizeof(int), cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  *n_out = hc[0];
+  if (hc[0] > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_out, d_out, sizeof(float4) * (size_t)hc[0], cudaMemcpyDeviceToHost, st));
+  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
+  return MLOAM_OK;
 }
 
 }  // namespace
@@ -1222,8 +1285,8 @@ int mloam_frame_device(mloam_ctx_t *h, const mloam_point_t *d_cloud, int n, cons
                        const mloam_point_t *d_surf_map, int n_surf_map, const mloam_point_t *d_corner_map, int n_corner_map,
                        int rebuild_maps, const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
   if (!h || !pose_init7 || !pose_out7 || n <= 0 || !d_cloud || !d_scan_start || !d_scan_end) return MLOAM_E_INVALID;
-  return frame_call(&h->c, ring_sweep(d_cloud, false, n, d_scan_start, d_scan_end, n_scans), d_surf_map, n_surf_map, d_corner_map,
-                    n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+  return frame_call(&h->c, MLOAM_OK, ring_sweep(d_cloud, false, n, d_scan_start, d_scan_end, n_scans), d_surf_map, n_surf_map,
+                    d_corner_map, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
 }
 
 // Look-ahead: announce the sweep of the NEXT mloam_frame* call.  While the coming frame is matched and solved, that sweep is extracted
@@ -1232,15 +1295,15 @@ int mloam_frame_device(mloam_ctx_t *h, const mloam_point_t *d_cloud, int n, cons
 // consumed by one frame; results are identical with or without it.
 int mloam_frame_set_next_device(mloam_ctx_t *h, const mloam_point_t *d_cloud, int n, const int *d_scan_start, const int *d_scan_end, int n_scans) {
   if (!h) return MLOAM_E_INVALID;
-  if (!d_cloud || n <= 0) return announce(&h->c, Sweep{}, MLOAM_OK);  // withdraw
+  if (!d_cloud || n <= 0) return announce(&h->c, MLOAM_OK, Sweep{});  // withdraw
   const int rc = (!d_scan_start || !d_scan_end || n_scans <= 0 || n_scans > MLOAM_MAX_RINGS) ? MLOAM_E_INVALID : MLOAM_OK;
-  return announce(&h->c, ring_sweep(d_cloud, false, n, d_scan_start, d_scan_end, n_scans), rc);
+  return announce(&h->c, rc, ring_sweep(d_cloud, false, n, d_scan_start, d_scan_end, n_scans));
 }
 int mloam_frame_set_next(mloam_ctx_t *h, const mloam_point_t *h_cloud, int n, const int *h_scan_start, const int *h_scan_end, int n_scans) {
   if (!h) return MLOAM_E_INVALID;
-  if (!h_cloud || n <= 0) return announce(&h->c, Sweep{}, MLOAM_OK);  // withdraw
+  if (!h_cloud || n <= 0) return announce(&h->c, MLOAM_OK, Sweep{});  // withdraw
   const int rc = (!h_scan_start || !h_scan_end || n_scans <= 0 || n_scans > MLOAM_MAX_RINGS) ? MLOAM_E_INVALID : MLOAM_OK;
-  return announce(&h->c, ring_sweep(h_cloud, true, n, h_scan_start, h_scan_end, n_scans), rc);
+  return announce(&h->c, rc, ring_sweep(h_cloud, true, n, h_scan_start, h_scan_end, n_scans));
 }
 
 int mloam_frame(mloam_ctx_t *h, const mloam_point_t *h_cloud, int n, const int *h_scan_start, const int *h_scan_end, int n_scans,
@@ -1248,8 +1311,8 @@ int mloam_frame(mloam_ctx_t *h, const mloam_point_t *h_cloud, int n, const int *
                 const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
   if (!h || !pose_init7 || !pose_out7 || n <= 0 || !h_cloud || !h_scan_start || !h_scan_end || n_scans <= 0 || n_scans > MLOAM_MAX_RINGS)
     return MLOAM_E_INVALID;
-  return frame_call(&h->c, ring_sweep(h_cloud, true, n, h_scan_start, h_scan_end, n_scans), h_surf_map, n_surf_map, h_corner_map,
-                    n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+  return frame_call(&h->c, MLOAM_OK, ring_sweep(h_cloud, true, n, h_scan_start, h_scan_end, n_scans), h_surf_map, n_surf_map,
+                    h_corner_map, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
 }
 
 // ------------------------------------------------------------------------------------------ raw driver sweeps
@@ -1297,34 +1360,9 @@ int mloam_set_front_end(mloam_ctx_t *h, int vertical_scans, int horizon_scans, d
 
 int mloam_front_end(mloam_ctx_t *h, const mloam_point_t *h_raw, const int *h_counts, mloam_point_t *h_out, int *n_out, int *h_scan_start,
                     int *h_scan_end) {
-  if (!h || !h_raw || !h_out || !n_out || !h_scan_start || !h_scan_end) return MLOAM_E_INVALID;
-  Ctx *c = &h->c;
-  *n_out = 0;
+  if (!h || !h_out || !n_out || !h_scan_start || !h_scan_end || !h_raw) return MLOAM_E_INVALID;
   Sweep sw;
-  int rc = raw_sweep(c, h_raw, true, h_counts, &sw);
-  if (rc) return rc;
-  cudaSetDevice(c->device);
-  const int n = sw.n, n_scans = sw.n_scans;
-  c->prefetched.valid = false;  // the front end's output buffer is the frame's
-  MLOAM_CUDA_OK(c, c->sweep_in.reserve(sizeof(float4) * (size_t)n));
-  float4 *d_out;
-  int *d_meta;  // [0] count, then scan starts, scan ends
-  MLOAM_CUDA_OK(c, carve(c->front_out, [&](Carve &cv) { d_out = cv.take<float4>((size_t)n + 1), d_meta = cv.take<int>(4 + 2 * (size_t)n_scans); }));
-  cudaStream_t st = c->stream;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(c->sweep_in.p, h_raw, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, st));
-  const FrontEnd &fe = c->cfg.front;
-  rc = project_cloud_device(c, c->sweep_in.as<float4>(), sw.L, fe.vertical_scans, fe.horizon_scans, fe.roi_range, &fe, d_out, d_meta + 4,
-                            d_meta + 4 + n_scans, d_meta, c->front_work);
-  if (rc) return rc;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_start, d_meta + 4, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_end, d_meta + 4 + n_scans, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
-  int *hc = c->pinned->counts;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_meta, sizeof(int), cudaMemcpyDeviceToHost, st));
-  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
-  *n_out = hc[0];
-  if (hc[0] > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_out, d_out, sizeof(float4) * (size_t)hc[0], cudaMemcpyDeviceToHost, st));
-  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
-  return MLOAM_OK;
+  return front_end_call(&h->c, raw_sweep(&h->c, h_raw, true, h_counts, &sw), sw, h_out, n_out, h_scan_start, h_scan_end);
 }
 
 int mloam_frame_raw(mloam_ctx_t *h, const mloam_point_t *h_raw, const int *h_counts, const mloam_point_t *h_surf_map, int n_surf_map,
@@ -1332,9 +1370,8 @@ int mloam_frame_raw(mloam_ctx_t *h, const mloam_point_t *h_raw, const int *h_cou
                     mloam_solve_stats_t *stats) {
   if (!h || !pose_init7 || !pose_out7 || !h_raw) return MLOAM_E_INVALID;
   Sweep sw;
-  const int rc = raw_sweep(&h->c, h_raw, true, h_counts, &sw);
-  if (rc) return rc;
-  return frame_call(&h->c, sw, h_surf_map, n_surf_map, h_corner_map, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+  return frame_call(&h->c, raw_sweep(&h->c, h_raw, true, h_counts, &sw), sw, h_surf_map, n_surf_map, h_corner_map, n_corner_map,
+                    rebuild_maps, pose_init7, pose_out7, stats);
 }
 
 int mloam_frame_raw_device(mloam_ctx_t *h, const mloam_point_t *d_raw, const int *h_counts, const mloam_point_t *d_surf_map, int n_surf_map,
@@ -1342,9 +1379,8 @@ int mloam_frame_raw_device(mloam_ctx_t *h, const mloam_point_t *d_raw, const int
                            mloam_solve_stats_t *stats) {
   if (!h || !pose_init7 || !pose_out7 || !d_raw) return MLOAM_E_INVALID;
   Sweep sw;
-  const int rc = raw_sweep(&h->c, d_raw, false, h_counts, &sw);
-  if (rc) return rc;
-  return frame_call(&h->c, sw, d_surf_map, n_surf_map, d_corner_map, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+  return frame_call(&h->c, raw_sweep(&h->c, d_raw, false, h_counts, &sw), sw, d_surf_map, n_surf_map, d_corner_map, n_corner_map,
+                    rebuild_maps, pose_init7, pose_out7, stats);
 }
 
 // Look-ahead for raw frames: as mloam_frame_set_next*, picked up by the next mloam_frame_raw* call with the same pointer and counts
@@ -1352,13 +1388,13 @@ int mloam_frame_set_next_raw(mloam_ctx_t *h, const mloam_point_t *h_raw, const i
   if (!h) return MLOAM_E_INVALID;
   Sweep sw;
   const int rc = h_raw ? raw_sweep(&h->c, h_raw, true, h_counts, &sw) : MLOAM_OK;  // nullptr: withdraw
-  return announce(&h->c, sw, rc);
+  return announce(&h->c, rc, sw);
 }
 int mloam_frame_set_next_raw_device(mloam_ctx_t *h, const mloam_point_t *d_raw, const int *h_counts) {
   if (!h) return MLOAM_E_INVALID;
   Sweep sw;
   const int rc = d_raw ? raw_sweep(&h->c, d_raw, false, h_counts, &sw) : MLOAM_OK;  // nullptr: withdraw
-  return announce(&h->c, sw, rc);
+  return announce(&h->c, rc, sw);
 }
 
 // ------------------------------------------------------------------------------------------ PointCloud2 messages
@@ -1388,69 +1424,15 @@ int mloam_set_front_end_layout(mloam_ctx_t *h, int n_lidars, const mloam_pc2_lay
 
 int mloam_front_end_msg(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs, mloam_point_t *h_out, int *n_out, int *h_scan_start, int *h_scan_end) {
   if (!h || !h_out || !n_out || !h_scan_start || !h_scan_end) return MLOAM_E_INVALID;
-  Ctx *c = &h->c;
-  *n_out = 0;
   Sweep sw;
-  int rc = msg_sweep(c, msgs, true, &sw);
-  if (rc) return rc;
-  cudaSetDevice(c->device);
-  const int n = sw.n, n_scans = sw.n_scans;
-  c->prefetched.valid = false;  // the front end's output buffer is the frame's
-  rc = sweep_to_device(c, c->sweep_in, &sw, true, nullptr, c->stream);
-  if (rc) return rc;
-  MLOAM_CUDA_OK(c, c->wire_out.reserve(sizeof(float4) * ((size_t)n + 1)));
-  rc = wire_unpack_device(c, sw, c->wire_out.as<float4>());
-  if (rc) return rc;
-  float4 *d_out;
-  int *d_meta;  // [0] count, then scan starts, scan ends
-  MLOAM_CUDA_OK(c, carve(c->front_out, [&](Carve &cv) { d_out = cv.take<float4>((size_t)n + 1), d_meta = cv.take<int>(4 + 2 * (size_t)n_scans); }));
-  cudaStream_t st = c->stream;
-  const FrontEnd &fe = c->cfg.front;
-  rc = project_cloud_device(c, c->wire_out.as<float4>(), sw.L, fe.vertical_scans, fe.horizon_scans, fe.roi_range, &fe, d_out, d_meta + 4,
-                            d_meta + 4 + n_scans, d_meta, c->front_work);
-  if (rc) return rc;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_start, d_meta + 4, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_end, d_meta + 4 + n_scans, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
-  int *hc = c->pinned->counts;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_meta, sizeof(int), cudaMemcpyDeviceToHost, st));
-  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
-  *n_out = hc[0];
-  if (hc[0] > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_out, d_out, sizeof(float4) * (size_t)hc[0], cudaMemcpyDeviceToHost, st));
-  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
-  return MLOAM_OK;
+  return front_end_call(&h->c, msg_sweep(&h->c, msgs, true, &sw), sw, h_out, n_out, h_scan_start, h_scan_end);
 }
 
 // The decode of the rig's ASCII PCD bodies (pcd.cu), then the raw front end, as mloam_front_end_msg
 int mloam_front_end_pcd(mloam_ctx_t *h, const mloam_pcd_t *pcds, mloam_point_t *h_out, int *n_out, int *h_scan_start, int *h_scan_end) {
   if (!h || !h_out || !n_out || !h_scan_start || !h_scan_end) return MLOAM_E_INVALID;
-  Ctx *c = &h->c;
-  *n_out = 0;
   Sweep sw;
-  int rc = pcd_sweep(c, pcds, true, &sw);
-  if (rc) return rc;
-  cudaSetDevice(c->device);
-  const int n = sw.n, n_scans = sw.n_scans;
-  c->prefetched.valid = false;  // the front end's output buffer is the frame's
-  MLOAM_CUDA_OK(c, c->wire_out.reserve(sizeof(float4) * ((size_t)n + 1)));
-  rc = pcd_decode_device(c, sw.L.n_lidars, pcds, true, c->wire_out.as<float4>());
-  if (rc) return rc;
-  float4 *d_out;
-  int *d_meta;  // [0] count, then scan starts, scan ends
-  MLOAM_CUDA_OK(c, carve(c->front_out, [&](Carve &cv) { d_out = cv.take<float4>((size_t)n + 1), d_meta = cv.take<int>(4 + 2 * (size_t)n_scans); }));
-  cudaStream_t st = c->stream;
-  const FrontEnd &fe = c->cfg.front;
-  rc = project_cloud_device(c, c->wire_out.as<float4>(), sw.L, fe.vertical_scans, fe.horizon_scans, fe.roi_range, &fe, d_out, d_meta + 4,
-                            d_meta + 4 + n_scans, d_meta, c->front_work);
-  if (rc) return rc;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_start, d_meta + 4, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_scan_end, d_meta + 4 + n_scans, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
-  int *hc = c->pinned->counts;
-  MLOAM_CUDA_OK(c, cudaMemcpyAsync(hc, d_meta, sizeof(int), cudaMemcpyDeviceToHost, st));
-  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
-  *n_out = hc[0];
-  if (hc[0] > 0) MLOAM_CUDA_OK(c, cudaMemcpyAsync(h_out, d_out, sizeof(float4) * (size_t)hc[0], cudaMemcpyDeviceToHost, st));
-  MLOAM_CUDA_OK(c, cudaStreamSynchronize(st));
-  return MLOAM_OK;
+  return front_end_call(&h->c, pcd_sweep(&h->c, pcds, true, &sw), sw, h_out, n_out, h_scan_start, h_scan_end);
 }
 
 int mloam_frame_msg(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs, const mloam_point_t *h_surf_map, int n_surf_map,
@@ -1458,9 +1440,8 @@ int mloam_frame_msg(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs, const mloam_poi
                     mloam_solve_stats_t *stats) {
   if (!h || !pose_init7 || !pose_out7) return MLOAM_E_INVALID;
   Sweep sw;
-  const int rc = msg_sweep(&h->c, msgs, true, &sw);
-  if (rc) return rc;
-  return frame_call(&h->c, sw, h_surf_map, n_surf_map, h_corner_map, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+  return frame_call(&h->c, msg_sweep(&h->c, msgs, true, &sw), sw, h_surf_map, n_surf_map, h_corner_map, n_corner_map,
+                    rebuild_maps, pose_init7, pose_out7, stats);
 }
 
 int mloam_frame_msg_device(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs, const mloam_point_t *d_surf_map, int n_surf_map,
@@ -1468,9 +1449,8 @@ int mloam_frame_msg_device(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs, const ml
                            double *pose_out7, mloam_solve_stats_t *stats) {
   if (!h || !pose_init7 || !pose_out7) return MLOAM_E_INVALID;
   Sweep sw;
-  const int rc = msg_sweep(&h->c, msgs, false, &sw);
-  if (rc) return rc;
-  return frame_call(&h->c, sw, d_surf_map, n_surf_map, d_corner_map, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+  return frame_call(&h->c, msg_sweep(&h->c, msgs, false, &sw), sw, d_surf_map, n_surf_map, d_corner_map, n_corner_map,
+                    rebuild_maps, pose_init7, pose_out7, stats);
 }
 
 // Look-ahead for message frames: as mloam_frame_set_next_raw*, picked up by the next mloam_frame_msg* call with the same messages
@@ -1478,13 +1458,13 @@ int mloam_frame_set_next_msg(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs) {
   if (!h) return MLOAM_E_INVALID;
   Sweep sw;
   const int rc = msgs ? msg_sweep(&h->c, msgs, true, &sw) : MLOAM_OK;  // nullptr: withdraw
-  return announce(&h->c, sw, rc);
+  return announce(&h->c, rc, sw);
 }
 int mloam_frame_set_next_msg_device(mloam_ctx_t *h, const mloam_pc2_msg_t *msgs) {
   if (!h) return MLOAM_E_INVALID;
   Sweep sw;
   const int rc = msgs ? msg_sweep(&h->c, msgs, false, &sw) : MLOAM_OK;  // nullptr: withdraw
-  return announce(&h->c, sw, rc);
+  return announce(&h->c, rc, sw);
 }
 
 // PCD frames: as mloam_frame_raw* on the sweep the decode of the rig's bodies gives
@@ -1492,9 +1472,8 @@ int mloam_frame_pcd(mloam_ctx_t *h, const mloam_pcd_t *pcds, const mloam_point_t
                     int n_corner_map, int rebuild_maps, const double *pose_init7, double *pose_out7, mloam_solve_stats_t *stats) {
   if (!h || !pose_init7 || !pose_out7) return MLOAM_E_INVALID;
   Sweep sw;
-  const int rc = pcd_sweep(&h->c, pcds, true, &sw);
-  if (rc) return rc;
-  return frame_call(&h->c, sw, h_surf_map, n_surf_map, h_corner_map, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+  return frame_call(&h->c, pcd_sweep(&h->c, pcds, true, &sw), sw, h_surf_map, n_surf_map, h_corner_map, n_corner_map,
+                    rebuild_maps, pose_init7, pose_out7, stats);
 }
 
 int mloam_frame_pcd_device(mloam_ctx_t *h, const mloam_pcd_t *pcds, const mloam_point_t *d_surf_map, int n_surf_map,
@@ -1502,9 +1481,8 @@ int mloam_frame_pcd_device(mloam_ctx_t *h, const mloam_pcd_t *pcds, const mloam_
                            double *pose_out7, mloam_solve_stats_t *stats) {
   if (!h || !pose_init7 || !pose_out7) return MLOAM_E_INVALID;
   Sweep sw;
-  const int rc = pcd_sweep(&h->c, pcds, false, &sw);
-  if (rc) return rc;
-  return frame_call(&h->c, sw, d_surf_map, n_surf_map, d_corner_map, n_corner_map, rebuild_maps, pose_init7, pose_out7, stats);
+  return frame_call(&h->c, pcd_sweep(&h->c, pcds, false, &sw), sw, d_surf_map, n_surf_map, d_corner_map, n_corner_map,
+                    rebuild_maps, pose_init7, pose_out7, stats);
 }
 
 // Look-ahead for PCD frames: as mloam_frame_set_next_msg*, picked up by the next mloam_frame_pcd* call with the same bodies
@@ -1512,13 +1490,13 @@ int mloam_frame_set_next_pcd(mloam_ctx_t *h, const mloam_pcd_t *pcds) {
   if (!h) return MLOAM_E_INVALID;
   Sweep sw;
   const int rc = pcds ? pcd_sweep(&h->c, pcds, true, &sw) : MLOAM_OK;  // nullptr: withdraw
-  return announce(&h->c, sw, rc);
+  return announce(&h->c, rc, sw);
 }
 int mloam_frame_set_next_pcd_device(mloam_ctx_t *h, const mloam_pcd_t *pcds) {
   if (!h) return MLOAM_E_INVALID;
   Sweep sw;
   const int rc = pcds ? pcd_sweep(&h->c, pcds, false, &sw) : MLOAM_OK;  // nullptr: withdraw
-  return announce(&h->c, sw, rc);
+  return announce(&h->c, rc, sw);
 }
 
 int mloam_set_lidars(mloam_ctx_t *h, int n_lidars, const double *ext7) {

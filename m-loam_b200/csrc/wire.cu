@@ -208,10 +208,21 @@ int cloud_msgs_pack(Ctx *c, int n, const int *sources, int *width, unsigned char
 
 }  // namespace
 
-size_t wire_stage_offset(const WireMsgs &w, int l) {
+// where LiDAR l's bytes lie in a host message sweep's device staging (256-byte aligned), and l = n_lidars: the staging's size
+static size_t wire_stage_offset(const WireMsgs &w, int l) {
   size_t off = 0;
   for (int k = 0; k < l; k++) off += ((size_t)w.msg[k].height * w.msg[k].row_step + 255) & ~(size_t)255;
   return off;
+}
+
+int wire_upload(Ctx *c, DevBuf &B, Sweep *sw, bool upload, cudaStream_t st) {
+  const WireMsgs &w = sw->wire;
+  MLOAM_CUDA_OK(c, B.reserve(wire_stage_offset(w, sw->L.n_lidars)));
+  sw->bytes = B.as<unsigned char>();
+  for (int l = 0; upload && l < sw->L.n_lidars; l++)
+    MLOAM_CUDA_OK(c, cudaMemcpyAsync(B.as<unsigned char>() + wire_stage_offset(w, l), w.msg[l].data, (size_t)w.msg[l].height * w.msg[l].row_step,
+                                     cudaMemcpyHostToDevice, st));
+  return MLOAM_OK;
 }
 
 int wire_unpack_device(Ctx *c, const Sweep &sw, float4 *out) {

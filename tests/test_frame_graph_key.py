@@ -5,9 +5,9 @@ frame's from_graph flag follow the schedule the key implies: a new key runs on t
 later sightings replay.
 
 The script changes, one at a time, settings that re-key (a params field, set_extrinsic, set_lidars values and count, each stage switch,
-the undistortion pose count, a gd_float evaluation frame, the raw front end, rebuild on / off, the map gate with maps built outside the
-frame) and values that are staged and must replay the same graph with the new value (the initial pose, the with_ua covariances and
-threshold, the outlier leaf, the undistortion poses, the gd_float threshold).  A frame's key also holds the half of the feature double
+the undistortion pose count, a gd_float evaluation frame, the raw front end, a message sweep, a PCD sweep and its POINTS, rebuild on /
+off, the map gate with maps built outside the frame) and values that are staged and must replay the same graph with the new value (the initial pose, the with_ua covariances and
+threshold, the outlier leaf, the undistortion poses, the gd_float threshold, the byte sizes of PCD bodies).  A frame's key also holds the half of the feature double
 buffer it extracts into, which alternates from frame to frame, so each setting runs six frames: stream, capture and replay per half."""
 import ctypes as C
 import math
@@ -17,7 +17,9 @@ import numpy as np
 import pytest
 
 import front_end_lib as fel
+import pcd_lib as pl
 import synthetic as syn
+import wire_lib as wl
 
 pytestmark = pytest.mark.gpu
 
@@ -69,13 +71,20 @@ def scene():
     cloud, ss, se = syn.make_sweep(sc, traj[1], RINGS, HORIZON, seed=3)
     rig, rss, rse, _ = syn.make_multi_sweep(sc, traj[1], 2, RINGS, HORIZON, seed=5)
     raw = np.ascontiguousarray(fel.raw_sweep(sc, traj[1], RINGS, HORIZON, seed=7), np.float32)
+    msg = wl.pack(raw, "xyzi32", height=2, row_pad=8)
+
+    def pcd(pts, prec):  # one PointXYZ body: %.9g and %.8g lines of the same points differ in byte size only
+        return [(pl.ascii_body([pts[:, 0], pts[:, 1], pts[:, 2]], prec=prec), pts.shape[0], 3, (0, 1, 2))]
+
     return dict(truth=traj[1], surf_map=surf_map, corner_map=corner_map, ring=(np.ascontiguousarray(cloud, np.float32), ss, se),
-                rig=(np.ascontiguousarray(rig, np.float32), rss, rse), raw=raw)
+                rig=(np.ascontiguousarray(rig, np.float32), rss, rse), raw=raw, msg=[wl.as_arg(msg)], msg_layout=msg,
+                pcd9=pcd(raw, 9), pcd8=pcd(raw, 8), pcd_short=pcd(raw[:-100], 9))
 
 
-def _script(sc):
+def _script(mloam, sc):
     """[(label, settings applied before the block's first frame, settings applied before its fourth, frames, sweep, rebuild)].  A new
-    label is a new key; a repeated label returns to the key the label had."""
+    label is a new key; a repeated label returns to the key the label had.  sweep: one name, or the names of the first three frames
+    and of the rest."""
     tiny_s, tiny_c = sc["surf_map"][:40], sc["corner_map"][:8]
     gf = [("set_params", dict(gf_method=3, gf_ratio=0.5)), ("set_gf_float", True, 1e9)]
     return [
@@ -92,6 +101,10 @@ def _script(sc):
         ("registered", [("set_registered", True)], [], 6, "ring", True),
         ("raw a", [("set_front_end", RINGS, HORIZON, 0.5)], [], 6, "raw", True),
         ("raw b", [("set_front_end", RINGS, HORIZON, 0.8)], [], 6, "raw", True),
+        ("message", [("set_front_end_layout", [wl.layout(mloam, sc["msg_layout"], None)])], [], 6, "msg", True),
+        # the bodies' byte sizes are staged: other files of the same POINTS replay the graph captured with the first ones
+        ("pcd", [], [], 6, ("pcd9", "pcd8"), True),
+        ("pcd points", [], [], 6, "pcd_short", True),
         ("2 lidars a", [("set_lidars", 2, [_ext(5), _ext(6)])], [], 6, "rig", True),
         ("2 lidars b", [("set_lidars", 2, [_ext(5), _ext(7)])], [], 6, "rig", True),
         # maps built outside the frame; the first host build grows the staging the host sweep shares, so it comes before the block
@@ -117,6 +130,10 @@ def _frame(mloam, cx, on, sc, sweep, rebuild, init, k):
     sm, cm = (sc["surf_map"], sc["corner_map"]) if rebuild else (None, None)
     if sweep == "raw":
         pose, st = cx.frame_raw(sc["raw"], [sc["raw"].shape[0]], sm, cm, init, rebuild_maps=rebuild)
+    elif sweep == "msg":
+        pose, st = cx.frame_msg(sc["msg"], sm, cm, init, rebuild_maps=rebuild)
+    elif sweep.startswith("pcd"):
+        pose, st = cx.frame_pcd(sc[sweep], sm, cm, init, rebuild_maps=rebuild)
     else:
         cloud, ss, se = sc[sweep]
         pose, st = cx.frame(cloud, ss, se, sm, cm, init, rebuild_maps=rebuild)
@@ -135,8 +152,9 @@ def test_frame_graph_key_schedule(mloam, scene):
     on = dict(set_distortion=False, set_outlier=False, set_registered=False)  # the stages whose outputs the script reads back
     sightings, parity, gf_frames, k = {}, 0, None, 0
     try:
-        for label, before, middle, n_frames, sweep, rebuild in _script(scene):
+        for label, before, middle, n_frames, sweeps, rebuild in _script(mloam, scene):
             for i in range(n_frames):
+                sweep = sweeps if isinstance(sweeps, str) else sweeps[i >= 3]
                 for s in before if i == 0 else middle if i == 3 else []:
                     for cx in (g, plain):
                         _apply(mloam, cx, s)
