@@ -11,7 +11,7 @@
 //   k_rig_fit        one thread per feature: match_fit.cuh fit_one with CHECK_FOV true
 //   k_rig_linearize  one thread per feature: its 1x6 row on its block; per block 21 + 6 packed sums and a row count, plus the shared
 //                    cost, reduced in a fixed order without atomics (as k_odom_linearize)
-//   k_rig_lm         the k_odom_lm state machine with one trust region over B blocks, on one warp: lane b scales, damps, factors and
+//   k_rig_lm         lm.cuh's state machine with one trust region over B blocks, on one warp: lane b scales, damps, factors and
 //                    solves block b; step norm, x_norm and model cost change are summed across blocks in column order, so that a
 //                    two-LiDAR rig without priors repeats the arithmetic of the coupled 12-dof [pose_i | ext_cal] solve bit for bit
 // then max_inner x (k_rig_linearize + k_rig_lm) at the candidate.  mloam_calib_frame is the two-LiDAR case; with its communicator
@@ -27,6 +27,7 @@
 #include "fit.cuh"
 #include "host_util.h"
 #include "knn.cuh"
+#include "lm.cuh"
 #include "match_fit.cuh"
 
 namespace mloam {
@@ -258,9 +259,6 @@ __device__ double rig_prior(const double *x, const double *x0, double sp, double
 }
 
 // ------------------------------------------------------------------------------------------ LM over B blocks, one lane per block
-__device__ constexpr double kRigMinDiag = 1e-6, kRigMaxDiag = 1e32, kRigMaxRadius = 1e16;
-__device__ constexpr double kRigFuncTol = 1e-6, kRigParamTol = 1e-8, kRigGradTol = 1e-10, kRigMinRel = 1e-3;
-
 // lane 0: sqrt of the sum of squares of the free blocks' parameters, block after block (od_xnorm's order)
 __device__ double rig_xnorm(const RigState *st, const double (*x)[7]) {
   double s = 0;
@@ -281,13 +279,13 @@ __device__ double rig_grad_max(const RigState *st, int lane) {
   return m;
 }
 
-// od_compute_step over the blocks: lane b owns block b; the decision is the warp's.  Returns with st->xc set, or with done.
+// lm.cuh's lm_compute_step over the blocks: lane b owns block b; the decision is the warp's.  Returns with st->xc set, or with done.
 __device__ void rig_compute_step(RigState *st, int lane) {
   const int B = st->B;
   while (true) {
     if (st->iteration >= st->max_inner) {
       __syncwarp();
-      if (lane == 0) st->done = 1, st->termination = 0;
+      if (lane == 0) st->done = 1, st->termination = kTermMaxIterations;
       return;
     }
     bool ok = true;
@@ -299,44 +297,15 @@ __device__ void rig_compute_step(RigState *st, int lane) {
         for (int b = 0; b < 6; b++) Hs[a * 6 + b] = sc[a] * H[a * 6 + b] * sc[b];
       }
       if (!st->reuse_diagonal)
-        for (int j = 0; j < 6; j++) st->diag[lane][j] = fmin(fmax(Hs[j * 6 + j], kRigMinDiag), kRigMaxDiag);
+        for (int j = 0; j < 6; j++) st->diag[lane][j] = lm_diag(Hs[j * 6 + j]);
       for (int i = 0; i < 36; i++) A[i] = Hs[i];
       for (int j = 0; j < 6; j++) {
         const double l = sqrt(st->diag[lane][j] / st->radius);
         A[j * 6 + j] += l * l;
       }
-      // Cholesky + solve of block `lane` (chol_d / chol_solve_d with D = 6)
-      for (int j = 0; j < 6 && ok; j++) {
-        double d = A[j * 6 + j];
-        for (int k = 0; k < j; k++) d -= A[j * 6 + k] * A[j * 6 + k];
-        if (!(d > 0.0)) {
-          ok = false;
-          break;
-        }
-        d = sqrt(d);
-        A[j * 6 + j] = d;
-        for (int i = j + 1; i < 6; i++) {
-          double s = A[i * 6 + j];
-          for (int k = 0; k < j; k++) s -= A[i * 6 + k] * A[j * 6 + k];
-          A[i * 6 + j] = s / d;
-        }
-      }
+      ok = chol<6>(A);
       if (ok) {
-        double y[6];
-#pragma unroll
-        for (int i = 0; i < 6; i++) {
-          double s = gs[i];
-#pragma unroll
-          for (int k = 0; k < i; k++) s -= A[i * 6 + k] * y[k];
-          y[i] = s / A[i * 6 + i];
-        }
-#pragma unroll
-        for (int i = 5; i >= 0; i--) {
-          double s = y[i];
-#pragma unroll
-          for (int k = i + 1; k < 6; k++) s -= A[k * 6 + i] * step[k];
-          step[i] = s / A[i * 6 + i];
-        }
+        chol_solve<6>(A, gs, step);
         for (int j = 0; j < 6; j++) {
           step[j] = -step[j];
           if (!isfinite(step[j])) ok = false;
@@ -370,8 +339,8 @@ __device__ void rig_compute_step(RigState *st, int lane) {
     if (!ok) {
       int stop = 0;
       if (lane == 0) {
-        if (++st->num_invalid >= 5) st->done = 1, st->termination = 4, stop = 1;
-        else st->radius *= 0.5;
+        if (++st->num_invalid >= kMaxInvalidSteps) st->done = 1, st->termination = kTermInvalidSteps, stop = 1;
+        else st->radius = lm_radius_invalid(st->radius);
       }
       if (__shfl_sync(MLOAM_FULL_MASK, stop, 0)) return;
       __syncwarp();
@@ -443,12 +412,12 @@ __global__ void __launch_bounds__(RIG_THREADS) k_rig_lm(const double *__restrict
     if (lane == 0) {
       st->cost = st->initial_cost = cost;
       st->x_norm = rig_xnorm(st, st->x);
-      st->radius = 1e4, st->decrease_factor = 2.0, st->reuse_diagonal = 0;
-      st->iteration = 0, st->num_invalid = 0, st->done = 0, st->termination = 0;
+      st->radius = kInitialRadius, st->decrease_factor = kDecreaseFactor, st->reuse_diagonal = 0;
+      st->iteration = 0, st->num_invalid = 0, st->done = 0, st->termination = kTermMaxIterations;
     }
     __syncwarp();
-    if (rig_grad_max(st, lane) <= kRigGradTol) {
-      if (lane == 0) st->done = 1, st->termination = 3;
+    if (rig_grad_max(st, lane) <= kGradTol) {
+      if (lane == 0) st->done = 1, st->termination = kTermGradientTol;
       return;
     }
     rig_compute_step(st, lane);
@@ -456,7 +425,7 @@ __global__ void __launch_bounds__(RIG_THREADS) k_rig_lm(const double *__restrict
   }
   if (st->done) return;
   const double cost = rig_gather(st, ne, st->xc, cH, cg, lane);
-  int verdict = 0;  // 1 stop, 2 accept, 3 reject
+  int verdict = 0;  // lane 0's lm_verdict, broadcast below
   if (lane == 0) {
     double sn = 0;
     for (int k = 0; k < 7; k++) {
@@ -465,29 +434,23 @@ __global__ void __launch_bounds__(RIG_THREADS) k_rig_lm(const double *__restrict
       sn += t;
     }
     sn = sqrt(sn);
-    const double cost_change = st->cost - cost;
-    const double rel = cost_change / st->model_cost_change;
-    if (sn <= kRigParamTol * (st->x_norm + kRigParamTol)) {
-      st->done = 1, st->termination = 2, verdict = 1;
-    } else if (fabs(cost_change) <= kRigFuncTol * st->cost) {
-      st->done = 1, st->termination = 1, verdict = 1;
-    } else if (rel > kRigMinRel) {
-      const double t = 2.0 * rel - 1.0;
-      st->radius = fmin(kRigMaxRadius, st->radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
-      st->decrease_factor = 2.0;
+    double rel;
+    verdict = lm_verdict(sn, st->x_norm, st->cost, cost, st->model_cost_change, rel);
+    if (verdict >= 0) {
+      st->done = 1, st->termination = verdict;
+    } else if (verdict == kLMAccept) {
+      st->radius = lm_radius_accept(st->radius, rel);
+      st->decrease_factor = kDecreaseFactor;
       st->reuse_diagonal = 0;
       st->cost = cost;
-      verdict = 2;
     } else {
-      st->radius = st->radius / st->decrease_factor;
-      st->decrease_factor *= 2.0;
+      lm_radius_reject(st->radius, st->decrease_factor);
       st->reuse_diagonal = 1;
-      verdict = 3;
     }
   }
   verdict = __shfl_sync(MLOAM_FULL_MASK, verdict, 0);
-  if (verdict == 1) return;
-  if (verdict == 2) {
+  if (verdict >= 0) return;
+  if (verdict == kLMAccept) {
     if (lane < B) {
       for (int k = 0; k < 7; k++) st->x[lane][k] = st->xc[lane][k];
       for (int i = 0; i < 36; i++) st->H[lane][i] = cH[lane][i];
@@ -496,8 +459,8 @@ __global__ void __launch_bounds__(RIG_THREADS) k_rig_lm(const double *__restrict
     __syncwarp();
     if (lane == 0) st->x_norm = rig_xnorm(st, st->x);
     __syncwarp();
-    if (rig_grad_max(st, lane) <= kRigGradTol) {
-      if (lane == 0) st->done = 1, st->termination = 3;
+    if (rig_grad_max(st, lane) <= kGradTol) {
+      if (lane == 0) st->done = 1, st->termination = kTermGradientTol;
       return;
     }
   }

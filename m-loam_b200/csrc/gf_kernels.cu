@@ -23,6 +23,7 @@
 #include "ctx.h"
 #include "factors.cuh"
 #include "host_util.h"
+#include "lm.cuh"
 
 namespace mloam {
 
@@ -114,21 +115,10 @@ __device__ __forceinline__ void gf_add_outer(double *H, const double *j) {
     for (int b = 0; b < 6; b++) H[a * 6 + b] += j[a] * j[b];
 }
 // common::logDet(A, true): LLT, 2 * sum log(diag)   (math.hpp:172-202); A is overwritten
-__device__ double gf_logdet(double *A) {
+__device__ __noinline__ double gf_logdet(double *A) {
+  if (!chol<6>(A)) return -INFINITY;
   double s = 0.0;
-  for (int c = 0; c < 6; c++) {
-    double d = A[c * 6 + c];
-    for (int k = 0; k < c; k++) d -= A[c * 6 + k] * A[c * 6 + k];
-    if (!(d > 0.0)) return -INFINITY;
-    d = sqrt(d);
-    A[c * 6 + c] = d;
-    for (int i = c + 1; i < 6; i++) {
-      double t = A[i * 6 + c];
-      for (int k = 0; k < c; k++) t -= A[i * 6 + k] * A[c * 6 + k];
-      A[i * 6 + c] = t / d;
-    }
-    s += log(d);
-  }
+  for (int c = 0; c < 6; c++) s += log(A[c * 6 + c]);
   return 2.0 * s;
 }
 __device__ double gf_logdet_with(const double *H, const double *j) {  // logDet(H + J^T J, true)

@@ -7,11 +7,12 @@
 // k_odom_linearize<D>: one thread per feature computes (r, row); the D(D+1)/2 + D + 2 packed sums are reduced
 // element by element with warp shuffles into a per-warp shared-memory accumulator (a 1x12 row would need 92 fp64
 // accumulators per thread otherwise), summed across warps in fixed order, one partial per CTA — no atomics.
-// k_odom_lm<D>: fixed-order partial sum + the same Levenberg-Marquardt state machine as solve_kernels.cu's k_lm,
-// generalised to D = 6 or 12 (two 6-dof blocks, PoseLocalParameterization::Plus per block).
+// k_odom_lm<D>: fixed-order partial sum + lm.cuh's Levenberg-Marquardt state machine on the odometry problem, D = 6 or 12
+// (two 6-dof blocks, PoseLocalParameterization::Plus per block).
 #include "ctx.h"
 #include "factors.cuh"
 #include "host_util.h"
+#include "lm.cuh"
 
 namespace mloam {
 
@@ -24,8 +25,8 @@ struct OdPack {
 };
 
 struct OdomState {
-  double xp[7], xi[7], xe[7];  // pivot (constant), pose_i, ext: accepted
-  double xic[7], xec[7];       // candidates
+  double xp[7];                // pivot (constant)
+  double x[14], xc[14];        // [pose_i | ext]: accepted, candidate
   double H[144], g[12], cost;
   double scale[12], diag[12];
   double radius, decrease_factor, model_cost_change, x_norm, initial_cost;
@@ -51,7 +52,7 @@ __global__ void __launch_bounds__(OD_THREADS) k_odom_linearize(OdomSets a, const
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   for (int k = lane; k < N; k += 32) acc[wid][k] = 0.0;
   __syncwarp();
-  const Chain ch = make_chain(st->xp, use_candidate ? st->xic : st->xi, use_candidate ? st->xec : st->xe);
+  const Chain ch = make_chain(st->xp, use_candidate ? st->xc : st->x, use_candidate ? st->xc + 7 : st->x + 7);
   const int fm = st->free_mask;
   for (int s = 0; s < OD_SETS; s++) {
     const int n = a.n[s];
@@ -116,131 +117,47 @@ __global__ void __launch_bounds__(OD_THREADS) k_odom_linearize(OdomSets a, const
 }
 
 // ------------------------------------------------------------------------------------------ LM (D = 6 | 12)
-template <int D>
-__device__ bool chol_d(double *A) {
-  for (int j = 0; j < D; j++) {
-    double d = A[j * D + j];
-    for (int k = 0; k < j; k++) d -= A[j * D + k] * A[j * D + k];
-    if (!(d > 0.0)) return false;
-    d = sqrt(d);
-    A[j * D + j] = d;
-    for (int i = j + 1; i < D; i++) {
-      double s = A[i * D + j];
-      for (int k = 0; k < j; k++) s -= A[i * D + k] * A[j * D + k];
-      A[i * D + j] = s / d;
+// The odometry problem of the single-thread machine (lm.cuh): x (+) delta over the free blocks with the identity V_update (the
+// odometry's per-block degeneracy remap, estimator.cpp:1610-1635, is not applied here — next tier), chol<D>.
+template <int D_>
+struct OdomProblem {
+  using State = OdomState;
+  static constexpr int D = D_, NX = 14;
+  __device__ static bool solve(double *A, const double *b, double *x) {
+    if (!chol<D>(A)) return false;
+    chol_solve<D>(A, b, x);
+    return true;
+  }
+  __device__ static void plus_into(const OdomState *st, const double *delta, double *out) {
+    const double I6[36] = {1, 0, 0, 0, 0, 0, 0, 1, 0, 0, 0, 0, 0, 0, 1, 0, 0, 0, 0, 0, 0, 1, 0, 0, 0, 0, 0, 0, 1, 0, 0, 0, 0, 0, 0, 1};
+    for (int k = 0; k < 14; k++) out[k] = st->x[k];
+    if (D == 12) {
+      pose_plus(st->x, delta, I6, out);
+      pose_plus(st->x + 7, delta + 6, I6, out + 7);
+    } else if (st->free_mask & 1) {
+      pose_plus(st->x, delta, I6, out);
+    } else {
+      pose_plus(st->x + 7, delta, I6, out + 7);
     }
   }
-  return true;
-}
-template <int D>
-__device__ void chol_solve_d(const double *L, const double *b, double *x) {
-  double y[D];
-  for (int i = 0; i < D; i++) {
-    double s = b[i];
-    for (int k = 0; k < i; k++) s -= L[i * D + k] * y[k];
-    y[i] = s / L[i * D + i];
+  __device__ static void plus(OdomState *st, const double *delta) { plus_into(st, delta, st->xc); }
+  __device__ static double x_norm(const OdomState *st) {  // the free blocks, pose_i then ext
+    double s = 0;
+    if (D == 12 || (st->free_mask & 1))
+      for (int k = 0; k < 7; k++) s += st->x[k] * st->x[k];
+    if (D == 12 || (st->free_mask & 2))
+      for (int k = 7; k < 14; k++) s += st->x[k] * st->x[k];
+    return sqrt(s);
   }
-  for (int i = D - 1; i >= 0; i--) {
-    double s = y[i];
-    for (int k = i + 1; k < D; k++) s -= L[k * D + i] * x[k];
-    x[i] = s / L[i * D + i];
+  __device__ static double grad_max(const OdomState *st) {
+    double neg[D], xo[14];
+    for (int j = 0; j < D; j++) neg[j] = -st->g[j];
+    plus_into(st, neg, xo);
+    double m = 0;
+    for (int k = 0; k < 14; k++) m = fmax(m, fabs(st->x[k] - xo[k]));
+    return m;
   }
-}
-
-__device__ constexpr double kOdMinDiag = 1e-6, kOdMaxDiag = 1e32, kOdMaxRadius = 1e16;
-__device__ constexpr double kOdFuncTol = 1e-6, kOdParamTol = 1e-8, kOdGradTol = 1e-10, kOdMinRel = 1e-3;
-
-// x (+) delta over the free blocks (identity V_update: the odometry's per-block degeneracy remap, estimator.cpp:1610-1635,
-// is not applied here — next tier)
-template <int D>
-__device__ void od_plus(const OdomState *st, const double *delta, double *xi_out, double *xe_out) {
-  const double I6[36] = {1, 0, 0, 0, 0, 0, 0, 1, 0, 0, 0, 0, 0, 0, 1, 0, 0, 0, 0, 0, 0, 1, 0, 0, 0, 0, 0, 0, 1, 0, 0, 0, 0, 0, 0, 1};
-  for (int k = 0; k < 7; k++) xi_out[k] = st->xi[k], xe_out[k] = st->xe[k];
-  if (D == 12) {
-    pose_plus(st->xi, delta, I6, xi_out);
-    pose_plus(st->xe, delta + 6, I6, xe_out);
-  } else if (st->free_mask & 1) {
-    pose_plus(st->xi, delta, I6, xi_out);
-  } else {
-    pose_plus(st->xe, delta, I6, xe_out);
-  }
-}
-template <int D>
-__device__ double od_xnorm(const OdomState *st, const double *xi, const double *xe) {
-  double s = 0;
-  if (D == 12 || (st->free_mask & 1))
-    for (int k = 0; k < 7; k++) s += xi[k] * xi[k];
-  if (D == 12 || (st->free_mask & 2))
-    for (int k = 0; k < 7; k++) s += xe[k] * xe[k];
-  return sqrt(s);
-}
-template <int D>
-__device__ double od_grad_max(const OdomState *st) {
-  double neg[D], xi[7], xe[7];
-  for (int j = 0; j < D; j++) neg[j] = -st->g[j];
-  od_plus<D>(st, neg, xi, xe);
-  double m = 0;
-  for (int k = 0; k < 7; k++) m = fmax(m, fmax(fabs(st->xi[k] - xi[k]), fabs(st->xe[k] - xe[k])));
-  return m;
-}
-template <int D>
-__device__ void od_compute_step(OdomState *st) {
-  while (true) {
-    if (st->iteration >= st->max_inner) {
-      st->done = 1, st->termination = 0;
-      return;
-    }
-    double Hs[D * D], gs[D], A[D * D], step[D];
-    for (int a = 0; a < D; a++) {
-      gs[a] = st->scale[a] * st->g[a];
-      for (int b = 0; b < D; b++) Hs[a * D + b] = st->scale[a] * st->H[a * D + b] * st->scale[b];
-    }
-    if (!st->reuse_diagonal)
-      for (int j = 0; j < D; j++) st->diag[j] = fmin(fmax(Hs[j * D + j], kOdMinDiag), kOdMaxDiag);
-    for (int i = 0; i < D * D; i++) A[i] = Hs[i];
-    for (int j = 0; j < D; j++) {
-      const double l = sqrt(st->diag[j] / st->radius);
-      A[j * D + j] += l * l;
-    }
-    bool ok = chol_d<D>(A);
-    if (ok) {
-      chol_solve_d<D>(A, gs, step);
-      for (int j = 0; j < D; j++) {
-        step[j] = -step[j];
-        if (!isfinite(step[j])) ok = false;
-      }
-    }
-    st->reuse_diagonal = 1;
-    st->iteration++;
-    st->total_iterations++;
-    double mcc = 0;
-    if (ok) {
-      double sg = 0, sHs = 0;
-      for (int a = 0; a < D; a++) {
-        sg += step[a] * gs[a];
-        double t = 0;
-        for (int b = 0; b < D; b++) t += Hs[a * D + b] * step[b];
-        sHs += step[a] * t;
-      }
-      mcc = -(sg + 0.5 * sHs);
-      if (mcc < 0) ok = false;
-    }
-    if (!ok) {
-      if (++st->num_invalid >= 5) {
-        st->done = 1, st->termination = 4;
-        return;
-      }
-      st->radius *= 0.5;
-      continue;
-    }
-    st->num_invalid = 0;
-    double delta[D];
-    for (int j = 0; j < D; j++) delta[j] = step[j] * st->scale[j];
-    od_plus<D>(st, delta, st->xic, st->xec);
-    st->model_cost_change = mcc;
-    return;
-  }
-}
+};
 
 template <int D>
 __global__ void __launch_bounds__(OD_THREADS) k_odom_lm(const double *__restrict__ partials, int n_blocks, OdomState *st, int mode) {
@@ -259,65 +176,23 @@ __global__ void __launch_bounds__(OD_THREADS) k_odom_lm(const double *__restrict
     for (int j = i; j < D; j++) H[i * D + j] = H[j * D + i] = ne[q++];
   for (int k = 0; k < D; k++) g[k] = ne[NH + k];
   const double cost = ne[NH + D];
-  if (mode == 1) {
-    for (int i = 0; i < D * D; i++) st->H[i] = H[i];
-    for (int i = 0; i < D; i++) st->g[i] = g[i];
-    st->cost = st->initial_cost = cost;
-    st->rows = (int)ne[NH + D + 1];
-    st->x_norm = od_xnorm<D>(st, st->xi, st->xe);
-    for (int j = 0; j < D; j++) st->scale[j] = 1.0 / (1.0 + sqrt(H[j * D + j]));
-    st->radius = 1e4, st->decrease_factor = 2.0, st->reuse_diagonal = 0;
-    st->iteration = 0, st->num_invalid = 0, st->done = 0, st->termination = 0;
-    for (int k = 0; k < 7; k++) st->xic[k] = st->xi[k], st->xec[k] = st->xe[k];
-    if (od_grad_max<D>(st) <= kOdGradTol) {
-      st->done = 1, st->termination = 3;
-      return;
-    }
-    od_compute_step<D>(st);
+  if (mode == 2) {
+    lm_digest<OdomProblem<D>>(st, H, g, cost);
     return;
   }
-  if (st->done) return;
-  double sn = 0;
-  for (int k = 0; k < 7; k++)
-    sn += (st->xi[k] - st->xic[k]) * (st->xi[k] - st->xic[k]) + (st->xe[k] - st->xec[k]) * (st->xe[k] - st->xec[k]);
-  sn = sqrt(sn);
-  if (sn <= kOdParamTol * (st->x_norm + kOdParamTol)) {
-    st->done = 1, st->termination = 2;
-    return;
-  }
-  const double cost_change = st->cost - cost;
-  if (fabs(cost_change) <= kOdFuncTol * st->cost) {
-    st->done = 1, st->termination = 1;
-    return;
-  }
-  const double rel = cost_change / st->model_cost_change;
-  if (rel > kOdMinRel) {
-    const double t = 2.0 * rel - 1.0;
-    st->radius = fmin(kOdMaxRadius, st->radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
-    st->decrease_factor = 2.0;
-    st->reuse_diagonal = 0;
-    for (int k = 0; k < 7; k++) st->xi[k] = st->xic[k], st->xe[k] = st->xec[k];
-    st->x_norm = od_xnorm<D>(st, st->xi, st->xe);
-    for (int i = 0; i < D * D; i++) st->H[i] = H[i];
-    for (int i = 0; i < D; i++) st->g[i] = g[i];
-    st->cost = cost;
-    if (od_grad_max<D>(st) <= kOdGradTol) {
-      st->done = 1, st->termination = 3;
-      return;
-    }
-  } else {
-    st->radius = st->radius / st->decrease_factor;
-    st->decrease_factor *= 2.0;
-    st->reuse_diagonal = 1;
-  }
-  od_compute_step<D>(st);
+  for (int i = 0; i < D * D; i++) st->H[i] = H[i];
+  for (int i = 0; i < D; i++) st->g[i] = g[i];
+  st->cost = st->initial_cost = cost;
+  st->rows = (int)ne[NH + D + 1];
+  lm_begin<OdomProblem<D>>(st);
 }
 
 __global__ void k_odom_init(OdomState *st, const double *x21, int free_mask, int max_inner) {
   if (threadIdx.x == 0) {
-    for (int k = 0; k < 7; k++) st->xp[k] = x21[k], st->xi[k] = st->xic[k] = x21[7 + k], st->xe[k] = st->xec[k] = x21[14 + k];
+    for (int k = 0; k < 7; k++) st->xp[k] = x21[k];
+    for (int k = 0; k < 14; k++) st->x[k] = st->xc[k] = x21[7 + k];
     st->free_mask = free_mask, st->max_inner = max_inner;
-    st->done = 0, st->termination = 0, st->total_iterations = 0, st->iteration = 0, st->rows = 0, st->cost = st->initial_cost = 0;
+    st->done = 0, st->termination = kTermMaxIterations, st->total_iterations = 0, st->iteration = 0, st->rows = 0, st->cost = st->initial_cost = 0;
   }
 }
 
@@ -405,7 +280,7 @@ extern "C" int mloam_odom_solve(mloam_ctx_t *h, int n, const unsigned char *h_ty
   OdomState *hs = odom_mirror(c);
   MLOAM_CUDA_OK(c, cudaMemcpyAsync(hs, st, sizeof(OdomState), cudaMemcpyDeviceToHost, c->stream));
   MLOAM_CUDA_OK(c, cudaStreamSynchronize(c->stream));
-  for (int k = 0; k < 7; k++) pose_i7[k] = hs->xi[k], ext7[k] = hs->xe[k];
+  for (int k = 0; k < 7; k++) pose_i7[k] = hs->x[k], ext7[k] = hs->x[7 + k];
   if (stats) {
     stats->ran = 1, stats->lm_iterations = hs->total_iterations, stats->termination = hs->termination;
     stats->final_cost = hs->cost, stats->n_surf = (int)pts[1].size(), stats->n_corner = (int)pts[0].size();

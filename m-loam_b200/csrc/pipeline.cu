@@ -11,6 +11,7 @@
 
 #include "ctx.h"
 #include "host_util.h"
+#include "lm.cuh"
 
 using namespace mloam;
 
@@ -201,16 +202,16 @@ int scan2map_finish(Ctx *c, const ScanRef &S, const double *pose_init7, bool wan
   if (!S.d_n_surf) h_cnt[0] = S.n_surf;
   if (!S.d_n_corner) h_cnt[1] = S.n_corner;
   for (int k = 0; k < 7; k++) pose_out7[k] = hs->x[k];
-  if (want_cov && hs->termination != 8 && hs->termination != 9) memcpy(c->pose_cov36, c->pinned->pose_cov, sizeof(c->pose_cov36));
-  if (hs->termination == 9) {  // the peer-memory exchange timed out or the ranks lost lock-step: the summed state is not trustworthy
+  if (want_cov && hs->termination != kTermBarrierTimeout && hs->termination != kTermExchangeFailed) memcpy(c->pose_cov36, c->pinned->pose_cov, sizeof(c->pose_cov36));
+  if (hs->termination == kTermExchangeFailed) {  // the peer-memory exchange timed out or the ranks lost lock-step: the summed state is not trustworthy
     for (int k = 0; k < 7; k++) pose_out7[k] = pose_init7[k];
-    if (stats) stats->ran = 1, stats->termination = 9;
+    if (stats) stats->ran = 1, stats->termination = kTermExchangeFailed;
     return fail(c, MLOAM_E_NCCL, "scan2map: peer-memory exchange failed (a rank did not arrive or the ranks lost lock-step); "
                                   "call mloam_comm_p2p_reset on every rank behind a barrier");
   }
-  if (hs->termination == 8) {  // k_linearize's grid barrier gave up: a block of the grid never became resident within ~2 s
+  if (hs->termination == kTermBarrierTimeout) {  // k_linearize's grid barrier gave up: a block of the grid never became resident within ~2 s
     for (int k = 0; k < 7; k++) pose_out7[k] = pose_init7[k];
-    if (stats) stats->ran = 1, stats->termination = 8;
+    if (stats) stats->ran = 1, stats->termination = kTermBarrierTimeout;
     return fail(c, MLOAM_E_STATE, "scan2map: the two-evaluation launch timed out at its grid barrier (GPU shared with a kernel that never "
                                    "yields?); set MLOAM_FUSE_ITER=0 to use one launch per evaluation");
   }

@@ -14,6 +14,7 @@
 
 #include "ctx.h"
 #include "factors.cuh"
+#include "lm.cuh"
 #include "match_fit.cuh"
 
 namespace mloam {
@@ -179,7 +180,7 @@ __global__ void __launch_bounds__(LIN_THREADS) k_linearize(LinArgs a, double *__
     }
     __syncthreads();
     if (barrier_failed) {
-      if (threadIdx.x == 0) a.state_rw->termination = 8, a.state_rw->done = 1;
+      if (threadIdx.x == 0) a.state_rw->termination = kTermBarrierTimeout, a.state_rw->done = 1;
       return;
     }
     if (__ldcg(&a.state_rw->done)) return;  // the step of pass 0 ended the Solve (tolerance, too few rows, invalid steps)
@@ -380,133 +381,31 @@ void eig_report_host(const double *H36, double *w6) {
   eig_sym6(H36, w6, V);
 }
 
-// In-place lower Cholesky factor of a 6x6; inv_diag[j] = 1 / L[j][j].  One square root and one division per column:
-// the off-diagonal entries are scaled by the reciprocal (double division is a ~100-cycle software sequence and this
-// runs on a single thread between two grid-wide kernels).
-__device__ __forceinline__ bool chol6(double *A, double *inv_diag) {
-  constexpr int N = 6;
-#pragma unroll
-  for (int j = 0; j < N; j++) {
-    double d = A[j * N + j];
-#pragma unroll
-    for (int k = 0; k < j; k++) d -= A[j * N + k] * A[j * N + k];
-    if (!(d > 0.0)) return false;
-    d = sqrt(d);
-    A[j * N + j] = d;
-    const double inv = 1.0 / d;
-    inv_diag[j] = inv;
-#pragma unroll
-    for (int i = j + 1; i < N; i++) {
-      double s = A[i * N + j];
-#pragma unroll
-      for (int k = 0; k < j; k++) s -= A[i * N + k] * A[j * N + k];
-      A[i * N + j] = s * inv;
-    }
-  }
-  return true;
-}
-__device__ __forceinline__ void chol6_solve(const double *L, const double *inv_diag, const double *b, double *x) {
-  constexpr int N = 6;
-  double y[6];
-#pragma unroll
-  for (int i = 0; i < N; i++) {
-    double s = b[i];
-#pragma unroll
-    for (int k = 0; k < i; k++) s -= L[i * N + k] * y[k];
-    y[i] = s * inv_diag[i];
-  }
-#pragma unroll
-  for (int i = N - 1; i >= 0; i--) {
-    double s = y[i];
-#pragma unroll
-    for (int k = i + 1; k < N; k++) s -= L[k * N + i] * x[k];
-    x[i] = s * inv_diag[i];
-  }
-}
-
-// Ceres defaults the reference relies on (never overridden in-tree; SURVEY.md §8c)
-__device__ constexpr double kMinDiag = 1e-6, kMaxDiag = 1e32, kMaxRadius = 1e16;
-__device__ constexpr double kFuncTol = 1e-6, kParamTol = 1e-8, kGradTol = 1e-10, kMinRelDecrease = 1e-3;
-
-__device__ double gradient_max_norm(const LMState *st) {
-  double neg[6], xp[7];
-  for (int j = 0; j < 6; j++) neg[j] = -st->g[j];
-  pose_plus(st->x, neg, st->V_update, xp);
-  double m = 0;
-  for (int k = 0; k < 7; k++) m = fmax(m, fabs(st->x[k] - xp[k]));
-  return m;
-}
-
-// LevenbergMarquardtStrategy::ComputeStep + the invalid-step loop of TrustRegionMinimizer.
-__device__ void lm_compute_step(LMState *st) {
-  while (true) {
-    if (st->iteration >= st->max_inner) {
-      st->done = 1, st->termination = 0;
-      return;
-    }
-    double Hs[36], gs[6], A[36], step[6];
-#pragma unroll
-    for (int a = 0; a < 6; a++) {
-      gs[a] = st->scale[a] * st->g[a];
-#pragma unroll
-      for (int b = 0; b < 6; b++) Hs[a * 6 + b] = st->scale[a] * st->H[a * 6 + b] * st->scale[b];
-    }
-    if (!st->reuse_diagonal) {
-#pragma unroll
-      for (int j = 0; j < 6; j++) st->diag[j] = fmin(fmax(Hs[j * 6 + j], kMinDiag), kMaxDiag);
-    }
-#pragma unroll
-    for (int i = 0; i < 36; i++) A[i] = Hs[i];
-#pragma unroll
-    for (int j = 0; j < 6; j++) {
-      const double l = sqrt(st->diag[j] / st->radius);
-      A[j * 6 + j] += l * l;
-    }
+// The pose problem of the single-thread machine (lm.cuh): one 6-DoF block, x (+) delta through the degeneracy remap V_update, chol6.
+struct PoseProblem {
+  using State = LMState;
+  static constexpr int D = 6, NX = 7;
+  __device__ static bool solve(double *A, const double *b, double *x) {
     double inv_diag[6];
-    bool ok = chol6(A, inv_diag);
-    if (ok) {
-      chol6_solve(A, inv_diag, gs, step);
-#pragma unroll
-      for (int j = 0; j < 6; j++) {
-        step[j] = -step[j];
-        if (!isfinite(step[j])) ok = false;
-      }
-    }
-    st->reuse_diagonal = 1;
-    st->iteration++;
-    st->total_iterations++;
-    double mcc = 0;
-    if (ok) {
-      double sg = 0, sHs = 0;
-#pragma unroll
-      for (int a = 0; a < 6; a++) {
-        sg += step[a] * gs[a];
-        double t = 0;
-#pragma unroll
-        for (int b = 0; b < 6; b++) t += Hs[a * 6 + b] * step[b];
-        sHs += step[a] * t;
-      }
-      mcc = -(sg + 0.5 * sHs);
-      if (mcc < 0) ok = false;
-    }
-    if (!ok) {
-      if (++st->num_invalid >= 5) {
-        st->done = 1, st->termination = 4;
-        return;
-      }
-      st->radius *= 0.5;
-      st->reuse_diagonal = 1;
-      continue;
-    }
-    st->num_invalid = 0;
-    double delta[6];
-#pragma unroll
-    for (int j = 0; j < 6; j++) delta[j] = step[j] * st->scale[j];
-    pose_plus(st->x, delta, st->V_update, st->xc);
-    st->model_cost_change = mcc;
-    return;
+    if (!chol6(A, inv_diag)) return false;
+    chol6_solve(A, inv_diag, b, x);
+    return true;
   }
-}
+  __device__ static void plus(LMState *st, const double *delta) { pose_plus(st->x, delta, st->V_update, st->xc); }
+  __device__ static double x_norm(const LMState *st) {
+    double xn = 0;
+    for (int k = 0; k < 7; k++) xn += st->x[k] * st->x[k];
+    return sqrt(xn);
+  }
+  __device__ static double grad_max(const LMState *st) {
+    double neg[6], xp[7];
+    for (int j = 0; j < 6; j++) neg[j] = -st->g[j];
+    pose_plus(st->x, neg, st->V_update, xp);
+    double m = 0;
+    for (int k = 0; k < 7; k++) m = fmax(m, fabs(st->x[k] - xp[k]));
+    return m;
+  }
+};
 
 __device__ void unpack_ne(const double *ne, double *H, double *g) {
   int q = 0;
@@ -543,93 +442,46 @@ __device__ void eig_remap(LMState *st, double eig_thre) {
       }
 }
 
-// One thread advances the state machine on a shared-memory copy of the state (lm_tail stages it in and out).
-// mode 1: begin a Solve with the evaluation at x.  mode 2: digest the evaluation at xc.
+// One thread advances the state machine on a shared-memory copy of the state (lm_tail stages it in and out): the pose's prologue of
+// a Solve around lm.cuh's machine.  mode 1: begin a Solve with the evaluation at x.  mode 2: digest the evaluation at xc.
 // The reference for lm_advance_warp (MLOAM_LM_TAIL=serial).
 __device__ void lm_advance(LMState *st, const double *ne, int mode, double eig_thre, int want_eig) {
   double H[36], g[6];
   unpack_ne(ne, H, g);
   const double cost = ne[NE_H + NE_G];
-  if (mode == 1) {
-    for (int i = 0; i < 36; i++) st->H[i] = H[i], st->H0[i] = H[i];
-    for (int i = 0; i < 6; i++) st->g[i] = g[i];
-    st->cost = cost;
-    st->initial_cost = cost;
-    st->n_valid[0] = (int)ne[NE_H + NE_G + 1];
-    st->n_valid[1] = (int)ne[NE_H + NE_G + 2];
-    st->rows = st->n_valid[0] + st->n_valid[1];
-    st->skipped = 0;
-    if (st->rows < st->min_corr) {  // "less correspondence": the outer iteration is skipped, pose untouched
-      st->done = 1, st->termination = 5, st->skipped = 1;
-      for (int k = 0; k < 7; k++) st->xc[k] = st->x[k];
-      return;
-    }
-    // PoseLocalParameterization::setParameter + evalDegenracy (lidar_mapper_keyframe.cpp:1172-1204)
-    for (int i = 0; i < 36; i++) st->V_update[i] = (i % 7 == 0) ? 1.0 : 0.0;
-    st->is_degenerate = 0;
-    for (int i = 0; i < 6; i++) st->eig[i] = 0.0;
-    // lambda_min(H) > eig_thre  <=>  H - eig_thre*I is positive definite: one 6x6 Cholesky decides the common,
-    // non-degenerate case; the Jacobi eigen-solver only runs when a direction is (nearly) degenerate or when the
-    // caller asked for the eigenvalue report (want_eig: last outer iteration).
-    bool need_eig = st->rows > 0 && eig_thre > 0.0;
-    if (need_eig && !want_eig) {
-      double S[36];
-      for (int i = 0; i < 36; i++) S[i] = H[i] - ((i % 7 == 0) ? eig_thre : 0.0);
-      double inv_diag[6];
-      if (chol6(S, inv_diag)) need_eig = false;
-    }
-    if (need_eig) eig_remap(st, eig_thre);
-    double xn = 0;
-    for (int k = 0; k < 7; k++) xn += st->x[k] * st->x[k];
-    st->x_norm = sqrt(xn);
-    for (int j = 0; j < 6; j++) st->scale[j] = 1.0 / (1.0 + sqrt(H[j * 6 + j]));
-    st->radius = 1e4, st->decrease_factor = 2.0, st->reuse_diagonal = 0;
-    st->iteration = 0, st->num_invalid = 0, st->done = 0, st->termination = 0;
+  if (mode == 2) {
+    lm_digest<PoseProblem>(st, H, g, cost);
+    return;
+  }
+  for (int i = 0; i < 36; i++) st->H[i] = H[i], st->H0[i] = H[i];
+  for (int i = 0; i < 6; i++) st->g[i] = g[i];
+  st->cost = cost;
+  st->initial_cost = cost;
+  st->n_valid[0] = (int)ne[NE_H + NE_G + 1];
+  st->n_valid[1] = (int)ne[NE_H + NE_G + 2];
+  st->rows = st->n_valid[0] + st->n_valid[1];
+  st->skipped = 0;
+  if (st->rows < st->min_corr) {  // "less correspondence": the outer iteration is skipped, pose untouched
+    st->done = 1, st->termination = kTermTooFewRows, st->skipped = 1;
     for (int k = 0; k < 7; k++) st->xc[k] = st->x[k];
-    if (gradient_max_norm(st) <= kGradTol) {
-      st->done = 1, st->termination = 3;
-      return;
-    }
-    lm_compute_step(st);
     return;
   }
-  // mode 2
-  if (st->done) return;
-  double sn = 0;
-  for (int k = 0; k < 7; k++) sn += (st->x[k] - st->xc[k]) * (st->x[k] - st->xc[k]);
-  sn = sqrt(sn);
-  if (sn <= kParamTol * (st->x_norm + kParamTol)) {
-    st->done = 1, st->termination = 2;
-    return;
+  // PoseLocalParameterization::setParameter + evalDegenracy (lidar_mapper_keyframe.cpp:1172-1204)
+  for (int i = 0; i < 36; i++) st->V_update[i] = (i % 7 == 0) ? 1.0 : 0.0;
+  st->is_degenerate = 0;
+  for (int i = 0; i < 6; i++) st->eig[i] = 0.0;
+  // lambda_min(H) > eig_thre  <=>  H - eig_thre*I is positive definite: one 6x6 Cholesky decides the common,
+  // non-degenerate case; the Jacobi eigen-solver only runs when a direction is (nearly) degenerate or when the
+  // caller asked for the eigenvalue report (want_eig: last outer iteration).
+  bool need_eig = st->rows > 0 && eig_thre > 0.0;
+  if (need_eig && !want_eig) {
+    double S[36];
+    for (int i = 0; i < 36; i++) S[i] = H[i] - ((i % 7 == 0) ? eig_thre : 0.0);
+    double inv_diag[6];
+    if (chol6(S, inv_diag)) need_eig = false;
   }
-  const double cost_change = st->cost - cost;
-  if (fabs(cost_change) <= kFuncTol * st->cost) {
-    st->done = 1, st->termination = 1;
-    return;
-  }
-  const double rel = cost_change / st->model_cost_change;
-  if (rel > kMinRelDecrease) {
-    const double t = 2.0 * rel - 1.0;
-    st->radius = st->radius / fmax(1.0 / 3.0, 1.0 - t * t * t);
-    st->radius = fmin(kMaxRadius, st->radius);
-    st->decrease_factor = 2.0;
-    st->reuse_diagonal = 0;
-    double xn = 0;
-    for (int k = 0; k < 7; k++) st->x[k] = st->xc[k], xn += st->xc[k] * st->xc[k];
-    st->x_norm = sqrt(xn);
-    for (int i = 0; i < 36; i++) st->H[i] = H[i];
-    for (int i = 0; i < 6; i++) st->g[i] = g[i];
-    st->cost = cost;
-    if (gradient_max_norm(st) <= kGradTol) {
-      st->done = 1, st->termination = 3;
-      return;
-    }
-  } else {
-    st->radius = st->radius / st->decrease_factor;
-    st->decrease_factor *= 2.0;
-    st->reuse_diagonal = 1;
-  }
-  lm_compute_step(st);
+  if (need_eig) eig_remap(st, eig_thre);
+  lm_begin<PoseProblem>(st);
 }
 
 // ---------------------------------------------------------------------------------------- the LM step on one warp
@@ -688,7 +540,7 @@ __device__ __forceinline__ StepTry lm_try_step_warp(const LMState *st, bool deg_
     hs[b] = st->scale[r] * st->H[r * 6 + b] * st->scale[b];
   }
   const double hrr = st->scale[r] * st->H[r * 7] * st->scale[r];
-  const double dg = st->reuse_diagonal ? st->diag[r] : fmin(fmax(hrr, kMinDiag), kMaxDiag);
+  const double dg = st->reuse_diagonal ? st->diag[r] : lm_diag(hrr);
   const double l = sqrt(dg / st->radius);
 #pragma unroll
   for (int b = 0; b < 6; b++) {
@@ -743,7 +595,7 @@ __device__ void lm_compute_step_warp(LMState *st, const StepTry *first, const do
   while (true) {
     if (st->iteration >= st->max_inner) {
       __syncwarp();
-      if (lane == 0) st->done = 1, st->termination = 0;
+      if (lane == 0) st->done = 1, st->termination = kTermMaxIterations;
       return;
     }
     StepTry t;
@@ -764,7 +616,7 @@ __device__ void lm_compute_step_warp(LMState *st, const StepTry *first, const do
     }
     const bool reuse = st->reuse_diagonal != 0;
     const int num_invalid = st->num_invalid + 1;
-    const double radius = st->radius * 0.5;
+    const double radius = lm_radius_invalid(st->radius);
     __syncwarp();
     if (lane == 0) {
       if (!reuse)
@@ -774,7 +626,7 @@ __device__ void lm_compute_step_warp(LMState *st, const StepTry *first, const do
       st->total_iterations++;
       if (!t.ok) {
         st->num_invalid = num_invalid;
-        if (num_invalid >= 5) st->done = 1, st->termination = 4;
+        if (num_invalid >= kMaxInvalidSteps) st->done = 1, st->termination = kTermInvalidSteps;
         else st->radius = radius;
       } else {
         st->num_invalid = 0;
@@ -783,7 +635,7 @@ __device__ void lm_compute_step_warp(LMState *st, const StepTry *first, const do
       }
     }
     __syncwarp();
-    if (t.ok || num_invalid >= 5) return;
+    if (t.ok || num_invalid >= kMaxInvalidSteps) return;
   }
 }
 
@@ -807,7 +659,7 @@ __device__ void lm_advance_warp(LMState *st, const double *ne, int mode, double 
       st->cost = cost, st->initial_cost = cost;
       st->n_valid[0] = n0, st->n_valid[1] = n1, st->rows = rows, st->skipped = 0;
       for (int k = 0; k < 7; k++) st->xc[k] = x[k];
-      if (skip) st->done = 1, st->termination = 5, st->skipped = 1;  // "less correspondence": pose untouched
+      if (skip) st->done = 1, st->termination = kTermTooFewRows, st->skipped = 1;  // "less correspondence": pose untouched
     }
     if (skip) return;
     bool need_eig = rows > 0 && eig_thre > 0.0;
@@ -821,8 +673,8 @@ __device__ void lm_advance_warp(LMState *st, const double *ne, int mode, double 
     if (lane == 0) {
       st->is_degenerate = 0;
       st->x_norm = sqrt(xn);
-      st->radius = 1e4, st->decrease_factor = 2.0, st->reuse_diagonal = 0;
-      st->iteration = 0, st->num_invalid = 0, st->done = 0, st->termination = 0;
+      st->radius = kInitialRadius, st->decrease_factor = kDecreaseFactor, st->reuse_diagonal = 0;
+      st->iteration = 0, st->num_invalid = 0, st->done = 0, st->termination = kTermMaxIterations;
     }
     __syncwarp();
     // V_update does not enter the step: factor it (group 0) next to the degeneracy test (group 1)
@@ -845,7 +697,7 @@ __device__ void lm_advance_warp(LMState *st, const double *ne, int mode, double 
 #pragma unroll
     for (int k = 0; k < 7; k++) xc[k] = __shfl_sync(MLOAM_FULL_MASK, xp[k], 1);
     if (m <= kGradTol) {
-      if (lane == 0) st->done = 1, st->termination = 3;
+      if (lane == 0) st->done = 1, st->termination = kTermGradientTol;
       return;
     }
     lm_compute_step_warp(st, &t, xc);
@@ -860,20 +712,14 @@ __device__ void lm_advance_warp(LMState *st, const double *ne, int mode, double 
 #pragma unroll
   for (int k = 0; k < 7; k++) sn += (x[k] - xc[k]) * (x[k] - xc[k]);
   sn = sqrt(sn);
-  if (sn <= kParamTol * (st->x_norm + kParamTol)) {
-    if (lane == 0) st->done = 1, st->termination = 2;
+  double rel;
+  const int v = lm_verdict(sn, st->x_norm, st->cost, cost, st->model_cost_change, rel);
+  if (v >= 0) {
+    if (lane == 0) st->done = 1, st->termination = v;
     return;
   }
-  const double cost_change = st->cost - cost;
-  if (fabs(cost_change) <= kFuncTol * st->cost) {
-    if (lane == 0) st->done = 1, st->termination = 1;
-    return;
-  }
-  const double rel = cost_change / st->model_cost_change;
-  if (rel > kMinRelDecrease) {
-    const double t = 2.0 * rel - 1.0;
-    double radius = st->radius / fmax(1.0 / 3.0, 1.0 - t * t * t);
-    radius = fmin(kMaxRadius, radius);
+  if (v == kLMAccept) {
+    const double radius = lm_radius_accept(st->radius, rel);
     double xn = 0;
 #pragma unroll
     for (int k = 0; k < 7; k++) xn += xc[k] * xc[k];
@@ -890,17 +736,18 @@ __device__ void lm_advance_warp(LMState *st, const double *ne, int mode, double 
       st->H[e] = ne[lo * 6 - lo * (lo - 1) / 2 + hi - lo];
     }
     if (lane == 0) {
-      st->radius = radius, st->decrease_factor = 2.0, st->reuse_diagonal = 0;
+      st->radius = radius, st->decrease_factor = kDecreaseFactor, st->reuse_diagonal = 0;
       for (int k = 0; k < 7; k++) st->x[k] = xc[k];
       st->x_norm = sqrt(xn);
       for (int i = 0; i < 6; i++) st->g[i] = ne[NE_H + i];
       st->cost = cost;
-      if (m <= kGradTol) st->done = 1, st->termination = 3;
+      if (m <= kGradTol) st->done = 1, st->termination = kTermGradientTol;
     }
     __syncwarp();
     if (m <= kGradTol) return;
   } else {
-    const double radius = st->radius / st->decrease_factor, df = st->decrease_factor * 2.0;
+    double radius = st->radius, df = st->decrease_factor;
+    lm_radius_reject(radius, df);
     __syncwarp();
     if (lane == 0) st->radius = radius, st->decrease_factor = df, st->reuse_diagonal = 1;
     __syncwarp();
@@ -956,7 +803,7 @@ __device__ __forceinline__ void lm_run(LMState *s, const double *ne, int mode, d
   }
   if (threadIdx.x == 0) {
     s->work[0] = 0, s->work[1] = 0;  // re-arm the match work queues
-    if (failed) s->done = 1, s->termination = 9;  // the peer-memory exchange failed: the state is not trustworthy
+    if (failed) s->done = 1, s->termination = kTermExchangeFailed;  // the peer-memory exchange failed: the state is not trustworthy
     s->dbg_cycles[0] += t1 - t0, s->dbg_cycles[1] += clock64() - t1, s->dbg_cycles[2] += 1;
   }
 }
@@ -1175,7 +1022,7 @@ __global__ void k_lm_init(LMState *st, const double *pose7, int max_inner, int m
     for (int k = 0; k < 7; k++) st->x[k] = pose7[k], st->xc[k] = pose7[k];
     st->max_inner = max_inner;
     st->min_corr = min_corr, st->skipped = 0;
-    st->done = 0, st->termination = 0, st->total_iterations = 0, st->iteration = 0;
+    st->done = 0, st->termination = kTermMaxIterations, st->total_iterations = 0, st->iteration = 0;
     st->is_degenerate = 0, st->rows = 0, st->n_valid[0] = st->n_valid[1] = 0;
     st->work[0] = st->work[1] = 0;
     st->cost = 0, st->initial_cost = 0;
